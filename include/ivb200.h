@@ -1,4 +1,4 @@
-/* ivb200.h — C ABI of libivb200.so: the B200 (sm_100a) compute path for InternVideo2 pre-training.
+/* ivb200.h — C ABI of libivb200.so: the H100 (sm_90a) compute path for InternVideo2 pre-training.
  *
  * The reference (OpenGVLab/InternVideo) has no FFI of its own: its "operator interface" for this
  * path is the nn.Module surface of
@@ -20,8 +20,12 @@
  *   - `stream` is a cudaStream_t passed as void* (torch.cuda.current_stream().cuda_stream).
  *   - return value: 0 = ok, non-zero = error; ivb_last_error() returns the text.  No exceptions
  *     cross this boundary.  The library allocates nothing persistent; all buffers are borrowed.
- *   - there is no CPU fallback: without a CUDA device of compute capability 10.x every compute
+ *   - there is no CPU fallback: without a CUDA device of compute capability 9.0 every compute
  *     entry point returns an error.
+ *   - parameter gradients (ivb_norm_bwd, ivb_rmsnorm_pair_bwd, ivb_rmsnorm_bwd_layerscale, ivb_layerscale_bwd,
+ *     ivb_colsum_bf16, ivb_ln_l2_bwd) are summed over rows in a fixed order through a per-device scratch of the
+ *     library, so the same inputs give the same bits on every run.  That scratch holds one reduction at a time:
+ *     these entry points must not be called concurrently from two streams of the same device.
  */
 #ifndef IVB200_H_
 #define IVB200_H_
@@ -42,8 +46,8 @@ extern "C" {
 
 #define IVB_FLAG_GELU_TANH 1 /* tanh-approx GELU (FA2 FusedMLP) instead of erf (nn.GELU)           */
 #define IVB_FLAG_ACCUM 2     /* accumulate into out0                                               */
-#define IVB_FLAG_1CTA 4      /* force the single-CTA kernel (tcgen05.mma.cta_group::1, 128-row tiles)  */
-#define IVB_FLAG_2CTA 8      /* force the CTA-pair kernel  (tcgen05.mma.cta_group::2, 256-row tiles)  */
+#define IVB_FLAG_1CTA 4      /* force the single-CTA kernel (128-row tiles)                                      */
+#define IVB_FLAG_2CTA 8      /* force the CTA-pair kernel (cluster of 2, 256-row tiles, B tile TMA-multicast)     */
 #define IVB_FLAG_GELU_SAVE_GRAD 16 /* EPI_BIAS_GELU: out1 receives gelu'(h) instead of h; EPI_GELU_BWD: aux IS
                                      that saved derivative (out0 = acc * aux) — the backward epilogue then has
                                      no transcendental work (the training path; h itself is never needed)   */
@@ -51,14 +55,14 @@ extern "C" {
 /* ---- status ---------------------------------------------------------------------------------- */
 const char* ivb_last_error(void);
 int ivb_version(void);
-/* 0 if the current CUDA device can run this library (compute capability 10.x), else error. */
+/* 0 if the current CUDA device can run this library (compute capability 9.0), else error. */
 int ivb_device_check(void);
 /* number of kernels this library has launched since the last reset (bench.py "gpu_launches"). */
 long ivb_launch_count(void);
 void ivb_reset_launch_count(void);
 
-/* ---- tcgen05 GEMM -----------------------------------------------------------------------------
- * D[M,N] = epilogue( sum_k A(m,k) * B(n,k) ), bf16 operands, fp32 accumulate in TMEM.
+/* ---- wgmma GEMM -------------------------------------------------------------------------------
+ * D[M,N] = epilogue( sum_k A(m,k) * B(n,k) ), bf16 operands, fp32 accumulate.
  *   a_mn_major = 0: A is stored [M,K] row-major (pitch lda);  1: stored [K,M] row-major.
  *   b_mn_major = 0: B is stored [N,K] row-major (pitch ldb);  1: stored [K,N] row-major.
  * Supported (A,B) majors: (0,0) forward y = x W^T; (0,1) dgrad dx = dy W; (1,1) wgrad dW = dy^T x.
@@ -80,7 +84,7 @@ int ivb_norm_fwd(const void* x, int x_is_f32, long ldx, const void* weight, cons
                  float eps, int is_layernorm, int M, int D, void* y, long ldy, float* mean,
                  float* rstd, void* stream);
 /* dx = d norm / dx (+ dx_in, fp32, pitch lddx_in, optional); dweight/dbias: fp32 [D], ACCUMULATED
- * (atomicAdd) — zero them first.  dx_out is fp32 or bf16.  In-place dx_out == dy is allowed.      */
+ * (summed in a fixed order) — zero them first.  dx_out is fp32 or bf16.  In-place dx_out == dy is allowed.      */
 int ivb_norm_bwd(const void* dy, long lddy, const void* x, int x_is_f32, long ldx,
                  const void* weight, const float* mean, const float* rstd, int is_layernorm, int M,
                  int D, const float* dx_in, long lddx_in, void* dx_out, int dx_out_is_f32,
@@ -109,10 +113,10 @@ int ivb_rmsnorm_bwd_layerscale(const void* dy, long lddy, const float* x, long l
 int ivb_layerscale_bwd(const float* dx, long lddx, const void* y, long ldy, const void* gamma,
                        int M, int D, void* dy, long lddy, float* dgamma, float* dcolsum,
                        const float* rowscale, void* stream);
-/* out[j] += sum_m x[m,j]   (bf16 in, fp32 atomics) — bias gradients. */
+/* out[j] += sum_m x[m,j]   (bf16 in, fp32, summed in a fixed order) — bias gradients. */
 int ivb_colsum_bf16(const void* x, long ldx, int M, int N, float* out, void* stream);
 
-/* ---- attention (tcgen05, flash-style) -----------------------------------------------------------
+/* ---- attention (wgmma, flash-style)  -----------------------------------------------------------
  * out[b,q,h,:] = softmax(scale * q k^T) v, non-causal, no dropout.  q/k/v are [B*n, ld*] projection
  * buffers; `q` points at (token 0, head 0, dim 0) of its slot, heads are contiguous (h d), so the
  * packed qkv[B,S,3,H,d] layout of FlashAttention.forward (flash_attention_class.py:27-50) is passed
@@ -155,7 +159,8 @@ int ivb_im2col_visible(const void* video, const int* idx, int idx_stride, int j0
 int ivb_gather_add(const float* src, long src_bstride, const void* table, const int* idx,
                    int idx_bstride, int idx_off, int B, int rows, int D, void* out, int out_is_f32,
                    long out_bstride, void* stream);
-/* table_grad[idx[b,j] + idx_off, :] += g[b,j,:]  (fp32 atomics) — backward of ivb_gather_add. */
+/* table_grad[idx[b,j] + idx_off, :] += g[b,j,:]  (fp32) — backward of ivb_gather_add.  Clips are added in order;
+ * when idx[b,:] has no repeats within a clip the result is the same on every run. */
 int ivb_scatter_add(const void* g, int g_is_f32, long g_bstride, const int* idx, int idx_bstride,
                     int idx_off, int B, int rows, int D, float* table_grad, void* stream);
 
@@ -167,7 +172,7 @@ int ivb_ln_l2_fwd(const void* z, long ldz, const void* weight, const void* bias,
                   int C, void* out, long ldo, float* stats, const void* target, int target_is_f32,
                   long ldt, float* loss_sum, void* stream);
 /* d_out = (gscale_host * *gscale_dev) * dout.  For the fused loss pass dout = target and
- * gscale_host = -2/rows.  Writes dz (bf16); accumulates dweight/dbias (fp32 atomics).               */
+ * gscale_host = -2/rows.  Writes dz (bf16); accumulates dweight/dbias (fp32).                    */
 int ivb_ln_l2_bwd(const void* z, long ldz, const void* weight, const void* bias, const float* stats,
                   int M, int C, const void* dout, int dout_is_f32, long lddo, float gscale_host,
                   const float* gscale_dev, void* dz, long lddz, float* dweight, float* dbias,

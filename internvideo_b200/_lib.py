@@ -1,7 +1,7 @@
 """ctypes binding of libivb200.so (the C ABI in include/ivb200.h).
 
 There is no fallback: if the shared library is missing, or a compute entry point is called
-without a B200-class device, an exception is raised.
+without an H100-class (sm_90) device, an exception is raised.
 """
 from __future__ import annotations
 

@@ -1,8 +1,8 @@
-"""Build libivb200.so (in-tree) with nvcc for sm_100a.
+"""Build libivb200.so (in-tree) with nvcc for sm_90a.
 
 The shared library is a plain C-ABI object (include/ivb200.h); it links only against the CUDA
 runtime (cuTensorMapEncodeTiled is resolved at run time through cudaGetDriverEntryPoint), so it
-cross-compiles on a GPU-less box and travels to the B200 box inside the repo snapshot.
+cross-compiles without a GPU; the H100 only loads the built library.
 """
 from __future__ import annotations
 
@@ -19,7 +19,7 @@ OUT = PKG / "libivb200.so"
 OBJ = PKG / "build"
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     "--use_fast_math", "-Xcompiler", "-fPIC",
     "-Xptxas", "-v",

@@ -4,7 +4,7 @@ Mirrors InternVideo2/multi_modality/models/criterions.py (`get_sim` :15-55, `VTC
 :65-103, `get_mask` :200-216) and models/utils.py `AllGather` (:193-212):
 
   * forward: ONE NCCL all-gather of a packed [B_loc, 2C+pad] buffer (vision | text | idx) instead of
-    the reference's three collectives, then normalise -> tcgen05 sim GEMM -> fused two-direction
+    the reference's three collectives, then normalise -> wgmma sim GEMM -> fused two-direction
     soft-target cross-entropy (libivb200);
   * backward: NO collective — each rank keeps only the gradient rows of its own samples, exactly like
     `AllGather.backward` (models/utils.py:205-209); the usual gradient all-reduce of the data-parallel

@@ -1,17 +1,16 @@
-// ivb_attn.cu — non-causal multi-head attention forward on tcgen05 (flash-style, online softmax).
+// ivb_attn.cu — non-causal multi-head attention forward on Hopper wgmma (flash-style, online softmax).
 //
 // Stands in for FA2 flash_attn_varlen_qkvpacked_func as called by the reference's
 // FlashAttention.forward (InternVideo2/single_modality/models/flash_attention_class.py:47-50) and for
 // Attention._naive_attn's softmax((q*scale) k^T) v (internvideo2_pretrain.py:183-188).
 //
-// One CTA per (128-query block, head, clip).  S = Q K_j^T and O += P_j V_j run on the
-// tensor core with accumulators in TMEM; the four warps own one query row per thread (TMEM lane),
-// do the online softmax in registers and hand P_j back through shared memory (bf16, 128B-swizzled
-// K-major tile).  The rescale of O is lazy: it only happens when the running row max grows by more
-// than 2^8, so the common path never reads O back from TMEM.  K/V tiles of 64 keys are double
-// buffered with TMA; q/k/v are read straight out of the [tokens, (3|2)*H*d] projection buffers
-// through 4-D tensor maps (d, head, token, clip), so head_dim 88 is zero-padded by TMA's OOB fill
-// and the sequence tail (n = 417, 833, 1025, 2049...) needs no host-side padding.
+// One CTA per (128-query block, head, clip), 384 threads: warpgroup 0 is the TMA producer (one elected thread),
+// warpgroups 1 and 2 own 64 query rows each.  Per 64-key tile a warpgroup computes S = Q K_j^T with wgmma from
+// shared memory, runs the online softmax on the accumulator fragments (a row lives in the four threads of a quad),
+// and issues O += P V_j with P taken straight from registers (the fp32 accumulator layout of S is the bf16
+// register-A layout of the next wgmma).  K/V tiles are double-buffered with TMA; q/k/v are read straight out of
+// the [tokens, (3|2)*H*d] projection buffers through 4-D tensor maps (d, head, token, clip), so head_dim 88 is
+// zero-padded by TMA's OOB fill and the sequence tail (n = 417, 833, 1025, 2049...) needs no host-side padding.
 #include <math.h>
 #include <stdlib.h>
 
@@ -20,8 +19,9 @@
 
 namespace ivb {
 
-constexpr int ATT_BQ = 128;   // queries per CTA (UMMA M)
+constexpr int ATT_BQ = 128;   // queries per CTA (two warpgroups of 64)
 constexpr int ATT_BKV = 64;   // keys per step
+constexpr int ATT_NS = 2;     // K/V stages
 
 struct AttnFwdParams {
   int B, n, H, d;
@@ -31,43 +31,38 @@ struct AttnFwdParams {
   float* lse2;       // [B, H, n]  log2-domain logsumexp of the scaled scores
 };
 
-// KA: number of 64-wide atoms covering head_dim (1: d<=64, 2: d<=128).  NO: UMMA N of P·V (d rounded to 16)
-//
-// Warp roles (192 threads, 2 CTAs/SM): warps 0-3 = softmax (one query row per thread), warp 4 = the
-// single-thread tcgen05.mma issuer, warp 5 = the TMA producer; they talk only through mbarriers
-// (the first version let thread 0 of a softmax warp issue MMAs/TMA and every tile paid its serial issue work
-// on the softmax critical path):
-//   bar_k[s]/bar_v[s]  TMA -> issuer     K / V tile landed (tx)
-//   bar_kf[s]/bar_vf[s] issuer -> TMA    S_j / P·V_j MMAs that read the stage retired (tcgen05.commit)
-//   bar_s[b]           issuer -> softmax S_j complete in TMEM buffer b
-//   bar_p              softmax -> issuer P_j written to smem, S buffer drained (4 warp arrivals)
-//   bar_o              issuer -> softmax P·V_j retired: sP reusable, O stable
+// Quad reductions: the four threads (lane & 3) of a quad share an accumulator row.
+__device__ __forceinline__ float quad_max(float v) {
+  v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
+  return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
+}
+__device__ __forceinline__ float quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  return v + __shfl_xor_sync(0xffffffffu, v, 2);
+}
+
+// KA: number of 64-wide atoms covering head_dim (1: d<=64, 2: d<=128).  NO: wgmma N of P·V (d rounded up).
 template <int KA, int NO>
-__global__ void __launch_bounds__(192, 2)
+__global__ void __launch_bounds__(384, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                 const __grid_constant__ CUtensorMap tmV, const AttnFwdParams p) {
   constexpr int Q_BYTES = KA * ATT_BQ * 128;        // KA atoms of [128 rows x 128 B]
   constexpr int KV_BYTES = KA * ATT_BKV * 128;      // KA atoms of [64 rows x 128 B]
-  constexpr int P_BYTES = ATT_BQ * 128;             // [128 x 64] bf16
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* sQ = smem;
-  uint8_t* sK = sQ + Q_BYTES;            // 2 stages
-  uint8_t* sV = sK + 2 * KV_BYTES;       // 2 stages
-  uint8_t* sP = sV + 2 * KV_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sP + P_BYTES);
-  uint64_t* bar_q = bars;        // 1
-  uint64_t* bar_k = bars + 1;    // 2
-  uint64_t* bar_v = bars + 3;    // 2
-  uint64_t* bar_kf = bars + 5;   // 2
-  uint64_t* bar_vf = bars + 7;   // 2
-  uint64_t* bar_s = bars + 9;    // 2
-  uint64_t* bar_p = bars + 11;   // 1 (4 arrivals)
-  uint64_t* bar_o = bars + 12;   // 1
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 13);
+  uint8_t* sK = sQ + Q_BYTES;                  // ATT_NS stages
+  uint8_t* sV = sK + ATT_NS * KV_BYTES;        // ATT_NS stages
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sV + ATT_NS * KV_BYTES);
+  uint64_t* bar_q = bars;                       // 1
+  uint64_t* full_k = bars + 1;                  // ATT_NS
+  uint64_t* full_v = full_k + ATT_NS;           // ATT_NS
+  uint64_t* empty_k = full_v + ATT_NS;          // ATT_NS (one arrival per MMA warpgroup)
+  uint64_t* empty_v = empty_k + ATT_NS;         // ATT_NS
 
   const int tid = threadIdx.x;
   const int warp = tid >> 5;
   const int lane = tid & 31;
+  const int wg = tid >> 7;
   const int q0 = blockIdx.x * ATT_BQ;
   const int h = blockIdx.y;
   const int b = blockIdx.z;
@@ -76,182 +71,131 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
 
   if (tid == 0) {
     if ((smem_u32(smem) & 1023u) != 0) __trap();
-    for (int i = 0; i < 13; ++i) mbar_init(&bars[i], i == 11 ? 4 : 1);
+    mbar_init(bar_q, 1);
+    for (int i = 0; i < ATT_NS; ++i) {
+      mbar_init(&full_k[i], 1); mbar_init(&full_v[i], 1);
+      mbar_init(&empty_k[i], 2); mbar_init(&empty_v[i], 2);
+    }
     fence_mbar_init();
   }
-  if (warp == 4) tmem_alloc<256>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tS = tmem_base;           // 2 x 64 columns
-  const uint32_t tO = tmem_base + 128;     // NO columns
 
-  if (warp == 5) {
+  if (wg == 0) {
+    setmaxnreg_dec<24>();
     // ===================== TMA producer =====================
-    if (elect_one()) {
+    if (warp == 0 && elect_one()) {
       tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmK); tma_prefetch_desc(&tmV);
       mbar_expect_tx(bar_q, Q_BYTES);
 #pragma unroll
       for (int a = 0; a < KA; ++a)
         tma_load_4d(sQ + a * (ATT_BQ * 128), &tmQ, a * 64, h, q0, b, bar_q);
       for (int j = 0; j < nblk; ++j) {
-        const int st = j & 1;
-        if (j >= 2) mbar_wait(&bar_kf[st], ((j >> 1) - 1) & 1);   // S_{j-2} retired: K stage free
-        mbar_expect_tx(&bar_k[st], KV_BYTES);
+        const int st = j % ATT_NS;
+        const uint32_t ph = ((j / ATT_NS) & 1) ^ 1;
+        mbar_wait(&empty_k[st], ph);
+        mbar_expect_tx(&full_k[st], KV_BYTES);
 #pragma unroll
         for (int a = 0; a < KA; ++a)
-          tma_load_4d(sK + st * KV_BYTES + a * (ATT_BKV * 128), &tmK, a * 64, h, j * ATT_BKV, b, &bar_k[st]);
-        if (j >= 2) mbar_wait(&bar_vf[st], ((j >> 1) - 1) & 1);   // P·V_{j-2} retired: V stage free
-        mbar_expect_tx(&bar_v[st], KV_BYTES);
+          tma_load_4d(sK + st * KV_BYTES + a * (ATT_BKV * 128), &tmK, a * 64, h, j * ATT_BKV, b, &full_k[st]);
+        mbar_wait(&empty_v[st], ph);
+        mbar_expect_tx(&full_v[st], KV_BYTES);
 #pragma unroll
         for (int a = 0; a < KA; ++a)
-          tma_load_4d(sV + st * KV_BYTES + a * (ATT_BKV * 128), &tmV, a * 64, h, j * ATT_BKV, b, &bar_v[st]);
-      }
-    }
-  } else if (warp == 4) {
-    // ===================== MMA issuer =====================
-    if (elect_one()) {
-      constexpr uint32_t idesc_s = umma_idesc_bf16(ATT_BQ, ATT_BKV, false, false);
-      constexpr uint32_t idesc_o = umma_idesc_bf16(ATT_BQ, NO, false, true);
-      const uint32_t qa = smem_u32(sQ), pa = smem_u32(sP);
-      auto issue_s = [&](int j) {  // S_j = Q K_j^T  -> tS + (j&1)*64
-        const int st = j & 1;
-        mbar_wait(&bar_k[st], (j >> 1) & 1);
-        tc_fence_after();
-        const uint32_t ka = smem_u32(sK + st * KV_BYTES);
-        for (int kk = 0; kk < ksteps; ++kk) {
-          const uint32_t ao = (kk >> 2) * (ATT_BQ * 128) + (kk & 3) * 32;
-          const uint32_t bo = (kk >> 2) * (ATT_BKV * 128) + (kk & 3) * 32;
-          umma_bf16(tS + st * 64, umma_desc(qa + ao, 16, 1024), umma_desc(ka + bo, 16, 1024), idesc_s,
-                    kk > 0 ? 1u : 0u);
-        }
-        umma_commit(&bar_s[st]);
-        umma_commit(&bar_kf[st]);
-      };
-      mbar_wait(bar_q, 0);
-      issue_s(0);
-      if (nblk > 1) issue_s(1);
-      for (int j = 0; j < nblk; ++j) {
-        const int st = j & 1;
-        mbar_wait(bar_p, j & 1);                 // P_j in smem, S buffer (j&1) drained
-        mbar_wait(&bar_v[st], (j >> 1) & 1);
-        tc_fence_after();
-        const uint32_t va = smem_u32(sV + st * KV_BYTES);
-#pragma unroll
-        for (int kk = 0; kk < ATT_BKV / 16; ++kk)
-          umma_bf16(tO, umma_desc(pa + kk * 32, 16, 1024),
-                    umma_desc(va + kk * 2048, ATT_BKV * 128, 1024), idesc_o, (j > 0 || kk > 0) ? 1u : 0u);
-        umma_commit(bar_o);
-        umma_commit(&bar_vf[st]);
-        if (j + 2 < nblk) issue_s(j + 2);
+          tma_load_4d(sV + st * KV_BYTES + a * (ATT_BKV * 128), &tmV, a * 64, h, j * ATT_BKV, b, &full_v[st]);
       }
     }
   } else {
-    // ===================== softmax warps (0..3) =====================
-    float m_used = -INFINITY;  // running (lazily updated) row max, log2 domain
-    float l_run = 0.f;
-    const uint32_t lane_off = static_cast<uint32_t>(warp * 32) << 16;
-    const int r = tid;  // row inside the Q block == TMEM lane
-    uint8_t* prow = sP + (r >> 3) * 1024 + (r & 7) * 128;
+    setmaxnreg_inc<240>();
+    // ===================== MMA + softmax warpgroups =====================
+    const int cw = wg - 1;                                  // query rows [64*cw, 64*cw + 64) of the block
+    const bool signal = (tid & 127) == 0;
+    const int rloc = cw * 64 + (warp & 3) * 16 + (lane >> 2);  // this thread's rows: rloc, rloc + 8
+    const uint32_t qa = smem_u32(sQ) + cw * 8192;
+    float o[NO / 2];
+#pragma unroll
+    for (int i = 0; i < NO / 2; ++i) o[i] = 0.f;
+    float m_run[2] = {-INFINITY, -INFINITY};
+    float l_run[2] = {0.f, 0.f};
 
+    mbar_wait(bar_q, 0);
     for (int j = 0; j < nblk; ++j) {
-      const int st = j & 1;
-      mbar_wait(&bar_s[st], (j >> 1) & 1);
-      tc_fence_after();
-      uint32_t sb[64];
-      tmem_ld32(tS + lane_off + st * 64, sb);
-      tmem_ld32(tS + lane_off + st * 64 + 32, sb + 32);
-      tmem_wait_ld();
+      const int st = j % ATT_NS;
+      const uint32_t ph = (j / ATT_NS) & 1;
+      mbar_wait(&full_k[st], ph);
+      const uint32_t ka = smem_u32(sK + st * KV_BYTES);
+      float s[ATT_BKV / 2];
+      wgmma_fence();
+      for (int kk = 0; kk < ksteps; ++kk) {
+        const uint32_t off = (kk & 3) * 32;
+        Wgmma<ATT_BKV>::ss<0, 0>(s, gmma_desc(qa + (kk >> 2) * (ATT_BQ * 128) + off, 16, 1024),
+                                 gmma_desc(ka + (kk >> 2) * (ATT_BKV * 128) + off, 16, 1024), kk > 0 ? 1u : 0u);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_reg_fence(s, ATT_BKV / 2);
+      if (signal) mbar_arrive(&empty_k[st]);
+
       const int valid = p.n - j * ATT_BKV;  // columns >= valid are beyond the sequence
-      float mx = -INFINITY;
+      float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
-      for (int c = 0; c < 64; ++c) {
-        float s = __uint_as_float(sb[c]) * p.sc_log2;
-        if (c >= valid) s = -INFINITY;
-        sb[c] = __float_as_uint(s);
-        mx = fmaxf(mx, s);
+      for (int i = 0; i < ATT_BKV / 2; ++i) {
+        const int col = 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
+        float v = s[i] * p.sc_log2;
+        if (col >= valid) v = -INFINITY;
+        s[i] = v;
+        mx[(i >> 1) & 1] = fmaxf(mx[(i >> 1) & 1], v);
       }
-      if (j > 0) {
-        mbar_wait(bar_o, (j - 1) & 1);  // P·V of step j-1 retired: sP reusable, O stable
-        tc_fence_after();
-      }
-      bool need = false;
-      float alpha = 1.f;
-      if (j == 0) {
-        m_used = mx;
-      } else if (mx > m_used + 8.0f) {
-        need = true;
-        alpha = exp2f(m_used - mx);
-        m_used = mx;
-      }
-      if (__any_sync(0xffffffffu, need)) {  // rare: rescale the accumulator rows of this warp
-        l_run *= alpha;
-#pragma unroll 1
-        for (int c = 0; c < NO; c += 32) {
-          uint32_t ob[32];
-          tmem_ld32(tO + lane_off + c, ob);
-          tmem_wait_ld();
+      float alpha[2];
 #pragma unroll
-          for (int i = 0; i < 32; ++i) ob[i] = __float_as_uint(__uint_as_float(ob[i]) * alpha);
-          tmem_st32(tO + lane_off + c, ob);
-        }
-        tmem_wait_st();
+      for (int r = 0; r < 2; ++r) {
+        const float m_new = fmaxf(m_run[r], quad_max(mx[r]));
+        alpha[r] = exp2f(m_run[r] - m_new);
+        m_run[r] = m_new;
       }
-      float rs = 0.f;
+      float rs[2] = {0.f, 0.f};
 #pragma unroll
-      for (int c8 = 0; c8 < 8; ++c8) {
-        float e[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          e[i] = exp2f(__uint_as_float(sb[c8 * 8 + i]) - m_used);
-          rs += e[i];
-        }
-        uint4 w;
-        w.x = pack_bf16(e[0], e[1]); w.y = pack_bf16(e[2], e[3]);
-        w.z = pack_bf16(e[4], e[5]); w.w = pack_bf16(e[6], e[7]);
-        *reinterpret_cast<uint4*>(prow + ((c8 ^ (r & 7)) << 4)) = w;
+      for (int i = 0; i < ATT_BKV / 2; ++i) {
+        const int r = (i >> 1) & 1;
+        s[i] = exp2f(s[i] - m_run[r]);
+        rs[r] += s[i];
       }
-      l_run += rs;
-      fence_proxy_async_smem();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_p);
+#pragma unroll
+      for (int r = 0; r < 2; ++r) l_run[r] = l_run[r] * alpha[r] + rs[r];
+#pragma unroll
+      for (int i = 0; i < NO / 2; ++i) o[i] *= alpha[(i >> 1) & 1];
+      uint32_t pa[ATT_BKV / 16][4];
+#pragma unroll
+      for (int kk = 0; kk < ATT_BKV / 16; ++kk) acc_to_a_frag(s, kk, pa[kk]);
+
+      mbar_wait(&full_v[st], ph);
+      const uint32_t va = smem_u32(sV + st * KV_BYTES);
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < ATT_BKV / 16; ++kk)
+        Wgmma<NO>::rs<1>(o, pa[kk], gmma_desc(va + kk * 2048, ATT_BKV * 128, 1024), 1u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_reg_fence(o, NO / 2);
+      if (signal) mbar_arrive(&empty_v[st]);
     }
 
-    mbar_wait(bar_o, (nblk - 1) & 1);
-    tc_fence_after();
-    const int q = q0 + r;
-    const float inv_l = 1.0f / l_run;
-    __nv_bfloat16* orow = p.out + (static_cast<long>(b) * p.n + q) * p.ldo + h * p.d;
-#pragma unroll 1
-    for (int c = 0; c < NO; c += 32) {
-      uint32_t ob[32];
-      tmem_ld32(tO + lane_off + c, ob);
-      tmem_wait_ld();
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      l_run[r] = quad_sum(l_run[r]);
+      const int q = q0 + rloc + 8 * r;
       if (q < p.n) {
+        const float inv_l = 1.0f / l_run[r];
+        __nv_bfloat16* orow = p.out + (static_cast<long>(b) * p.n + q) * p.ldo + h * p.d;
 #pragma unroll
-        for (int i = 0; i < 32; i += 8) {
-          if (c + i < p.d) {
-            uint4 w;
-            w.x = pack_bf16(__uint_as_float(ob[i + 0]) * inv_l, __uint_as_float(ob[i + 1]) * inv_l);
-            w.y = pack_bf16(__uint_as_float(ob[i + 2]) * inv_l, __uint_as_float(ob[i + 3]) * inv_l);
-            w.z = pack_bf16(__uint_as_float(ob[i + 4]) * inv_l, __uint_as_float(ob[i + 5]) * inv_l);
-            w.w = pack_bf16(__uint_as_float(ob[i + 6]) * inv_l, __uint_as_float(ob[i + 7]) * inv_l);
-            *reinterpret_cast<uint4*>(orow + c + i) = w;
-          }
+        for (int jn = 0; jn < NO / 8; ++jn) {
+          const int c = 8 * jn + 2 * (lane & 3);
+          if (c < p.d)
+            *reinterpret_cast<uint32_t*>(orow + c) = pack_bf16(o[4 * jn + 2 * r] * inv_l, o[4 * jn + 2 * r + 1] * inv_l);
         }
+        if (p.lse2 != nullptr && (lane & 3) == 0)
+          p.lse2[(static_cast<long>(b) * p.H + h) * p.n + q] = m_run[r] + log2f(l_run[r]);
       }
     }
-    if (q < p.n && p.lse2 != nullptr)
-      p.lse2[(static_cast<long>(b) * p.H + h) * p.n + q] = m_used + log2f(l_run);
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 4) {
-    tc_fence_after();
-    tmem_dealloc<256>(tmem_base);
   }
 }
 
@@ -267,7 +211,7 @@ int make_head_tmap(CUtensorMap* tm, const void* base, long ld, int B, int n, int
 template <int KA, int NO>
 static int launch_attn_fwd(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv,
                            const AttnFwdParams& p, cudaStream_t stream) {
-  constexpr int SMEM = KA * ATT_BQ * 128 + 4 * KA * ATT_BKV * 128 + ATT_BQ * 128 + 128;  // tiles + barriers
+  constexpr int SMEM = KA * ATT_BQ * 128 + 2 * ATT_NS * KA * ATT_BKV * 128 + 128;  // tiles + barriers
   auto kern = attn_fwd_kernel<KA, NO>;
   static bool attr_set[64] = {};
   if (first_use_on_device(attr_set)) {
@@ -275,18 +219,12 @@ static int launch_attn_fwd(const CUtensorMap& tq, const CUtensorMap& tk, const C
     if (e != cudaSuccess) return set_error_cuda("cudaFuncSetAttribute(attn_fwd)", e);
   }
   dim3 grid((p.n + ATT_BQ - 1) / ATT_BQ, p.H, p.B);
-  kern<<<grid, 192, SMEM, stream>>>(tq, tk, tv, p);
+  kern<<<grid, 384, SMEM, stream>>>(tq, tk, tv, p);
   count_launch();
   return check_launch("attn_fwd_kernel");
 }
 
 }  // namespace ivb
-
-namespace ivb {
-int attn_fwd2_dispatch(const void* q, long ldq, const void* k, long ldk, const void* v, long ldv, void* out,
-                       long ldo, float* lse2, int B, int n, int H, int d, float softmax_scale,
-                       cudaStream_t stream);
-}
 
 using namespace ivb;
 
@@ -297,10 +235,6 @@ extern "C" int ivb_attn_fwd(const void* q, long ldq, const void* k, long ldk, co
   if (B <= 0 || n <= 0) return 0;
   if (d % 8 != 0 || d > 128 || d < 16) return set_error("ivb_attn_fwd: head_dim must be a multiple of 8 in [16,128]");
   if ((ldq & 7) || (ldk & 7) || (ldv & 7) || (ldo & 7)) return set_error("ivb_attn_fwd: pitches must be multiples of 8");
-  // second-generation kernel (ivb_attn2.cu: persistent, 2 query tiles / CTA, 128-key tiles, P through TMEM);
-  // IVB_ATTN_FWD_V1=1 selects the first kernel below (kept as the comparison point of profiles/r02_attention_*.md)
-  static const bool use_v1 = [] { const char* e = getenv("IVB_ATTN_FWD_V1"); return e && e[0] == '1'; }();
-  if (!use_v1) return attn_fwd2_dispatch(q, ldq, k, ldk, v, ldv, out, ldo, lse2, B, n, H, d, softmax_scale, stream);
   CUtensorMap tq, tk, tv;
   int rc;
   if ((rc = make_head_tmap(&tq, q, ldq, B, n, H, d, ATT_BQ))) return rc;
@@ -310,11 +244,97 @@ extern "C" int ivb_attn_fwd(const void* q, long ldq, const void* k, long ldk, co
   p.B = B; p.n = n; p.H = H; p.d = d;
   p.sc_log2 = softmax_scale * 1.4426950408889634f;
   p.out = reinterpret_cast<__nv_bfloat16*>(out); p.ldo = ldo; p.lse2 = lse2;
-  const int no = (d + 15) / 16 * 16;
+  const int no = (d + 31) / 32 * 32;
   if (d <= 64) {
     if (no <= 32) return launch_attn_fwd<1, 32>(tq, tk, tv, p, stream);
     return launch_attn_fwd<1, 64>(tq, tk, tv, p, stream);
   }
   if (no <= 96) return launch_attn_fwd<2, 96>(tq, tk, tv, p, stream);
   return launch_attn_fwd<2, 128>(tq, tk, tv, p, stream);
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// Head-axis attention of the VideoMAEv2 teacher AS THE REFERENCE COMPUTES IT: videomae.py:94-97 hands
+// flash_attn_func q/k/v of shape [B, H, N, d] (after permute(2,0,3,1,4)), whereas FA2's convention is
+// [B, seqlen, nheads, d] — so the softmax runs over the H (= 16) heads of EACH TOKEN, not over the tokens, and the
+// [B, H, N, d] result is then reinterpreted by `.reshape(B, N, -1)`.  Reproduced here for drop-in parity (the
+// standard token-axis attention is the wgmma kernel above).  Tiny and HBM-bound: one warp per token stages the
+// token's q/k/v ([H, d] each) in shared memory, lane (i, half) owns score row i / key half.
+namespace ivb {
+
+template <int HMAX>
+__global__ void __launch_bounds__(128)
+headaxis_attn_kernel(const __nv_bfloat16* __restrict__ qkv, long ld, int B, int N, int H, int d, float scale,
+                     __nv_bfloat16* __restrict__ out) {
+  extern __shared__ __align__(16) uint8_t hsm[];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const long tok = static_cast<long>(blockIdx.x) * 4 + warp;
+  if (tok >= static_cast<long>(B) * N) return;
+  const int D = H * d;
+  __nv_bfloat16* sq = reinterpret_cast<__nv_bfloat16*>(hsm) + static_cast<long>(warp) * 3 * D;
+  __nv_bfloat16* sk = sq + D;
+  __nv_bfloat16* sv = sk + D;
+  const __nv_bfloat16* row = qkv + tok * ld;
+  for (int c = lane * 8; c < 3 * D; c += 256)
+    *reinterpret_cast<uint4*>(sq + c) = *reinterpret_cast<const uint4*>(row + c);
+  __syncwarp();
+  const int b = static_cast<int>(tok / N), t = static_cast<int>(tok % N);
+  // lane -> (i = lane % H ... ) : each lane owns one query head i = lane (lanes >= H idle); H <= 32
+  const int i = lane;
+  if (i < H) {
+    float s[HMAX];
+    float mx = -INFINITY;
+#pragma unroll
+    for (int j = 0; j < HMAX; ++j) {
+      if (j < H) {
+        float acc = 0.f;
+        for (int c = 0; c < d; c += 2) {
+          const float2 a = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(sq + i * d + c));
+          const float2 k2 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(sk + j * d + c));
+          acc += a.x * k2.x + a.y * k2.y;
+        }
+        s[j] = acc * scale;
+        mx = fmaxf(mx, s[j]);
+      }
+    }
+    float l = 0.f;
+#pragma unroll
+    for (int j = 0; j < HMAX; ++j)
+      if (j < H) { s[j] = __expf(s[j] - mx); l += s[j]; }
+    const float inv = 1.f / l;
+    __nv_bfloat16* o = out + ((static_cast<long>(b) * H + i) * N + t) * d;     // [B, H, N, d] contiguous
+    for (int c = 0; c < d; c += 2) {
+      float ox = 0.f, oy = 0.f;
+#pragma unroll
+      for (int j = 0; j < HMAX; ++j) {
+        if (j < H) {
+          const float2 v2 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(sv + j * d + c));
+          ox += s[j] * v2.x; oy += s[j] * v2.y;
+        }
+      }
+      *reinterpret_cast<__nv_bfloat162*>(o + c) = __floats2bfloat162_rn(ox * inv, oy * inv);
+    }
+  }
+}
+
+}  // namespace ivb
+
+extern "C" int ivb_headaxis_attn_fwd(const void* qkv, long ld, int B, int N, int H, int d, float softmax_scale,
+                                     void* out, void* stream_) {
+  using namespace ivb;
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  if (B <= 0 || N <= 0) return 0;
+  if (H > 32 || H < 1) return set_error("ivb_headaxis_attn_fwd: 1 <= heads <= 32");
+  if ((d & 7) || (ld & 7)) return set_error("ivb_headaxis_attn_fwd: head_dim / pitch must be multiples of 8");
+  const long toks = static_cast<long>(B) * N;
+  const size_t smem = static_cast<size_t>(4) * 3 * H * d * sizeof(__nv_bfloat16);
+  auto kern = H <= 16 ? headaxis_attn_kernel<16> : headaxis_attn_kernel<32>;
+  if (smem > 48 * 1024) {
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return set_error_cuda("cudaFuncSetAttribute(headaxis_attn)", e);
+  }
+  kern<<<(unsigned)((toks + 3) / 4), 128, smem, stream>>>(reinterpret_cast<const __nv_bfloat16*>(qkv), ld, B, N, H, d,
+                                                          softmax_scale, reinterpret_cast<__nv_bfloat16*>(out));
+  count_launch();
+  return check_launch("headaxis_attn_kernel");
 }

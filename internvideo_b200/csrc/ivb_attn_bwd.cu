@@ -1,4 +1,4 @@
-// ivb_attn_bwd.cu — attention backward on tcgen05 (two passes, no atomics, recompute of P from lse).
+// ivb_attn_bwd.cu — attention backward on Hopper wgmma (two passes, no atomics, recompute of P from lse).
 //
 // Stands in for FA2's backward of flash_attn_varlen_qkvpacked_func (the autograd of
 // FlashAttention.forward, flash_attention_class.py:47-50) / autograd of _naive_attn
@@ -6,34 +6,20 @@
 //
 //   delta[q]   = sum_d dO[q,d] * O[q,d]                                  (attn_bwd_prep_kernel)
 //   MODE 1 (dK,dV): CTA owns 128 keys; streams 64-query tiles:
-//        S^T = K Q_i^T, dP^T = V dO_i^T      (TMEM, lane = key)
+//        S^T = K Q_i^T, dP^T = V dO_i^T      (register accumulators, row = key)
 //        P^T = exp2(S^T*sc - lse2[q]),  dS^T = P^T * (dP^T - delta[q]) * scale
-//        dV += P^T dO_i,  dK += dS^T Q_i     (Q_i / dO_i tiles re-used as MN-major B operands)
+//        dV += P^T dO_i,  dK += dS^T Q_i     (P^T / dS^T from registers, Q_i / dO_i tiles as MN-major B operands)
 //   MODE 0 (dQ):    CTA owns 128 queries; streams 64-key tiles:
 //        S = Q K_j^T, dP = dO V_j^T;  dS = P * (dP - delta[q]) * scale;  dQ += dS K_j
 // Transposed operands are never materialised: the same 128B-swizzled TMA tile [rows x 64 cols] is a
 // K-major operand (rows = M/N index) for one MMA and an MN-major operand (rows = K index) for the
-// other, only the UMMA descriptor differs.
+// other, only the wgmma descriptor differs.
 //
-// Warp roles (320 threads): warps 0-7 = math (warps w and w+4 share 32 TMEM lanes = rows and split the
-// 64 streamed columns in halves; the backward has no row reductions so the split is free), warp 8 = the
-// single-thread tcgen05.mma issuer, warp 9 = the TMA producer.  The first version let thread 0 of a math
-// warp issue the MMAs and TMA loads; ncu showed every other warp parked on the per-tile CTA barrier
-// behind that thread's serial descriptor/issue work (28 % of stall samples), so issue and math are now
-// decoupled and talk only through mbarriers:
-//   bar_col[s]  TMA -> issuer     streamed tile s landed          (tx)
-//   bar_free[s] issuer -> TMA     accumulate MMAs of the tile in stage s retired (tcgen05.commit)
-//   bar_s[b]    issuer -> math    score MMAs of the tile in TMEM buffer b retired
-//   bar_t[b]    math -> issuer    P^T / dS^T tiles of a tile with parity b written to smem buffer b, S/dP
-//                                 buffer b drained (8 warp arrivals)
-//   bar_a[b]    issuer -> math    accumulate MMAs of that tile retired: smem buffer b reusable / accumulators final
-//   bar_row     TMA -> issuer     X,Y (the 128 owned rows) of the current work item landed
-//   bar_xfree   issuer -> TMA     the item's last score MMAs retired: X,Y may be overwritten by the next item
-//   bar_e       math -> issuer    the item's accumulators were drained to global (8 warp arrivals)
-// The bf16 P^T/dS^T tiles are double-buffered so the math warps of tile i+1 never wait for the accumulate
-// MMAs of tile i, and (MODE 1) the per-query lse/delta of a streamed tile arrive with it by bulk copy.
-// The kernel is persistent (one CTA per SM walks the (clip, head, 128-row) items; see the kernel comment);
-// "CTA owns" above reads "work item owns".
+// Warp roles (384 threads): warpgroup 0 = the TMA producer (one elected thread), warpgroups 1 and 2 own 64 of the
+// 128 rows each.  mbarriers only:
+//   bar_row     TMA -> MMA        X,Y (the 128 owned rows) landed
+//   full[s]     TMA -> MMA        streamed tiles U_j, W_j of stage s landed (tx)
+//   empty[s]    MMA -> TMA        both warpgroups retired every MMA that reads stage s
 #include <math.h>
 #include <stdlib.h>
 
@@ -45,7 +31,7 @@ namespace ivb {
 int make_head_tmap(CUtensorMap* tm, const void* base, long ld, int B, int n, int H, int d,
                    int box_tokens);
 
-constexpr int BWD_ROWS = 128;  // rows owned by the CTA (UMMA M)
+constexpr int BWD_ROWS = 128;  // rows owned by the CTA (two warpgroups of 64)
 constexpr int BWD_COLS = 64;   // streamed tile
 
 struct AttnBwdParams {
@@ -85,362 +71,182 @@ __global__ void attn_bwd_prep_kernel(const __nv_bfloat16* __restrict__ o, long l
   lse2p[(b * H + h) * n_pad + q] = lse2[(b * H + h) * n + q];
 }
 
-__device__ __forceinline__ void bwd_tmem_st16(uint32_t taddr, const uint32_t* r) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-      "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-__device__ __forceinline__ void bwd_tmem_st8(uint32_t taddr, const uint32_t* r) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"r"(taddr),
-               "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-               : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem]; A is K-major in tensor memory (row i = lane i, two bf16 per 32-bit column).
-__device__ __forceinline__ void bwd_umma_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t bdesc, uint32_t idesc,
-                                            uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}\n" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
+constexpr int BWD_NST = 2;  // streamed-tile stages
 
-// NXB: row-operand (X,Y) buffers (1 or 2); NST: streamed-tile stages.  Shared memory holds either 2 x (X,Y) + 3 stages
-// or 1 x (X,Y) + 5 stages at head_dim > 64: a deeper ring hides the TMA refill latency of the streamed tiles (a stage
-// is refilled only after the tile NST-1 positions earlier retired), a second X,Y buffer hides the item boundary.
-// NCG: column groups = math warps per TMEM lane quadrant (2 or 4).  The math warps are latency-bound (ncu: issue slots
-// 44 % busy with two warps per SM sub-partition); with NCG = 4 sixteen math warps take 16 of the 64 streamed columns each.
-template <int MODE, int KA, int NO, int NXB, int NST, int NCG>
-__global__ void __launch_bounds__(64 + 128 * NCG, 1)
+// KA: 64-wide atoms covering head_dim (1: d <= 64, 2: d <= 128); NO: wgmma N of the accumulate MMAs.
+template <int MODE, int KA, int NO>
+__global__ void __launch_bounds__(384, 1)
 attn_bwd_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmY,
                 const __grid_constant__ CUtensorMap tmU, const __grid_constant__ CUtensorMap tmW,
                 const AttnBwdParams p) {
-  // X,Y: row operands (128 rows).  U,W: streamed operands (64 rows per tile).
-  // MODE 0: X=Q Y=dO U=K W=V.   MODE 1: X=K Y=V U=Q W=dO.
-  //
-  // PERSISTENT, CONTINUOUS: one CTA per SM walks work items (b, h, 128-row tile), item = blockIdx.x + k * gridDim.x, and
-  // every ring (smem stages, TMEM score buffers) runs on a GLOBAL tile counter G across items.  Round 2:
-  //   * the bf16 P^T / dS^T tiles no longer go through shared memory: the math warps write them back to TENSOR MEMORY over
-  //     the score columns they were computed from (tcgen05.st) and the accumulate MMAs take them as TMEM A operands — no
-  //     swizzled st.shared, no generic->async proxy fence, and 32-64 KB of shared memory freed;
-  //   * that memory double-buffers the item's row operands X,Y: the next item's rows are resident before the current
-  //     item ends, so the issuer keeps its steady pattern (accumulate tile G, then scores of tile G+2) ACROSS the item
-  //     boundary instead of refilling the pipeline per item (6.2 us of 12.4 us per item were fixed cost at n = 417).
-  constexpr int ROW_BYTES = KA * BWD_ROWS * 128;
-  constexpr int COL_BYTES = KA * BWD_COLS * 128;
+  constexpr int ROW_BYTES = KA * BWD_ROWS * 128;   // one owned-row operand
+  constexpr int COL_BYTES = KA * BWD_COLS * 128;   // one streamed tile
   extern __shared__ __align__(1024) uint8_t smem[];
-  uint8_t* sX = smem;                              // NXB item buffers
-  uint8_t* sY = sX + NXB * ROW_BYTES;              // NXB item buffers
-  uint8_t* sU = sY + NXB * ROW_BYTES;              // NST stages
-  uint8_t* sW = sU + NST * COL_BYTES;       // NST stages
-  float* sStat = reinterpret_cast<float*>(sW + NST * COL_BYTES);   // MODE1: [stage][lse2 64 | delta 64]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(sStat) + NST * 512);
-  constexpr int S = NST;
-  uint64_t* bar_row = bars;                  // 2   X,Y of an item landed in buffer (k&1)
-  uint64_t* bar_xfree = bars + 2;            // 2   all score MMAs of the item in buffer (k&1) retired
-  uint64_t* bar_col = bars + 4;              // S   streamed tile g landed                     (ring on g)
-  uint64_t* bar_free = bars + 4 + S;         // S   accumulate MMAs of tile g retired
-  uint64_t* bar_s = bars + 4 + 2 * S;        // 2   score MMAs of tile g retired
-  uint64_t* bar_t = bars + 6 + 2 * S;        // 2   (8 arrivals each) P^T/dS^T of tile g in TMEM, S/dP drained
-  uint64_t* bar_a = bars + 8 + 2 * S;        // 2   accumulate MMAs of tile g retired
-  uint64_t* bar_e = bars + 10 + 2 * S;       // 1   (8 arrivals) accumulators of item k drained  (phase per item)
-  constexpr int NBARS = 11 + 2 * S;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + NBARS);
+  uint8_t* sX = smem;
+  uint8_t* sY = sX + ROW_BYTES;
+  uint8_t* sU = sY + ROW_BYTES;                 // BWD_NST stages
+  uint8_t* sW = sU + BWD_NST * COL_BYTES;       // BWD_NST stages
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sW + BWD_NST * COL_BYTES);
+  uint64_t* bar_row = bars;
+  uint64_t* full = bars + 1;
+  uint64_t* empty = full + BWD_NST;
 
   const int tid = threadIdx.x;
   const int warp = tid >> 5;
   const int lane = tid & 31;
-  const int ntile = (p.n + BWD_COLS - 1) / BWD_COLS;
+  const int wg = tid >> 7;
+  const int r0 = blockIdx.x * BWD_ROWS;
+  const int h = blockIdx.y;
+  const int b = blockIdx.z;
+  const int nblk = (p.n + BWD_COLS - 1) / BWD_COLS;
   const int ksteps = (p.d + 15) / 16;
-  const int rt_per = (p.n + BWD_ROWS - 1) / BWD_ROWS;
-  const int items = rt_per * p.H * p.B;
-  const int my_items = (items - static_cast<int>(blockIdx.x) + static_cast<int>(gridDim.x) - 1) / static_cast<int>(gridDim.x);
 
   if (tid == 0) {
     if ((smem_u32(smem) & 1023u) != 0) __trap();
-    for (int i = 0; i < NBARS; ++i)
-      mbar_init(&bars[i], (i == 6 + 2 * S || i == 7 + 2 * S || i == 10 + 2 * S) ? 4 * NCG : 1);
+    mbar_init(bar_row, 1);
+    for (int i = 0; i < BWD_NST; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 2); }
     fence_mbar_init();
   }
-  constexpr int W_MMA = 4 * NCG, W_TMA = 4 * NCG + 1;     // warp roles: math 0 .. 4*NCG-1, then issuer, then producer
-  constexpr int CW = BWD_COLS / NCG;                      // streamed columns per math thread
-  if (warp == W_MMA) tmem_alloc<512>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_wait();
   pdl_launch_dependents();
-  const uint32_t tS = tmem_base;          // 2 x 64   (P^T of a tile is written back over its own S columns)
-  const uint32_t tP = tmem_base + 128;    // 2 x 64   (dS^T / dS over the dP columns)
-  const uint32_t tA1 = tmem_base + 256;   // NO
-  const uint32_t tA2 = tmem_base + 384;   // NO (MODE 1)
 
-  if (warp == W_TMA) {
+  if (wg == 0) {
+    setmaxnreg_dec<24>();
     // ===================== TMA producer =====================
-    if (elect_one()) {
+    if (warp == 0 && elect_one()) {
       tma_prefetch_desc(&tmX); tma_prefetch_desc(&tmY); tma_prefetch_desc(&tmU); tma_prefetch_desc(&tmW);
-      int g = 0;
-      for (int k = 0; k < my_items; ++k) {
-        const int item = blockIdx.x + k * gridDim.x;
-        const int r0 = (item % rt_per) * BWD_ROWS;
-        const int h = (item / rt_per) % p.H;
-        const int b = item / (rt_per * p.H);
-        const int xb = k % NXB;
-        if (k >= NXB) mbar_wait(&bar_xfree[xb], ((k / NXB) - 1) & 1);   // score MMAs of item k-NXB no longer read this buffer
-        mbar_expect_tx(&bar_row[xb], 2 * ROW_BYTES);
+      mbar_expect_tx(bar_row, 2 * ROW_BYTES);
+#pragma unroll
+      for (int a = 0; a < KA; ++a) {
+        tma_load_4d(sX + a * (BWD_ROWS * 128), &tmX, a * 64, h, r0, b, bar_row);
+        tma_load_4d(sY + a * (BWD_ROWS * 128), &tmY, a * 64, h, r0, b, bar_row);
+      }
+      for (int j = 0; j < nblk; ++j) {
+        const int st = j % BWD_NST;
+        mbar_wait(&empty[st], ((j / BWD_NST) & 1) ^ 1);
+        mbar_expect_tx(&full[st], 2 * COL_BYTES);
 #pragma unroll
         for (int a = 0; a < KA; ++a) {
-          tma_load_4d(sX + xb * ROW_BYTES + a * (BWD_ROWS * 128), &tmX, a * 64, h, r0, b, &bar_row[xb]);
-          tma_load_4d(sY + xb * ROW_BYTES + a * (BWD_ROWS * 128), &tmY, a * 64, h, r0, b, &bar_row[xb]);
+          tma_load_4d(sU + st * COL_BYTES + a * (BWD_COLS * 128), &tmU, a * 64, h, j * BWD_COLS, b, &full[st]);
+          tma_load_4d(sW + st * COL_BYTES + a * (BWD_COLS * 128), &tmW, a * 64, h, j * BWD_COLS, b, &full[st]);
         }
-        for (int i = 0; i < ntile; ++i, ++g) {
-          const int st = g % NST;
-          if (g >= NST) mbar_wait(&bar_free[st], ((g / NST) - 1) & 1);  // tile g-STAGES fully consumed
-          mbar_expect_tx(&bar_col[st], 2 * COL_BYTES + (MODE == 1 ? 512 : 0));
-          if (MODE == 1) {   // per-query statistics of the streamed tile (padded workspace: always 64 in-bounds floats)
-            const long so = (static_cast<long>(b) * p.H + h) * p.n_pad + i * BWD_COLS;
-            bulk_load_1d(sStat + st * 128, p.lse2p + so, 256, &bar_col[st]);
-            bulk_load_1d(sStat + st * 128 + 64, p.deltap + so, 256, &bar_col[st]);
-          }
-#pragma unroll
-          for (int a = 0; a < KA; ++a) {
-            tma_load_4d(sU + st * COL_BYTES + a * (BWD_COLS * 128), &tmU, a * 64, h, i * BWD_COLS, b, &bar_col[st]);
-            tma_load_4d(sW + st * COL_BYTES + a * (BWD_COLS * 128), &tmW, a * 64, h, i * BWD_COLS, b, &bar_col[st]);
-          }
-        }
-      }
-    }
-  } else if (warp == W_MMA) {
-    // ===================== MMA issuer =====================
-    if (elect_one()) {
-      constexpr uint32_t idesc_s = umma_idesc_bf16(BWD_ROWS, BWD_COLS, false, false);
-      constexpr uint32_t idesc_a = umma_idesc_bf16(BWD_ROWS, NO, false, true);
-      const int total = my_items * ntile;
-      // score MMAs of global tile G = (item k = G / ntile, tile i = G % ntile)
-      auto issue_scores = [&](int G) {
-        const int k = G / ntile, i = G - k * ntile;
-        const int xb = k % NXB;
-        const int st = G % NST;
-        const int buf = G & 1;
-        if (i == 0) mbar_wait(&bar_row[xb], (k / NXB) & 1);      // the item's X,Y landed
-        mbar_wait(&bar_col[st], (G / NST) & 1);
-        tc_fence_after();
-        const uint32_t xa = smem_u32(sX + xb * ROW_BYTES), ya = smem_u32(sY + xb * ROW_BYTES);
-        const uint32_t ua = smem_u32(sU + st * COL_BYTES), wa = smem_u32(sW + st * COL_BYTES);
-        for (int kk = 0; kk < ksteps; ++kk) {
-          const uint32_t ro = (kk >> 2) * (BWD_ROWS * 128) + (kk & 3) * 32;
-          const uint32_t co = (kk >> 2) * (BWD_COLS * 128) + (kk & 3) * 32;
-          umma_bf16(tS + buf * 64, umma_desc(xa + ro, 16, 1024), umma_desc(ua + co, 16, 1024), idesc_s, kk > 0);
-        }
-        for (int kk = 0; kk < ksteps; ++kk) {
-          const uint32_t ro = (kk >> 2) * (BWD_ROWS * 128) + (kk & 3) * 32;
-          const uint32_t co = (kk >> 2) * (BWD_COLS * 128) + (kk & 3) * 32;
-          umma_bf16(tP + buf * 64, umma_desc(ya + ro, 16, 1024), umma_desc(wa + co, 16, 1024), idesc_s, kk > 0);
-        }
-        umma_commit(&bar_s[buf]);
-        if (i == ntile - 1) umma_commit(&bar_xfree[xb]);
-      };
-      // both S/dP buffers are free at the start; afterwards scores(G+2) follow the accumulate MMAs of tile G, whose
-      // TMEM A operands alias the score buffer (G&1): the tensor pipe executes them in issue order
-      if (total > 0) issue_scores(0);
-      if (total > 1) issue_scores(1);
-      for (int G = 0; G < total; ++G) {
-        const int k = G / ntile, i = G - k * ntile;
-        const int st = G % NST;
-        const int buf = G & 1;
-        mbar_wait(&bar_t[buf], (G >> 1) & 1);   // math wrote P^T/dS^T of tile G into TMEM (and drained S/dP)
-        if (i == 0 && k > 0) mbar_wait(bar_e, (k - 1) & 1);   // previous item's accumulators drained to global
-        tc_fence_after();
-        const uint32_t ua = smem_u32(sU + st * COL_BYTES), wa = smem_u32(sW + st * COL_BYTES);
-        // packed bf16 A operands: the CW streamed rows of column group g sit at columns [g*CW, g*CW + CW/2) of the tile's
-        // score buffer (each math warp writes over ITS OWN score columns); one MMA consumes 16 K values = 8 columns
-        auto acol = [](int kk) -> uint32_t { return static_cast<uint32_t>(((kk * 16) / CW) * CW + ((kk * 16) % CW) / 2); };
-        if (MODE == 0) {  // dQ += dS K_j
-#pragma unroll
-          for (int kk = 0; kk < BWD_COLS / 16; ++kk)
-            bwd_umma_ts(tA1, tP + buf * 64 + acol(kk),
-                        umma_desc(ua + kk * 2048, BWD_COLS * 128, 1024), idesc_a, (i > 0 || kk > 0) ? 1u : 0u);
-        } else {          // dV += P^T dO_i ; dK += dS^T Q_i
-#pragma unroll
-          for (int kk = 0; kk < BWD_COLS / 16; ++kk)
-            bwd_umma_ts(tA1, tS + buf * 64 + acol(kk),
-                        umma_desc(wa + kk * 2048, BWD_COLS * 128, 1024), idesc_a, (i > 0 || kk > 0) ? 1u : 0u);
-#pragma unroll
-          for (int kk = 0; kk < BWD_COLS / 16; ++kk)
-            bwd_umma_ts(tA2, tP + buf * 64 + acol(kk),
-                        umma_desc(ua + kk * 2048, BWD_COLS * 128, 1024), idesc_a, (i > 0 || kk > 0) ? 1u : 0u);
-        }
-        umma_commit(&bar_free[st]);   // stage st reusable by the producer
-        umma_commit(&bar_a[buf]);     // accumulators final after the item's last tile
-        if (G + 2 < total) issue_scores(G + 2);   // into TMEM buffer (G&1), behind the MMAs that read it
       }
     }
   } else {
-    // ===================== math warps (0..7) =====================
-    const int hc = warp >> 2;            // column group: columns [hc*CW, hc*CW + CW) of the streamed tile
-    const int r = (warp & 3) * 32 + lane;   // row inside the CTA tile == TMEM lane
-    const uint32_t lane_off = static_cast<uint32_t>((warp & 3) * 32) << 16;
+    setmaxnreg_inc<240>();
+    // ===================== MMA + math warpgroups =====================
+    const int cw = wg - 1;
+    const bool signal = (tid & 127) == 0;
+    const int rloc = cw * 64 + (warp & 3) * 16 + (lane >> 2);  // this thread's rows: rloc, rloc + 8
+    const uint32_t xa = smem_u32(sX) + cw * 8192, ya = smem_u32(sY) + cw * 8192;
+    const long hb = (static_cast<long>(b) * p.H + h) * p.n_pad;
+    float acc1[NO / 2];                     // MODE 1: dV   MODE 0: dQ
+    float acc2[MODE == 1 ? NO / 2 : 1];     // MODE 1: dK
+#pragma unroll
+    for (int i = 0; i < NO / 2; ++i) acc1[i] = 0.f;
+#pragma unroll
+    for (int i = 0; i < (MODE == 1 ? NO / 2 : 1); ++i) acc2[i] = 0.f;
+    float row_lse[2] = {0.f, 0.f}, row_delta[2] = {0.f, 0.f};
+    if (MODE == 0) {
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        const int q = r0 + rloc + 8 * r;
+        if (q < p.n_pad) { row_lse[r] = p.lse2p[hb + q]; row_delta[r] = p.deltap[hb + q]; }
+      }
+    }
 
-    int g0 = 0;
-    for (int k = 0; k < my_items; ++k, g0 += ntile) {
-      const int item = blockIdx.x + k * gridDim.x;
-      const int r0 = (item % rt_per) * BWD_ROWS;
-      const int h = (item / rt_per) % p.H;
-      const int b = item / (rt_per * p.H);
-      const int row = r0 + r;
-      const long stat_base = (static_cast<long>(b) * p.H + h) * p.n_pad;
-      float row_l2 = 0.f, row_dl = 0.f;
-      if (MODE == 0 && row < p.n) { row_l2 = p.lse2p[stat_base + row]; row_dl = p.deltap[stat_base + row]; }
-      const float row_dls = row_dl * p.scale;
+    mbar_wait(bar_row, 0);
+    for (int j = 0; j < nblk; ++j) {
+      const int st = j % BWD_NST;
+      mbar_wait(&full[st], (j / BWD_NST) & 1);
+      const uint32_t ua = smem_u32(sU + st * COL_BYTES), wa = smem_u32(sW + st * COL_BYTES);
+      float sc[BWD_COLS / 2], dp[BWD_COLS / 2];
+      wgmma_fence();
+      for (int kk = 0; kk < ksteps; ++kk) {
+        const uint32_t off = (kk & 3) * 32;
+        const uint32_t ro = (kk >> 2) * (BWD_ROWS * 128) + off, co = (kk >> 2) * (BWD_COLS * 128) + off;
+        Wgmma<BWD_COLS>::ss<0, 0>(sc, gmma_desc(xa + ro, 16, 1024), gmma_desc(ua + co, 16, 1024), kk > 0 ? 1u : 0u);
+        Wgmma<BWD_COLS>::ss<0, 0>(dp, gmma_desc(ya + ro, 16, 1024), gmma_desc(wa + co, 16, 1024), kk > 0 ? 1u : 0u);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_reg_fence(sc, BWD_COLS / 2);
+      wgmma_reg_fence(dp, BWD_COLS / 2);
 
-      for (int i = 0; i < ntile; ++i) {
-        const int G = g0 + i;
-        const int buf = G & 1;
-        const int st = G % NST;
-        const float* cl2 = sStat + st * 128 + hc * CW;
-        const float* cdl = cl2 + 64;
-        if (MODE == 1) mbar_wait(&bar_col[st], (G / NST) & 1);
-        mbar_wait(&bar_s[buf], (G >> 1) & 1);
-        tc_fence_after();
-        const uint32_t tSc = tS + lane_off + buf * 64 + hc * CW;
-        const uint32_t tPc = tP + lane_off + buf * 64 + hc * CW;
-        uint32_t sb[CW], db[CW];
-        if (CW == 32) { tmem_ld32(tSc, sb); tmem_ld32(tPc, db); } else { tmem_ld16(tSc, sb); tmem_ld16(tPc, db); }
-        tmem_wait_ld();
-        const int valid = p.n - i * BWD_COLS - hc * CW;   // local columns >= valid are beyond the sequence
-        if (valid >= CW) {           // full tile (all but the sequence tail): no masking selects
+      // P and dS in place of S and dP.  Columns beyond the sequence get P = 0.
 #pragma unroll
-          for (int c = 0; c < CW; ++c) {
-            const float l2 = (MODE == 0) ? row_l2 : cl2[c];
-            sb[c] = __float_as_uint(exp2f(fmaf(__uint_as_float(sb[c]), p.sc_log2, -l2)));
-          }
-        } else {
+      for (int i = 0; i < BWD_COLS / 2; ++i) {
+        const int col = j * BWD_COLS + 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
+        float lse, dl;
+        if (MODE == 1) { lse = p.lse2p[hb + col]; dl = p.deltap[hb + col]; }
+        else { lse = row_lse[(i >> 1) & 1]; dl = row_delta[(i >> 1) & 1]; }
+        const float pv = col < p.n ? exp2f(fmaf(sc[i], p.sc_log2, -lse)) : 0.f;
+        sc[i] = pv;
+        dp[i] = pv * (dp[i] - dl) * p.scale;
+      }
+      wgmma_fence();
 #pragma unroll
-          for (int c = 0; c < CW; ++c) {
-            const float l2 = (MODE == 0) ? row_l2 : cl2[c];
-            float pv = exp2f(fmaf(__uint_as_float(sb[c]), p.sc_log2, -l2));
-            if (c >= valid) pv = 0.f;
-            sb[c] = __float_as_uint(pv);
-          }
-        }
-        // dS = P * (dP - delta) * scale = P * fma(dP, scale, -delta*scale)
-        uint32_t pk[CW / 2];
-#pragma unroll
-        for (int c = 0; c < CW; c += 2) {
-          const float dl0 = (MODE == 0) ? row_dls : cdl[c] * p.scale;
-          const float dl1 = (MODE == 0) ? row_dls : cdl[c + 1] * p.scale;
-          const float e0 = __uint_as_float(sb[c]) * fmaf(__uint_as_float(db[c]), p.scale, -dl0);
-          const float e1 = __uint_as_float(sb[c + 1]) * fmaf(__uint_as_float(db[c + 1]), p.scale, -dl1);
-          pk[c >> 1] = pack_bf16(e0, e1);
-        }
-        if (CW == 32) bwd_tmem_st16(tPc, pk); else bwd_tmem_st8(tPc, pk);   // dS^T (MODE 1) / dS (MODE 0) over this warp's own dP columns
+      for (int kk = 0; kk < BWD_COLS / 16; ++kk) {
+        uint32_t fa[4];
         if (MODE == 1) {
-#pragma unroll
-          for (int c = 0; c < CW; c += 2) pk[c >> 1] = pack_bf16(__uint_as_float(sb[c]), __uint_as_float(sb[c + 1]));
-          if (CW == 32) bwd_tmem_st16(tSc, pk); else bwd_tmem_st8(tSc, pk);   // P^T over this warp's own S columns
+          acc_to_a_frag(sc, kk, fa);
+          Wgmma<NO>::rs<1>(acc1, fa, gmma_desc(wa + kk * 2048, BWD_COLS * 128, 1024), 1u);   // dV += P^T dO
+          acc_to_a_frag(dp, kk, fa);
+          Wgmma<NO>::rs<1>(acc2, fa, gmma_desc(ua + kk * 2048, BWD_COLS * 128, 1024), 1u);   // dK += dS^T Q
+        } else {
+          acc_to_a_frag(dp, kk, fa);
+          Wgmma<NO>::rs<1>(acc1, fa, gmma_desc(ua + kk * 2048, BWD_COLS * 128, 1024), 1u);   // dQ += dS K
         }
-        tmem_wait_st();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&bar_t[buf]);
       }
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_reg_fence(acc1, NO / 2);
+      if (MODE == 1) wgmma_reg_fence(acc2, NO / 2);
+      if (signal) mbar_arrive(&empty[st]);
+    }
 
-      // ---- item epilogue: accumulators final once the accumulate MMAs of the item's last tile retired (commits are
-      // cumulative: bar_a of the last tile covers every earlier MMA)
-      {
-        const int GL = g0 + ntile - 1;
-        mbar_wait(&bar_a[GL & 1], (GL >> 1) & 1);
-        tc_fence_after();
-      }
-#pragma unroll 1
-      for (int which = 0; which < (MODE == 1 ? 2 : 1); ++which) {
-        __nv_bfloat16* base = which == 0 ? p.out1 : p.out2;
-        const long ld = which == 0 ? p.ld1 : p.ld2;
-        __nv_bfloat16* orow = base + (static_cast<long>(b) * p.n + row) * ld + h * p.d;
-        const uint32_t ta = which == 0 ? tA1 : tA2;
-#pragma unroll 1
-        for (int c = hc * 32; c < NO; c += 32 * NCG) {   // the column groups alternate 32-column chunks
-          uint32_t ob[32];
-          tmem_ld32(ta + lane_off + c, ob);
-          tmem_wait_ld();
-          if (row < p.n) {
 #pragma unroll
-            for (int kq = 0; kq < 32; kq += 8) {
-              if (c + kq < p.d) {
-                uint4 w;
-                w.x = pack_bf16(__uint_as_float(ob[kq + 0]), __uint_as_float(ob[kq + 1]));
-                w.y = pack_bf16(__uint_as_float(ob[kq + 2]), __uint_as_float(ob[kq + 3]));
-                w.z = pack_bf16(__uint_as_float(ob[kq + 4]), __uint_as_float(ob[kq + 5]));
-                w.w = pack_bf16(__uint_as_float(ob[kq + 6]), __uint_as_float(ob[kq + 7]));
-                *reinterpret_cast<uint4*>(orow + c + kq) = w;
-              }
-            }
-          }
+    for (int r = 0; r < 2; ++r) {
+      const int row = r0 + rloc + 8 * r;
+      if (row >= p.n) continue;
+      __nv_bfloat16* o1 = p.out1 + (static_cast<long>(b) * p.n + row) * p.ld1 + h * p.d;
+      __nv_bfloat16* o2 = MODE == 1 ? p.out2 + (static_cast<long>(b) * p.n + row) * p.ld2 + h * p.d : nullptr;
+#pragma unroll
+      for (int jn = 0; jn < NO / 8; ++jn) {
+        const int c = 8 * jn + 2 * (lane & 3);
+        if (c < p.d) {
+          *reinterpret_cast<uint32_t*>(o1 + c) = pack_bf16(acc1[4 * jn + 2 * r], acc1[4 * jn + 2 * r + 1]);
+          if (MODE == 1)
+            *reinterpret_cast<uint32_t*>(o2 + c) = pack_bf16(acc2[4 * jn + 2 * r], acc2[4 * jn + 2 * r + 1]);
         }
       }
-      tc_fence_before();      // accumulator reads (tcgen05.ld) ordered before the arrive: the issuer may overwrite them
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_e);
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == W_MMA) {
-    tc_fence_after();
-    tmem_dealloc<512>(tmem_base);
-  }
-}
-
-template <int MODE, int KA, int NO, int NXB, int NST, int NCG>
-static int launch_attn_bwd_cfg(const CUtensorMap& tx, const CUtensorMap& ty, const CUtensorMap& tu,
-                               const CUtensorMap& tw, const AttnBwdParams& p, cudaStream_t stream) {
-  constexpr int SMEM = 2 * NXB * KA * BWD_ROWS * 128 + 2 * NST * KA * BWD_COLS * 128 + NST * 512 + 256;
-  static_assert(SMEM <= 227 * 1024, "attention backward: shared-memory budget");
-  auto kern = attn_bwd_kernel<MODE, KA, NO, NXB, NST, NCG>;
-  static bool attr_set[64] = {};
-  if (first_use_on_device(attr_set)) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM);
-    if (e != cudaSuccess) return set_error_cuda("cudaFuncSetAttribute(attn_bwd)", e);
-  }
-  const long items = (long)((p.n + BWD_ROWS - 1) / BWD_ROWS) * p.H * p.B;
-  const int grid = (int)(items < num_sms() ? items : num_sms());   // persistent: one CTA per SM
-  cudaError_t le = launch_pdl(kern, dim3(grid), dim3(64 + 128 * NCG), SMEM, stream, tx, ty, tu, tw, p);
-  if (le != cudaSuccess) return set_error_cuda("launch(attn_bwd_kernel)", le);
-  count_launch();
-  return check_launch("attn_bwd_kernel");
 }
 
 template <int MODE, int KA, int NO>
 static int launch_attn_bwd(const CUtensorMap& tx, const CUtensorMap& ty, const CUtensorMap& tu,
                            const CUtensorMap& tw, const AttnBwdParams& p, cudaStream_t stream) {
-  // two (X,Y) buffers + a 3 / 6-deep streamed ring for short sequences (the item boundary matters: cfg-2 321 vs 347 us),
-  // one (X,Y) buffer + a 5 / 8-deep ring from 2048 tokens on (the refill latency matters: n = 12544 4.03 vs 4.21 ms);
-  // IVB_ATTN_BWD_RING=deep|shallow overrides
-  static const int force = [] { const char* e = getenv("IVB_ATTN_BWD_RING"); return !e ? 0 : (e[0] == 'd' ? 1 : (e[0] == 's' ? 2 : 0)); }();
-  const bool deep = force == 1 || (force == 0 && p.n >= 2048);
-  // IVB_ATTN_BWD_WARPS=16: sixteen math warps (4 column groups); default 8
-  static const bool w16 = [] { const char* e = getenv("IVB_ATTN_BWD_WARPS"); return e && e[0] == '1' && e[1] == '6'; }();
-#define IVB_BWD_CFG(NXB_, NST_)                                                                                 \
-  (w16 ? launch_attn_bwd_cfg<MODE, KA, NO, NXB_, NST_, 4>(tx, ty, tu, tw, p, stream)                            \
-       : launch_attn_bwd_cfg<MODE, KA, NO, NXB_, NST_, 2>(tx, ty, tu, tw, p, stream))
-  if constexpr (KA == 2) {
-    return deep ? IVB_BWD_CFG(1, 5) : IVB_BWD_CFG(2, 3);
-  } else {
-    return deep ? IVB_BWD_CFG(1, 8) : IVB_BWD_CFG(2, 6);
+  constexpr int SMEM = 2 * KA * BWD_ROWS * 128 + 2 * BWD_NST * KA * BWD_COLS * 128 + 128;
+  static_assert(SMEM <= 227 * 1024, "attention backward: shared-memory budget");
+  auto kern = attn_bwd_kernel<MODE, KA, NO>;
+  static bool attr_set[64] = {};
+  if (first_use_on_device(attr_set)) {
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM);
+    if (e != cudaSuccess) return set_error_cuda("cudaFuncSetAttribute(attn_bwd)", e);
   }
-#undef IVB_BWD_CFG
+  dim3 grid((p.n + BWD_ROWS - 1) / BWD_ROWS, p.H, p.B);
+  cudaError_t le = launch_pdl(kern, grid, dim3(384), SMEM, stream, tx, ty, tu, tw, p);
+  if (le != cudaSuccess) return set_error_cuda("launch(attn_bwd_kernel)", le);
+  count_launch();
+  return check_launch("attn_bwd_kernel");
 }
 
 template <int MODE>
 static int dispatch_bwd(int d, const CUtensorMap& tx, const CUtensorMap& ty, const CUtensorMap& tu,
                         const CUtensorMap& tw, const AttnBwdParams& p, cudaStream_t stream) {
-  const int no = (d + 15) / 16 * 16;
+  const int no = (d + 31) / 32 * 32;
   if (d <= 64) {
     if (no <= 32) return launch_attn_bwd<MODE, 1, 32>(tx, ty, tu, tw, p, stream);
     return launch_attn_bwd<MODE, 1, 64>(tx, ty, tu, tw, p, stream);

@@ -210,13 +210,21 @@ extern "C" int ivb_scatter_add(const void* g, int g_is_f32, long g_bstride, cons
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (B <= 0 || rows <= 0) return 0;
   if (D & 7) return set_error("ivb_scatter_add: D must be a multiple of 8");
-  const long total = static_cast<long>(B) * rows;
+  // One launch per clip, in clip order: the rows of one clip name distinct table rows, so every table row receives its
+  // contributions in the same order on every run (one launch over all clips would add them in whatever order the
+  // clips' warps arrive, and the table's AdamW update would differ from run to run).
   const int wpb = 8;
-  const unsigned grid = (unsigned)((total + wpb - 1) / wpb);
-  if (g_is_f32)
-    scatter_add_kernel<true><<<grid, wpb * 32, 0, stream>>>(g, g_bstride, idx, idx_bstride, idx_off, B, rows, D, table_grad);
-  else
-    scatter_add_kernel<false><<<grid, wpb * 32, 0, stream>>>(g, g_bstride, idx, idx_bstride, idx_off, B, rows, D, table_grad);
-  count_launch();
-  return check_launch("scatter_add_kernel");
+  const unsigned grid = (unsigned)((rows + wpb - 1) / wpb);
+  const char* gb = reinterpret_cast<const char*>(g);
+  const long gstep = g_bstride * (g_is_f32 ? 4 : 2);
+  for (int b = 0; b < B; ++b) {
+    const int* ib = idx ? idx + static_cast<long>(b) * idx_bstride : nullptr;
+    if (g_is_f32)
+      scatter_add_kernel<true><<<grid, wpb * 32, 0, stream>>>(gb + b * gstep, g_bstride, ib, idx_bstride, idx_off, 1, rows, D, table_grad);
+    else
+      scatter_add_kernel<false><<<grid, wpb * 32, 0, stream>>>(gb + b * gstep, g_bstride, ib, idx_bstride, idx_off, 1, rows, D, table_grad);
+    count_launch();
+    if (int rc = check_launch("scatter_add_kernel")) return rc;
+  }
+  return 0;
 }

@@ -1,21 +1,13 @@
-// ivb_gemm_common.cuh — GEMM parameter block and the fused epilogue shared by the 1-CTA and the
-// 2-CTA (cta_group::2) tcgen05 GEMM kernels.
+// ivb_gemm_common.cuh — GEMM parameter block and the fused epilogue of the wgmma GEMM (ivb_gemm.cu).
 //
-// Epilogue data path: tcgen05.ld hands every thread ONE accumulator row (32 consecutive columns); the
-// thread applies the fused epilogue and writes its row segment straight to global memory with
-// 256-bit accesses (STG.256 / LDG.256 on sm_100: one full 32-byte sector per thread per instruction).
-// Measured on the fc1 GEMM (13344x6144x1408): plain store 1470 TFLOP/s, tanh-GELU 1400, but GELU + the
-// saved pre-activation (two bf16 outputs) only 760-920 with 128-bit stores — the second output's
-// half-sector stores saturate the LSU, not the math.  (A smem-transposed, fully coalesced variant was
-// measured slower: its LDS/STS traffic and per-row loop cost more than the coalescing saved.)
+// Epilogue data path: the MMA warps stage their accumulator fragments through a small per-warp shared-memory
+// tile so that every thread ends up with a contiguous row segment (16 columns); the thread applies the fused
+// epilogue and writes the segment straight to global memory with 128-bit accesses.
 #pragma once
 #include "ivb_internal.h"
 #include "ivb_ptx.cuh"
 
 namespace ivb {
-
-// epilogue warps per CTA (multiple of 4: one per TMEM lane quadrant).
-constexpr int EPI_WARPS = 12;
 
 struct GemmParams {
   int M, N, K;
@@ -30,18 +22,16 @@ struct GemmParams {
   const void* aux;
   long ldaux;
   const float* rowscale;  // EPI_RESID: optional per-row multiplier of the branch (DropPath keep/scale)
-  int sched_slot;         // >= 0: dynamic tile scheduler (gemm2): index of the global tile counter; < 0: static stride
 };
 
+// 32-byte row pieces as two 128-bit accesses (sm_90 has no 256-bit global load / store).
 __device__ __forceinline__ void st_global_256(void* p, const uint32_t r[8]) {
-  asm volatile("st.global.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(p), "r"(r[0]), "r"(r[1]),
-               "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-               : "memory");
+  reinterpret_cast<uint4*>(p)[0] = make_uint4(r[0], r[1], r[2], r[3]);
+  reinterpret_cast<uint4*>(p)[1] = make_uint4(r[4], r[5], r[6], r[7]);
 }
 __device__ __forceinline__ void ld_global_256(const void* p, uint32_t r[8]) {
-  asm volatile("ld.global.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "l"(p));
+  const uint4 a = reinterpret_cast<const uint4*>(p)[0], b = reinterpret_cast<const uint4*>(p)[1];
+  r[0] = a.x; r[1] = a.y; r[2] = a.z; r[3] = a.w; r[4] = b.x; r[5] = b.y; r[6] = b.z; r[7] = b.w;
 }
 
 // Row-segment I/O: W elements starting at `ptr`; `nvalid` (multiple of 8) of them are inside the matrix.
@@ -118,37 +108,10 @@ __device__ __forceinline__ void load_row_f32(const float* ptr, float* v, int nva
   }
 }
 
-// ------------------------------------------------------------------ epilogue operand prefetch
-// The epilogue's global READS (residual stream / saved pre-activation / gradient being accumulated)
-// come from HBM: a dependent ~1 us load in front of every 32-column chunk, which for the short-K GEMMs
-// (K = 1408) makes the epilogue as long as the next tile's main loop.  Each epilogue thread therefore
-// pulls its row segments into L2 while it would otherwise idle on the accumulator barrier
-// (prefetch.global.L2: no registers, no dependency).
-__device__ __forceinline__ void prefetch_l2(const void* ptr) {
-  asm volatile("prefetch.global.L2 [%0];" ::"l"(ptr));
-}
-// one 32-column chunk of row `row` starting at column col0
-__device__ __forceinline__ void epilogue_prefetch_chunk(const GemmParams& p, long row, int col0) {
-  if (col0 >= p.N) return;
-  if (p.epi == IVB_EPI_RESID) {
-    prefetch_l2(reinterpret_cast<const float*>(p.aux) + row * p.ldaux + col0);          // 128 B
-  } else if (p.epi == IVB_EPI_GELU_BWD) {
-    prefetch_l2(reinterpret_cast<const __nv_bfloat16*>(p.aux) + row * p.ldaux + col0);  // 64 B
-  } else if ((p.flags & IVB_FLAG_ACCUM) != 0) {
-    if (p.epi == IVB_EPI_F32) prefetch_l2(reinterpret_cast<const float*>(p.out0) + row * p.ld0 + col0);
-    else prefetch_l2(reinterpret_cast<const __nv_bfloat16*>(p.out0) + row * p.ld0 + col0);
-  }
-}
-
 // ------------------------------------------------------------------ epilogue for W columns of one row
-// acc_bits: W fp32 accumulators of (row, col0 .. col0+W-1).  W is 32 or 16.
-// sbias / sgamma: optional shared-memory copies (fp32, W values) of bias[col0..] / gamma[col0..] staged by the
-// calling warp before it waited for the accumulator (ivb_gemm2.cu): ncu attributed 6 % of the fused-GELU
-// kernel's stall samples to the dependent global bias load in front of every chunk.
+// acc_bits: W fp32 accumulators of (row, col0 .. col0+W-1).  W is a multiple of 16.
 template <int W>
-__device__ __forceinline__ void epilogue_chunk(const GemmParams& p, const uint32_t* acc_bits,
-                                               long row, int col0, const float* sbias = nullptr,
-                                               const float* sgamma = nullptr) {
+__device__ __forceinline__ void epilogue_chunk(const GemmParams& p, const uint32_t* acc_bits, long row, int col0) {
   int nvalid = p.N - col0;
   if (nvalid <= 0) return;
   if (nvalid > W) nvalid = W;
@@ -156,18 +119,10 @@ __device__ __forceinline__ void epilogue_chunk(const GemmParams& p, const uint32
 #pragma unroll
   for (int i = 0; i < W; ++i) v[i] = __uint_as_float(acc_bits[i]);
   if (p.bias != nullptr) {
-    if (sbias != nullptr) {
+    float bv[W];
+    load_row_bf16<W>(p.bias + col0, bv, nvalid);
 #pragma unroll
-      for (int i = 0; i < W; i += 4) {
-        const float4 b4 = *reinterpret_cast<const float4*>(sbias + i);
-        v[i] += b4.x; v[i + 1] += b4.y; v[i + 2] += b4.z; v[i + 3] += b4.w;
-      }
-    } else {
-      float bv[W];
-      load_row_bf16<W>(p.bias + col0, bv, nvalid);
-#pragma unroll
-      for (int i = 0; i < W; ++i) v[i] += bv[i];
-    }
+    for (int i = 0; i < W; ++i) v[i] += bv[i];
   }
   const bool accum = (p.flags & IVB_FLAG_ACCUM) != 0;
   const bool tanh_mode = (p.flags & IVB_FLAG_GELU_TANH) != 0;
@@ -235,15 +190,7 @@ __device__ __forceinline__ void epilogue_chunk(const GemmParams& p, const uint32
       load_row_f32<W>(reinterpret_cast<const float*>(p.aux) + row * p.ldaux + col0, res, nvalid);
       if (p.gamma != nullptr) {
         float gm[W];
-        if (sgamma != nullptr) {
-#pragma unroll
-          for (int i = 0; i < W; i += 4) {
-            const float4 g4 = *reinterpret_cast<const float4*>(sgamma + i);
-            gm[i] = g4.x; gm[i + 1] = g4.y; gm[i + 2] = g4.z; gm[i + 3] = g4.w;
-          }
-        } else {
-          load_row_bf16<W>(p.gamma + col0, gm, nvalid);
-        }
+        load_row_bf16<W>(p.gamma + col0, gm, nvalid);
 #pragma unroll
         for (int i = 0; i < W; ++i) v[i] = fmaf(gm[i] * rs, v[i], res[i]);
       } else {

@@ -7,6 +7,8 @@
 //   pixel-reconstruction target  InternVideo1/Pretrain/VideoMAE/engine_for_pretraining.py:66-98 + MSE :43,106
 #include <math.h>
 
+#define IVB_COLRED_FLOATS (4L << 20)
+#include "ivb_colred.cuh"
 #include "ivb_internal.h"
 #include "ivb_ptx.cuh"
 
@@ -99,7 +101,7 @@ ln_l2_fwd_kernel(const __nv_bfloat16* __restrict__ z, long ldz, const __nv_bfloa
 }
 
 // d_out = gscale * dout_tensor  (dout_tensor is the upstream gradient, or the TARGET itself when the
-// loss is (2-2<out,tgt>).mean(): then gscale = -2 * g / rows).  Computes dz (bf16), dw, db (fp32 atomics).
+// loss is (2-2<out,tgt>).mean(): then gscale = -2 * g / rows).  Computes dz (bf16), dw, db (fp32, accumulated in a fixed order).
 // dynamic smem: float acc[2][warps][C]
 template <bool DO_F32>
 __global__ void __launch_bounds__(256)
@@ -176,8 +178,8 @@ ln_l2_bwd_kernel(const __nv_bfloat16* __restrict__ z, long ldz, const __nv_bfloa
     for (int i = threadIdx.x; i < C; i += blockDim.x) {
       float sw = 0.f, sb = 0.f;
       for (int k = 0; k < wpb; ++k) { sw += acc_smem[static_cast<long>(k) * C + i]; sb += acc_smem[static_cast<long>(wpb + k) * C + i]; }
-      atomicAdd(dw + i, sw);
-      if (db) atomicAdd(db + i, sb);
+      colred_put(0, gridDim.x, blockIdx.x, C, i, sw);
+      if (db) colred_put(1, gridDim.x, blockIdx.x, C, i, sb);
     }
   }
 }
@@ -259,7 +261,7 @@ __global__ void adamw_kernel(float* __restrict__ master, float* __restrict__ m, 
 }
 
 // ---------------------------------------------------------------- contrastive loss (video-text)
-// cosv2t [G,G] fp32 = vn @ tn^T (tcgen05 GEMM).  S = cos / temp.  idx int64 [G].
+// cosv2t [G,G] fp32 = vn @ tn^T (wgmma GEMM).  S = cos / temp.  idx int64 [G].
 // row pass: lse_r[i], tsum_r[i] = sum_j tg[i,j] S[i,j] ; col pass: lse_c[i], tsum_c[i] = sum_j tg[i,j] S[j,i]
 // loss = 1/(2G) sum_i [(lse_r[i] - tsum_r[i]) + (lse_c[i] - tsum_c[i])]          (criterions.py:93-102)
 __global__ void __launch_bounds__(256)
@@ -524,8 +526,8 @@ ln_l2_bwd_reg_kernel(const __nv_bfloat16* __restrict__ z, long ldz, const __nv_b
     for (int i = threadIdx.x; i < C; i += blockDim.x) {
       float sw = 0.f, sb = 0.f;
       for (int k = 0; k < wpb; ++k) { sw += acc_smem[static_cast<long>(k) * C + i]; sb += acc_smem[static_cast<long>(wpb + k) * C + i]; }
-      atomicAdd(dw + i, sw);
-      if (db) atomicAdd(db + i, sb);
+      colred_put(0, gridDim.x, blockIdx.x, C, i, sw);
+      if (db) colred_put(1, gridDim.x, blockIdx.x, C, i, sb);
     }
   }
 }
@@ -566,8 +568,6 @@ extern "C" int ivb_ln_l2_fwd(const void* z, long ldz, const void* weight, const 
   auto ww = reinterpret_cast<const __nv_bfloat16*>(weight);
   auto bb = reinterpret_cast<const __nv_bfloat16*>(bias);
   auto oo = reinterpret_cast<__nv_bfloat16*>(out);
-  // (a register-resident forward — ln_l2_fwd_reg_kernel — measured SLOWER at C = 3200: 104 us vs 58 us; at 222
-  //  registers only 8 warps fit an SM and the four sweeps over 100 values per lane become issue-bound)
   if (target_is_f32) ln_l2_fwd_kernel<true><<<(int)blocks, 256, 0, stream>>>(zz, ldz, ww, bb, eps, M, C, oo, ldo, stats, target, ldt, loss_sum);
   else ln_l2_fwd_kernel<false><<<(int)blocks, 256, 0, stream>>>(zz, ldz, ww, bb, eps, M, C, oo, ldo, stats, target, ldt, loss_sum);
   count_launch();
@@ -593,12 +593,14 @@ static int launch_ln_l2_bwd(const void* z, long ldz, const void* weight, const v
   const long cap = static_cast<long>(num_sms()) * (smem > 96 * 1024 ? 2 : 4);
   if (blocks > cap) blocks = cap;
   if (blocks < 1) blocks = 1;
+  if (colred_check(2, blocks, C, "ln_l2_bwd: gradient scratch too small")) return 1;
   kern<<<(int)blocks, wpb * 32, smem, stream>>>(
       reinterpret_cast<const __nv_bfloat16*>(z), ldz, reinterpret_cast<const __nv_bfloat16*>(weight),
       reinterpret_cast<const __nv_bfloat16*>(bias), stats, M, C, dout, lddo, gh, gd,
       reinterpret_cast<__nv_bfloat16*>(dz), lddz, dw, db);
   count_launch();
-  return check_launch("ln_l2_bwd_kernel");
+  if (int rc = check_launch("ln_l2_bwd_kernel")) return rc;
+  return dw ? colred_finish(2, (int)blocks, C, dw, db, nullptr, stream) : 0;
 }
 
 template <int NCH>
@@ -619,12 +621,14 @@ static int launch_ln_l2_bwd_reg(const void* z, long ldz, const void* weight, con
   const long cap = static_cast<long>(num_sms()) * 2;
   if (blocks > cap) blocks = cap;
   if (blocks < 1) blocks = 1;
+  if (colred_check(2, blocks, C, "ln_l2_bwd: gradient scratch too small")) return 1;
   kern<<<(int)blocks, wpb * 32, smem, stream>>>(
       reinterpret_cast<const __nv_bfloat16*>(z), ldz, reinterpret_cast<const __nv_bfloat16*>(weight),
       reinterpret_cast<const __nv_bfloat16*>(bias), stats, M, C, reinterpret_cast<const __nv_bfloat16*>(dout), lddo,
       gh, gd, reinterpret_cast<__nv_bfloat16*>(dz), lddz, dw, db);
   count_launch();
-  return check_launch("ln_l2_bwd_reg_kernel");
+  if (int rc = check_launch("ln_l2_bwd_reg_kernel")) return rc;
+  return dw ? colred_finish(2, (int)blocks, C, dw, db, nullptr, stream) : 0;
 }
 
 extern "C" int ivb_ln_l2_bwd(const void* z, long ldz, const void* weight, const void* bias,

@@ -5,9 +5,11 @@
 //   LayerScale backward                      (internvideo2_pretrain.py:131-146)
 //   bias-gradient column sums
 // One warp per row, 16-byte vector loads, warp-shuffle reductions; parameter gradients are
-// accumulated per warp in shared memory and flushed with one atomicAdd per column per CTA.
+// accumulated per warp in shared memory, stored as one partial per column per CTA and summed in a fixed
+// order by colred_finish (ivb_colred.cuh).
 #include <stdlib.h>
 
+#include "ivb_colred.cuh"
 #include "ivb_internal.h"
 #include "ivb_ptx.cuh"
 
@@ -190,8 +192,8 @@ norm_bwd_kernel(const __nv_bfloat16* dy, long lddy, const void* __restrict__ x, 
         sw += acc_smem[(long)k * D + i];
         if (LN) sb += acc_smem[(long)(warps_per_block + k) * D + i];
       }
-      atomicAdd(dweight + i, sw);
-      if (LN && dbias != nullptr) atomicAdd(dbias + i, sb);
+      colred_put(0, gridDim.x, blockIdx.x, D, i, sw);
+      if (LN && dbias != nullptr) colred_put(1, gridDim.x, blockIdx.x, D, i, sb);
     }
   }
 }
@@ -245,10 +247,11 @@ layerscale_bwd_kernel(const float* __restrict__ dx, long lddx, const __nv_bfloat
     float sg = 0.f, ss = 0.f;
 #pragma unroll
     for (int k = 0; k < 8; ++k) { sg += red[0][k][c]; ss += red[1][k][c]; }
-    if (HAS_Y && dgamma != nullptr) atomicAdd(dgamma + strip * 256 + c, sg);
+    const int nrb = gridDim.x / nstrips;
+    if (HAS_Y && dgamma != nullptr) colred_put(0, nrb, rb, D, strip * 256 + c, sg);
     // bias gradient of the branch Linear: d/db [gamma * (acc + b)] = gamma * sum_m dx'
     if (dcolsum != nullptr)
-      atomicAdd(dcolsum + strip * 256 + c, gamma != nullptr ? ss * __bfloat162float(gamma[strip * 256 + c]) : ss);
+      colred_put(1, nrb, rb, D, strip * 256 + c, gamma != nullptr ? ss * __bfloat162float(gamma[strip * 256 + c]) : ss);
   }
 }
 
@@ -283,7 +286,7 @@ colsum_bf16_kernel(const __nv_bfloat16* __restrict__ x, long ldx, int M, int N,
     float s = 0.f;
 #pragma unroll
     for (int k = 0; k < 8; ++k) s += red[k][c];
-    atomicAdd(out + strip * 256 + c, s);
+    colred_put(0, gridDim.x / nstrips, rb, N, strip * 256 + c, s);
   }
 }
 
@@ -428,12 +431,12 @@ rms_bwd_reg_kernel(const __nv_bfloat16* dy, long lddy, const void* __restrict__ 
       if (PAIR) {
         float s0 = 0.f, s1 = 0.f;
         for (int k = 0; k < wpb; k += 2) { s0 += acc_smem[(long)k * D + i]; s1 += acc_smem[(long)(k + 1) * D + i]; }
-        atomicAdd(dweight + i, s0);
-        atomicAdd(dweight1 + i, s1);
+        colred_put(0, gridDim.x, blockIdx.x, D, i, s0);
+        colred_put(1, gridDim.x, blockIdx.x, D, i, s1);
       } else {
         float sw = 0.f;
         for (int k = 0; k < wpb; ++k) sw += acc_smem[(long)k * D + i];
-        atomicAdd(dweight + i, sw);
+        colred_put(0, gridDim.x, blockIdx.x, D, i, sw);
       }
     }
   }
@@ -442,10 +445,8 @@ rms_bwd_reg_kernel(const __nv_bfloat16* dy, long lddy, const void* __restrict__ 
 // ------------------------------------------------------------------ bulk-copy (TMA) row pipeline
 // Every warp owns a ring of NBUF row slots in shared memory that lane 0 keeps full with cp.async.bulk (1-D bulk copies
 // completing on per-slot mbarriers); the arithmetic reads the row from shared memory (conflict-free 16-byte lanes), so
-// four input rows per token cost no registers.  Measured (profiles/r02_membound_ncu.md): for the PLAIN RMSNorm
-// forward / backward this pipeline is no faster than the register-resident kernels above (an 80-190 MB launch is
-// dominated by ramp-up, not by steady-state bandwidth: 0.46-0.63 of the copy rate either way), so it is only used where
-// it removes a whole kernel: the backward fused with the LayerScale backward.
+// four input rows per token cost no registers.  It is used where it removes a whole kernel: the backward fused with the
+// LayerScale backward.
 
 // RMSNorm backward on the fp32 stream, optionally FUSED with the LayerScale backward that follows it in the block
 // (Block.backward: dx = rmsnorm_bwd(dy, x) + dx_in is the gradient of the residual stream, which the preceding branch's
@@ -563,10 +564,10 @@ rms_bwd_tma_kernel(const __nv_bfloat16* __restrict__ dy, long lddy, const float*
       sw += accs[(static_cast<long>(k) * NACC) * D + i];
       if (LS) { sg += accs[(static_cast<long>(k) * NACC + 1) * D + i]; sc += accs[(static_cast<long>(k) * NACC + 2) * D + i]; }
     }
-    if (dweight) atomicAdd(dweight + i, sw);
+    if (dweight) colred_put(0, gridDim.x, blockIdx.x, D, i, sw);
     if (LS) {
-      if (dgamma) atomicAdd(dgamma + i, sg);
-      if (dcolsum) atomicAdd(dcolsum + i, sc * __bfloat162float(gamma[i]));
+      if (dgamma) colred_put(1, gridDim.x, blockIdx.x, D, i, sg);
+      if (dcolsum) colred_put(2, gridDim.x, blockIdx.x, D, i, sc * __bfloat162float(gamma[i]));
     }
   }
 }
@@ -591,6 +592,7 @@ static int launch_rms_bwd_tma(const void* dy, long lddy, const void* x, long ldx
   int grid = num_sms();
   const int need = (M + NW - 1) / NW;
   if (grid > need) grid = need;
+  if (colred_check(3, grid, D, "rms_bwd_tma: gradient scratch too small")) return 1;
   launch_pdl(kern, dim3(grid), dim3(NW * 32), smem, stream, reinterpret_cast<const __nv_bfloat16*>(dy), lddy, reinterpret_cast<const float*>(x), ldx,
                                         reinterpret_cast<const __nv_bfloat16*>(w), rstd, M, D, dx_in, lddx_in,
                                         reinterpret_cast<float*>(dx_out), lddx, dweight,
@@ -598,7 +600,8 @@ static int launch_rms_bwd_tma(const void* dy, long lddy, const void* x, long ldx
                                         reinterpret_cast<const __nv_bfloat16*>(gamma), rowscale,
                                         reinterpret_cast<__nv_bfloat16*>(dyb), lddyb, dgamma, dcolsum);
   count_launch();
-  return check_launch("rms_bwd_tma_kernel");
+  if (int rc = check_launch("rms_bwd_tma_kernel")) return rc;
+  return colred_finish(3, grid, D, dweight, LS ? dgamma : nullptr, LS ? dcolsum : nullptr, stream);
 }
 
 template <bool XF32, int NCH, bool PAIR = false>
@@ -637,13 +640,16 @@ static int launch_rms_bwd_reg(const void* dy, long lddy, const void* x, long ldx
   const long cap = (long)num_sms() * 2;   // 2 CTAs/SM resident (<=128 registers): one persistent wave
   if (blocks > cap) blocks = cap;
   if (blocks < 1) blocks = 1;
+  if (colred_check(2, blocks, D, "rms_bwd_reg: gradient scratch too small")) return 1;
   launch_pdl(kern, dim3((int)blocks), dim3(wpb * 32), smem, stream, reinterpret_cast<const __nv_bfloat16*>(dy), lddy, x, ldx,
                                                 reinterpret_cast<const __nv_bfloat16*>(w), rstd, (int)rows, D, dx_in,
                                                 lddx_in, dx_out, lddx, dweight,
                                                 reinterpret_cast<const __nv_bfloat16*>(w1), dweight1, x_pair_off,
                                                 dy_pair_off, dx_pair_off);
   count_launch();
-  return check_launch("rms_bwd_reg_kernel");
+  if (int rc = check_launch("rms_bwd_reg_kernel")) return rc;
+  if (dweight == nullptr) return 0;
+  return colred_finish(PAIR ? 2 : 1, (int)blocks, D, dweight, PAIR ? dweight1 : nullptr, nullptr, stream);
 }
 
 }  // namespace ivb
@@ -708,12 +714,15 @@ static int launch_norm_bwd(const void* dy, long lddy, const void* x, long ldx, c
   const long cap = (long)num_sms() * (smem > 96 * 1024 ? 2 : 4);
   if (blocks > cap) blocks = cap;
   if (blocks < 1) blocks = 1;
+  if (colred_check(2, blocks, D, "norm_bwd: gradient scratch too small")) return 1;
   launch_pdl(kern, dim3((int)blocks), dim3(wpb * 32), smem, stream, 
       reinterpret_cast<const __nv_bfloat16*>(dy), lddy, x, ldx,
       reinterpret_cast<const __nv_bfloat16*>(weight), mean, rstd, M, D, dx_in, lddx_in, dx_out,
       lddx, dweight, dbias);
   count_launch();
-  return check_launch("norm_bwd_kernel");
+  if (int rc = check_launch("norm_bwd_kernel")) return rc;
+  if (dweight == nullptr) return 0;
+  return colred_finish(2, (int)blocks, D, dweight, LN ? dbias : nullptr, nullptr, stream);
 }
 
 extern "C" int ivb_norm_bwd(const void* dy, long lddy, const void* x, int x_is_f32, long ldx,
@@ -763,12 +772,14 @@ extern "C" int ivb_layerscale_bwd(const float* dx, long lddx, const void* y, lon
   const __nv_bfloat16* yy = reinterpret_cast<const __nv_bfloat16*>(y);
   const __nv_bfloat16* gg = reinterpret_cast<const __nv_bfloat16*>(gamma);
   __nv_bfloat16* dyo = reinterpret_cast<__nv_bfloat16*>(dy);
+  if (colred_check(2, rbs, D, "ivb_layerscale_bwd: gradient scratch too small")) return 1;
   if (y != nullptr)
     launch_pdl(layerscale_bwd_kernel<true>, dim3(nstrips * rbs), dim3(256), 0, stream, dx, lddx, yy, ldy, gg, M, D, dyo, lddy, dgamma, dcolsum, nstrips, rowscale);
   else
     launch_pdl(layerscale_bwd_kernel<false>, dim3(nstrips * rbs), dim3(256), 0, stream, dx, lddx, yy, ldy, gg, M, D, dyo, lddy, dgamma, dcolsum, nstrips, rowscale);
   count_launch();
-  return check_launch("layerscale_bwd_kernel");
+  if (int rc = check_launch("layerscale_bwd_kernel")) return rc;
+  return colred_finish(2, rbs, D, y != nullptr ? dgamma : nullptr, dcolsum, nullptr, stream);
 }
 
 extern "C" int ivb_colsum_bf16(const void* x, long ldx, int M, int N, float* out, void* stream_) {
@@ -778,10 +789,12 @@ extern "C" int ivb_colsum_bf16(const void* x, long ldx, int M, int N, float* out
   const int nstrips = (N + 255) / 256;
   const int rows_per_cta = 128;
   const int rbs = (M + rows_per_cta - 1) / rows_per_cta;
+  if (colred_check(1, rbs, N, "ivb_colsum_bf16: gradient scratch too small")) return 1;
   launch_pdl(colsum_bf16_kernel, dim3(nstrips * rbs), dim3(256), 0, stream, reinterpret_cast<const __nv_bfloat16*>(x),
                                                         ldx, M, N, out, nstrips, rows_per_cta);
   count_launch();
-  return check_launch("colsum_bf16_kernel");
+  if (int rc = check_launch("colsum_bf16_kernel")) return rc;
+  return colred_finish(1, rbs, N, out, nullptr, nullptr, stream);
 }
 
 // q-norm and k-norm of one block in a single launch: the two [M, D] column slices x and x + pair_off of a

@@ -2,8 +2,7 @@
 // (SURVEY §8 row a19/e: the reference's DDP/DeepSpeed gradient reduction, run_pretraining.py:378 + utils.py:814-834).
 //
 // Why not ncclAllReduce: on an 8-GPU NVSwitch box NCCL's NVLS all-reduce runs 24 channels = 24 CTAs that each hold an SM
-// for the whole bucket; under the persistent one-CTA-per-SM tcgen05 GEMMs of the backward pass that inflated the in-step
-// GEMM time by 9 % (profiles/r02_8gpu_cfg2.log).  The gradients only need ~2 GB per ~75 ms of backward, so this kernel
+// for the whole bucket; under the persistent one-CTA-per-SM GEMMs of the backward pass those SMs are taken from the GEMMs.  The gradients only need ~2 GB per ~75 ms of backward, so this kernel
 // trades bandwidth for footprint: a handful of CTAs, no staging buffers, no protocol — the switch does the arithmetic.
 //
 // Every rank maps the SAME symmetric buffer (the flat bf16 gradient buffer) through a multicast address `mc`.  Two-shot:
@@ -113,23 +112,9 @@ extern "C" int ivb_nvls_allreduce_bf16(void* mc_base, long elem_off, long numel,
     return set_error("ivb_nvls_allreduce_bf16: range must start and end on 16-byte boundaries (8 bf16 elements)");
   if (numel == 0) return 0;
   uint4* mc = reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(mc_base) + elem_off);
-  // CTAs are launched as clusters of two: a pair always lands on the two SMs of one TPC, so the CTA-pair (cta_group::2)
-  // GEMMs running beside it lose whole TPCs instead of one SM out of many (IVB_NVLS_CLUSTER=0: plain grid).
-  static const bool paired = [] { const char* e = getenv("IVB_NVLS_CLUSTER"); return e == nullptr || atoi(e) != 0; }();
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(nblocks);
-  cfg.blockDim = dim3(NVLS_THREADS);
-  cfg.dynamicSmemBytes = 0;
-  cfg.stream = static_cast<cudaStream_t>(stream);
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = (paired && nblocks % 2 == 0) ? 1 : 0;
   const long nvec = numel / 8;
   uint32_t* const* flags = reinterpret_cast<uint32_t* const*>(flag_ptrs_dev);
-  cudaError_t e = cudaLaunchKernelEx(&cfg, nvls_allreduce_bf16_kernel, mc, nvec, flags, rank, world);
-  if (e != cudaSuccess) return set_error_cuda("cudaLaunchKernelEx(nvls_allreduce_bf16_kernel)", e);
+  nvls_allreduce_bf16_kernel<<<nblocks, NVLS_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(mc, nvec, flags, rank, world);
   count_launch();
   return check_launch("nvls_allreduce_bf16_kernel");
 }

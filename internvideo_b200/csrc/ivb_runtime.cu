@@ -35,11 +35,11 @@ bool pdl_enabled() {
 int num_sms() {
   static int cached[64] = {0};
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
   if (cached[dev] == 0) {
     int n = 0;
     if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0)
-      n = 148;
+      n = 132;
     cached[dev] = n;
   }
   return cached[dev];
@@ -124,9 +124,10 @@ extern "C" int ivb_device_check(void) {
   int n = 0;
   cudaError_t e = cudaGetDeviceCount(&n);
   if (e != cudaSuccess || n == 0) return set_error("libivb200: no CUDA device (there is no CPU fallback)");
-  int dev = 0, major = 0;
+  int dev = 0, major = 0, minor = 0;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
-  if (major != 10) return set_error("libivb200: device is not compute capability 10.x (sm_100a only)");
+  cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev);
+  if (major != 9 || minor != 0) return set_error("libivb200: device is not compute capability 9.0 (sm_90a only)");
   return 0;
 }

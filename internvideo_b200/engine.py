@@ -2,12 +2,12 @@
 
 What it replaces in the reference: DDP / DeepSpeed ZeRO-1 gradient reduction + AdamW
 (InternVideo2/single_modality/run_pretraining.py:368-382, utils.py:814-908, optim_factory.py:56-190)
-for the one data-parallel path this repo accelerates.  Design (B200-first):
+for the one data-parallel path this repo accelerates.  Design (H100-first):
 
   * all parameters live in ONE flat bf16 buffer (16-byte aligned slices, what the TMA descriptors and
     vector loads want), all gradients in one flat bf16 buffer that `param.grad` aliases, fp32 master
     weights + Adam moments in three flat fp32 buffers: 16 B/param -> 17 GB for the 1B model, 95 GB
-    for 6B, inside one B200's 180 GB without sharding;
+    for 6B, which exceeds one H100's 80 GB: 6B needs zero1=True over several GPUs;
   * gradient all-reduce is bucketed over contiguous slices of the flat gradient and launched as soon as
     a bucket is complete, so NCCL (NVLS/ring over NVSwitch) overlaps the remaining backward GEMMs.
     Stream ordering is explicit: every "gradient written" signal records an event on the stream it was
@@ -456,7 +456,7 @@ class GraphedStep:
     """Capture `fn(*static_inputs) -> loss` (forward + backward + engine.step) into ONE CUDA graph.
 
     The training step issues ~5 000 kernel launches; replaying them from a graph removes the Python /
-    ctypes / autograd issue cost from the critical path (the B200 finishes the small row kernels faster
+    ctypes / autograd issue cost from the critical path (the GPU finishes the small row kernels faster
     than the host can enqueue them).  Inputs are copied into static device buffers before each replay;
     TMA tensor maps are encoded at capture time and stay valid because the graph's private memory pool
     pins every activation address."""

@@ -491,7 +491,7 @@ _OPPROF = [None]
 
 
 class OpProfiler:
-    """CUDA-event timing of every lowlevel op, in situ (warm caches, real overlap) — tools/step_profile.py."""
+    """CUDA-event timing of every lowlevel op, in situ (warm caches, real overlap)."""
 
     def __init__(self):
         self.records = []

@@ -127,7 +127,7 @@ class LayerScale(nn.Module):
 
 class Attention(nn.Module):
     """internvideo2_pretrain.py:149-217.  `use_flash_attn` is accepted for signature parity; there is
-    one implementation (tcgen05 flash-style attention)."""
+    one implementation (wgmma flash-style attention)."""
 
     def __init__(self, dim, num_heads=8, qkv_bias=False, attn_drop=0.0, proj_drop=0.0, use_flash_attn=False,
                  causal=False, norm_layer=nn.LayerNorm, qk_normalization=False, use_fused_rmsnorm=False):
@@ -198,7 +198,7 @@ class Block(nn.Module):
                               force_fp32=(not layerscale_no_force_fp32)) if init_values else nn.Identity()
         self.drop_path2 = DropPath(drop_path) if drop_path > 0.0 else nn.Identity()
         # activation checkpointing (reference :294-295): only the block input is kept, backward recomputes the
-        # forward (ops.BlockFn).  Unnecessary for the 1B recipe on 180 GB HBM3e, needed for 6B / large unmasked batches
+        # forward (ops.BlockFn).  Unnecessary for the 1B recipe on an 80 GB H100, needed for 6B / large unmasked batches
         self.with_cp = bool(with_cp)
         self.use_fused_rmsnorm = use_fused_rmsnorm
         self.num_heads = num_heads
@@ -252,7 +252,7 @@ class Block(nn.Module):
 
 
 class PatchEmbed(nn.Module):
-    """internvideo2_pretrain.py:300-331 — Conv3d(k=s=(tubelet,p,p)) as an im2col GEMM on tcgen05."""
+    """internvideo2_pretrain.py:300-331 — Conv3d(k=s=(tubelet,p,p)) as an im2col GEMM on wgmma."""
 
     def __init__(self, img_size=224, patch_size=16, in_chans=3, embed_dim=768, num_frames=8, tubelet_size=1,
                  norm_layer=None):

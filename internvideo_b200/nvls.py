@@ -29,8 +29,7 @@ class NvlsUnavailable(RuntimeError):
 
 def default_blocks(world: int = 8) -> int:
     """CTAs per reduction.  A rank pulls 1/world of every range through the switch, so small worlds need more requests in
-    flight per rank: 2 GPUs 16 CTAs (same-box A/B: 120.9 ms/step against 122.6 with 8 and 122.5 with NCCL), >= 4 GPUs 8
-    (8 GPUs: 467 GB/s isolated, already past NCCL's 373)."""
+    flight per rank: 16 CTAs below 4 GPUs, else 8 (IVB_NVLS_BLOCKS overrides).  Not measured on H100."""
     env = os.environ.get("IVB_NVLS_BLOCKS")
     if env:
         return int(env)

@@ -1,6 +1,6 @@
 """torch.autograd.Function wrappers over the C ABI (lowlevel.py): the differentiable op surface.
 
-Everything here runs on the B200 through libivb200.so; there is no eager/PyTorch fallback for the
+Everything here runs on the H100 through libivb200.so; there is no eager/PyTorch fallback for the
 compute (tiny O(D) vector glue such as `gamma * colsum` uses torch elementwise ops on CUDA tensors).
 Activations are bf16, the residual stream is fp32, parameters are bf16 (the reference's bf16
 DeepSpeed mode converts the whole model: engines/engine_for_pretraining.py:128, SURVEY App.B-18).
@@ -28,7 +28,7 @@ def _pdt(g, p):
 
 # ------------------------------------------------------------------------------------------ Linear
 class LinearFn(torch.autograd.Function):
-    """y = x W^T + b on the tcgen05 GEMM (nn.Linear: internvideo2_pretrain.py:61-77,195,211,356)."""
+    """y = x W^T + b on the wgmma GEMM (nn.Linear: internvideo2_pretrain.py:61-77,195,211,356)."""
 
     @staticmethod
     def forward(ctx, x, w, b, out_f32=False):

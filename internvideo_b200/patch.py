@@ -2,7 +2,7 @@
 
   FlashAttention            the reference's attention seam (single_modality/models/flash_attention_class.py:10-70): same
                             ctor and `forward(qkv[B,S,3,H,d], key_padding_mask=None, causal=False) -> (out[B,S,H,d], None)`
-                            contract, on the tcgen05 attention kernels, differentiable.
+                            contract, on the wgmma attention kernels, differentiable.
   patch_flash_attention(m)  swap every `inner_attn` FlashAttention instance of a reference-built model for the one above
                             (the reference's own blocks then call libivb200 for attention and nothing else changes).
   from_reference(m)         rebuild a reference-built PretrainInternVideo2 as the ivb200 model with the same

@@ -248,7 +248,7 @@ def vtm_triplets(vision_embeds, text_embeds, text_atts, vision_neg, txt_neg):
 @torch.no_grad()
 def get_sim(vision_proj, text_proj, temp=1.0, agg_method="mean"):
     """criterions.py:15-55 — cosine similarities / temp, both directions.  vision_proj [B,C] or [B,T,C] (per-frame), text
-    [B,C] or [B,1/K,C].  CUDA bf16/fp32 inputs run the [B,B] product on the tcgen05 GEMM (fp32 accumulate)."""
+    [B,C] or [B,1/K,C].  CUDA bf16/fp32 inputs run the [B,B] product on the wgmma GEMM (fp32 accumulate)."""
     v = F.normalize(vision_proj.float(), dim=-1)
     t = F.normalize(text_proj.float(), dim=-1)
     if v.ndim == 3:

@@ -9,7 +9,7 @@ Mirrors (constructor kwargs, parameter names / state_dict keys, forward contract
   InternVideo2/single_modality/engines/engine_for_pretraining.py:97-125 attention-guided mask + target selection
 
 In the real recipe the two teachers cost ~30 TFLOP/clip against ~2.7 for the student step: end-to-end clips/s is
-teacher-bound, which is why they run through the same tcgen05 GEMM / attention kernels.
+teacher-bound, which is why they run through the same wgmma GEMM / attention kernels.
 """
 from __future__ import annotations
 

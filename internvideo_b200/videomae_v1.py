@@ -13,7 +13,7 @@ Mirrors InternVideo1/Pretrain/VideoMAE:
 Same constructor arguments, same state_dict keys, same forward contract
 `model(x[B,3,T,H,W], mask[B,N] bool) -> [B, N_mask, 3*tubelet*p*p]`.
 
-Built from the differentiable primitives of ops.py (LayerNorm rows, tcgen05 GEMM with bias / GELU epilogues, tcgen05 flash
+Built from the differentiable primitives of ops.py (LayerNorm rows, wgmma GEMM with bias / GELU epilogues, wgmma flash
 attention, visible-only im2col embed); the residual stream is fp32, everything else bf16.  No CPU path.
 """
 from __future__ import annotations

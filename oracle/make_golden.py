@@ -21,6 +21,9 @@ Fixtures
                      rank, loss, and the per-rank input gradients (local-slice backward semantics).
   pixel_target.npz   IV1 VideoMAE target construction: the reference's own statements
                      (engine_for_pretraining.py:66-98) exec'd on a seeded clip.
+  ref_checks.npz     what the CPU tests compare against the reference: mask generator draws, VTM triplets, UTA /
+                     get_sim / itm_eval results, the IV1 VideoMAE init (SHA-256 per tensor), sin-cos and separable
+                     position tables and interpolate_pos_embed, all under the seeds the tests use.
 """
 from __future__ import annotations
 
@@ -616,12 +619,165 @@ def make_iv1_videomae():
     print("iv1_videomae: out", tuple(out.shape), "loss", float(loss), "enc", tuple(blob["enc_out"].shape))
 
 
+def _sha(t) -> np.ndarray:
+    import hashlib
+    a = np.ascontiguousarray(t.detach().cpu().numpy() if torch.is_tensor(t) else t)
+    return np.frombuffer(hashlib.sha256(a.tobytes()).digest(), dtype=np.uint8).copy()
+
+
+def _txt(s: str) -> np.ndarray:
+    return np.frombuffer(s.encode(), dtype=np.uint8).copy()
+
+
+def sdims_params(shapes):
+    """Seeded parameters for the InternVideo2-S comparison: N(0, 0.02) per tensor in sorted-key order, norm weights 1 + that."""
+    g = torch.Generator().manual_seed(0)
+    p = {}
+    for k in sorted(shapes):
+        t = torch.randn(shapes[k], generator=g) * 0.02
+        p[k] = 1.0 + t if ("norm" in k and k.endswith("weight")) else t
+    return p
+
+
+def sdims_inputs():
+    """2 clips x 4 frames x 224^2 and an 80 % mask (52 visible patches per frame, cls visible)."""
+    x = torch.randn(2, 3, 4, 224, 224, generator=torch.Generator().manual_seed(1))
+    g = torch.Generator().manual_seed(3)
+    mask = torch.ones(2, 1 + 4 * 256, dtype=torch.bool); mask[:, 0] = False
+    for b in range(2):
+        for t in range(4):
+            mask[b, 1 + t * 256 + torch.randperm(256, generator=g)[:52]] = False
+    return x, mask
+
+
+def sdims_sample(numel, n=4096):
+    if numel <= n:
+        return torch.arange(numel)
+    return torch.randint(0, numel, (n,), generator=torch.Generator().manual_seed(5))
+
+
+def make_ref_checks():
+    """Reference results for tests/test_{masking,stage2,videomae_v1,modules}_cpu.py (same seeds and inputs as the tests)."""
+    import importlib
+    import importlib.util
+    import types
+    blob = {}
+
+    def load(path, name):
+        spec = importlib.util.spec_from_file_location(name, path)
+        mod = importlib.util.module_from_spec(spec)
+        spec.loader.exec_module(mod)
+        return mod
+    # masking (test_masking_cpu.py)
+    mm = load(os.path.join(ref_shim.IV2_MM, "models", "mask.py"), "_ivref_mm_mask")
+    for i, (size, ratio, B) in enumerate((((8, 16, 16), 0.8, 4), ((1, 14, 14), 0.5, 3), ((4, 16, 16), 0.9, 2))):
+        np.random.seed(11); blob[f"mm_tube/{i}"] = mm.TubeMaskingGenerator(size, ratio, B, device="cpu").numpy()
+        np.random.seed(12); blob[f"mm_rand/{i}"] = mm.RandomMaskingGenerator(size, ratio, B, device="cpu").numpy()
+    sm = load(os.path.join(ref_shim.IV2_SM, "datasets", "masking_generator.py"), "_ivref_sm_maskgen")
+    for i, (size, ratio) in enumerate((((8, 14, 14), 0.9), ((4, 16, 16), 0.8))):
+        np.random.seed(5); blob[f"sm_tube/{i}"] = np.stack([sm.TubeMaskingGenerator(size, ratio)() for _ in range(3)])
+        blob[f"sm_tube_repr/{i}"] = _txt(repr(sm.TubeMaskingGenerator(size, ratio)))
+        np.random.seed(6); blob[f"sm_rand/{i}"] = np.stack([sm.RandomMaskingGenerator(size, ratio)() for _ in range(3)])
+    # stage 2 (test_stage2_cpu.py)
+    crit, _ = ref_shim.import_criterions()
+    for hard in (True, False):
+        g = torch.Generator().manual_seed(3)
+        B, Lv, Lt, C = 12, 5, 4, 16
+        vis = torch.randn(B, Lv, C, generator=g); txt = torch.randn(B, Lt, C, generator=g)
+        vp = torch.randn(B, C, generator=g); tp = torch.randn(B, C, generator=g)
+        atts = (torch.rand(B, Lt, generator=g) > 0.3).long()
+        idx = torch.arange(B); idx[7] = 2
+        seen = {}
+
+        def encoder(encoder_embeds, attention_mask, encoder_hidden_states, encoder_attention_mask, return_dict, mode):
+            seen.update(text=encoder_embeds, atts=attention_mask, vision=encoder_hidden_states)
+            return types.SimpleNamespace(last_hidden_state=encoder_embeds)
+        head = torch.nn.Linear(C, 2)
+        torch.manual_seed(77)
+        crit.VTC_VTM_Loss(hard).vtm_loss(encoder, head, 0.07, vis, txt, vp, tp, atts, idx)
+        for k in ("vision", "text", "atts"):
+            blob[f"vtm/{int(hard)}/{k}"] = seen[k].numpy()
+    g = torch.Generator().manual_seed(9)
+    s_ = torch.randn(2, 3, 7, 20, generator=g); c_ = torch.randn(2, 3, 7, 20, generator=g)
+    for norm in ("l2", "none"):
+        for kind in ("l2", "mse", "smooth_l1"):
+            blob[f"uta/{norm}/{kind}"] = crit.UTA_Loss(norm, kind).uta_loss(s_, c_).numpy()
+    v = torch.randn(6, 16, generator=g); t = torch.randn(5, 16, generator=g)
+    for j, a in enumerate(crit.get_sim(v, t, 0.07)):
+        blob[f"sim/vt/{j}"] = a.numpy()
+    v3 = torch.randn(6, 4, 16, generator=g)
+    for agg in ("mean", "max"):
+        for j, a in enumerate(crit.get_sim(v3, t, 0.07, agg)):
+            blob[f"sim/v3t/{agg}/{j}"] = a.numpy()
+    t3 = torch.randn(5, 3, 16, generator=g)
+    for agg in ("mean", "max"):
+        for j, a in enumerate(crit.get_sim(v, t3, 0.07, agg)):
+            blob[f"sim/vt3/{agg}/{j}"] = a.numpy()
+    path = os.path.join(ref_shim.IV2_MM, "tasks_clip", "retrieval_utils.py")
+    src = open(path).read()
+    start = src.index("def itm_eval(")
+    ns = {"np": np}
+    exec(compile(src[start:src.index("\n\n\n", start)] if "\n\n\n" in src[start:] else src[start:], path, "exec"), ns)
+    rg = np.random.default_rng(4)
+    sc = rg.standard_normal((9, 13)).astype(np.float32)
+    txt2img = [int(x) for x in rg.integers(0, 9, 13)]
+    img2txt = [[j for j in range(13) if txt2img[j] == i] or [0] for i in range(9)]
+    blob["itm_eval"] = _txt(json.dumps(ns["itm_eval"](sc, sc.T.copy(), txt2img, img2txt)))
+    # IV1 VideoMAE init (test_videomae_v1_cpu.py)
+    iv1 = ref_shim.import_iv1_videomae()
+    kw = dict(img_size=32, patch_size=16, encoder_embed_dim=128, encoder_depth=1, encoder_num_heads=2, decoder_num_classes=1536,
+              decoder_embed_dim=64, decoder_depth=1, decoder_num_heads=1, qkv_bias=True, init_values=0.1)
+    torch.manual_seed(3); ref = iv1.PretrainVisionTransformer(**kw)
+    blob["iv1/keys"] = _txt("\n".join(ref.state_dict()))
+    for k, w in ref.state_dict().items():
+        blob[f"iv1/shape/{k}"] = np.array(tuple(w.shape), dtype=np.int64)
+        blob[f"iv1/sha/{k}"] = _sha(w)
+    blob["iv1/pos_embed"] = _sha(ref.pos_embed)
+    blob["iv1/encoder_pos_embed"] = _sha(ref.encoder.pos_embed)
+    # position tables (test_modules_cpu.py)
+    sm_mod = ref_shim.import_single_modality()
+    blob["sincos_64_4_2"] = np.asarray(sm_mod.get_3d_sincos_pos_embed(64, 4, 2, cls_token=True), dtype=np.float32)
+    kw = dict(sep_pos_embed=True, embed_dim=64, depth=1, num_heads=2, num_frames=2, img_size=28,
+              clip_teacher_embed_dim=32, clip_teacher_final_dim=16, mae_teacher_embed_dim=64, attn_pool_num_heads=2,
+              clip_embed_dim=16)
+    rs = ref_shim.build_reference_model(**kw).state_dict()
+    blob["sep/keys"] = _txt("\n".join(rs))
+    for k in rs:
+        if "pos_embed" in k:
+            blob[f"sep/{k}"] = rs[k].numpy()
+    ref_shim.import_clip_vision()
+    pe = importlib.import_module("_ivref_mm_backbone.pos_embed")
+    from internvideo_b200.clip_modules import InternVideo2
+    tower = InternVideo2(embed_dim=64, depth=1, num_heads=2, num_frames=8, img_size=112, attn_pool_num_heads=2,
+                         clip_embed_dim=16, use_flash_attn=False, use_fused_rmsnorm=False, use_fused_mlp=False)
+    g = torch.Generator().manual_seed(0)
+    ck = {"vision_encoder.pos_embed": torch.randn(1, 1 + 4 * 16, 64, generator=g)}
+    pe.interpolate_pos_embed(ck, tower, orig_t_size=4)
+    blob["interp_pos_embed"] = ck["vision_encoder.pos_embed"].numpy()
+    # restatement vs reference at InternVideo2-S dims (test_oracle_cpu.py): seeded parameters, sampled outputs
+    kw = dict(embed_dim=384, depth=12, num_heads=6, mlp_ratio=4, num_frames=4, drop_path_rate=0.0,
+              clip_return_layer=1, mae_return_layer=1, attn_pool_num_heads=16, init_values=0.1)
+    model = ref_shim.build_reference_model(**kw).eval()
+    model.load_state_dict(sdims_params({k: tuple(v.shape) for k, v in model.state_dict().items()}), strict=True)
+    torch.manual_seed(0)
+    x, mask = sdims_inputs()
+    with torch.no_grad():
+        outs = model(x, mask)
+    for i, o in enumerate(outs):
+        idx = sdims_sample(o.numel())
+        blob[f"sdims/{i}/shape"] = np.array(tuple(o.shape), dtype=np.int64)
+        blob[f"sdims/{i}"] = o.reshape(-1)[idx].numpy()
+    np.savez_compressed(GOLD / "ref_checks.npz", **blob)
+    print("ref_checks:", len(blob), "arrays")
+
+
 if __name__ == "__main__":
     assert ref_shim.available(), "reference not mounted"
     GOLD.mkdir(parents=True, exist_ok=True)
-    which = sys.argv[1:] or ["pretrain_tiny", "pretrain_d88", "pretrain_dp", "block_cfg2", "clip_small", "teachers", "vtc", "pixel_target", "stage2", "iv1_videomae"]
+    which = sys.argv[1:] or ["pretrain_tiny", "pretrain_d88", "pretrain_dp", "block_cfg2", "clip_small", "teachers", "vtc", "pixel_target", "stage2", "iv1_videomae", "ref_checks"]
     makers = {"pretrain_tiny": make_pretrain_tiny, "pretrain_d88": make_pretrain_d88, "vtc": make_vtc,
               "pixel_target": make_pixel_target, "pretrain_dp": make_pretrain_dp, "block_cfg2": make_block_cfg2,
-              "clip_small": make_clip_small, "teachers": make_teachers, "stage2": make_stage2, "iv1_videomae": make_iv1_videomae}
+              "clip_small": make_clip_small, "teachers": make_teachers, "stage2": make_stage2, "iv1_videomae": make_iv1_videomae,
+              "ref_checks": make_ref_checks}
     for w in which:      # e.g. `python oracle/make_golden.py pretrain_d88` regenerates one fixture only
         makers[w]()

@@ -44,8 +44,15 @@ FILES = [
 ]
 
 
+def _mounted() -> bool:
+    try:
+        return SRC.is_dir()
+    except OSError:          # present but not readable by this user
+        return False
+
+
 def stage(verbose=True) -> bool:
-    if not SRC.is_dir():
+    if not _mounted():
         if verbose:
             print(f"stage_ref: {SRC} not mounted; keeping whatever is already under {DST}")
         return DST.is_dir()

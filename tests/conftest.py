@@ -10,7 +10,7 @@ if str(ROOT) not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a B200 GPU (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 GPU (run with -m gpu on the GPU box)")
 
 
 @pytest.fixture(scope="session")

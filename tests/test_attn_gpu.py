@@ -1,4 +1,4 @@
-"""tcgen05 attention forward/backward vs fp32 softmax attention on the same bf16 inputs (gpu)."""
+"""wgmma attention forward/backward vs fp32 softmax attention on the same bf16 inputs (gpu)."""
 import math
 
 import pytest
@@ -24,8 +24,7 @@ def ref_attn(q, k, v, B, n, H, d, scale):
 
 CASES = [(2, 417, 16, 88), (1, 64, 2, 64), (2, 209, 6, 64), (1, 1025, 4, 64), (1, 833, 5, 128),
          (3, 13, 2, 64), (1, 128, 1, 88), (1, 1568, 2, 88), (1, 129, 3, 128),
-         # more (clip, head, 256-query pair) items than SMs: the persistent forward's cross-item path (stages, barrier
-         # phases and TMEM running across items; inactive second slot; 1, 2, 4 and 9 key tiles per item)
+         # grids larger than one wave, ragged last query / key tiles, 1, 2, 4 and 9 key tiles per block
          (5, 417, 16, 88), (40, 64, 4, 64), (6, 300, 25, 64), (2, 1025, 16, 64), (20, 144, 8, 128), (3, 257, 40, 32)]
 
 

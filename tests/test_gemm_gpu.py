@@ -1,4 +1,4 @@
-"""tcgen05 GEMM vs torch fp32 matmul on the same bf16-rounded operands (gpu)."""
+"""wgmma GEMM vs torch fp32 matmul on the same bf16-rounded operands (gpu)."""
 import pytest
 import torch
 
@@ -114,7 +114,7 @@ def test_gemm_large_full_size(cuda_lib):
     assert torch.equal(out2, out * 2)
 
 
-# ---------------------------------------------------------------- CTA-pair (cta_group::2) kernel
+# ---------------------------------------------------------------- CTA-pair (cluster of 2, multicast B) kernel
 @pytest.mark.parametrize("M,N,K", [(256, 256, 64), (512, 1408, 1408), (1000, 4224, 1408), (417, 6144, 1408),
                                    (834, 1408, 6144), (130, 768, 592), (2049, 1024, 1024)])
 @pytest.mark.parametrize("tile_n", [0, 128, 176, 192, 256])

@@ -1,4 +1,4 @@
-"""Fit attention-backward time to  CTAs/148 * (F + ntile * I): F = per-CTA fixed cost (prologue + epilogue),
+"""Fit attention-backward time to  CTAs/SMs * (F + ntile * I): F = per-CTA fixed cost (prologue + epilogue),
 I = cost per streamed 64-token tile.  B*H = 512 heads of d=88 (cfg-2 head shape), n swept."""
 import sys
 sys.path.insert(0, ".")
@@ -6,6 +6,7 @@ import torch
 from internvideo_b200 import lowlevel as ll
 
 bf = torch.bfloat16
+SMS = torch.cuda.get_device_properties(0).multi_processor_count
 B, H, d = 32, 16, 88
 D = H * d
 res = []
@@ -26,8 +27,8 @@ for n in (128, 256, 384, 417, 512, 768, 1024, 2048):
     rt, nt = (n + 127) // 128, (n + 63) // 64
     ctas = 2 * B * H * rt          # two passes (dK/dV and dQ)
     fl = 2.5 * 4 * n * n * d * B * H
-    print(f"n={n:5d} row_tiles={rt:3d} tiles={nt:3d}  {us:9.1f} us   per-CTA-slot {us * 148 / ctas:7.2f} us   {fl / us / 1e6:7.1f} TFLOP/s", flush=True)
-    res.append((nt, us * 148 / ctas))
+    print(f"n={n:5d} row_tiles={rt:3d} tiles={nt:3d}  {us:9.1f} us   per-CTA-slot {us * SMS / ctas:7.2f} us   {fl / us / 1e6:7.1f} TFLOP/s", flush=True)
+    res.append((nt, us * SMS / ctas))
 import numpy as np
 A = np.array([[1.0, nt] for nt, _ in res]); y = np.array([t for _, t in res])
 (F, I), *_ = np.linalg.lstsq(A, y, rcond=None)

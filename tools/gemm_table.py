@@ -1,6 +1,6 @@
 """Every GEMM shape of the cfg-2 (InternVideo2-1B, B=32, n=417) step — forward (NT), dgrad (NN) and wgrad (TT) — on
 libivb200's default kernel (what the step launches) against cuBLAS via torch.matmul on the same operands.
-usage: python tools/gemm_table.py > profiles/r02_gemm_vs_cublas.md      (device-timed, 20 launches after 3 warm-ups)"""
+usage: python tools/gemm_table.py > gemm_vs_cublas.md      (device-timed, 20 launches after 3 warm-ups)"""
 import json, os, sys
 sys.path.insert(0, ".")
 import torch
@@ -28,7 +28,7 @@ except Exception:
     pass
 M = 13344          # 32 clips x 417 visible tokens
 layers = [("qkv", 1408, 4224), ("proj", 1408, 1408), ("fc1", 1408, 6144), ("fc2", 6144, 1408), ("clip head", 1408, 3200)]
-print("# libivb200 tcgen05 GEMM (default CTA-pair kernel, dynamic tile scheduler) vs cuBLAS, cfg-2 shapes, one B200\n")
+print(f"# libivb200 wgmma GEMM (default single-CTA kernel) vs cuBLAS, cfg-2 shapes, {torch.cuda.get_device_name()}\n")
 print(f"M = {M} tokens; TF/s = 2MNK / device time (CUDA events, 20 launches, same operands for both); "
       f"sustained bf16 peak of this pool {peak} TF/s (MEASURED_PEAKS.json).\n")
 print("| GEMM | role | M x N x K | cuBLAS TF/s | ivb200 TF/s | ivb/cuBLAS | ivb / peak |")

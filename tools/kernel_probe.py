@@ -7,7 +7,6 @@ from internvideo_b200 import lowlevel as ll
 which = sys.argv[1] if len(sys.argv) > 1 else "all"
 bf = torch.bfloat16
 M = 13344
-ll.set_default_2cta(True)
 if which in ("gemm", "all"):
     a = torch.randn(M, 1408, device="cuda").to(bf); w = (torch.randn(6144, 1408, device="cuda") * 0.02).to(bf)
     b = torch.zeros(6144, device="cuda", dtype=bf)

@@ -1,6 +1,6 @@
 """One launch each of the memory-bound kernels at cfg-2 shapes (M = 32*417 rows, D = 1408, decoder width 3200,
 1.07 B-parameter AdamW slice), for an `ncu --metrics dram__bytes_read.sum,dram__bytes_write.sum,gpu__time_duration.sum` pass
-(tools/summarize_membound.py turns the CSV into achieved GB/s vs the measured HBM peak).  Inputs exceed the 126 MB L2
+(bytes over duration gives the achieved GB/s).  Inputs exceed the 50 MB L2
 or the L2 is flushed before each launch."""
 import sys
 sys.path.insert(0, ".")

@@ -1,11 +1,11 @@
 """GPU-side anchors for the headline number (BASELINE.md §4 comparators, reported, not the reference arm): the UNMODIFIED
-reference PretrainInternVideo2-1B on the SAME B200, bf16, training step (fwd + bwd + torch fused AdamW):
+reference PretrainInternVideo2-1B on the same GPU, bf16, training step (fwd + bwd + torch fused AdamW):
   reference-naive : the reference's pure-PyTorch path (use_flash_attn = use_fused_* = False)
   reference-flash : the reference's FlashAttention class (FA2) with its all-or-nothing fused flags on; FA2's
                     DropoutAddRMSNorm / FusedMLP extensions are not installed in this image, so they are provided by
                     the reference's OWN RMSNorm / Mlp wrapped to the fused calling convention (SURVEY §8c).
 Needs the reference sources: /root/reference, or the copies oracle/stage_ref.py staged under oracle/_ref/.
-  python tools/ref_gpu_compare.py [--batch 8] > profiles/r02_reference_gpu_comparators.log"""
+  python tools/ref_gpu_compare.py [--batch 8] > reference_gpu_comparators.log"""
 import argparse
 import sys
 import time
