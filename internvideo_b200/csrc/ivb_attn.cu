@@ -41,8 +41,39 @@ __device__ __forceinline__ float quad_sum(float v) {
   return v + __shfl_xor_sync(0xffffffffu, v, 2);
 }
 
+// Online-softmax update of one S tile in place: S -> P = exp2(S*sc - m_new) (columns >= valid get 0); returns the
+// rescale factor alpha = exp2(m_old - m_new) of each of the thread's two rows, and folds the row sums into l_run.
+__device__ __forceinline__ void softmax_tile(float (&s)[ATT_BKV / 2], int valid, int lane, float sc_log2,
+                                             float m_run[2], float l_run[2], float alpha[2]) {
+  float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+  for (int i = 0; i < ATT_BKV / 2; ++i) {
+    const int col = 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
+    float v = s[i] * sc_log2;
+    if (col >= valid) v = -INFINITY;
+    s[i] = v;
+    mx[(i >> 1) & 1] = fmaxf(mx[(i >> 1) & 1], v);
+  }
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const float m_new = fmaxf(m_run[r], quad_max(mx[r]));
+    alpha[r] = exp2f(m_run[r] - m_new);
+    m_run[r] = m_new;
+  }
+  float rs[2] = {0.f, 0.f};
+#pragma unroll
+  for (int i = 0; i < ATT_BKV / 2; ++i) {
+    const int r = (i >> 1) & 1;
+    s[i] = exp2f(s[i] - m_run[r]);
+    rs[r] += s[i];
+  }
+#pragma unroll
+  for (int r = 0; r < 2; ++r) l_run[r] = l_run[r] * alpha[r] + rs[r];
+}
+
 // KA: number of 64-wide atoms covering head_dim (1: d<=64, 2: d<=128).  NO: wgmma N of P·V (d rounded up).
-template <int KA, int NO>
+// KS: k16 steps of S = Q K^T, ceil(d / 16).
+template <int KA, int NO, int KS>
 __global__ void __launch_bounds__(384, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                 const __grid_constant__ CUtensorMap tmV, const AttnFwdParams p) {
@@ -56,7 +87,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   uint64_t* bar_q = bars;                       // 1
   uint64_t* full_k = bars + 1;                  // ATT_NS
   uint64_t* full_v = full_k + ATT_NS;           // ATT_NS
-  uint64_t* empty_k = full_v + ATT_NS;          // ATT_NS (one arrival per MMA warpgroup)
+  uint64_t* empty_k = full_v + ATT_NS;          // ATT_NS (one arrival per live MMA warpgroup)
   uint64_t* empty_v = empty_k + ATT_NS;         // ATT_NS
 
   const int tid = threadIdx.x;
@@ -67,14 +98,14 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   const int h = blockIdx.y;
   const int b = blockIdx.z;
   const int nblk = (p.n + ATT_BKV - 1) / ATT_BKV;
-  const int ksteps = (p.d + 15) / 16;
+  const int live = min(2, (p.n - q0 + 63) / 64);   // warpgroups that own at least one query < n
 
   if (tid == 0) {
     if ((smem_u32(smem) & 1023u) != 0) __trap();
     mbar_init(bar_q, 1);
     for (int i = 0; i < ATT_NS; ++i) {
       mbar_init(&full_k[i], 1); mbar_init(&full_v[i], 1);
-      mbar_init(&empty_k[i], 2); mbar_init(&empty_v[i], 2);
+      mbar_init(&empty_k[i], live); mbar_init(&empty_v[i], live);
     }
     fence_mbar_init();
   }
@@ -107,7 +138,10 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   } else {
     setmaxnreg_inc<240>();
     // ===================== MMA + softmax warpgroups =====================
+    // Pipelined within the warpgroup: S_{j+1} = Q K_{j+1}^T is issued before O += P_j V_j, so the tensor core runs
+    // both while the softmax of tile j+1 waits only for S_{j+1}; O is rescaled once P_j V_j has retired.
     const int cw = wg - 1;                                  // query rows [64*cw, 64*cw + 64) of the block
+    if (cw >= live) return;
     const bool signal = (tid & 127) == 0;
     const int rloc = cw * 64 + (warp & 3) * 16 + (lane >> 2);  // this thread's rows: rloc, rloc + 8
     const uint32_t qa = smem_u32(sQ) + cw * 8192;
@@ -116,68 +150,61 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     for (int i = 0; i < NO / 2; ++i) o[i] = 0.f;
     float m_run[2] = {-INFINITY, -INFINITY};
     float l_run[2] = {0.f, 0.f};
+    float s[ATT_BKV / 2];
+    float alpha[2];
+    uint32_t pa[ATT_BKV / 16][4];
 
-    mbar_wait(bar_q, 0);
-    for (int j = 0; j < nblk; ++j) {
-      const int st = j % ATT_NS;
-      const uint32_t ph = (j / ATT_NS) & 1;
-      mbar_wait(&full_k[st], ph);
-      const uint32_t ka = smem_u32(sK + st * KV_BYTES);
-      float s[ATT_BKV / 2];
+    auto issue_s = [&](int j) {
+      const uint32_t ka = smem_u32(sK + (j % ATT_NS) * KV_BYTES);
       wgmma_fence();
-      for (int kk = 0; kk < ksteps; ++kk) {
+#pragma unroll
+      for (int kk = 0; kk < KS; ++kk) {
         const uint32_t off = (kk & 3) * 32;
         Wgmma<ATT_BKV>::ss<0, 0>(s, gmma_desc(qa + (kk >> 2) * (ATT_BQ * 128) + off, 16, 1024),
                                  gmma_desc(ka + (kk >> 2) * (ATT_BKV * 128) + off, 16, 1024), kk > 0 ? 1u : 0u);
       }
       wgmma_commit();
-      wgmma_wait<0>();
-      wgmma_reg_fence(s, ATT_BKV / 2);
-      if (signal) mbar_arrive(&empty_k[st]);
+    };
 
-      const int valid = p.n - j * ATT_BKV;  // columns >= valid are beyond the sequence
-      float mx[2] = {-INFINITY, -INFINITY};
+    mbar_wait(bar_q, 0);
+    mbar_wait(&full_k[0], 0);
+    issue_s(0);
+    wgmma_wait<0>();
+    wgmma_reg_fence(s, ATT_BKV / 2);
+    if (signal) mbar_arrive(&empty_k[0]);
+    softmax_tile(s, p.n, lane, p.sc_log2, m_run, l_run, alpha);
 #pragma unroll
-      for (int i = 0; i < ATT_BKV / 2; ++i) {
-        const int col = 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
-        float v = s[i] * p.sc_log2;
-        if (col >= valid) v = -INFINITY;
-        s[i] = v;
-        mx[(i >> 1) & 1] = fmaxf(mx[(i >> 1) & 1], v);
-      }
-      float alpha[2];
-#pragma unroll
-      for (int r = 0; r < 2; ++r) {
-        const float m_new = fmaxf(m_run[r], quad_max(mx[r]));
-        alpha[r] = exp2f(m_run[r] - m_new);
-        m_run[r] = m_new;
-      }
-      float rs[2] = {0.f, 0.f};
-#pragma unroll
-      for (int i = 0; i < ATT_BKV / 2; ++i) {
-        const int r = (i >> 1) & 1;
-        s[i] = exp2f(s[i] - m_run[r]);
-        rs[r] += s[i];
-      }
-#pragma unroll
-      for (int r = 0; r < 2; ++r) l_run[r] = l_run[r] * alpha[r] + rs[r];
-#pragma unroll
-      for (int i = 0; i < NO / 2; ++i) o[i] *= alpha[(i >> 1) & 1];
-      uint32_t pa[ATT_BKV / 16][4];
-#pragma unroll
-      for (int kk = 0; kk < ATT_BKV / 16; ++kk) acc_to_a_frag(s, kk, pa[kk]);
+    for (int kk = 0; kk < ATT_BKV / 16; ++kk) acc_to_a_frag(s, kk, pa[kk]);
 
-      mbar_wait(&full_v[st], ph);
+    auto issue_pv = [&](int j) {
+      const int st = j % ATT_NS;
+      mbar_wait(&full_v[st], (j / ATT_NS) & 1);
       const uint32_t va = smem_u32(sV + st * KV_BYTES);
       wgmma_fence();
 #pragma unroll
       for (int kk = 0; kk < ATT_BKV / 16; ++kk)
         Wgmma<NO>::rs<1>(o, pa[kk], gmma_desc(va + kk * 2048, ATT_BKV * 128, 1024), 1u);
       wgmma_commit();
+    };
+    for (int j = 0; j + 1 < nblk; ++j) {
+      mbar_wait(&full_k[(j + 1) % ATT_NS], ((j + 1) / ATT_NS) & 1);
+      issue_s(j + 1);
+      issue_pv(j);
+      wgmma_wait<1>();
+      wgmma_reg_fence(s, ATT_BKV / 2);
+      if (signal) mbar_arrive(&empty_k[(j + 1) % ATT_NS]);
+      softmax_tile(s, p.n - (j + 1) * ATT_BKV, lane, p.sc_log2, m_run, l_run, alpha);
       wgmma_wait<0>();
       wgmma_reg_fence(o, NO / 2);
-      if (signal) mbar_arrive(&empty_v[st]);
+      if (signal) mbar_arrive(&empty_v[j % ATT_NS]);
+#pragma unroll
+      for (int i = 0; i < NO / 2; ++i) o[i] *= alpha[(i >> 1) & 1];
+#pragma unroll
+      for (int kk = 0; kk < ATT_BKV / 16; ++kk) acc_to_a_frag(s, kk, pa[kk]);
     }
+    issue_pv(nblk - 1);
+    wgmma_wait<0>();
+    wgmma_reg_fence(o, NO / 2);
 
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
@@ -208,11 +235,11 @@ int make_head_tmap(CUtensorMap* tm, const void* base, long ld, int B, int n, int
   return make_tmap_4d(tm, base, dims, strides, box);
 }
 
-template <int KA, int NO>
+template <int KA, int NO, int KS>
 static int launch_attn_fwd(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv,
                            const AttnFwdParams& p, cudaStream_t stream) {
   constexpr int SMEM = KA * ATT_BQ * 128 + 2 * ATT_NS * KA * ATT_BKV * 128 + 128;  // tiles + barriers
-  auto kern = attn_fwd_kernel<KA, NO>;
+  auto kern = attn_fwd_kernel<KA, NO, KS>;
   static bool attr_set[64] = {};
   if (first_use_on_device(attr_set)) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM);
@@ -222,6 +249,14 @@ static int launch_attn_fwd(const CUtensorMap& tq, const CUtensorMap& tk, const C
   kern<<<grid, 384, SMEM, stream>>>(tq, tk, tv, p);
   count_launch();
   return check_launch("attn_fwd_kernel");
+}
+
+// A head_dim with P·V width NO needs NO/16 or NO/16 - 1 k16 steps.
+template <int KA, int NO>
+static int dispatch_fwd_ks(int d, const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv,
+                           const AttnFwdParams& p, cudaStream_t stream) {
+  if ((d + 15) / 16 == NO / 16) return launch_attn_fwd<KA, NO, NO / 16>(tq, tk, tv, p, stream);
+  return launch_attn_fwd<KA, NO, NO / 16 - 1>(tq, tk, tv, p, stream);
 }
 
 }  // namespace ivb
@@ -246,11 +281,11 @@ extern "C" int ivb_attn_fwd(const void* q, long ldq, const void* k, long ldk, co
   p.out = reinterpret_cast<__nv_bfloat16*>(out); p.ldo = ldo; p.lse2 = lse2;
   const int no = (d + 31) / 32 * 32;
   if (d <= 64) {
-    if (no <= 32) return launch_attn_fwd<1, 32>(tq, tk, tv, p, stream);
-    return launch_attn_fwd<1, 64>(tq, tk, tv, p, stream);
+    if (no <= 32) return dispatch_fwd_ks<1, 32>(d, tq, tk, tv, p, stream);
+    return dispatch_fwd_ks<1, 64>(d, tq, tk, tv, p, stream);
   }
-  if (no <= 96) return launch_attn_fwd<2, 96>(tq, tk, tv, p, stream);
-  return launch_attn_fwd<2, 128>(tq, tk, tv, p, stream);
+  if (no <= 96) return dispatch_fwd_ks<2, 96>(d, tq, tk, tv, p, stream);
+  return dispatch_fwd_ks<2, 128>(d, tq, tk, tv, p, stream);
 }
 
 // ---------------------------------------------------------------------------------------------------------------

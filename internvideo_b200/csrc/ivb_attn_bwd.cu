@@ -16,10 +16,15 @@
 // other, only the wgmma descriptor differs.
 //
 // Warp roles (384 threads): warpgroup 0 = the TMA producer (one elected thread), warpgroups 1 and 2 own 64 of the
-// 128 rows each.  mbarriers only:
+// 128 rows each.  A warpgroup whose 64 rows all lie beyond the sequence does no work at all.  mbarriers:
 //   bar_row     TMA -> MMA        X,Y (the 128 owned rows) landed
-//   full[s]     TMA -> MMA        streamed tiles U_j, W_j of stage s landed (tx)
-//   empty[s]    MMA -> TMA        both warpgroups retired every MMA that reads stage s
+//   full[s]     TMA -> MMA        streamed tiles U_j, W_j of stage s landed (tx); MODE 1 also lse2/delta of the
+//                                 tile's 64 queries, so the math reads them from shared memory
+//   empty[s]    MMA -> TMA        every live warpgroup retired every MMA that reads stage s
+// When both warpgroups are live they take turns issuing S/dP (named barriers 1 and 2): one warpgroup's MMAs run on
+// the tensor core while the other computes P / dS.  Software pipelining inside a warpgroup (S/dP of tile j+1 in
+// flight during the math of tile j) does not fit the register file at d > 64 in MODE 1: dK + dV take NO registers,
+// two S/dP tiles 128 and the A fragments 32.
 #include <math.h>
 #include <stdlib.h>
 
@@ -71,22 +76,26 @@ __global__ void attn_bwd_prep_kernel(const __nv_bfloat16* __restrict__ o, long l
   lse2p[(b * H + h) * n_pad + q] = lse2[(b * H + h) * n + q];
 }
 
-constexpr int BWD_NST = 2;  // streamed-tile stages
+constexpr int BWD_NST = 3;  // streamed-tile stages
 
-// KA: 64-wide atoms covering head_dim (1: d <= 64, 2: d <= 128); NO: wgmma N of the accumulate MMAs.
-template <int MODE, int KA, int NO>
+// KA: 64-wide atoms covering head_dim (1: d <= 64, 2: d <= 128); NO: wgmma N of the accumulate MMAs;
+// KS: k16 steps of the S/dP MMAs, ceil(d / 16).
+template <int MODE, int KA, int NO, int KS>
 __global__ void __launch_bounds__(384, 1)
 attn_bwd_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmY,
                 const __grid_constant__ CUtensorMap tmU, const __grid_constant__ CUtensorMap tmW,
                 const AttnBwdParams p) {
   constexpr int ROW_BYTES = KA * BWD_ROWS * 128;   // one owned-row operand
   constexpr int COL_BYTES = KA * BWD_COLS * 128;   // one streamed tile
+  constexpr int VEC_BYTES = BWD_COLS * 4;          // lse2 or delta of one streamed tile (MODE 1)
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* sX = smem;
   uint8_t* sY = sX + ROW_BYTES;
   uint8_t* sU = sY + ROW_BYTES;                 // BWD_NST stages
   uint8_t* sW = sU + BWD_NST * COL_BYTES;       // BWD_NST stages
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sW + BWD_NST * COL_BYTES);
+  float* sLse = reinterpret_cast<float*>(sW + BWD_NST * COL_BYTES);   // BWD_NST x 64
+  float* sDelta = sLse + BWD_NST * BWD_COLS;                          // BWD_NST x 64
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sDelta + BWD_NST * BWD_COLS);
   uint64_t* bar_row = bars;
   uint64_t* full = bars + 1;
   uint64_t* empty = full + BWD_NST;
@@ -99,12 +108,13 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__
   const int h = blockIdx.y;
   const int b = blockIdx.z;
   const int nblk = (p.n + BWD_COLS - 1) / BWD_COLS;
-  const int ksteps = (p.d + 15) / 16;
+  const int live = min(2, (p.n - r0 + 63) / 64);   // warpgroups that own at least one row < n
+  const long hb = (static_cast<long>(b) * p.H + h) * p.n_pad;
 
   if (tid == 0) {
     if ((smem_u32(smem) & 1023u) != 0) __trap();
     mbar_init(bar_row, 1);
-    for (int i = 0; i < BWD_NST; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 2); }
+    for (int i = 0; i < BWD_NST; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], live); }
     fence_mbar_init();
   }
   __syncthreads();
@@ -125,11 +135,15 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__
       for (int j = 0; j < nblk; ++j) {
         const int st = j % BWD_NST;
         mbar_wait(&empty[st], ((j / BWD_NST) & 1) ^ 1);
-        mbar_expect_tx(&full[st], 2 * COL_BYTES);
+        mbar_expect_tx(&full[st], 2 * COL_BYTES + (MODE == 1 ? 2 * VEC_BYTES : 0));
 #pragma unroll
         for (int a = 0; a < KA; ++a) {
           tma_load_4d(sU + st * COL_BYTES + a * (BWD_COLS * 128), &tmU, a * 64, h, j * BWD_COLS, b, &full[st]);
           tma_load_4d(sW + st * COL_BYTES + a * (BWD_COLS * 128), &tmW, a * 64, h, j * BWD_COLS, b, &full[st]);
+        }
+        if (MODE == 1) {   // the padded workspaces hold whole 64-query tiles, 256-byte aligned
+          bulk_load_1d(sLse + st * BWD_COLS, p.lse2p + hb + j * BWD_COLS, VEC_BYTES, &full[st]);
+          bulk_load_1d(sDelta + st * BWD_COLS, p.deltap + hb + j * BWD_COLS, VEC_BYTES, &full[st]);
         }
       }
     }
@@ -137,10 +151,11 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__
     setmaxnreg_inc<240>();
     // ===================== MMA + math warpgroups =====================
     const int cw = wg - 1;
+    if (cw >= live) return;
+    const bool pingpong = live == 2;
     const bool signal = (tid & 127) == 0;
     const int rloc = cw * 64 + (warp & 3) * 16 + (lane >> 2);  // this thread's rows: rloc, rloc + 8
     const uint32_t xa = smem_u32(sX) + cw * 8192, ya = smem_u32(sY) + cw * 8192;
-    const long hb = (static_cast<long>(b) * p.H + h) * p.n_pad;
     float acc1[NO / 2];                     // MODE 1: dV   MODE 0: dQ
     float acc2[MODE == 1 ? NO / 2 : 1];     // MODE 1: dK
 #pragma unroll
@@ -156,20 +171,26 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__
       }
     }
 
+    // Named barrier 1 + cw: "warpgroup cw may issue S/dP".  Warpgroup 0 goes first.
+    if (pingpong && cw == 1) named_bar_arrive(1, 256);
     mbar_wait(bar_row, 0);
     for (int j = 0; j < nblk; ++j) {
       const int st = j % BWD_NST;
       mbar_wait(&full[st], (j / BWD_NST) & 1);
       const uint32_t ua = smem_u32(sU + st * COL_BYTES), wa = smem_u32(sW + st * COL_BYTES);
       float sc[BWD_COLS / 2], dp[BWD_COLS / 2];
+      if (pingpong) named_bar_sync(1 + cw, 256);
       wgmma_fence();
-      for (int kk = 0; kk < ksteps; ++kk) {
+#pragma unroll
+      for (int kk = 0; kk < KS; ++kk) {
         const uint32_t off = (kk & 3) * 32;
         const uint32_t ro = (kk >> 2) * (BWD_ROWS * 128) + off, co = (kk >> 2) * (BWD_COLS * 128) + off;
         Wgmma<BWD_COLS>::ss<0, 0>(sc, gmma_desc(xa + ro, 16, 1024), gmma_desc(ua + co, 16, 1024), kk > 0 ? 1u : 0u);
         Wgmma<BWD_COLS>::ss<0, 0>(dp, gmma_desc(ya + ro, 16, 1024), gmma_desc(wa + co, 16, 1024), kk > 0 ? 1u : 0u);
       }
       wgmma_commit();
+      // Hand the turn over; warpgroup 1 skips its last hand-over, which no one would wait for.
+      if (pingpong && !(cw == 1 && j == nblk - 1)) named_bar_arrive(2 - cw, 256);
       wgmma_wait<0>();
       wgmma_reg_fence(sc, BWD_COLS / 2);
       wgmma_reg_fence(dp, BWD_COLS / 2);
@@ -177,26 +198,29 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__
       // P and dS in place of S and dP.  Columns beyond the sequence get P = 0.
 #pragma unroll
       for (int i = 0; i < BWD_COLS / 2; ++i) {
-        const int col = j * BWD_COLS + 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
+        const int c = 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
         float lse, dl;
-        if (MODE == 1) { lse = p.lse2p[hb + col]; dl = p.deltap[hb + col]; }
+        if (MODE == 1) { lse = sLse[st * BWD_COLS + c]; dl = sDelta[st * BWD_COLS + c]; }
         else { lse = row_lse[(i >> 1) & 1]; dl = row_delta[(i >> 1) & 1]; }
-        const float pv = col < p.n ? exp2f(fmaf(sc[i], p.sc_log2, -lse)) : 0.f;
+        const float pv = j * BWD_COLS + c < p.n ? exp2f(fmaf(sc[i], p.sc_log2, -lse)) : 0.f;
         sc[i] = pv;
         dp[i] = pv * (dp[i] - dl) * p.scale;
+      }
+      // Every A fragment is built before the fence: no register an in-flight wgmma reads is written after it.
+      uint32_t pf[MODE == 1 ? BWD_COLS / 16 : 1][4], sf[BWD_COLS / 16][4];
+#pragma unroll
+      for (int kk = 0; kk < BWD_COLS / 16; ++kk) {
+        if (MODE == 1) acc_to_a_frag(sc, kk, pf[kk]);
+        acc_to_a_frag(dp, kk, sf[kk]);
       }
       wgmma_fence();
 #pragma unroll
       for (int kk = 0; kk < BWD_COLS / 16; ++kk) {
-        uint32_t fa[4];
         if (MODE == 1) {
-          acc_to_a_frag(sc, kk, fa);
-          Wgmma<NO>::rs<1>(acc1, fa, gmma_desc(wa + kk * 2048, BWD_COLS * 128, 1024), 1u);   // dV += P^T dO
-          acc_to_a_frag(dp, kk, fa);
-          Wgmma<NO>::rs<1>(acc2, fa, gmma_desc(ua + kk * 2048, BWD_COLS * 128, 1024), 1u);   // dK += dS^T Q
+          Wgmma<NO>::rs<1>(acc1, pf[kk], gmma_desc(wa + kk * 2048, BWD_COLS * 128, 1024), 1u);   // dV += P^T dO
+          Wgmma<NO>::rs<1>(acc2, sf[kk], gmma_desc(ua + kk * 2048, BWD_COLS * 128, 1024), 1u);   // dK += dS^T Q
         } else {
-          acc_to_a_frag(dp, kk, fa);
-          Wgmma<NO>::rs<1>(acc1, fa, gmma_desc(ua + kk * 2048, BWD_COLS * 128, 1024), 1u);   // dQ += dS K
+          Wgmma<NO>::rs<1>(acc1, sf[kk], gmma_desc(ua + kk * 2048, BWD_COLS * 128, 1024), 1u);   // dQ += dS K
         }
       }
       wgmma_commit();
@@ -225,12 +249,12 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__
   }
 }
 
-template <int MODE, int KA, int NO>
+template <int MODE, int KA, int NO, int KS>
 static int launch_attn_bwd(const CUtensorMap& tx, const CUtensorMap& ty, const CUtensorMap& tu,
                            const CUtensorMap& tw, const AttnBwdParams& p, cudaStream_t stream) {
-  constexpr int SMEM = 2 * KA * BWD_ROWS * 128 + 2 * BWD_NST * KA * BWD_COLS * 128 + 128;
+  constexpr int SMEM = 2 * KA * BWD_ROWS * 128 + 2 * BWD_NST * KA * BWD_COLS * 128 + 2 * BWD_NST * BWD_COLS * 4 + 128;
   static_assert(SMEM <= 227 * 1024, "attention backward: shared-memory budget");
-  auto kern = attn_bwd_kernel<MODE, KA, NO>;
+  auto kern = attn_bwd_kernel<MODE, KA, NO, KS>;
   static bool attr_set[64] = {};
   if (first_use_on_device(attr_set)) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM);
@@ -243,16 +267,24 @@ static int launch_attn_bwd(const CUtensorMap& tx, const CUtensorMap& ty, const C
   return check_launch("attn_bwd_kernel");
 }
 
+// A head_dim with accumulate width NO needs NO/16 or NO/16 - 1 k16 steps.
+template <int MODE, int KA, int NO>
+static int dispatch_bwd_ks(int d, const CUtensorMap& tx, const CUtensorMap& ty, const CUtensorMap& tu,
+                           const CUtensorMap& tw, const AttnBwdParams& p, cudaStream_t stream) {
+  if ((d + 15) / 16 == NO / 16) return launch_attn_bwd<MODE, KA, NO, NO / 16>(tx, ty, tu, tw, p, stream);
+  return launch_attn_bwd<MODE, KA, NO, NO / 16 - 1>(tx, ty, tu, tw, p, stream);
+}
+
 template <int MODE>
 static int dispatch_bwd(int d, const CUtensorMap& tx, const CUtensorMap& ty, const CUtensorMap& tu,
                         const CUtensorMap& tw, const AttnBwdParams& p, cudaStream_t stream) {
   const int no = (d + 31) / 32 * 32;
   if (d <= 64) {
-    if (no <= 32) return launch_attn_bwd<MODE, 1, 32>(tx, ty, tu, tw, p, stream);
-    return launch_attn_bwd<MODE, 1, 64>(tx, ty, tu, tw, p, stream);
+    if (no <= 32) return dispatch_bwd_ks<MODE, 1, 32>(d, tx, ty, tu, tw, p, stream);
+    return dispatch_bwd_ks<MODE, 1, 64>(d, tx, ty, tu, tw, p, stream);
   }
-  if (no <= 96) return launch_attn_bwd<MODE, 2, 96>(tx, ty, tu, tw, p, stream);
-  return launch_attn_bwd<MODE, 2, 128>(tx, ty, tu, tw, p, stream);
+  if (no <= 96) return dispatch_bwd_ks<MODE, 2, 96>(d, tx, ty, tu, tw, p, stream);
+  return dispatch_bwd_ks<MODE, 2, 128>(d, tx, ty, tu, tw, p, stream);
 }
 
 }  // namespace ivb

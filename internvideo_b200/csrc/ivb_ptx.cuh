@@ -156,6 +156,10 @@ __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.
 __device__ __forceinline__ void named_bar_sync(int id, int threads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
 }
+// Arrive on a named barrier without waiting for it; it completes once `threads` threads have arrived or synced on it.
+__device__ __forceinline__ void named_bar_arrive(int id, int threads) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
 
 // ---------------------------------------------------------------- wgmma m64nNk16, bf16 x bf16 -> f32
 // d: N/2 fp32 accumulators per thread (layout: row = 16*(warp%4) + lane/4 + 8*((i>>1)&1),
