@@ -121,7 +121,8 @@ int ivb_colsum_bf16(const void* x, long ldx, int M, int N, float* out, void* str
  * buffers; `q` points at (token 0, head 0, dim 0) of its slot, heads are contiguous (h d), so the
  * packed qkv[B,S,3,H,d] layout of FlashAttention.forward (flash_attention_class.py:27-50) is passed
  * as q=qkv, k=qkv+H*d, v=qkv+2*H*d with ld=3*H*d.  lse2[B,H,n] (optional) = log2-domain logsumexp
- * of the scaled scores, consumed by ivb_attn_bwd.  head_dim: multiple of 8, <= 128 (64/88/128).   */
+ * of the scaled scores, consumed by ivb_attn_bwd.  head_dim: multiple of 8 in [16, 128] (the model
+ * uses 64/88/128); every pitch a multiple of 8.  B = 0 or n = 0 is a no-op.                           */
 int ivb_attn_fwd(const void* q, long ldq, const void* k, long ldk, const void* v, long ldv,
                  void* out, long ldo, float* lse2, int B, int n, int H, int d, float softmax_scale,
                  void* stream);
@@ -207,7 +208,8 @@ int ivb_mse_loss(const void* pred_bf16, const float* label, long n, float* loss_
 
 /* ---- single-query attention pooling (AttentionPoolingBlock / CrossAttention with 1 query per clip,
  * internvideo2_pretrain.py:61-76,107-114).  q: bf16 [B, H*d]; k, v: bf16 [B*n, ld]; out: bf16 [B, H*d];
- * probs: fp32 [B,H,n] (saved for the backward).  dq/dk/dv are written, not accumulated.               */
+ * probs: fp32 [B,H,n] (saved for the backward).  dq/dk/dv are written, not accumulated.  The scores of
+ * one (clip, head) live in 48 KB of shared memory: n <= 12280 - d (forward), n <= 12280 - 2d (backward). */
 int ivb_pool_attn_fwd(const void* q, const void* k, long ldk, const void* v, long ldv, int B, int n,
                       int H, int d, float scale, void* out, float* probs, void* stream);
 int ivb_pool_attn_bwd(const void* q, const void* k, long ldk, const void* v, long ldv,
