@@ -46,11 +46,14 @@ extern "C" {
 
 #define IVB_FLAG_GELU_TANH 1 /* tanh-approx GELU (FA2 FusedMLP) instead of erf (nn.GELU)           */
 #define IVB_FLAG_ACCUM 2     /* accumulate into out0                                               */
-#define IVB_FLAG_1CTA 4      /* force the single-CTA kernel (128-row tiles)                                      */
+#define IVB_FLAG_1CTA 4      /* force the cooperative single-CTA kernel (128-row tiles, both MMA warpgroups on one tile) */
 #define IVB_FLAG_2CTA 8      /* force the CTA-pair kernel (cluster of 2, 256-row tiles, B tile TMA-multicast)     */
 #define IVB_FLAG_GELU_SAVE_GRAD 16 /* EPI_BIAS_GELU: out1 receives gelu'(h) instead of h; EPI_GELU_BWD: aux IS
                                      that saved derivative (out0 = acc * aux) — the backward epilogue then has
                                      no transcendental work (the training path; h itself is never needed)   */
+#define IVB_FLAG_PINGPONG 32 /* force the ping-pong kernel (one 128 x 128 tile per MMA warpgroup, each tile's epilogue
+                                under the other warpgroup's MMAs); tile_n must be 0 or 128.  For tests and tools:
+                                the library picks ping-pong or cooperative by itself                                 */
 
 /* ---- status ---------------------------------------------------------------------------------- */
 const char* ivb_last_error(void);

@@ -18,6 +18,10 @@
 //                   (accumulator fragments -> per-warp smem staging tile -> row segments -> global)
 // The ring keeps streaming the next tile's operands while the MMA warpgroups run the epilogue.
 //
+// Ping-pong form (gemm_bf16_pingpong_kernel, the default for most shapes, see use_pingpong): same producer, ring and
+// epilogue, but each MMA warpgroup owns a whole 128 x 128 tile and the two alternate, so one runs its epilogue while
+// the other issues its MMAs.
+//
 // CL = 2 (the CTA-pair form, IVB_FLAG_2CTA / ivb_set_default_2cta): a cluster of two CTAs on neighbouring SMs computes
 // a 256 x BN tile.  Each CTA loads its own 128 A rows and HALF of the B tile, which TMA multicasts into both CTAs'
 // rings, so B is read from L2 once per 256 rows instead of once per 128.  A stage is refilled only when the MMA
@@ -43,7 +47,45 @@ struct GemmCfg {
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + EPI_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
 };
 
-// ------------------------------------------------------------------ the kernel
+// ------------------------------------------------------------------ epilogue of one warpgroup's 64 x BN accumulators
+// 32 columns at a time: fragments -> the warp's 16 x 32 staging tile -> one 16-column row segment per thread.
+// row0: first row of the warpgroup's 64-row band.
+template <int BN>
+__device__ __forceinline__ void epilogue_band(const GemmParams& p, const float* acc, float* st, long row0, int n0) {
+  const int lane = threadIdx.x & 31;
+  const int wr = (threadIdx.x >> 5) & 3;   // warp inside the warpgroup: accumulator rows [16*wr, 16*wr + 16)
+  const long row = row0 + wr * 16 + (lane >> 1);
+  const int half = lane & 1;
+#pragma unroll
+  for (int c = 0; c < (BN + 31) / 32; ++c) {
+#pragma unroll
+    for (int jj = 0; jj < 4; ++jj) {
+      const int j = 4 * c + jj;
+      if (j < BN / 8) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+          *reinterpret_cast<float2*>(st + ((lane >> 2) + 8 * h) * EPI_PITCH + 8 * jj + 2 * (lane & 3)) =
+              make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+      }
+    }
+    __syncwarp();
+    const int col = c * 32 + half * 16;
+    if (col < BN && row < p.M) {
+      uint32_t bits[16];
+      const float* src = st + (lane >> 1) * EPI_PITCH + half * 16;
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const float4 v = reinterpret_cast<const float4*>(src)[i];
+        bits[4 * i] = __float_as_uint(v.x); bits[4 * i + 1] = __float_as_uint(v.y);
+        bits[4 * i + 2] = __float_as_uint(v.z); bits[4 * i + 3] = __float_as_uint(v.w);
+      }
+      epilogue_chunk<16>(p, bits, row, n0 + col);
+    }
+    __syncwarp();
+  }
+}
+
+// ------------------------------------------------------------------ the cooperative kernel
 template <int BN, bool A_MN, bool B_MN, int CL>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
@@ -61,7 +103,6 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   uint64_t* empty = bars + STAGES;
 
   const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
   const int wg = threadIdx.x >> 7;
 
   const uint32_t rank = CL == 2 ? cluster_ctarank() : 0;   // 128-row half of the cluster's tile
@@ -133,7 +174,6 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     setmaxnreg_inc<232>();
     // ===================== MMA + epilogue warpgroups =====================
     const int cw = wg - 1;              // rows [64*cw, 64*cw + 64) of the tile
-    const int wr = warp & 3;            // warp inside the warpgroup: accumulator rows [16*wr, 16*wr + 16)
     const bool signal = (threadIdx.x & 127) == 0;
     auto release = [&](int s_) {   // this warpgroup no longer reads stage s_ (of either CTA's ring)
       if (!signal) return;
@@ -171,40 +211,139 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       wgmma_wait<0>();
       wgmma_reg_fence(acc, BN / 2);
       release(prev);
-
-      // epilogue, 32 columns at a time: fragments -> staging tile -> one 16-column row segment per thread
-      const long row = m0 + cw * 64 + wr * 16 + (lane >> 1);
-      const int half = lane & 1;
-#pragma unroll
-      for (int c = 0; c < (BN + 31) / 32; ++c) {
-#pragma unroll
-        for (int jj = 0; jj < 4; ++jj) {
-          const int j = 4 * c + jj;
-          if (j < BN / 8) {
-#pragma unroll
-            for (int h = 0; h < 2; ++h)
-              *reinterpret_cast<float2*>(st + ((lane >> 2) + 8 * h) * EPI_PITCH + 8 * jj + 2 * (lane & 3)) =
-                  make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
-          }
-        }
-        __syncwarp();
-        const int col = c * 32 + half * 16;
-        if (col < BN && row < p.M) {
-          uint32_t bits[16];
-          const float* src = st + (lane >> 1) * EPI_PITCH + half * 16;
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const float4 v = reinterpret_cast<const float4*>(src)[i];
-            bits[4 * i] = __float_as_uint(v.x); bits[4 * i + 1] = __float_as_uint(v.y);
-            bits[4 * i + 2] = __float_as_uint(v.z); bits[4 * i + 3] = __float_as_uint(v.w);
-          }
-          epilogue_chunk<16>(p, bits, row, n0 + col);
-        }
-        __syncwarp();
-      }
+      epilogue_band<BN>(p, acc, st, m0 + cw * 64, n0);
     }
   }
   if (CL == 2) cluster_sync_all();   // the peer may still multicast into / arrive on this CTA's ring
+}
+
+// ------------------------------------------------------------------ the ping-pong kernel
+// Same producer, ring and epilogue as the cooperative kernel at BN = 128, but each MMA warpgroup owns a whole 128 x 128
+// tile: the CTA's j-th tile (static persistent order) goes to warpgroup j & 1, which issues two m64n128k16 wgmmas per
+// k16 step, one per 64-row half of the A stage.  The producer streams the tiles' k-blocks in that same order, and a
+// token passed between the warpgroups on named barriers 1 and 2 keeps the ring consumed strictly in order: a warpgroup
+// takes the token before its first k-block of a tile and hands it on as soon as the tile's last wgmma is committed,
+// so the other warpgroup's MMAs queue behind them while this one waits for its MMAs and runs the epilogue.  The
+// tensor cores stay busy through every epilogue except the CTA's last.
+constexpr int PP_BN = 128;
+
+template <bool A_MN, bool B_MN>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+gemm_bf16_pingpong_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                          const GemmParams p) {
+  using Cfg = GemmCfg<PP_BN, B_MN>;
+  constexpr int STAGES = Cfg::STAGES;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
+                                             ~static_cast<uintptr_t>(1023));
+  uint8_t* smem_a = smem;
+  uint8_t* smem_b = smem + STAGES * A_STAGE_BYTES;
+  float* epi = reinterpret_cast<float*>(smem + STAGES * Cfg::STAGE_BYTES);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES + EPI_BYTES);
+  uint64_t* full = bars;
+  uint64_t* empty = bars + STAGES;
+
+  const int warp = threadIdx.x >> 5;
+  const int wg = threadIdx.x >> 7;
+  const int num_n = (p.N + PP_BN - 1) / PP_BN;
+  const int num_tiles = ((p.M + BM - 1) / BM) * num_n;
+  const int num_kb = (p.K + BK - 1) / BK;
+
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmA);
+    tma_prefetch_desc(&tmB);
+    for (int i = 0; i < STAGES; ++i) {
+      mbar_init(&full[i], 1);
+      mbar_init(&empty[i], 1);  // each stage is read by exactly one MMA warpgroup
+    }
+    fence_mbar_init();
+  }
+  __syncthreads();
+  pdl_wait();
+  pdl_launch_dependents();
+
+  if (wg == 0) {
+    setmaxnreg_dec<40>();
+    if (warp == 0 && elect_one()) {
+      // ===================== TMA producer: every k-block of every tile of this CTA, in tile order =====================
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        const int m0 = (tile / num_n) * BM;
+        const int n0 = (tile % num_n) * PP_BN;
+        for (int kb = 0; kb < num_kb; ++kb) {
+          mbar_wait(&empty[stage], phase ^ 1);
+          mbar_expect_tx(&full[stage], Cfg::STAGE_BYTES);
+          uint8_t* sa = smem_a + stage * A_STAGE_BYTES;
+          uint8_t* sb = smem_b + stage * Cfg::B_STAGE_BYTES;
+          const int k0 = kb * BK;
+          if (!A_MN) {
+            tma_load_2d(sa, &tmA, k0, m0, &full[stage]);
+          } else {
+#pragma unroll
+            for (int i = 0; i < BM / 64; ++i)
+              tma_load_2d(sa + i * 8192, &tmA, m0 + i * 64, k0, &full[stage]);
+          }
+          if (!B_MN) {
+            tma_load_2d(sb, &tmB, k0, n0, &full[stage]);
+          } else {
+#pragma unroll
+            for (int i = 0; i < Cfg::B_ATOMS; ++i)
+              tma_load_2d(sb + i * 8192, &tmB, n0 + i * 64, k0, &full[stage]);
+          }
+          if (++stage == STAGES) { stage = 0; phase ^= 1; }
+        }
+      }
+    }
+  } else {
+    setmaxnreg_inc<232>();
+    // ===================== MMA + epilogue warpgroups, one whole tile each =====================
+    const int cw = wg - 1;              // this warpgroup takes the CTA's tiles j with (j & 1) == cw
+    const bool signal = (threadIdx.x & 127) == 0;
+    float* st = epi + (warp - 4) * 16 * EPI_PITCH;
+    float acc[2][PP_BN / 2];            // rows [0, 64) and [64, 128) of the tile
+    for (int j = cw, tile = blockIdx.x + cw * gridDim.x; tile < num_tiles; j += 2, tile += 2 * gridDim.x) {
+      const int m0 = (tile / num_n) * BM;
+      const int n0 = (tile % num_n) * PP_BN;
+      const int it = j * num_kb;        // ring position of this tile's first k-block
+      int stage = it % STAGES;
+      uint32_t phase = (it / STAGES) & 1;
+      // the token: the other warpgroup has committed every MMA of the previous tile (tile 0 needs none)
+      if (j > 0) named_bar_sync(1 + cw, 256);
+      int prev = 0;
+      for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait(&full[stage], phase);
+        const uint32_t sa = smem_u32(smem_a + stage * A_STAGE_BYTES);
+        const uint32_t sb = smem_u32(smem_b + stage * Cfg::B_STAGE_BYTES);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BK / 16; ++k) {
+          const uint64_t bd = B_MN ? gmma_desc(sb + k * 2048, 8192, 1024) : gmma_desc(sb + k * 32, 16, 1024);
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const uint64_t ad = A_MN ? gmma_desc(sa + h * 8192 + k * 2048, 8192, 1024)
+                                     : gmma_desc(sa + h * 8192 + k * 32, 16, 1024);
+            Wgmma<PP_BN>::template ss<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc[h], ad, bd, (kb > 0 || k > 0) ? 1u : 0u);
+          }
+        }
+        wgmma_commit();
+        if (kb > 0) {  // the MMAs of the previous k-block retired: its smem slot is free
+          wgmma_wait<1>();
+          if (signal) mbar_arrive(&empty[prev]);
+        }
+        prev = stage;
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      }
+      // hand the token on (only if the CTA has a next tile: an arrival nobody waits for would outlive the CTA)
+      if (tile + gridDim.x < num_tiles) named_bar_arrive(2 - cw, 256);
+      wgmma_wait<0>();
+      wgmma_reg_fence(acc[0], PP_BN / 2);
+      wgmma_reg_fence(acc[1], PP_BN / 2);
+      if (signal) mbar_arrive(&empty[prev]);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) epilogue_band<PP_BN>(p, acc[h], st, m0 + h * 64, n0);
+    }
+  }
 }
 
 // ------------------------------------------------------------------ host side
@@ -253,6 +392,39 @@ static int launch_gemm(const void* A, long lda, const void* B, long ldb, const G
   return check_launch("gemm_bf16_kernel");
 }
 
+template <bool A_MN, bool B_MN>
+static int launch_gemm_pingpong(const void* A, long lda, const void* B, long ldb, const GemmParams& p,
+                                cudaStream_t stream) {
+  using Cfg = GemmCfg<PP_BN, B_MN>;
+  CUtensorMap tmA, tmB;
+  int rc;
+  if (!A_MN) rc = make_tmap_2d(&tmA, A, (uint64_t)p.K, (uint64_t)p.M, lda, 64, BM);
+  else       rc = make_tmap_2d(&tmA, A, (uint64_t)p.M, (uint64_t)p.K, lda, 64, 64);
+  if (rc) return rc;
+  if (!B_MN) rc = make_tmap_2d(&tmB, B, (uint64_t)p.K, (uint64_t)p.N, ldb, 64, PP_BN);
+  else       rc = make_tmap_2d(&tmB, B, (uint64_t)p.N, (uint64_t)p.K, ldb, 64, 64);
+  if (rc) return rc;
+  auto kern = gemm_bf16_pingpong_kernel<A_MN, B_MN>;
+  static bool attr_set[64] = {};
+  if (first_use_on_device(attr_set)) {
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
+    if (e != cudaSuccess) return set_error_cuda("cudaFuncSetAttribute(gemm pingpong)", e);
+  }
+  const int num_tiles = ((p.M + BM - 1) / BM) * ((p.N + PP_BN - 1) / PP_BN);
+  const int ctas = num_sms() < num_tiles ? num_sms() : num_tiles;
+  cudaError_t le = launch_pdl(kern, dim3(ctas), dim3(GEMM_THREADS), Cfg::SMEM_BYTES, stream, tmA, tmB, p);
+  if (le != cudaSuccess) return set_error_cuda("launch(gemm_bf16_pingpong_kernel)", le);
+  count_launch();
+  return check_launch("gemm_bf16_pingpong_kernel");
+}
+
+static int dispatch_pingpong(bool a_mn, bool b_mn, const void* A, long lda, const void* B, long ldb,
+                             const GemmParams& p, cudaStream_t stream) {
+  if (!a_mn && !b_mn) return launch_gemm_pingpong<false, false>(A, lda, B, ldb, p, stream);
+  if (!a_mn && b_mn) return launch_gemm_pingpong<false, true>(A, lda, B, ldb, p, stream);
+  return launch_gemm_pingpong<true, true>(A, lda, B, ldb, p, stream);
+}
+
 template <bool A_MN, bool B_MN, int CL>
 static int dispatch_bn(int bn, const void* A, long lda, const void* B, long ldb,
                        const GemmParams& p, cudaStream_t stream) {
@@ -293,6 +465,18 @@ static int choose_bn(int M, int N, int cl) {
   return best_bn;
 }
 
+// Ping-pong or cooperative (single-CTA kernels).  The ping-pong kernel hides a tile's epilogue under the next tile's
+// MMAs, so it needs at least two tiles per CTA; with one, a single warpgroup issues all the MMAs and the kernel is
+// slower (wgrad 1408 x 1408 x 13344: 0.095 against 0.090 ms).  Its price is the 128-wide tile, which reads a third
+// more operand bytes from shared memory per flop than a 128 x 256 one: at long K, where the epilogue is a small share
+// of a tile, the cooperative kernel with BN = 256 stays ahead (wgrad 1408 x 6144 x 13344: 0.318 against 0.400 ms).
+// Every other GEMM of the cfg-2 step is 0.5-28 % faster on the ping-pong kernel (DESIGN.md 4.1, tools/gemm_table.py).
+static bool use_pingpong(int M, int N, int K) {
+  const long tiles = (long)((M + BM - 1) / BM) * ((N + PP_BN - 1) / PP_BN);
+  if (tiles <= num_sms()) return false;
+  return !(K >= 8192 && choose_bn(M, N, 1) == 256);
+}
+
 static bool g_default_2cta = false;
 
 }  // namespace ivb
@@ -321,9 +505,16 @@ extern "C" int ivb_gemm_bf16(const void* A, int a_mn_major, long lda, const void
   p.gamma = reinterpret_cast<const __nv_bfloat16*>(gamma);
   p.aux = aux; p.ldaux = ldaux; p.rowscale = rowscale;
   // kernel selection: the CTA-pair (cluster) kernel when forced, or by default for problems tall enough to fill
-  // 256-row tiles; the single-CTA kernel otherwise / when IVB_FLAG_1CTA is set.
+  // 256-row tiles; the ping-pong kernel when forced or chosen by use_pingpong; the cooperative single-CTA kernel
+  // otherwise / when IVB_FLAG_1CTA is set.
   const bool force2 = (flags & IVB_FLAG_2CTA) != 0, force1 = (flags & IVB_FLAG_1CTA) != 0;
-  const int cl = (force2 || (!force1 && g_default_2cta && M >= 512)) ? 2 : 1;
+  const bool forcepp = (flags & IVB_FLAG_PINGPONG) != 0;
+  if ((int)force2 + (int)force1 + (int)forcepp > 1)
+    return set_error("ivb_gemm_bf16: IVB_FLAG_1CTA, IVB_FLAG_2CTA and IVB_FLAG_PINGPONG exclude each other");
+  if (forcepp && tile_n != 0 && tile_n != PP_BN) return set_error("ivb_gemm_bf16: the ping-pong kernel has tile_n 128");
+  const int cl = (force2 || (!force1 && !forcepp && g_default_2cta && M >= 512)) ? 2 : 1;
+  if (forcepp || (cl == 1 && !force1 && (tile_n == 0 || tile_n == PP_BN) && use_pingpong(M, N, K)))
+    return dispatch_pingpong(a_mn_major != 0, b_mn_major != 0, A, lda, B, ldb, p, stream);
   const int bn = tile_n > 0 ? tile_n : choose_bn(M, N, cl);
   if (cl == 2) return dispatch_major<2>(bn, a_mn_major != 0, b_mn_major != 0, A, lda, B, ldb, p, stream);
   return dispatch_major<1>(bn, a_mn_major != 0, b_mn_major != 0, A, lda, B, ldb, p, stream);
