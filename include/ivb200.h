@@ -70,7 +70,11 @@ void ivb_reset_launch_count(void);
  *   b_mn_major = 0: B is stored [N,K] row-major (pitch ldb);  1: stored [K,N] row-major.
  * Supported (A,B) majors: (0,0) forward y = x W^T; (0,1) dgrad dx = dy W; (1,1) wgrad dW = dy^T x.
  * Stands in for nn.Linear / F.linear (cuBLAS) at internvideo2_pretrain.py:61-77,195,211,239-242,
- * 356,394 and FA2 fused_dense (FusedMLP :269).  tile_n: 0 = auto, or one of 128/176/192/256.     */
+ * 356,394 and FA2 fused_dense (FusedMLP :269).  tile_n: 0 = auto, or one of 128/176/192/256.
+ * The fused epilogue moves every row of out0 / out1 / aux and the bias / gamma vectors in 16-byte vectors, so:
+ * N, lda, ldb, ld0 and (when out1 is given) ld1 are multiples of 8 elements; ldaux (when aux is given) is a multiple
+ * of 8 bf16 elements, or of 4 for the fp32 aux of IVB_EPI_RESID; out0, out1, aux, bias and gamma are 16-byte aligned.
+ * A call that breaks one of these rules is refused before any CUDA call.                          */
 /* process-wide default for problems with M >= 512: 1 = CTA-pair kernel, 0 = single-CTA kernel. */
 void ivb_set_default_2cta(int enable);
 int ivb_gemm_bf16(const void* A, int a_mn_major, long lda, const void* B, int b_mn_major, long ldb,

@@ -497,6 +497,16 @@ extern "C" int ivb_gemm_bf16(const void* A, int a_mn_major, long lda, const void
   if (out0 == nullptr) return set_error("ivb_gemm_bf16: out0 is null");
   if ((epilogue == IVB_EPI_RESID || epilogue == IVB_EPI_GELU_BWD) && aux == nullptr)
     return set_error("ivb_gemm_bf16: epilogue needs aux");
+  // the epilogue reads and writes every operand in 16-byte vectors (epilogue_chunk): each row must start on 16 bytes
+  if (out1 != nullptr && (ld1 & 7)) return set_error("ivb_gemm_bf16: ld1 must be a multiple of 8 elements");
+  if (aux != nullptr && (ldaux & (epilogue == IVB_EPI_RESID ? 3 : 7)))
+    return set_error("ivb_gemm_bf16: ldaux must be a multiple of 8 bf16 or 4 fp32 elements");
+  const void* vec_ptrs[5] = {out0, out1, aux, bias, gamma};
+  const char* vec_msgs[5] = {"ivb_gemm_bf16: out0 must be 16-byte aligned", "ivb_gemm_bf16: out1 must be 16-byte aligned",
+                             "ivb_gemm_bf16: aux must be 16-byte aligned", "ivb_gemm_bf16: bias must be 16-byte aligned",
+                             "ivb_gemm_bf16: gamma must be 16-byte aligned"};
+  for (int i = 0; i < 5; ++i)
+    if (reinterpret_cast<uintptr_t>(vec_ptrs[i]) & 15) return set_error(vec_msgs[i]);
   if (a_mn_major && !b_mn_major) return set_error("ivb_gemm_bf16: (A MN-major, B K-major) unused");
   GemmParams p;
   p.M = M; p.N = N; p.K = K; p.epi = epilogue; p.flags = flags;

@@ -323,6 +323,14 @@ __device__ __forceinline__ float warp_max(float v) {
 //   erfc(z) = (a1 t + ... + a5 t^5) e^{-z^2},  t = 1/(1 + p z),  z >= 0,  |error| <= 1.5e-7,
 // one MUFU.RCP + one MUFU.EX2 + 8 FMA; the derivative reuses the same exponential (phi(x) ~ e^{-x^2/2}).
 // These run in the GEMM epilogue: 256 evaluations per thread per tile, so instruction count matters.
+// Domain (pinned by tests/test_gemm_epilogue_gpu.py::test_gelu_every_bf16_value):
+//   - the A-S bound is absolute: in the left tail, where Phi(x) < ~1e-6, gelu_erf(x) = x Phi(x) keeps an absolute error
+//     of at most 7.5e-8 |x| but its RELATIVE error grows (1.6e-3 at x = -5, 2e-2 at x = -10, against half a bf16 ulp of
+//     2e-3); gelu_erf and gelu_erf_grad are finite for every finite x.
+//   - the tanh form goes through tanh.approx.f32 (MUFU.TANH, relative error about 2^-11).  gelu_tanh is finite for every
+//     finite x; gelu_tanh_grad is finite for |x| < 2^64 and NaN beyond, where x * x overflows and 0 * inf is formed.
+//     Live activations are many orders of magnitude below that; a guard would cost an instruction per element.
+//   - NaN in gives NaN out; subnormal inputs and results flush to zero (the library builds with --use_fast_math).
 __device__ __forceinline__ void gelu_cdf_pdf(float x, float& cdf, float& pdf) {
   const float z = fabsf(x) * 0.70710678118654752f;
   const float t = __fdividef(1.0f, fmaf(0.3275911f, z, 1.0f));   // MUFU.RCP (no IEEE fix-up: |err| << bf16 ulp)
