@@ -47,39 +47,80 @@ struct GemmCfg {
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + EPI_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
 };
 
-// ------------------------------------------------------------------ epilogue of one warpgroup's 64 x BN accumulators
-// 32 columns at a time: fragments -> the warp's 16 x 32 staging tile -> one 16-column row segment per thread.
-// row0: first row of the warpgroup's 64-row band.
-template <int BN>
-__device__ __forceinline__ void epilogue_band(const GemmParams& p, const float* acc, float* st, long row0, int n0) {
-  const int lane = threadIdx.x & 31;
-  const int wr = (threadIdx.x >> 5) & 3;   // warp inside the warpgroup: accumulator rows [16*wr, 16*wr + 16)
-  const long row = row0 + wr * 16 + (lane >> 1);
-  const int half = lane & 1;
+// ------------------------------------------------------------------ epilogue of one warpgroup's accumulators
+// acc[h] holds rows [row0 + 64h, row0 + 64h + 64) x BN columns: NH = 1 for a cooperative warpgroup's band, NH = 2 for a
+// ping-pong warpgroup's whole tile.  The epilogue walks it in chunks of 32 columns of one 64-row band, the band index
+// running fastest: fragments -> the warp's 16 x 32 staging tile -> one 16-column row segment per thread.
+//
+// The chunk loop is rolled, so the kernel holds one copy of the epilogue body.  Unrolled, every chunk carried its own
+// copy of all six epilogue forms (17 K instructions per kernel), and the fc1 epilogue ran at the speed of the
+// instruction fetch.  Only the fragment -> staging copy is selected per chunk (epilogue_stage), so acc is indexed with
+// constants and stays in registers.  Each chunk's global inputs are loaded during the previous chunk; bias and gamma
+// are loaded once per 32-column strip, and the NH bands of the strip share them.
+template <int BN, int NH>
+__device__ __forceinline__ void epilogue_stage(const float (&acc)[NH][BN / 2], float* st, int chunk, int lane) {
 #pragma unroll
-  for (int c = 0; c < (BN + 31) / 32; ++c) {
+  for (int k = 0; k < NH * ((BN + 31) / 32); ++k) {
+    if (k != chunk) continue;
+    const int h = k % NH, c = k / NH;
 #pragma unroll
     for (int jj = 0; jj < 4; ++jj) {
       const int j = 4 * c + jj;
       if (j < BN / 8) {
 #pragma unroll
-        for (int h = 0; h < 2; ++h)
-          *reinterpret_cast<float2*>(st + ((lane >> 2) + 8 * h) * EPI_PITCH + 8 * jj + 2 * (lane & 3)) =
-              make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+        for (int q = 0; q < 2; ++q)
+          *reinterpret_cast<float2*>(st + ((lane >> 2) + 8 * q) * EPI_PITCH + 8 * jj + 2 * (lane & 3)) =
+              make_float2(acc[h][4 * j + 2 * q], acc[h][4 * j + 2 * q + 1]);
       }
     }
+  }
+}
+
+template <int BN, int NH>
+__device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float (&acc)[NH][BN / 2], float* st, long row0,
+                                              int n0) {
+  constexpr int CHUNKS = NH * ((BN + 31) / 32);
+  const int lane = threadIdx.x & 31;
+  const int wr = (threadIdx.x >> 5) & 3;   // warp inside the warpgroup: rows [16*wr, 16*wr + 16) of each band
+  const long row_b0 = row0 + wr * 16 + (lane >> 1);
+  const int half = lane & 1;
+  const bool accum = (p.flags & IVB_FLAG_ACCUM) != 0;
+  const bool tanh_mode = (p.flags & IVB_FLAG_GELU_TANH) != 0;
+  const bool save_grad = (p.flags & IVB_FLAG_GELU_SAVE_GRAD) != 0;
+  // this thread's row, first column (in the tile) and columns inside the matrix in chunk i
+  auto row_of = [&](int i) { return row_b0 + 64 * (i % NH); };
+  auto col_of = [&](int i) { return (i / NH) * 32 + half * 16; };
+  auto nvalid_of = [&](int i) {
+    const int col = col_of(i);
+    if (col >= BN || row_of(i) >= p.M) return 0;
+    return min(16, p.N - n0 - col);
+  };
+  EpiIn<16> next;
+  if (nvalid_of(0) > 0) epilogue_load<16>(p, accum, next, row_of(0), n0 + col_of(0), nvalid_of(0));
+  uint32_t bias[8] = {}, gamma[8] = {};
+#pragma unroll 1
+  for (int i = 0; i < CHUNKS; ++i) {
+    const long row = row_of(i);
+    const int col = col_of(i), nvalid = nvalid_of(i);
+    const EpiIn<16> in = next;
+    if (i + 1 < CHUNKS && nvalid_of(i + 1) > 0)
+      epilogue_load<16>(p, accum, next, row_of(i + 1), n0 + col_of(i + 1), nvalid_of(i + 1));
+    if (i % NH == 0 && col < BN && n0 + col < p.N) {
+      const int ncols = min(16, p.N - n0 - col);
+      if (p.bias != nullptr) load_bits_bf16<16>(p.bias + n0 + col, bias, ncols);
+      if (p.gamma != nullptr) load_bits_bf16<16>(p.gamma + n0 + col, gamma, ncols);
+    }
+    epilogue_stage<BN, NH>(acc, st, i, lane);
     __syncwarp();
-    const int col = c * 32 + half * 16;
-    if (col < BN && row < p.M) {
-      uint32_t bits[16];
+    if (nvalid > 0) {
+      float v[16];
       const float* src = st + (lane >> 1) * EPI_PITCH + half * 16;
 #pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const float4 v = reinterpret_cast<const float4*>(src)[i];
-        bits[4 * i] = __float_as_uint(v.x); bits[4 * i + 1] = __float_as_uint(v.y);
-        bits[4 * i + 2] = __float_as_uint(v.z); bits[4 * i + 3] = __float_as_uint(v.w);
+      for (int k = 0; k < 4; ++k) {
+        const float4 f = reinterpret_cast<const float4*>(src)[k];
+        v[4 * k] = f.x; v[4 * k + 1] = f.y; v[4 * k + 2] = f.z; v[4 * k + 3] = f.w;
       }
-      epilogue_chunk<16>(p, bits, row, n0 + col);
+      epilogue_chunk<16>(p, accum, tanh_mode, save_grad, v, in, bias, gamma, row, n0 + col, nvalid);
     }
     __syncwarp();
   }
@@ -181,7 +222,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       if (CL == 2) mbar_arrive_cluster(mapa_u32(smem_u32(&empty[s_]), rank ^ 1));
     };
     float* st = epi + (warp - 4) * 16 * EPI_PITCH;
-    float acc[BN / 2];
+    float acc[1][BN / 2];
     int stage = 0;
     uint32_t phase = 0;
     for (int tile = cid; tile < num_tiles; tile += ncl) {
@@ -198,7 +239,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           const uint64_t ad = A_MN ? gmma_desc(sa + cw * 8192 + k * 2048, 8192, 1024)
                                    : gmma_desc(sa + cw * 8192 + k * 32, 16, 1024);
           const uint64_t bd = B_MN ? gmma_desc(sb + k * 2048, 8192, 1024) : gmma_desc(sb + k * 32, 16, 1024);
-          Wgmma<BN>::template ss<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, ad, bd, (kb > 0 || k > 0) ? 1u : 0u);
+          Wgmma<BN>::template ss<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc[0], ad, bd, (kb > 0 || k > 0) ? 1u : 0u);
         }
         wgmma_commit();
         if (kb > 0) {  // the MMAs of the previous k-block retired: its smem slot is free
@@ -209,9 +250,9 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
       wgmma_wait<0>();
-      wgmma_reg_fence(acc, BN / 2);
+      wgmma_reg_fence(acc[0], BN / 2);
       release(prev);
-      epilogue_band<BN>(p, acc, st, m0 + cw * 64, n0);
+      epilogue_tile<BN, 1>(p, acc, st, m0 + cw * 64, n0);
     }
   }
   if (CL == 2) cluster_sync_all();   // the peer may still multicast into / arrive on this CTA's ring
@@ -340,8 +381,7 @@ gemm_bf16_pingpong_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_
       wgmma_reg_fence(acc[0], PP_BN / 2);
       wgmma_reg_fence(acc[1], PP_BN / 2);
       if (signal) mbar_arrive(&empty[prev]);
-#pragma unroll
-      for (int h = 0; h < 2; ++h) epilogue_band<PP_BN>(p, acc[h], st, m0 + h * 64, n0);
+      epilogue_tile<PP_BN, 2>(p, acc, st, m0, n0);
     }
   }
 }

@@ -51,21 +51,27 @@ __device__ __forceinline__ void store_row_bf16(__nv_bfloat16* ptr, const float* 
     }
   }
 }
+// Raw bits of W bf16 (W / 2 words) starting at `ptr`; words of elements past `nvalid` are zero.
 template <int W>
-__device__ __forceinline__ void load_row_bf16(const __nv_bfloat16* ptr, float* v, int nvalid) {
+__device__ __forceinline__ void load_bits_bf16(const __nv_bfloat16* ptr, uint32_t* r, int nvalid) {
   const bool wide = (reinterpret_cast<uintptr_t>(ptr) & 31) == 0;
 #pragma unroll
   for (int i = 0; i < W; i += 16) {
-    uint32_t r[8] = {0u, 0u, 0u, 0u, 0u, 0u, 0u, 0u};
+    uint32_t* q = r + i / 2;
     if (wide && i + 16 <= nvalid) {
-      ld_global_256(ptr + i, r);
+      ld_global_256(ptr + i, q);
     } else {
-      if (i < nvalid) { const uint4 a = *reinterpret_cast<const uint4*>(ptr + i); r[0] = a.x; r[1] = a.y; r[2] = a.z; r[3] = a.w; }
-      if (i + 8 < nvalid) { const uint4 a = *reinterpret_cast<const uint4*>(ptr + i + 8); r[4] = a.x; r[5] = a.y; r[6] = a.z; r[7] = a.w; }
+      uint4 a = make_uint4(0u, 0u, 0u, 0u), b = a;
+      if (i < nvalid) a = *reinterpret_cast<const uint4*>(ptr + i);
+      if (i + 8 < nvalid) b = *reinterpret_cast<const uint4*>(ptr + i + 8);
+      q[0] = a.x; q[1] = a.y; q[2] = a.z; q[3] = a.w; q[4] = b.x; q[5] = b.y; q[6] = b.z; q[7] = b.w;
     }
-#pragma unroll
-    for (int k = 0; k < 8; ++k) { const float2 f = unpack_bf16(r[k]); v[i + 2 * k] = f.x; v[i + 2 * k + 1] = f.y; }
   }
+}
+template <int W>
+__device__ __forceinline__ void unpack_row_bf16(const uint32_t* r, float* v) {
+#pragma unroll
+  for (int k = 0; k < W / 2; ++k) { const float2 f = unpack_bf16(r[k]); v[2 * k] = f.x; v[2 * k + 1] = f.y; }
 }
 template <int W>
 __device__ __forceinline__ void store_row_f32(float* ptr, const float* v, int nvalid) {
@@ -85,73 +91,93 @@ __device__ __forceinline__ void store_row_f32(float* ptr, const float* v, int nv
     }
   }
 }
+// Raw bits of W fp32 starting at `ptr`; words of elements past `nvalid` are zero.
 template <int W>
-__device__ __forceinline__ void load_row_f32(const float* ptr, float* v, int nvalid) {
+__device__ __forceinline__ void load_bits_f32(const float* ptr, uint32_t* r, int nvalid) {
   const bool wide = (reinterpret_cast<uintptr_t>(ptr) & 31) == 0;
 #pragma unroll
   for (int i = 0; i < W; i += 8) {
     if (i < nvalid) {
       if (wide) {
-        uint32_t r[8];
-        ld_global_256(ptr + i, r);
-#pragma unroll
-        for (int k = 0; k < 8; ++k) v[i + k] = __uint_as_float(r[k]);
+        ld_global_256(ptr + i, r + i);
       } else {
-        const float4 a = *reinterpret_cast<const float4*>(ptr + i), b = *reinterpret_cast<const float4*>(ptr + i + 4);
-        v[i] = a.x; v[i + 1] = a.y; v[i + 2] = a.z; v[i + 3] = a.w;
-        v[i + 4] = b.x; v[i + 5] = b.y; v[i + 6] = b.z; v[i + 7] = b.w;
+        const uint4 a = *reinterpret_cast<const uint4*>(ptr + i), b = *reinterpret_cast<const uint4*>(ptr + i + 4);
+        r[i] = a.x; r[i + 1] = a.y; r[i + 2] = a.z; r[i + 3] = a.w;
+        r[i + 4] = b.x; r[i + 5] = b.y; r[i + 6] = b.z; r[i + 7] = b.w;
       }
     } else {
 #pragma unroll
-      for (int k = 0; k < 8; ++k) v[i + k] = 0.f;
+      for (int k = 0; k < 8; ++k) r[i + k] = 0u;
     }
   }
 }
 
 // ------------------------------------------------------------------ epilogue for W columns of one row
-// acc_bits: W fp32 accumulators of (row, col0 .. col0+W-1).  W is a multiple of 16.
+// What one row segment reads from global memory besides bias and gamma: aux (EPI_RESID: the fp32 residual stream;
+// EPI_GELU_BWD: the bf16 pre-activation or saved GELU'), out0's old values under IVB_FLAG_ACCUM, and the EPI_RESID row
+// scale.  epilogue_tile loads it a chunk ahead, so its HBM latency is not on the epilogue's critical path.
 template <int W>
-__device__ __forceinline__ void epilogue_chunk(const GemmParams& p, const uint32_t* acc_bits, long row, int col0) {
-  int nvalid = p.N - col0;
-  if (nvalid <= 0) return;
-  if (nvalid > W) nvalid = W;
-  float v[W];
-#pragma unroll
-  for (int i = 0; i < W; ++i) v[i] = __uint_as_float(acc_bits[i]);
+struct EpiIn {
+  uint32_t x[W];   // raw bits: W fp32, or W bf16 in the first W / 2 words
+  float rs;
+};
+
+template <int W>
+__device__ __forceinline__ void epilogue_load(const GemmParams& p, bool accum, EpiIn<W>& in, long row, int col0,
+                                              int nvalid) {
+  switch (p.epi) {
+    case IVB_EPI_BF16:
+      if (accum) load_bits_bf16<W>(reinterpret_cast<const __nv_bfloat16*>(p.out0) + row * p.ld0 + col0, in.x, nvalid);
+      break;
+    case IVB_EPI_F32:
+      if (accum) load_bits_f32<W>(reinterpret_cast<const float*>(p.out0) + row * p.ld0 + col0, in.x, nvalid);
+      break;
+    case IVB_EPI_RESID:
+      in.rs = p.rowscale ? p.rowscale[row] : 1.0f;
+      load_bits_f32<W>(reinterpret_cast<const float*>(p.aux) + row * p.ldaux + col0, in.x, nvalid);
+      break;
+    case IVB_EPI_GELU_BWD:
+      load_bits_bf16<W>(reinterpret_cast<const __nv_bfloat16*>(p.aux) + row * p.ldaux + col0, in.x, nvalid);
+      break;
+    default:
+      break;
+  }
+}
+
+// v: the W fp32 accumulators of (row, col0 .. col0+W-1), 0 < nvalid <= W of them inside the matrix.  in: what
+// epilogue_load read for them.  bias_bits / gamma_bits: the W bf16 of bias / gamma at col0 (when the GEMM has them).
+template <int W>
+__device__ __forceinline__ void epilogue_chunk(const GemmParams& p, bool accum, bool tanh_mode, bool save_grad,
+                                               float* v, const EpiIn<W>& in, const uint32_t* bias_bits,
+                                               const uint32_t* gamma_bits, long row, int col0, int nvalid) {
   if (p.bias != nullptr) {
     float bv[W];
-    load_row_bf16<W>(p.bias + col0, bv, nvalid);
+    unpack_row_bf16<W>(bias_bits, bv);
 #pragma unroll
     for (int i = 0; i < W; ++i) v[i] += bv[i];
   }
-  const bool accum = (p.flags & IVB_FLAG_ACCUM) != 0;
-  const bool tanh_mode = (p.flags & IVB_FLAG_GELU_TANH) != 0;
   switch (p.epi) {
     case IVB_EPI_BF16: {
-      __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(p.out0) + row * p.ld0 + col0;
       if (accum) {
         float old[W];
-        load_row_bf16<W>(o, old, nvalid);
+        unpack_row_bf16<W>(in.x, old);
 #pragma unroll
         for (int i = 0; i < W; ++i) v[i] += old[i];
       }
-      store_row_bf16<W>(o, v, nvalid);
+      store_row_bf16<W>(reinterpret_cast<__nv_bfloat16*>(p.out0) + row * p.ld0 + col0, v, nvalid);
     } break;
     case IVB_EPI_F32: {
-      float* o = reinterpret_cast<float*>(p.out0) + row * p.ld0 + col0;
       if (accum) {
-        float old[W];
-        load_row_f32<W>(o, old, nvalid);
 #pragma unroll
-        for (int i = 0; i < W; ++i) v[i] += old[i];
+        for (int i = 0; i < W; ++i) v[i] += __uint_as_float(in.x[i]);
       }
-      store_row_f32<W>(o, v, nvalid);
+      store_row_f32<W>(reinterpret_cast<float*>(p.out0) + row * p.ld0 + col0, v, nvalid);
     } break;
     case IVB_EPI_BIAS_GELU: {
       // NOTE: the erf/tanh choice is hoisted out of the element loops on purpose.  With the branch inside,
       // every element became its own basic block and the MUFU latency chains of the 32 elements could not
       // be interleaved: the epilogue ran at ~8K cycles per 32-column chunk instead of ~1K.
-      if (p.out1 != nullptr && (p.flags & IVB_FLAG_GELU_SAVE_GRAD) != 0) {
+      if (p.out1 != nullptr && save_grad) {
         // save gelu'(h) (shares the exponential with gelu(h)) so the backward epilogue is one multiply
         float dv[W];
         if (tanh_mode) {
@@ -185,25 +211,23 @@ __device__ __forceinline__ void epilogue_chunk(const GemmParams& p, const uint32
       // out0(fp32) = aux(fp32 residual stream) + rowscale * gamma * y
       if (p.out1 != nullptr)
         store_row_bf16<W>(reinterpret_cast<__nv_bfloat16*>(p.out1) + row * p.ld1 + col0, v, nvalid);
-      const float rs = p.rowscale ? p.rowscale[row] : 1.0f;
-      float res[W];
-      load_row_f32<W>(reinterpret_cast<const float*>(p.aux) + row * p.ldaux + col0, res, nvalid);
+      const float rs = in.rs;
       if (p.gamma != nullptr) {
         float gm[W];
-        load_row_bf16<W>(p.gamma + col0, gm, nvalid);
+        unpack_row_bf16<W>(gamma_bits, gm);
 #pragma unroll
-        for (int i = 0; i < W; ++i) v[i] = fmaf(gm[i] * rs, v[i], res[i]);
+        for (int i = 0; i < W; ++i) v[i] = fmaf(gm[i] * rs, v[i], __uint_as_float(in.x[i]));
       } else {
 #pragma unroll
-        for (int i = 0; i < W; ++i) v[i] = fmaf(rs, v[i], res[i]);
+        for (int i = 0; i < W; ++i) v[i] = fmaf(rs, v[i], __uint_as_float(in.x[i]));
       }
       store_row_f32<W>(reinterpret_cast<float*>(p.out0) + row * p.ld0 + col0, v, nvalid);
     } break;
     case IVB_EPI_GELU_BWD: {
       // out0(bf16) = acc * gelu'(aux(bf16 pre-activation))   [or acc * aux with GELU_SAVE_GRAD]
       float hv[W];
-      load_row_bf16<W>(reinterpret_cast<const __nv_bfloat16*>(p.aux) + row * p.ldaux + col0, hv, nvalid);
-      if ((p.flags & IVB_FLAG_GELU_SAVE_GRAD) != 0) {
+      unpack_row_bf16<W>(in.x, hv);
+      if (save_grad) {
 #pragma unroll
         for (int i = 0; i < W; ++i) v[i] *= hv[i];
       } else if (tanh_mode) {

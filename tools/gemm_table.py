@@ -2,14 +2,19 @@
 layouts, epilogues and flags, one row per launch of one block (forward qkv / proj / fc1 / fc2; backward dh, dn2, da,
 dn1 and the four ACCUM wgrads) and of the CLIP (x6) and MAE (x4) decoder heads.
 
-Columns (device time per launch, CUDA events, 20 launches after 3 warm-ups, same operands for every column):
+Columns (device time per launch, CUDA events, 50 launches after 3 warm-ups, same operands for every column):
   coop      the cooperative single-CTA kernel (IVB_FLAG_1CTA) with the real epilogue, its own BN choice
   pingpong  the ping-pong kernel (IVB_FLAG_PINGPONG) with the real epilogue
   default   what ivb_gemm_bf16 picks by itself (what the step runs)
   plain     the cooperative kernel with a plain EPI_BF16 epilogue (no bias, no out1, no aux) at its own BN
   plain128  the same at tile_n = 128
+  pp plain  the ping-pong kernel with a plain EPI_BF16 epilogue: what the ping-pong kernel costs with its epilogue hidden
   cuBLAS    torch.matmul on the same operands (bf16 out)
-coop - plain is a lower bound on the exposed epilogue time; plain128 - plain is the mainloop cost of the 128-wide tile.
+coop - plain is a lower bound on the exposed epilogue time; plain128 - plain is the mainloop cost of the 128-wide tile;
+pingpong - pp plain is the epilogue time the ping-pong kernel leaves exposed.
+A second table runs fwd fc1 on the ping-pong kernel with its epilogue taken apart (bias only; tanh-GELU without and with
+the pre-activation output; with GELU'(h) saved; the erf forms), which separates the cost of the stores, of the MUFU work
+and of the epilogue's code length.
 Per-step totals weight each row by its launches per step (x40 blocks, x6 / x4 heads).  With a library that has no
 ping-pong kernel the pingpong column is left out.
 usage: python tools/gemm_table.py > gemm_table.md"""
@@ -26,7 +31,7 @@ M, Mm, D, HD, DEPTH, CLIP_K, MAE_K = 13344, 13312, 1408, 6144, 40, 6, 4   # Mm =
 GELU_TRAIN = ll.FLAG_GELU_TANH | ll.FLAG_GELU_SAVE_GRAD
 
 
-def timeit(fn, iters=20, warm=3):
+def timeit(fn, iters=50, warm=3):
     for _ in range(warm):
         fn()
     torch.cuda.synchronize()
@@ -107,12 +112,13 @@ def main():
     card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
                           capture_output=True, text=True).stdout.strip()
     pp = has_pingpong()
-    cols = ["coop"] + (["pingpong"] if pp else []) + ["default", "plain", "plain128", "cuBLAS"]
+    cols = ["coop"] + (["pingpong"] if pp else []) + ["default", "plain", "plain128"] + (["pp plain"] if pp else []) \
+        + ["cuBLAS"]
     print(f"# libivb200 GEMMs of the cfg-2 step, one launch each (ms, CUDA events)\n\nGPU: {card} "
           f"(name, power limit, max SM clock)\n")
     print("| GEMM | per step | M x N x K | " + " | ".join(cols) + " | coop-plain | plain128-plain |"
-          + (" pingpong/coop |" if pp else ""))
-    print("|---|---|---|" + "---|" * (len(cols) + 2 + pp))
+          + (" pingpong-pp plain | pingpong/coop |" if pp else ""))
+    print("|---|---|---|" + "---|" * (len(cols) + 2 + 2 * pp))
     tot = dict.fromkeys(cols, 0.0)
     tot_epi = tot_pen = 0.0
     tflop = 0.0
@@ -129,6 +135,7 @@ def main():
             "default": lambda: ll.gemm(a, b, a_t=a_t, b_t=b_t, flags=flags, **kw),
             "plain": lambda: ll.gemm(a, b, a_t=a_t, b_t=b_t, flags=ll.FLAG_1CTA),
             "plain128": lambda: ll.gemm(a, b, a_t=a_t, b_t=b_t, flags=ll.FLAG_1CTA, tile_n=128),
+            "pp plain": lambda: ll.gemm(a, b, a_t=a_t, b_t=b_t, flags=ll.FLAG_PINGPONG),
             "cuBLAS": lambda: torch.matmul(ta, tb, out=cout),
         }
         t = {c: timeit(fns[c]) for c in cols}
@@ -140,7 +147,7 @@ def main():
         row = f"| {name} | {per_step} | {m} x {n} x {k} | " + " | ".join(f"{t[c]:.3f}" for c in cols)
         row += f" | {t['coop'] - t['plain']:+.3f} | {t['plain128'] - t['plain']:+.3f} |"
         if pp:
-            row += f" {t['pingpong'] / t['coop']:.3f} |"
+            row += f" {t['pingpong'] - t['pp plain']:+.3f} | {t['pingpong'] / t['coop']:.3f} |"
         print(row, flush=True)
     print("\nPer step (ms, each row x its launches per step; TFLOP/s = the step's GEMM flops / that time):\n")
     print("| | " + " | ".join(cols) + " |\n|---|" + "---|" * len(cols))
@@ -148,6 +155,34 @@ def main():
     print("| TFLOP/s | " + " | ".join(f"{tflop / tot[c] * 1e3:.0f}" for c in cols) + " |")
     print(f"\nExposed epilogue (coop - plain): {tot_epi:.1f} ms/step; 128-wide tile penalty (plain128 - plain): "
           f"{tot_pen:.1f} ms/step.")
+    if pp:
+        fc1_ablation()
+
+
+def fc1_ablation():
+    """fwd fc1 on the ping-pong kernel, one epilogue ingredient at a time (same operands, ms per launch)."""
+    n2, fc1w, fc1b = rnd(M, D), rnd(HD, D, scale=0.02), rnd(HD, scale=0.1)
+    h = torch.empty(M, HD, device="cuda", dtype=bf)
+    PP, TANH, SAVE, GELU = ll.FLAG_PINGPONG, ll.FLAG_GELU_TANH, ll.FLAG_GELU_SAVE_GRAD, ll.EPI_BIAS_GELU
+    rows = [
+        ("plain EPI_BF16", dict()),
+        ("bias", dict(bias=fc1b)),
+        ("bias + GELU tanh", dict(epi=GELU, flags=TANH, bias=fc1b)),
+        ("bias + GELU tanh, out1 = h", dict(epi=GELU, flags=TANH, bias=fc1b, out1=h)),
+        ("bias + GELU tanh, out1 = GELU'(h) (the step's fc1)", dict(epi=GELU, flags=TANH | SAVE, bias=fc1b, out1=h)),
+        ("bias + GELU erf", dict(epi=GELU, bias=fc1b)),
+        ("bias + GELU erf, out1 = h", dict(epi=GELU, bias=fc1b, out1=h)),
+        ("bias + GELU erf, out1 = GELU'(h)", dict(epi=GELU, flags=SAVE, bias=fc1b, out1=h)),
+    ]
+    print(f"\nfwd fc1 {M} x {HD} x {D} on the ping-pong kernel, epilogue taken apart (ms per launch):\n")
+    print("| epilogue | ms | - plain |\n|---|---|---|")
+    base = None
+    for name, kw in rows:
+        kw = dict(kw)
+        flags = kw.pop("flags", 0) | PP
+        t = timeit(lambda: ll.gemm(n2, fc1w, flags=flags, **kw))
+        base = t if base is None else base
+        print(f"| {name} | {t:.3f} | {t - base:+.3f} |", flush=True)
 
 
 if __name__ == "__main__":
