@@ -24,6 +24,60 @@ __device__ __forceinline__ void colred_put(int out, int nslots, int slot, int D,
   g_colred[(static_cast<long>(out) * nslots + slot) * D + col] = v;
 }
 
+// Inside a CTA, every warp adds the rows it visits, in visiting order, into its own `nacc` accumulator rows of D fp32
+// in shared memory, laid out [warp][nacc][D].  colred_zero returns the calling warp's rows, zeroed.
+__device__ __forceinline__ float* colred_zero(float* smem, int nacc, int D) {
+  float* acc = smem + static_cast<long>(threadIdx.x >> 5) * nacc * D;
+  for (int i = threadIdx.x & 31; i < nacc * D; i += 32) acc[i] = 0.f;
+  __syncwarp();
+  return acc;
+}
+
+// acc[0, N) += a * b (or += a) for N = 4 or 8 columns, as 16-byte read-modify-writes.
+template <int N>
+__device__ __forceinline__ void colred_add(float* acc, const float* a, const float* b) {
+#pragma unroll
+  for (int q = 0; q < N / 4; ++q) {
+    float4* p = reinterpret_cast<float4*>(acc) + q;
+    float4 s = *p;
+    s.x += a[4 * q] * b[4 * q]; s.y += a[4 * q + 1] * b[4 * q + 1];
+    s.z += a[4 * q + 2] * b[4 * q + 2]; s.w += a[4 * q + 3] * b[4 * q + 3];
+    *p = s;
+  }
+}
+template <int N>
+__device__ __forceinline__ void colred_add(float* acc, const float* a) {
+#pragma unroll
+  for (int q = 0; q < N / 4; ++q) {
+    float4* p = reinterpret_cast<float4*>(acc) + q;
+    float4 s = *p;
+    s.x += a[4 * q]; s.y += a[4 * q + 1]; s.z += a[4 * q + 2]; s.w += a[4 * q + 3];
+    *p = s;
+  }
+}
+
+// End of the CTA's rows (after __syncthreads): for every column, slot blockIdx.x of output o < NACC * STEP (when bit o
+// of `want` is set) receives accumulator o / STEP summed over warps o % STEP, o % STEP + STEP, ... < nwarps in
+// increasing order, times scale[col] for the last output when scale is given.  STEP = 2 serves two gradients, one from
+// the even and one from the odd warps.
+template <int NACC, int STEP = 1>
+__device__ __forceinline__ void colred_flush(const float* smem, int nwarps, int D, unsigned want,
+                                             const __nv_bfloat16* scale = nullptr) {
+  constexpr int NOUT = NACC * STEP;
+  for (int i = threadIdx.x; i < D; i += blockDim.x) {
+    float s[NOUT] = {};
+    for (int k = 0; k < nwarps; k += STEP) {
+#pragma unroll
+      for (int o = 0; o < NOUT; ++o) s[o] += smem[(static_cast<long>(k + o % STEP) * NACC + o / STEP) * D + i];
+    }
+#pragma unroll
+    for (int o = 0; o < NOUT; ++o)
+      if (want & (1u << o))
+        colred_put(o, gridDim.x, blockIdx.x, D, i,
+                   scale != nullptr && o == NOUT - 1 ? s[o] * __bfloat162float(scale[i]) : s[o]);
+  }
+}
+
 static __global__ void __launch_bounds__(256) colred_finish_kernel(int nslots, int D, float* o0, float* o1, float* o2) {
   const int col = blockIdx.x * blockDim.x + threadIdx.x;
   const int out = blockIdx.y;

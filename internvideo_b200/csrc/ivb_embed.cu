@@ -8,6 +8,7 @@
 //   * the scatter-add backward of those gathers.
 #include "ivb_internal.h"
 #include "ivb_ptx.cuh"
+#include "ivb_rows.cuh"
 
 namespace ivb {
 
@@ -94,29 +95,15 @@ __global__ void gather_add_kernel(const float* __restrict__ src, long src_bstrid
     t = table + static_cast<long>(ti) * D;
   }
   for (int c = lane * 8; c < D; c += 256) {
-    float v[8];
-#pragma unroll
-    for (int k = 0; k < 8; ++k) v[k] = 0.f;
-    if (s) {
-      float4 a = *reinterpret_cast<const float4*>(s + c), bb = *reinterpret_cast<const float4*>(s + c + 4);
-      v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = bb.x; v[5] = bb.y; v[6] = bb.z; v[7] = bb.w;
-    }
+    float v[8] = {};
+    if (s) load8<true>(s, c, v);
     if (t) {
-      uint4 u = *reinterpret_cast<const uint4*>(t + c);
-      float2 f0 = unpack_bf16(u.x), f1 = unpack_bf16(u.y), f2 = unpack_bf16(u.z), f3 = unpack_bf16(u.w);
-      v[0] += f0.x; v[1] += f0.y; v[2] += f1.x; v[3] += f1.y; v[4] += f2.x; v[5] += f2.y; v[6] += f3.x; v[7] += f3.y;
+      float tv[8];
+      load8<false>(t, c, tv);
+#pragma unroll
+      for (int k = 0; k < 8; ++k) v[k] += tv[k];
     }
-    if (OUT_F32) {
-      float* o = reinterpret_cast<float*>(out) + b * out_bstride + static_cast<long>(j) * D + c;
-      *reinterpret_cast<float4*>(o) = make_float4(v[0], v[1], v[2], v[3]);
-      *reinterpret_cast<float4*>(o + 4) = make_float4(v[4], v[5], v[6], v[7]);
-    } else {
-      __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(out) + b * out_bstride + static_cast<long>(j) * D + c;
-      uint4 w;
-      w.x = pack_bf16(v[0], v[1]); w.y = pack_bf16(v[2], v[3]);
-      w.z = pack_bf16(v[4], v[5]); w.w = pack_bf16(v[6], v[7]);
-      *reinterpret_cast<uint4*>(o) = w;
-    }
+    store8<OUT_F32>(out, b * out_bstride + static_cast<long>(j) * D + c, v);
   }
 }
 
@@ -138,16 +125,7 @@ __global__ void scatter_add_kernel(const void* __restrict__ g, long g_bstride, c
   float* dst = table_grad + static_cast<long>(ti) * D;
   for (int c = lane * 8; c < D; c += 256) {
     float v[8];
-    if (G_F32) {
-      const float* s = reinterpret_cast<const float*>(g) + b * g_bstride + static_cast<long>(j) * D + c;
-      float4 a = *reinterpret_cast<const float4*>(s), bb = *reinterpret_cast<const float4*>(s + 4);
-      v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = bb.x; v[5] = bb.y; v[6] = bb.z; v[7] = bb.w;
-    } else {
-      const __nv_bfloat16* s = reinterpret_cast<const __nv_bfloat16*>(g) + b * g_bstride + static_cast<long>(j) * D + c;
-      uint4 u = *reinterpret_cast<const uint4*>(s);
-      float2 f0 = unpack_bf16(u.x), f1 = unpack_bf16(u.y), f2 = unpack_bf16(u.z), f3 = unpack_bf16(u.w);
-      v[0] = f0.x; v[1] = f0.y; v[2] = f1.x; v[3] = f1.y; v[4] = f2.x; v[5] = f2.y; v[6] = f3.x; v[7] = f3.y;
-    }
+    load8<G_F32>(g, b * g_bstride + static_cast<long>(j) * D + c, v);
     // two 128-bit vector reductions per 8 columns (red.global.add.v4.f32, sm_90+): a quarter of the atomic
     // operations of scalar atomicAdd — the scalar form ran at 0.12 of the HBM rate (18.8 M atomics per call)
     red_add_v4(dst + c, v[0], v[1], v[2], v[3]);

@@ -25,6 +25,26 @@ inline bool first_use_on_device(bool (&flags)[64]) {
   flags[dev] = true;
   return true;
 }
+// Raises Kern's dynamic shared-memory limit to `bytes` on the current device, once per device: the device is marked
+// only after the call succeeds, so a failed attempt is retried (and reported) by the next launch.
+template <auto Kern>
+inline int raise_smem_limit(int bytes, const char* what) {
+  static bool set[64] = {};
+  int dev = 0;
+  cudaGetDevice(&dev);
+  const bool tracked = dev >= 0 && dev < 64;
+  if (tracked && set[dev]) return 0;
+  const cudaError_t e = cudaFuncSetAttribute(Kern, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+  if (e != cudaSuccess) return set_error_cuda(what, e);
+  if (tracked) set[dev] = true;
+  return 0;
+}
+// Grid of a persistent row kernel: one CTA per `rows_per_cta` rows, at most `per_sm` CTAs per SM, at least one.
+inline int persistent_grid(long rows, int rows_per_cta, int per_sm) {
+  const long blocks = (rows + rows_per_cta - 1) / rows_per_cta;
+  const long cap = static_cast<long>(num_sms()) * per_sm;
+  return static_cast<int>(blocks > cap ? cap : (blocks < 1 ? 1 : blocks));
+}
 
 // Programmatic dependent launch (IVB_PDL=0 disables): the kernel may be scheduled while the previous kernel of the stream
 // is still draining; it must execute pdl_wait() (ivb_ptx.cuh) before its first global-memory access.  ~1 100 of the

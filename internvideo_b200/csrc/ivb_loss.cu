@@ -11,29 +11,9 @@
 #include "ivb_colred.cuh"
 #include "ivb_internal.h"
 #include "ivb_ptx.cuh"
+#include "ivb_rows.cuh"
 
 namespace ivb {
-
-__device__ __forceinline__ void ld8_bf16(const __nv_bfloat16* p, float v[8]) {
-  uint4 u = *reinterpret_cast<const uint4*>(p);
-  float2 f0 = unpack_bf16(u.x), f1 = unpack_bf16(u.y), f2 = unpack_bf16(u.z), f3 = unpack_bf16(u.w);
-  v[0] = f0.x; v[1] = f0.y; v[2] = f1.x; v[3] = f1.y; v[4] = f2.x; v[5] = f2.y; v[6] = f3.x; v[7] = f3.y;
-}
-__device__ __forceinline__ void ld8_f32(const float* p, float v[8]) {
-  float4 a = *reinterpret_cast<const float4*>(p), b = *reinterpret_cast<const float4*>(p + 4);
-  v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
-}
-__device__ __forceinline__ void st8_bf16(__nv_bfloat16* p, const float v[8]) {
-  uint4 w;
-  w.x = pack_bf16(v[0], v[1]); w.y = pack_bf16(v[2], v[3]);
-  w.z = pack_bf16(v[4], v[5]); w.w = pack_bf16(v[6], v[7]);
-  *reinterpret_cast<uint4*>(p) = w;
-}
-template <bool F32>
-__device__ __forceinline__ void ld8(const void* p, long off, float v[8]) {
-  if (F32) ld8_f32(reinterpret_cast<const float*>(p) + off, v);
-  else ld8_bf16(reinterpret_cast<const __nv_bfloat16*>(p) + off, v);
-}
 
 // ---------------------------------------------------------------- LayerNorm + L2 normalise
 // out = y / ||y||,  y = LN(z) * w + b.   stats[row] = {mean, rstd, 1/||y||}.
@@ -52,21 +32,21 @@ ln_l2_fwd_kernel(const __nv_bfloat16* __restrict__ z, long ldz, const __nv_bfloa
        row += static_cast<long>(gridDim.x) * wpb) {
     const __nv_bfloat16* zr = z + row * ldz;
     float s = 0.f;
-    for (int c = lane * 8; c < C; c += 256) { float v[8]; ld8_bf16(zr + c, v);
+    for (int c = lane * 8; c < C; c += 256) { float v[8]; load8<false>(zr, c, v);
 #pragma unroll
       for (int k = 0; k < 8; ++k) s += v[k]; }
     const float mean = warp_sum(s) * invC;
     float ss = 0.f;
-    for (int c = lane * 8; c < C; c += 256) { float v[8]; ld8_bf16(zr + c, v);
+    for (int c = lane * 8; c < C; c += 256) { float v[8]; load8<false>(zr, c, v);
 #pragma unroll
       for (int k = 0; k < 8; ++k) { const float d = v[k] - mean; ss += d * d; } }
     const float rstd = rsqrtf(warp_sum(ss) * invC + eps);
     float n2 = 0.f, dot = 0.f;
     for (int c = lane * 8; c < C; c += 256) {
       float v[8], wv[8], bv[8];
-      ld8_bf16(zr + c, v); ld8_bf16(w + c, wv); ld8_bf16(bsh + c, bv);
+      load8<false>(zr, c, v); load8<false>(w, c, wv); load8<false>(bsh, c, bv);
       float t[8];
-      if (tgt) ld8<TGT_F32>(tgt, row * ldt + c, t);
+      if (tgt) load8<TGT_F32>(tgt, row * ldt + c, t);
 #pragma unroll
       for (int k = 0; k < 8; ++k) {
         const float y = (v[k] - mean) * rstd * wv[k] + bv[k];
@@ -80,10 +60,10 @@ ln_l2_fwd_kernel(const __nv_bfloat16* __restrict__ z, long ldz, const __nv_bfloa
     if (out) {
       for (int c = lane * 8; c < C; c += 256) {
         float v[8], wv[8], bv[8], o[8];
-        ld8_bf16(zr + c, v); ld8_bf16(w + c, wv); ld8_bf16(bsh + c, bv);
+        load8<false>(zr, c, v); load8<false>(w, c, wv); load8<false>(bsh, c, bv);
 #pragma unroll
         for (int k = 0; k < 8; ++k) o[k] = ((v[k] - mean) * rstd * wv[k] + bv[k]) * inv_n;
-        st8_bf16(out + row * ldo + c, o);
+        store8<false>(out, row * ldo + c, o);
       }
     }
     if (lane == 0 && stats) { stats[row * 3 + 0] = mean; stats[row * 3 + 1] = rstd; stats[row * 3 + 2] = inv_n; }
@@ -100,9 +80,59 @@ ln_l2_fwd_kernel(const __nv_bfloat16* __restrict__ z, long ldz, const __nv_bfloa
   }
 }
 
+// LN -> L2 backward of 8 columns of a row (v = z, g = upstream gradient, col = first column):
+//   xh = (z - mean) * rstd, out = (xh*w + b) * inv_n, dy = inv_n * (g*gs - out*a) with a = <g*gs, out>,
+//   dz = rstd * (dy*w - s1 - xh*s2) with s1 = mean(dy*w), s2 = mean(dy*w*xh); dweight += dy*xh, dbias += dy.
+// The three sweeps over a row: ln_l2_dot8 sums a, ln_l2_sums8 sums s1 and s2, ln_l2_dz8 writes dz.
+struct LnL2Bwd {
+  const __nv_bfloat16* w;
+  const __nv_bfloat16* b;
+  float mean, rstd, inv_n, gs;
+};
+__device__ __forceinline__ void ln_l2_dot8(const LnL2Bwd& p, const float v[8], const float g[8], int col, float& a) {
+  float wv[8], bv[8];
+  load8<false>(p.w, col, wv); load8<false>(p.b, col, bv);
+#pragma unroll
+  for (int k = 0; k < 8; ++k) a += g[k] * p.gs * ((v[k] - p.mean) * p.rstd * wv[k] + bv[k]) * p.inv_n;
+}
+__device__ __forceinline__ void ln_l2_dy8(const LnL2Bwd& p, const float v[8], const float g[8], const float wv[8],
+                                          const float bv[8], float a, float dy[8], float xh[8]) {
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    xh[k] = (v[k] - p.mean) * p.rstd;
+    const float o = (xh[k] * wv[k] + bv[k]) * p.inv_n;
+    dy[k] = p.inv_n * (g[k] * p.gs - o * a);
+  }
+}
+__device__ __forceinline__ void ln_l2_sums8(const LnL2Bwd& p, const float v[8], const float g[8], int col, float a,
+                                            float& s1, float& s2) {
+  float wv[8], bv[8], dy[8], xh[8];
+  load8<false>(p.w, col, wv); load8<false>(p.b, col, bv);
+  ln_l2_dy8(p, v, g, wv, bv, a, dy, xh);
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    s1 += dy[k] * wv[k];
+    s2 += dy[k] * wv[k] * xh[k];
+  }
+}
+// acc: the warp's colred rows [2][C] offset by col, or null when no parameter gradient is wanted
+__device__ __forceinline__ void ln_l2_dz8(const LnL2Bwd& p, const float v[8], const float g[8], int col, float a,
+                                          float s1, float s2, __nv_bfloat16* dz, long dz_off, float* acc, int C) {
+  float wv[8], bv[8], dy[8], xh[8], o[8];
+  load8<false>(p.w, col, wv); load8<false>(p.b, col, bv);
+  ln_l2_dy8(p, v, g, wv, bv, a, dy, xh);
+#pragma unroll
+  for (int k = 0; k < 8; ++k) o[k] = p.rstd * (dy[k] * wv[k] - s1 - xh[k] * s2);
+  store8<false>(dz, dz_off, o);
+  if (acc != nullptr) {
+    colred_add<8>(acc, dy, xh);
+    colred_add<8>(acc + C, dy);
+  }
+}
+
 // d_out = gscale * dout_tensor  (dout_tensor is the upstream gradient, or the TARGET itself when the
 // loss is (2-2<out,tgt>).mean(): then gscale = -2 * g / rows).  Computes dz (bf16), dw, db (fp32, accumulated in a fixed order).
-// dynamic smem: float acc[2][warps][C]
+// dynamic smem: colred rows [warps][2][C]
 template <bool DO_F32>
 __global__ void __launch_bounds__(256)
 ln_l2_bwd_kernel(const __nv_bfloat16* __restrict__ z, long ldz, const __nv_bfloat16* __restrict__ w,
@@ -117,70 +147,33 @@ ln_l2_bwd_kernel(const __nv_bfloat16* __restrict__ z, long ldz, const __nv_bfloa
   const float invC = 1.f / C;
   const float gs = gscale_host * (gscale_dev ? *gscale_dev : 1.f);
   const bool want = dw != nullptr;
-  float* accw = acc_smem + static_cast<long>(warp) * C;
-  float* accb = acc_smem + static_cast<long>(wpb + warp) * C;
-  if (want) for (int i = lane; i < C; i += 32) { accw[i] = 0.f; accb[i] = 0.f; }
-  __syncwarp();
+  float* acc = want ? colred_zero(acc_smem, 2, C) : nullptr;
   for (long row = static_cast<long>(blockIdx.x) * wpb + warp; row < M; row += static_cast<long>(gridDim.x) * wpb) {
     const __nv_bfloat16* zr = z + row * ldz;
-    const float mean = stats[row * 3], rstd = stats[row * 3 + 1], inv_n = stats[row * 3 + 2];
-    // pass 1: a = <do, out> (out = y*inv_n)
+    const LnL2Bwd p{w, bsh, stats[row * 3], stats[row * 3 + 1], stats[row * 3 + 2], gs};
     float a = 0.f;
     for (int c = lane * 8; c < C; c += 256) {
-      float v[8], wv[8], bv[8], g[8];
-      ld8_bf16(zr + c, v); ld8_bf16(w + c, wv); ld8_bf16(bsh + c, bv); ld8<DO_F32>(dout, row * lddo + c, g);
-#pragma unroll
-      for (int k = 0; k < 8; ++k) a += g[k] * gs * ((v[k] - mean) * rstd * wv[k] + bv[k]) * inv_n;
+      float v[8], g[8];
+      load8<false>(zr, c, v); load8<DO_F32>(dout, row * lddo + c, g);
+      ln_l2_dot8(p, v, g, c, a);
     }
     a = warp_sum(a);
-    // dy = inv_n * (do - out * a);  LN backward: g = dy*w ; dx = rstd*(g - mean(g) - xhat*mean(g*xhat))
     float s1 = 0.f, s2 = 0.f;
     for (int c = lane * 8; c < C; c += 256) {
-      float v[8], wv[8], bv[8], g[8];
-      ld8_bf16(zr + c, v); ld8_bf16(w + c, wv); ld8_bf16(bsh + c, bv); ld8<DO_F32>(dout, row * lddo + c, g);
-#pragma unroll
-      for (int k = 0; k < 8; ++k) {
-        const float xh = (v[k] - mean) * rstd;
-        const float o = (xh * wv[k] + bv[k]) * inv_n;
-        const float dy = inv_n * (g[k] * gs - o * a);
-        s1 += dy * wv[k];
-        s2 += dy * wv[k] * xh;
-      }
+      float v[8], g[8];
+      load8<false>(zr, c, v); load8<DO_F32>(dout, row * lddo + c, g);
+      ln_l2_sums8(p, v, g, c, a, s1, s2);
     }
     s1 = warp_sum(s1) * invC; s2 = warp_sum(s2) * invC;
     for (int c = lane * 8; c < C; c += 256) {
-      float v[8], wv[8], bv[8], g[8], o8[8];
-      ld8_bf16(zr + c, v); ld8_bf16(w + c, wv); ld8_bf16(bsh + c, bv); ld8<DO_F32>(dout, row * lddo + c, g);
-      float dyv[8], xhv[8];
-#pragma unroll
-      for (int k = 0; k < 8; ++k) {
-        const float xh = (v[k] - mean) * rstd;
-        const float o = (xh * wv[k] + bv[k]) * inv_n;
-        const float dy = inv_n * (g[k] * gs - o * a);
-        dyv[k] = dy; xhv[k] = xh;
-        o8[k] = rstd * (dy * wv[k] - s1 - xh * s2);
-      }
-      st8_bf16(dz + row * lddz + c, o8);
-      if (want) {
-        float4* aw = reinterpret_cast<float4*>(accw + c);
-        float4* ab = reinterpret_cast<float4*>(accb + c);
-        float4 w0 = aw[0], w1 = aw[1], b0 = ab[0], b1 = ab[1];
-        w0.x += dyv[0] * xhv[0]; w0.y += dyv[1] * xhv[1]; w0.z += dyv[2] * xhv[2]; w0.w += dyv[3] * xhv[3];
-        w1.x += dyv[4] * xhv[4]; w1.y += dyv[5] * xhv[5]; w1.z += dyv[6] * xhv[6]; w1.w += dyv[7] * xhv[7];
-        b0.x += dyv[0]; b0.y += dyv[1]; b0.z += dyv[2]; b0.w += dyv[3];
-        b1.x += dyv[4]; b1.y += dyv[5]; b1.z += dyv[6]; b1.w += dyv[7];
-        aw[0] = w0; aw[1] = w1; ab[0] = b0; ab[1] = b1;
-      }
+      float v[8], g[8];
+      load8<false>(zr, c, v); load8<DO_F32>(dout, row * lddo + c, g);
+      ln_l2_dz8(p, v, g, c, a, s1, s2, dz, row * lddz + c, want ? acc + c : nullptr, C);
     }
   }
   if (want) {
     __syncthreads();
-    for (int i = threadIdx.x; i < C; i += blockDim.x) {
-      float sw = 0.f, sb = 0.f;
-      for (int k = 0; k < wpb; ++k) { sw += acc_smem[static_cast<long>(k) * C + i]; sb += acc_smem[static_cast<long>(wpb + k) * C + i]; }
-      colred_put(0, gridDim.x, blockIdx.x, C, i, sw);
-      if (db) colred_put(1, gridDim.x, blockIdx.x, C, i, sb);
-    }
+    colred_flush<2>(acc_smem, wpb, C, db ? 3u : 1u);
   }
 }
 
@@ -352,15 +345,15 @@ __global__ void l2norm_rows_kernel(const void* __restrict__ x, long ldx, int M, 
   const int lane = threadIdx.x & 31;
   if (row >= M) return;
   float ss = 0.f;
-  for (int c = lane * 8; c < C; c += 256) { float v[8]; ld8<XF32>(x, row * ldx + c, v);
+  for (int c = lane * 8; c < C; c += 256) { float v[8]; load8<XF32>(x, row * ldx + c, v);
 #pragma unroll
     for (int k = 0; k < 8; ++k) ss += v[k] * v[k]; }
   ss = warp_sum(ss);
   const float inv = 1.f / fmaxf(sqrtf(ss), 1e-12f);
-  for (int c = lane * 8; c < C; c += 256) { float v[8], o[8]; ld8<XF32>(x, row * ldx + c, v);
+  for (int c = lane * 8; c < C; c += 256) { float v[8], o[8]; load8<XF32>(x, row * ldx + c, v);
 #pragma unroll
     for (int k = 0; k < 8; ++k) o[k] = v[k] * inv;
-    st8_bf16(out + row * ldo + c, o); }
+    store8<false>(out, row * ldo + c, o); }
   if (lane == 0 && inv_norm) inv_norm[row] = inv;
 }
 // backward of F.normalize: dx = inv * (dy - xn * <dy, xn>)   (dy fp32, xn bf16) -> dx fp32
@@ -371,15 +364,15 @@ __global__ void l2norm_rows_bwd_kernel(const float* __restrict__ dy, long lddy, 
   const int lane = threadIdx.x & 31;
   if (row >= M) return;
   float dot = 0.f;
-  for (int c = lane * 8; c < C; c += 256) { float g[8], v[8]; ld8_f32(dy + row * lddy + c, g); ld8_bf16(xn + row * ldxn + c, v);
+  for (int c = lane * 8; c < C; c += 256) { float g[8], v[8]; load8<true>(dy, row * lddy + c, g); load8<false>(xn, row * ldxn + c, v);
 #pragma unroll
     for (int k = 0; k < 8; ++k) dot += g[k] * v[k]; }
   dot = warp_sum(dot);
   const float inv = inv_norm[row];
-  for (int c = lane * 8; c < C; c += 256) { float g[8], v[8]; ld8_f32(dy + row * lddy + c, g); ld8_bf16(xn + row * ldxn + c, v);
-    float* o = dx + row * lddx + c;
-    *reinterpret_cast<float4*>(o) = make_float4(inv * (g[0] - v[0] * dot), inv * (g[1] - v[1] * dot), inv * (g[2] - v[2] * dot), inv * (g[3] - v[3] * dot));
-    *reinterpret_cast<float4*>(o + 4) = make_float4(inv * (g[4] - v[4] * dot), inv * (g[5] - v[5] * dot), inv * (g[6] - v[6] * dot), inv * (g[7] - v[7] * dot)); }
+  for (int c = lane * 8; c < C; c += 256) { float g[8], v[8], o[8]; load8<true>(dy, row * lddy + c, g); load8<false>(xn, row * ldxn + c, v);
+#pragma unroll
+    for (int k = 0; k < 8; ++k) o[k] = inv * (g[k] - v[k] * dot);
+    store8<true>(dx, row * lddx + c, o); }
 }
 
 // ---------------------------------------------------------------- IV1 pixel targets + MSE
@@ -424,15 +417,10 @@ __global__ void pixel_target_kernel(const __nv_bfloat16* __restrict__ video, con
   }
 }
 
-__device__ __forceinline__ void unpack8q(const uint4& u, float v[8]) {
-  float2 f0 = unpack_bf16(u.x), f1 = unpack_bf16(u.y), f2 = unpack_bf16(u.z), f3 = unpack_bf16(u.w);
-  v[0] = f0.x; v[1] = f0.y; v[2] = f1.x; v[3] = f1.y; v[4] = f2.x; v[5] = f2.y; v[6] = f3.x; v[7] = f3.y;
-}
-
 // Register-resident backward (C <= 256*NCH, bf16 upstream gradient / target): z and dout rows read once, all loads
 // in flight together, the three sweeps run over registers (210 us vs 247 us for the streaming kernel at C = 3200;
 // the same treatment of the FORWARD was slower — see ivb_ln_l2_fwd — and is not kept).
-// dynamic smem: float acc[2][warps][C]
+// dynamic smem: colred rows [warps][2][C]
 template <int NCH>
 __global__ void __launch_bounds__(128, 2)
 ln_l2_bwd_reg_kernel(const __nv_bfloat16* __restrict__ z, long ldz, const __nv_bfloat16* __restrict__ w,
@@ -448,10 +436,7 @@ ln_l2_bwd_reg_kernel(const __nv_bfloat16* __restrict__ z, long ldz, const __nv_b
   const float invC = 1.f / C;
   const float gs = gscale_host * (gscale_dev ? *gscale_dev : 1.f);
   const bool want = dw != nullptr;
-  float* accw = acc_smem + static_cast<long>(warp) * C;
-  float* accb = acc_smem + static_cast<long>(wpb + warp) * C;
-  if (want) for (int i = lane; i < C; i += 32) { accw[i] = 0.f; accb[i] = 0.f; }
-  __syncwarp();
+  float* acc = want ? colred_zero(acc_smem, 2, C) : nullptr;
   for (long row = static_cast<long>(blockIdx.x) * wpb + warp; row < M; row += static_cast<long>(gridDim.x) * wpb) {
     uint4 zq[NCH], gq[NCH];
 #pragma unroll
@@ -462,16 +447,15 @@ ln_l2_bwd_reg_kernel(const __nv_bfloat16* __restrict__ z, long ldz, const __nv_b
         gq[i] = *reinterpret_cast<const uint4*>(dout + row * lddo + c * 8);
       }
     }
-    const float mean = stats[row * 3], rstd = stats[row * 3 + 1], inv_n = stats[row * 3 + 2];
-    float a = 0.f;     // <do, out>, out = y * inv_n
+    const LnL2Bwd p{w, bsh, stats[row * 3], stats[row * 3 + 1], stats[row * 3 + 2], gs};
+    float a = 0.f;
 #pragma unroll
     for (int i = 0; i < NCH; ++i) {
       const int c = lane + 32 * i;
       if (c < nch) {
-        float v[8], wv[8], bv[8], g[8];
-        unpack8q(zq[i], v); unpack8q(gq[i], g); ld8_bf16(w + c * 8, wv); ld8_bf16(bsh + c * 8, bv);
-#pragma unroll
-        for (int k = 0; k < 8; ++k) a += g[k] * gs * ((v[k] - mean) * rstd * wv[k] + bv[k]) * inv_n;
+        float v[8], g[8];
+        unpack8(zq[i], v); unpack8(gq[i], g);
+        ln_l2_dot8(p, v, g, c * 8, a);
       }
     }
     a = warp_sum(a);
@@ -480,16 +464,9 @@ ln_l2_bwd_reg_kernel(const __nv_bfloat16* __restrict__ z, long ldz, const __nv_b
     for (int i = 0; i < NCH; ++i) {
       const int c = lane + 32 * i;
       if (c < nch) {
-        float v[8], wv[8], bv[8], g[8];
-        unpack8q(zq[i], v); unpack8q(gq[i], g); ld8_bf16(w + c * 8, wv); ld8_bf16(bsh + c * 8, bv);
-#pragma unroll
-        for (int k = 0; k < 8; ++k) {
-          const float xh = (v[k] - mean) * rstd;
-          const float o = (xh * wv[k] + bv[k]) * inv_n;
-          const float dy = inv_n * (g[k] * gs - o * a);
-          s1 += dy * wv[k];
-          s2 += dy * wv[k] * xh;
-        }
+        float v[8], g[8];
+        unpack8(zq[i], v); unpack8(gq[i], g);
+        ln_l2_sums8(p, v, g, c * 8, a, s1, s2);
       }
     }
     s1 = warp_sum(s1) * invC; s2 = warp_sum(s2) * invC;
@@ -497,38 +474,15 @@ ln_l2_bwd_reg_kernel(const __nv_bfloat16* __restrict__ z, long ldz, const __nv_b
     for (int i = 0; i < NCH; ++i) {
       const int c = lane + 32 * i;
       if (c < nch) {
-        float v[8], wv[8], bv[8], g[8], o8[8], dyv[8], xhv[8];
-        unpack8q(zq[i], v); unpack8q(gq[i], g); ld8_bf16(w + c * 8, wv); ld8_bf16(bsh + c * 8, bv);
-#pragma unroll
-        for (int k = 0; k < 8; ++k) {
-          const float xh = (v[k] - mean) * rstd;
-          const float o = (xh * wv[k] + bv[k]) * inv_n;
-          const float dy = inv_n * (g[k] * gs - o * a);
-          dyv[k] = dy; xhv[k] = xh;
-          o8[k] = rstd * (dy * wv[k] - s1 - xh * s2);
-        }
-        st8_bf16(dz + row * lddz + c * 8, o8);
-        if (want) {
-          float4* aw = reinterpret_cast<float4*>(accw + c * 8);
-          float4* ab = reinterpret_cast<float4*>(accb + c * 8);
-          float4 w0 = aw[0], w1 = aw[1], b0 = ab[0], b1 = ab[1];
-          w0.x += dyv[0] * xhv[0]; w0.y += dyv[1] * xhv[1]; w0.z += dyv[2] * xhv[2]; w0.w += dyv[3] * xhv[3];
-          w1.x += dyv[4] * xhv[4]; w1.y += dyv[5] * xhv[5]; w1.z += dyv[6] * xhv[6]; w1.w += dyv[7] * xhv[7];
-          b0.x += dyv[0]; b0.y += dyv[1]; b0.z += dyv[2]; b0.w += dyv[3];
-          b1.x += dyv[4]; b1.y += dyv[5]; b1.z += dyv[6]; b1.w += dyv[7];
-          aw[0] = w0; aw[1] = w1; ab[0] = b0; ab[1] = b1;
-        }
+        float v[8], g[8];
+        unpack8(zq[i], v); unpack8(gq[i], g);
+        ln_l2_dz8(p, v, g, c * 8, a, s1, s2, dz, row * lddz + c * 8, want ? acc + c * 8 : nullptr, C);
       }
     }
   }
   if (want) {
     __syncthreads();
-    for (int i = threadIdx.x; i < C; i += blockDim.x) {
-      float sw = 0.f, sb = 0.f;
-      for (int k = 0; k < wpb; ++k) { sw += acc_smem[static_cast<long>(k) * C + i]; sb += acc_smem[static_cast<long>(wpb + k) * C + i]; }
-      colred_put(0, gridDim.x, blockIdx.x, C, i, sw);
-      if (db) colred_put(1, gridDim.x, blockIdx.x, C, i, sb);
-    }
+    colred_flush<2>(acc_smem, wpb, C, db ? 3u : 1u);
   }
 }
 
@@ -561,15 +515,13 @@ extern "C" int ivb_ln_l2_fwd(const void* z, long ldz, const void* weight, const 
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (M <= 0) return 0;
   if ((C & 7) || (ldz & 7)) return set_error("ivb_ln_l2_fwd: C/ld must be multiples of 8");
-  long blocks = (M + 7) / 8;
-  const long cap = static_cast<long>(num_sms()) * 8;
-  if (blocks > cap) blocks = cap;
+  const int blocks = persistent_grid(M, 8, 8);
   auto zz = reinterpret_cast<const __nv_bfloat16*>(z);
   auto ww = reinterpret_cast<const __nv_bfloat16*>(weight);
   auto bb = reinterpret_cast<const __nv_bfloat16*>(bias);
   auto oo = reinterpret_cast<__nv_bfloat16*>(out);
-  if (target_is_f32) ln_l2_fwd_kernel<true><<<(int)blocks, 256, 0, stream>>>(zz, ldz, ww, bb, eps, M, C, oo, ldo, stats, target, ldt, loss_sum);
-  else ln_l2_fwd_kernel<false><<<(int)blocks, 256, 0, stream>>>(zz, ldz, ww, bb, eps, M, C, oo, ldo, stats, target, ldt, loss_sum);
+  if (target_is_f32) ln_l2_fwd_kernel<true><<<blocks, 256, 0, stream>>>(zz, ldz, ww, bb, eps, M, C, oo, ldo, stats, target, ldt, loss_sum);
+  else ln_l2_fwd_kernel<false><<<blocks, 256, 0, stream>>>(zz, ldz, ww, bb, eps, M, C, oo, ldo, stats, target, ldt, loss_sum);
   count_launch();
   return check_launch("ln_l2_fwd_kernel");
 }
@@ -582,25 +534,17 @@ static int launch_ln_l2_bwd(const void* z, long ldz, const void* weight, const v
   int wpb = 8;
   size_t smem = dw ? static_cast<size_t>(2) * wpb * C * sizeof(float) : 0;
   while (smem > 200 * 1024 && wpb > 1) { wpb /= 2; smem /= 2; }
-  if (smem > 48 * 1024) {
-    static bool set[64] = {};
-    if (first_use_on_device(set)) {
-      cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
-      if (e != cudaSuccess) return set_error_cuda("cudaFuncSetAttribute(ln_l2_bwd)", e);
-    }
-  }
-  long blocks = (M + wpb * 2 - 1) / (wpb * 2);
-  const long cap = static_cast<long>(num_sms()) * (smem > 96 * 1024 ? 2 : 4);
-  if (blocks > cap) blocks = cap;
-  if (blocks < 1) blocks = 1;
+  if (smem > 48 * 1024)
+    if (int rc = raise_smem_limit<ln_l2_bwd_kernel<DO_F32>>(220 * 1024, "cudaFuncSetAttribute(ln_l2_bwd)")) return rc;
+  const int blocks = persistent_grid(M, wpb * 2, smem > 96 * 1024 ? 2 : 4);
   if (colred_check(2, blocks, C, "ln_l2_bwd: gradient scratch too small")) return 1;
-  kern<<<(int)blocks, wpb * 32, smem, stream>>>(
+  kern<<<blocks, wpb * 32, smem, stream>>>(
       reinterpret_cast<const __nv_bfloat16*>(z), ldz, reinterpret_cast<const __nv_bfloat16*>(weight),
       reinterpret_cast<const __nv_bfloat16*>(bias), stats, M, C, dout, lddo, gh, gd,
       reinterpret_cast<__nv_bfloat16*>(dz), lddz, dw, db);
   count_launch();
   if (int rc = check_launch("ln_l2_bwd_kernel")) return rc;
-  return dw ? colred_finish(2, (int)blocks, C, dw, db, nullptr, stream) : 0;
+  return dw ? colred_finish(2, blocks, C, dw, db, nullptr, stream) : 0;
 }
 
 template <int NCH>
@@ -610,25 +554,17 @@ static int launch_ln_l2_bwd_reg(const void* z, long ldz, const void* weight, con
   auto kern = ln_l2_bwd_reg_kernel<NCH>;
   const int wpb = 4;
   const size_t smem = dw ? static_cast<size_t>(2) * wpb * C * sizeof(float) : 0;   // <= 104 KB at C = 3200: 2 CTAs/SM
-  if (smem > 48 * 1024) {
-    static bool set[64] = {};
-    if (first_use_on_device(set)) {
-      cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 110 * 1024);
-      if (e != cudaSuccess) return set_error_cuda("cudaFuncSetAttribute(ln_l2_bwd_reg)", e);
-    }
-  }
-  long blocks = (M + wpb * 2 - 1) / (wpb * 2);
-  const long cap = static_cast<long>(num_sms()) * 2;
-  if (blocks > cap) blocks = cap;
-  if (blocks < 1) blocks = 1;
+  if (smem > 48 * 1024)
+    if (int rc = raise_smem_limit<ln_l2_bwd_reg_kernel<NCH>>(110 * 1024, "cudaFuncSetAttribute(ln_l2_bwd_reg)")) return rc;
+  const int blocks = persistent_grid(M, wpb * 2, 2);
   if (colred_check(2, blocks, C, "ln_l2_bwd: gradient scratch too small")) return 1;
-  kern<<<(int)blocks, wpb * 32, smem, stream>>>(
+  kern<<<blocks, wpb * 32, smem, stream>>>(
       reinterpret_cast<const __nv_bfloat16*>(z), ldz, reinterpret_cast<const __nv_bfloat16*>(weight),
       reinterpret_cast<const __nv_bfloat16*>(bias), stats, M, C, reinterpret_cast<const __nv_bfloat16*>(dout), lddo,
       gh, gd, reinterpret_cast<__nv_bfloat16*>(dz), lddz, dw, db);
   count_launch();
   if (int rc = check_launch("ln_l2_bwd_reg_kernel")) return rc;
-  return dw ? colred_finish(2, (int)blocks, C, dw, db, nullptr, stream) : 0;
+  return dw ? colred_finish(2, blocks, C, dw, db, nullptr, stream) : 0;
 }
 
 extern "C" int ivb_ln_l2_bwd(const void* z, long ldz, const void* weight, const void* bias,
@@ -729,10 +665,7 @@ extern "C" int ivb_mse_loss(const void* pred_bf16, const float* label, long n, f
                             float gscale_host, const float* gscale_dev, void* dpred_bf16, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (n <= 0) return 0;
-  long blocks = (n + 255) / 256;
-  const long cap = static_cast<long>(num_sms()) * 8;
-  if (blocks > cap) blocks = cap;
-  mse_kernel<<<(unsigned)blocks, 256, 0, stream>>>(reinterpret_cast<const __nv_bfloat16*>(pred_bf16), label, n, loss_sum, gscale_host, gscale_dev, reinterpret_cast<__nv_bfloat16*>(dpred_bf16));
+  mse_kernel<<<persistent_grid(n, 256, 8), 256, 0, stream>>>(reinterpret_cast<const __nv_bfloat16*>(pred_bf16), label, n, loss_sum, gscale_host, gscale_dev, reinterpret_cast<__nv_bfloat16*>(dpred_bf16));
   count_launch();
   return check_launch("mse_kernel");
 }
@@ -769,7 +702,7 @@ pool_attn_fwd_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* _
     float s = 0.f;
     for (int c = 0; c < d; c += 8) {
       float kv[8];
-      ld8_bf16(kr + c, kv);
+      load8<false>(kr, c, kv);
 #pragma unroll
       for (int t = 0; t < 8; ++t) s += kv[t] * sq[c + t];
     }
@@ -820,7 +753,7 @@ pool_attn_bwd_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* _
     float dp = 0.f;
     for (int c = 0; c < d; c += 8) {
       float vv[8];
-      ld8_bf16(vr + c, vv);
+      load8<false>(vr, c, vv);
 #pragma unroll
       for (int t = 0; t < 8; ++t) dp += vv[t] * sdo[c + t];
     }
@@ -839,8 +772,8 @@ pool_attn_bwd_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* _
       float a[8], bb[8];
 #pragma unroll
       for (int t = 0; t < 8; ++t) { a[t] = ds * sq[c + t]; bb[t] = pj * sdo[c + t]; }
-      st8_bf16(dkr + c, a);
-      st8_bf16(dvr + c, bb);
+      store8<false>(dkr, c, a);
+      store8<false>(dvr, c, bb);
     }
   }
   __syncthreads();
