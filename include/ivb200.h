@@ -82,6 +82,38 @@ int ivb_gemm_bf16(const void* A, int a_mn_major, long lda, const void* B, int b_
                   long ld1, const void* bias, const void* gamma, const void* aux, long ldaux,
                   const float* rowscale, int tile_n, void* stream);
 
+/* ---- FP8 (opt-in FP8 mode of the ViT block) ---------------------------------------------------
+ * Formats: IVB_FP8_E4M3 (4 exponent, 3 mantissa bits, max 448: activations and weights) and IVB_FP8_E5M2 (max 57 344:
+ * gradients).  Per-tensor current scaling: the scale comes from the tensor's own amax in the same call.
+ *
+ * ivb_fp8_quantize: x bf16 [M, K] (pitch ldx, a multiple of 8) ->
+ *   *amax      = max |x| (fp32, device; exact: the max of the bf16 magnitudes, the same bits on every run)
+ *   scale      = 2^floor(log2(fmax / amax)), fmax = 448 or 57 344; 1 when amax = 0 (exponent clamped to [-126, 126])
+ *   out        = round-to-nearest-even(x * scale) in `format`, [M, K] row-major, pitch ldo (a multiple of 16)
+ *   out_t      = out^T, [K, M] row-major, pitch ldt (a multiple of 16), optional (NULL: not written)
+ *   *scale_inv = 1 / scale (fp32, device), or NaN when amax is Inf or NaN, so that a GEMM reading it gives NaN
+ * amax and scale_inv are device floats; amax is also the kernels' workspace (the call zeroes it first).  Columns
+ * K .. ldo of out (and M .. ldt of out_t) are not written.  x, out, out_t are 16-byte aligned.  Three stream-ordered
+ * operations (a 4-byte memset and two kernels); capturable in a CUDA graph.                          */
+#define IVB_FP8_E4M3 0
+#define IVB_FP8_E5M2 1
+int ivb_fp8_quantize(const void* x, long ldx, int M, int K, int format, void* out, long ldo, void* out_t, long ldt,
+                     float* amax, float* scale_inv, void* stream);
+/* D[M,N] = epilogue( a_scale_inv * b_scale_inv * sum_k A(m,k) * B(n,k) ), fp8 operands, fp32 accumulate.
+ * A: [M,K] row-major in a_format (E4M3 or E5M2); B: [N,K] row-major, E4M3.  Both operands K-major (a_mn_major =
+ * b_mn_major = 0; fp8 wgmma has no transposed form): y = x W^T takes W's E4M3 copy, dx = dy W takes the E4M3 copy of W^T
+ * (ivb_fp8_quantize's out_t).  lda, ldb: multiples of 16 elements.  a_scale_inv / b_scale_inv: device fp32 scalars
+ * (ivb_fp8_quantize's), read by the kernel, never by the host.  Epilogue, flags and their operand rules as for
+ * ivb_gemm_bf16, except: no IVB_FLAG_2CTA; tile_n is 0 (auto), 128 or 192.  IVB_FLAG_PINGPONG forces the ping-pong
+ * kernel, which accumulates in the tensor core; IVB_FLAG_1CTA forces the cooperative kernel, which adds each 128-element
+ * k-block's partial sum to an fp32 accumulator on the CUDA cores.  By default the library picks between them as
+ * ivb_gemm_bf16 picks between its ping-pong and cooperative kernels.  A call that breaks one of these rules is refused
+ * before any CUDA call.                                                                            */
+int ivb_gemm_fp8(const void* A, int a_mn_major, long lda, int a_format, const float* a_scale_inv, const void* B,
+                 int b_mn_major, long ldb, const float* b_scale_inv, int M, int N, int K, int epilogue, int flags,
+                 void* out0, long ld0, void* out1, long ld1, const void* bias, const void* gamma, const void* aux,
+                 long ldaux, const float* rowscale, int tile_n, void* stream);
+
 /* ---- RMSNorm / LayerNorm (row reductions, HBM-bound) -------------------------------------------
  * y(bf16) = norm(x) * weight (+ bias).  is_layernorm=0: RMSNorm (internvideo2_pretrain.py:117-128,
  * FA2 DropoutAddRMSNorm :467; eps 1e-6); 1: nn.LayerNorm (eps 1e-5, :525,:532).

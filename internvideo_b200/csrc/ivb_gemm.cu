@@ -18,6 +18,15 @@
 //                   (accumulator fragments -> per-warp smem staging tile -> row segments -> global)
 // The ring keeps streaming the next tile's operands while the MMA warpgroups run the epilogue.
 //
+// FP8 (ivb_gemm_fp8): the same kernels with the operand format as a template parameter (Op).  A 128-byte swizzle row
+// holds 64 bf16 or 128 fp8 elements, so a stage has the same byte layout, a k-block is still four wgmmas (k16 bf16 or
+// k32 fp8) 32 B apart, and only the instruction and the k-block's element count change.  FP8 operands are K-major
+// (fp8 wgmma has no transpose bits).  The epilogue first multiplies the accumulator by a_scale_inv * b_scale_inv (two
+// device scalars read once per CTA, so a captured graph stays valid), then runs the bf16 epilogues unchanged.
+// Accumulation: the tensor core's fp8 MMA keeps fewer mantissa bits in its running sum than fp32 (about 14, DeepSeek-V3
+// technical report 3.3.2).  The ping-pong kernel accumulates in the tensor core; the FP8 cooperative kernel promotes:
+// each 128-element k-block goes into a fresh register tile, which the CUDA cores add to the fp32 accumulator.
+//
 // Ping-pong form (gemm_bf16_pingpong_kernel, the default for most shapes, see use_pingpong): same producer, ring and
 // epilogue, but each MMA warpgroup owns a whole 128 x 128 tile and the two alternate, so one runs its epilogue while
 // the other issues its MMAs.
@@ -26,16 +35,37 @@
 // a 256 x BN tile.  Each CTA loads its own 128 A rows and HALF of the B tile, which TMA multicasts into both CTAs'
 // rings, so B is read from L2 once per 256 rows instead of once per 128.  A stage is refilled only when the MMA
 // warpgroups of BOTH CTAs released it (each arrives on its own and on the peer's empty barrier).
+#include <cstdio>
+
 #include "ivb_gemm_common.cuh"
 
 namespace ivb {
 
 constexpr int BM = 128;
-constexpr int BK = 64;                 // 64 bf16 = 128 B = one swizzle atom
+constexpr int K_MMAS = 4;              // wgmmas per k-block, 32 B apart along the 128-byte swizzle row
 constexpr int GEMM_THREADS = 384;
-constexpr int A_STAGE_BYTES = BM * BK * 2;  // 16 KB either major
+constexpr int A_STAGE_BYTES = BM * 128;     // 16 KB: 128 rows of one 128-byte k-block, either major
 constexpr int EPI_PITCH = 36;               // floats per staged row: 32 columns + 4 (bank spread, 16-B rows)
 constexpr int EPI_BYTES = 8 * 16 * EPI_PITCH * 4;  // one 16 x 32 fp32 staging tile per MMA warp
+
+// Operand formats: bf16 x bf16, or fp8 (A E4M3 or E5M2, B E4M3).  BK: elements in a 128-byte k-block.
+struct OpBf16 {
+  static constexpr bool FP8 = false;
+  static constexpr int BK = 64;
+};
+template <bool A_E5M2_>
+struct OpFp8 {
+  static constexpr bool FP8 = true, A_E5M2 = A_E5M2_;
+  static constexpr int BK = 128;
+};
+
+template <class Op, int N, bool A_MN, bool B_MN>
+__device__ __forceinline__ void mma(float* d, uint64_t da, uint64_t db, uint32_t scale_d) {
+  if constexpr (Op::FP8)
+    WgmmaF8<N>::template ss<Op::A_E5M2>(d, da, db, scale_d);
+  else
+    Wgmma<N>::template ss<A_MN ? 1 : 0, B_MN ? 1 : 0>(d, da, db, scale_d);
+}
 
 template <int BN, bool B_MN>
 struct GemmCfg {
@@ -126,8 +156,22 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float (
   }
 }
 
+// fp8: dequantise the accumulators in place before the epilogue.  (Scaling them as the epilogue stages them lets the
+// compiler hoist every product out of the rolled chunk loop, which needs a second copy of acc and spills.)
+template <class Op, int BN, int NH>
+__device__ __forceinline__ void dequantise(float (&acc)[NH][BN / 2], float dq) {
+  if constexpr (Op::FP8) {
+#pragma unroll
+    for (int h = 0; h < NH; ++h)
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc[h][i] *= dq;
+  }
+}
+
 // ------------------------------------------------------------------ the cooperative kernel
-template <int BN, bool A_MN, bool B_MN, int CL>
+// Op: operand format.  The FP8 form promotes (see the top of the file): each k-block's four wgmmas accumulate into
+// `part`, which is added to acc once they retire; BN <= 192 keeps both tiles in the 232 registers of a thread.
+template <class Op, int BN, bool A_MN, bool B_MN, int CL>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                  const GemmParams p) {
@@ -151,6 +195,8 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   const int num_m = (p.M + CL * BM - 1) / (CL * BM);
   const int num_n = (p.N + BN - 1) / BN;
   const int num_tiles = num_m * num_n;
+  constexpr int BK = Op::BK;
+  constexpr bool PROMOTE = Op::FP8;
   const int num_kb = (p.K + BK - 1) / BK;
 
   if (threadIdx.x == 0) {
@@ -222,36 +268,55 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       if (CL == 2) mbar_arrive_cluster(mapa_u32(smem_u32(&empty[s_]), rank ^ 1));
     };
     float* st = epi + (warp - 4) * 16 * EPI_PITCH;
+    float dq = 1.0f;
+    if constexpr (Op::FP8) dq = *p.a_scale_inv * *p.b_scale_inv;
     float acc[1][BN / 2];
+    float part[PROMOTE ? BN / 2 : 1];
     int stage = 0;
     uint32_t phase = 0;
     for (int tile = cid; tile < num_tiles; tile += ncl) {
       const int m0 = (tile / num_n) * (CL * BM) + rank * BM;
       const int n0 = (tile % num_n) * BN;
       int prev = 0;
+      if constexpr (PROMOTE) {
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc[0][i] = 0.0f;
+      }
       for (int kb = 0; kb < num_kb; ++kb) {
         mbar_wait(&full[stage], phase);
         const uint32_t sa = smem_u32(smem_a + stage * A_STAGE_BYTES);
         const uint32_t sb = smem_u32(smem_b + stage * Cfg::B_STAGE_BYTES);
         wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < BK / 16; ++k) {
+        for (int k = 0; k < K_MMAS; ++k) {
           const uint64_t ad = A_MN ? gmma_desc(sa + cw * 8192 + k * 2048, 8192, 1024)
                                    : gmma_desc(sa + cw * 8192 + k * 32, 16, 1024);
           const uint64_t bd = B_MN ? gmma_desc(sb + k * 2048, 8192, 1024) : gmma_desc(sb + k * 32, 16, 1024);
-          Wgmma<BN>::template ss<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc[0], ad, bd, (kb > 0 || k > 0) ? 1u : 0u);
+          if constexpr (PROMOTE)
+            mma<Op, BN, A_MN, B_MN>(part, ad, bd, k > 0 ? 1u : 0u);
+          else
+            mma<Op, BN, A_MN, B_MN>(acc[0], ad, bd, (kb > 0 || k > 0) ? 1u : 0u);
         }
         wgmma_commit();
-        if (kb > 0) {  // the MMAs of the previous k-block retired: its smem slot is free
+        if constexpr (PROMOTE) {  // this k-block's partial sum, added in fp32; its smem slot is free
+          wgmma_wait<0>();
+          wgmma_reg_fence(part, BN / 2);
+          release(stage);
+#pragma unroll
+          for (int i = 0; i < BN / 2; ++i) acc[0][i] += part[i];
+        } else if (kb > 0) {  // the MMAs of the previous k-block retired: its smem slot is free
           wgmma_wait<1>();
           release(prev);
         }
         prev = stage;
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
-      wgmma_wait<0>();
-      wgmma_reg_fence(acc[0], BN / 2);
-      release(prev);
+      if constexpr (!PROMOTE) {
+        wgmma_wait<0>();
+        wgmma_reg_fence(acc[0], BN / 2);
+        release(prev);
+      }
+      dequantise<Op, BN, 1>(acc, dq);
       epilogue_tile<BN, 1>(p, acc, st, m0 + cw * 64, n0);
     }
   }
@@ -268,7 +333,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 // tensor cores stay busy through every epilogue except the CTA's last.
 constexpr int PP_BN = 128;
 
-template <bool A_MN, bool B_MN>
+template <class Op, bool A_MN, bool B_MN>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_bf16_pingpong_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                           const GemmParams p) {
@@ -288,6 +353,7 @@ gemm_bf16_pingpong_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_
   const int wg = threadIdx.x >> 7;
   const int num_n = (p.N + PP_BN - 1) / PP_BN;
   const int num_tiles = ((p.M + BM - 1) / BM) * num_n;
+  constexpr int BK = Op::BK;
   const int num_kb = (p.K + BK - 1) / BK;
 
   if (threadIdx.x == 0) {
@@ -342,6 +408,8 @@ gemm_bf16_pingpong_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_
     const int cw = wg - 1;              // this warpgroup takes the CTA's tiles j with (j & 1) == cw
     const bool signal = (threadIdx.x & 127) == 0;
     float* st = epi + (warp - 4) * 16 * EPI_PITCH;
+    float dq = 1.0f;
+    if constexpr (Op::FP8) dq = *p.a_scale_inv * *p.b_scale_inv;
     float acc[2][PP_BN / 2];            // rows [0, 64) and [64, 128) of the tile
     for (int j = cw, tile = blockIdx.x + cw * gridDim.x; tile < num_tiles; j += 2, tile += 2 * gridDim.x) {
       const int m0 = (tile / num_n) * BM;
@@ -358,13 +426,13 @@ gemm_bf16_pingpong_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_
         const uint32_t sb = smem_u32(smem_b + stage * Cfg::B_STAGE_BYTES);
         wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < BK / 16; ++k) {
+        for (int k = 0; k < K_MMAS; ++k) {
           const uint64_t bd = B_MN ? gmma_desc(sb + k * 2048, 8192, 1024) : gmma_desc(sb + k * 32, 16, 1024);
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
             const uint64_t ad = A_MN ? gmma_desc(sa + h * 8192 + k * 2048, 8192, 1024)
                                      : gmma_desc(sa + h * 8192 + k * 32, 16, 1024);
-            Wgmma<PP_BN>::template ss<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc[h], ad, bd, (kb > 0 || k > 0) ? 1u : 0u);
+            mma<Op, PP_BN, A_MN, B_MN>(acc[h], ad, bd, (kb > 0 || k > 0) ? 1u : 0u);
           }
         }
         wgmma_commit();
@@ -381,25 +449,27 @@ gemm_bf16_pingpong_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_
       wgmma_reg_fence(acc[0], PP_BN / 2);
       wgmma_reg_fence(acc[1], PP_BN / 2);
       if (signal) mbar_arrive(&empty[prev]);
+      dequantise<Op, PP_BN, 2>(acc, dq);
       epilogue_tile<PP_BN, 2>(p, acc, st, m0, n0);
     }
   }
 }
 
 // ------------------------------------------------------------------ host side
-template <int BN, bool A_MN, bool B_MN, int CL>
+template <class Op, int BN, bool A_MN, bool B_MN, int CL>
 static int launch_gemm(const void* A, long lda, const void* B, long ldb, const GemmParams& p,
                        cudaStream_t stream) {
   using Cfg = GemmCfg<BN, B_MN>;
+  constexpr int EB = Op::FP8 ? 1 : 2;
   CUtensorMap tmA, tmB;
   int rc;
-  if (!A_MN) rc = make_tmap_2d(&tmA, A, (uint64_t)p.K, (uint64_t)p.M, lda, 64, BM);
+  if (!A_MN) rc = make_tmap_2d(&tmA, A, (uint64_t)p.K, (uint64_t)p.M, lda, Op::BK, BM, EB);
   else       rc = make_tmap_2d(&tmA, A, (uint64_t)p.M, (uint64_t)p.K, lda, 64, 64);
   if (rc) return rc;
-  if (!B_MN) rc = make_tmap_2d(&tmB, B, (uint64_t)p.K, (uint64_t)p.N, ldb, 64, BN / CL);
+  if (!B_MN) rc = make_tmap_2d(&tmB, B, (uint64_t)p.K, (uint64_t)p.N, ldb, Op::BK, BN / CL, EB);
   else       rc = make_tmap_2d(&tmB, B, (uint64_t)p.N, (uint64_t)p.K, ldb, 64, 64);
   if (rc) return rc;
-  auto kern = gemm_bf16_kernel<BN, A_MN, B_MN, CL>;
+  auto kern = gemm_bf16_kernel<Op, BN, A_MN, B_MN, CL>;
   static bool attr_set[64] = {};
   if (first_use_on_device(attr_set)) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -432,19 +502,20 @@ static int launch_gemm(const void* A, long lda, const void* B, long ldb, const G
   return check_launch("gemm_bf16_kernel");
 }
 
-template <bool A_MN, bool B_MN>
+template <class Op, bool A_MN, bool B_MN>
 static int launch_gemm_pingpong(const void* A, long lda, const void* B, long ldb, const GemmParams& p,
                                 cudaStream_t stream) {
   using Cfg = GemmCfg<PP_BN, B_MN>;
+  constexpr int EB = Op::FP8 ? 1 : 2;
   CUtensorMap tmA, tmB;
   int rc;
-  if (!A_MN) rc = make_tmap_2d(&tmA, A, (uint64_t)p.K, (uint64_t)p.M, lda, 64, BM);
+  if (!A_MN) rc = make_tmap_2d(&tmA, A, (uint64_t)p.K, (uint64_t)p.M, lda, Op::BK, BM, EB);
   else       rc = make_tmap_2d(&tmA, A, (uint64_t)p.M, (uint64_t)p.K, lda, 64, 64);
   if (rc) return rc;
-  if (!B_MN) rc = make_tmap_2d(&tmB, B, (uint64_t)p.K, (uint64_t)p.N, ldb, 64, PP_BN);
+  if (!B_MN) rc = make_tmap_2d(&tmB, B, (uint64_t)p.K, (uint64_t)p.N, ldb, Op::BK, PP_BN, EB);
   else       rc = make_tmap_2d(&tmB, B, (uint64_t)p.N, (uint64_t)p.K, ldb, 64, 64);
   if (rc) return rc;
-  auto kern = gemm_bf16_pingpong_kernel<A_MN, B_MN>;
+  auto kern = gemm_bf16_pingpong_kernel<Op, A_MN, B_MN>;
   static bool attr_set[64] = {};
   if (first_use_on_device(attr_set)) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
@@ -460,19 +531,19 @@ static int launch_gemm_pingpong(const void* A, long lda, const void* B, long ldb
 
 static int dispatch_pingpong(bool a_mn, bool b_mn, const void* A, long lda, const void* B, long ldb,
                              const GemmParams& p, cudaStream_t stream) {
-  if (!a_mn && !b_mn) return launch_gemm_pingpong<false, false>(A, lda, B, ldb, p, stream);
-  if (!a_mn && b_mn) return launch_gemm_pingpong<false, true>(A, lda, B, ldb, p, stream);
-  return launch_gemm_pingpong<true, true>(A, lda, B, ldb, p, stream);
+  if (!a_mn && !b_mn) return launch_gemm_pingpong<OpBf16, false, false>(A, lda, B, ldb, p, stream);
+  if (!a_mn && b_mn) return launch_gemm_pingpong<OpBf16, false, true>(A, lda, B, ldb, p, stream);
+  return launch_gemm_pingpong<OpBf16, true, true>(A, lda, B, ldb, p, stream);
 }
 
 template <bool A_MN, bool B_MN, int CL>
 static int dispatch_bn(int bn, const void* A, long lda, const void* B, long ldb,
                        const GemmParams& p, cudaStream_t stream) {
   switch (bn) {
-    case 256: return launch_gemm<256, A_MN, B_MN, CL>(A, lda, B, ldb, p, stream);
-    case 192: return launch_gemm<192, A_MN, B_MN, CL>(A, lda, B, ldb, p, stream);
-    case 176: return launch_gemm<176, A_MN, B_MN, CL>(A, lda, B, ldb, p, stream);
-    case 128: return launch_gemm<128, A_MN, B_MN, CL>(A, lda, B, ldb, p, stream);
+    case 256: return launch_gemm<OpBf16, 256, A_MN, B_MN, CL>(A, lda, B, ldb, p, stream);
+    case 192: return launch_gemm<OpBf16, 192, A_MN, B_MN, CL>(A, lda, B, ldb, p, stream);
+    case 176: return launch_gemm<OpBf16, 176, A_MN, B_MN, CL>(A, lda, B, ldb, p, stream);
+    case 128: return launch_gemm<OpBf16, 128, A_MN, B_MN, CL>(A, lda, B, ldb, p, stream);
     default: return set_error("ivb_gemm_bf16: unsupported BN");
   }
 }
@@ -485,14 +556,15 @@ static int dispatch_major(int bn, bool a_mn, bool b_mn, const void* A, long lda,
   return dispatch_bn<true, true, CL>(bn, A, lda, B, ldb, p, stream);
 }
 
-// Pick the N tile that wastes the fewest padded columns / partial waves.
-static int choose_bn(int M, int N, int cl) {
+// Pick the N tile that wastes the fewest padded columns / partial waves (fp8: of the two tiles its cooperative kernel has).
+static int choose_bn(int M, int N, int cl, bool fp8 = false) {
   const int cand[4] = {256, 192, 176, 128};
+  const int first = fp8 ? 1 : 0, step = fp8 ? 2 : 1;
   const int sms = num_sms() / cl;
   const int num_m = (M + cl * BM - 1) / (cl * BM);
   double best = 1e30;
   int best_bn = 256;
-  for (int i = 0; i < 4; ++i) {
+  for (int i = first; i < 4; i += step) {
     const int bn = cand[i];
     const int num_n = (N + bn - 1) / bn;
     const long tiles = (long)num_m * num_n;
@@ -519,6 +591,54 @@ static bool use_pingpong(int M, int N, int K) {
 
 static bool g_default_2cta = false;
 
+// Operand rules of the fused epilogue (ivb200.h), shared by both entry points; `fn` names the entry point in messages.
+static int check_epilogue_args(const char* fn, int epilogue, const void* out0, const void* out1, long ld1,
+                               const void* aux, long ldaux, const void* bias, const void* gamma) {
+  char msg[128];
+  auto fail = [&](const char* what) {
+    std::snprintf(msg, sizeof(msg), "%s: %s", fn, what);
+    return set_error(msg);
+  };
+  if (out0 == nullptr) return fail("out0 is null");
+  if ((epilogue == IVB_EPI_RESID || epilogue == IVB_EPI_GELU_BWD) && aux == nullptr) return fail("epilogue needs aux");
+  // the epilogue reads and writes every operand in 16-byte vectors (epilogue_chunk): each row must start on 16 bytes
+  if (out1 != nullptr && (ld1 & 7)) return fail("ld1 must be a multiple of 8 elements");
+  if (aux != nullptr && (ldaux & (epilogue == IVB_EPI_RESID ? 3 : 7)))
+    return fail("ldaux must be a multiple of 8 bf16 or 4 fp32 elements");
+  const void* vec_ptrs[5] = {out0, out1, aux, bias, gamma};
+  const char* vec_msgs[5] = {"out0 must be 16-byte aligned", "out1 must be 16-byte aligned", "aux must be 16-byte aligned",
+                             "bias must be 16-byte aligned", "gamma must be 16-byte aligned"};
+  for (int i = 0; i < 5; ++i)
+    if (reinterpret_cast<uintptr_t>(vec_ptrs[i]) & 15) return fail(vec_msgs[i]);
+  return 0;
+}
+
+static GemmParams make_params(int M, int N, int K, int epilogue, int flags, void* out0, long ld0, void* out1, long ld1,
+                              const void* bias, const void* gamma, const void* aux, long ldaux, const float* rowscale) {
+  GemmParams p;
+  p.M = M; p.N = N; p.K = K; p.epi = epilogue; p.flags = flags;
+  p.out0 = out0; p.ld0 = ld0; p.out1 = out1; p.ld1 = ld1;
+  p.bias = reinterpret_cast<const __nv_bfloat16*>(bias);
+  p.gamma = reinterpret_cast<const __nv_bfloat16*>(gamma);
+  p.aux = aux; p.ldaux = ldaux; p.rowscale = rowscale;
+  p.a_scale_inv = p.b_scale_inv = nullptr;
+  return p;
+}
+
+// FP8 kernel choice: the ping-pong kernel (accumulation in the tensor core) where use_pingpong picks it, otherwise the
+// cooperative kernel, which promotes each k-block to fp32 (BN 192 or 128).  Promotion is not needed for accuracy at
+// the step's shapes: the tensor-core accumulation adds at most 4.5 % of the error the fp8 quantisation already carries
+// (fc2, K = 6144; tests/test_gemm_fp8_gpu.py::test_accumulation_error_at_step_shapes, DESIGN.md 4.1), and ping-pong is
+// the faster form at every one of them.
+
+template <class Op>
+static int dispatch_fp8(bool pingpong, int bn, const void* A, long lda, const void* B, long ldb, const GemmParams& p,
+                        cudaStream_t stream) {
+  if (pingpong) return launch_gemm_pingpong<Op, false, false>(A, lda, B, ldb, p, stream);
+  if (bn == 192) return launch_gemm<Op, 192, false, false, 1>(A, lda, B, ldb, p, stream);
+  return launch_gemm<Op, 128, false, false, 1>(A, lda, B, ldb, p, stream);
+}
+
 }  // namespace ivb
 
 using namespace ivb;
@@ -534,26 +654,9 @@ extern "C" int ivb_gemm_bf16(const void* A, int a_mn_major, long lda, const void
   if (M <= 0 || N <= 0 || K <= 0) return set_error("ivb_gemm_bf16: empty problem");
   if ((N & 7) || (lda & 7) || (ldb & 7) || (ld0 & 7))
     return set_error("ivb_gemm_bf16: N and leading dimensions must be multiples of 8 elements");
-  if (out0 == nullptr) return set_error("ivb_gemm_bf16: out0 is null");
-  if ((epilogue == IVB_EPI_RESID || epilogue == IVB_EPI_GELU_BWD) && aux == nullptr)
-    return set_error("ivb_gemm_bf16: epilogue needs aux");
-  // the epilogue reads and writes every operand in 16-byte vectors (epilogue_chunk): each row must start on 16 bytes
-  if (out1 != nullptr && (ld1 & 7)) return set_error("ivb_gemm_bf16: ld1 must be a multiple of 8 elements");
-  if (aux != nullptr && (ldaux & (epilogue == IVB_EPI_RESID ? 3 : 7)))
-    return set_error("ivb_gemm_bf16: ldaux must be a multiple of 8 bf16 or 4 fp32 elements");
-  const void* vec_ptrs[5] = {out0, out1, aux, bias, gamma};
-  const char* vec_msgs[5] = {"ivb_gemm_bf16: out0 must be 16-byte aligned", "ivb_gemm_bf16: out1 must be 16-byte aligned",
-                             "ivb_gemm_bf16: aux must be 16-byte aligned", "ivb_gemm_bf16: bias must be 16-byte aligned",
-                             "ivb_gemm_bf16: gamma must be 16-byte aligned"};
-  for (int i = 0; i < 5; ++i)
-    if (reinterpret_cast<uintptr_t>(vec_ptrs[i]) & 15) return set_error(vec_msgs[i]);
+  if (int rc = check_epilogue_args("ivb_gemm_bf16", epilogue, out0, out1, ld1, aux, ldaux, bias, gamma)) return rc;
   if (a_mn_major && !b_mn_major) return set_error("ivb_gemm_bf16: (A MN-major, B K-major) unused");
-  GemmParams p;
-  p.M = M; p.N = N; p.K = K; p.epi = epilogue; p.flags = flags;
-  p.out0 = out0; p.ld0 = ld0; p.out1 = out1; p.ld1 = ld1;
-  p.bias = reinterpret_cast<const __nv_bfloat16*>(bias);
-  p.gamma = reinterpret_cast<const __nv_bfloat16*>(gamma);
-  p.aux = aux; p.ldaux = ldaux; p.rowscale = rowscale;
+  const GemmParams p = make_params(M, N, K, epilogue, flags, out0, ld0, out1, ld1, bias, gamma, aux, ldaux, rowscale);
   // kernel selection: the CTA-pair (cluster) kernel when forced, or by default for problems tall enough to fill
   // 256-row tiles; the ping-pong kernel when forced or chosen by use_pingpong; the cooperative single-CTA kernel
   // otherwise / when IVB_FLAG_1CTA is set.
@@ -568,4 +671,31 @@ extern "C" int ivb_gemm_bf16(const void* A, int a_mn_major, long lda, const void
   const int bn = tile_n > 0 ? tile_n : choose_bn(M, N, cl);
   if (cl == 2) return dispatch_major<2>(bn, a_mn_major != 0, b_mn_major != 0, A, lda, B, ldb, p, stream);
   return dispatch_major<1>(bn, a_mn_major != 0, b_mn_major != 0, A, lda, B, ldb, p, stream);
+}
+
+extern "C" int ivb_gemm_fp8(const void* A, int a_mn_major, long lda, int a_format, const float* a_scale_inv,
+                            const void* B, int b_mn_major, long ldb, const float* b_scale_inv, int M, int N, int K,
+                            int epilogue, int flags, void* out0, long ld0, void* out1, long ld1, const void* bias,
+                            const void* gamma, const void* aux, long ldaux, const float* rowscale, int tile_n,
+                            void* stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  if (M <= 0 || N <= 0 || K <= 0) return set_error("ivb_gemm_fp8: empty problem");
+  if (a_mn_major || b_mn_major) return set_error("ivb_gemm_fp8: both operands must be K-major");
+  if ((lda & 15) || (ldb & 15)) return set_error("ivb_gemm_fp8: lda and ldb must be multiples of 16 elements");
+  if ((N & 7) || (ld0 & 7)) return set_error("ivb_gemm_fp8: N and ld0 must be multiples of 8 elements");
+  if (a_format != IVB_FP8_E4M3 && a_format != IVB_FP8_E5M2) return set_error("ivb_gemm_fp8: unknown a_format");
+  if (a_scale_inv == nullptr || b_scale_inv == nullptr) return set_error("ivb_gemm_fp8: scale_inv pointers are null");
+  if (int rc = check_epilogue_args("ivb_gemm_fp8", epilogue, out0, out1, ld1, aux, ldaux, bias, gamma)) return rc;
+  const bool force1 = (flags & IVB_FLAG_1CTA) != 0, forcepp = (flags & IVB_FLAG_PINGPONG) != 0;
+  if (flags & IVB_FLAG_2CTA) return set_error("ivb_gemm_fp8: no CTA-pair kernel");
+  if (force1 && forcepp) return set_error("ivb_gemm_fp8: IVB_FLAG_1CTA and IVB_FLAG_PINGPONG exclude each other");
+  if (tile_n != 0 && tile_n != 128 && tile_n != 192) return set_error("ivb_gemm_fp8: tile_n must be 0, 128 or 192");
+  if (forcepp && tile_n == 192) return set_error("ivb_gemm_fp8: the ping-pong kernel has tile_n 128");
+  GemmParams p = make_params(M, N, K, epilogue, flags, out0, ld0, out1, ld1, bias, gamma, aux, ldaux, rowscale);
+  p.a_scale_inv = a_scale_inv;
+  p.b_scale_inv = b_scale_inv;
+  const bool pingpong = forcepp || (!force1 && tile_n != 192 && use_pingpong(M, N, K));
+  const int bn = tile_n > 0 ? tile_n : choose_bn(M, N, 1, true);
+  if (a_format == IVB_FP8_E5M2) return dispatch_fp8<OpFp8<true>>(pingpong, bn, A, lda, B, ldb, p, stream);
+  return dispatch_fp8<OpFp8<false>>(pingpong, bn, A, lda, B, ldb, p, stream);
 }

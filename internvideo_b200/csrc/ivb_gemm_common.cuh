@@ -22,6 +22,8 @@ struct GemmParams {
   const void* aux;
   long ldaux;
   const float* rowscale;  // EPI_RESID: optional per-row multiplier of the branch (DropPath keep/scale)
+  const float* a_scale_inv;  // fp8 operands: device scalars, the accumulator is multiplied by their product
+  const float* b_scale_inv;
 };
 
 // 32-byte row pieces as two 128-bit accesses (sm_90 has no 256-bit global load / store).

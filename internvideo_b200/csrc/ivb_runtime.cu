@@ -63,16 +63,17 @@ static PFN_encodeTiled get_encode() {
 }
 
 int make_tmap_2d(CUtensorMap* out, const void* base, uint64_t inner, uint64_t outer,
-                 long ld_elems, uint32_t box_inner, uint32_t box_outer) {
+                 long ld_elems, uint32_t box_inner, uint32_t box_outer, int elem_bytes) {
   PFN_encodeTiled enc = get_encode();
   if (!enc) return set_error("cuTensorMapEncodeTiled unavailable (no CUDA driver?)");
   if ((reinterpret_cast<uintptr_t>(base) & 15) != 0)
     return set_error("TMA base pointer must be 16-byte aligned");
   cuuint64_t dims[2] = {inner, outer};
-  cuuint64_t strides[1] = {static_cast<cuuint64_t>(ld_elems) * 2};
+  cuuint64_t strides[1] = {static_cast<cuuint64_t>(ld_elems) * elem_bytes};
   cuuint32_t box[2] = {box_inner, box_outer};
   cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims,
+  const CUtensorMapDataType dtype = elem_bytes == 1 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+  CUresult r = enc(out, dtype, 2, const_cast<void*>(base), dims,
                    strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {

@@ -108,12 +108,81 @@ def gemm(a, b, *, a_t=False, b_t=False, epi=EPI_BF16, flags=0, out0=None, out1=N
     return out0
 
 
+# ----------------------------------------------------------------------------------------- FP8
+FP8_E4M3, FP8_E5M2 = 0, 1
+FP8_DTYPES = {FP8_E4M3: torch.float8_e4m3fn, FP8_E5M2: torch.float8_e5m2}
+
+
+def _pad16(n):
+    return (n + 15) // 16 * 16
+
+
+def fp8_quantize(x, fmt=FP8_E4M3, transpose=False):
+    """Per-tensor current-scaling cast of a bf16 [M, K] tensor (any row pitch) to FP8 (ivb_fp8_quantize).
+
+    Returns (q [M, K], q_t [K, M] = q^T or None, scale_inv fp32 [1], amax fp32 [1]): x ~ q * scale_inv, with a
+    power-of-two scale.  q and q_t are views of buffers whose row pitch is rounded up to 16 elements (the fp8 GEMM's
+    operand rule)."""
+    _chk(x, bf16, "x")
+    ldx = _rows2d(x, "x")
+    M, K = x.shape
+    dt = FP8_DTYPES[fmt]
+    q = torch.empty((M, _pad16(K)), device=x.device, dtype=dt)[:, :K]
+    q_t = torch.empty((K, _pad16(M)), device=x.device, dtype=dt)[:, :M] if transpose else None
+    stats = torch.empty((2,), device=x.device, dtype=f32)
+    amax, scale_inv = stats[0:1], stats[1:2]
+    ev0 = _prof_begin()
+    rc = _lib_().ivb_fp8_quantize(_p(x), ldx, M, K, fmt, _p(q), q.stride(0), _p(q_t),
+                                  q_t.stride(0) if transpose else 0, _p(amax), _p(scale_inv), _stream())
+    _lib.check(rc, "ivb_fp8_quantize")
+    _prof_end(ev0, 0.0, "fp8_quantize")
+    return q, q_t, scale_inv, amax
+
+
+def gemm_fp8(a, a_scale_inv, b, b_scale_inv, *, epi=EPI_BF16, flags=0, out0=None, out1=None, bias=None, gamma=None,
+             aux=None, rowscale=None, tile_n=0):
+    """D[M,N] = epi(a_scale_inv * b_scale_inv * sum_k A(m,k) B(n,k)) on the FP8 tensor cores (ivb_gemm_fp8).
+
+    a: [M,K] float8_e4m3fn or float8_e5m2; b: [N,K] float8_e4m3fn; both K-major (fp8_quantize's q, or q_t for a
+    transposed operand).  a_scale_inv / b_scale_inv: fp32 [1] CUDA tensors.  Epilogue arguments as for gemm()."""
+    if a.dtype not in FP8_DTYPES.values() or not a.is_cuda:
+        raise _lib.IvbError(f"gemm_fp8: a must be a CUDA float8_e4m3fn / float8_e5m2 tensor, got {a.dtype}")
+    _chk(b, torch.float8_e4m3fn, "b"); _chk(a_scale_inv, f32, "a_scale_inv"); _chk(b_scale_inv, f32, "b_scale_inv")
+    lda = _rows2d(a, "a"); ldb = _rows2d(b, "b")
+    M, K = a.shape
+    N, Kb = b.shape
+    if K != Kb:
+        raise _lib.IvbError(f"gemm_fp8: contraction mismatch {K} vs {Kb}")
+    out_dtype = f32 if epi in (EPI_F32, EPI_RESID) else bf16
+    if out0 is None:
+        out0 = torch.empty((M, N), device=a.device, dtype=out_dtype)
+    _chk(out0, out_dtype, "out0")
+    ld0 = _rows2d(out0, "out0")
+    ld1 = 0
+    if out1 is not None:
+        _chk(out1, bf16, "out1"); ld1 = _rows2d(out1, "out1")
+    _chk(bias, bf16, "bias"); _chk(gamma, bf16, "gamma")
+    ldaux = 0
+    if aux is not None:
+        _chk(aux, f32 if epi == EPI_RESID else bf16, "aux")
+        ldaux = _rows2d(aux, "aux")
+    fmt = FP8_E5M2 if a.dtype == torch.float8_e5m2 else FP8_E4M3
+    ev0 = _prof_begin()
+    rc = _lib_().ivb_gemm_fp8(_p(a), 0, lda, fmt, _p(a_scale_inv), _p(b), 0, ldb, _p(b_scale_inv), M, N, K, epi, flags,
+                              _p(out0), ld0, _p(out1), ld1, _p(bias), _p(gamma), _p(aux), ldaux, _p(rowscale), tile_n,
+                              _stream())
+    _lib.check(rc, "ivb_gemm_fp8")
+    _prof_end(ev0, 2.0 * M * N * K, "gemm")
+    return out0
+
+
 _PROF = [None]
 
 
 class GemmProfiler:
-    """CUDA-event timing of every tensor-core launch (GEMMs, attention forward / backward) on the launching stream
-    (bench.py roofline).  Records (start, stop, algorithmic flops, kind)."""
+    """CUDA-event timing of every tensor-core launch (GEMMs, bf16 and fp8, attention forward / backward) and of the
+    fp8 casts that feed the fp8 GEMMs (kind "fp8_quantize", no flops) on the launching stream (bench.py roofline).
+    Records (start, stop, algorithmic flops, kind)."""
 
     def __init__(self):
         self.records = []
@@ -537,5 +606,5 @@ def _gemm_name(a, b, *, a_t=False, b_t=False, epi=EPI_BF16, **_):
 gemm = _timed(gemm, _gemm_name)
 for _n in ("norm_fwd", "norm_bwd", "layerscale_bwd", "colsum", "attn_fwd", "attn_bwd", "visible_indices",
            "im2col_visible", "gather_add", "scatter_add", "ln_l2_fwd", "ln_l2_bwd", "vtc_loss_fwd", "vtc_loss_bwd",
-           "l2norm_rows_fwd", "l2norm_rows_bwd", "pixel_targets", "mse_loss", "adamw_step"):
+           "l2norm_rows_fwd", "l2norm_rows_bwd", "pixel_targets", "mse_loss", "adamw_step", "fp8_quantize", "gemm_fp8"):
     globals()[_n] = _timed(globals()[_n])

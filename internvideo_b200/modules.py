@@ -202,6 +202,8 @@ class Block(nn.Module):
         self.with_cp = bool(with_cp)
         self.use_fused_rmsnorm = use_fused_rmsnorm
         self.num_heads = num_heads
+        # FP8 GEMMs for the forward and input-gradient passes (set_fp8); read at call time
+        self.fp8 = False
 
     def forward_stream(self, x2d, B, n, rowscale=None):
         """fp32 residual stream [B*n, D] -> [B*n, D] (the hot path used by the model).
@@ -220,7 +222,7 @@ class Block(nn.Module):
         if not torch.is_grad_enabled():
             return self.forward_infer(x2d, B, n, (rs1, rs2))
         return ops.BlockFn.apply(
-            x2d, (B, n, self.num_heads, self.mlp.gelu_tanh, self.with_cp), self.norm1.weight, a.qkv.weight, a.qkv.bias,
+            x2d, (B, n, self.num_heads, self.mlp.gelu_tanh, self.with_cp, self.fp8), self.norm1.weight, a.qkv.weight, a.qkv.bias,
             a.q_norm.weight if a.qk_normalization else None, a.k_norm.weight if a.qk_normalization else None,
             a.proj.weight, a.proj.bias, g1, self.norm2.weight, self.mlp.fc1.weight, self.mlp.fc1.bias,
             self.mlp.fc2.weight, self.mlp.fc2.bias, g2, rs1, rs2)
@@ -237,8 +239,8 @@ class Block(nn.Module):
     def forward_infer(self, x2d, B, n, rowscale=(None, None)):
         """No-grad form (frozen towers / teachers): 14 kernels, nothing saved, no GELU' / pre-LayerScale copies."""
         with torch.no_grad():
-            out, _ = ops.block_forward(x2d, (B, n, self.num_heads, self.mlp.gelu_tanh), self._param_tuple(),
-                                       rowscale[0], rowscale[1], save=False)
+            out, _ = ops.block_forward(x2d, (B, n, self.num_heads, self.mlp.gelu_tanh, False, self.fp8),
+                                       self._param_tuple(), rowscale[0], rowscale[1], save=False)
         return out
 
     def forward(self, x, residual=None):
@@ -249,6 +251,22 @@ class Block(nn.Module):
             return torch.zeros_like(x), out.to(residual.dtype)
         out = self.forward_stream(x.float().reshape(B * n, D).contiguous(), B, n)
         return out.reshape(B, n, D).to(x.dtype)
+
+
+def set_fp8(model: nn.Module, enabled: bool = True) -> int:
+    """Switch the FP8 mode of every ViT Block in `model` (stage-1 student, CLIP tower, stage-2 tower, InternVL teacher)
+    on or off; returns how many blocks were switched.
+
+    In FP8 mode a block runs its forward GEMMs (qkv, proj, fc1, fc2) and its input-gradient GEMMs on the FP8 tensor
+    cores: activations and weights in E4M3, gradients in E5M2, each tensor with a power-of-two scale from its own amax
+    (no state, nothing in the state_dict).  Weight gradients, attention, norms and everything outside the blocks stay
+    bf16.  The mode is read when a block runs: switch it before capturing a CUDA graph of the step."""
+    n = 0
+    for mod in model.modules():
+        if isinstance(mod, Block):
+            mod.fp8 = bool(enabled)
+            n += 1
+    return n
 
 
 class PatchEmbed(nn.Module):

@@ -194,6 +194,23 @@ class PoolAttnFn(torch.autograd.Function):
 
 
 # ------------------------------------------------------------------------------------------ fused ViT block
+def _block_fp8(dims):
+    """dims = (B, n, H, gelu_tanh[, checkpoint[, fp8]]): the block's FP8 mode (modules.set_fp8)."""
+    return len(dims) > 5 and bool(dims[5])
+
+
+def _fp8_linear(act, w8, **epilogue):
+    """act (bf16) cast to FP8 with its own scale, times an FP8 weight copy w8 = (q, scale_inv), fused epilogue."""
+    q, _, s, _ = ll.fp8_quantize(act, ll.FP8_E4M3)
+    return ll.gemm_fp8(q, s, w8[0], w8[1], **epilogue)
+
+
+def _fp8_dgrad(dy, wt8, ws, **epilogue):
+    """dx = dy W with dy cast to E5M2 and wt8 the E4M3 copy of W^T (scale_inv ws)."""
+    q, _, s, _ = ll.fp8_quantize(dy, ll.FP8_E5M2)
+    return ll.gemm_fp8(q, s, wt8, ws, **epilogue)
+
+
 def block_forward(x, dims, params, rs1=None, rs2=None, save=True):
     """One spatio-temporal ViT block over the fp32 residual stream [B*n, D] (Block.forward,
     internvideo2_pretrain.py:279-297):
@@ -204,15 +221,27 @@ def block_forward(x, dims, params, rs1=None, rs2=None, save=True):
 
     14 kernels.  save=True also writes what the backward needs (pre-LayerScale branch outputs, GELU') and returns
     it; save=False is the inference / recompute-later form (frozen towers, activation checkpointing): nothing
-    extra is written.  Returns (x2, saved | None)."""
+    extra is written.  Returns (x2, saved | None).
+
+    FP8 mode (dims[5]): the four weights are cast to E4M3 (with save, also transposed, for the backward's dgrad) and
+    n1, a, n2 and g before their GEMM, each with its own per-tensor scale; the GEMMs keep their fused epilogues."""
     B, n, H, gelu_tanh = dims[:4]
     n1w, qkvw, qkvb, qnw, knw, projw, projb, g1, n2w, fc1w, fc1b, fc2w, fc2b, g2 = params
     M, D = x.shape
     d = D // H
     if x.dtype != f32 or not x.is_cuda:
         raise ll._lib.IvbError("block_forward: residual stream must be a CUDA fp32 tensor [B*n, D]")
+    w8 = None
+    if _block_fp8(dims):
+        # (q, q_t, scale_inv) per weight; q_t only when the backward will need it
+        w8 = [ll.fp8_quantize(w, ll.FP8_E4M3, transpose=save)[:3] for w in (qkvw, projw, fc1w, fc2w)]
+
+    def linear(act, i, w, **epilogue):
+        if w8 is None:
+            return ll.gemm(act, w, **epilogue)
+        return _fp8_linear(act, (w8[i][0], w8[i][2]), **epilogue)
     n1, _, rstd1 = ll.norm_fwd(x, n1w, want_stats=save)
-    qkv = ll.gemm(n1, qkvw, bias=qkvb)
+    qkv = linear(n1, 0, qkvw, bias=qkvb)
     rq = rk = None
     if qnw is not None:
         qkn = torch.empty((M, 2 * D), device=x.device, dtype=bf16)
@@ -227,7 +256,7 @@ def block_forward(x, dims, params, rs1=None, rs2=None, save=True):
         q, k = qkv[:, :D], qkv[:, D:2 * D]
     a, lse = ll.attn_fwd(q, k, qkv[:, 2 * D:], B, n, H, d, d ** -0.5, want_lse=save)
     y1 = torch.empty((M, D), device=x.device, dtype=bf16) if (g1 is not None and save) else None
-    x1 = ll.gemm(a, projw, epi=ll.EPI_RESID, bias=projb, gamma=g1, aux=x, out1=y1, rowscale=rs1)
+    x1 = linear(a, 1, projw, epi=ll.EPI_RESID, bias=projb, gamma=g1, aux=x, out1=y1, rowscale=rs1)
     n2, _, rstd2 = ll.norm_fwd(x1, n2w, want_stats=save)
     Hd = fc1w.shape[0]
     flags = ll.FLAG_GELU_TANH if gelu_tanh else 0
@@ -236,12 +265,14 @@ def block_forward(x, dims, params, rs1=None, rs2=None, save=True):
         # h holds gelu'(pre-activation): the only thing the backward needs of it (FLAG_GELU_SAVE_GRAD)
         h = torch.empty((M, Hd), device=x.device, dtype=bf16)
         flags |= ll.FLAG_GELU_SAVE_GRAD
-    g = ll.gemm(n2, fc1w, epi=ll.EPI_BIAS_GELU, flags=flags, bias=fc1b, out1=h)
+    g = linear(n2, 2, fc1w, epi=ll.EPI_BIAS_GELU, flags=flags, bias=fc1b, out1=h)
     y2 = torch.empty((M, D), device=x.device, dtype=bf16) if (g2 is not None and save) else None
-    x2 = ll.gemm(g, fc2w, epi=ll.EPI_RESID, bias=fc2b, gamma=g2, aux=x1, out1=y2, rowscale=rs2)
+    x2 = linear(g, 3, fc2w, epi=ll.EPI_RESID, bias=fc2b, gamma=g2, aux=x1, out1=y2, rowscale=rs2)
     if not save:
         return x2, None
-    return x2, (n1, qkv, qkn, a, lse, rstd1, rq, rk, x1, y1, n2, rstd2, h, g, y2, flags)
+    # the E4M3 copies of W^T and their scales (None without FP8): the dgrad operands of the backward
+    wt8 = tuple(t for q, q_t, s in w8 for t in (q_t, s)) if w8 is not None else (None,) * 8
+    return x2, (n1, qkv, qkn, a, lse, rstd1, rq, rk, x1, y1, n2, rstd2, h, g, y2) + wt8 + (flags,)
 
 
 def block_forward_ln_infer(x, B, n, H, scale, params, head_axis_attention=False):
@@ -273,7 +304,8 @@ def block_forward_ln_infer(x, B, n, H, scale, params, head_axis_attention=False)
 def block_backward(x, saved, dims, tensors, P, dx2, rs1, rs2):
     """Backward of block_forward: 26 kernels.  `tensors` are the parameter tensors as autograd handed them back,
     `P` the nn.Parameter objects (gradient sink).  Returns (dx0, per-parameter gradients | None when the sink took them)."""
-    n1, qkv, qkn, a, lse, rstd1, rq, rk, x1, y1, n2, rstd2, h, g, y2, flags = saved
+    n1, qkv, qkn, a, lse, rstd1, rq, rk, x1, y1, n2, rstd2, h, g, y2 = saved[:15]
+    wt8, flags = saved[15:23], saved[23]
     n1w, qkvw, qkvb, qnw, knw, projw, projb, g1, n2w, fc1w, fc1b, fc2w, fc2b, g2 = tensors
     B, n, H = dims[:3]
     M, D = x.shape
@@ -296,6 +328,11 @@ def block_backward(x, saved, dims, tensors, P, dx2, rs1, rs2):
     dqnw, dknw, dn1w, dfc1b, dqkvb = seg["qnw"], seg["knw"], seg["n1w"], seg["fc1b"], seg["qkvb"]
     pn1w, pqkvw, pqkvb, pqnw, pknw, pprojw, pprojb, pg1, pn2w, pfc1w, pfc1b, pfc2w, pfc2b, pg2 = P
 
+    def dgrad(dy, i, w, **epilogue):   # dx = dy W; in FP8 mode on the E5M2 gradient and the E4M3 copy of W^T
+        if wt8[2 * i] is None:
+            return ll.gemm(dy, w, b_t=True, **epilogue)
+        return _fp8_dgrad(dy, wt8[2 * i], wt8[2 * i + 1], **epilogue)
+
     def wgrad(dy, act, param):
         if sink is None:
             return ll.gemm(dy, act, a_t=True, b_t=True)
@@ -305,10 +342,10 @@ def block_backward(x, saved, dims, tensors, P, dx2, rs1, rs2):
     # ---- MLP branch
     dy2 = ll.layerscale_bwd(dx2, y2, g2, dg2 if g2 is not None else None, dcs2, rowscale=rs2)
     dfc2w = wgrad(dy2, g, pfc2w)
-    dh = ll.gemm(dy2, fc2w, b_t=True, epi=ll.EPI_GELU_BWD, flags=flags, aux=h)
+    dh = dgrad(dy2, 3, fc2w, epi=ll.EPI_GELU_BWD, flags=flags, aux=h)
     ll.colsum(dh, out=dfc1b)
     dfc1w = wgrad(dh, n2, pfc1w)
-    dn2 = ll.gemm(dh, fc1w, b_t=True)
+    dn2 = dgrad(dh, 2, fc1w)
     # ---- attention branch
     if g1 is not None and D <= 1536 and M >= 1024:
         # norm2 backward fused with the attention branch's LayerScale backward: the gradient of the residual
@@ -318,7 +355,7 @@ def block_backward(x, saved, dims, tensors, P, dx2, rs1, rs2):
         dx1 = ll.norm_bwd(dn2, x1, n2w, None, rstd2, dx_in=dx2, dweight=dn2w)
         dy1 = ll.layerscale_bwd(dx1, y1, g1, dg1 if g1 is not None else None, dcs1, rowscale=rs1)
     dprojw = wgrad(dy1, a, pprojw)
-    da = ll.gemm(dy1, projw, b_t=True)
+    da = dgrad(dy1, 1, projw)
     dqkv = torch.empty((M, 3 * D), device=x.device, dtype=bf16)
     if qkn is not None:
         q, k = qkn[:, :D], qkn[:, D:]
@@ -334,7 +371,7 @@ def block_backward(x, saved, dims, tensors, P, dx2, rs1, rs2):
     dqkvw = wgrad(dqkv, n1, pqkvw)
     if qkvb is not None:
         ll.colsum(dqkv, out=dqkvb)
-    dn1 = ll.gemm(dqkv, qkvw, b_t=True)
+    dn1 = dgrad(dqkv, 0, qkvw)
     dx0 = ll.norm_bwd(dn1, x, n1w, None, rstd1, dx_in=dx1, dweight=dn1w)
     # ---- O(D) glue: bias grads through LayerScale (layerscale_bwd already folds gamma into the
     # bias-gradient column sums), cast to the parameter dtype
@@ -353,7 +390,7 @@ def block_backward(x, saved, dims, tensors, P, dx2, rs1, rs2):
 
 
 class BlockFn(torch.autograd.Function):
-    """Differentiable block_forward.  dims = (B, n, H, gelu_tanh[, checkpoint]).
+    """Differentiable block_forward.  dims = (B, n, H, gelu_tanh[, checkpoint[, fp8]]).
 
     checkpoint=True is the reference's `with_cp` / `use_checkpoint` (internvideo2_pretrain.py:294-295,
     torch.utils.checkpoint around the block): only the block INPUT (4 D bytes/token) is kept; backward first
@@ -367,7 +404,7 @@ class BlockFn(torch.autograd.Function):
         params = (n1w, qkvw, qkvb, qnw, knw, projw, projb, g1, n2w, fc1w, fc1b, fc2w, fc2b, g2)
         ckpt = len(dims) > 4 and bool(dims[4])
         x2, saved = block_forward(x, dims, params, rs1, rs2, save=not ckpt)
-        ctx.dims, ctx.ckpt = tuple(dims[:4]), ckpt
+        ctx.dims, ctx.ckpt = tuple(dims[:4]) + (False, _block_fp8(dims)), ckpt
         ctx.params = params
         if ckpt:
             ctx.nsaved = 0
