@@ -114,6 +114,33 @@ int ivb_gemm_fp8(const void* A, int a_mn_major, long lda, int a_format, const fl
                  void* out0, long ld0, void* out1, long ld1, const void* bias, const void* gamma, const void* aux,
                  long ldaux, const float* rowscale, int tile_n, void* stream);
 
+/* ---- FP8 with per-row scales (FP8 inference of frozen towers) ----------------------------------
+ * Each row gets its own power-of-two scale, chosen from the row's amax by the ivb_fp8_quantize rule (E4M3, fmax 448):
+ *   scale_r = 2^floor(log2(448 / amax_r)); 1 when amax_r = 0; row_scale_inv[r] = 1 / scale_r, or NaN when the row
+ *   holds an Inf or NaN.  out[r, :] = round-to-nearest-even(row * scale_r) in E4M3.
+ * Dequantisation (q * scale_inv) is exact, and a row's grid refines the whole tensor's, so no element's cast error
+ * exceeds the per-tensor cast's.  The same bits on every run (no atomics).  One stream-ordered kernel per call;
+ * capturable in a CUDA graph.  Columns D (or K) .. ldo of out are not written.  A call that breaks a rule below is
+ * refused before any CUDA call.
+ *
+ * ivb_fp8_quantize_rows: x bf16 [M, K] (pitch ldx, a multiple of 8; K <= IVB_FP8_ROWS_MAX_K) -> out E4M3 [M, K]
+ *   (pitch ldo, a multiple of 16) and row_scale_inv fp32 [M].  Weights take it with rows = output channels (the
+ *   per-channel scales of the GEMM's B operand).  x and out are 16-byte aligned.
+ * ivb_norm_fwd_fp8: y = norm(x) * weight (+ bias) as ivb_norm_fwd computes it (fp32 statistics; x fp32 or bf16,
+ *   pitch ldx a multiple of 8), written only as E4M3 [M, D] (pitch ldo, a multiple of 16) plus row_scale_inv [M]: each
+ *   row is read once and no bf16 copy is written.  D a multiple of 8, D <= IVB_NORM_FP8_MAX_D.  x, weight, bias and
+ *   out are 16-byte aligned.
+ * ivb_gemm_fp8 with IVB_FLAG_FP8_VECTOR_SCALES: a_scale_inv points at M floats and b_scale_inv at N floats, and the
+ *   accumulator (m, n) is multiplied by a_scale_inv[m] * b_scale_inv[n] before the epilogue.  A must be E4M3 and both
+ *   vectors 8-byte aligned; the flag with IVB_FLAG_2CTA or a null vector is refused.                                              */
+#define IVB_FLAG_FP8_VECTOR_SCALES 64
+#define IVB_FP8_ROWS_MAX_K 16384
+#define IVB_NORM_FP8_MAX_D 4096
+int ivb_fp8_quantize_rows(const void* x, long ldx, int M, int K, void* out, long ldo, float* row_scale_inv,
+                          void* stream);
+int ivb_norm_fwd_fp8(const void* x, int x_is_f32, long ldx, const void* weight, const void* bias, float eps,
+                     int is_layernorm, int M, int D, void* out, long ldo, float* row_scale_inv, void* stream);
+
 /* ---- RMSNorm / LayerNorm (row reductions, HBM-bound) -------------------------------------------
  * y(bf16) = norm(x) * weight (+ bias).  is_layernorm=0: RMSNorm (internvideo2_pretrain.py:117-128,
  * FA2 DropoutAddRMSNorm :467; eps 1e-6); 1: nn.LayerNorm (eps 1e-5, :525,:532).

@@ -27,6 +27,8 @@ PROTOTYPES = {
     "ivb_fp8_quantize": (_i, [_vp, _l, _i, _i, _i, _vp, _l, _vp, _l, _vp, _vp, _vp]),
     "ivb_gemm_fp8": (_i, [_vp, _i, _l, _i, _vp, _vp, _i, _l, _vp, _i, _i, _i, _i, _i, _vp, _l, _vp, _l, _vp, _vp,
                           _vp, _l, _vp, _i, _vp]),
+    "ivb_fp8_quantize_rows": (_i, [_vp, _l, _i, _i, _vp, _l, _vp, _vp]),
+    "ivb_norm_fwd_fp8": (_i, [_vp, _i, _l, _vp, _vp, _f, _i, _i, _i, _vp, _l, _vp, _vp]),
     "ivb_norm_fwd": (_i, [_vp, _i, _l, _vp, _vp, _f, _i, _i, _i, _vp, _l, _vp, _vp, _vp]),
     "ivb_norm_bwd": (_i, [_vp, _l, _vp, _i, _l, _vp, _vp, _vp, _i, _i, _i, _vp, _l, _vp, _i, _l,
                           _vp, _vp, _vp]),

@@ -8,8 +8,12 @@
 // A power-of-two scale makes x * scale and the dequantisation exact in fp32, and amax * scale <= fmax means the
 // cast never saturates.  A non-finite amax writes scale_inv = NaN: satfinite alone would clamp an Inf to fmax and
 // hide the overflow, while NaN reaches the GEMM output and the training step's finiteness check.
+//
+// ivb_fp8_quantize_rows applies the same rule to each row on its own (E4M3 only): a row's scale comes from the row's
+// amax, so a row's grid is never coarser than the whole tensor's, and the cast error of an element never larger.
+#include "ivb_fp8.cuh"
 #include "ivb_internal.h"
-#include "ivb_ptx.cuh"
+#include "ivb_rows.cuh"
 
 namespace ivb {
 
@@ -41,35 +45,6 @@ __global__ void __launch_bounds__(256) fp8_amax_kernel(const __nv_bfloat16* __re
   }
   m = __reduce_max_sync(0xffffffffu, m);
   if ((threadIdx.x & 31) == 0 && m != 0) atomicMax(amax_bits, m << 16);
-}
-
-// scale = 2^e with e the largest integer such that amax * 2^e <= fmax = 1.75 * 2^F, from the bits of amax (exact, no
-// rounding of fmax / amax); e is clamped to [-126, 126] so that scale and 1 / scale are normal floats.
-__device__ __forceinline__ void fp8_scale(unsigned amax_bits, int F, float& scale, float& scale_inv) {
-  if ((amax_bits & 0x7f800000u) == 0x7f800000u) {   // Inf or NaN
-    scale = 1.0f;
-    scale_inv = __int_as_float(0x7fc00000);
-    return;
-  }
-  if (amax_bits == 0) {
-    scale = scale_inv = 1.0f;
-    return;
-  }
-  const int E = static_cast<int>((amax_bits >> 23) & 0xff) - 127;
-  int e = F - E - ((amax_bits & 0x7fffffu) > 0x600000u ? 1 : 0);
-  e = min(126, max(-126, e));
-  scale = __int_as_float((e + 127) << 23);
-  scale_inv = __int_as_float((127 - e) << 23);
-}
-
-template <bool E5M2>
-__device__ __forceinline__ uint32_t cvt_fp8x2(float lo, float hi) {
-  uint16_t r;
-  if constexpr (E5M2)
-    asm("cvt.rn.satfinite.e5m2x2.f32 %0, %1, %2;" : "=h"(r) : "f"(hi), "f"(lo));
-  else
-    asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(r) : "f"(hi), "f"(lo));
-  return r;
 }
 
 // One 64 x 64 tile per CTA: thread t converts 16 elements of row t / 4 and writes them to `out`; with out_t, the tile
@@ -129,9 +104,102 @@ __global__ void __launch_bounds__(Q_THREADS) fp8_cast_kernel(const __nv_bfloat16
   }
 }
 
+// ------------------------------------------------------------------ per-row scaling (ivb_fp8_quantize_rows)
+// One CTA per row: thread t holds the row's 8-element chunks t, t + 128, ... in registers (NV of them, packed bf16),
+// so the row is read from HBM once; the row's amax is a max over integer magnitude bits (no atomics, the same bits on
+// every run), then each chunk is scaled, cast and stored.
+constexpr int R_THREADS = 128;
+
+template <int NV>
+__global__ void __launch_bounds__(R_THREADS) fp8_rows_kernel(const __nv_bfloat16* __restrict__ x, long ldx, int K,
+                                                            uint8_t* __restrict__ out, long ldo,
+                                                            float* __restrict__ scale_inv) {
+  __shared__ unsigned red[R_THREADS / 32];
+  pdl_wait();
+  pdl_launch_dependents();
+  const long row = blockIdx.x;
+  const __nv_bfloat16* src = x + row * ldx;
+  uint4 v[NV];
+  unsigned m = 0;   // bf16 magnitude bits: NaN > Inf > every finite value
+#pragma unroll
+  for (int i = 0; i < NV; ++i) {
+    const int c = (threadIdx.x + R_THREADS * i) * 8;
+    v[i] = make_uint4(0u, 0u, 0u, 0u);
+    if (c + 8 <= K) {
+      v[i] = *reinterpret_cast<const uint4*>(src + c);
+    } else if (c < K) {   // the row's last, partial chunk: no read past element K - 1
+      const uint16_t* s16 = reinterpret_cast<const uint16_t*>(src + c);
+      uint32_t w[4] = {0u, 0u, 0u, 0u};
+#pragma unroll
+      for (int k = 0; k < 8; ++k)
+        if (c + k < K) w[k >> 1] |= static_cast<uint32_t>(s16[k]) << (16 * (k & 1));
+      v[i] = make_uint4(w[0], w[1], w[2], w[3]);
+    }
+    const uint32_t w[4] = {v[i].x, v[i].y, v[i].z, v[i].w};
+#pragma unroll
+    for (int k = 0; k < 4; ++k) m = max(m, max(w[k] & 0x7fffu, (w[k] >> 16) & 0x7fffu));
+  }
+  m = __reduce_max_sync(0xffffffffu, m);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = m;
+  __syncthreads();
+#pragma unroll
+  for (int w = 0; w < R_THREADS / 32; ++w) m = max(m, red[w]);
+  float scale, sinv;
+  fp8_scale(m << 16, 8, scale, sinv);
+  if (threadIdx.x == 0) scale_inv[row] = sinv;
+  uint8_t* dst = out + row * ldo;
+#pragma unroll
+  for (int i = 0; i < NV; ++i) {
+    const int c = (threadIdx.x + R_THREADS * i) * 8;
+    if (c >= K) continue;
+    float f[8];
+    unpack8(v[i], f);
+    const uint2 q = cvt_e4m3x8(f, scale);
+    if (c + 8 <= K) {
+      *reinterpret_cast<uint2*>(dst + c) = q;
+    } else {
+#pragma unroll
+      for (int k = 0; k < 8; ++k)
+        if (c + k < K) dst[c + k] = static_cast<uint8_t>((k < 4 ? q.x : q.y) >> (8 * (k & 3)));
+    }
+  }
+}
+
+template <int NV>
+static cudaError_t launch_fp8_rows(const __nv_bfloat16* x, long ldx, int M, int K, uint8_t* out, long ldo,
+                                   float* scale_inv, cudaStream_t stream) {
+  return launch_pdl(fp8_rows_kernel<NV>, dim3(M), dim3(R_THREADS), 0, stream, x, ldx, K, out, ldo, scale_inv);
+}
+
 }  // namespace ivb
 
 using namespace ivb;
+
+extern "C" int ivb_fp8_quantize_rows(const void* x, long ldx, int M, int K, void* out, long ldo, float* row_scale_inv,
+                                     void* stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  if (M <= 0 || K <= 0) return set_error("ivb_fp8_quantize_rows: empty tensor");
+  if (K > IVB_FP8_ROWS_MAX_K) return set_error("ivb_fp8_quantize_rows: K > IVB_FP8_ROWS_MAX_K");
+  if (x == nullptr || out == nullptr || row_scale_inv == nullptr)
+    return set_error("ivb_fp8_quantize_rows: x, out or row_scale_inv is null");
+  if ((ldx & 7) || ldx < K) return set_error("ivb_fp8_quantize_rows: ldx must be a multiple of 8 elements and >= K");
+  if ((ldo & 15) || ldo < K) return set_error("ivb_fp8_quantize_rows: ldo must be a multiple of 16 elements and >= K");
+  if ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(out)) & 15)
+    return set_error("ivb_fp8_quantize_rows: x and out must be 16-byte aligned");
+  if (reinterpret_cast<uintptr_t>(row_scale_inv) & 3)
+    return set_error("ivb_fp8_quantize_rows: row_scale_inv must be 4-byte aligned");
+  const auto* xb = reinterpret_cast<const __nv_bfloat16*>(x);
+  auto* o = reinterpret_cast<uint8_t*>(out);
+  const int chunks = (K + 7) / 8;   // per row; each thread holds NV of them
+  cudaError_t e;
+  if (chunks <= R_THREADS * 2) e = launch_fp8_rows<2>(xb, ldx, M, K, o, ldo, row_scale_inv, stream);
+  else if (chunks <= R_THREADS * 4) e = launch_fp8_rows<4>(xb, ldx, M, K, o, ldo, row_scale_inv, stream);
+  else if (chunks <= R_THREADS * 8) e = launch_fp8_rows<8>(xb, ldx, M, K, o, ldo, row_scale_inv, stream);
+  else e = launch_fp8_rows<16>(xb, ldx, M, K, o, ldo, row_scale_inv, stream);
+  if (e != cudaSuccess) return set_error_cuda("launch(fp8_rows_kernel)", e);
+  count_launch();
+  return check_launch("fp8_rows_kernel");
+}
 
 extern "C" int ivb_fp8_quantize(const void* x, long ldx, int M, int K, int format, void* out, long ldo, void* out_t,
                                 long ldt, float* amax, float* scale_inv, void* stream_) {

@@ -26,6 +26,8 @@
 // Accumulation: the tensor core's fp8 MMA keeps fewer mantissa bits in its running sum than fp32 (about 14, DeepSeek-V3
 // technical report 3.3.2).  The ping-pong kernel accumulates in the tensor core; the FP8 cooperative kernel promotes:
 // each 128-element k-block goes into a fresh register tile, which the CUDA cores add to the fp32 accumulator.
+// Vector scales (IVB_FLAG_FP8_VECTOR_SCALES, Op = OpVecFp8): a_scale_inv[M] per row and b_scale_inv[N] per column;
+// the same in-place dequantisation multiplies each accumulator by its row's and its column's factor.
 //
 // Ping-pong form (gemm_bf16_pingpong_kernel, the default for most shapes, see use_pingpong): same producer, ring and
 // epilogue, but each MMA warpgroup owns a whole 128 x 128 tile and the two alternate, so one runs its epilogue while
@@ -49,13 +51,18 @@ constexpr int EPI_PITCH = 36;               // floats per staged row: 32 columns
 constexpr int EPI_BYTES = 8 * 16 * EPI_PITCH * 4;  // one 16 x 32 fp32 staging tile per MMA warp
 
 // Operand formats: bf16 x bf16, or fp8 (A E4M3 or E5M2, B E4M3).  BK: elements in a 128-byte k-block.
+// VEC: per-row / per-column scale vectors instead of two scalars (E4M3 A only).
 struct OpBf16 {
-  static constexpr bool FP8 = false;
+  static constexpr bool FP8 = false, VEC = false;
   static constexpr int BK = 64;
 };
 template <bool A_E5M2_>
 struct OpFp8 {
-  static constexpr bool FP8 = true, A_E5M2 = A_E5M2_;
+  static constexpr bool FP8 = true, A_E5M2 = A_E5M2_, VEC = false;
+  static constexpr int BK = 128;
+};
+struct OpVecFp8 {
+  static constexpr bool FP8 = true, A_E5M2 = false, VEC = true;
   static constexpr int BK = 128;
 };
 
@@ -158,9 +165,33 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float (
 
 // fp8: dequantise the accumulators in place before the epilogue.  (Scaling them as the epilogue stages them lets the
 // compiler hoist every product out of the rolled chunk loop, which needs a second copy of acc and spills.)
+// Vector scales: acc[h][4j + 2q + e] is the accumulator of row row0 + 64h + 16 * (warp in the warpgroup) + lane / 4 +
+// 8q and column n0 + 8j + 2 * (lane % 4) + e (the wgmma fragment layout, as epilogue_stage reads it).  A thread
+// holds 2 NH rows, whose factors it loads once, and reads each column pair's factors as one 8-byte load.  Rows and
+// columns outside the matrix are never stored: they get factor 0 and no load.
 template <class Op, int BN, int NH>
-__device__ __forceinline__ void dequantise(float (&acc)[NH][BN / 2], float dq) {
-  if constexpr (Op::FP8) {
+__device__ __forceinline__ void dequantise(const GemmParams& p, float (&acc)[NH][BN / 2], float dq, long row0, int n0) {
+  if constexpr (Op::VEC) {
+    const int lane = threadIdx.x & 31;
+    const long r0 = row0 + ((threadIdx.x >> 5) & 3) * 16 + (lane >> 2);
+    float ra[NH][2];
+#pragma unroll
+    for (int h = 0; h < NH; ++h)
+#pragma unroll
+      for (int q = 0; q < 2; ++q) ra[h][q] = r0 + 64 * h + 8 * q < p.M ? p.a_scale_inv[r0 + 64 * h + 8 * q] : 0.0f;
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+      const int col = n0 + 8 * j + 2 * (lane & 3);
+      const float2 cb = col < p.N ? *reinterpret_cast<const float2*>(p.b_scale_inv + col) : make_float2(0.0f, 0.0f);
+#pragma unroll
+      for (int h = 0; h < NH; ++h)
+#pragma unroll
+        for (int q = 0; q < 2; ++q) {
+          acc[h][4 * j + 2 * q] *= ra[h][q] * cb.x;
+          acc[h][4 * j + 2 * q + 1] *= ra[h][q] * cb.y;
+        }
+    }
+  } else if constexpr (Op::FP8) {
 #pragma unroll
     for (int h = 0; h < NH; ++h)
 #pragma unroll
@@ -269,7 +300,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     };
     float* st = epi + (warp - 4) * 16 * EPI_PITCH;
     float dq = 1.0f;
-    if constexpr (Op::FP8) dq = *p.a_scale_inv * *p.b_scale_inv;
+    if constexpr (Op::FP8 && !Op::VEC) dq = *p.a_scale_inv * *p.b_scale_inv;
     float acc[1][BN / 2];
     float part[PROMOTE ? BN / 2 : 1];
     int stage = 0;
@@ -316,7 +347,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         wgmma_reg_fence(acc[0], BN / 2);
         release(prev);
       }
-      dequantise<Op, BN, 1>(acc, dq);
+      dequantise<Op, BN, 1>(p, acc, dq, m0 + cw * 64, n0);
       epilogue_tile<BN, 1>(p, acc, st, m0 + cw * 64, n0);
     }
   }
@@ -409,7 +440,7 @@ gemm_bf16_pingpong_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_
     const bool signal = (threadIdx.x & 127) == 0;
     float* st = epi + (warp - 4) * 16 * EPI_PITCH;
     float dq = 1.0f;
-    if constexpr (Op::FP8) dq = *p.a_scale_inv * *p.b_scale_inv;
+    if constexpr (Op::FP8 && !Op::VEC) dq = *p.a_scale_inv * *p.b_scale_inv;
     float acc[2][PP_BN / 2];            // rows [0, 64) and [64, 128) of the tile
     for (int j = cw, tile = blockIdx.x + cw * gridDim.x; tile < num_tiles; j += 2, tile += 2 * gridDim.x) {
       const int m0 = (tile / num_n) * BM;
@@ -449,7 +480,7 @@ gemm_bf16_pingpong_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_
       wgmma_reg_fence(acc[0], PP_BN / 2);
       wgmma_reg_fence(acc[1], PP_BN / 2);
       if (signal) mbar_arrive(&empty[prev]);
-      dequantise<Op, PP_BN, 2>(acc, dq);
+      dequantise<Op, PP_BN, 2>(p, acc, dq, m0, n0);
       epilogue_tile<PP_BN, 2>(p, acc, st, m0, n0);
     }
   }
@@ -685,6 +716,10 @@ extern "C" int ivb_gemm_fp8(const void* A, int a_mn_major, long lda, int a_forma
   if ((N & 7) || (ld0 & 7)) return set_error("ivb_gemm_fp8: N and ld0 must be multiples of 8 elements");
   if (a_format != IVB_FP8_E4M3 && a_format != IVB_FP8_E5M2) return set_error("ivb_gemm_fp8: unknown a_format");
   if (a_scale_inv == nullptr || b_scale_inv == nullptr) return set_error("ivb_gemm_fp8: scale_inv pointers are null");
+  const bool vec = (flags & IVB_FLAG_FP8_VECTOR_SCALES) != 0;
+  if (vec && a_format != IVB_FP8_E4M3) return set_error("ivb_gemm_fp8: vector scales need an E4M3 A operand");
+  if (vec && ((reinterpret_cast<uintptr_t>(a_scale_inv) | reinterpret_cast<uintptr_t>(b_scale_inv)) & 7))
+    return set_error("ivb_gemm_fp8: scale vectors must be 8-byte aligned");
   if (int rc = check_epilogue_args("ivb_gemm_fp8", epilogue, out0, out1, ld1, aux, ldaux, bias, gamma)) return rc;
   const bool force1 = (flags & IVB_FLAG_1CTA) != 0, forcepp = (flags & IVB_FLAG_PINGPONG) != 0;
   if (flags & IVB_FLAG_2CTA) return set_error("ivb_gemm_fp8: no CTA-pair kernel");
@@ -696,6 +731,7 @@ extern "C" int ivb_gemm_fp8(const void* A, int a_mn_major, long lda, int a_forma
   p.b_scale_inv = b_scale_inv;
   const bool pingpong = forcepp || (!force1 && tile_n != 192 && use_pingpong(M, N, K));
   const int bn = tile_n > 0 ? tile_n : choose_bn(M, N, 1, true);
+  if (vec) return dispatch_fp8<OpVecFp8>(pingpong, bn, A, lda, B, ldb, p, stream);
   if (a_format == IVB_FP8_E5M2) return dispatch_fp8<OpFp8<true>>(pingpong, bn, A, lda, B, ldb, p, stream);
   return dispatch_fp8<OpFp8<false>>(pingpong, bn, A, lda, B, ldb, p, stream);
 }

@@ -11,6 +11,7 @@
 #include <type_traits>
 
 #include "ivb_colred.cuh"
+#include "ivb_fp8.cuh"
 #include "ivb_internal.h"
 #include "ivb_ptx.cuh"
 #include "ivb_rows.cuh"
@@ -302,6 +303,77 @@ rms_fwd_reg_kernel(const void* __restrict__ x, long ldx, const __nv_bfloat16* __
       }
     }
     if (lane == 0 && rstd_out) rstd_out[row] = rstd;
+  }
+}
+
+// ------------------------------------------------------------------ norm -> E4M3 row (D <= 256*NCH)
+// The frozen towers' FP8 inference: the normalised row never exists in bf16.  One warp per row holds it in registers
+// (one HBM read), so the row's amax, and with it the row's power-of-two scale (fp8_scale), is known before the first
+// byte is stored.  The statistics and y = (x - mean) * rstd * w (+ b) are the fp32 expressions of norm_fwd_kernel
+// (LayerNorm) and rms_fwd_reg_kernel (RMSNorm), so y is the value ivb_norm_fwd rounds to bf16.
+template <bool XF32, bool LN, int NCH>
+__global__ void __launch_bounds__(256)
+norm_fwd_fp8_kernel(const void* __restrict__ x, long ldx, const __nv_bfloat16* __restrict__ w,
+                    const __nv_bfloat16* __restrict__ b, float eps, int M, int D, uint8_t* __restrict__ out, long ldo,
+                    float* __restrict__ scale_inv) {
+  pdl_wait();
+  pdl_launch_dependents();
+  const int lane = threadIdx.x & 31;
+  const int wpb = blockDim.x >> 5;
+  const int nch = D >> 3;
+  const float invD = 1.0f / static_cast<float>(D);
+  for (long row = (long)blockIdx.x * wpb + (threadIdx.x >> 5); row < M; row += (long)gridDim.x * wpb) {
+    float v[NCH][8];
+#pragma unroll
+    for (int i = 0; i < NCH; ++i)
+      if (lane + 32 * i < nch) load8<XF32>(x, row * ldx + (lane + 32 * i) * 8, v[i]);
+    float mean = 0.f;
+    if (LN) {
+      float s = 0.f;
+#pragma unroll
+      for (int i = 0; i < NCH; ++i)
+        if (lane + 32 * i < nch) {
+#pragma unroll
+          for (int j = 0; j < 8; ++j) s += v[i][j];
+        }
+      mean = warp_sum(s) * invD;
+    }
+    float ss = 0.f;
+#pragma unroll
+    for (int i = 0; i < NCH; ++i)
+      if (lane + 32 * i < nch) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) { const float d = v[i][j] - mean; ss += d * d; }
+      }
+    const float rstd = rsqrtf(warp_sum(ss) * invD + eps);
+    unsigned m = 0;   // fp32 magnitude bits: NaN > Inf > every finite value
+#pragma unroll
+    for (int i = 0; i < NCH; ++i) {
+      const int c = lane + 32 * i;
+      if (c < nch) {
+        float wv[8];
+        load8<false>(w, c * 8, wv);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) v[i][j] = (v[i][j] - mean) * rstd * wv[j];
+        if (LN && b != nullptr) {
+          float bv[8];
+          load8<false>(b, c * 8, bv);
+#pragma unroll
+          for (int j = 0; j < 8; ++j) v[i][j] += bv[j];
+        }
+#pragma unroll
+        for (int j = 0; j < 8; ++j) m = max(m, __float_as_uint(v[i][j]) & 0x7fffffffu);
+      }
+    }
+    m = __reduce_max_sync(0xffffffffu, m);
+    float scale, sinv;
+    fp8_scale(m, 8, scale, sinv);
+#pragma unroll
+    for (int i = 0; i < NCH; ++i) {
+      const int c = lane + 32 * i;
+      if (c < nch) *reinterpret_cast<uint2*>(out + row * ldo + c * 8) = cvt_e4m3x8(v[i], scale);
+    }
+    if (lane == 0) scale_inv[row] = sinv;
   }
 }
 
@@ -614,6 +686,41 @@ extern "C" int ivb_norm_fwd(const void* x, int x_is_f32, long ldx, const void* w
   });
   count_launch();
   return check_launch("norm_fwd_kernel");
+}
+
+extern "C" int ivb_norm_fwd_fp8(const void* x, int x_is_f32, long ldx, const void* weight, const void* bias, float eps,
+                                int is_layernorm, int M, int D, void* out, long ldo, float* row_scale_inv,
+                                void* stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  if (M <= 0) return set_error("ivb_norm_fwd_fp8: empty tensor");
+  if (D <= 0 || D > IVB_NORM_FP8_MAX_D || (D & 7))
+    return set_error("ivb_norm_fwd_fp8: D must be a multiple of 8 in [8, IVB_NORM_FP8_MAX_D]");
+  if ((ldx & 7) || ldx < D) return set_error("ivb_norm_fwd_fp8: ldx must be a multiple of 8 elements and >= D");
+  if ((ldo & 15) || ldo < D) return set_error("ivb_norm_fwd_fp8: ldo must be a multiple of 16 elements and >= D");
+  if (x == nullptr || weight == nullptr || out == nullptr || row_scale_inv == nullptr)
+    return set_error("ivb_norm_fwd_fp8: x, weight, out or row_scale_inv is null");
+  if ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(weight) | reinterpret_cast<uintptr_t>(bias) |
+       reinterpret_cast<uintptr_t>(out)) & 15)
+    return set_error("ivb_norm_fwd_fp8: x, weight, bias and out must be 16-byte aligned");
+  if (reinterpret_cast<uintptr_t>(row_scale_inv) & 3)
+    return set_error("ivb_norm_fwd_fp8: row_scale_inv must be 4-byte aligned");
+  const __nv_bfloat16* w = reinterpret_cast<const __nv_bfloat16*>(weight);
+  const __nv_bfloat16* b = reinterpret_cast<const __nv_bfloat16*>(bias);
+  uint8_t* o = reinterpret_cast<uint8_t*>(out);
+  const int blocks = persistent_grid(M, 8, 8);
+  const cudaError_t e = pick_bool(x_is_f32, [&](auto xf) {
+    return pick_bool(is_layernorm, [&](auto ln) {
+      auto go = [&](auto nch) {
+        return launch_pdl(norm_fwd_fp8_kernel<xf, ln, nch>, dim3(blocks), dim3(256), 0, stream, x, ldx, w, b, eps, M, D,
+                          o, ldo, row_scale_inv);
+      };
+      if (D > 1536) return go(std::integral_constant<int, 16>{});
+      return static_cast<cudaError_t>(pick_nch(D, [&](auto nch) { return static_cast<int>(go(nch)); }));
+    });
+  });
+  if (e != cudaSuccess) return set_error_cuda("launch(norm_fwd_fp8_kernel)", e);
+  count_launch();
+  return check_launch("norm_fwd_fp8_kernel");
 }
 
 extern "C" int ivb_norm_bwd(const void* dy, long lddy, const void* x, int x_is_f32, long ldx,

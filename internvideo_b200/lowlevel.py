@@ -11,6 +11,7 @@ from . import _lib
 
 EPI_BF16, EPI_F32, EPI_BIAS_GELU, EPI_RESID, EPI_GELU_BWD = 0, 1, 2, 3, 4
 FLAG_GELU_TANH, FLAG_ACCUM, FLAG_1CTA, FLAG_2CTA, FLAG_GELU_SAVE_GRAD, FLAG_PINGPONG = 1, 2, 4, 8, 16, 32
+FLAG_FP8_VECTOR_SCALES = 64
 
 bf16 = torch.bfloat16
 f32 = torch.float32
@@ -139,12 +140,51 @@ def fp8_quantize(x, fmt=FP8_E4M3, transpose=False):
     return q, q_t, scale_inv, amax
 
 
+def fp8_quantize_rows(x):
+    """Per-row current-scaling cast of a bf16 [M, K] tensor (any row pitch) to E4M3 (ivb_fp8_quantize_rows).
+
+    Returns (q [M, K], row_scale_inv fp32 [M]): x[m] ~ q[m] * row_scale_inv[m], each row with its own power-of-two
+    scale.  A weight [N, K] quantised this way has one scale per output channel.  q is a view of a buffer whose row
+    pitch is rounded up to 16 elements (the fp8 GEMM's operand rule)."""
+    _chk(x, bf16, "x")
+    ldx = _rows2d(x, "x")
+    M, K = x.shape
+    q = torch.empty((M, _pad16(K)), device=x.device, dtype=torch.float8_e4m3fn)[:, :K]
+    sinv = torch.empty((M,), device=x.device, dtype=f32)
+    ev0 = _prof_begin()
+    rc = _lib_().ivb_fp8_quantize_rows(_p(x), ldx, M, K, _p(q), q.stride(0), _p(sinv), _stream())
+    _lib.check(rc, "ivb_fp8_quantize_rows")
+    _prof_end(ev0, 0.0, "fp8_quantize")
+    return q, sinv
+
+
+def norm_fwd_fp8(x, weight, bias=None, eps=1e-6, layernorm=False):
+    """RMSNorm / LayerNorm of x [M, D] (fp32 or bf16, any row pitch) written only as E4M3 rows with per-row scales
+    (ivb_norm_fwd_fp8).  Returns (q [M, D] float8_e4m3fn, row_scale_inv fp32 [M]): q[m] * row_scale_inv[m] is the
+    row norm_fwd would round to bf16, rounded to E4M3 instead."""
+    if x.dtype not in (f32, bf16):
+        raise _lib.IvbError("norm_fwd_fp8: x must be fp32 or bf16")
+    _chk(x, x.dtype, "x"); _chk(weight, bf16, "weight"); _chk(bias, bf16, "bias")
+    ldx = _rows2d(x, "x")
+    M, D = x.shape
+    q = torch.empty((M, _pad16(D)), device=x.device, dtype=torch.float8_e4m3fn)[:, :D]
+    sinv = torch.empty((M,), device=x.device, dtype=f32)
+    ev0 = _prof_begin()
+    rc = _lib_().ivb_norm_fwd_fp8(_p(x), int(x.dtype == f32), ldx, _p(weight), _p(bias), float(eps), int(layernorm), M,
+                                  D, _p(q), q.stride(0), _p(sinv), _stream())
+    _lib.check(rc, "ivb_norm_fwd_fp8")
+    _prof_end(ev0, 0.0, "norm_fwd_fp8")
+    return q, sinv
+
+
 def gemm_fp8(a, a_scale_inv, b, b_scale_inv, *, epi=EPI_BF16, flags=0, out0=None, out1=None, bias=None, gamma=None,
              aux=None, rowscale=None, tile_n=0):
     """D[M,N] = epi(a_scale_inv * b_scale_inv * sum_k A(m,k) B(n,k)) on the FP8 tensor cores (ivb_gemm_fp8).
 
     a: [M,K] float8_e4m3fn or float8_e5m2; b: [N,K] float8_e4m3fn; both K-major (fp8_quantize's q, or q_t for a
-    transposed operand).  a_scale_inv / b_scale_inv: fp32 [1] CUDA tensors.  Epilogue arguments as for gemm()."""
+    transposed operand).  a_scale_inv / b_scale_inv: fp32 [1] CUDA tensors (per-tensor scales), or fp32 [M] and [N]
+    vectors (per-row scales of a, per-output-channel scales of b, as fp8_quantize_rows / norm_fwd_fp8 give them; a
+    must then be E4M3), which sets FLAG_FP8_VECTOR_SCALES.  Epilogue arguments as for gemm()."""
     if a.dtype not in FP8_DTYPES.values() or not a.is_cuda:
         raise _lib.IvbError(f"gemm_fp8: a must be a CUDA float8_e4m3fn / float8_e5m2 tensor, got {a.dtype}")
     _chk(b, torch.float8_e4m3fn, "b"); _chk(a_scale_inv, f32, "a_scale_inv"); _chk(b_scale_inv, f32, "b_scale_inv")
@@ -167,6 +207,12 @@ def gemm_fp8(a, a_scale_inv, b, b_scale_inv, *, epi=EPI_BF16, flags=0, out0=None
         _chk(aux, f32 if epi == EPI_RESID else bf16, "aux")
         ldaux = _rows2d(aux, "aux")
     fmt = FP8_E5M2 if a.dtype == torch.float8_e5m2 else FP8_E4M3
+    if a_scale_inv.numel() != 1 or b_scale_inv.numel() != 1:
+        if (a_scale_inv.shape != (M,) or b_scale_inv.shape != (N,) or not a_scale_inv.is_contiguous()
+                or not b_scale_inv.is_contiguous()):
+            raise _lib.IvbError(f"gemm_fp8: vector scales must be contiguous [M] = [{M}] and [N] = [{N}], got "
+                                f"{tuple(a_scale_inv.shape)} and {tuple(b_scale_inv.shape)}")
+        flags |= FLAG_FP8_VECTOR_SCALES
     ev0 = _prof_begin()
     rc = _lib_().ivb_gemm_fp8(_p(a), 0, lda, fmt, _p(a_scale_inv), _p(b), 0, ldb, _p(b_scale_inv), M, N, K, epi, flags,
                               _p(out0), ld0, _p(out1), ld1, _p(bias), _p(gamma), _p(aux), ldaux, _p(rowscale), tile_n,
@@ -181,7 +227,8 @@ _PROF = [None]
 
 class GemmProfiler:
     """CUDA-event timing of every tensor-core launch (GEMMs, bf16 and fp8, attention forward / backward) and of the
-    fp8 casts that feed the fp8 GEMMs (kind "fp8_quantize", no flops) on the launching stream (bench.py roofline).
+    fp8 casts that feed the fp8 GEMMs (kind "fp8_quantize", no flops) and the norms that write FP8 rows (kind
+    "norm_fwd_fp8", no flops) on the launching stream (bench.py roofline).
     Records (start, stop, algorithmic flops, kind)."""
 
     def __init__(self):
@@ -606,5 +653,6 @@ def _gemm_name(a, b, *, a_t=False, b_t=False, epi=EPI_BF16, **_):
 gemm = _timed(gemm, _gemm_name)
 for _n in ("norm_fwd", "norm_bwd", "layerscale_bwd", "colsum", "attn_fwd", "attn_bwd", "visible_indices",
            "im2col_visible", "gather_add", "scatter_add", "ln_l2_fwd", "ln_l2_bwd", "vtc_loss_fwd", "vtc_loss_bwd",
-           "l2norm_rows_fwd", "l2norm_rows_bwd", "pixel_targets", "mse_loss", "adamw_step", "fp8_quantize", "gemm_fp8"):
+           "l2norm_rows_fwd", "l2norm_rows_bwd", "pixel_targets", "mse_loss", "adamw_step", "fp8_quantize", "gemm_fp8",
+           "fp8_quantize_rows", "norm_fwd_fp8"):
     globals()[_n] = _timed(globals()[_n])

@@ -204,6 +204,8 @@ class Block(nn.Module):
         self.num_heads = num_heads
         # FP8 GEMMs for the forward and input-gradient passes (set_fp8); read at call time
         self.fp8 = False
+        # FP8 inference with per-channel weight copies (set_fp8_inference); None when off
+        self.fp8_inference = None
 
     def forward_stream(self, x2d, B, n, rowscale=None):
         """fp32 residual stream [B*n, D] -> [B*n, D] (the hot path used by the model).
@@ -221,6 +223,8 @@ class Block(nn.Module):
             rs2 = s2.repeat_interleave(n) if s2 is not None else None
         if not torch.is_grad_enabled():
             return self.forward_infer(x2d, B, n, (rs1, rs2))
+        if self.fp8_inference is not None:
+            raise ll._lib.IvbError("Block: FP8 inference mode (set_fp8_inference) has no gradient; switch it off to train")
         return ops.BlockFn.apply(
             x2d, (B, n, self.num_heads, self.mlp.gelu_tanh, self.with_cp, self.fp8), self.norm1.weight, a.qkv.weight, a.qkv.bias,
             a.q_norm.weight if a.qk_normalization else None, a.k_norm.weight if a.qk_normalization else None,
@@ -240,8 +244,12 @@ class Block(nn.Module):
         """No-grad form (frozen towers / teachers): 14 kernels, nothing saved, no GELU' / pre-LayerScale copies."""
         with torch.no_grad():
             out, _ = ops.block_forward(x2d, (B, n, self.num_heads, self.mlp.gelu_tanh, False, self.fp8),
-                                       self._param_tuple(), rowscale[0], rowscale[1], save=False)
+                                       self._param_tuple(), rowscale[0], rowscale[1], save=False,
+                                       fp8_weights=fp8_inference_weights(self))
         return out
+
+    def _fp8_linears(self):
+        return (self.attn.qkv, self.attn.proj, self.mlp.fc1, self.mlp.fc2)
 
     def forward(self, x, residual=None):
         B, n, D = x.shape
@@ -267,6 +275,60 @@ def set_fp8(model: nn.Module, enabled: bool = True) -> int:
             mod.fp8 = bool(enabled)
             n += 1
     return n
+
+
+class Fp8InferenceWeights:
+    """The E4M3 copies of a block's four GEMM weights (qkv, proj, fc1, fc2) with one power-of-two scale per output
+    channel (lowlevel.fp8_quantize_rows), for FP8 inference.  get() re-quantises a weight whose storage or version
+    counter changed since its copy was made (a .to(), an in-place update, load_state_dict): a host-side check that
+    needs no device sync.  Not module state: nothing here is in the state_dict."""
+
+    def __init__(self, linears):
+        self.linears = linears
+        self.keys = [None] * len(linears)
+        self.copies = [None] * len(linears)
+
+    def get(self):
+        for i, lin in enumerate(self.linears):
+            w = lin.weight
+            key = (w.data_ptr(), w._version)
+            if key != self.keys[i]:
+                with torch.no_grad():
+                    self.copies[i] = ll.fp8_quantize_rows(w.detach())
+                self.keys[i] = key
+        return tuple(self.copies)
+
+
+def fp8_inference_weights(block):
+    """The FP8 weight copies a no-grad forward of `block` (Block or teachers.TeacherBlock) runs with, or None."""
+    if block.fp8_inference is None:
+        return None
+    if getattr(block, "fp8", False):
+        raise ll._lib.IvbError("FP8 inference (set_fp8_inference) and FP8 training (set_fp8) are both on for a block")
+    return block.fp8_inference.get()
+
+
+def set_fp8_inference(model: nn.Module, enabled: bool = True) -> int:
+    """Switch FP8 inference on or off for every ViT Block and VideoMAE TeacherBlock in `model` (frozen towers: the
+    InternVL and VideoMAE teachers, the frozen CLIP and stage-2 towers); returns how many blocks were switched.
+
+    In this mode a block's no-grad forward runs its four GEMMs (qkv, proj, fc1, fc2) on the FP8 tensor cores with
+    per-token activation scales, computed where each activation is produced (n1 and n2 inside the norm kernel, a and
+    g by a row-wise cast), and per-output-channel weight scales.  Switching on quantises each block's weights once;
+    they are re-quantised only when a weight changes.  Attention, the q/k norms and the fp32 residual stream stay
+    bf16 / fp32, and switching off restores the bf16 path bit for bit.  A switched Block refuses a forward that
+    needs a gradient, and the mode excludes set_fp8 on the same block."""
+    from .teachers import TeacherBlock
+    blocks = [m for m in model.modules() if isinstance(m, (Block, TeacherBlock))]
+    if enabled and any(getattr(m, "fp8", False) for m in blocks):
+        raise ll._lib.IvbError("set_fp8_inference: a block is in FP8 training mode (set_fp8); switch that off first")
+    for m in blocks:
+        if not enabled:
+            m.fp8_inference = None
+        elif m.fp8_inference is None:
+            m.fp8_inference = Fp8InferenceWeights(m._fp8_linears())
+            m.fp8_inference.get()
+    return len(blocks)
 
 
 class PatchEmbed(nn.Module):

@@ -211,7 +211,14 @@ def _fp8_dgrad(dy, wt8, ws, **epilogue):
     return ll.gemm_fp8(q, s, wt8, ws, **epilogue)
 
 
-def block_forward(x, dims, params, rs1=None, rs2=None, save=True):
+def _rowwise_linear(act, w8, **epilogue):
+    """FP8 inference GEMM with per-row activation and per-output-channel weight scales.  act: a bf16 activation (cast
+    row by row here) or the (E4M3 rows, scale_inv) pair norm_fwd_fp8 wrote; w8 = (E4M3 weight, scale_inv)."""
+    q, s = ll.fp8_quantize_rows(act) if torch.is_tensor(act) else act
+    return ll.gemm_fp8(q, s, w8[0], w8[1], **epilogue)
+
+
+def block_forward(x, dims, params, rs1=None, rs2=None, save=True, fp8_weights=None):
     """One spatio-temporal ViT block over the fp32 residual stream [B*n, D] (Block.forward,
     internvideo2_pretrain.py:279-297):
 
@@ -224,7 +231,12 @@ def block_forward(x, dims, params, rs1=None, rs2=None, save=True):
     extra is written.  Returns (x2, saved | None).
 
     FP8 mode (dims[5]): the four weights are cast to E4M3 (with save, also transposed, for the backward's dgrad) and
-    n1, a, n2 and g before their GEMM, each with its own per-tensor scale; the GEMMs keep their fused epilogues."""
+    n1, a, n2 and g before their GEMM, each with its own per-tensor scale; the GEMMs keep their fused epilogues.
+
+    FP8 inference (fp8_weights, save=False only): fp8_weights holds the E4M3 copies of the four weights with one scale
+    per output channel ((q, scale_inv) for qkv, proj, fc1, fc2; modules.set_fp8_inference).  n1 and n2 come out of
+    the norm kernel as E4M3 rows with per-row scales, a and g are cast row by row, and the four GEMMs apply row and
+    column scales before their fused epilogues.  Attention, the q/k norms and the residual stream stay as above."""
     B, n, H, gelu_tanh = dims[:4]
     n1w, qkvw, qkvb, qnw, knw, projw, projb, g1, n2w, fc1w, fc1b, fc2w, fc2b, g2 = params
     M, D = x.shape
@@ -232,15 +244,26 @@ def block_forward(x, dims, params, rs1=None, rs2=None, save=True):
     if x.dtype != f32 or not x.is_cuda:
         raise ll._lib.IvbError("block_forward: residual stream must be a CUDA fp32 tensor [B*n, D]")
     w8 = None
-    if _block_fp8(dims):
+    if fp8_weights is not None:
+        if save or _block_fp8(dims):
+            raise ll._lib.IvbError("block_forward: FP8 inference is a no-grad form and excludes the FP8 training mode")
+    elif _block_fp8(dims):
         # (q, q_t, scale_inv) per weight; q_t only when the backward will need it
         w8 = [ll.fp8_quantize(w, ll.FP8_E4M3, transpose=save)[:3] for w in (qkvw, projw, fc1w, fc2w)]
 
+    def norm(t, w):   # n1, n2 (and rstd for the backward)
+        if fp8_weights is not None:
+            return ll.norm_fwd_fp8(t, w), None
+        y, _, rstd = ll.norm_fwd(t, w, want_stats=save)
+        return y, rstd
+
     def linear(act, i, w, **epilogue):
+        if fp8_weights is not None:
+            return _rowwise_linear(act, fp8_weights[i], **epilogue)
         if w8 is None:
             return ll.gemm(act, w, **epilogue)
         return _fp8_linear(act, (w8[i][0], w8[i][2]), **epilogue)
-    n1, _, rstd1 = ll.norm_fwd(x, n1w, want_stats=save)
+    n1, rstd1 = norm(x, n1w)
     qkv = linear(n1, 0, qkvw, bias=qkvb)
     rq = rk = None
     if qnw is not None:
@@ -257,7 +280,7 @@ def block_forward(x, dims, params, rs1=None, rs2=None, save=True):
     a, lse = ll.attn_fwd(q, k, qkv[:, 2 * D:], B, n, H, d, d ** -0.5, want_lse=save)
     y1 = torch.empty((M, D), device=x.device, dtype=bf16) if (g1 is not None and save) else None
     x1 = linear(a, 1, projw, epi=ll.EPI_RESID, bias=projb, gamma=g1, aux=x, out1=y1, rowscale=rs1)
-    n2, _, rstd2 = ll.norm_fwd(x1, n2w, want_stats=save)
+    n2, rstd2 = norm(x1, n2w)
     Hd = fc1w.shape[0]
     flags = ll.FLAG_GELU_TANH if gelu_tanh else 0
     h = None
@@ -275,30 +298,43 @@ def block_forward(x, dims, params, rs1=None, rs2=None, save=True):
     return x2, (n1, qkv, qkn, a, lse, rstd1, rq, rk, x1, y1, n2, rstd2, h, g, y2) + wt8 + (flags,)
 
 
-def block_forward_ln_infer(x, B, n, H, scale, params, head_axis_attention=False):
+def block_forward_ln_infer(x, B, n, H, scale, params, head_axis_attention=False, fp8_weights=None):
     """Inference-only LayerNorm pre-norm block of the VideoMAEv2 teacher (videomae.py:104-132; attention with q/v
     bias :62-101, erf GELU, optional gamma_1/gamma_2) over the fp32 residual stream [B*n, D]: 9 kernels,
     LayerScale + residual fused in the GEMM epilogues, nothing saved.  params = (n1w, n1b, eps1, qkvw, qkvb, projw,
     projb, g1, n2w, n2b, eps2, fc1w, fc1b, fc2w, fc2b, g2).  head_axis_attention=True reproduces the reference's
-    flash_attn_func call on [B,H,N,d] tensors (softmax over the heads of each token); False is token-axis attention."""
+    flash_attn_func call on [B,H,N,d] tensors (softmax over the heads of each token); False is token-axis attention.
+    fp8_weights: FP8 inference as in block_forward (the two LayerNorms write E4M3 rows with per-row scales)."""
     n1w, n1b, eps1, qkvw, qkvb, projw, projb, g1, n2w, n2b, eps2, fc1w, fc1b, fc2w, fc2b, g2 = params
     M, D = x.shape
     d = D // H
     if x.dtype != f32 or not x.is_cuda:
         raise ll._lib.IvbError("block_forward_ln_infer: residual stream must be a CUDA fp32 tensor [B*n, D]")
+    if fp8_weights is not None:
+        def norm(t, w, b, eps):
+            return ll.norm_fwd_fp8(t, w, b, eps=eps, layernorm=True)
+
+        def linear(act, i, w, **epilogue):
+            return _rowwise_linear(act, fp8_weights[i], **epilogue)
+    else:
+        def norm(t, w, b, eps):
+            return ll.norm_fwd(t, w, b, eps=eps, layernorm=True, want_stats=False)[0]
+
+        def linear(act, i, w, **epilogue):
+            return ll.gemm(act, w, **epilogue)
     with torch.no_grad():
-        n1, _, _ = ll.norm_fwd(x, n1w, n1b, eps=eps1, layernorm=True, want_stats=False)
-        qkv = ll.gemm(n1, qkvw, bias=qkvb)
+        n1 = norm(x, n1w, n1b, eps1)
+        qkv = linear(n1, 0, qkvw, bias=qkvb)
         if head_axis_attention:
             # the reference's call (videomae.py:94-97) attends over the heads of each token and reinterprets the
             # [B, H, N, d] result as [B, N, H*d]: reproduced bit-for-layout
             a = ll.headaxis_attn_fwd(qkv, B, n, H, d, scale).reshape(M, D)
         else:
             a, _ = ll.attn_fwd(qkv[:, :D], qkv[:, D:2 * D], qkv[:, 2 * D:], B, n, H, d, scale, want_lse=False)
-        x1 = ll.gemm(a, projw, epi=ll.EPI_RESID, bias=projb, gamma=g1, aux=x)
-        n2, _, _ = ll.norm_fwd(x1, n2w, n2b, eps=eps2, layernorm=True, want_stats=False)
-        g = ll.gemm(n2, fc1w, epi=ll.EPI_BIAS_GELU, bias=fc1b)
-        return ll.gemm(g, fc2w, epi=ll.EPI_RESID, bias=fc2b, gamma=g2, aux=x1)
+        x1 = linear(a, 1, projw, epi=ll.EPI_RESID, bias=projb, gamma=g1, aux=x)
+        n2 = norm(x1, n2w, n2b, eps2)
+        g = linear(n2, 2, fc1w, epi=ll.EPI_BIAS_GELU, bias=fc1b)
+        return linear(g, 3, fc2w, epi=ll.EPI_RESID, bias=fc2b, gamma=g2, aux=x1)
 
 
 def block_backward(x, saved, dims, tensors, P, dx2, rs1, rs2):

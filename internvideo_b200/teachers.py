@@ -21,7 +21,8 @@ import torch.nn as nn
 
 from . import lowlevel as ll
 from . import ops
-from .modules import AttentionPoolingBlock, Block, LayerNormB, RMSNorm, bf16, f32, to_2tuple, trunc_normal_
+from .modules import (AttentionPoolingBlock, Block, LayerNormB, RMSNorm, bf16, f32, fp8_inference_weights, to_2tuple,
+                      trunc_normal_)
 
 
 # ------------------------------------------------------------------------------------------------ CLIP teacher
@@ -165,6 +166,10 @@ class TeacherBlock(nn.Module):
             self.gamma_2 = nn.Parameter(init_values * torch.ones(dim))
         else:
             self.gamma_1 = self.gamma_2 = None
+        self.fp8_inference = None   # modules.set_fp8_inference
+
+    def _fp8_linears(self):
+        return (self.attn.qkv, self.attn.proj, self.mlp.fc1, self.mlp.fc2)
 
     def forward_infer(self, x2d, B, n, head_axis_attention=True):
         """fp32 residual stream [B*n, D] -> same; 9 kernels, nothing saved."""
@@ -173,7 +178,8 @@ class TeacherBlock(nn.Module):
             x2d, B, n, a.num_heads, a.scale, head_axis_attention=head_axis_attention, params=
             (self.norm1.weight, self.norm1.bias, self.norm1.eps, a.qkv.weight, a.qkv_bias_vector(), a.proj.weight,
              a.proj.bias, self.gamma_1, self.norm2.weight, self.norm2.bias, self.norm2.eps, self.mlp.fc1.weight,
-             self.mlp.fc1.bias, self.mlp.fc2.weight, self.mlp.fc2.bias, self.gamma_2))
+             self.mlp.fc1.bias, self.mlp.fc2.weight, self.mlp.fc2.bias, self.gamma_2),
+            fp8_weights=fp8_inference_weights(self))
 
 
 class TubeletPatchEmbed(nn.Module):
