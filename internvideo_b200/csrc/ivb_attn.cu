@@ -240,11 +240,7 @@ static int launch_attn_fwd(const CUtensorMap& tq, const CUtensorMap& tk, const C
                            const AttnFwdParams& p, cudaStream_t stream) {
   constexpr int SMEM = KA * ATT_BQ * 128 + 2 * ATT_NS * KA * ATT_BKV * 128 + 128;  // tiles + barriers
   auto kern = attn_fwd_kernel<KA, NO, KS>;
-  static bool attr_set[64] = {};
-  if (first_use_on_device(attr_set)) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM);
-    if (e != cudaSuccess) return set_error_cuda("cudaFuncSetAttribute(attn_fwd)", e);
-  }
+  if (int rc = raise_smem_limit<attn_fwd_kernel<KA, NO, KS>>(SMEM, "cudaFuncSetAttribute(attn_fwd)")) return rc;
   dim3 grid((p.n + ATT_BQ - 1) / ATT_BQ, p.H, p.B);
   kern<<<grid, 384, SMEM, stream>>>(tq, tk, tv, p);
   count_launch();

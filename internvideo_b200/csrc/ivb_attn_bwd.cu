@@ -255,11 +255,7 @@ static int launch_attn_bwd(const CUtensorMap& tx, const CUtensorMap& ty, const C
   constexpr int SMEM = 2 * KA * BWD_ROWS * 128 + 2 * BWD_NST * KA * BWD_COLS * 128 + 2 * BWD_NST * BWD_COLS * 4 + 128;
   static_assert(SMEM <= 227 * 1024, "attention backward: shared-memory budget");
   auto kern = attn_bwd_kernel<MODE, KA, NO, KS>;
-  static bool attr_set[64] = {};
-  if (first_use_on_device(attr_set)) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM);
-    if (e != cudaSuccess) return set_error_cuda("cudaFuncSetAttribute(attn_bwd)", e);
-  }
+  if (int rc = raise_smem_limit<attn_bwd_kernel<MODE, KA, NO, KS>>(SMEM, "cudaFuncSetAttribute(attn_bwd)")) return rc;
   dim3 grid((p.n + BWD_ROWS - 1) / BWD_ROWS, p.H, p.B);
   cudaError_t le = launch_pdl(kern, grid, dim3(384), SMEM, stream, tx, ty, tu, tw, p);
   if (le != cudaSuccess) return set_error_cuda("launch(attn_bwd_kernel)", le);

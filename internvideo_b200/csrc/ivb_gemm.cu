@@ -37,6 +37,11 @@
 // a 256 x BN tile.  Each CTA loads its own 128 A rows and HALF of the B tile, which TMA multicasts into both CTAs'
 // rings, so B is read from L2 once per 256 rows instead of once per 128.  A stage is refilled only when the MMA
 // warpgroups of BOTH CTAs released it (each arrives on its own and on the peer's empty barrier).
+//
+// Both kernels are built from the same pieces (gemm_prologue, produce, mma_kblock, dequantise, epilogue_tile) and keep
+// only how their MMA warpgroups consume and release the ring: FP8 promotion and the CTA pair's remote arrivals in the
+// cooperative kernel, the token in the ping-pong kernel.  Both C entry points share choose_kernel, dispatch and
+// launch_gemm.
 #include <cstdio>
 
 #include "ivb_gemm_common.cuh"
@@ -65,14 +70,6 @@ struct OpVecFp8 {
   static constexpr bool FP8 = true, A_E5M2 = false, VEC = true;
   static constexpr int BK = 128;
 };
-
-template <class Op, int N, bool A_MN, bool B_MN>
-__device__ __forceinline__ void mma(float* d, uint64_t da, uint64_t db, uint32_t scale_d) {
-  if constexpr (Op::FP8)
-    WgmmaF8<N>::template ss<Op::A_E5M2>(d, da, db, scale_d);
-  else
-    Wgmma<N>::template ss<A_MN ? 1 : 0, B_MN ? 1 : 0>(d, da, db, scale_d);
-}
 
 template <int BN, bool B_MN>
 struct GemmCfg {
@@ -199,6 +196,124 @@ __device__ __forceinline__ void dequantise(const GemmParams& p, float (&acc)[NH]
   }
 }
 
+// ------------------------------------------------------------------ pieces of both kernels
+// Shared memory, aligned to 1024 bytes for the 128-byte swizzle: the ring (STAGES A stages, then STAGES B stages), one
+// 16 x 32 fp32 staging tile per MMA warp, then each stage's full and empty barrier.
+struct Smem {
+  uint8_t* a;
+  uint8_t* b;
+  float* epi;
+  uint64_t* full;
+  uint64_t* empty;
+};
+
+// Carves up shared memory, initialises the barriers and waits for the previous kernel (PDL).  `empty_arrivals`: the
+// releases a stage waits for before the producer refills it.
+template <int BN, bool B_MN, int CL>
+__device__ __forceinline__ Smem gemm_prologue(const CUtensorMap& tmA, const CUtensorMap& tmB, uint32_t empty_arrivals) {
+  using Cfg = GemmCfg<BN, B_MN>;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
+                                             ~static_cast<uintptr_t>(1023));
+  Smem s;
+  s.a = smem;
+  s.b = smem + Cfg::STAGES * A_STAGE_BYTES;
+  s.epi = reinterpret_cast<float*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES);
+  s.full = reinterpret_cast<uint64_t*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES + EPI_BYTES);
+  s.empty = s.full + Cfg::STAGES;
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmA);
+    tma_prefetch_desc(&tmB);
+    for (int i = 0; i < Cfg::STAGES; ++i) {
+      mbar_init(&s.full[i], 1);
+      mbar_init(&s.empty[i], empty_arrivals);
+    }
+    fence_mbar_init();
+  }
+  __syncthreads();
+  if (CL == 2) cluster_sync_all();   // the peer's barriers exist before any multicast or remote arrive reaches them
+  pdl_wait();
+  pdl_launch_dependents();
+  return s;
+}
+
+// The TMA producer (one elected thread): every k-block of the tiles first_tile, first_tile + stride, ... in that order.
+// CL = 2: the cluster's tile has 256 rows; this CTA (rank) loads its own 128 A rows and half of the B tile, which TMA
+// multicasts into both CTAs' rings.
+template <class Op, int BN, bool A_MN, bool B_MN, int CL>
+__device__ __forceinline__ void produce(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p,
+                                        const Smem& s, int first_tile, int stride, uint32_t rank) {
+  using Cfg = GemmCfg<BN, B_MN>;
+  const int num_n = (p.N + BN - 1) / BN;
+  const int num_tiles = ((p.M + CL * BM - 1) / (CL * BM)) * num_n;
+  const int num_kb = (p.K + Op::BK - 1) / Op::BK;
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int tile = first_tile; tile < num_tiles; tile += stride) {
+    const int m0 = (tile / num_n) * (CL * BM) + rank * BM;
+    const int n0 = (tile % num_n) * BN;
+    for (int kb = 0; kb < num_kb; ++kb) {
+      mbar_wait(&s.empty[stage], phase ^ 1);
+      mbar_expect_tx(&s.full[stage], Cfg::STAGE_BYTES);
+      uint8_t* sa = s.a + stage * A_STAGE_BYTES;
+      uint8_t* sb = s.b + stage * Cfg::B_STAGE_BYTES;
+      const int k0 = kb * Op::BK;
+      if (!A_MN) {
+        tma_load_2d(sa, &tmA, k0, m0, &s.full[stage]);
+      } else {
+#pragma unroll
+        for (int i = 0; i < BM / 64; ++i)
+          tma_load_2d(sa + i * 8192, &tmA, m0 + i * 64, k0, &s.full[stage]);
+      }
+      if (CL == 1) {
+        if (!B_MN) {
+          tma_load_2d(sb, &tmB, k0, n0, &s.full[stage]);
+        } else {
+#pragma unroll
+          for (int i = 0; i < Cfg::B_ATOMS; ++i)
+            tma_load_2d(sb + i * 8192, &tmB, n0 + i * 64, k0, &s.full[stage]);
+        }
+      } else {  // this CTA's half of B, into both CTAs (K-major: BN/2 rows; MN-major: every other 64-wide atom)
+        if (!B_MN) {
+          tma_load_2d_mc(sb + rank * (BN / 2) * 128, &tmB, k0, n0 + rank * (BN / 2), &s.full[stage], 0x3);
+        } else {
+#pragma unroll
+          for (int i = 0; i < Cfg::B_ATOMS; ++i)
+            if ((i & 1) == static_cast<int>(rank))
+              tma_load_2d_mc(sb + i * 8192, &tmB, n0 + i * 64, k0, &s.full[stage], 0x3);
+        }
+      }
+      if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
+    }
+  }
+}
+
+// Issues and commits one k-block's wgmmas from ring stage `stage`: K_MMAS steps 32 B apart along the k-block, each with
+// one wgmma per 64-row band h0, h0 + 1, ..., h0 + NH - 1 of the A stage into d[0 .. NH-1].  accumulate = false: the
+// first step overwrites d.
+template <class Op, int BN, bool A_MN, bool B_MN, int NH>
+__device__ __forceinline__ void mma_kblock(float (&d)[NH][BN / 2], const Smem& s, int stage, int h0, bool accumulate) {
+  using Cfg = GemmCfg<BN, B_MN>;
+  const uint32_t sa = smem_u32(s.a + stage * A_STAGE_BYTES);
+  const uint32_t sb = smem_u32(s.b + stage * Cfg::B_STAGE_BYTES);
+  wgmma_fence();
+#pragma unroll
+  for (int k = 0; k < K_MMAS; ++k) {
+    const uint64_t bd = B_MN ? gmma_desc(sb + k * 2048, 8192, 1024) : gmma_desc(sb + k * 32, 16, 1024);
+#pragma unroll
+    for (int h = 0; h < NH; ++h) {
+      const uint64_t ad = A_MN ? gmma_desc(sa + (h0 + h) * 8192 + k * 2048, 8192, 1024)
+                               : gmma_desc(sa + (h0 + h) * 8192 + k * 32, 16, 1024);
+      const uint32_t scale_d = (accumulate || k > 0) ? 1u : 0u;
+      if constexpr (Op::FP8)
+        WgmmaF8<BN>::template ss<Op::A_E5M2>(d[h], ad, bd, scale_d);
+      else
+        Wgmma<BN>::template ss<A_MN ? 1 : 0, B_MN ? 1 : 0>(d[h], ad, bd, scale_d);
+    }
+  }
+  wgmma_commit();
+}
+
 // ------------------------------------------------------------------ the cooperative kernel
 // Op: operand format.  The FP8 form promotes (see the top of the file): each k-block's four wgmmas accumulate into
 // `part`, which is added to acc once they retire; BN <= 192 keeps both tiles in the 232 registers of a thread.
@@ -206,18 +321,7 @@ template <class Op, int BN, bool A_MN, bool B_MN, int CL>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                  const GemmParams p) {
-  using Cfg = GemmCfg<BN, B_MN>;
-  constexpr int STAGES = Cfg::STAGES;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
-                                             ~static_cast<uintptr_t>(1023));
-  uint8_t* smem_a = smem;
-  uint8_t* smem_b = smem + STAGES * A_STAGE_BYTES;
-  float* epi = reinterpret_cast<float*>(smem + STAGES * Cfg::STAGE_BYTES);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES + EPI_BYTES);
-  uint64_t* full = bars;
-  uint64_t* empty = bars + STAGES;
-
+  constexpr int STAGES = GemmCfg<BN, B_MN>::STAGES;
   const int warp = threadIdx.x >> 5;
   const int wg = threadIdx.x >> 7;
 
@@ -226,68 +330,14 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   const int num_m = (p.M + CL * BM - 1) / (CL * BM);
   const int num_n = (p.N + BN - 1) / BN;
   const int num_tiles = num_m * num_n;
-  constexpr int BK = Op::BK;
   constexpr bool PROMOTE = Op::FP8;
-  const int num_kb = (p.K + BK - 1) / BK;
+  const int num_kb = (p.K + Op::BK - 1) / Op::BK;
 
-  if (threadIdx.x == 0) {
-    tma_prefetch_desc(&tmA);
-    tma_prefetch_desc(&tmB);
-    for (int i = 0; i < STAGES; ++i) {
-      mbar_init(&full[i], 1);
-      mbar_init(&empty[i], 2 * CL);  // one arrival per MMA warpgroup of the cluster
-    }
-    fence_mbar_init();
-  }
-  __syncthreads();
-  if (CL == 2) cluster_sync_all();   // the peer's barriers exist before any multicast or remote arrive reaches them
-  pdl_wait();
-  pdl_launch_dependents();
+  const Smem s = gemm_prologue<BN, B_MN, CL>(tmA, tmB, 2 * CL);   // one arrival per MMA warpgroup of the cluster
 
   if (wg == 0) {
     setmaxnreg_dec<40>();
-    if (warp == 0 && elect_one()) {
-      // ===================== TMA producer =====================
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int tile = cid; tile < num_tiles; tile += ncl) {
-        const int m0 = (tile / num_n) * (CL * BM) + rank * BM;
-        const int n0 = (tile % num_n) * BN;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&empty[stage], phase ^ 1);
-          mbar_expect_tx(&full[stage], Cfg::STAGE_BYTES);
-          uint8_t* sa = smem_a + stage * A_STAGE_BYTES;
-          uint8_t* sb = smem_b + stage * Cfg::B_STAGE_BYTES;
-          const int k0 = kb * BK;
-          if (!A_MN) {
-            tma_load_2d(sa, &tmA, k0, m0, &full[stage]);
-          } else {
-#pragma unroll
-            for (int i = 0; i < BM / 64; ++i)
-              tma_load_2d(sa + i * 8192, &tmA, m0 + i * 64, k0, &full[stage]);
-          }
-          if (CL == 1) {
-            if (!B_MN) {
-              tma_load_2d(sb, &tmB, k0, n0, &full[stage]);
-            } else {
-#pragma unroll
-              for (int i = 0; i < Cfg::B_ATOMS; ++i)
-                tma_load_2d(sb + i * 8192, &tmB, n0 + i * 64, k0, &full[stage]);
-            }
-          } else {  // this CTA's half of B, into both CTAs (K-major: BN/2 rows; MN-major: every other 64-wide atom)
-            if (!B_MN) {
-              tma_load_2d_mc(sb + rank * (BN / 2) * 128, &tmB, k0, n0 + rank * (BN / 2), &full[stage], 0x3);
-            } else {
-#pragma unroll
-              for (int i = 0; i < Cfg::B_ATOMS; ++i)
-                if ((i & 1) == static_cast<int>(rank))
-                  tma_load_2d_mc(sb + i * 8192, &tmB, n0 + i * 64, k0, &full[stage], 0x3);
-            }
-          }
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
+    if (warp == 0 && elect_one()) produce<Op, BN, A_MN, B_MN, CL>(tmA, tmB, p, s, cid, ncl, rank);
   } else {
     setmaxnreg_inc<232>();
     // ===================== MMA + epilogue warpgroups =====================
@@ -295,14 +345,14 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     const bool signal = (threadIdx.x & 127) == 0;
     auto release = [&](int s_) {   // this warpgroup no longer reads stage s_ (of either CTA's ring)
       if (!signal) return;
-      mbar_arrive(&empty[s_]);
-      if (CL == 2) mbar_arrive_cluster(mapa_u32(smem_u32(&empty[s_]), rank ^ 1));
+      mbar_arrive(&s.empty[s_]);
+      if (CL == 2) mbar_arrive_cluster(mapa_u32(smem_u32(&s.empty[s_]), rank ^ 1));
     };
-    float* st = epi + (warp - 4) * 16 * EPI_PITCH;
+    float* st = s.epi + (warp - 4) * 16 * EPI_PITCH;
     float dq = 1.0f;
     if constexpr (Op::FP8 && !Op::VEC) dq = *p.a_scale_inv * *p.b_scale_inv;
     float acc[1][BN / 2];
-    float part[PROMOTE ? BN / 2 : 1];
+    float part[1][PROMOTE ? BN / 2 : 1];
     int stage = 0;
     uint32_t phase = 0;
     for (int tile = cid; tile < num_tiles; tile += ncl) {
@@ -314,30 +364,20 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         for (int i = 0; i < BN / 2; ++i) acc[0][i] = 0.0f;
       }
       for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(&full[stage], phase);
-        const uint32_t sa = smem_u32(smem_a + stage * A_STAGE_BYTES);
-        const uint32_t sb = smem_u32(smem_b + stage * Cfg::B_STAGE_BYTES);
-        wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < K_MMAS; ++k) {
-          const uint64_t ad = A_MN ? gmma_desc(sa + cw * 8192 + k * 2048, 8192, 1024)
-                                   : gmma_desc(sa + cw * 8192 + k * 32, 16, 1024);
-          const uint64_t bd = B_MN ? gmma_desc(sb + k * 2048, 8192, 1024) : gmma_desc(sb + k * 32, 16, 1024);
-          if constexpr (PROMOTE)
-            mma<Op, BN, A_MN, B_MN>(part, ad, bd, k > 0 ? 1u : 0u);
-          else
-            mma<Op, BN, A_MN, B_MN>(acc[0], ad, bd, (kb > 0 || k > 0) ? 1u : 0u);
-        }
-        wgmma_commit();
+        mbar_wait(&s.full[stage], phase);
         if constexpr (PROMOTE) {  // this k-block's partial sum, added in fp32; its smem slot is free
+          mma_kblock<Op, BN, A_MN, B_MN, 1>(part, s, stage, cw, false);
           wgmma_wait<0>();
-          wgmma_reg_fence(part, BN / 2);
+          wgmma_reg_fence(part[0], BN / 2);
           release(stage);
 #pragma unroll
-          for (int i = 0; i < BN / 2; ++i) acc[0][i] += part[i];
-        } else if (kb > 0) {  // the MMAs of the previous k-block retired: its smem slot is free
-          wgmma_wait<1>();
-          release(prev);
+          for (int i = 0; i < BN / 2; ++i) acc[0][i] += part[0][i];
+        } else {
+          mma_kblock<Op, BN, A_MN, B_MN, 1>(acc, s, stage, cw, kb > 0);
+          if (kb > 0) {  // the MMAs of the previous k-block retired: its smem slot is free
+            wgmma_wait<1>();
+            release(prev);
+          }
         }
         prev = stage;
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
@@ -368,77 +408,24 @@ template <class Op, bool A_MN, bool B_MN>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_bf16_pingpong_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                           const GemmParams p) {
-  using Cfg = GemmCfg<PP_BN, B_MN>;
-  constexpr int STAGES = Cfg::STAGES;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
-                                             ~static_cast<uintptr_t>(1023));
-  uint8_t* smem_a = smem;
-  uint8_t* smem_b = smem + STAGES * A_STAGE_BYTES;
-  float* epi = reinterpret_cast<float*>(smem + STAGES * Cfg::STAGE_BYTES);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES + EPI_BYTES);
-  uint64_t* full = bars;
-  uint64_t* empty = bars + STAGES;
-
+  constexpr int STAGES = GemmCfg<PP_BN, B_MN>::STAGES;
   const int warp = threadIdx.x >> 5;
   const int wg = threadIdx.x >> 7;
   const int num_n = (p.N + PP_BN - 1) / PP_BN;
   const int num_tiles = ((p.M + BM - 1) / BM) * num_n;
-  constexpr int BK = Op::BK;
-  const int num_kb = (p.K + BK - 1) / BK;
+  const int num_kb = (p.K + Op::BK - 1) / Op::BK;
 
-  if (threadIdx.x == 0) {
-    tma_prefetch_desc(&tmA);
-    tma_prefetch_desc(&tmB);
-    for (int i = 0; i < STAGES; ++i) {
-      mbar_init(&full[i], 1);
-      mbar_init(&empty[i], 1);  // each stage is read by exactly one MMA warpgroup
-    }
-    fence_mbar_init();
-  }
-  __syncthreads();
-  pdl_wait();
-  pdl_launch_dependents();
+  const Smem s = gemm_prologue<PP_BN, B_MN, 1>(tmA, tmB, 1);   // each stage is read by exactly one MMA warpgroup
 
   if (wg == 0) {
     setmaxnreg_dec<40>();
-    if (warp == 0 && elect_one()) {
-      // ===================== TMA producer: every k-block of every tile of this CTA, in tile order =====================
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        const int m0 = (tile / num_n) * BM;
-        const int n0 = (tile % num_n) * PP_BN;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&empty[stage], phase ^ 1);
-          mbar_expect_tx(&full[stage], Cfg::STAGE_BYTES);
-          uint8_t* sa = smem_a + stage * A_STAGE_BYTES;
-          uint8_t* sb = smem_b + stage * Cfg::B_STAGE_BYTES;
-          const int k0 = kb * BK;
-          if (!A_MN) {
-            tma_load_2d(sa, &tmA, k0, m0, &full[stage]);
-          } else {
-#pragma unroll
-            for (int i = 0; i < BM / 64; ++i)
-              tma_load_2d(sa + i * 8192, &tmA, m0 + i * 64, k0, &full[stage]);
-          }
-          if (!B_MN) {
-            tma_load_2d(sb, &tmB, k0, n0, &full[stage]);
-          } else {
-#pragma unroll
-            for (int i = 0; i < Cfg::B_ATOMS; ++i)
-              tma_load_2d(sb + i * 8192, &tmB, n0 + i * 64, k0, &full[stage]);
-          }
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
+    if (warp == 0 && elect_one()) produce<Op, PP_BN, A_MN, B_MN, 1>(tmA, tmB, p, s, blockIdx.x, gridDim.x, 0);
   } else {
     setmaxnreg_inc<232>();
     // ===================== MMA + epilogue warpgroups, one whole tile each =====================
     const int cw = wg - 1;              // this warpgroup takes the CTA's tiles j with (j & 1) == cw
     const bool signal = (threadIdx.x & 127) == 0;
-    float* st = epi + (warp - 4) * 16 * EPI_PITCH;
+    float* st = s.epi + (warp - 4) * 16 * EPI_PITCH;
     float dq = 1.0f;
     if constexpr (Op::FP8 && !Op::VEC) dq = *p.a_scale_inv * *p.b_scale_inv;
     float acc[2][PP_BN / 2];            // rows [0, 64) and [64, 128) of the tile
@@ -452,24 +439,11 @@ gemm_bf16_pingpong_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_
       if (j > 0) named_bar_sync(1 + cw, 256);
       int prev = 0;
       for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(&full[stage], phase);
-        const uint32_t sa = smem_u32(smem_a + stage * A_STAGE_BYTES);
-        const uint32_t sb = smem_u32(smem_b + stage * Cfg::B_STAGE_BYTES);
-        wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < K_MMAS; ++k) {
-          const uint64_t bd = B_MN ? gmma_desc(sb + k * 2048, 8192, 1024) : gmma_desc(sb + k * 32, 16, 1024);
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const uint64_t ad = A_MN ? gmma_desc(sa + h * 8192 + k * 2048, 8192, 1024)
-                                     : gmma_desc(sa + h * 8192 + k * 32, 16, 1024);
-            mma<Op, PP_BN, A_MN, B_MN>(acc[h], ad, bd, (kb > 0 || k > 0) ? 1u : 0u);
-          }
-        }
-        wgmma_commit();
+        mbar_wait(&s.full[stage], phase);
+        mma_kblock<Op, PP_BN, A_MN, B_MN, 2>(acc, s, stage, 0, kb > 0);
         if (kb > 0) {  // the MMAs of the previous k-block retired: its smem slot is free
           wgmma_wait<1>();
-          if (signal) mbar_arrive(&empty[prev]);
+          if (signal) mbar_arrive(&s.empty[prev]);
         }
         prev = stage;
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
@@ -479,7 +453,7 @@ gemm_bf16_pingpong_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_
       wgmma_wait<0>();
       wgmma_reg_fence(acc[0], PP_BN / 2);
       wgmma_reg_fence(acc[1], PP_BN / 2);
-      if (signal) mbar_arrive(&empty[prev]);
+      if (signal) mbar_arrive(&s.empty[prev]);
       dequantise<Op, PP_BN, 2>(p, acc, dq, m0, n0);
       epilogue_tile<PP_BN, 2>(p, acc, st, m0, n0);
     }
@@ -487,7 +461,14 @@ gemm_bf16_pingpong_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_
 }
 
 // ------------------------------------------------------------------ host side
-template <class Op, int BN, bool A_MN, bool B_MN, int CL>
+template <class Op, bool PINGPONG, int BN, bool A_MN, bool B_MN, int CL>
+constexpr auto gemm_kernel() {
+  if constexpr (PINGPONG) return gemm_bf16_pingpong_kernel<Op, A_MN, B_MN>;
+  else return gemm_bf16_kernel<Op, BN, A_MN, B_MN, CL>;
+}
+
+// Launches either kernel form (PINGPONG: BN = PP_BN, CL = 1) on at most one CTA per SM and one cluster per tile.
+template <class Op, bool PINGPONG, int BN, bool A_MN, bool B_MN, int CL>
 static int launch_gemm(const void* A, long lda, const void* B, long ldb, const GemmParams& p,
                        cudaStream_t stream) {
   using Cfg = GemmCfg<BN, B_MN>;
@@ -500,13 +481,8 @@ static int launch_gemm(const void* A, long lda, const void* B, long ldb, const G
   if (!B_MN) rc = make_tmap_2d(&tmB, B, (uint64_t)p.K, (uint64_t)p.N, ldb, Op::BK, BN / CL, EB);
   else       rc = make_tmap_2d(&tmB, B, (uint64_t)p.N, (uint64_t)p.K, ldb, 64, 64);
   if (rc) return rc;
-  auto kern = gemm_bf16_kernel<Op, BN, A_MN, B_MN, CL>;
-  static bool attr_set[64] = {};
-  if (first_use_on_device(attr_set)) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         Cfg::SMEM_BYTES);
-    if (e != cudaSuccess) return set_error_cuda("cudaFuncSetAttribute(gemm)", e);
-  }
+  constexpr auto kern = gemm_kernel<Op, PINGPONG, BN, A_MN, B_MN, CL>();
+  if ((rc = raise_smem_limit<kern>(Cfg::SMEM_BYTES, "cudaFuncSetAttribute(gemm)"))) return rc;
   const int num_tiles = ((p.M + CL * BM - 1) / (CL * BM)) * ((p.N + BN - 1) / BN);
   int clusters = num_sms() / CL;
   if (clusters > num_tiles) clusters = num_tiles;
@@ -528,63 +504,10 @@ static int launch_gemm(const void* A, long lda, const void* B, long ldb, const G
     cfg.numAttrs = pdl_enabled() ? 2 : 1;
     le = cudaLaunchKernelEx(&cfg, kern, tmA, tmB, p);
   }
-  if (le != cudaSuccess) return set_error_cuda("launch(gemm_bf16_kernel)", le);
+  const char* name = PINGPONG ? "gemm_bf16_pingpong_kernel" : "gemm_bf16_kernel";
+  if (le != cudaSuccess) return set_error_cuda(name, le);
   count_launch();
-  return check_launch("gemm_bf16_kernel");
-}
-
-template <class Op, bool A_MN, bool B_MN>
-static int launch_gemm_pingpong(const void* A, long lda, const void* B, long ldb, const GemmParams& p,
-                                cudaStream_t stream) {
-  using Cfg = GemmCfg<PP_BN, B_MN>;
-  constexpr int EB = Op::FP8 ? 1 : 2;
-  CUtensorMap tmA, tmB;
-  int rc;
-  if (!A_MN) rc = make_tmap_2d(&tmA, A, (uint64_t)p.K, (uint64_t)p.M, lda, Op::BK, BM, EB);
-  else       rc = make_tmap_2d(&tmA, A, (uint64_t)p.M, (uint64_t)p.K, lda, 64, 64);
-  if (rc) return rc;
-  if (!B_MN) rc = make_tmap_2d(&tmB, B, (uint64_t)p.K, (uint64_t)p.N, ldb, Op::BK, PP_BN, EB);
-  else       rc = make_tmap_2d(&tmB, B, (uint64_t)p.N, (uint64_t)p.K, ldb, 64, 64);
-  if (rc) return rc;
-  auto kern = gemm_bf16_pingpong_kernel<Op, A_MN, B_MN>;
-  static bool attr_set[64] = {};
-  if (first_use_on_device(attr_set)) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
-    if (e != cudaSuccess) return set_error_cuda("cudaFuncSetAttribute(gemm pingpong)", e);
-  }
-  const int num_tiles = ((p.M + BM - 1) / BM) * ((p.N + PP_BN - 1) / PP_BN);
-  const int ctas = num_sms() < num_tiles ? num_sms() : num_tiles;
-  cudaError_t le = launch_pdl(kern, dim3(ctas), dim3(GEMM_THREADS), Cfg::SMEM_BYTES, stream, tmA, tmB, p);
-  if (le != cudaSuccess) return set_error_cuda("launch(gemm_bf16_pingpong_kernel)", le);
-  count_launch();
-  return check_launch("gemm_bf16_pingpong_kernel");
-}
-
-static int dispatch_pingpong(bool a_mn, bool b_mn, const void* A, long lda, const void* B, long ldb,
-                             const GemmParams& p, cudaStream_t stream) {
-  if (!a_mn && !b_mn) return launch_gemm_pingpong<OpBf16, false, false>(A, lda, B, ldb, p, stream);
-  if (!a_mn && b_mn) return launch_gemm_pingpong<OpBf16, false, true>(A, lda, B, ldb, p, stream);
-  return launch_gemm_pingpong<OpBf16, true, true>(A, lda, B, ldb, p, stream);
-}
-
-template <bool A_MN, bool B_MN, int CL>
-static int dispatch_bn(int bn, const void* A, long lda, const void* B, long ldb,
-                       const GemmParams& p, cudaStream_t stream) {
-  switch (bn) {
-    case 256: return launch_gemm<OpBf16, 256, A_MN, B_MN, CL>(A, lda, B, ldb, p, stream);
-    case 192: return launch_gemm<OpBf16, 192, A_MN, B_MN, CL>(A, lda, B, ldb, p, stream);
-    case 176: return launch_gemm<OpBf16, 176, A_MN, B_MN, CL>(A, lda, B, ldb, p, stream);
-    case 128: return launch_gemm<OpBf16, 128, A_MN, B_MN, CL>(A, lda, B, ldb, p, stream);
-    default: return set_error("ivb_gemm_bf16: unsupported BN");
-  }
-}
-
-template <int CL>
-static int dispatch_major(int bn, bool a_mn, bool b_mn, const void* A, long lda, const void* B, long ldb,
-                          const GemmParams& p, cudaStream_t stream) {
-  if (!a_mn && !b_mn) return dispatch_bn<false, false, CL>(bn, A, lda, B, ldb, p, stream);
-  if (!a_mn && b_mn) return dispatch_bn<false, true, CL>(bn, A, lda, B, ldb, p, stream);
-  return dispatch_bn<true, true, CL>(bn, A, lda, B, ldb, p, stream);
+  return check_launch(name);
 }
 
 // Pick the N tile that wastes the fewest padded columns / partial waves (fp8: of the two tiles its cooperative kernel has).
@@ -656,18 +579,52 @@ static GemmParams make_params(int M, int N, int K, int epilogue, int flags, void
   return p;
 }
 
-// FP8 kernel choice: the ping-pong kernel (accumulation in the tensor core) where use_pingpong picks it, otherwise the
-// cooperative kernel, which promotes each k-block to fp32 (BN 192 or 128).  Promotion is not needed for accuracy at
-// the step's shapes: the tensor-core accumulation adds at most 4.5 % of the error the fp8 quantisation already carries
-// (fc2, K = 6144; tests/test_gemm_fp8_gpu.py::test_accumulation_error_at_step_shapes, DESIGN.md 4.1), and ping-pong is
-// the faster form at every one of them.
+struct KernelChoice {
+  bool pingpong;
+  int bn, cl;
+};
 
-template <class Op>
-static int dispatch_fp8(bool pingpong, int bn, const void* A, long lda, const void* B, long ldb, const GemmParams& p,
-                        cudaStream_t stream) {
-  if (pingpong) return launch_gemm_pingpong<Op, false, false>(A, lda, B, ldb, p, stream);
-  if (bn == 192) return launch_gemm<Op, 192, false, false, 1>(A, lda, B, ldb, p, stream);
-  return launch_gemm<Op, 128, false, false, 1>(A, lda, B, ldb, p, stream);
+// The kernel of a GEMM whose force flags and tile_n the entry point has checked.  The CTA-pair (cluster) kernel when
+// forced, or by default (default_2cta) for problems tall enough to fill 256-row tiles; the ping-pong kernel when forced
+// or chosen by use_pingpong; the single-CTA cooperative kernel otherwise / when IVB_FLAG_1CTA is set, at tile_n or
+// choose_bn's width.  FP8 has no CTA-pair kernel, and its cooperative kernel promotes each k-block to fp32 (BN 192 or
+// 128).  Promotion is not needed for accuracy at the step's shapes: the tensor-core accumulation adds at most 4.5 % of
+// the error the fp8 quantisation already carries (fc2, K = 6144;
+// tests/test_gemm_fp8_gpu.py::test_accumulation_error_at_step_shapes, DESIGN.md 4.1), and ping-pong is the faster
+// form at every one of them, so FP8 selects like bf16.
+static KernelChoice choose_kernel(int M, int N, int K, int flags, int tile_n, bool fp8, bool default_2cta) {
+  const bool force2 = (flags & IVB_FLAG_2CTA) != 0, force1 = (flags & IVB_FLAG_1CTA) != 0;
+  const bool forcepp = (flags & IVB_FLAG_PINGPONG) != 0;
+  KernelChoice k;
+  k.cl = (force2 || (!force1 && !forcepp && default_2cta && M >= 512)) ? 2 : 1;
+  k.pingpong = forcepp || (k.cl == 1 && !force1 && (tile_n == 0 || tile_n == PP_BN) && use_pingpong(M, N, K));
+  k.bn = k.pingpong ? PP_BN : tile_n > 0 ? tile_n : choose_bn(M, N, k.cl, fp8);
+  return k;
+}
+
+// The kernel k names, for operands of format Op and majors A_MN / B_MN.  Together with the entry points' choice of Op
+// and majors this instantiates the library's 36 kernels: the ping-pong kernel of every Op and major; the bf16
+// cooperative kernel at BN 256 / 192 / 176 / 128 and CL 1 or 2; the FP8 one (K-major only) at BN 192 or 128, CL 1.
+template <class Op, bool A_MN, bool B_MN>
+static int dispatch(const KernelChoice& k, const void* A, long lda, const void* B, long ldb, const GemmParams& p,
+                    cudaStream_t stream) {
+  if (k.pingpong) return launch_gemm<Op, true, PP_BN, A_MN, B_MN, 1>(A, lda, B, ldb, p, stream);
+  // the cooperative kernel, by (BN, CL): the bf16-only pairs, then those FP8 has too
+  if constexpr (!Op::FP8) {
+    switch (k.bn * 4 + k.cl) {
+      case 256 * 4 + 1: return launch_gemm<Op, false, 256, A_MN, B_MN, 1>(A, lda, B, ldb, p, stream);
+      case 176 * 4 + 1: return launch_gemm<Op, false, 176, A_MN, B_MN, 1>(A, lda, B, ldb, p, stream);
+      case 256 * 4 + 2: return launch_gemm<Op, false, 256, A_MN, B_MN, 2>(A, lda, B, ldb, p, stream);
+      case 192 * 4 + 2: return launch_gemm<Op, false, 192, A_MN, B_MN, 2>(A, lda, B, ldb, p, stream);
+      case 176 * 4 + 2: return launch_gemm<Op, false, 176, A_MN, B_MN, 2>(A, lda, B, ldb, p, stream);
+      case 128 * 4 + 2: return launch_gemm<Op, false, 128, A_MN, B_MN, 2>(A, lda, B, ldb, p, stream);
+    }
+  }
+  switch (k.bn * 4 + k.cl) {
+    case 192 * 4 + 1: return launch_gemm<Op, false, 192, A_MN, B_MN, 1>(A, lda, B, ldb, p, stream);
+    case 128 * 4 + 1: return launch_gemm<Op, false, 128, A_MN, B_MN, 1>(A, lda, B, ldb, p, stream);
+  }
+  return set_error("ivb_gemm_bf16: unsupported BN");
 }
 
 }  // namespace ivb
@@ -688,20 +645,15 @@ extern "C" int ivb_gemm_bf16(const void* A, int a_mn_major, long lda, const void
   if (int rc = check_epilogue_args("ivb_gemm_bf16", epilogue, out0, out1, ld1, aux, ldaux, bias, gamma)) return rc;
   if (a_mn_major && !b_mn_major) return set_error("ivb_gemm_bf16: (A MN-major, B K-major) unused");
   const GemmParams p = make_params(M, N, K, epilogue, flags, out0, ld0, out1, ld1, bias, gamma, aux, ldaux, rowscale);
-  // kernel selection: the CTA-pair (cluster) kernel when forced, or by default for problems tall enough to fill
-  // 256-row tiles; the ping-pong kernel when forced or chosen by use_pingpong; the cooperative single-CTA kernel
-  // otherwise / when IVB_FLAG_1CTA is set.
   const bool force2 = (flags & IVB_FLAG_2CTA) != 0, force1 = (flags & IVB_FLAG_1CTA) != 0;
   const bool forcepp = (flags & IVB_FLAG_PINGPONG) != 0;
   if ((int)force2 + (int)force1 + (int)forcepp > 1)
     return set_error("ivb_gemm_bf16: IVB_FLAG_1CTA, IVB_FLAG_2CTA and IVB_FLAG_PINGPONG exclude each other");
   if (forcepp && tile_n != 0 && tile_n != PP_BN) return set_error("ivb_gemm_bf16: the ping-pong kernel has tile_n 128");
-  const int cl = (force2 || (!force1 && !forcepp && g_default_2cta && M >= 512)) ? 2 : 1;
-  if (forcepp || (cl == 1 && !force1 && (tile_n == 0 || tile_n == PP_BN) && use_pingpong(M, N, K)))
-    return dispatch_pingpong(a_mn_major != 0, b_mn_major != 0, A, lda, B, ldb, p, stream);
-  const int bn = tile_n > 0 ? tile_n : choose_bn(M, N, cl);
-  if (cl == 2) return dispatch_major<2>(bn, a_mn_major != 0, b_mn_major != 0, A, lda, B, ldb, p, stream);
-  return dispatch_major<1>(bn, a_mn_major != 0, b_mn_major != 0, A, lda, B, ldb, p, stream);
+  const KernelChoice k = choose_kernel(M, N, K, flags, tile_n, false, g_default_2cta);
+  if (!a_mn_major && !b_mn_major) return dispatch<OpBf16, false, false>(k, A, lda, B, ldb, p, stream);
+  if (!a_mn_major) return dispatch<OpBf16, false, true>(k, A, lda, B, ldb, p, stream);
+  return dispatch<OpBf16, true, true>(k, A, lda, B, ldb, p, stream);
 }
 
 extern "C" int ivb_gemm_fp8(const void* A, int a_mn_major, long lda, int a_format, const float* a_scale_inv,
@@ -729,9 +681,8 @@ extern "C" int ivb_gemm_fp8(const void* A, int a_mn_major, long lda, int a_forma
   GemmParams p = make_params(M, N, K, epilogue, flags, out0, ld0, out1, ld1, bias, gamma, aux, ldaux, rowscale);
   p.a_scale_inv = a_scale_inv;
   p.b_scale_inv = b_scale_inv;
-  const bool pingpong = forcepp || (!force1 && tile_n != 192 && use_pingpong(M, N, K));
-  const int bn = tile_n > 0 ? tile_n : choose_bn(M, N, 1, true);
-  if (vec) return dispatch_fp8<OpVecFp8>(pingpong, bn, A, lda, B, ldb, p, stream);
-  if (a_format == IVB_FP8_E5M2) return dispatch_fp8<OpFp8<true>>(pingpong, bn, A, lda, B, ldb, p, stream);
-  return dispatch_fp8<OpFp8<false>>(pingpong, bn, A, lda, B, ldb, p, stream);
+  const KernelChoice k = choose_kernel(M, N, K, flags, tile_n, true, false);
+  if (vec) return dispatch<OpVecFp8, false, false>(k, A, lda, B, ldb, p, stream);
+  if (a_format == IVB_FP8_E5M2) return dispatch<OpFp8<true>, false, false>(k, A, lda, B, ldb, p, stream);
+  return dispatch<OpFp8<false>, false, false>(k, A, lda, B, ldb, p, stream);
 }

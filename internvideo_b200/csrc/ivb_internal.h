@@ -15,16 +15,6 @@ int set_error_cuda(const char* what, cudaError_t e);
 int check_launch(const char* what);  // cudaGetLastError() -> status
 void count_launch();                 // bumps the library-wide launch counter
 int num_sms();
-// per-DEVICE once-flag for cudaFuncSetAttribute (a process may drive several GPUs): returns true the first time it is
-// called for (flags, current device) and marks it.
-inline bool first_use_on_device(bool (&flags)[64]) {
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (dev < 0 || dev >= 64) return true;
-  if (flags[dev]) return false;
-  flags[dev] = true;
-  return true;
-}
 // Raises Kern's dynamic shared-memory limit to `bytes` on the current device, once per device: the device is marked
 // only after the call succeeds, so a failed attempt is retried (and reported) by the next launch.
 template <auto Kern>

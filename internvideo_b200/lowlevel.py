@@ -83,9 +83,22 @@ def gemm(a, b, *, a_t=False, b_t=False, epi=EPI_BF16, flags=0, out0=None, out1=N
         N, Kb = b.shape
     if K != Kb:
         raise _lib.IvbError(f"gemm: contraction mismatch {K} vs {Kb}")
+    out0, ld0, ld1, ldaux = _epilogue_operands(M, N, epi, out0, out1, bias, gamma, aux, a.device)
+    ev0 = _prof_begin()
+    rc = _lib_().ivb_gemm_bf16(_p(a), int(a_t), lda, _p(b), int(b_t), ldb, M, N, K, epi, flags,
+                               _p(out0), ld0, _p(out1), ld1, _p(bias), _p(gamma), _p(aux), ldaux,
+                               _p(rowscale), tile_n, _stream())
+    _lib.check(rc, "ivb_gemm_bf16")
+    _prof_end(ev0, 2.0 * M * N * K, "gemm")
+    return out0
+
+
+def _epilogue_operands(M, N, epi, out0, out1, bias, gamma, aux, device):
+    """Checks the fused epilogue's operands of an [M, N] GEMM (allocating out0 if it is None).
+    Returns (out0, ld0, ld1, ldaux), with 0 for an absent operand."""
     out_dtype = f32 if epi in (EPI_F32, EPI_RESID) else bf16
     if out0 is None:
-        out0 = torch.empty((M, N), device=a.device, dtype=out_dtype)
+        out0 = torch.empty((M, N), device=device, dtype=out_dtype)
     _chk(out0, out_dtype, "out0")
     ld0 = _rows2d(out0, "out0")
     ld1 = 0
@@ -96,17 +109,7 @@ def gemm(a, b, *, a_t=False, b_t=False, epi=EPI_BF16, flags=0, out0=None, out1=N
     if aux is not None:
         _chk(aux, f32 if epi == EPI_RESID else bf16, "aux")
         ldaux = _rows2d(aux, "aux")
-    prof = _PROF[0]
-    if prof is not None:
-        ev0 = torch.cuda.Event(enable_timing=True); ev0.record()
-    rc = _lib_().ivb_gemm_bf16(_p(a), int(a_t), lda, _p(b), int(b_t), ldb, M, N, K, epi, flags,
-                               _p(out0), ld0, _p(out1), ld1, _p(bias), _p(gamma), _p(aux), ldaux,
-                               _p(rowscale), tile_n, _stream())
-    _lib.check(rc, "ivb_gemm_bf16")
-    if prof is not None:
-        ev1 = torch.cuda.Event(enable_timing=True); ev1.record()
-        prof.records.append((ev0, ev1, 2.0 * M * N * K, "gemm"))
-    return out0
+    return out0, ld0, ld1, ldaux
 
 
 # ----------------------------------------------------------------------------------------- FP8
@@ -193,19 +196,7 @@ def gemm_fp8(a, a_scale_inv, b, b_scale_inv, *, epi=EPI_BF16, flags=0, out0=None
     N, Kb = b.shape
     if K != Kb:
         raise _lib.IvbError(f"gemm_fp8: contraction mismatch {K} vs {Kb}")
-    out_dtype = f32 if epi in (EPI_F32, EPI_RESID) else bf16
-    if out0 is None:
-        out0 = torch.empty((M, N), device=a.device, dtype=out_dtype)
-    _chk(out0, out_dtype, "out0")
-    ld0 = _rows2d(out0, "out0")
-    ld1 = 0
-    if out1 is not None:
-        _chk(out1, bf16, "out1"); ld1 = _rows2d(out1, "out1")
-    _chk(bias, bf16, "bias"); _chk(gamma, bf16, "gamma")
-    ldaux = 0
-    if aux is not None:
-        _chk(aux, f32 if epi == EPI_RESID else bf16, "aux")
-        ldaux = _rows2d(aux, "aux")
+    out0, ld0, ld1, ldaux = _epilogue_operands(M, N, epi, out0, out1, bias, gamma, aux, a.device)
     fmt = FP8_E5M2 if a.dtype == torch.float8_e5m2 else FP8_E4M3
     if a_scale_inv.numel() != 1 or b_scale_inv.numel() != 1:
         if (a_scale_inv.shape != (M,) or b_scale_inv.shape != (N,) or not a_scale_inv.is_contiguous()
