@@ -1,0 +1,178 @@
+// ivb_attn.cuh — the pieces the attention forward (ivb_attn.cu) and backward (ivb_attn_bwd.cu) kernels share: one CTA
+// per (128-row block, head, clip) that streams 64-row tiles of the other operands through a ring.
+#pragma once
+#include <stdio.h>
+
+#include <initializer_list>
+
+#include "ivb_internal.h"
+#include "ivb_ptx.cuh"
+
+namespace ivb {
+
+constexpr int ATT_ROWS = 128;     // rows owned by a CTA (two MMA warpgroups of 64)
+constexpr int ATT_COLS = 64;      // rows of a streamed tile
+constexpr int ATT_THREADS = 384;  // the producer warpgroup and the two MMA warpgroups
+
+// 4-D view (d, head, token, clip) of a [B*n, ld] projection buffer starting at `base`, box_tokens rows per load.
+inline int make_head_tmap(CUtensorMap* tm, const void* base, long ld, int B, int n, int H, int d, int box_tokens) {
+  const uint64_t dims[4] = {(uint64_t)d, (uint64_t)H, (uint64_t)n, (uint64_t)B};
+  const long strides[3] = {(long)d, ld, (long)n * ld};
+  const uint32_t box[4] = {64, 1, (uint32_t)box_tokens, 1};
+  return make_tmap_4d(tm, base, dims, strides, box);
+}
+
+extern __shared__ __align__(1024) uint8_t attn_smem[];
+
+// Shared memory of a CTA (1024-byte aligned for the 128-byte swizzle): ROWS operands of the CTA's rows, two rings of NS
+// streamed tiles, VECS rings of NS x 64 floats, then the barriers: `row`, BARS x NS `full` and BARS x NS `empty`.
+template <int KA, int ROWS, int NS_, int VECS, int BARS_>
+struct AttnSmem {
+  static constexpr int NS = NS_, BARS = BARS_, VEC_BYTES = ATT_COLS * 4;
+  static constexpr int ROW_BYTES = KA * ATT_ROWS * 128, TILE_BYTES = KA * ATT_COLS * 128;   // KA 64-column atoms
+  static constexpr int RING = ROWS * ROW_BYTES, VEC = RING + 2 * NS * TILE_BYTES, BAR = VEC + VECS * NS * VEC_BYTES;
+  static constexpr int BYTES = BAR + 128;
+  static_assert((1 + 2 * BARS * NS) * 8 <= 128 && BYTES <= 227 * 1024, "attention: shared-memory budget");
+
+  static __device__ __forceinline__ uint8_t* rows(int i) { return attn_smem + i * ROW_BYTES; }
+  static __device__ __forceinline__ uint8_t* tile(int ring, int st) {
+    return attn_smem + RING + (ring * NS + st) * TILE_BYTES;
+  }
+  static __device__ __forceinline__ float* vec(int v, int st) {
+    return reinterpret_cast<float*>(attn_smem + VEC + (v * NS + st) * VEC_BYTES);
+  }
+  static __device__ __forceinline__ uint64_t* bar_row() { return reinterpret_cast<uint64_t*>(attn_smem + BAR); }
+  static __device__ __forceinline__ uint64_t* full(int ring, int st) { return bar_row() + 1 + ring * NS + st; }
+  static __device__ __forceinline__ uint64_t* empty(int ring, int st) { return bar_row() + 1 + (BARS + ring) * NS + st; }
+};
+
+// The j-th use of a ring of NS stages: its stage, and the parity the MMA warpgroups wait for on `full` (the producer
+// waits for ph ^ 1 on `empty`, so a stage's first fill does not wait).
+template <int NS>
+struct RingSlot {
+  int st;
+  uint32_t ph;
+  __device__ __forceinline__ explicit RingSlot(int j) : st(j % NS), ph((j / NS) & 1) {}
+};
+
+struct AttnCta {
+  int warp, lane, wg, row0, h, b;  // row0: the CTA's first row; h: its head; b: its clip
+  int nblk, live;  // streamed tiles; MMA warpgroups that own a row < n (each arrives once on an `empty`)
+  int rloc;        // in an MMA warpgroup: this thread's accumulator rows of the CTA are rloc and rloc + 8
+  bool signal;     // the thread that arrives on `empty` for its warpgroup
+};
+
+template <class Smem>
+__device__ __forceinline__ AttnCta attn_prologue(int n) {
+  AttnCta c;
+  const int tid = threadIdx.x;
+  c.warp = tid >> 5; c.lane = tid & 31; c.wg = tid >> 7;
+  c.row0 = blockIdx.x * ATT_ROWS; c.h = blockIdx.y; c.b = blockIdx.z;
+  c.nblk = (n + ATT_COLS - 1) / ATT_COLS;
+  c.live = min(2, (n - c.row0 + 63) / 64);
+  c.rloc = (c.wg - 1) * 64 + (c.warp & 3) * 16 + (c.lane >> 2);
+  c.signal = (tid & 127) == 0;
+  if (tid == 0) {
+    if ((smem_u32(attn_smem) & 1023u) != 0) __trap();
+    mbar_init(Smem::bar_row(), 1);
+    for (int i = 0; i < Smem::NS; ++i) {
+      for (int r = 0; r < Smem::BARS; ++r) mbar_init(Smem::full(r, i), 1);
+      for (int r = 0; r < Smem::BARS; ++r) mbar_init(Smem::empty(r, i), c.live);
+    }
+    fence_mbar_init();
+  }
+  __syncthreads();
+  return c;
+}
+
+// Warpgroup 0 gives its registers up and one elected thread runs produce(); each live MMA warpgroup cw takes them and
+// runs consume(cw).
+template <class Produce, class Consume>
+__device__ __forceinline__ void attn_roles(const AttnCta& c, Produce&& produce, Consume&& consume) {
+  if (c.wg == 0) {
+    setmaxnreg_dec<24>();
+    if (c.warp == 0 && elect_one()) produce();
+  } else {
+    setmaxnreg_inc<240>();
+    const int cw = c.wg - 1;
+    if (cw >= c.live) return;
+    consume(cw);
+  }
+}
+
+// TMA of rows [row, row + BOX) of head h of clip b (a make_head_tmap view with a BOX-row box) into KA 64-column atoms.
+template <int KA, int BOX>
+__device__ __forceinline__ void load_head_rows(uint8_t* dst, const CUtensorMap* tm, int h, int row, int b,
+                                               uint64_t* bar) {
+#pragma unroll
+  for (int a = 0; a < KA; ++a) tma_load_4d(dst + a * (BOX * 128), tm, a * 64, h, row, b, bar);
+}
+
+// Writes this thread's rows (< n) of a 64 x NO accumulator, row r times factor[r], as bf16 to head h of the [B*n, ld]
+// buffer out.  Fragment row r holds columns 8 jn + 2 (lane % 4) + {0, 1} in acc[4 jn + 2 r], acc[4 jn + 2 r + 1].
+template <int NO>
+__device__ __forceinline__ void store_rows(const float (&acc)[NO / 2], __nv_bfloat16* out, long ld, const AttnCta& c,
+                                           int n, int d, const float (&factor)[2] = {1.f, 1.f}) {
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const int row = c.row0 + c.rloc + 8 * r;
+    if (row >= n) continue;
+    __nv_bfloat16* orow = out + (static_cast<long>(c.b) * n + row) * ld + c.h * d;
+#pragma unroll
+    for (int jn = 0; jn < NO / 8; ++jn) {
+      const int col = 8 * jn + 2 * (c.lane & 3);
+      if (col < d)
+        *reinterpret_cast<uint32_t*>(orow + col) =
+            pack_bf16(acc[4 * jn + 2 * r] * factor[r], acc[4 * jn + 2 * r + 1] * factor[r]);
+    }
+  }
+}
+
+// ------------------------------------------------------------------ host side
+// Refuses, as entry point fn, a head dim that is not a multiple of 8 in [16, 128] and a pitch that is not a multiple of 8.
+inline int check_head_args(const char* fn, int d, std::initializer_list<long> pitches) {
+  const char* why = d % 8 != 0 || d > 128 || d < 16 ? "head_dim must be a multiple of 8 in [16,128]" : nullptr;
+  for (long ld : pitches)
+    if (why == nullptr && (ld & 7)) why = "pitches must be multiples of 8";
+  if (why == nullptr) return 0;
+  char msg[128];
+  snprintf(msg, sizeof(msg), "%s: %s", fn, why);
+  return set_error(msg);
+}
+
+template <int KA_, int NO_, int KS_> struct HeadDim { static constexpr int KA = KA_, NO = NO_, KS = KS_; };
+
+// Calls f(HeadDim<KA, NO, KS>{}) for head dim d: KA 64-column atoms, NO = d rounded up to 32 (the N of the accumulate
+// MMAs) and KS = ceil(d / 16) k16 steps of the score MMAs.
+template <class F>
+int dispatch_head_dim(int d, F&& f) {
+  const bool ks_even = (d + 15) / 16 % 2 == 0;
+  switch ((d + 31) / 32) {
+    case 1: return ks_even ? f(HeadDim<1, 32, 2>{}) : f(HeadDim<1, 32, 1>{});
+    case 2: return ks_even ? f(HeadDim<1, 64, 4>{}) : f(HeadDim<1, 64, 3>{});
+    case 3: return ks_even ? f(HeadDim<2, 96, 6>{}) : f(HeadDim<2, 96, 5>{});
+    default: return ks_even ? f(HeadDim<2, 128, 8>{}) : f(HeadDim<2, 128, 7>{});
+  }
+}
+
+// Raises Kern's shared-memory limit (`attr` names that call in an error) and launches it on one CTA per (128-row block,
+// head, clip), through launch_pdl when PDL.
+template <auto Kern, bool PDL, class... Args>
+int launch_attn(const char* attr, const char* name, int smem, int B, int n, int H, cudaStream_t stream,
+                const Args&... args) {
+  if (int rc = raise_smem_limit<Kern>(smem, attr)) return rc;
+  const dim3 grid((n + ATT_ROWS - 1) / ATT_ROWS, H, B);
+  if constexpr (PDL) {
+    if (const cudaError_t e = launch_pdl(Kern, grid, dim3(ATT_THREADS), smem, stream, args...)) {
+      char what[64];
+      snprintf(what, sizeof(what), "launch(%s)", name);
+      return set_error_cuda(what, e);
+    }
+  } else {
+    Kern<<<grid, ATT_THREADS, smem, stream>>>(args...);
+  }
+  count_launch();
+  return check_launch(name);
+}
+
+}  // namespace ivb

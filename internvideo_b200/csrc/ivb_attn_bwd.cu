@@ -15,29 +15,17 @@
 // K-major operand (rows = M/N index) for one MMA and an MN-major operand (rows = K index) for the
 // other, only the wgmma descriptor differs.
 //
-// Warp roles (384 threads): warpgroup 0 = the TMA producer (one elected thread), warpgroups 1 and 2 own 64 of the
-// 128 rows each.  A warpgroup whose 64 rows all lie beyond the sequence does no work at all.  mbarriers:
-//   bar_row     TMA -> MMA        X,Y (the 128 owned rows) landed
-//   full[s]     TMA -> MMA        streamed tiles U_j, W_j of stage s landed (tx); MODE 1 also lse2/delta of the
-//                                 tile's 64 queries, so the math reads them from shared memory
-//   empty[s]    MMA -> TMA        every live warpgroup retired every MMA that reads stage s
-// When both warpgroups are live they take turns issuing S/dP (named barriers 1 and 2): one warpgroup's MMAs run on
+// CTA roles and barriers as in ivb_attn.cuh: `row` covers X and Y (the 128 owned rows), full[s] the streamed tiles
+// U_j, W_j and, in MODE 1, the tile's 64 lse2/delta values.  When both warpgroups are live they take turns issuing S/dP (named barriers 1 and 2): one warpgroup's MMAs run on
 // the tensor core while the other computes P / dS.  Software pipelining inside a warpgroup (S/dP of tile j+1 in
 // flight during the math of tile j) does not fit the register file at d > 64 in MODE 1: dK + dV take NO registers,
 // two S/dP tiles 128 and the A fragments 32.
 #include <math.h>
 #include <stdlib.h>
 
-#include "ivb_internal.h"
-#include "ivb_ptx.cuh"
+#include "ivb_attn.cuh"
 
 namespace ivb {
-
-int make_head_tmap(CUtensorMap* tm, const void* base, long ld, int B, int n, int H, int d,
-                   int box_tokens);
-
-constexpr int BWD_ROWS = 128;  // rows owned by the CTA (two warpgroups of 64)
-constexpr int BWD_COLS = 64;   // streamed tile
 
 struct AttnBwdParams {
   int B, n, H, d;
@@ -78,84 +66,45 @@ __global__ void attn_bwd_prep_kernel(const __nv_bfloat16* __restrict__ o, long l
 
 constexpr int BWD_NST = 3;  // streamed-tile stages
 
+// X and Y; the U and W rings under one full/empty pair per stage; lse2 and delta of each streamed tile (MODE 1).
+template <int KA>
+using BwdSmem = AttnSmem<KA, 2, BWD_NST, 2, 1>;
+
 // KA: 64-wide atoms covering head_dim (1: d <= 64, 2: d <= 128); NO: wgmma N of the accumulate MMAs;
 // KS: k16 steps of the S/dP MMAs, ceil(d / 16).
 template <int MODE, int KA, int NO, int KS>
-__global__ void __launch_bounds__(384, 1)
+__global__ void __launch_bounds__(ATT_THREADS, 1)
 attn_bwd_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmY,
                 const __grid_constant__ CUtensorMap tmU, const __grid_constant__ CUtensorMap tmW,
                 const AttnBwdParams p) {
-  constexpr int ROW_BYTES = KA * BWD_ROWS * 128;   // one owned-row operand
-  constexpr int COL_BYTES = KA * BWD_COLS * 128;   // one streamed tile
-  constexpr int VEC_BYTES = BWD_COLS * 4;          // lse2 or delta of one streamed tile (MODE 1)
-  extern __shared__ __align__(1024) uint8_t smem[];
-  uint8_t* sX = smem;
-  uint8_t* sY = sX + ROW_BYTES;
-  uint8_t* sU = sY + ROW_BYTES;                 // BWD_NST stages
-  uint8_t* sW = sU + BWD_NST * COL_BYTES;       // BWD_NST stages
-  float* sLse = reinterpret_cast<float*>(sW + BWD_NST * COL_BYTES);   // BWD_NST x 64
-  float* sDelta = sLse + BWD_NST * BWD_COLS;                          // BWD_NST x 64
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sDelta + BWD_NST * BWD_COLS);
-  uint64_t* bar_row = bars;
-  uint64_t* full = bars + 1;
-  uint64_t* empty = full + BWD_NST;
-
-  const int tid = threadIdx.x;
-  const int warp = tid >> 5;
-  const int lane = tid & 31;
-  const int wg = tid >> 7;
-  const int r0 = blockIdx.x * BWD_ROWS;
-  const int h = blockIdx.y;
-  const int b = blockIdx.z;
-  const int nblk = (p.n + BWD_COLS - 1) / BWD_COLS;
-  const int live = min(2, (p.n - r0 + 63) / 64);   // warpgroups that own at least one row < n
-  const long hb = (static_cast<long>(b) * p.H + h) * p.n_pad;
-
-  if (tid == 0) {
-    if ((smem_u32(smem) & 1023u) != 0) __trap();
-    mbar_init(bar_row, 1);
-    for (int i = 0; i < BWD_NST; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], live); }
-    fence_mbar_init();
-  }
-  __syncthreads();
+  using Smem = BwdSmem<KA>;
+  const AttnCta c = attn_prologue<Smem>(p.n);
+  const long hb = (static_cast<long>(c.b) * p.H + c.h) * p.n_pad;
   pdl_wait();
   pdl_launch_dependents();
 
-  if (wg == 0) {
-    setmaxnreg_dec<24>();
+  attn_roles(c, [&] {
     // ===================== TMA producer =====================
-    if (warp == 0 && elect_one()) {
-      tma_prefetch_desc(&tmX); tma_prefetch_desc(&tmY); tma_prefetch_desc(&tmU); tma_prefetch_desc(&tmW);
-      mbar_expect_tx(bar_row, 2 * ROW_BYTES);
-#pragma unroll
-      for (int a = 0; a < KA; ++a) {
-        tma_load_4d(sX + a * (BWD_ROWS * 128), &tmX, a * 64, h, r0, b, bar_row);
-        tma_load_4d(sY + a * (BWD_ROWS * 128), &tmY, a * 64, h, r0, b, bar_row);
-      }
-      for (int j = 0; j < nblk; ++j) {
-        const int st = j % BWD_NST;
-        mbar_wait(&empty[st], ((j / BWD_NST) & 1) ^ 1);
-        mbar_expect_tx(&full[st], 2 * COL_BYTES + (MODE == 1 ? 2 * VEC_BYTES : 0));
-#pragma unroll
-        for (int a = 0; a < KA; ++a) {
-          tma_load_4d(sU + st * COL_BYTES + a * (BWD_COLS * 128), &tmU, a * 64, h, j * BWD_COLS, b, &full[st]);
-          tma_load_4d(sW + st * COL_BYTES + a * (BWD_COLS * 128), &tmW, a * 64, h, j * BWD_COLS, b, &full[st]);
-        }
-        if (MODE == 1) {   // the padded workspaces hold whole 64-query tiles, 256-byte aligned
-          bulk_load_1d(sLse + st * BWD_COLS, p.lse2p + hb + j * BWD_COLS, VEC_BYTES, &full[st]);
-          bulk_load_1d(sDelta + st * BWD_COLS, p.deltap + hb + j * BWD_COLS, VEC_BYTES, &full[st]);
-        }
+    tma_prefetch_desc(&tmX); tma_prefetch_desc(&tmY); tma_prefetch_desc(&tmU); tma_prefetch_desc(&tmW);
+    mbar_expect_tx(Smem::bar_row(), 2 * Smem::ROW_BYTES);
+    load_head_rows<KA, ATT_ROWS>(Smem::rows(0), &tmX, c.h, c.row0, c.b, Smem::bar_row());
+    load_head_rows<KA, ATT_ROWS>(Smem::rows(1), &tmY, c.h, c.row0, c.b, Smem::bar_row());
+    for (int j = 0; j < c.nblk; ++j) {
+      const RingSlot<BWD_NST> s(j);
+      uint64_t* full = Smem::full(0, s.st);
+      mbar_wait(Smem::empty(0, s.st), s.ph ^ 1);
+      mbar_expect_tx(full, 2 * Smem::TILE_BYTES + (MODE == 1 ? 2 * Smem::VEC_BYTES : 0));
+      load_head_rows<KA, ATT_COLS>(Smem::tile(0, s.st), &tmU, c.h, j * ATT_COLS, c.b, full);
+      load_head_rows<KA, ATT_COLS>(Smem::tile(1, s.st), &tmW, c.h, j * ATT_COLS, c.b, full);
+      if (MODE == 1) {   // the padded workspaces hold whole 64-query tiles, 256-byte aligned
+        bulk_load_1d(Smem::vec(0, s.st), p.lse2p + hb + j * ATT_COLS, Smem::VEC_BYTES, full);
+        bulk_load_1d(Smem::vec(1, s.st), p.deltap + hb + j * ATT_COLS, Smem::VEC_BYTES, full);
       }
     }
-  } else {
-    setmaxnreg_inc<240>();
+  }, [&](int cw) {
     // ===================== MMA + math warpgroups =====================
-    const int cw = wg - 1;
-    if (cw >= live) return;
-    const bool pingpong = live == 2;
-    const bool signal = (tid & 127) == 0;
-    const int rloc = cw * 64 + (warp & 3) * 16 + (lane >> 2);  // this thread's rows: rloc, rloc + 8
-    const uint32_t xa = smem_u32(sX) + cw * 8192, ya = smem_u32(sY) + cw * 8192;
+    const bool pingpong = c.live == 2;
+    const uint32_t xa = smem_u32(Smem::rows(0)) + cw * 8192, ya = smem_u32(Smem::rows(1)) + cw * 8192;
     float acc1[NO / 2];                     // MODE 1: dV   MODE 0: dQ
     float acc2[MODE == 1 ? NO / 2 : 1];     // MODE 1: dK
 #pragma unroll
@@ -166,121 +115,75 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__
     if (MODE == 0) {
 #pragma unroll
       for (int r = 0; r < 2; ++r) {
-        const int q = r0 + rloc + 8 * r;
+        const int q = c.row0 + c.rloc + 8 * r;
         if (q < p.n_pad) { row_lse[r] = p.lse2p[hb + q]; row_delta[r] = p.deltap[hb + q]; }
       }
     }
 
     // Named barrier 1 + cw: "warpgroup cw may issue S/dP".  Warpgroup 0 goes first.
     if (pingpong && cw == 1) named_bar_arrive(1, 256);
-    mbar_wait(bar_row, 0);
-    for (int j = 0; j < nblk; ++j) {
-      const int st = j % BWD_NST;
-      mbar_wait(&full[st], (j / BWD_NST) & 1);
-      const uint32_t ua = smem_u32(sU + st * COL_BYTES), wa = smem_u32(sW + st * COL_BYTES);
-      float sc[BWD_COLS / 2], dp[BWD_COLS / 2];
+    mbar_wait(Smem::bar_row(), 0);
+    for (int j = 0; j < c.nblk; ++j) {
+      const RingSlot<BWD_NST> s(j);
+      mbar_wait(Smem::full(0, s.st), s.ph);
+      const uint32_t ua = smem_u32(Smem::tile(0, s.st)), wa = smem_u32(Smem::tile(1, s.st));
+      const float* lse_tile = Smem::vec(0, s.st);
+      const float* delta_tile = Smem::vec(1, s.st);
+      float sc[ATT_COLS / 2], dp[ATT_COLS / 2];
       if (pingpong) named_bar_sync(1 + cw, 256);
       wgmma_fence();
 #pragma unroll
       for (int kk = 0; kk < KS; ++kk) {
         const uint32_t off = (kk & 3) * 32;
-        const uint32_t ro = (kk >> 2) * (BWD_ROWS * 128) + off, co = (kk >> 2) * (BWD_COLS * 128) + off;
-        Wgmma<BWD_COLS>::ss<0, 0>(sc, gmma_desc(xa + ro, 16, 1024), gmma_desc(ua + co, 16, 1024), kk > 0 ? 1u : 0u);
-        Wgmma<BWD_COLS>::ss<0, 0>(dp, gmma_desc(ya + ro, 16, 1024), gmma_desc(wa + co, 16, 1024), kk > 0 ? 1u : 0u);
+        const uint32_t ro = (kk >> 2) * (ATT_ROWS * 128) + off, co = (kk >> 2) * (ATT_COLS * 128) + off;
+        Wgmma<ATT_COLS>::ss<0, 0>(sc, gmma_desc(xa + ro, 16, 1024), gmma_desc(ua + co, 16, 1024), kk > 0 ? 1u : 0u);
+        Wgmma<ATT_COLS>::ss<0, 0>(dp, gmma_desc(ya + ro, 16, 1024), gmma_desc(wa + co, 16, 1024), kk > 0 ? 1u : 0u);
       }
       wgmma_commit();
       // Hand the turn over; warpgroup 1 skips its last hand-over, which no one would wait for.
-      if (pingpong && !(cw == 1 && j == nblk - 1)) named_bar_arrive(2 - cw, 256);
+      if (pingpong && !(cw == 1 && j == c.nblk - 1)) named_bar_arrive(2 - cw, 256);
       wgmma_wait<0>();
-      wgmma_reg_fence(sc, BWD_COLS / 2);
-      wgmma_reg_fence(dp, BWD_COLS / 2);
+      wgmma_reg_fence(sc, ATT_COLS / 2);
+      wgmma_reg_fence(dp, ATT_COLS / 2);
 
       // P and dS in place of S and dP.  Columns beyond the sequence get P = 0.
 #pragma unroll
-      for (int i = 0; i < BWD_COLS / 2; ++i) {
-        const int c = 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
+      for (int i = 0; i < ATT_COLS / 2; ++i) {
+        const int col = 8 * (i >> 2) + 2 * (c.lane & 3) + (i & 1);
         float lse, dl;
-        if (MODE == 1) { lse = sLse[st * BWD_COLS + c]; dl = sDelta[st * BWD_COLS + c]; }
+        if (MODE == 1) { lse = lse_tile[col]; dl = delta_tile[col]; }
         else { lse = row_lse[(i >> 1) & 1]; dl = row_delta[(i >> 1) & 1]; }
-        const float pv = j * BWD_COLS + c < p.n ? exp2f(fmaf(sc[i], p.sc_log2, -lse)) : 0.f;
+        const float pv = j * ATT_COLS + col < p.n ? exp2f(fmaf(sc[i], p.sc_log2, -lse)) : 0.f;
         sc[i] = pv;
         dp[i] = pv * (dp[i] - dl) * p.scale;
       }
       // Every A fragment is built before the fence: no register an in-flight wgmma reads is written after it.
-      uint32_t pf[MODE == 1 ? BWD_COLS / 16 : 1][4], sf[BWD_COLS / 16][4];
+      uint32_t pf[MODE == 1 ? ATT_COLS / 16 : 1][4], sf[ATT_COLS / 16][4];
 #pragma unroll
-      for (int kk = 0; kk < BWD_COLS / 16; ++kk) {
+      for (int kk = 0; kk < ATT_COLS / 16; ++kk) {
         if (MODE == 1) acc_to_a_frag(sc, kk, pf[kk]);
         acc_to_a_frag(dp, kk, sf[kk]);
       }
       wgmma_fence();
 #pragma unroll
-      for (int kk = 0; kk < BWD_COLS / 16; ++kk) {
+      for (int kk = 0; kk < ATT_COLS / 16; ++kk) {
         if (MODE == 1) {
-          Wgmma<NO>::rs<1>(acc1, pf[kk], gmma_desc(wa + kk * 2048, BWD_COLS * 128, 1024), 1u);   // dV += P^T dO
-          Wgmma<NO>::rs<1>(acc2, sf[kk], gmma_desc(ua + kk * 2048, BWD_COLS * 128, 1024), 1u);   // dK += dS^T Q
+          Wgmma<NO>::rs<1>(acc1, pf[kk], gmma_desc(wa + kk * 2048, ATT_COLS * 128, 1024), 1u);   // dV += P^T dO
+          Wgmma<NO>::rs<1>(acc2, sf[kk], gmma_desc(ua + kk * 2048, ATT_COLS * 128, 1024), 1u);   // dK += dS^T Q
         } else {
-          Wgmma<NO>::rs<1>(acc1, sf[kk], gmma_desc(ua + kk * 2048, BWD_COLS * 128, 1024), 1u);   // dQ += dS K
+          Wgmma<NO>::rs<1>(acc1, sf[kk], gmma_desc(ua + kk * 2048, ATT_COLS * 128, 1024), 1u);   // dQ += dS K
         }
       }
       wgmma_commit();
       wgmma_wait<0>();
       wgmma_reg_fence(acc1, NO / 2);
       if (MODE == 1) wgmma_reg_fence(acc2, NO / 2);
-      if (signal) mbar_arrive(&empty[st]);
+      if (c.signal) mbar_arrive(Smem::empty(0, s.st));
     }
 
-#pragma unroll
-    for (int r = 0; r < 2; ++r) {
-      const int row = r0 + rloc + 8 * r;
-      if (row >= p.n) continue;
-      __nv_bfloat16* o1 = p.out1 + (static_cast<long>(b) * p.n + row) * p.ld1 + h * p.d;
-      __nv_bfloat16* o2 = MODE == 1 ? p.out2 + (static_cast<long>(b) * p.n + row) * p.ld2 + h * p.d : nullptr;
-#pragma unroll
-      for (int jn = 0; jn < NO / 8; ++jn) {
-        const int c = 8 * jn + 2 * (lane & 3);
-        if (c < p.d) {
-          *reinterpret_cast<uint32_t*>(o1 + c) = pack_bf16(acc1[4 * jn + 2 * r], acc1[4 * jn + 2 * r + 1]);
-          if (MODE == 1)
-            *reinterpret_cast<uint32_t*>(o2 + c) = pack_bf16(acc2[4 * jn + 2 * r], acc2[4 * jn + 2 * r + 1]);
-        }
-      }
-    }
-  }
-}
-
-template <int MODE, int KA, int NO, int KS>
-static int launch_attn_bwd(const CUtensorMap& tx, const CUtensorMap& ty, const CUtensorMap& tu,
-                           const CUtensorMap& tw, const AttnBwdParams& p, cudaStream_t stream) {
-  constexpr int SMEM = 2 * KA * BWD_ROWS * 128 + 2 * BWD_NST * KA * BWD_COLS * 128 + 2 * BWD_NST * BWD_COLS * 4 + 128;
-  static_assert(SMEM <= 227 * 1024, "attention backward: shared-memory budget");
-  auto kern = attn_bwd_kernel<MODE, KA, NO, KS>;
-  if (int rc = raise_smem_limit<attn_bwd_kernel<MODE, KA, NO, KS>>(SMEM, "cudaFuncSetAttribute(attn_bwd)")) return rc;
-  dim3 grid((p.n + BWD_ROWS - 1) / BWD_ROWS, p.H, p.B);
-  cudaError_t le = launch_pdl(kern, grid, dim3(384), SMEM, stream, tx, ty, tu, tw, p);
-  if (le != cudaSuccess) return set_error_cuda("launch(attn_bwd_kernel)", le);
-  count_launch();
-  return check_launch("attn_bwd_kernel");
-}
-
-// A head_dim with accumulate width NO needs NO/16 or NO/16 - 1 k16 steps.
-template <int MODE, int KA, int NO>
-static int dispatch_bwd_ks(int d, const CUtensorMap& tx, const CUtensorMap& ty, const CUtensorMap& tu,
-                           const CUtensorMap& tw, const AttnBwdParams& p, cudaStream_t stream) {
-  if ((d + 15) / 16 == NO / 16) return launch_attn_bwd<MODE, KA, NO, NO / 16>(tx, ty, tu, tw, p, stream);
-  return launch_attn_bwd<MODE, KA, NO, NO / 16 - 1>(tx, ty, tu, tw, p, stream);
-}
-
-template <int MODE>
-static int dispatch_bwd(int d, const CUtensorMap& tx, const CUtensorMap& ty, const CUtensorMap& tu,
-                        const CUtensorMap& tw, const AttnBwdParams& p, cudaStream_t stream) {
-  const int no = (d + 31) / 32 * 32;
-  if (d <= 64) {
-    if (no <= 32) return dispatch_bwd_ks<MODE, 1, 32>(d, tx, ty, tu, tw, p, stream);
-    return dispatch_bwd_ks<MODE, 1, 64>(d, tx, ty, tu, tw, p, stream);
-  }
-  if (no <= 96) return dispatch_bwd_ks<MODE, 2, 96>(d, tx, ty, tu, tw, p, stream);
-  return dispatch_bwd_ks<MODE, 2, 128>(d, tx, ty, tu, tw, p, stream);
+    store_rows<NO>(acc1, p.out1, p.ld1, c, p.n, p.d);
+    if constexpr (MODE == 1) store_rows<NO>(acc2, p.out2, p.ld2, c, p.n, p.d);
+  });
 }
 
 }  // namespace ivb
@@ -289,7 +192,7 @@ using namespace ivb;
 
 // workspace (floats) needed by ivb_attn_bwd: padded lse2 + delta, [2][B][H][round_up(n,64)]
 extern "C" long ivb_attn_bwd_workspace_floats(int B, int n, int H) {
-  const long n_pad = (static_cast<long>(n) + BWD_COLS - 1) / BWD_COLS * BWD_COLS;
+  const long n_pad = (static_cast<long>(n) + ATT_COLS - 1) / ATT_COLS * ATT_COLS;
   return 2 * static_cast<long>(B) * H * n_pad;
 }
 
@@ -300,48 +203,41 @@ extern "C" int ivb_attn_bwd(const void* q, long ldq, const void* k, long ldk, co
                             float softmax_scale, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (B <= 0 || n <= 0) return 0;
-  if (d % 8 != 0 || d > 128 || d < 16) return set_error("ivb_attn_bwd: head_dim must be a multiple of 8 in [16,128]");
-  if ((ldq & 7) || (ldk & 7) || (ldv & 7) || (ldo & 7) || (lddo & 7) || (lddq & 7) || (lddk & 7) || (lddv & 7))
-    return set_error("ivb_attn_bwd: pitches must be multiples of 8");
+  int rc;
+  if ((rc = check_head_args("ivb_attn_bwd", d, {ldq, ldk, ldv, ldo, lddo, lddq, lddk, lddv}))) return rc;
   if (lse2 == nullptr || delta_ws == nullptr) return set_error("ivb_attn_bwd: lse2 and the workspace are required");
   if ((reinterpret_cast<uintptr_t>(delta_ws) & 15) != 0) return set_error("ivb_attn_bwd: workspace must be 16-byte aligned");
-  const int n_pad = (n + BWD_COLS - 1) / BWD_COLS * BWD_COLS;
+  const int n_pad = (n + ATT_COLS - 1) / ATT_COLS * ATT_COLS;
   const long half = static_cast<long>(B) * H * n_pad;
   float* lse2p = delta_ws;
   float* deltap = delta_ws + half;
-  {
-    cudaError_t e = cudaMemsetAsync(delta_ws, 0, 2 * half * sizeof(float), stream);   // zero padding (0 * pad must stay 0)
-    if (e != cudaSuccess) return set_error_cuda("cudaMemsetAsync(attn_bwd workspace)", e);
-    const long total = static_cast<long>(B) * n * H;
-    const int threads = 128;
-    attn_bwd_prep_kernel<<<(unsigned)((total + threads - 1) / threads), threads, 0, stream>>>(
-        reinterpret_cast<const __nv_bfloat16*>(out), ldo, reinterpret_cast<const __nv_bfloat16*>(dout),
-        lddo, lse2, lse2p, deltap, B, n, n_pad, H, d);
-    count_launch();
-    int rc = check_launch("attn_bwd_prep_kernel");
-    if (rc) return rc;
-  }
-  CUtensorMap tq128, tdo128, tk128, tv128, tq64, tdo64, tk64, tv64;
-  int rc;
-  if ((rc = make_head_tmap(&tq128, q, ldq, B, n, H, d, BWD_ROWS))) return rc;
-  if ((rc = make_head_tmap(&tdo128, dout, lddo, B, n, H, d, BWD_ROWS))) return rc;
-  if ((rc = make_head_tmap(&tk128, k, ldk, B, n, H, d, BWD_ROWS))) return rc;
-  if ((rc = make_head_tmap(&tv128, v, ldv, B, n, H, d, BWD_ROWS))) return rc;
-  if ((rc = make_head_tmap(&tq64, q, ldq, B, n, H, d, BWD_COLS))) return rc;
-  if ((rc = make_head_tmap(&tdo64, dout, lddo, B, n, H, d, BWD_COLS))) return rc;
-  if ((rc = make_head_tmap(&tk64, k, ldk, B, n, H, d, BWD_COLS))) return rc;
-  if ((rc = make_head_tmap(&tv64, v, ldv, B, n, H, d, BWD_COLS))) return rc;
-  AttnBwdParams p;
-  p.B = B; p.n = n; p.H = H; p.d = d; p.n_pad = n_pad;
-  p.scale = softmax_scale;
-  p.sc_log2 = softmax_scale * 1.4426950408889634f;
-  p.lse2p = lse2p; p.deltap = deltap;
-  // dK, dV
-  p.out1 = reinterpret_cast<__nv_bfloat16*>(dv); p.ld1 = lddv;
-  p.out2 = reinterpret_cast<__nv_bfloat16*>(dk); p.ld2 = lddk;
-  if ((rc = dispatch_bwd<1>(d, tk128, tv128, tq64, tdo64, p, stream))) return rc;
-  // dQ
-  p.out1 = reinterpret_cast<__nv_bfloat16*>(dq); p.ld1 = lddq;
-  p.out2 = nullptr; p.ld2 = 0;
-  return dispatch_bwd<0>(d, tq128, tdo128, tk64, tv64, p, stream);
+  if (cudaError_t e = cudaMemsetAsync(delta_ws, 0, 2 * half * sizeof(float), stream))   // zero padding (0 * pad must stay 0)
+    return set_error_cuda("cudaMemsetAsync(attn_bwd workspace)", e);
+  const long total = static_cast<long>(B) * n * H;
+  attn_bwd_prep_kernel<<<(unsigned)((total + 127) / 128), 128, 0, stream>>>(
+      reinterpret_cast<const __nv_bfloat16*>(out), ldo, reinterpret_cast<const __nv_bfloat16*>(dout),
+      lddo, lse2, lse2p, deltap, B, n, n_pad, H, d);
+  count_launch();
+  if ((rc = check_launch("attn_bwd_prep_kernel"))) return rc;
+  // q, dO, k, v, each with a 128-row box (the rows a CTA owns) and a 64-row box (a streamed tile)
+  const void* src[4] = {q, dout, k, v};
+  const long ld[4] = {ldq, lddo, ldk, ldv};
+  CUtensorMap rows[4], tiles[4];
+  for (int i = 0; i < 4; ++i)
+    if ((rc = make_head_tmap(&rows[i], src[i], ld[i], B, n, H, d, ATT_ROWS)) ||
+        (rc = make_head_tmap(&tiles[i], src[i], ld[i], B, n, H, d, ATT_COLS)))
+      return rc;
+  const float sc_log2 = softmax_scale * 1.4426950408889634f;
+  const auto bf = [](void* x) { return reinterpret_cast<__nv_bfloat16*>(x); };
+  const AttnBwdParams pkv{B, n, H, d, n_pad, sc_log2, softmax_scale, lse2p, deltap, bf(dv), lddv, bf(dk), lddk};
+  const AttnBwdParams pq{B, n, H, d, n_pad, sc_log2, softmax_scale, lse2p, deltap, bf(dq), lddq, nullptr, 0};
+  return dispatch_head_dim(d, [&](auto hd) {
+    constexpr int smem = BwdSmem<hd.KA>::BYTES;
+    const char* attr = "cudaFuncSetAttribute(attn_bwd)";
+    if ((rc = launch_attn<attn_bwd_kernel<1, hd.KA, hd.NO, hd.KS>, true>(attr, "attn_bwd_kernel", smem, B, n, H, stream,
+                                                                          rows[2], rows[3], tiles[0], tiles[1], pkv)))
+      return rc;
+    return launch_attn<attn_bwd_kernel<0, hd.KA, hd.NO, hd.KS>, true>(attr, "attn_bwd_kernel", smem, B, n, H, stream,
+                                                                       rows[0], rows[1], tiles[2], tiles[3], pq);
+  });
 }
