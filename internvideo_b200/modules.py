@@ -210,9 +210,6 @@ class Block(nn.Module):
     def forward_stream(self, x2d, B, n, rowscale=None):
         """fp32 residual stream [B*n, D] -> [B*n, D] (the hot path used by the model).
         rowscale: optional (rs1, rs2) fp32 [B*n] DropPath factors sampled by the caller for all blocks at once."""
-        a = self.attn
-        g1 = self.ls1.gamma if isinstance(self.ls1, LayerScale) else None
-        g2 = self.ls2.gamma if isinstance(self.ls2, LayerScale) else None
         rs1 = rs2 = None
         if rowscale is not None:
             rs1, rs2 = rowscale
@@ -223,29 +220,28 @@ class Block(nn.Module):
             rs2 = s2.repeat_interleave(n) if s2 is not None else None
         if not torch.is_grad_enabled():
             return self.forward_infer(x2d, B, n, (rs1, rs2))
-        if self.fp8_inference is not None:
-            raise ll._lib.IvbError("Block: FP8 inference mode (set_fp8_inference) has no gradient; switch it off to train")
-        return ops.BlockFn.apply(
-            x2d, (B, n, self.num_heads, self.mlp.gelu_tanh, self.with_cp, self.fp8), self.norm1.weight, a.qkv.weight, a.qkv.bias,
-            a.q_norm.weight if a.qk_normalization else None, a.k_norm.weight if a.qk_normalization else None,
-            a.proj.weight, a.proj.bias, g1, self.norm2.weight, self.mlp.fc1.weight, self.mlp.fc1.bias,
-            self.mlp.fc2.weight, self.mlp.fc2.bias, g2, rs1, rs2)
+        return ops.BlockFn.apply(x2d, self._spec(B, n, training=True), rs1, rs2, *self._param_tuple())
+
+    def _spec(self, B, n, training):
+        return ops.BlockSpec(B, n, self.num_heads, self.mlp.gelu_tanh, eps1=self.norm1.variance_epsilon,
+                             eps2=self.norm2.variance_epsilon, checkpoint=self.with_cp,
+                             precision=block_precision(self, training))
 
     def _param_tuple(self):
         a = self.attn
-        g1 = self.ls1.gamma if isinstance(self.ls1, LayerScale) else None
-        g2 = self.ls2.gamma if isinstance(self.ls2, LayerScale) else None
-        return (self.norm1.weight, a.qkv.weight, a.qkv.bias,
-                a.q_norm.weight if a.qk_normalization else None, a.k_norm.weight if a.qk_normalization else None,
-                a.proj.weight, a.proj.bias, g1, self.norm2.weight, self.mlp.fc1.weight, self.mlp.fc1.bias,
-                self.mlp.fc2.weight, self.mlp.fc2.bias, g2)
+        return ops.BlockParams(
+            n1w=self.norm1.weight, qkvw=a.qkv.weight, qkvb=a.qkv.bias,
+            qnw=a.q_norm.weight if a.qk_normalization else None, knw=a.k_norm.weight if a.qk_normalization else None,
+            projw=a.proj.weight, projb=a.proj.bias, g1=self.ls1.gamma if isinstance(self.ls1, LayerScale) else None,
+            n2w=self.norm2.weight, fc1w=self.mlp.fc1.weight, fc1b=self.mlp.fc1.bias, fc2w=self.mlp.fc2.weight,
+            fc2b=self.mlp.fc2.bias, g2=self.ls2.gamma if isinstance(self.ls2, LayerScale) else None)
 
     def forward_infer(self, x2d, B, n, rowscale=(None, None)):
-        """No-grad form (frozen towers / teachers): 14 kernels, nothing saved, no GELU' / pre-LayerScale copies."""
+        """No-grad form (frozen towers / teachers): ops.block_forward with nothing saved, no GELU' / pre-LayerScale
+        copies."""
         with torch.no_grad():
-            out, _ = ops.block_forward(x2d, (B, n, self.num_heads, self.mlp.gelu_tanh, False, self.fp8),
-                                       self._param_tuple(), rowscale[0], rowscale[1], save=False,
-                                       fp8_weights=fp8_inference_weights(self))
+            out, _ = ops.block_forward(x2d, self._spec(B, n, training=False), self._param_tuple(), rowscale[0],
+                                       rowscale[1], save=False)
         return out
 
     def _fp8_linears(self):
@@ -299,11 +295,15 @@ class Fp8InferenceWeights:
         return tuple(self.copies)
 
 
-def fp8_inference_weights(block):
-    """The FP8 weight copies a no-grad forward of `block` (Block or teachers.TeacherBlock) runs with, or None."""
+def block_precision(block, training=False):
+    """The ops.BlockSpec precision a forward of `block` (Block or teachers.TeacherBlock) runs at, from its switches:
+    set_fp8 (Block.fp8) and set_fp8_inference (fp8_inference).  training: the forward needs a gradient."""
+    fp8 = getattr(block, "fp8", False)
     if block.fp8_inference is None:
-        return None
-    if getattr(block, "fp8", False):
+        return ops.FP8_TENSOR if fp8 else ops.BF16
+    if training:
+        raise ll._lib.IvbError("Block: FP8 inference mode (set_fp8_inference) has no gradient; switch it off to train")
+    if fp8:
         raise ll._lib.IvbError("FP8 inference (set_fp8_inference) and FP8 training (set_fp8) are both on for a block")
     return block.fp8_inference.get()
 

@@ -7,6 +7,9 @@ DeepSpeed mode converts the whole model: engines/engine_for_pretraining.py:128, 
 """
 from __future__ import annotations
 
+from collections import namedtuple
+from typing import NamedTuple
+
 import torch
 
 from . import lowlevel as ll
@@ -194,159 +197,135 @@ class PoolAttnFn(torch.autograd.Function):
 
 
 # ------------------------------------------------------------------------------------------ fused ViT block
-def _block_fp8(dims):
-    """dims = (B, n, H, gelu_tanh[, checkpoint[, fp8]]): the block's FP8 mode (modules.set_fp8)."""
-    return len(dims) > 5 and bool(dims[5])
+# A block's precision (BlockSpec.precision): BF16; FP8_TENSOR, FP8 with per-tensor scales and the weights cast in the
+# call (modules.set_fp8); or per-token FP8 (modules.set_fp8_inference, no-grad calls only), given as the four weights'
+# per-channel E4M3 copies themselves: ((q, scale_inv) for qkv, proj, fc1, fc2).
+BF16, FP8_TENSOR = "bf16", "fp8"
 
 
-def _fp8_linear(act, w8, **epilogue):
-    """act (bf16) cast to FP8 with its own scale, times an FP8 weight copy w8 = (q, scale_inv), fused epilogue."""
-    q, _, s, _ = ll.fp8_quantize(act, ll.FP8_E4M3)
-    return ll.gemm_fp8(q, s, w8[0], w8[1], **epilogue)
+class BlockSpec(NamedTuple):
+    """Everything a fused block call needs besides its tensors.  layernorm: the VideoMAEv2 teacher's LayerNorm block
+    (inference only) instead of the RMSNorm block; eps1 / eps2 are the eps of its two norms.  scale: the attention scale
+    (None: d ** -0.5).  head_axis: the VideoMAEv2 teacher's attention over the heads of each token (inference only).
+    checkpoint: BlockFn keeps only the block input and recomputes the forward in the backward."""
+    B: int
+    n: int
+    H: int
+    gelu_tanh: bool = False
+    layernorm: bool = False
+    eps1: float = 1e-6
+    eps2: float = 1e-6
+    scale: float | None = None
+    head_axis: bool = False
+    checkpoint: bool = False
+    precision: object = BF16
+
+    def attn_scale(self, d):
+        return d ** -0.5 if self.scale is None else self.scale
+
+    def gelu_flags(self, save):
+        """fc1's epilogue flags; with save, h holds gelu'(pre-activation), the only thing the backward needs of it."""
+        return (ll.FLAG_GELU_TANH if self.gelu_tanh else 0) | (ll.FLAG_GELU_SAVE_GRAD if save else 0)
 
 
-def _fp8_dgrad(dy, wt8, ws, **epilogue):
-    """dx = dy W with dy cast to E5M2 and wt8 the E4M3 copy of W^T (scale_inv ws)."""
-    q, _, s, _ = ll.fp8_quantize(dy, ll.FP8_E5M2)
-    return ll.gemm_fp8(q, s, wt8, ws, **epilogue)
+# A block's tensors.  qkvb, qnw / knw (q/k norms) and g1 / g2 (LayerScale) may be None; n1b / n2b are the LayerNorm
+# biases, None on RMSNorm blocks.
+BlockParams = namedtuple("BlockParams", "n1w qkvw qkvb qnw knw projw projb g1 n2w fc1w fc1b fc2w fc2b g2 n1b n2b",
+                         defaults=(None, None))
+
+# What block_forward(save=True) keeps for block_backward: activations and norm statistics, and in FP8_TENSOR the E4M3
+# copies of the four weights' transposes with their scales (the input-gradient GEMMs' operands; None in bf16).
+BlockSaved = namedtuple("BlockSaved", "n1 qkv qkn a lse rstd1 rq rk x1 y1 n2 rstd2 h g y2 "
+                                      "qkvw_t qkvw_s projw_t projw_s fc1w_t fc1w_s fc2w_t fc2w_s")
 
 
-def _rowwise_linear(act, w8, **epilogue):
-    """FP8 inference GEMM with per-row activation and per-output-channel weight scales.  act: a bf16 activation (cast
-    row by row here) or the (E4M3 rows, scale_inv) pair norm_fwd_fp8 wrote; w8 = (E4M3 weight, scale_inv)."""
-    q, s = ll.fp8_quantize_rows(act) if torch.is_tensor(act) else act
-    return ll.gemm_fp8(q, s, w8[0], w8[1], **epilogue)
+def block_forward(x, spec, p, rs1=None, rs2=None, save=True):
+    """One pre-norm ViT block over the fp32 residual stream [B*n, D]: spec a BlockSpec, p the BlockParams.  The
+    InternVideo2 block (Block.forward, internvideo2_pretrain.py:279-297), or with spec.layernorm the VideoMAEv2 teacher
+    block (videomae.py:104-132: LayerNorm with bias, q/v bias on qkv, no q/k norm, erf GELU):
 
-
-def block_forward(x, dims, params, rs1=None, rs2=None, save=True, fp8_weights=None):
-    """One spatio-temporal ViT block over the fp32 residual stream [B*n, D] (Block.forward,
-    internvideo2_pretrain.py:279-297):
-
-      n1 = RMSNorm(x) ; qkv = n1 Wqkv^T ; (q,k) = RMSNorm_C(q), RMSNorm_C(k) ; a = attn(q,k,v)
+      n1 = Norm(x) ; qkv = n1 Wqkv^T + bqkv ; (q,k) = RMSNorm_C(q), RMSNorm_C(k) ; a = attn(q,k,v)
       x1 = x + rs1 * g1 * (a Wp^T + bp)                [LayerScale + DropPath + residual fused in the GEMM epilogue]
-      n2 = RMSNorm(x1) ; h = n2 W1^T + b1 ; g = GELU(h) [fused epilogue] ; x2 = x1 + rs2 * g2 * (g W2^T + b2)
+      n2 = Norm(x1) ; h = n2 W1^T + b1 ; g = GELU(h) [fused epilogue] ; x2 = x1 + rs2 * g2 * (g W2^T + b2)
 
-    14 kernels.  save=True also writes what the backward needs (pre-LayerScale branch outputs, GELU') and returns
-    it; save=False is the inference / recompute-later form (frozen towers, activation checkpointing): nothing
-    extra is written.  Returns (x2, saved | None).
+    In bf16, 7 library calls, and 1 more for the q/k norms (2 when D > 1536).  save=True also writes what the backward
+    needs (pre-LayerScale branch outputs, GELU') and returns it; save=False is the inference / recompute-later form
+    (frozen towers, teachers, activation checkpointing): nothing extra is written.  Returns (x2, BlockSaved | None).
 
-    FP8 mode (dims[5]): the four weights are cast to E4M3 (with save, also transposed, for the backward's dgrad) and
-    n1, a, n2 and g before their GEMM, each with its own per-tensor scale; the GEMMs keep their fused epilogues.
-
-    FP8 inference (fp8_weights, save=False only): fp8_weights holds the E4M3 copies of the four weights with one scale
-    per output channel ((q, scale_inv) for qkv, proj, fc1, fc2; modules.set_fp8_inference).  n1 and n2 come out of
-    the norm kernel as E4M3 rows with per-row scales, a and g are cast row by row, and the four GEMMs apply row and
-    column scales before their fused epilogues.  Attention, the q/k norms and the residual stream stay as above."""
-    B, n, H, gelu_tanh = dims[:4]
-    n1w, qkvw, qkvb, qnw, knw, projw, projb, g1, n2w, fc1w, fc1b, fc2w, fc2b, g2 = params
+    FP8_TENSOR (8 more calls): the four weights are cast to E4M3 (with save, also transposed, for the backward's dgrad)
+    and n1, a, n2 and g before their GEMM, each with its own per-tensor scale; the GEMMs keep their fused epilogues.
+    Per-token FP8 (save=False only; 2 more calls): n1 and n2 come out of the norm kernel as E4M3 rows with per-row
+    scales, a and g are cast row by row, and the four GEMMs apply row and column scales before their fused epilogues.
+    Attention, the q/k norms and the residual stream stay as above."""
+    B, n, H = spec.B, spec.n, spec.H
     M, D = x.shape
     d = D // H
     if x.dtype != f32 or not x.is_cuda:
         raise ll._lib.IvbError("block_forward: residual stream must be a CUDA fp32 tensor [B*n, D]")
+    prec = spec.precision
+    per_token = not isinstance(prec, str)
     w8 = None
-    if fp8_weights is not None:
-        if save or _block_fp8(dims):
-            raise ll._lib.IvbError("block_forward: FP8 inference is a no-grad form and excludes the FP8 training mode")
-    elif _block_fp8(dims):
+    if prec == FP8_TENSOR:
         # (q, q_t, scale_inv) per weight; q_t only when the backward will need it
-        w8 = [ll.fp8_quantize(w, ll.FP8_E4M3, transpose=save)[:3] for w in (qkvw, projw, fc1w, fc2w)]
+        w8 = [ll.fp8_quantize(w, ll.FP8_E4M3, transpose=save)[:3] for w in (p.qkvw, p.projw, p.fc1w, p.fc2w)]
 
-    def norm(t, w):   # n1, n2 (and rstd for the backward)
-        if fp8_weights is not None:
-            return ll.norm_fwd_fp8(t, w), None
-        y, _, rstd = ll.norm_fwd(t, w, want_stats=save)
+    def norm(t, w, b, eps):   # n1, n2 (and rstd for the backward)
+        if per_token:
+            return ll.norm_fwd_fp8(t, w, b, eps=eps, layernorm=spec.layernorm), None
+        y, _, rstd = ll.norm_fwd(t, w, b, eps=eps, layernorm=spec.layernorm, want_stats=save)
         return y, rstd
 
     def linear(act, i, w, **epilogue):
-        if fp8_weights is not None:
-            return _rowwise_linear(act, fp8_weights[i], **epilogue)
-        if w8 is None:
+        if prec == BF16:
             return ll.gemm(act, w, **epilogue)
-        return _fp8_linear(act, (w8[i][0], w8[i][2]), **epilogue)
-    n1, rstd1 = norm(x, n1w)
-    qkv = linear(n1, 0, qkvw, bias=qkvb)
-    rq = rk = None
-    if qnw is not None:
+        if per_token:     # act: bf16, or the (E4M3 rows, scale_inv) pair norm_fwd_fp8 wrote
+            q, s = ll.fp8_quantize_rows(act) if torch.is_tensor(act) else act
+            wq, ws = prec[i]
+        else:
+            q, _, s, _ = ll.fp8_quantize(act, ll.FP8_E4M3)
+            wq, _, ws = w8[i]
+        return ll.gemm_fp8(q, s, wq, ws, **epilogue)
+    n1, rstd1 = norm(x, p.n1w, p.n1b, spec.eps1)
+    qkv = linear(n1, 0, p.qkvw, bias=p.qkvb)
+    q, k, v = qkv[:, :D], qkv[:, D:2 * D], qkv[:, 2 * D:]
+    qkn = rq = rk = lse = None
+    if p.qnw is not None:
         qkn = torch.empty((M, 2 * D), device=x.device, dtype=bf16)
         if D <= 1536:      # q-norm and k-norm in ONE launch; rq holds rstd [M, 2] for both
-            rq = ll.rmsnorm_pair_fwd(qkv, D, qnw, knw, qkn, want_stats=save)
+            rq = ll.rmsnorm_pair_fwd(qkv, D, p.qnw, p.knw, qkn, want_stats=save)
         else:
-            _, _, rq = ll.norm_fwd(qkv[:, :D], qnw, out=qkn[:, :D], want_stats=save)
-            _, _, rk = ll.norm_fwd(qkv[:, D:2 * D], knw, out=qkn[:, D:], want_stats=save)
+            _, _, rq = ll.norm_fwd(q, p.qnw, out=qkn[:, :D], want_stats=save)
+            _, _, rk = ll.norm_fwd(k, p.knw, out=qkn[:, D:], want_stats=save)
         q, k = qkn[:, :D], qkn[:, D:]
+    if spec.head_axis:
+        # the reference's call (videomae.py:94-97) attends over the heads of each token and reinterprets the
+        # [B, H, N, d] result as [B, N, H*d]: reproduced bit-for-layout
+        a = ll.headaxis_attn_fwd(qkv, B, n, H, d, spec.attn_scale(d)).reshape(M, D)
     else:
-        qkn = None
-        q, k = qkv[:, :D], qkv[:, D:2 * D]
-    a, lse = ll.attn_fwd(q, k, qkv[:, 2 * D:], B, n, H, d, d ** -0.5, want_lse=save)
-    y1 = torch.empty((M, D), device=x.device, dtype=bf16) if (g1 is not None and save) else None
-    x1 = linear(a, 1, projw, epi=ll.EPI_RESID, bias=projb, gamma=g1, aux=x, out1=y1, rowscale=rs1)
-    n2, rstd2 = norm(x1, n2w)
-    Hd = fc1w.shape[0]
-    flags = ll.FLAG_GELU_TANH if gelu_tanh else 0
-    h = None
-    if save:
-        # h holds gelu'(pre-activation): the only thing the backward needs of it (FLAG_GELU_SAVE_GRAD)
-        h = torch.empty((M, Hd), device=x.device, dtype=bf16)
-        flags |= ll.FLAG_GELU_SAVE_GRAD
-    g = linear(n2, 2, fc1w, epi=ll.EPI_BIAS_GELU, flags=flags, bias=fc1b, out1=h)
-    y2 = torch.empty((M, D), device=x.device, dtype=bf16) if (g2 is not None and save) else None
-    x2 = linear(g, 3, fc2w, epi=ll.EPI_RESID, bias=fc2b, gamma=g2, aux=x1, out1=y2, rowscale=rs2)
+        a, lse = ll.attn_fwd(q, k, v, B, n, H, d, spec.attn_scale(d), want_lse=save)
+    y1 = torch.empty((M, D), device=x.device, dtype=bf16) if (p.g1 is not None and save) else None
+    x1 = linear(a, 1, p.projw, epi=ll.EPI_RESID, bias=p.projb, gamma=p.g1, aux=x, out1=y1, rowscale=rs1)
+    n2, rstd2 = norm(x1, p.n2w, p.n2b, spec.eps2)
+    h = torch.empty((M, p.fc1w.shape[0]), device=x.device, dtype=bf16) if save else None
+    g = linear(n2, 2, p.fc1w, epi=ll.EPI_BIAS_GELU, flags=spec.gelu_flags(save), bias=p.fc1b, out1=h)
+    y2 = torch.empty((M, D), device=x.device, dtype=bf16) if (p.g2 is not None and save) else None
+    x2 = linear(g, 3, p.fc2w, epi=ll.EPI_RESID, bias=p.fc2b, gamma=p.g2, aux=x1, out1=y2, rowscale=rs2)
     if not save:
         return x2, None
-    # the E4M3 copies of W^T and their scales (None without FP8): the dgrad operands of the backward
-    wt8 = tuple(t for q, q_t, s in w8 for t in (q_t, s)) if w8 is not None else (None,) * 8
-    return x2, (n1, qkv, qkn, a, lse, rstd1, rq, rk, x1, y1, n2, rstd2, h, g, y2) + wt8 + (flags,)
+    wt8 = [t for _, q_t, s in w8 for t in (q_t, s)] if w8 is not None else [None] * 8
+    return x2, BlockSaved(n1, qkv, qkn, a, lse, rstd1, rq, rk, x1, y1, n2, rstd2, h, g, y2, *wt8)
 
 
-def block_forward_ln_infer(x, B, n, H, scale, params, head_axis_attention=False, fp8_weights=None):
-    """Inference-only LayerNorm pre-norm block of the VideoMAEv2 teacher (videomae.py:104-132; attention with q/v
-    bias :62-101, erf GELU, optional gamma_1/gamma_2) over the fp32 residual stream [B*n, D]: 9 kernels,
-    LayerScale + residual fused in the GEMM epilogues, nothing saved.  params = (n1w, n1b, eps1, qkvw, qkvb, projw,
-    projb, g1, n2w, n2b, eps2, fc1w, fc1b, fc2w, fc2b, g2).  head_axis_attention=True reproduces the reference's
-    flash_attn_func call on [B,H,N,d] tensors (softmax over the heads of each token); False is token-axis attention.
-    fp8_weights: FP8 inference as in block_forward (the two LayerNorms write E4M3 rows with per-row scales)."""
-    n1w, n1b, eps1, qkvw, qkvb, projw, projb, g1, n2w, n2b, eps2, fc1w, fc1b, fc2w, fc2b, g2 = params
+def block_backward(x, s, spec, t, P, dx2, rs1, rs2):
+    """Backward of block_forward(save=True) for the RMSNorm block, from its BlockSaved s: 13 to 17 library calls in bf16
+    (with or without the q/k norms and the qkv bias, the fused norm2 + LayerScale backward), and in FP8_TENSOR one more
+    per input-gradient GEMM (the E5M2 cast of its gradient).  `t` are the block's tensors as autograd handed them back,
+    `P` the nn.Parameter objects (gradient sink), both BlockParams.  Returns (dx0, BlockParams of gradients | None when
+    the sink took them)."""
+    B, n, H = spec.B, spec.n, spec.H
     M, D = x.shape
     d = D // H
-    if x.dtype != f32 or not x.is_cuda:
-        raise ll._lib.IvbError("block_forward_ln_infer: residual stream must be a CUDA fp32 tensor [B*n, D]")
-    if fp8_weights is not None:
-        def norm(t, w, b, eps):
-            return ll.norm_fwd_fp8(t, w, b, eps=eps, layernorm=True)
-
-        def linear(act, i, w, **epilogue):
-            return _rowwise_linear(act, fp8_weights[i], **epilogue)
-    else:
-        def norm(t, w, b, eps):
-            return ll.norm_fwd(t, w, b, eps=eps, layernorm=True, want_stats=False)[0]
-
-        def linear(act, i, w, **epilogue):
-            return ll.gemm(act, w, **epilogue)
-    with torch.no_grad():
-        n1 = norm(x, n1w, n1b, eps1)
-        qkv = linear(n1, 0, qkvw, bias=qkvb)
-        if head_axis_attention:
-            # the reference's call (videomae.py:94-97) attends over the heads of each token and reinterprets the
-            # [B, H, N, d] result as [B, N, H*d]: reproduced bit-for-layout
-            a = ll.headaxis_attn_fwd(qkv, B, n, H, d, scale).reshape(M, D)
-        else:
-            a, _ = ll.attn_fwd(qkv[:, :D], qkv[:, D:2 * D], qkv[:, 2 * D:], B, n, H, d, scale, want_lse=False)
-        x1 = linear(a, 1, projw, epi=ll.EPI_RESID, bias=projb, gamma=g1, aux=x)
-        n2 = norm(x1, n2w, n2b, eps2)
-        g = linear(n2, 2, fc1w, epi=ll.EPI_BIAS_GELU, bias=fc1b)
-        return linear(g, 3, fc2w, epi=ll.EPI_RESID, bias=fc2b, gamma=g2, aux=x1)
-
-
-def block_backward(x, saved, dims, tensors, P, dx2, rs1, rs2):
-    """Backward of block_forward: 26 kernels.  `tensors` are the parameter tensors as autograd handed them back,
-    `P` the nn.Parameter objects (gradient sink).  Returns (dx0, per-parameter gradients | None when the sink took them)."""
-    n1, qkv, qkn, a, lse, rstd1, rq, rk, x1, y1, n2, rstd2, h, g, y2 = saved[:15]
-    wt8, flags = saved[15:23], saved[23]
-    n1w, qkvw, qkvb, qnw, knw, projw, projb, g1, n2w, fc1w, fc1b, fc2w, fc2b, g2 = tensors
-    B, n, H = dims[:3]
-    M, D = x.shape
-    d = D // H
-    Hd = fc1w.shape[0]
+    Hd = t.fc1w.shape[0]
     dx2 = dx2.contiguous()
     if dx2.dtype != f32:
         dx2 = dx2.float()
@@ -355,19 +334,18 @@ def block_backward(x, saved, dims, tensors, P, dx2, rs1, rs2):
     # O(D) gradients land with ONE fused add per block — no autograd AccumulateGrad kernels (16 per
     # block, each re-reading and re-writing the gradient).
     sink = _common_sink(P)
-    small = (("g2", g2, D), ("fc2b", fc2b, D), ("n2w", n2w, D), ("g1", g1, D), ("projb", projb, D),
-             ("qnw", qnw, D), ("knw", knw, D), ("n1w", n1w, D), ("fc1b", fc1b, Hd), ("qkvb", qkvb, 3 * D))
-    seg, vec, span, base = _plan_small(small, P, sink, x.device)
+    small = [(nm, getattr(t, nm), D) for nm in ("g2", "fc2b", "n2w", "g1", "projb", "qnw", "knw", "n1w")]
+    small += [("fc1b", t.fc1b, Hd), ("qkvb", t.qkvb, 3 * D)]
+    seg, vec, span, base = _plan_small(small, sink, x.device)
     if sink is not None and span is None:
         sink = None           # small parameters not contiguous in the flat buffer: autograd path
     dg2, dcs2, dn2w, dg1, dcs1 = seg["g2"], seg["fc2b"], seg["n2w"], seg["g1"], seg["projb"]
-    dqnw, dknw, dn1w, dfc1b, dqkvb = seg["qnw"], seg["knw"], seg["n1w"], seg["fc1b"], seg["qkvb"]
-    pn1w, pqkvw, pqkvb, pqnw, pknw, pprojw, pprojb, pg1, pn2w, pfc1w, pfc1b, pfc2w, pfc2b, pg2 = P
 
-    def dgrad(dy, i, w, **epilogue):   # dx = dy W; in FP8 mode on the E5M2 gradient and the E4M3 copy of W^T
-        if wt8[2 * i] is None:
+    def dgrad(dy, w, w_t, w_s, **epilogue):   # dx = dy W; in FP8_TENSOR on the E5M2 gradient and the E4M3 copy of W^T
+        if spec.precision != FP8_TENSOR:
             return ll.gemm(dy, w, b_t=True, **epilogue)
-        return _fp8_dgrad(dy, wt8[2 * i], wt8[2 * i + 1], **epilogue)
+        q, _, sc, _ = ll.fp8_quantize(dy, ll.FP8_E5M2)
+        return ll.gemm_fp8(q, sc, w_t, w_s, **epilogue)
 
     def wgrad(dy, act, param):
         if sink is None:
@@ -376,94 +354,79 @@ def block_backward(x, saved, dims, tensors, P, dx2, rs1, rs2):
         sink.grad_written(param)
         return None
     # ---- MLP branch
-    dy2 = ll.layerscale_bwd(dx2, y2, g2, dg2 if g2 is not None else None, dcs2, rowscale=rs2)
-    dfc2w = wgrad(dy2, g, pfc2w)
-    dh = dgrad(dy2, 3, fc2w, epi=ll.EPI_GELU_BWD, flags=flags, aux=h)
-    ll.colsum(dh, out=dfc1b)
-    dfc1w = wgrad(dh, n2, pfc1w)
-    dn2 = dgrad(dh, 2, fc1w)
+    dy2 = ll.layerscale_bwd(dx2, s.y2, t.g2, dg2 if t.g2 is not None else None, dcs2, rowscale=rs2)
+    dfc2w = wgrad(dy2, s.g, P.fc2w)
+    dh = dgrad(dy2, t.fc2w, s.fc2w_t, s.fc2w_s, epi=ll.EPI_GELU_BWD, flags=spec.gelu_flags(True), aux=s.h)
+    ll.colsum(dh, out=seg["fc1b"])
+    dfc1w = wgrad(dh, s.n2, P.fc1w)
+    dn2 = dgrad(dh, t.fc1w, s.fc1w_t, s.fc1w_s)
     # ---- attention branch
-    if g1 is not None and D <= 1536 and M >= 1024:
+    if t.g1 is not None and D <= 1536 and M >= 1024:
         # norm2 backward fused with the attention branch's LayerScale backward: the gradient of the residual
         # stream is produced and consumed in one pass over the rows
-        dx1, dy1 = ll.rmsnorm_bwd_layerscale(dn2, x1, n2w, rstd2, dx2, y1, g1, dn2w, dg1, dcs1, rowscale=rs1)
+        dx1, dy1 = ll.rmsnorm_bwd_layerscale(dn2, s.x1, t.n2w, s.rstd2, dx2, s.y1, t.g1, dn2w, dg1, dcs1, rowscale=rs1)
     else:
-        dx1 = ll.norm_bwd(dn2, x1, n2w, None, rstd2, dx_in=dx2, dweight=dn2w)
-        dy1 = ll.layerscale_bwd(dx1, y1, g1, dg1 if g1 is not None else None, dcs1, rowscale=rs1)
-    dprojw = wgrad(dy1, a, pprojw)
-    da = dgrad(dy1, 1, projw)
+        dx1 = ll.norm_bwd(dn2, s.x1, t.n2w, None, s.rstd2, dx_in=dx2, dweight=dn2w)
+        dy1 = ll.layerscale_bwd(dx1, s.y1, t.g1, dg1 if t.g1 is not None else None, dcs1, rowscale=rs1)
+    dprojw = wgrad(dy1, s.a, P.projw)
+    da = dgrad(dy1, t.projw, s.projw_t, s.projw_s)
     dqkv = torch.empty((M, 3 * D), device=x.device, dtype=bf16)
-    if qkn is not None:
-        q, k = qkn[:, :D], qkn[:, D:]
-    else:
-        q, k = qkv[:, :D], qkv[:, D:2 * D]
-    ll.attn_bwd(q, k, qkv[:, 2 * D:], a, da, lse, B, n, H, d, d ** -0.5,
+    qk = s.qkn if s.qkn is not None else s.qkv
+    ll.attn_bwd(qk[:, :D], qk[:, D:2 * D], s.qkv[:, 2 * D:], s.a, da, s.lse, B, n, H, d, spec.attn_scale(d),
                 dqkv[:, :D], dqkv[:, D:2 * D], dqkv[:, 2 * D:])
-    if qkn is not None and rk is None:
-        ll.rmsnorm_pair_bwd(dqkv, qkv, D, qnw, knw, rq, dqnw, dknw)
-    elif qkn is not None:
-        ll.norm_bwd(dqkv[:, :D], qkv[:, :D], qnw, None, rq, dx_out=dqkv[:, :D], dweight=dqnw)
-        ll.norm_bwd(dqkv[:, D:2 * D], qkv[:, D:2 * D], knw, None, rk, dx_out=dqkv[:, D:2 * D], dweight=dknw)
-    dqkvw = wgrad(dqkv, n1, pqkvw)
-    if qkvb is not None:
-        ll.colsum(dqkv, out=dqkvb)
-    dn1 = dgrad(dqkv, 0, qkvw)
-    dx0 = ll.norm_bwd(dn1, x, n1w, None, rstd1, dx_in=dx1, dweight=dn1w)
+    if s.qkn is not None and s.rk is None:
+        ll.rmsnorm_pair_bwd(dqkv, s.qkv, D, t.qnw, t.knw, s.rq, seg["qnw"], seg["knw"])
+    elif s.qkn is not None:
+        ll.norm_bwd(dqkv[:, :D], s.qkv[:, :D], t.qnw, None, s.rq, dx_out=dqkv[:, :D], dweight=seg["qnw"])
+        ll.norm_bwd(dqkv[:, D:2 * D], s.qkv[:, D:2 * D], t.knw, None, s.rk, dx_out=dqkv[:, D:2 * D], dweight=seg["knw"])
+    dqkvw = wgrad(dqkv, s.n1, P.qkvw)
+    if t.qkvb is not None:
+        ll.colsum(dqkv, out=seg["qkvb"])
+    dn1 = dgrad(dqkv, t.qkvw, s.qkvw_t, s.qkvw_s)
+    dx0 = ll.norm_bwd(dn1, x, t.n1w, None, s.rstd1, dx_in=dx1, dweight=seg["n1w"])
     # ---- O(D) glue: bias grads through LayerScale (layerscale_bwd already folds gamma into the
     # bias-gradient column sums), cast to the parameter dtype
     if sink is not None:
         sink.flat_grad[base:base + span].add_(vec[:span])
-        for prm in (pn1w, pqkvb, pqnw, pknw, pprojb, pg1, pn2w, pfc1b, pfc2b, pg2):
-            if prm is not None:
-                sink.grad_written(prm)
+        for nm in BlockParams._fields:
+            if nm in seg and getattr(P, nm) is not None:
+                sink.grad_written(getattr(P, nm))
         return dx0, None
-    vb = vec.to(n1w.dtype)
-    sl = lambda t: vb[t.storage_offset():t.storage_offset() + t.numel()]  # noqa: E731
-    return dx0, (sl(dn1w), dqkvw, sl(dqkvb) if qkvb is not None else None,
-                 sl(dqnw) if qnw is not None else None, sl(dknw) if knw is not None else None,
-                 dprojw, sl(dcs1), sl(dg1) if g1 is not None else None, sl(dn2w),
-                 dfc1w, sl(dfc1b), dfc2w, sl(dcs2), sl(dg2) if g2 is not None else None)
+    vb = vec.to(t.n1w.dtype)
+    small_grads = {nm: None if prm is None else vb[seg[nm].storage_offset():seg[nm].storage_offset() + seg[nm].numel()]
+                   for nm, prm, _ in small}
+    return dx0, BlockParams(qkvw=dqkvw, projw=dprojw, fc1w=dfc1w, fc2w=dfc2w, **small_grads)
 
 
 class BlockFn(torch.autograd.Function):
-    """Differentiable block_forward.  dims = (B, n, H, gelu_tanh[, checkpoint[, fp8]]).
+    """Differentiable block_forward of the RMSNorm block: apply(x, spec, rs1, rs2, *params) with spec a BlockSpec,
+    params the BlockParams and rs1 / rs2 optional fp32 [B*n] per-row DropPath keep/scale factors of the two branches.
 
-    checkpoint=True is the reference's `with_cp` / `use_checkpoint` (internvideo2_pretrain.py:294-295,
+    spec.checkpoint is the reference's `with_cp` / `use_checkpoint` (internvideo2_pretrain.py:294-295,
     torch.utils.checkpoint around the block): only the block INPUT (4 D bytes/token) is kept; backward first
-    re-runs the 14 forward kernels to rebuild the 44 D bytes/token of saved activations, then the 26 backward
-    kernels.  DropPath factors are inputs (rs1/rs2), so the recomputation sees the same draw."""
+    re-runs the forward to rebuild the 44 D bytes/token of saved activations, then the backward.  DropPath factors
+    are inputs, so the recomputation sees the same draw."""
 
     @staticmethod
-    def forward(ctx, x, dims, n1w, qkvw, qkvb, qnw, knw, projw, projb, g1, n2w, fc1w, fc1b, fc2w, fc2b, g2,
-                rs1=None, rs2=None):
-        # rs1/rs2: optional fp32 [B*n] per-row DropPath keep/scale factors of the two branches
-        params = (n1w, qkvw, qkvb, qnw, knw, projw, projb, g1, n2w, fc1w, fc1b, fc2w, fc2b, g2)
-        ckpt = len(dims) > 4 and bool(dims[4])
-        x2, saved = block_forward(x, dims, params, rs1, rs2, save=not ckpt)
-        ctx.dims, ctx.ckpt = tuple(dims[:4]) + (False, _block_fp8(dims)), ckpt
-        ctx.params = params
-        if ckpt:
-            ctx.nsaved = 0
-            ctx.save_for_backward(x, rs1, rs2, *params)
-        else:
-            ctx.flags = saved[-1]
-            ctx.save_for_backward(x, rs1, rs2, *params, *saved[:-1])
+    def forward(ctx, x, spec, rs1, rs2, *params):
+        params = BlockParams(*params)
+        x2, saved = block_forward(x, spec, params, rs1, rs2, save=not spec.checkpoint)
+        ctx.spec, ctx.params = spec, params
+        ctx.save_for_backward(x, rs1, rs2, *params, *(saved or ()))
         return x2
 
     @staticmethod
     def backward(ctx, dx2):
-        st = ctx.saved_tensors
-        x, rs1, rs2 = st[:3]
-        tensors = st[3:17]
-        if ctx.ckpt:
+        x, rs1, rs2, *rest = ctx.saved_tensors
+        nparams = len(BlockParams._fields)
+        tensors = BlockParams._make(rest[:nparams])
+        if ctx.spec.checkpoint:
             with torch.no_grad():
-                _, saved = block_forward(x, ctx.dims, tensors, rs1, rs2, save=True)
+                _, saved = block_forward(x, ctx.spec._replace(checkpoint=False), tensors, rs1, rs2, save=True)
         else:
-            saved = tuple(st[17:]) + (ctx.flags,)
-        dx0, grads = block_backward(x, saved, ctx.dims, tensors, ctx.params, dx2, rs1, rs2)
-        if grads is None:
-            return (dx0,) + (None,) * 17
-        return (dx0, None) + tuple(grads) + (None, None)
+            saved = BlockSaved._make(rest[nparams:])
+        dx0, grads = block_backward(x, saved, ctx.spec, tensors, ctx.params, dx2, rs1, rs2)
+        return (dx0, None, None, None) + (grads or (None,) * nparams)
 
 
 def _common_sink(params):
@@ -479,7 +442,7 @@ def _common_sink(params):
     return sink if (sink is not None and sink.direct_enabled()) else None
 
 
-def _plan_small(small, params, sink, device):
+def _plan_small(small, sink, device):
     """fp32 scratch for the block's O(D) gradients.  With a sink the segments sit at the parameters'
     relative offsets inside the flat gradient buffer, so a single add_ lands them all.
     Returns (segments by name, scratch, span or None, base offset)."""

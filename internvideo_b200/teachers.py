@@ -21,7 +21,7 @@ import torch.nn as nn
 
 from . import lowlevel as ll
 from . import ops
-from .modules import (AttentionPoolingBlock, Block, LayerNormB, RMSNorm, bf16, f32, fp8_inference_weights, to_2tuple,
+from .modules import (AttentionPoolingBlock, Block, LayerNormB, RMSNorm, bf16, block_precision, f32, to_2tuple,
                       trunc_normal_)
 
 
@@ -171,15 +171,22 @@ class TeacherBlock(nn.Module):
     def _fp8_linears(self):
         return (self.attn.qkv, self.attn.proj, self.mlp.fc1, self.mlp.fc2)
 
-    def forward_infer(self, x2d, B, n, head_axis_attention=True):
-        """fp32 residual stream [B*n, D] -> same; 9 kernels, nothing saved."""
+    def _param_tuple(self):
         a = self.attn
-        return ops.block_forward_ln_infer(
-            x2d, B, n, a.num_heads, a.scale, head_axis_attention=head_axis_attention, params=
-            (self.norm1.weight, self.norm1.bias, self.norm1.eps, a.qkv.weight, a.qkv_bias_vector(), a.proj.weight,
-             a.proj.bias, self.gamma_1, self.norm2.weight, self.norm2.bias, self.norm2.eps, self.mlp.fc1.weight,
-             self.mlp.fc1.bias, self.mlp.fc2.weight, self.mlp.fc2.bias, self.gamma_2),
-            fp8_weights=fp8_inference_weights(self))
+        return ops.BlockParams(
+            n1w=self.norm1.weight, n1b=self.norm1.bias, qkvw=a.qkv.weight, qkvb=a.qkv_bias_vector(), qnw=None, knw=None,
+            projw=a.proj.weight, projb=a.proj.bias, g1=self.gamma_1, n2w=self.norm2.weight, n2b=self.norm2.bias,
+            fc1w=self.mlp.fc1.weight, fc1b=self.mlp.fc1.bias, fc2w=self.mlp.fc2.weight, fc2b=self.mlp.fc2.bias,
+            g2=self.gamma_2)
+
+    def forward_infer(self, x2d, B, n, head_axis_attention=True):
+        """fp32 residual stream [B*n, D] -> same: ops.block_forward's LayerNorm form, nothing saved."""
+        a = self.attn
+        with torch.no_grad():
+            params = self._param_tuple()
+            spec = ops.BlockSpec(B, n, a.num_heads, layernorm=True, eps1=self.norm1.eps, eps2=self.norm2.eps,
+                                 scale=a.scale, head_axis=head_axis_attention, precision=block_precision(self))
+            return ops.block_forward(x2d, spec, params, save=False)[0]
 
 
 class TubeletPatchEmbed(nn.Module):

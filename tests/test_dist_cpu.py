@@ -255,7 +255,7 @@ def test_gradient_sink_planning_cpu():
     assert sink is e
     small = (("g2", m.g2, D), ("fc2b", m.fc2b, D), ("n2w", m.n2w, D), ("g1", m.g1, D), ("projb", m.projb, D),
              ("qnw", m.qnw, D), ("knw", m.knw, D), ("n1w", m.n1w, D), ("fc1b", m.fc1b, Hd), ("qkvb", None, 3 * D))
-    seg, vec, span, base = ops._plan_small(small, params, sink, torch.device("cpu"))
+    seg, vec, span, base = ops._plan_small(small, sink, torch.device("cpu"))
     assert span is not None and vec.dtype == torch.float32
     # every present parameter's segment sits at its flat-buffer offset relative to `base`
     for j, (name, p, sz) in enumerate(small):
@@ -275,5 +275,5 @@ def test_gradient_sink_planning_cpu():
     stray = torch.nn.Parameter(torch.zeros(D, dtype=torch.bfloat16))
     assert ops._common_sink(params + (stray,)) is None
     # without a sink the scratch is simply packed
-    seg2, vec2, span2, _ = ops._plan_small(small, params, None, torch.device("cpu"))
+    seg2, vec2, span2, _ = ops._plan_small(small, None, torch.device("cpu"))
     assert span2 is None and vec2.numel() == 8 * D + Hd + 3 * D

@@ -55,7 +55,7 @@ def timed(fn, iters):
 
 
 def _epilogue(t, name, M, N):
-    """The fused epilogue the teacher's block gives this GEMM (ops.block_forward / block_forward_ln_infer): InternVL
+    """The fused epilogue the teacher's block gives this GEMM (ops.block_forward, RMSNorm or LayerNorm form): InternVL
     qkv without bias, proj and fc2 into the residual stream with LayerScale gamma, fc1 with tanh GELU; VideoMAE-g qkv
     with the q/v bias, proj and fc2 into the stream without gamma (init_values 0), fc1 with erf GELU."""
     bias = (torch.randn(N, device="cuda") * 0.02).to(torch.bfloat16)
