@@ -11,20 +11,15 @@ wrapper takes any module/callable as `text_encoder`; the default accepts pre-com
 """
 from __future__ import annotations
 
-import math
-from functools import partial
-
 import torch
 import torch.nn as nn
 
-from . import lowlevel as ll
 from . import ops
 from .contrastive import VTC_VTM_Loss
-from .modules import (AttentionPoolingBlock, Block, LayerNormB, PatchEmbed, RMSNorm, bf16, f32,
-                      get_1d_sincos_pos_embed, get_2d_sincos_pos_embed, get_3d_sincos_pos_embed, trunc_normal_)
+from .modules import InternVideo2Tower, LayerNormB, check_input, embed_tokens, run_blocks
 
 
-class InternVideo2(nn.Module):
+class InternVideo2(InternVideo2Tower):
     """internvideo2_clip_vision.py:340-548 — unmasked tower: every one of the 1 + T*L tokens goes through the
     blocks, then the attention-pooling projector.  forward(x[B,C,T,H,W], use_image=False) -> [B, clip_embed_dim]."""
 
@@ -33,113 +28,27 @@ class InternVideo2(nn.Module):
                  qk_normalization=True, depth=40, use_flash_attn=True, use_fused_rmsnorm=True, use_fused_mlp=True,
                  fused_mlp_heuristic=1, attn_pool_num_heads=16, clip_embed_dim=768, layerscale_no_force_fp32=False,
                  num_frames=8, tubelet_size=1, sep_pos_embed=False, use_checkpoint=False, checkpoint_num=0):
-        super().__init__()
-        assert use_flash_attn == use_fused_rmsnorm == use_fused_mlp, \
-            "use_flash_attn, use_fused_rmsnorm and use_fused_mlp should be consistent"
         if head_drop_path_rate:
             raise NotImplementedError("ivb200 InternVideo2: head_drop_path_rate is 0 in every recipe")
-        self.use_flash_attn = use_flash_attn
-        self.embed_dim = embed_dim
+        super().__init__(in_chans, patch_size, img_size, qkv_bias, drop_path_rate, embed_dim, num_heads, mlp_ratio,
+                         init_values, qk_normalization, depth, use_flash_attn, use_fused_rmsnorm, use_fused_mlp,
+                         fused_mlp_heuristic, attn_pool_num_heads, clip_embed_dim, layerscale_no_force_fp32, num_frames,
+                         tubelet_size, sep_pos_embed, use_checkpoint, checkpoint_num)
         self.T = num_frames // tubelet_size
         self.num_frames, self.tubelet_size = num_frames, tubelet_size
-        self.patch_embed = PatchEmbed(img_size, patch_size, in_chans, embed_dim, num_frames=num_frames,
-                                      tubelet_size=tubelet_size)
-        num_patches = self.patch_embed.num_patches
-        self.cls_token = nn.Parameter(torch.zeros(1, 1, embed_dim))
-        self.sep_pos_embed = bool(sep_pos_embed)
-        if self.sep_pos_embed:
-            gs = self.grid_size = self.patch_embed.grid_size
-            self.pos_embed_spatial = nn.Parameter(torch.zeros(1, gs[1] * gs[2], embed_dim))
-            self.pos_embed_temporal = nn.Parameter(torch.zeros(1, gs[0], embed_dim))
-            self.pos_embed_cls = nn.Parameter(torch.zeros(1, 1, embed_dim))
-        else:
-            self.pos_embed = nn.Parameter(torch.zeros(1, num_patches + 1, embed_dim))
-        dpr = [drop_path_rate * i / (depth - 1) if depth > 1 else 0.0 for i in range(depth)]
-        with_cp = [bool(use_checkpoint) and i < checkpoint_num for i in range(depth)]
-        self.blocks = nn.ModuleList([
-            Block(embed_dim, num_heads, mlp_ratio, qkv_bias=qkv_bias, norm_layer=RMSNorm, drop_path=dpr[i],
-                  init_values=init_values, attn_drop=0.0, use_flash_attn=use_flash_attn, use_fused_mlp=use_fused_mlp,
-                  fused_mlp_heuristic=fused_mlp_heuristic, with_cp=with_cp[i], qk_normalization=qk_normalization,
-                  layerscale_no_force_fp32=layerscale_no_force_fp32, use_fused_rmsnorm=use_fused_rmsnorm)
-            for i in range(depth)])
-        self.clip_projector = AttentionPoolingBlock(dim=embed_dim, num_heads=attn_pool_num_heads, qkv_bias=True,
-                                                    qk_scale=None, drop=0.0, attn_drop=0.0,
-                                                    norm_layer=partial(nn.LayerNorm, eps=1e-5), out_dim=clip_embed_dim)
         self.fc_norm = nn.Identity()
-        self.init_pos_embed()
-        trunc_normal_(self.cls_token, std=0.02)
-        self.apply(self._init_weights)
-        self.fix_init_weight()
-
-    # ---- init (:434-481)
-    def init_pos_embed(self):
-        gs = self.patch_embed.grid_size
-        if self.sep_pos_embed:
-            D = self.pos_embed_spatial.shape[-1]
-            self.pos_embed_spatial.data.copy_(torch.from_numpy(get_2d_sincos_pos_embed(D, gs[1])).float().unsqueeze(0))
-            self.pos_embed_temporal.data.copy_(torch.from_numpy(get_1d_sincos_pos_embed(D, gs[0])).float().unsqueeze(0))
-        else:
-            pe = get_3d_sincos_pos_embed(self.pos_embed.shape[-1], gs[1], gs[0], cls_token=True)
-            self.pos_embed.data.copy_(torch.from_numpy(pe).float().unsqueeze(0))
-
-    def _init_weights(self, m):
-        if isinstance(m, nn.Linear):
-            trunc_normal_(m.weight, std=0.02)
-            if m.bias is not None:
-                nn.init.constant_(m.bias, 0)
-        elif isinstance(m, nn.LayerNorm):
-            nn.init.constant_(m.bias, 0)
-            nn.init.constant_(m.weight, 1.0)
-
-    def fix_init_weight(self):
-        for layer_id, layer in enumerate(self.blocks):
-            layer.attn.proj.weight.data.div_(math.sqrt(2.0 * (layer_id + 1)))
-            layer.mlp.fc2.weight.data.div_(math.sqrt(2.0 * (layer_id + 1)))
-
-    @property
-    def dtype(self):
-        return self.patch_embed.proj.weight.dtype
-
-    def get_num_layers(self):
-        return len(self.blocks)
-
-    @torch.jit.ignore
-    def no_weight_decay(self):
-        return {"pos_embed", "pos_embed_spatial", "pos_embed_temporal", "pos_embed_cls", "cls_token"}
+        self.init_tower()
 
     # ---- forward (:497-548)
-    def _pos_table(self, use_image):
-        """[1, 1+tokens, D] table: joint / separable, video / single image (temporal mean of the joint table, :524-527)."""
-        if self.sep_pos_embed:
-            if use_image:
-                pe = self.pos_embed_spatial
-            else:
-                gs = self.grid_size
-                pe = self.pos_embed_spatial.repeat(1, gs[0], 1) + torch.repeat_interleave(
-                    self.pos_embed_temporal, gs[1] * gs[2], dim=1)
-            return torch.cat([self.pos_embed_cls.expand(pe.shape[0], -1, -1), pe], 1)
-        if use_image:
-            L = self.patch_embed.grid_size[1] * self.patch_embed.grid_size[2]
-            C = self.pos_embed.shape[-1]
-            img = self.pos_embed[:, 1:, :].view(1, self.T, L, C).mean(dim=1)
-            return torch.cat([self.pos_embed[:, :1, :], img], dim=1)
-        return self.pos_embed
-
     def forward_tokens(self, x, use_image=False):
         """-> fp32 residual stream [B*n, D] after the last block, B, n."""
-        if self.dtype != bf16:
-            raise ll._lib.IvbError("ivb200 InternVideo2 computes in bf16: call model.bfloat16() first")
-        if not x.is_cuda:
-            raise ll._lib.IvbError("ivb200 InternVideo2: input must be a CUDA tensor (no CPU fallback)")
+        check_input(self, x, self.dtype)
         B = x.shape[0]
         pe = self.patch_embed
-        tokens = (x.shape[2] // pe.tubelet_size) * pe.grid_size[1] * pe.grid_size[2]
-        n = tokens + 1
+        n = 1 + (x.shape[2] // pe.tubelet_size) * pe.grid_size[1] * pe.grid_size[2]
         idx = torch.arange(0, n, device=x.device, dtype=torch.int32).repeat(B, 1).contiguous()   # nothing is masked
-        h = ops.EmbedFn.apply(x.to(bf16), idx, pe.proj.weight, pe.proj.bias, self.cls_token, self._pos_table(use_image),
-                              pe.tubelet_size, pe.patch_size[0])
-        for blk in self.blocks:
-            h = blk.forward_stream(h, B, n)
+        h = embed_tokens(pe, x, idx, self.cls_token, self._pos_table("", use_image))
+        h, _ = run_blocks(self.blocks, h, lambda i, blk, h: blk.forward_stream(h, B, n))
         return h, B, n
 
     def forward(self, x, use_image=False):

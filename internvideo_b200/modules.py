@@ -70,6 +70,80 @@ def get_1d_sincos_pos_embed(embed_dim, t_size):
     return _sincos_1d(embed_dim, np.arange(t_size, dtype=np.float32))
 
 
+def get_sinusoid_encoding_table(n_position, d_hid):
+    """The VideoMAE towers' fixed table (IV1 modeling_finetune.py:224-242; videomae.py:152-205 for the recipe case
+    n_position == pre_n_position, no interpolation): [1, n_position, d_hid] fp32, sin on even / cos on odd channels."""
+    pos = np.arange(n_position, dtype=np.float64)[:, None]
+    j = np.arange(d_hid)[None, :]
+    table = pos / np.power(10000, 2 * (j // 2) / d_hid)
+    table[:, 0::2] = np.sin(table[:, 0::2])
+    table[:, 1::2] = np.cos(table[:, 1::2])
+    return torch.tensor(table, dtype=torch.float).unsqueeze(0)
+
+
+def _pos_tensor(a):
+    """numpy table -> a new fp32 [1, rows, D] tensor."""
+    return torch.tensor(a, dtype=torch.float).unsqueeze(0)
+
+
+# ------------------------------------------------------------------------------- pieces every tower shares
+def init_weights(m):
+    """The towers' Linear / LayerNorm init (internvideo2_pretrain.py:589-597, videomae.py:238-245)."""
+    if isinstance(m, nn.Linear):
+        trunc_normal_(m.weight, std=0.02)
+        if m.bias is not None:
+            nn.init.constant_(m.bias, 0)
+    elif isinstance(m, nn.LayerNorm):
+        nn.init.constant_(m.bias, 0)
+        nn.init.constant_(m.weight, 1.0)
+
+
+def check_input(tower, x, dtype):
+    """The refusal at the top of every tower forward: the parameters must be bf16 and the input a CUDA tensor."""
+    if dtype != bf16:
+        raise ll._lib.IvbError(f"ivb200 {type(tower).__name__} computes in bf16: call model.bfloat16() first")
+    if not x.is_cuda:
+        raise ll._lib.IvbError(f"ivb200 {type(tower).__name__}: input must be a CUDA tensor (no CPU fallback)")
+
+
+def index_poison(err):
+    """0, or NaN when the int32[1] device flag of a visible-token index build is set (the clips of a ragged mask keep
+    different numbers of tokens): added to an output, it surfaces the error without a host sync."""
+    z = torch.zeros((), device=err.device, dtype=f32)
+    return torch.where(err[0] != 0, torch.full_like(z, float("nan")), z)
+
+
+def embed_tokens(patch_embed, x, idx, cls_token, table):
+    """The token front-end of every tower (ops.EmbedFn): the patch embed's Conv3d on the tokens idx[:, 1:] names, as an
+    im2col + wgmma GEMM, plus their rows of the position table, behind `cls_token + table[0]`.  x: video [B,C,T,H,W];
+    idx: int32 [B, n], column 0 the cls slot.  Returns the fp32 residual stream [B*n, D].
+    cls_token None (towers without one): `table` holds the patch rows only; EmbedFn gets a zero cls token and a zero
+    table row, and the cls row is dropped again, giving [B*(n-1), D]."""
+    tubelet, patch, _ = patch_embed.proj.kernel_size
+    w, b = patch_embed.proj.weight, patch_embed.proj.bias
+    if cls_token is not None:
+        return ops.EmbedFn.apply(x.to(bf16), idx, w, b, cls_token, table, tubelet, patch)
+    B, n = idx.shape
+    D = w.shape[0]
+    table = torch.cat([table.new_zeros(1, 1, D), table], 1).to(bf16)
+    zcls = torch.zeros((1, 1, D), device=x.device, dtype=bf16)
+    h = ops.EmbedFn.apply(x.to(bf16), idx, w, b, zcls, table, tubelet, patch)
+    return h.reshape(B, n, D)[:, 1:].reshape(B * (n - 1), D)
+
+
+def run_blocks(blocks, h, call, taps=(), last=None):
+    """Runs blocks 0..last (all when `last` is no block index) over the stream h, block i as `call(i, block, h)`.
+    Returns the final stream and {i: output of block i} for each i in `taps`, in block order."""
+    out = {}
+    for i, blk in enumerate(blocks):
+        h = call(i, blk, h)
+        if i in taps:
+            out[i] = h
+        if i == last:
+            break
+    return h, out
+
+
 class DropPath(nn.Module):
     """Per-sample stochastic depth.  In the fused Block the keep/scale factor is applied as the
     GEMM epilogue's `rowscale` (timm DropPath semantics: Bernoulli(keep)/keep, training only)."""
@@ -350,16 +424,18 @@ class PatchEmbed(nn.Module):
 
     def forward(self, x):
         """All-token embed [B,C,T,H,W] -> [B, T', L, D] (bf16), same layout as the reference."""
-        B, C, T, H, W = x.shape
-        D = self.proj.weight.shape[0]
-        N = self.num_patches
+        B, N, D = x.shape[0], self.num_patches, self.proj.weight.shape[0]
         idx = torch.arange(0, N + 1, device=x.device, dtype=torch.int32).repeat(B, 1).contiguous()
-        zeros_tab = torch.zeros((N + 1, D), device=x.device, dtype=bf16)
-        zcls = torch.zeros((1, 1, D), device=x.device, dtype=bf16)
-        out = ops.EmbedFn.apply(x.to(bf16), idx, self.proj.weight, self.proj.bias, zcls, zeros_tab,
-                                self.tubelet_size, self.patch_size[0])
-        out = out.reshape(B, N + 1, D)[:, 1:]
+        out = embed_tokens(self, x, idx, None, torch.zeros((1, N, D), device=x.device, dtype=bf16))
         return out.reshape(B, self.grid_size[0], self.grid_size[1] * self.grid_size[2], D).to(bf16)
+
+
+class TubeletPatchEmbed(PatchEmbed):
+    """The VideoMAE towers' patch embed (videomae.py:135-149, IV1 modeling_finetune.py:184-219): PatchEmbed with their
+    defaults, 16 frames in tubelets of 2."""
+
+    def __init__(self, img_size=224, patch_size=16, in_chans=3, embed_dim=768, num_frames=16, tubelet_size=2):
+        super().__init__(img_size, patch_size, in_chans, embed_dim, num_frames, int(tubelet_size))
 
 
 class CrossAttention(nn.Module):
@@ -483,109 +559,80 @@ class MLP_Decoder(Linear_Decoder):
         return ops.linear(g, self.head[2].weight, self.head[2].bias)
 
 
-class PretrainInternVideo2(nn.Module):
-    """internvideo2_pretrain.py:406-744 — same ctor kwargs, same state_dict keys, same forward contract:
-    forward(x[B,3,T,H,W], mask[B,1+T*L] bool) -> (x_clip_align[K,B,n,Ct], x_align[B,Cf], x_mae_align[K',B,n-1,Cm]).
-    """
+def vit_stack(embed_dim, depth, num_heads, mlp_ratio, drop_path_rate, attn_pool_num_heads, clip_embed_dim,
+              checkpoint_num=0, **block_kw):
+    """`blocks` and `clip_projector` of the InternVideo2 towers and the InternVL teacher (internvideo2_pretrain.py:
+    495-518): `depth` RMSNorm Blocks whose DropPath rate rises linearly from 0 to drop_path_rate, the first
+    checkpoint_num of them recomputing their forward in backward, then the attention-pooling projector.
+    block_kw: the Block switches (qkv_bias, init_values, qk_normalization, layerscale_no_force_fp32, use_*)."""
+    dpr = [drop_path_rate * i / (depth - 1) if depth > 1 else 0.0 for i in range(depth)]  # == linspace(0, r, depth)
+    blocks = nn.ModuleList([Block(embed_dim, num_heads, mlp_ratio, norm_layer=RMSNorm, drop_path=dpr[i], attn_drop=0.0,
+                                  with_cp=i < checkpoint_num, **block_kw) for i in range(depth)])
+    return blocks, AttentionPoolingBlock(dim=embed_dim, num_heads=attn_pool_num_heads, qkv_bias=True, qk_scale=None,
+                                         drop=0.0, attn_drop=0.0, norm_layer=partial(nn.LayerNorm, eps=1e-5),
+                                         out_dim=clip_embed_dim)
 
-    def __init__(self, in_chans=3, patch_size=14, img_size=224, qkv_bias=False, drop_path_rate=0.25,
-                 embed_dim=1408, num_heads=16, mlp_ratio=4.3637, init_values=1e-5, qk_normalization=True,
-                 depth=40, use_flash_attn=True, use_fused_rmsnorm=True, use_fused_mlp=True, fused_mlp_heuristic=1,
-                 attn_pool_num_heads=16, clip_embed_dim=768, layerscale_no_force_fp32=False, num_frames=8,
-                 tubelet_size=1, sep_pos_embed=False, use_checkpoint=False, checkpoint_num=0,
-                 clip_teacher_embed_dim=3200, clip_teacher_final_dim=768, clip_norm_type="l2", clip_return_layer=1,
-                 clip_student_return_interval=1, mae_teacher_embed_dim=1408, mae_norm_type="l2", mae_return_layer=1,
-                 mae_student_return_interval=1):
+
+class InternVideo2Tower(nn.Module):
+    """What the InternVideo2 towers share (the student, the stage-2 tower and the CLIP tower): `patch_embed`,
+    `cls_token`, the position tables of `pos_prefixes` ('' for the blocks, 'clip_' / 'mae_' for the decoders; joint,
+    or spatial / temporal / cls with sep_pos_embed), `blocks` and `clip_projector`, registered in this order.
+    A subclass registers its heads and then calls init_tower(), so the init draws follow every constructor draw."""
+
+    pos_prefixes = ("",)
+    sep_image_video_pos_embed = False
+
+    def __init__(self, in_chans, patch_size, img_size, qkv_bias, drop_path_rate, embed_dim, num_heads, mlp_ratio,
+                 init_values, qk_normalization, depth, use_flash_attn, use_fused_rmsnorm, use_fused_mlp,
+                 fused_mlp_heuristic, attn_pool_num_heads, clip_embed_dim, layerscale_no_force_fp32, num_frames,
+                 tubelet_size, sep_pos_embed, use_checkpoint, checkpoint_num):
         super().__init__()
         assert use_flash_attn == use_fused_rmsnorm == use_fused_mlp, \
             "use_flash_attn, use_fused_rmsnorm and use_fused_mlp should be consistent"
         self.use_flash_attn = use_flash_attn
         self.embed_dim = embed_dim
         self.depth = depth
-        self.clip_norm_type, self.mae_norm_type = clip_norm_type, mae_norm_type
-        self.clip_return_index = [depth - int(i * clip_student_return_interval) - 1 for i in range(clip_return_layer)]
-        self.mae_return_index = [depth - int(i * mae_student_return_interval) - 1 for i in range(mae_return_layer)]
         self.patch_embed = PatchEmbed(img_size, patch_size, in_chans, embed_dim, num_frames=num_frames,
                                       tubelet_size=tubelet_size)
-        num_patches = self.patch_embed.num_patches
         self.cls_token = nn.Parameter(torch.zeros(1, 1, embed_dim))
         self.sep_pos_embed = bool(sep_pos_embed)
-        if self.sep_pos_embed:      # :481-493 — separable spatial / temporal / cls tables, one set per consumer
-            gs = self.grid_size = self.patch_embed.grid_size
-            Z = lambda *shape: nn.Parameter(torch.zeros(*shape))  # noqa: E731
-            self.pos_embed_spatial, self.pos_embed_temporal = Z(1, gs[1] * gs[2], embed_dim), Z(1, gs[0], embed_dim)
-            self.pos_embed_cls = Z(1, 1, embed_dim)
-            self.clip_pos_embed_spatial, self.clip_pos_embed_temporal = Z(1, gs[1] * gs[2], embed_dim), Z(1, gs[0], embed_dim)
-            self.clip_pos_embed_cls = Z(1, 1, embed_dim)
-            self.mae_pos_embed_spatial, self.mae_pos_embed_temporal = Z(1, gs[1] * gs[2], embed_dim), Z(1, gs[0], embed_dim)
-        else:
-            self.pos_embed = nn.Parameter(torch.zeros(1, num_patches + 1, embed_dim))
-            self.clip_pos_embed = nn.Parameter(torch.zeros(1, num_patches + 1, embed_dim))
-            self.mae_pos_embed = nn.Parameter(torch.zeros(1, num_patches, embed_dim))
-        dpr = [drop_path_rate * i / (depth - 1) if depth > 1 else 0.0 for i in range(depth)]  # == linspace(0, r, depth)
-        with_cp = [bool(use_checkpoint) and i < checkpoint_num for i in range(depth)]           # :503-507
-        self.blocks = nn.ModuleList([
-            Block(embed_dim, num_heads, mlp_ratio, qkv_bias=qkv_bias, norm_layer=RMSNorm, drop_path=dpr[i],
-                  init_values=init_values, attn_drop=0.0, use_flash_attn=use_flash_attn, use_fused_mlp=use_fused_mlp,
-                  fused_mlp_heuristic=fused_mlp_heuristic, with_cp=with_cp[i], qk_normalization=qk_normalization,
-                  layerscale_no_force_fp32=layerscale_no_force_fp32, use_fused_rmsnorm=use_fused_rmsnorm)
-            for i in range(depth)])
-        self.clip_projector = AttentionPoolingBlock(dim=embed_dim, num_heads=attn_pool_num_heads, qkv_bias=True,
-                                                    qk_scale=None, drop=0.0, attn_drop=0.0,
-                                                    norm_layer=partial(nn.LayerNorm, eps=1e-5), out_dim=clip_embed_dim)
-        ln = partial(nn.LayerNorm, eps=1e-5)
-        self.clip_decoder = nn.ModuleList([
-            Linear_Decoder(embed_dim, clip_teacher_embed_dim, norm_layer=ln, norm_type=clip_norm_type)
-            for _ in range(clip_return_layer)])
-        self.final_clip_decoder = nn.Identity()
-        if clip_teacher_final_dim > 0:
-            self.final_clip_decoder = Linear_Decoder(clip_embed_dim, clip_teacher_final_dim, norm_layer=ln,
-                                                     norm_type=clip_norm_type)
-        self.mae_decoder = nn.ModuleList([
-            MLP_Decoder(embed_dim, mae_teacher_embed_dim, norm_layer=ln, norm_type=mae_norm_type)
-            for _ in range(mae_return_layer)])
+        gs = self.grid_size = self.patch_embed.grid_size
+        self.image_pos_groups = gs[0]        # an image's joint table: the mean over these groups of the video table
+        Z = lambda *shape: nn.Parameter(torch.zeros(*shape))  # noqa: E731
+        for pre in self.pos_prefixes:        # :481-493 — a table (set) per consumer; the MAE decoder's has no cls row
+            if not self.sep_pos_embed:
+                setattr(self, pre + "pos_embed", Z(1, self.patch_embed.num_patches + (pre != "mae_"), embed_dim))
+                continue
+            setattr(self, pre + "pos_embed_spatial", Z(1, gs[1] * gs[2], embed_dim))
+            setattr(self, pre + "pos_embed_temporal", Z(1, gs[0], embed_dim))
+            if pre != "mae_":
+                setattr(self, pre + "pos_embed_cls", Z(1, 1, embed_dim))
+        self.blocks, self.clip_projector = vit_stack(
+            embed_dim, depth, num_heads, mlp_ratio, drop_path_rate, attn_pool_num_heads, clip_embed_dim,
+            checkpoint_num if use_checkpoint else 0, qkv_bias=qkv_bias, init_values=init_values,
+            use_flash_attn=use_flash_attn, use_fused_mlp=use_fused_mlp, fused_mlp_heuristic=fused_mlp_heuristic,
+            qk_normalization=qk_normalization, layerscale_no_force_fp32=layerscale_no_force_fp32,
+            use_fused_rmsnorm=use_fused_rmsnorm)
+
+    # ---- init (internvideo2_pretrain.py:547-603)
+    def init_tower(self):
         self.init_pos_embed()
         trunc_normal_(self.cls_token, std=0.02)
-        self.apply(self._init_weights)
+        self.apply(init_weights)
         self.fix_init_weight()
 
-    # ---- init (internvideo2_pretrain.py:560-603)
     def init_pos_embed(self):
-        gs = self.patch_embed.grid_size
+        gs, D = self.grid_size, self.embed_dim
         if self.sep_pos_embed:
-            D = self.pos_embed_spatial.shape[-1]
-            sp = torch.from_numpy(get_2d_sincos_pos_embed(D, gs[1])).float().unsqueeze(0)
-            tp = torch.from_numpy(get_1d_sincos_pos_embed(D, gs[0])).float().unsqueeze(0)
-            for pre in ("", "clip_", "mae_"):
+            sp, tp = _pos_tensor(get_2d_sincos_pos_embed(D, gs[1])), _pos_tensor(get_1d_sincos_pos_embed(D, gs[0]))
+            for pre in self.pos_prefixes:
                 getattr(self, pre + "pos_embed_spatial").data.copy_(sp)
                 getattr(self, pre + "pos_embed_temporal").data.copy_(tp)
             return
-        pe = get_3d_sincos_pos_embed(self.pos_embed.shape[-1], gs[1], gs[0], cls_token=True)
-        t = torch.from_numpy(pe).float().unsqueeze(0)
-        self.pos_embed.data.copy_(t)
-        self.clip_pos_embed.data.copy_(t)
-        self.mae_pos_embed.data.copy_(t[:, 1:])
-
-    def _pos_table(self, which):
-        """The [1, 1+T*L, D] ('' / 'clip_') or [1, T*L, D] ('mae_') position table: the joint parameter, or the
-        separable tables composed exactly like :640-656 / :700-711 / :727-734 (torch glue, O(N*D), differentiable)."""
-        if not self.sep_pos_embed:
-            return getattr(self, which + "pos_embed")
-        gs = self.grid_size
-        sp, tp = getattr(self, which + "pos_embed_spatial"), getattr(self, which + "pos_embed_temporal")
-        pe = sp.repeat(1, gs[0], 1) + torch.repeat_interleave(tp, gs[1] * gs[2], dim=1)
-        if which == "mae_":
-            return pe
-        return torch.cat([getattr(self, which + "pos_embed_cls").expand(pe.shape[0], -1, -1), pe], 1)
-
-    def _init_weights(self, m):
-        if isinstance(m, nn.Linear):
-            trunc_normal_(m.weight, std=0.02)
-            if m.bias is not None:
-                nn.init.constant_(m.bias, 0)
-        elif isinstance(m, nn.LayerNorm):
-            nn.init.constant_(m.bias, 0)
-            nn.init.constant_(m.weight, 1.0)
+        t = _pos_tensor(get_3d_sincos_pos_embed(D, gs[1], gs[0], cls_token=True))
+        for pre in self.pos_prefixes:
+            pe = getattr(self, pre + "pos_embed")
+            pe.data.copy_(t[:, -pe.shape[1]:])
 
     def fix_init_weight(self):
         for layer_id, layer in enumerate(self.blocks):
@@ -601,16 +648,73 @@ class PretrainInternVideo2(nn.Module):
 
     @torch.jit.ignore
     def no_weight_decay(self):
-        return {"pos_embed", "pos_embed_spatial", "pos_embed_temporal", "pos_embed_cls", "cls_token",
-                "clip_pos_embed", "clip_pos_embed_spatial", "clip_pos_embed_temporal", "clip_pos_embed_cls",
-                "mae_pos_embed", "mae_pos_embed_spatial", "mae_pos_embed_temporal"}
+        names = {"cls_token"}
+        for pre in self.pos_prefixes:
+            names |= {pre + "pos_embed", pre + "pos_embed_spatial", pre + "pos_embed_temporal"}
+            if pre != "mae_":
+                names.add(pre + "pos_embed_cls")
+        return names
+
+    def _pos_table(self, prefix, use_image=False):
+        """The position table a forward adds for the blocks ('') or a decoder ('clip_', 'mae_'): [1, 1+tokens, D]
+        ([1, tokens, D] for 'mae_'), torch glue, O(N*D), differentiable.  Separable: the spatial table, for a video plus
+        the temporal one (:640-656 / :700-711 / :727-734), behind the cls table.  Joint: the parameter for a video; for
+        an image stage 2's image parameter (sep_image_video_pos_embed), else the mean of the video table over
+        `image_pos_groups` groups (internvideo2_clip_vision.py:524-527, internvideo2.py:598-606)."""
+        gs = self.grid_size
+        if self.sep_pos_embed:
+            pe = getattr(self, prefix + "pos_embed_spatial")
+            if not use_image:
+                pe = pe.repeat(1, gs[0], 1) + torch.repeat_interleave(getattr(self, prefix + "pos_embed_temporal"),
+                                                                       gs[1] * gs[2], dim=1)
+            if prefix == "mae_":
+                return pe
+            return torch.cat([getattr(self, prefix + "pos_embed_cls").expand(pe.shape[0], -1, -1), pe], 1)
+        pe = getattr(self, prefix + "pos_embed")
+        if not use_image:
+            return pe
+        if self.sep_image_video_pos_embed:
+            return getattr(self, prefix + "img_pos_embed")
+        img = pe[:, 1:, :].view(1, self.image_pos_groups, -1, pe.shape[-1]).mean(dim=1)
+        return torch.cat([pe[:, :1, :], img], dim=1)
+
+
+class PretrainInternVideo2(InternVideo2Tower):
+    """internvideo2_pretrain.py:406-744 — same ctor kwargs, same state_dict keys, same forward contract:
+    forward(x[B,3,T,H,W], mask[B,1+T*L] bool) -> (x_clip_align[K,B,n,Ct], x_align[B,Cf], x_mae_align[K',B,n-1,Cm]).
+    """
+
+    pos_prefixes = ("", "clip_", "mae_")
+
+    def __init__(self, in_chans=3, patch_size=14, img_size=224, qkv_bias=False, drop_path_rate=0.25,
+                 embed_dim=1408, num_heads=16, mlp_ratio=4.3637, init_values=1e-5, qk_normalization=True,
+                 depth=40, use_flash_attn=True, use_fused_rmsnorm=True, use_fused_mlp=True, fused_mlp_heuristic=1,
+                 attn_pool_num_heads=16, clip_embed_dim=768, layerscale_no_force_fp32=False, num_frames=8,
+                 tubelet_size=1, sep_pos_embed=False, use_checkpoint=False, checkpoint_num=0,
+                 clip_teacher_embed_dim=3200, clip_teacher_final_dim=768, clip_norm_type="l2", clip_return_layer=1,
+                 clip_student_return_interval=1, mae_teacher_embed_dim=1408, mae_norm_type="l2", mae_return_layer=1,
+                 mae_student_return_interval=1):
+        super().__init__(in_chans, patch_size, img_size, qkv_bias, drop_path_rate, embed_dim, num_heads, mlp_ratio,
+                         init_values, qk_normalization, depth, use_flash_attn, use_fused_rmsnorm, use_fused_mlp,
+                         fused_mlp_heuristic, attn_pool_num_heads, clip_embed_dim, layerscale_no_force_fp32, num_frames,
+                         tubelet_size, sep_pos_embed, use_checkpoint, checkpoint_num)
+        self.clip_norm_type, self.mae_norm_type = clip_norm_type, mae_norm_type
+        self.clip_return_index = [depth - int(i * clip_student_return_interval) - 1 for i in range(clip_return_layer)]
+        self.mae_return_index = [depth - int(i * mae_student_return_interval) - 1 for i in range(mae_return_layer)]
+        ln = partial(nn.LayerNorm, eps=1e-5)
+        self.clip_decoder = nn.ModuleList([
+            Linear_Decoder(embed_dim, clip_teacher_embed_dim, norm_layer=ln, norm_type=clip_norm_type)
+            for _ in range(clip_return_layer)])
+        self.final_clip_decoder = nn.Identity()
+        if clip_teacher_final_dim > 0:
+            self.final_clip_decoder = Linear_Decoder(clip_embed_dim, clip_teacher_final_dim, norm_layer=ln,
+                                                     norm_type=clip_norm_type)
+        self.mae_decoder = nn.ModuleList([
+            MLP_Decoder(embed_dim, mae_teacher_embed_dim, norm_layer=ln, norm_type=mae_norm_type)
+            for _ in range(mae_return_layer)])
+        self.init_tower()
 
     # ---- the hot path
-    def _check(self):
-        if self.dtype != bf16:
-            raise ll._lib.IvbError("ivb200 PretrainInternVideo2 computes in bf16: call model.bfloat16() first "
-                                   "(engine_for_pretraining.py:128 does the same in the reference's bf16 mode)")
-
     def visible_index(self, mask, n_visible=None):
         """int32 [B, n] positions of the kept tokens in `x[~mask]` order (bit-exact)."""
         if n_visible is None:
@@ -618,29 +722,24 @@ class PretrainInternVideo2(nn.Module):
         idx, err = ll.visible_indices(mask.to(self.cls_token.device, non_blocking=True), n_visible)
         return idx, err, n_visible
 
-    def forward_features(self, x, mask, n_visible=None, drop_path_factors=None):
+    def forward_features(self, x, mask, n_visible=None, drop_path_factors=None, use_image=False, last=None):
         """-> (taps: dict block_idx -> fp32 [B*n, D], final fp32 [B*n, D], idx int32 [B,n], B, n).
         drop_path_factors: optional fp32 [2*depth, B] per-sample stochastic-depth factors (Bernoulli(keep)/keep;
         rows 2i, 2i+1 = the two branches of block i) used instead of a fresh draw — parity tests inject the
-        draw the reference made (SURVEY App.B-16: RNG-dependent pieces are injected, not compared)."""
-        self._check()
-        if not x.is_cuda:
-            raise ll._lib.IvbError("ivb200 PretrainInternVideo2: input must be a CUDA tensor (no CPU fallback)")
+        draw the reference made (SURVEY App.B-16: RNG-dependent pieces are injected, not compared).
+        use_image / last: stage 2's image position table and early exit after block `last`."""
+        check_input(self, x, self.dtype)
         B = x.shape[0]
         idx, err, n = self.visible_index(mask, n_visible)
         self.index_error = err       # int32[1] on the device: 0, or 1 + (a clip whose visible-token count != n)
-        pe = self.patch_embed
-        h = ops.EmbedFn.apply(x.to(bf16), idx, pe.proj.weight, pe.proj.bias, self.cls_token, self._pos_table(""),
-                              pe.tubelet_size, pe.patch_size[0])
-        taps = {}
+        h = embed_tokens(self.patch_embed, x, idx, self.cls_token, self._pos_table("", use_image))
         if drop_path_factors is not None:
-            rs_all = drop_path_factors.to(device=h.device, dtype=f32).repeat_interleave(n, dim=1).contiguous()
+            rs = drop_path_factors.to(device=h.device, dtype=f32).repeat_interleave(n, dim=1).contiguous()
         else:
-            rs_all = self._sample_drop_path(B, n, h.device)
-        for i, blk in enumerate(self.blocks):
-            h = blk.forward_stream(h, B, n, None if rs_all is None else (rs_all[2 * i], rs_all[2 * i + 1]))
-            if i in self.clip_return_index or i in self.mae_return_index:
-                taps[i] = h
+            rs = self._sample_drop_path(B, n, h.device)
+        def block(i, blk, h):
+            return blk.forward_stream(h, B, n, None if rs is None else (rs[2 * i], rs[2 * i + 1]))
+        h, taps = run_blocks(self.blocks, h, block, self.clip_return_index + self.mae_return_index, last)
         return taps, h, idx, B, n
 
     def _sample_drop_path(self, B, n, device):
@@ -676,7 +775,7 @@ class PretrainInternVideo2(nn.Module):
         clip_in, mae_in = self._decoder_inputs(taps, idx, B, n)
         x_clip_align = torch.stack([dec(xi).reshape(B, n, -1) for dec, xi in zip(self.clip_decoder, clip_in)])
         x_align = self.final_clip_decoder(pooled)
-        x_align = x_align + self._index_poison().to(x_align.dtype)      # ragged mask -> NaN, no sync (see forward_loss)
+        x_align = x_align + index_poison(self.index_error).to(x_align.dtype)   # ragged mask -> NaN (see forward_loss)
         x_mae_align = torch.stack([dec(xi).reshape(B, n - 1, -1) for dec, xi in zip(self.mae_decoder, mae_in)])
         return x_clip_align, x_align, x_mae_align
 
@@ -699,12 +798,8 @@ class PretrainInternVideo2(nn.Module):
         # a mask whose rows keep different numbers of tokens cannot be reshaped to [B, n, C] (the reference raises at
         # :659); here the flag lives on the device, so it is surfaced without a sync: the loss becomes NaN
         # (and engine.step(check_finite=True) skips the update)
-        loss_final = loss_final + self._index_poison()
+        loss_final = loss_final + index_poison(self.index_error)
         return loss_clip, loss_final, loss_mae
-
-    def _index_poison(self):
-        z = torch.zeros((), device=self.index_error.device, dtype=f32)
-        return torch.where(self.index_error[0] != 0, torch.full_like(z, float("nan")), z)
 
 
 def pretrain_internvideo2_1B_patch14_224(pretrained=False, **kwargs):

@@ -26,6 +26,7 @@ import torch.nn.functional as F
 from . import lowlevel as ll
 from . import ops
 from .modules import PretrainInternVideo2 as _SingleModalityTower
+from .modules import _pos_tensor, get_3d_sincos_pos_embed, index_poison
 
 bf16, f32 = torch.bfloat16, torch.float32
 
@@ -34,6 +35,8 @@ class PretrainInternVideo2(_SingleModalityTower):
     """internvideo2.py:380-668.  Differences to the single-modality tower (modules.PretrainInternVideo2): no MAE branch,
     `mask` is optional, images use the temporal mean of the video position table (or their own tables with
     `sep_image_video_pos_embed`), the block loop can stop early (`x_vis_return_idx`) and `x_vis` is returned."""
+
+    pos_prefixes = ("", "clip_")         # the stage-2 tower has no MAE branch (keys must match the reference's)
 
     def __init__(self, in_chans=3, patch_size=14, img_size=224, qkv_bias=False, drop_path_rate=0.25, embed_dim=1408,
                  num_heads=16, mlp_ratio=4.3637, init_values=1e-5, qk_normalization=True, depth=40, use_flash_attn=True,
@@ -54,87 +57,39 @@ class PretrainInternVideo2(_SingleModalityTower):
                          clip_teacher_embed_dim=clip_teacher_embed_dim, clip_teacher_final_dim=clip_teacher_final_dim,
                          clip_norm_type=clip_norm_type, clip_return_layer=clip_return_layer,
                          clip_student_return_interval=clip_student_return_interval, mae_return_layer=0)
-        del self.mae_pos_embed                  # the stage-2 tower has no MAE branch (keys must match the reference's)
-        self.mae_return_index = []
         self.return_index = self.clip_return_index
         self.num_frames = num_frames
         self.tubelet_size = tubelet_size
+        self.image_pos_groups = num_frames      # :601,663 — an image's table averages groups of frames, not tubelets
         self.sep_image_video_pos_embed = bool(sep_image_video_pos_embed)
         self.num_img_patches = self.patch_embed.grid_size[1] * self.patch_embed.grid_size[2]
         if self.sep_image_video_pos_embed:      # :455-460 — images get their own tables
-            self.img_pos_embed = nn.Parameter(torch.zeros(1, self.num_img_patches + 1, embed_dim))
-            self.clip_img_pos_embed = nn.Parameter(torch.zeros(1, self.num_img_patches + 1, embed_dim))
-            self._init_img_pos_embed()
-
-    def init_pos_embed(self):
-        # :509-530 — the same 3-D sincos table for the backbone and the CLIP decoder; image tables in _init_img_pos_embed
-        from .modules import get_3d_sincos_pos_embed
-        gs = self.patch_embed.grid_size
-        t = torch.from_numpy(get_3d_sincos_pos_embed(self.pos_embed.shape[-1], gs[1], gs[0], cls_token=True)).float()
-        self.pos_embed.data.copy_(t.unsqueeze(0))
-        self.clip_pos_embed.data.copy_(t.unsqueeze(0))
-
-    def _init_img_pos_embed(self):
-        from .modules import get_3d_sincos_pos_embed
-        gs = self.patch_embed.grid_size
-        t = torch.from_numpy(get_3d_sincos_pos_embed(self.pos_embed.shape[-1], gs[1], 1, cls_token=True)).float()
-        self.img_pos_embed.data.copy_(t.unsqueeze(0))
-        self.clip_img_pos_embed.data.copy_(t.unsqueeze(0))
+            t = get_3d_sincos_pos_embed(embed_dim, self.patch_embed.grid_size[1], 1, cls_token=True)
+            self.img_pos_embed = nn.Parameter(_pos_tensor(t))
+            self.clip_img_pos_embed = nn.Parameter(_pos_tensor(t))
 
     @torch.jit.ignore
     def no_weight_decay(self):
-        return {"pos_embed", "pos_embed_spatial", "pos_embed_temporal", "pos_embed_cls", "img_pos_embed", "cls_token",
-                "clip_pos_embed", "clip_pos_embed_spatial", "clip_pos_embed_temporal", "clip_pos_embed_cls",
-                "clip_img_pos_embed"}
-
-    def _table(self, which, use_image):
-        """Position table of the backbone ('') or the CLIP decoder ('clip_'): video table, the image parameter, or the
-        temporal mean of the video table (:598-606 / :658-667)."""
-        pe = getattr(self, which + "pos_embed")
-        if not use_image:
-            return pe
-        if self.sep_image_video_pos_embed:
-            return getattr(self, which + "img_pos_embed")
-        D = pe.shape[-1]
-        img = pe[:, 1:, :].view(1, self.num_frames, self.patch_embed.num_patches // self.num_frames, D).mean(dim=1)
-        return torch.cat([pe[:, 0:1, :], img], dim=1)
+        return super().no_weight_decay() | {"img_pos_embed", "clip_img_pos_embed"}
 
     def forward(self, x, mask=None, use_image=False, x_vis_return_idx=-1, x_vis_only=False):
-        self._check()
-        if not x.is_cuda:
-            raise ll._lib.IvbError("ivb200 PretrainInternVideo2 (stage 2): input must be a CUDA tensor (no CPU fallback)")
-        B, T = x.shape[0], x.shape[2]
-        pe = self.patch_embed
-        ntok = 1 + (T // pe.tubelet_size) * self.num_img_patches
+        B, ntok = x.shape[0], 1 + (x.shape[2] // self.patch_embed.tubelet_size) * self.num_img_patches
+        n_visible = None
         if mask is None:                                      # every token visible (:613-616)
             mask = torch.zeros((B, ntok), dtype=torch.bool, device=x.device)
             n_visible = ntok
-        else:
-            n_visible = None
-        idx, err, n = self.visible_index(mask, n_visible)
-        self.index_error = err
-        h = ops.EmbedFn.apply(x.to(bf16), idx, pe.proj.weight, pe.proj.bias, self.cls_token, self._table("", use_image),
-                              pe.tubelet_size, pe.patch_size[0])
-        rs_all = self._sample_drop_path(B, n, h.device)
-        taps = {}
-        last = self.depth + x_vis_return_idx
-        for i, blk in enumerate(self.blocks):
-            h = blk.forward_stream(h, B, n, None if rs_all is None else (rs_all[2 * i], rs_all[2 * i + 1]))
-            if i in self.return_index:
-                taps[i] = h
-            if i == last:                                     # :631-633
-                break
+        taps, h, idx, B, n = self.forward_features(x, mask, n_visible, use_image=use_image,
+                                                   last=self.depth + x_vis_return_idx)      # early exit (:631-633)
         D = self.embed_dim
         x_vis = h.reshape(B, n, D).to(bf16)
-        x_vis = x_vis + self._index_poison().to(bf16)         # ragged mask -> NaN (the reference's reshape raises)
+        x_vis = x_vis + index_poison(self.index_error).to(bf16)   # ragged mask -> NaN (the reference's reshape raises)
         if x_vis_only:
             return x_vis
         x_pool_vis = self.clip_projector(h.reshape(B, n, D))
         x_align = self.final_clip_decoder(x_pool_vis)
-        cpe = self._table("clip_", use_image)
+        cpe = self._pos_table("clip_", use_image)
         # the reference stacks the taps in block order (x_clip.append inside the loop) and feeds decoder k with tap k
-        order = sorted(taps)
-        clip_in = [ops.GatherAddFn.apply(taps[i], cpe, idx, B, n, 0, 0) for i in order]
+        clip_in = [ops.GatherAddFn.apply(taps[i], cpe, idx, B, n, 0, 0) for i in sorted(taps)]
         x_clip_align = torch.stack([dec(xi).reshape(B, n, -1) for dec, xi in zip(self.clip_decoder, clip_in)])
         return x_vis, x_pool_vis, x_clip_align, x_align
 

@@ -13,16 +13,13 @@ teacher-bound, which is why they run through the same wgmma GEMM / attention ker
 """
 from __future__ import annotations
 
-from functools import partial
-
-import numpy as np
 import torch
 import torch.nn as nn
 
 from . import lowlevel as ll
 from . import ops
-from .modules import (AttentionPoolingBlock, Block, LayerNormB, RMSNorm, bf16, block_precision, f32, to_2tuple,
-                      trunc_normal_)
+from .modules import (LayerNormB, TubeletPatchEmbed, bf16, block_precision, check_input, embed_tokens,
+                      get_sinusoid_encoding_table, init_weights, run_blocks, to_2tuple, vit_stack)
 
 
 # ------------------------------------------------------------------------------------------------ CLIP teacher
@@ -60,16 +57,11 @@ class InternVL_CLIP(nn.Module):
         self.num_patches = self.patch_embed.num_patches
         self.pos_embed = nn.Parameter(torch.zeros(1, self.num_patches + 1, embed_dim), requires_grad=False)
         self.cls_token = nn.Parameter(torch.zeros(1, 1, embed_dim))
-        dpr = [drop_path_rate * i / (depth - 1) if depth > 1 else 0.0 for i in range(depth)]
-        self.blocks = nn.ModuleList([
-            Block(embed_dim, num_heads, mlp_ratio, qkv_bias=qkv_bias, norm_layer=RMSNorm, drop_path=dpr[i],
-                  init_values=init_values, attn_drop=0.0, use_flash_attn=use_flash_attn, use_fused_mlp=use_fused_mlp,
-                  fused_mlp_heuristic=fused_mlp_heuristic, with_cp=False, qk_normalization=qk_normalization,
-                  layerscale_no_force_fp32=layerscale_no_force_fp32, use_fused_rmsnorm=use_fused_rmsnorm)
-            for i in range(depth)])
-        self.clip_projector = AttentionPoolingBlock(dim=embed_dim, num_heads=attn_pool_num_heads, qkv_bias=True,
-                                                    qk_scale=None, drop=0.0, attn_drop=0.0,
-                                                    norm_layer=partial(nn.LayerNorm, eps=1e-5), out_dim=clip_embed_dim)
+        self.blocks, self.clip_projector = vit_stack(
+            embed_dim, depth, num_heads, mlp_ratio, drop_path_rate, attn_pool_num_heads, clip_embed_dim,
+            qkv_bias=qkv_bias, init_values=init_values, use_flash_attn=use_flash_attn, use_fused_mlp=use_fused_mlp,
+            fused_mlp_heuristic=fused_mlp_heuristic, qk_normalization=qk_normalization,
+            layerscale_no_force_fp32=layerscale_no_force_fp32, use_fused_rmsnorm=use_fused_rmsnorm)
 
     @property
     def dtype(self):
@@ -77,20 +69,16 @@ class InternVL_CLIP(nn.Module):
 
     @torch.no_grad()
     def forward(self, image):
-        if self.dtype != bf16 or not image.is_cuda:
-            raise ll._lib.IvbError("ivb200 InternVL_CLIP: bf16 parameters and a CUDA input are required (no CPU path)")
+        check_input(self, image, self.dtype)
         B, C, T, H, W = image.shape
         D, L = self.embed_dim, self.num_patches
         n = L + 1
-        pe = self.patch_embed
         frames = image.to(bf16).permute(0, 2, 1, 3, 4).reshape(B * T, C, 1, H, W).contiguous()   # one sequence per frame
         idx = torch.arange(0, n, device=image.device, dtype=torch.int32).repeat(B * T, 1).contiguous()
-        h = ops.EmbedFn.apply(frames, idx, pe.proj.weight, pe.proj.bias, self.cls_token, self.pos_embed, 1, pe.patch_size[0])
-        z = []
-        for i, blk in enumerate(self.blocks):
-            h = blk.forward_infer(h, B * T, n)
-            if i in self.return_index:
-                z.append(h)
+        h = embed_tokens(self.patch_embed, frames, idx, self.cls_token, self.pos_embed)
+        # forward_infer: under no_grad in train mode forward_stream would draw DropPath factors
+        h, taps = run_blocks(self.blocks, h, lambda i, blk, h: blk.forward_infer(h, B * T, n), self.return_index)
+        z = list(taps.values())
         pooled, attn = self.clip_projector(h.reshape(B * T, n, D), return_attn=self.return_attn)
         if self.clip_norm_type == "l2":
             z = torch.stack(z).reshape(len(z), B, T, n, D)                       # fp32 stream taps
@@ -109,17 +97,6 @@ class InternVL_CLIP(nn.Module):
 
 
 # ------------------------------------------------------------------------------------------------ MAE teacher
-def get_sinusoid_encoding_table(n_position, d_hid):
-    """videomae.py:152-205 for the recipe case n_position == pre_n_position (8 temporal positions, 14x14 or 16x16 grid):
-    the plain 1-D sinusoid table [1, n_position, d_hid] (no interpolation branch)."""
-    pos = np.arange(n_position, dtype=np.float64)[:, None]
-    hid = np.arange(d_hid)[None, :]
-    table = pos / np.power(10000, 2 * (hid // 2) / d_hid)
-    table[:, 0::2] = np.sin(table[:, 0::2])
-    table[:, 1::2] = np.cos(table[:, 1::2])
-    return torch.tensor(table, dtype=torch.float).unsqueeze(0)
-
-
 class TeacherAttention(nn.Module):
     """videomae.py:62-101 (parameter layout: qkv without bias + separate q_bias / v_bias)."""
 
@@ -189,19 +166,6 @@ class TeacherBlock(nn.Module):
             return ops.block_forward(x2d, spec, params, save=False)[0]
 
 
-class TubeletPatchEmbed(nn.Module):
-    """videomae.py:135-149."""
-
-    def __init__(self, img_size=224, patch_size=16, in_chans=3, embed_dim=768, num_frames=16, tubelet_size=2):
-        super().__init__()
-        img_size, patch_size = to_2tuple(img_size), to_2tuple(patch_size)
-        self.tubelet_size = int(tubelet_size)
-        self.img_size, self.patch_size = img_size, patch_size
-        self.num_patches = (img_size[1] // patch_size[1]) * (img_size[0] // patch_size[0]) * (num_frames // self.tubelet_size)
-        self.proj = nn.Conv3d(in_chans, embed_dim, kernel_size=(self.tubelet_size, patch_size[0], patch_size[1]),
-                              stride=(self.tubelet_size, patch_size[0], patch_size[1]))
-
-
 class VisionTransformer(nn.Module):
     """videomae.py:207-313 — the VideoMAEv2 teacher.  forward(x[B,C,T,H,W]) -> [K, B, N, C] L2-normalised features of
     the last K blocks (the final LayerNorm is applied to the last block's output before it is tapped, :291-292)."""
@@ -231,16 +195,7 @@ class VisionTransformer(nn.Module):
             TeacherBlock(embed_dim, num_heads, mlp_ratio, qkv_bias=qkv_bias, qk_scale=qk_scale, norm_layer=mk,
                          init_values=init_values) for _ in range(depth)])
         self.norm = mk(embed_dim)
-        self.apply(self._init_weights)
-
-    def _init_weights(self, m):
-        if isinstance(m, nn.Linear):
-            trunc_normal_(m.weight, std=0.02)
-            if m.bias is not None:
-                nn.init.constant_(m.bias, 0)
-        elif isinstance(m, nn.LayerNorm):
-            nn.init.constant_(m.bias, 0)
-            nn.init.constant_(m.weight, 1.0)
+        self.apply(init_weights)
 
     def get_num_layers(self):
         return len(self.blocks)
@@ -249,26 +204,18 @@ class VisionTransformer(nn.Module):
     def forward(self, x, mask=None):
         if mask is not None:
             raise NotImplementedError("the teacher sees the full clip (engine_for_pretraining.py:102)")
-        w = self.patch_embed.proj.weight
-        if w.dtype != bf16 or not x.is_cuda:
-            raise ll._lib.IvbError("ivb200 VideoMAE teacher: bf16 parameters and a CUDA input are required (no CPU path)")
+        check_input(self, x, self.patch_embed.proj.weight.dtype)
         B = x.shape[0]
         D, N = self.embed_dim, self.patch_embed.num_patches
-        pe = self.patch_embed
-        # EmbedFn embeds tokens idx[:, 1:] and puts `cls + pos[0]` in front: give it a zero cls row and drop it again
         idx = torch.arange(0, N + 1, device=x.device, dtype=torch.int32).repeat(B, 1).contiguous()
-        pos = torch.cat([torch.zeros(1, 1, D, device=x.device), self.pos_embed.to(x.device).float()], 1).to(bf16)   # videomae.py:293
-        zcls = torch.zeros(1, 1, D, device=x.device, dtype=bf16)
-        h = ops.EmbedFn.apply(x.to(bf16), idx, pe.proj.weight, pe.proj.bias, zcls, pos, pe.tubelet_size, pe.patch_size[0])
-        h = h.reshape(B, N + 1, D)[:, 1:].reshape(B * N, D).contiguous()
-        z = []
-        for i, blk in enumerate(self.blocks):
+        h = embed_tokens(self.patch_embed, x, idx, None, self.pos_embed.to(x.device).float())     # videomae.py:293
+
+        def block(i, blk, h):
             h = blk.forward_infer(h, B, N, self.head_axis_attention)
-            if i == self.depth - 1:
-                h = self.norm(h)                                                   # bf16 [B*N, D]
-            if i in self.return_index:
-                z.append(h.float().reshape(B, N, D))
-        out = torch.stack(z)
+            return self.norm(h) if i == self.depth - 1 else h                     # bf16 [B*N, D] after the last
+
+        h, taps = run_blocks(self.blocks, h, block, self.return_index)
+        out = torch.stack([t.float().reshape(B, N, D) for t in taps.values()])
         if self.mae_norm_type == "l2":
             out = out / out.norm(dim=-1, keepdim=True)
         elif self.mae_norm_type != "none":

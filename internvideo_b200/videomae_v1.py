@@ -20,30 +20,17 @@ from __future__ import annotations
 
 from functools import partial
 
-import numpy as np
 import torch
 import torch.nn as nn
 
 from . import lowlevel as ll
 from . import ops
+from .modules import TubeletPatchEmbed as PatchEmbed  # modeling_finetune.py:184-219 (parameters; im2col + GEMM)
+from .modules import bf16, check_input, embed_tokens, f32, get_sinusoid_encoding_table, index_poison, run_blocks
+from .modules import to_2tuple  # noqa: F401  (a name of the reference module)
 
-bf16, f32 = torch.bfloat16, torch.float32
 IMAGENET_DEFAULT_MEAN = (0.485, 0.456, 0.406)
 IMAGENET_DEFAULT_STD = (0.229, 0.224, 0.225)
-
-
-def to_2tuple(x):
-    return tuple(x) if isinstance(x, (tuple, list)) else (x, x)
-
-
-def get_sinusoid_encoding_table(n_position, d_hid):
-    """modeling_finetune.py:224-242 — [1, n_position, d_hid] fp32, sin on even / cos on odd channels."""
-    pos = np.arange(n_position, dtype=np.float64)[:, None]
-    j = np.arange(d_hid)[None, :]
-    table = pos / np.power(10000, 2 * (j // 2) / d_hid)
-    table[:, 0::2] = np.sin(table[:, 0::2])
-    table[:, 1::2] = np.cos(table[:, 1::2])
-    return torch.tensor(table, dtype=torch.float, requires_grad=False).unsqueeze(0)
 
 
 def _drop_path_rows(a, B, n, p, training):
@@ -134,18 +121,14 @@ class Block(nn.Module):
         return self.forward_rows(x.reshape(B * n, D).float(), B, n).reshape(B, n, D)
 
 
-class PatchEmbed(nn.Module):
-    """modeling_finetune.py:184-219 (parameters only; the convolution runs as im2col of the visible patches + GEMM)."""
-
-    def __init__(self, img_size=224, patch_size=16, in_chans=3, embed_dim=768, num_frames=16, tubelet_size=2):
-        super().__init__()
-        img_size, patch_size = to_2tuple(img_size), to_2tuple(patch_size)
-        self.tubelet_size = int(tubelet_size)
-        self.num_patches = (img_size[1] // patch_size[1]) * (img_size[0] // patch_size[0]) * (num_frames // self.tubelet_size)
-        self.img_size, self.patch_size = img_size, patch_size
-        self.proj = nn.Conv3d(in_channels=in_chans, out_channels=embed_dim,
-                              kernel_size=(self.tubelet_size, patch_size[0], patch_size[1]),
-                              stride=(self.tubelet_size, patch_size[0], patch_size[1]))
+def _run_blocks(blocks, h, B, n, with_cp):
+    """The encoder's and the decoder's block loop over the fp32 stream [B*n, D]; with_cp: each block keeps only its
+    input and recomputes its forward in backward (torch.utils.checkpoint)."""
+    def block(i, blk, h):
+        if with_cp and torch.is_grad_enabled():
+            return torch.utils.checkpoint.checkpoint(blk.forward_rows, h, B, n, use_reentrant=False)
+        return blk.forward_rows(h, B, n)
+    return run_blocks(blocks, h, block)[0]
 
 
 def _xavier_init(m):
@@ -207,25 +190,15 @@ class PretrainVisionTransformerEncoder(nn.Module):
     def forward_rows(self, x, idx, B, nv):
         """x bf16 video, idx int32 [B, 1+nv] (cls slot + visible patches) -> bf16 [B*nv, C_e] after the final LayerNorm."""
         pe = self.patch_embed
-        D = self.embed_dim
         pos = self.pos_embed[:, -pe.num_patches:].to(device=x.device)          # learnable table has an unused first row
-        # EmbedFn embeds tokens idx[:, 1:] and puts `cls + pos[0]` in front: give it a zero cls row and drop it again
-        table = torch.cat([torch.zeros(1, 1, D, device=x.device, dtype=pos.dtype), pos], 1).to(bf16)
-        zcls = torch.zeros(1, 1, D, device=x.device, dtype=bf16)
-        h = ops.EmbedFn.apply(x, idx, pe.proj.weight, pe.proj.bias, zcls, table, pe.tubelet_size, pe.patch_size[0])
-        h = h.reshape(B, nv + 1, D)[:, 1:].reshape(B * nv, D)
-        for blk in self.blocks:
-            if self.with_cp and torch.is_grad_enabled():
-                h = torch.utils.checkpoint.checkpoint(blk.forward_rows, h, B, nv, use_reentrant=False)
-            else:
-                h = blk.forward_rows(h, B, nv)
+        h = _run_blocks(self.blocks, embed_tokens(pe, x, idx, None, pos), B, nv, self.with_cp)
         h = ops.layernorm(h, self.norm.weight, self.norm.bias, self.norm.eps)
         if isinstance(self.head, nn.Linear):
             h = ops.linear(h, self.head.weight, self.head.bias)
         return h
 
     def forward(self, x, mask):
-        _check_input(self.patch_embed.proj.weight, x)
+        check_input(self, x, self.patch_embed.proj.weight.dtype)
         idx, err, nv = kept_indices(mask.to(x.device))
         B = x.shape[0]
         return self.forward_rows(x.to(bf16), idx, B, nv).reshape(B, nv, -1)
@@ -257,11 +230,7 @@ class PretrainVisionTransformerDecoder(nn.Module):
 
     def forward_rows(self, h, B, N, return_token_num):
         """h fp32 [B*N, C_d] -> bf16 [B, return_token_num (or N), num_classes]."""
-        for blk in self.blocks:
-            if self.with_cp and torch.is_grad_enabled():
-                h = torch.utils.checkpoint.checkpoint(blk.forward_rows, h, B, N, use_reentrant=False)
-            else:
-                h = blk.forward_rows(h, B, N)
+        h = _run_blocks(self.blocks, h, B, N, self.with_cp)
         C = h.shape[-1]
         h = h.reshape(B, N, C)
         if return_token_num > 0:
@@ -275,13 +244,6 @@ class PretrainVisionTransformerDecoder(nn.Module):
     def forward(self, x, return_token_num):
         B, N, C = x.shape
         return self.forward_rows(x.reshape(B * N, C).float(), B, N, return_token_num)
-
-
-def _check_input(w, x):
-    if w.dtype != bf16:
-        raise ll._lib.IvbError("ivb200 VideoMAE computes in bf16: call model.bfloat16() first")
-    if not x.is_cuda:
-        raise ll._lib.IvbError("ivb200 VideoMAE: input must be a CUDA tensor (no CPU fallback)")
 
 
 class PretrainVisionTransformer(nn.Module):
@@ -320,7 +282,7 @@ class PretrainVisionTransformer(nn.Module):
 
     def forward(self, x, mask, return_indices=False, n_masked=None):
         """n_masked: masked tubelets per clip when known (the recipes use a fixed ratio): no host read of the mask."""
-        _check_input(self.encoder.patch_embed.proj.weight, x)
+        check_input(self, x, self.encoder.patch_embed.proj.weight.dtype)
         B = x.shape[0]
         mask = mask.to(x.device)
         N = mask.shape[1]
@@ -334,13 +296,8 @@ class PretrainVisionTransformer(nn.Module):
         pos_msk = pos[(msk[:, 1:] - 1).long()]
         x_full = torch.cat([h + pos_vis, self.mask_token.float() + pos_msk], dim=1)           # :380-383
         out = self.decoder.forward_rows(x_full.reshape(B * N, -1), B, N, nm)
-        out = out + _poison(self.index_error).to(out.dtype)
+        out = out + index_poison(self.index_error).to(out.dtype)
         return (out, msk[:, 1:] - 1) if return_indices else out
-
-
-def _poison(err):
-    z = torch.zeros((), device=err.device, dtype=f32)
-    return torch.where(err[0] != 0, torch.full_like(z, float("nan")), z)
 
 
 def pixel_labels(images, masked_idx, patch_size, tubelet_size=2, normalize_target=True):
