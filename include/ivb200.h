@@ -145,12 +145,13 @@ int ivb_norm_fwd_fp8(const void* x, int x_is_f32, long ldx, const void* weight, 
  * y(bf16) = norm(x) * weight (+ bias).  is_layernorm=0: RMSNorm (internvideo2_pretrain.py:117-128,
  * FA2 DropoutAddRMSNorm :467; eps 1e-6); 1: nn.LayerNorm (eps 1e-5, :525,:532).
  * x is fp32 (x_is_f32=1, the fp32 residual stream) or bf16.  rstd[M] (and mean[M] for LayerNorm)
- * are written for the backward pass.                                                              */
+ * are written for the backward pass.  bias, mean and rstd may be NULL.                            */
 int ivb_norm_fwd(const void* x, int x_is_f32, long ldx, const void* weight, const void* bias,
                  float eps, int is_layernorm, int M, int D, void* y, long ldy, float* mean,
                  float* rstd, void* stream);
 /* dx = d norm / dx (+ dx_in, fp32, pitch lddx_in, optional); dweight/dbias: fp32 [D], ACCUMULATED
- * (summed in a fixed order) — zero them first.  dx_out is fp32 or bf16.  In-place dx_out == dy is allowed.      */
+ * (summed in a fixed order) — zero them first, or NULL.  mean is NULL for RMSNorm.  dx_out is fp32 or bf16.
+ * In-place dx_out == dy is allowed.                                                              */
 int ivb_norm_bwd(const void* dy, long lddy, const void* x, int x_is_f32, long ldx,
                  const void* weight, const float* mean, const float* rstd, int is_layernorm, int M,
                  int D, const float* dx_in, long lddx_in, void* dx_out, int dx_out_is_f32,
@@ -167,7 +168,7 @@ int ivb_rmsnorm_pair_bwd(const void* dy, long lddy, long dy_pair_off, const void
 /* RMSNorm backward on the fp32 residual stream FUSED with the LayerScale backward that consumes its result in Block.backward
  * (internvideo2_pretrain.py:284-291 differentiated): dx_out = rmsnorm_bwd(dy, x, w, rstd) + dx_in (fp32 [M,D]);
  * dyb (bf16) = rowscale[m] * gamma * dx_out; dgamma += sum_m rowscale*dx_out*ybr; dcolsum += gamma * sum_m rowscale*dx_out;
- * dweight += RMSNorm weight gradient.  rowscale (DropPath factors) and dx_in are optional. */
+ * dweight += RMSNorm weight gradient.  rowscale (DropPath factors), dx_in, dweight, dgamma and dcolsum are optional. */
 int ivb_rmsnorm_bwd_layerscale(const void* dy, long lddy, const float* x, long ldx, const void* weight, const float* rstd,
                                int M, int D, const float* dx_in, long lddx_in, float* dx_out, long lddx, float* dweight,
                                const void* ybr, long ldyb, const void* gamma, const float* rowscale, void* dyb, long lddyb,
@@ -175,7 +176,7 @@ int ivb_rmsnorm_bwd_layerscale(const void* dy, long lddy, const float* x, long l
 /* ---- LayerScale backward (internvideo2_pretrain.py:131-146 + residual :284-291) -----------------
  * dx' = rowscale[m] * dx (rowscale optional: DropPath); dy(bf16) = gamma * dx' ;
  * dgamma[j] += sum_m dx'*y ; dcolsum[j] += gamma[j] * sum_m dx'  (= the branch Linear's bias gradient).
- * gamma may be NULL (no LayerScale: dy = dx').                                                     */
+ * gamma may be NULL (no LayerScale: dy = dx'); y, dgamma and dcolsum may be NULL.                 */
 int ivb_layerscale_bwd(const float* dx, long lddx, const void* y, long ldy, const void* gamma,
                        int M, int D, void* dy, long lddy, float* dgamma, float* dcolsum,
                        const float* rowscale, void* stream);
@@ -226,8 +227,8 @@ int ivb_im2col_visible(const void* video, const int* idx, int idx_stride, int j0
 int ivb_gather_add(const float* src, long src_bstride, const void* table, const int* idx,
                    int idx_bstride, int idx_off, int B, int rows, int D, void* out, int out_is_f32,
                    long out_bstride, void* stream);
-/* table_grad[idx[b,j] + idx_off, :] += g[b,j,:]  (fp32) — backward of ivb_gather_add.  Clips are added in order;
- * when idx[b,:] has no repeats within a clip the result is the same on every run. */
+/* table_grad[idx[b,j] + idx_off, :] += g[b,j,:]  (fp32) — backward of ivb_gather_add (idx NULL means j).  Clips are
+ * added in order; when idx[b,:] has no repeats within a clip the result is the same on every run. */
 int ivb_scatter_add(const void* g, int g_is_f32, long g_bstride, const int* idx, int idx_bstride,
                     int idx_off, int B, int rows, int D, float* table_grad, void* stream);
 
@@ -238,8 +239,8 @@ int ivb_scatter_add(const void* g, int g_is_f32, long g_bstride, const int* idx,
 int ivb_ln_l2_fwd(const void* z, long ldz, const void* weight, const void* bias, float eps, int M,
                   int C, void* out, long ldo, float* stats, const void* target, int target_is_f32,
                   long ldt, float* loss_sum, void* stream);
-/* d_out = (gscale_host * *gscale_dev) * dout.  For the fused loss pass dout = target and
- * gscale_host = -2/rows.  Writes dz (bf16); accumulates dweight/dbias (fp32).                    */
+/* d_out = (gscale_host * *gscale_dev) * dout (gscale_dev NULL: 1).  For the fused loss pass dout = target and
+ * gscale_host = -2/rows.  Writes dz (bf16); accumulates dweight/dbias (fp32, optional).          */
 int ivb_ln_l2_bwd(const void* z, long ldz, const void* weight, const void* bias, const float* stats,
                   int M, int C, const void* dout, int dout_is_f32, long lddo, float gscale_host,
                   const float* gscale_dev, void* dz, long lddz, float* dweight, float* dbias,
@@ -252,7 +253,8 @@ int ivb_ln_l2_bwd(const void* z, long ldz, const void* weight, const void* bias,
  * (internvideo2_clip_small.py:45,96-99), no host read per step, valid inside a captured CUDA graph.  */
 int ivb_vtc_loss_fwd(const float* cos_v2t, const long long* idx, int G, float temp,
                      const float* temp_dev, float* lse_row, float* lse_col, float* loss, void* stream);
-/* dcos (bf16 [G,G]) = d loss / d cos_v2t * gscale; *dtemp += d loss / d temp * gscale.              */
+/* dcos (bf16 [G,G]) = d loss / d cos_v2t * gscale; *dtemp += d loss / d temp * gscale, with gscale = gscale_host *
+ * *gscale_dev (gscale_dev optional).                                                                */
 int ivb_vtc_loss_bwd(const float* cos_v2t, const long long* idx, int G, float temp,
                      const float* temp_dev, const float* lse_row, const float* lse_col, float gscale_host,
                      const float* gscale_dev, void* dcos_bf16, float* dtemp, void* stream);
@@ -268,7 +270,8 @@ int ivb_l2norm_rows_bwd(const float* dy, long lddy, const void* xn, long ldxn, c
 int ivb_pixel_targets(const void* video, const int* masked_idx, int n_mask, int B, int C, int T,
                       int H, int W, int tubelet, int patch, int normalize, const float* mean3,
                       const float* std3, float* labels, void* stream);
-/* *loss_sum += sum (pred-label)^2 ; dpred (bf16, optional) = gscale * 2 (pred-label).               */
+/* *loss_sum += sum (pred-label)^2 ; dpred (bf16, optional) = gscale * 2 (pred-label), gscale = gscale_host *
+ * *gscale_dev.  loss_sum and gscale_dev are optional.                                               */
 int ivb_mse_loss(const void* pred_bf16, const float* label, long n, float* loss_sum,
                  float gscale_host, const float* gscale_dev, void* dpred_bf16, void* stream);
 
@@ -284,7 +287,8 @@ int ivb_pool_attn_bwd(const void* q, const void* k, long ldk, const void* v, lon
 
 /* ---- flat AdamW (decoupled weight decay; fp32 master/moments, bf16 model copy) --------------------
  * torch.optim.AdamW semantics (optim_factory.py:141-142; DeepSpeed adam_w_mode utils.py:821-834).
- * Gradients are multiplied by grad_scale * (*grad_scale_dev) first (1/world_size, clip coefficient). */
+ * Gradients are multiplied by grad_scale * (*grad_scale_dev) first (1/world_size, clip coefficient; grad_scale_dev
+ * optional). */
 int ivb_adamw_step(float* master, float* exp_avg, float* exp_avg_sq, const void* grad,
                    int grad_is_f32, void* param_bf16, long n, float lr, float beta1, float beta2,
                    float eps, float weight_decay, int step, float grad_scale,

@@ -1,66 +1,48 @@
 """ctypes binding of libivb200.so (the C ABI in include/ivb200.h).
 
-There is no fallback: if the shared library is missing, or a compute entry point is called
-without an H100-class (sm_90) device, an exception is raised.
+The header is the only declaration of the ABI: load() attaches the prototypes parse_prototypes() reads from it.
+There is no fallback: if the shared library is missing, or a compute entry point is called without an H100-class
+(sm_90) device, an exception is raised.
 """
 from __future__ import annotations
 
 import ctypes as C
 import os
+import re
 from pathlib import Path
 
 _PKG = Path(__file__).resolve().parent
 LIB_PATH = _PKG / "libivb200.so"
+HEADER = _PKG.parent / "include" / "ivb200.h"
 
-_vp, _i, _l, _f = C.c_void_p, C.c_int, C.c_long, C.c_float
+_SCALARS = {"int": C.c_int, "long": C.c_long, "float": C.c_float, "void": None}
 
-# name -> (restype, argtypes); must list every symbol declared in include/ivb200.h
-PROTOTYPES = {
-    "ivb_last_error": (C.c_char_p, []),
-    "ivb_version": (_i, []),
-    "ivb_device_check": (_i, []),
-    "ivb_launch_count": (_l, []),
-    "ivb_reset_launch_count": (None, []),
-    "ivb_set_default_2cta": (None, [_i]),
-    "ivb_gemm_bf16": (_i, [_vp, _i, _l, _vp, _i, _l, _i, _i, _i, _i, _i, _vp, _l, _vp, _l, _vp, _vp,
-                           _vp, _l, _vp, _i, _vp]),
-    "ivb_fp8_quantize": (_i, [_vp, _l, _i, _i, _i, _vp, _l, _vp, _l, _vp, _vp, _vp]),
-    "ivb_gemm_fp8": (_i, [_vp, _i, _l, _i, _vp, _vp, _i, _l, _vp, _i, _i, _i, _i, _i, _vp, _l, _vp, _l, _vp, _vp,
-                          _vp, _l, _vp, _i, _vp]),
-    "ivb_fp8_quantize_rows": (_i, [_vp, _l, _i, _i, _vp, _l, _vp, _vp]),
-    "ivb_norm_fwd_fp8": (_i, [_vp, _i, _l, _vp, _vp, _f, _i, _i, _i, _vp, _l, _vp, _vp]),
-    "ivb_norm_fwd": (_i, [_vp, _i, _l, _vp, _vp, _f, _i, _i, _i, _vp, _l, _vp, _vp, _vp]),
-    "ivb_norm_bwd": (_i, [_vp, _l, _vp, _i, _l, _vp, _vp, _vp, _i, _i, _i, _vp, _l, _vp, _i, _l,
-                          _vp, _vp, _vp]),
-    "ivb_rmsnorm_pair_fwd": (_i, [_vp, _l, _l, _vp, _vp, _f, _i, _i, _vp, _l, _l, _vp, _vp]),
-    "ivb_rmsnorm_pair_bwd": (_i, [_vp, _l, _l, _vp, _l, _l, _vp, _vp, _vp, _i, _i, _vp, _l, _l, _vp, _vp, _vp]),
-    "ivb_rmsnorm_bwd_layerscale": (_i, [_vp, _l, _vp, _l, _vp, _vp, _i, _i, _vp, _l, _vp, _l, _vp, _vp, _l, _vp, _vp, _vp, _l,
-                                        _vp, _vp, _vp]),
-    "ivb_layerscale_bwd": (_i, [_vp, _l, _vp, _l, _vp, _i, _i, _vp, _l, _vp, _vp, _vp, _vp]),
-    "ivb_colsum_bf16": (_i, [_vp, _l, _i, _i, _vp, _vp]),
-    "ivb_attn_fwd": (_i, [_vp, _l, _vp, _l, _vp, _l, _vp, _l, _vp, _i, _i, _i, _i, _f, _vp]),
-    "ivb_headaxis_attn_fwd": (_i, [_vp, _l, _i, _i, _i, _i, _f, _vp, _vp]),
-    "ivb_attn_bwd": (_i, [_vp, _l, _vp, _l, _vp, _l, _vp, _l, _vp, _l, _vp, _vp, _vp, _l, _vp, _l,
-                          _vp, _l, _i, _i, _i, _i, _f, _vp]),
-    "ivb_attn_bwd_workspace_floats": (_l, [_i, _i, _i]),
-    "ivb_visible_indices": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp]),
-    "ivb_im2col_visible": (_i, [_vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp]),
-    "ivb_gather_add": (_i, [_vp, _l, _vp, _vp, _i, _i, _i, _i, _i, _vp, _i, _l, _vp]),
-    "ivb_scatter_add": (_i, [_vp, _i, _l, _vp, _i, _i, _i, _i, _i, _vp, _vp]),
-    "ivb_ln_l2_fwd": (_i, [_vp, _l, _vp, _vp, _f, _i, _i, _vp, _l, _vp, _vp, _i, _l, _vp, _vp]),
-    "ivb_ln_l2_bwd": (_i, [_vp, _l, _vp, _vp, _vp, _i, _i, _vp, _i, _l, _f, _vp, _vp, _l, _vp, _vp, _vp]),
-    "ivb_vtc_loss_fwd": (_i, [_vp, _vp, _i, _f, _vp, _vp, _vp, _vp, _vp]),
-    "ivb_vtc_loss_bwd": (_i, [_vp, _vp, _i, _f, _vp, _vp, _vp, _f, _vp, _vp, _vp, _vp]),
-    "ivb_l2norm_rows_fwd": (_i, [_vp, _i, _l, _i, _i, _vp, _l, _vp, _vp]),
-    "ivb_l2norm_rows_bwd": (_i, [_vp, _l, _vp, _l, _vp, _i, _i, _vp, _l, _vp]),
-    "ivb_pixel_targets": (_i, [_vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp]),
-    "ivb_mse_loss": (_i, [_vp, _vp, _l, _vp, _f, _vp, _vp, _vp]),
-    "ivb_pool_attn_fwd": (_i, [_vp, _vp, _l, _vp, _l, _i, _i, _i, _i, _f, _vp, _vp, _vp]),
-    "ivb_pool_attn_bwd": (_i, [_vp, _vp, _l, _vp, _l, _vp, _vp, _i, _i, _i, _i, _f, _vp, _vp, _l, _vp, _l, _vp]),
-    "ivb_adamw_step": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _l, _f, _f, _f, _f, _f, _i, _f, _vp, _vp, _vp]),
-    "ivb_nvls_allreduce_bf16": (_i, [_vp, _l, _l, _vp, _i, _i, _i, _vp]),
-    "ivb_nvls_flag_words": (_i, []),
-}
+
+def _ctype(decl: str, ret: bool = False):
+    """ctypes type of a C return type, or of a parameter declaration (type and name).  Every pointer is c_void_p, except
+    a `const char*` return (c_char_p); a scalar type the binding does not know raises."""
+    if "*" in decl:
+        return C.c_char_p if ret and "".join(decl.split()) == "constchar*" else C.c_void_p
+    words = [w for w in decl.split() if w != "const"]
+    base = " ".join(words if ret else words[:-1])
+    if base not in _SCALARS:
+        raise ValueError(f"unknown C type in {decl!r}")
+    return _SCALARS[base]
+
+
+def parse_prototypes(header: str) -> dict:
+    """{name: (restype, argtypes)} for every ivb_* function declared in the C header text."""
+    text = re.sub(r"/\*.*?\*/|//[^\n]*", "", header, flags=re.S)
+    text = re.sub(r"^\s*#[^\n]*", "", text, flags=re.M)
+    protos = {}
+    for ret, name, params in re.findall(r"([\w\s*]+?)\s*\b(ivb_\w+)\s*\(([^()]*)\)\s*;", text):
+        params = " ".join(params.split())
+        args = [] if params in ("", "void") else [_ctype(p) for p in params.split(",")]
+        protos[name] = (_ctype(ret, ret=True), args)
+    return protos
+
+
+PROTOTYPES = parse_prototypes(HEADER.read_text())
 
 _lib = None
 
@@ -99,7 +81,5 @@ def check(rc: int, what: str = "") -> None:
 
 def header_symbols() -> list[str]:
     """Function names declared in include/ivb200.h (used by the CPU ABI test)."""
-    import re
-    text = (_PKG.parent / "include" / "ivb200.h").read_text()
-    text = re.sub(r"/\*.*?\*/", "", text, flags=re.S)
+    text = re.sub(r"/\*.*?\*/", "", HEADER.read_text(), flags=re.S)
     return sorted(set(re.findall(r"\b(ivb_[a-z0-9_]+)\s*\(", text)))

@@ -193,7 +193,7 @@ extern "C" int ivb_attn_fwd(const void* q, long ldq, const void* k, long ldk, co
   if ((rc = make_head_tmap(&tv, v, ldv, B, n, H, d, ATT_COLS))) return rc;
   const AttnFwdParams p{B, n, H, d, softmax_scale * 1.4426950408889634f, reinterpret_cast<__nv_bfloat16*>(out), ldo, lse2};
   return dispatch_head_dim(d, [&](auto hd) {
-    return launch_attn<attn_fwd_kernel<hd.KA, hd.NO, hd.KS>, false>(
+    return launch_attn<attn_fwd_kernel<hd.KA, hd.NO, hd.KS>, NO_PDL>(
         "cudaFuncSetAttribute(attn_fwd)", "attn_fwd_kernel", FwdSmem<hd.KA>::BYTES, B, n, H, stream, tq, tk, tv, p);
   });
 }
@@ -278,8 +278,7 @@ extern "C" int ivb_headaxis_attn_fwd(const void* qkv, long ld, int B, int N, int
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return set_error_cuda("cudaFuncSetAttribute(headaxis_attn)", e);
   }
-  kern<<<(unsigned)((toks + 3) / 4), 128, smem, stream>>>(reinterpret_cast<const __nv_bfloat16*>(qkv), ld, B, N, H, d,
-                                                          softmax_scale, reinterpret_cast<__nv_bfloat16*>(out));
-  count_launch();
-  return check_launch("headaxis_attn_kernel");
+  return launch("headaxis_attn_kernel", kern, (unsigned)((toks + 3) / 4), 128, smem, stream, NO_PDL,
+                reinterpret_cast<const __nv_bfloat16*>(qkv), ld, B, N, H, d, softmax_scale,
+                reinterpret_cast<__nv_bfloat16*>(out));
 }

@@ -156,23 +156,12 @@ int dispatch_head_dim(int d, F&& f) {
 }
 
 // Raises Kern's shared-memory limit (`attr` names that call in an error) and launches it on one CTA per (128-row block,
-// head, clip), through launch_pdl when PDL.
-template <auto Kern, bool PDL, class... Args>
+// head, clip); the forward passes NO_PDL and the backward ALLOW_PDL.
+template <auto Kern, LaunchPdl PDL, class... Args>
 int launch_attn(const char* attr, const char* name, int smem, int B, int n, int H, cudaStream_t stream,
                 const Args&... args) {
   if (int rc = raise_smem_limit<Kern>(smem, attr)) return rc;
-  const dim3 grid((n + ATT_ROWS - 1) / ATT_ROWS, H, B);
-  if constexpr (PDL) {
-    if (const cudaError_t e = launch_pdl(Kern, grid, dim3(ATT_THREADS), smem, stream, args...)) {
-      char what[64];
-      snprintf(what, sizeof(what), "launch(%s)", name);
-      return set_error_cuda(what, e);
-    }
-  } else {
-    Kern<<<grid, ATT_THREADS, smem, stream>>>(args...);
-  }
-  count_launch();
-  return check_launch(name);
+  return launch(name, Kern, dim3((n + ATT_ROWS - 1) / ATT_ROWS, H, B), ATT_THREADS, smem, stream, PDL, args...);
 }
 
 }  // namespace ivb

@@ -214,11 +214,10 @@ extern "C" int ivb_attn_bwd(const void* q, long ldq, const void* k, long ldk, co
   if (cudaError_t e = cudaMemsetAsync(delta_ws, 0, 2 * half * sizeof(float), stream))   // zero padding (0 * pad must stay 0)
     return set_error_cuda("cudaMemsetAsync(attn_bwd workspace)", e);
   const long total = static_cast<long>(B) * n * H;
-  attn_bwd_prep_kernel<<<(unsigned)((total + 127) / 128), 128, 0, stream>>>(
-      reinterpret_cast<const __nv_bfloat16*>(out), ldo, reinterpret_cast<const __nv_bfloat16*>(dout),
-      lddo, lse2, lse2p, deltap, B, n, n_pad, H, d);
-  count_launch();
-  if ((rc = check_launch("attn_bwd_prep_kernel"))) return rc;
+  if ((rc = launch("attn_bwd_prep_kernel", attn_bwd_prep_kernel, (unsigned)((total + 127) / 128), 128, 0, stream, NO_PDL,
+                   reinterpret_cast<const __nv_bfloat16*>(out), ldo, reinterpret_cast<const __nv_bfloat16*>(dout),
+                   lddo, lse2, lse2p, deltap, B, n, n_pad, H, d)))
+    return rc;
   // q, dO, k, v, each with a 128-row box (the rows a CTA owns) and a 64-row box (a streamed tile)
   const void* src[4] = {q, dout, k, v};
   const long ld[4] = {ldq, lddo, ldk, ldv};
@@ -234,10 +233,11 @@ extern "C" int ivb_attn_bwd(const void* q, long ldq, const void* k, long ldk, co
   return dispatch_head_dim(d, [&](auto hd) {
     constexpr int smem = BwdSmem<hd.KA>::BYTES;
     const char* attr = "cudaFuncSetAttribute(attn_bwd)";
-    if ((rc = launch_attn<attn_bwd_kernel<1, hd.KA, hd.NO, hd.KS>, true>(attr, "attn_bwd_kernel", smem, B, n, H, stream,
-                                                                          rows[2], rows[3], tiles[0], tiles[1], pkv)))
+    if ((rc = launch_attn<attn_bwd_kernel<1, hd.KA, hd.NO, hd.KS>, ALLOW_PDL>(attr, "attn_bwd_kernel", smem, B, n, H,
+                                                                               stream, rows[2], rows[3], tiles[0],
+                                                                               tiles[1], pkv)))
       return rc;
-    return launch_attn<attn_bwd_kernel<0, hd.KA, hd.NO, hd.KS>, true>(attr, "attn_bwd_kernel", smem, B, n, H, stream,
-                                                                       rows[0], rows[1], tiles[2], tiles[3], pq);
+    return launch_attn<attn_bwd_kernel<0, hd.KA, hd.NO, hd.KS>, ALLOW_PDL>(attr, "attn_bwd_kernel", smem, B, n, H, stream,
+                                                                            rows[0], rows[1], tiles[2], tiles[3], pq);
   });
 }

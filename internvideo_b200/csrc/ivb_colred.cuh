@@ -98,9 +98,8 @@ static inline int colred_check(int nout, long nslots, int D, const char* who) {
 // dst_o[col] += sum over slots (in slot order) of the partials of output o, for the non-null outputs among o0..o2.
 static inline int colred_finish(int nout, int nslots, int D, float* o0, float* o1, float* o2, cudaStream_t stream) {
   if (o0 == nullptr && o1 == nullptr && o2 == nullptr) return 0;
-  colred_finish_kernel<<<dim3((D + 255) / 256, nout), 256, 0, stream>>>(nslots, D, o0, o1, o2);
-  count_launch();
-  return check_launch("colred_finish_kernel");
+  return launch("colred_finish_kernel", colred_finish_kernel, dim3((D + 255) / 256, nout), 256, 0, stream, NO_PDL, nslots,
+                D, o0, o1, o2);
 }
 
 }  // namespace ivb

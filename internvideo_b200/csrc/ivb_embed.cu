@@ -142,10 +142,8 @@ extern "C" int ivb_visible_indices(const void* mask_u8, int B, int N, int n_keep
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (B <= 0) return 0;
   const int wpb = 4;
-  visible_indices_kernel<<<(B + wpb - 1) / wpb, wpb * 32, 0, stream>>>(
-      reinterpret_cast<const uint8_t*>(mask_u8), B, N, n_keep, idx, err_flag);
-  count_launch();
-  return check_launch("visible_indices_kernel");
+  return launch("visible_indices_kernel", visible_indices_kernel, (B + wpb - 1) / wpb, wpb * 32, 0, stream, NO_PDL,
+                reinterpret_cast<const uint8_t*>(mask_u8), B, N, n_keep, idx, err_flag);
 }
 
 extern "C" int ivb_im2col_visible(const void* video, const int* idx, int idx_stride, int j0,
@@ -157,11 +155,9 @@ extern "C" int ivb_im2col_visible(const void* video, const int* idx, int idx_str
     return set_error("ivb_im2col_visible: patch/W must be even, Kpad a multiple of 8 and >= C*t*p*p");
   const long rows = static_cast<long>(B) * rows_per_clip;
   const int wpb = 8;
-  im2col_visible_kernel<<<(unsigned)((rows + wpb - 1) / wpb), wpb * 32, 0, stream>>>(
-      reinterpret_cast<const __nv_bfloat16*>(video), idx, idx_stride, j0, rows_per_clip, B, C, T, H, W,
-      tubelet, patch, Kpad, reinterpret_cast<__nv_bfloat16*>(cols));
-  count_launch();
-  return check_launch("im2col_visible_kernel");
+  return launch("im2col_visible_kernel", im2col_visible_kernel, (unsigned)((rows + wpb - 1) / wpb), wpb * 32, 0, stream,
+                NO_PDL, reinterpret_cast<const __nv_bfloat16*>(video), idx, idx_stride, j0, rows_per_clip, B, C, T, H, W,
+                tubelet, patch, Kpad, reinterpret_cast<__nv_bfloat16*>(cols));
 }
 
 extern "C" int ivb_gather_add(const float* src, long src_bstride, const void* table, const int* idx,
@@ -174,12 +170,8 @@ extern "C" int ivb_gather_add(const float* src, long src_bstride, const void* ta
   const int wpb = 8;
   const unsigned grid = (unsigned)((total + wpb - 1) / wpb);
   const __nv_bfloat16* t = reinterpret_cast<const __nv_bfloat16*>(table);
-  if (out_is_f32)
-    gather_add_kernel<true><<<grid, wpb * 32, 0, stream>>>(src, src_bstride, t, idx, idx_bstride, idx_off, B, rows, D, out, out_bstride);
-  else
-    gather_add_kernel<false><<<grid, wpb * 32, 0, stream>>>(src, src_bstride, t, idx, idx_bstride, idx_off, B, rows, D, out, out_bstride);
-  count_launch();
-  return check_launch("gather_add_kernel");
+  return launch("gather_add_kernel", out_is_f32 ? gather_add_kernel<true> : gather_add_kernel<false>, grid, wpb * 32, 0,
+                stream, NO_PDL, src, src_bstride, t, idx, idx_bstride, idx_off, B, rows, D, out, out_bstride);
 }
 
 extern "C" int ivb_scatter_add(const void* g, int g_is_f32, long g_bstride, const int* idx,
@@ -195,14 +187,12 @@ extern "C" int ivb_scatter_add(const void* g, int g_is_f32, long g_bstride, cons
   const unsigned grid = (unsigned)((rows + wpb - 1) / wpb);
   const char* gb = reinterpret_cast<const char*>(g);
   const long gstep = g_bstride * (g_is_f32 ? 4 : 2);
+  const auto kern = g_is_f32 ? scatter_add_kernel<true> : scatter_add_kernel<false>;
   for (int b = 0; b < B; ++b) {
     const int* ib = idx ? idx + static_cast<long>(b) * idx_bstride : nullptr;
-    if (g_is_f32)
-      scatter_add_kernel<true><<<grid, wpb * 32, 0, stream>>>(gb + b * gstep, g_bstride, ib, idx_bstride, idx_off, 1, rows, D, table_grad);
-    else
-      scatter_add_kernel<false><<<grid, wpb * 32, 0, stream>>>(gb + b * gstep, g_bstride, ib, idx_bstride, idx_off, 1, rows, D, table_grad);
-    count_launch();
-    if (int rc = check_launch("scatter_add_kernel")) return rc;
+    if (int rc = launch("scatter_add_kernel", kern, grid, wpb * 32, 0, stream, NO_PDL, gb + b * gstep, g_bstride, ib,
+                        idx_bstride, idx_off, 1, rows, D, table_grad))
+      return rc;
   }
   return 0;
 }

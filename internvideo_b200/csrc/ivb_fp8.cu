@@ -165,12 +165,6 @@ __global__ void __launch_bounds__(R_THREADS) fp8_rows_kernel(const __nv_bfloat16
   }
 }
 
-template <int NV>
-static cudaError_t launch_fp8_rows(const __nv_bfloat16* x, long ldx, int M, int K, uint8_t* out, long ldo,
-                                   float* scale_inv, cudaStream_t stream) {
-  return launch_pdl(fp8_rows_kernel<NV>, dim3(M), dim3(R_THREADS), 0, stream, x, ldx, K, out, ldo, scale_inv);
-}
-
 }  // namespace ivb
 
 using namespace ivb;
@@ -191,14 +185,10 @@ extern "C" int ivb_fp8_quantize_rows(const void* x, long ldx, int M, int K, void
   const auto* xb = reinterpret_cast<const __nv_bfloat16*>(x);
   auto* o = reinterpret_cast<uint8_t*>(out);
   const int chunks = (K + 7) / 8;   // per row; each thread holds NV of them
-  cudaError_t e;
-  if (chunks <= R_THREADS * 2) e = launch_fp8_rows<2>(xb, ldx, M, K, o, ldo, row_scale_inv, stream);
-  else if (chunks <= R_THREADS * 4) e = launch_fp8_rows<4>(xb, ldx, M, K, o, ldo, row_scale_inv, stream);
-  else if (chunks <= R_THREADS * 8) e = launch_fp8_rows<8>(xb, ldx, M, K, o, ldo, row_scale_inv, stream);
-  else e = launch_fp8_rows<16>(xb, ldx, M, K, o, ldo, row_scale_inv, stream);
-  if (e != cudaSuccess) return set_error_cuda("launch(fp8_rows_kernel)", e);
-  count_launch();
-  return check_launch("fp8_rows_kernel");
+  const auto kern = chunks <= R_THREADS * 2 ? fp8_rows_kernel<2>
+                  : chunks <= R_THREADS * 4 ? fp8_rows_kernel<4>
+                  : chunks <= R_THREADS * 8 ? fp8_rows_kernel<8> : fp8_rows_kernel<16>;
+  return launch("fp8_rows_kernel", kern, M, R_THREADS, 0, stream, ALLOW_PDL, xb, ldx, K, o, ldo, row_scale_inv);
 }
 
 extern "C" int ivb_fp8_quantize(const void* x, long ldx, int M, int K, int format, void* out, long ldo, void* out_t,
@@ -222,20 +212,10 @@ extern "C" int ivb_fp8_quantize(const void* x, long ldx, int M, int K, int forma
   unsigned* bits = reinterpret_cast<unsigned*>(amax);
   const long chunks = static_cast<long>(M) * ((K + 7) / 8);
   const int grid = persistent_grid(chunks, 256, 8);
-  e = launch_pdl(fp8_amax_kernel, dim3(grid), dim3(256), 0, stream, xb, ldx, M, K, bits);
-  if (e != cudaSuccess) return set_error_cuda("launch(fp8_amax_kernel)", e);
-  count_launch();
-  if (int rc = check_launch("fp8_amax_kernel")) return rc;
+  if (int rc = launch("fp8_amax_kernel", fp8_amax_kernel, grid, 256, 0, stream, ALLOW_PDL, xb, ldx, M, K, bits))
+    return rc;
   const dim3 cast_grid((K + Q_TILE - 1) / Q_TILE, (M + Q_TILE - 1) / Q_TILE);
-  auto* o = reinterpret_cast<uint8_t*>(out);
-  auto* ot = reinterpret_cast<uint8_t*>(out_t);
-  if (format == IVB_FP8_E5M2)
-    e = launch_pdl(fp8_cast_kernel<true>, cast_grid, dim3(Q_THREADS), 0, stream, xb, ldx, M, K, bits, o, ldo, ot, ldt,
-                   scale_inv);
-  else
-    e = launch_pdl(fp8_cast_kernel<false>, cast_grid, dim3(Q_THREADS), 0, stream, xb, ldx, M, K, bits, o, ldo, ot, ldt,
-                   scale_inv);
-  if (e != cudaSuccess) return set_error_cuda("launch(fp8_cast_kernel)", e);
-  count_launch();
-  return check_launch("fp8_cast_kernel");
+  return launch("fp8_cast_kernel", format == IVB_FP8_E5M2 ? fp8_cast_kernel<true> : fp8_cast_kernel<false>, cast_grid,
+                Q_THREADS, 0, stream, ALLOW_PDL, xb, ldx, M, K, bits, reinterpret_cast<uint8_t*>(out), ldo,
+                reinterpret_cast<uint8_t*>(out_t), ldt, scale_inv);
 }

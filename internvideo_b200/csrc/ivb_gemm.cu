@@ -486,28 +486,8 @@ static int launch_gemm(const void* A, long lda, const void* B, long ldb, const G
   const int num_tiles = ((p.M + CL * BM - 1) / (CL * BM)) * ((p.N + BN - 1) / BN);
   int clusters = num_sms() / CL;
   if (clusters > num_tiles) clusters = num_tiles;
-  cudaError_t le;
-  if (CL == 1) {
-    le = launch_pdl(kern, dim3(clusters), dim3(GEMM_THREADS), Cfg::SMEM_BYTES, stream, tmA, tmB, p);
-  } else {
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(clusters * CL);
-    cfg.blockDim = dim3(GEMM_THREADS);
-    cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[2];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = CL; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-    attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[1].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = pdl_enabled() ? 2 : 1;
-    le = cudaLaunchKernelEx(&cfg, kern, tmA, tmB, p);
-  }
-  const char* name = PINGPONG ? "gemm_bf16_pingpong_kernel" : "gemm_bf16_kernel";
-  if (le != cudaSuccess) return set_error_cuda(name, le);
-  count_launch();
-  return check_launch(name);
+  return launch<CL>(PINGPONG ? "gemm_bf16_pingpong_kernel" : "gemm_bf16_kernel", kern, clusters * CL, GEMM_THREADS,
+                    Cfg::SMEM_BYTES, stream, ALLOW_PDL, tmA, tmB, p);
 }
 
 // Pick the N tile that wastes the fewest padded columns / partial waves (fp8: of the two tiles its cooperative kernel has).

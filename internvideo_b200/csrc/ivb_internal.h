@@ -12,7 +12,6 @@ namespace ivb {
 // error reporting: every entry point returns 0 or a non-zero status; text via ivb_last_error().
 int set_error(const char* msg);
 int set_error_cuda(const char* what, cudaError_t e);
-int check_launch(const char* what);  // cudaGetLastError() -> status
 void count_launch();                 // bumps the library-wide launch counter
 int num_sms();
 // Raises Kern's dynamic shared-memory limit to `bytes` on the current device, once per device: the device is marked
@@ -36,24 +35,44 @@ inline int persistent_grid(long rows, int rows_per_cta, int per_sm) {
   return static_cast<int>(blocks > cap ? cap : (blocks < 1 ? 1 : blocks));
 }
 
-// Programmatic dependent launch (IVB_PDL=0 disables): the kernel may be scheduled while the previous kernel of the stream
-// is still draining; it must execute pdl_wait() (ivb_ptx.cuh) before its first global-memory access.  ~1 100 of the
-// ~1 500 launches of a training step go through here; the launch/drain gap between them was ~5 us each.
+// Programmatic dependent launch (PDL) is opt-in: pdl_enabled() is true only when IVB_PDL is set to a non-zero value.
+// A PDL-launched kernel may be scheduled while the previous kernel of the stream is still draining, so it must execute
+// pdl_wait() (ivb_ptx.cuh) before its first global-memory access; only such kernels are launched with ALLOW_PDL.
+// ~1 100 of the ~1 500 launches of a training step allow it; the launch/drain gap between them was ~5 us each.
 bool pdl_enabled();
-template <typename... KArgs, typename... Args>
-inline cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream,
-                              Args&&... args) {
+enum LaunchPdl : bool { NO_PDL = false, ALLOW_PDL = true };
+
+// The one launch path of the library: launches `kern` (in clusters of CLUSTER CTAs along x when CLUSTER > 1), with the
+// PDL attribute when `pdl` allows it and pdl_enabled(), and counts it.  Returns 0, or a status whose ivb_last_error()
+// text is `name` and the CUDA error.
+template <int CLUSTER = 1, typename... KArgs, typename... Args>
+inline int launch(const char* name, void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream,
+                  LaunchPdl pdl, Args&&... args) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = grid;
   cfg.blockDim = block;
   cfg.dynamicSmemBytes = smem;
   cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cudaLaunchAttribute attr[2];
+  unsigned n = 0;
+  if (CLUSTER > 1) {
+    attr[n].id = cudaLaunchAttributeClusterDimension;
+    attr[n].val.clusterDim.x = CLUSTER; attr[n].val.clusterDim.y = 1; attr[n].val.clusterDim.z = 1;
+    ++n;
+  }
+  if (pdl && pdl_enabled()) {
+    attr[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[n].val.programmaticStreamSerializationAllowed = 1;
+    ++n;
+  }
   cfg.attrs = attr;
-  cfg.numAttrs = pdl_enabled() ? 1 : 0;
-  return cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
+  cfg.numAttrs = n;
+  cudaError_t e = cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
+  const cudaError_t last = cudaGetLastError();   // clears the launch's error, and reports one left by earlier work
+  if (e == cudaSuccess) e = last;
+  if (e != cudaSuccess) return set_error_cuda(name, e);
+  count_launch();
+  return 0;
 }
 
 // cuTensorMapEncodeTiled through cudaGetDriverEntryPoint (no link-time libcuda dependency).

@@ -520,17 +520,14 @@ extern "C" int ivb_ln_l2_fwd(const void* z, long ldz, const void* weight, const 
   auto ww = reinterpret_cast<const __nv_bfloat16*>(weight);
   auto bb = reinterpret_cast<const __nv_bfloat16*>(bias);
   auto oo = reinterpret_cast<__nv_bfloat16*>(out);
-  if (target_is_f32) ln_l2_fwd_kernel<true><<<blocks, 256, 0, stream>>>(zz, ldz, ww, bb, eps, M, C, oo, ldo, stats, target, ldt, loss_sum);
-  else ln_l2_fwd_kernel<false><<<blocks, 256, 0, stream>>>(zz, ldz, ww, bb, eps, M, C, oo, ldo, stats, target, ldt, loss_sum);
-  count_launch();
-  return check_launch("ln_l2_fwd_kernel");
+  return launch("ln_l2_fwd_kernel", target_is_f32 ? ln_l2_fwd_kernel<true> : ln_l2_fwd_kernel<false>, blocks, 256, 0,
+                stream, NO_PDL, zz, ldz, ww, bb, eps, M, C, oo, ldo, stats, target, ldt, loss_sum);
 }
 
 template <bool DO_F32>
 static int launch_ln_l2_bwd(const void* z, long ldz, const void* weight, const void* bias,
                             const float* stats, int M, int C, const void* dout, long lddo, float gh,
                             const float* gd, void* dz, long lddz, float* dw, float* db, cudaStream_t stream) {
-  auto kern = ln_l2_bwd_kernel<DO_F32>;
   int wpb = 8;
   size_t smem = dw ? static_cast<size_t>(2) * wpb * C * sizeof(float) : 0;
   while (smem > 200 * 1024 && wpb > 1) { wpb /= 2; smem /= 2; }
@@ -538,12 +535,11 @@ static int launch_ln_l2_bwd(const void* z, long ldz, const void* weight, const v
     if (int rc = raise_smem_limit<ln_l2_bwd_kernel<DO_F32>>(220 * 1024, "cudaFuncSetAttribute(ln_l2_bwd)")) return rc;
   const int blocks = persistent_grid(M, wpb * 2, smem > 96 * 1024 ? 2 : 4);
   if (colred_check(2, blocks, C, "ln_l2_bwd: gradient scratch too small")) return 1;
-  kern<<<blocks, wpb * 32, smem, stream>>>(
-      reinterpret_cast<const __nv_bfloat16*>(z), ldz, reinterpret_cast<const __nv_bfloat16*>(weight),
-      reinterpret_cast<const __nv_bfloat16*>(bias), stats, M, C, dout, lddo, gh, gd,
-      reinterpret_cast<__nv_bfloat16*>(dz), lddz, dw, db);
-  count_launch();
-  if (int rc = check_launch("ln_l2_bwd_kernel")) return rc;
+  if (int rc = launch("ln_l2_bwd_kernel", ln_l2_bwd_kernel<DO_F32>, blocks, wpb * 32, smem, stream, NO_PDL,
+                      reinterpret_cast<const __nv_bfloat16*>(z), ldz, reinterpret_cast<const __nv_bfloat16*>(weight),
+                      reinterpret_cast<const __nv_bfloat16*>(bias), stats, M, C, dout, lddo, gh, gd,
+                      reinterpret_cast<__nv_bfloat16*>(dz), lddz, dw, db))
+    return rc;
   return dw ? colred_finish(2, blocks, C, dw, db, nullptr, stream) : 0;
 }
 
@@ -551,19 +547,18 @@ template <int NCH>
 static int launch_ln_l2_bwd_reg(const void* z, long ldz, const void* weight, const void* bias,
                                 const float* stats, int M, int C, const void* dout, long lddo, float gh,
                                 const float* gd, void* dz, long lddz, float* dw, float* db, cudaStream_t stream) {
-  auto kern = ln_l2_bwd_reg_kernel<NCH>;
   const int wpb = 4;
   const size_t smem = dw ? static_cast<size_t>(2) * wpb * C * sizeof(float) : 0;   // <= 104 KB at C = 3200: 2 CTAs/SM
   if (smem > 48 * 1024)
     if (int rc = raise_smem_limit<ln_l2_bwd_reg_kernel<NCH>>(110 * 1024, "cudaFuncSetAttribute(ln_l2_bwd_reg)")) return rc;
   const int blocks = persistent_grid(M, wpb * 2, 2);
   if (colred_check(2, blocks, C, "ln_l2_bwd: gradient scratch too small")) return 1;
-  kern<<<blocks, wpb * 32, smem, stream>>>(
-      reinterpret_cast<const __nv_bfloat16*>(z), ldz, reinterpret_cast<const __nv_bfloat16*>(weight),
-      reinterpret_cast<const __nv_bfloat16*>(bias), stats, M, C, reinterpret_cast<const __nv_bfloat16*>(dout), lddo,
-      gh, gd, reinterpret_cast<__nv_bfloat16*>(dz), lddz, dw, db);
-  count_launch();
-  if (int rc = check_launch("ln_l2_bwd_reg_kernel")) return rc;
+  if (int rc = launch("ln_l2_bwd_reg_kernel", ln_l2_bwd_reg_kernel<NCH>, blocks, wpb * 32, smem, stream, NO_PDL,
+                      reinterpret_cast<const __nv_bfloat16*>(z), ldz, reinterpret_cast<const __nv_bfloat16*>(weight),
+                      reinterpret_cast<const __nv_bfloat16*>(bias), stats, M, C,
+                      reinterpret_cast<const __nv_bfloat16*>(dout), lddo, gh, gd, reinterpret_cast<__nv_bfloat16*>(dz),
+                      lddz, dw, db))
+    return rc;
   return dw ? colred_finish(2, blocks, C, dw, db, nullptr, stream) : 0;
 }
 
@@ -594,12 +589,9 @@ extern "C" int ivb_adamw_step(float* master, float* exp_avg, float* exp_avg_sq, 
   const float bc2 = 1.f - powf(beta2, static_cast<float>(step));
   const int threads = 256;
   const long blocks = (n + threads * 4 - 1) / (threads * 4);
-  if (grad_is_f32)
-    adamw_kernel<true><<<(unsigned)blocks, threads, 0, stream>>>(master, exp_avg, exp_avg_sq, grad, reinterpret_cast<__nv_bfloat16*>(param_bf16), n, lr, beta1, beta2, eps, weight_decay, bc1, bc2, grad_scale, grad_scale_dev, dyn_lr_step);
-  else
-    adamw_kernel<false><<<(unsigned)blocks, threads, 0, stream>>>(master, exp_avg, exp_avg_sq, grad, reinterpret_cast<__nv_bfloat16*>(param_bf16), n, lr, beta1, beta2, eps, weight_decay, bc1, bc2, grad_scale, grad_scale_dev, dyn_lr_step);
-  count_launch();
-  return check_launch("adamw_kernel");
+  return launch("adamw_kernel", grad_is_f32 ? adamw_kernel<true> : adamw_kernel<false>, (unsigned)blocks, threads, 0,
+                stream, NO_PDL, master, exp_avg, exp_avg_sq, grad, reinterpret_cast<__nv_bfloat16*>(param_bf16), n, lr,
+                beta1, beta2, eps, weight_decay, bc1, bc2, grad_scale, grad_scale_dev, dyn_lr_step);
 }
 
 extern "C" int ivb_vtc_loss_fwd(const float* cos_v2t, const long long* idx, int G, float temp,
@@ -608,9 +600,8 @@ extern "C" int ivb_vtc_loss_fwd(const float* cos_v2t, const long long* idx, int 
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (G <= 0) return 0;
   if (temp_dev == nullptr && !(temp > 0.f)) return set_error("ivb_vtc_loss_fwd: temp must be > 0");
-  vtc_stats_kernel<<<2 * G, 256, 0, stream>>>(cos_v2t, idx, G, 1.f / temp, temp_dev, lse_row, lse_col, loss);
-  count_launch();
-  return check_launch("vtc_stats_kernel");
+  return launch("vtc_stats_kernel", vtc_stats_kernel, 2 * G, 256, 0, stream, NO_PDL, cos_v2t, idx, G, 1.f / temp, temp_dev,
+                lse_row, lse_col, loss);
 }
 
 extern "C" int ivb_vtc_loss_bwd(const float* cos_v2t, const long long* idx, int G, float temp,
@@ -619,10 +610,8 @@ extern "C" int ivb_vtc_loss_bwd(const float* cos_v2t, const long long* idx, int 
                                 const float* gscale_dev, void* dcos_bf16, float* dtemp, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (G <= 0) return 0;
-  vtc_grad_kernel<<<G, 256, 0, stream>>>(cos_v2t, idx, G, 1.f / temp, temp_dev, lse_row, lse_col, gscale_host,
-                                         gscale_dev, reinterpret_cast<__nv_bfloat16*>(dcos_bf16), dtemp);
-  count_launch();
-  return check_launch("vtc_grad_kernel");
+  return launch("vtc_grad_kernel", vtc_grad_kernel, G, 256, 0, stream, NO_PDL, cos_v2t, idx, G, 1.f / temp, temp_dev,
+                lse_row, lse_col, gscale_host, gscale_dev, reinterpret_cast<__nv_bfloat16*>(dcos_bf16), dtemp);
 }
 
 extern "C" int ivb_l2norm_rows_fwd(const void* x, int x_is_f32, long ldx, int M, int C, void* out,
@@ -632,10 +621,8 @@ extern "C" int ivb_l2norm_rows_fwd(const void* x, int x_is_f32, long ldx, int M,
   if ((C & 7) || (ldx & 7) || (ldo & 7)) return set_error("ivb_l2norm_rows_fwd: C/ld must be multiples of 8");
   const int wpb = 8;
   const unsigned grid = (M + wpb - 1) / wpb;
-  if (x_is_f32) l2norm_rows_kernel<true><<<grid, wpb * 32, 0, stream>>>(x, ldx, M, C, reinterpret_cast<__nv_bfloat16*>(out), ldo, inv_norm);
-  else l2norm_rows_kernel<false><<<grid, wpb * 32, 0, stream>>>(x, ldx, M, C, reinterpret_cast<__nv_bfloat16*>(out), ldo, inv_norm);
-  count_launch();
-  return check_launch("l2norm_rows_kernel");
+  return launch("l2norm_rows_kernel", x_is_f32 ? l2norm_rows_kernel<true> : l2norm_rows_kernel<false>, grid, wpb * 32, 0,
+                stream, NO_PDL, x, ldx, M, C, reinterpret_cast<__nv_bfloat16*>(out), ldo, inv_norm);
 }
 
 extern "C" int ivb_l2norm_rows_bwd(const float* dy, long lddy, const void* xn, long ldxn,
@@ -645,9 +632,8 @@ extern "C" int ivb_l2norm_rows_bwd(const float* dy, long lddy, const void* xn, l
   if (M <= 0) return 0;
   if ((C & 7) || (lddy & 7) || (ldxn & 7) || (lddx & 7)) return set_error("ivb_l2norm_rows_bwd: C/ld must be multiples of 8");
   const int wpb = 8;
-  l2norm_rows_bwd_kernel<<<(M + wpb - 1) / wpb, wpb * 32, 0, stream>>>(dy, lddy, reinterpret_cast<const __nv_bfloat16*>(xn), ldxn, inv_norm, M, C, dx, lddx);
-  count_launch();
-  return check_launch("l2norm_rows_bwd_kernel");
+  return launch("l2norm_rows_bwd_kernel", l2norm_rows_bwd_kernel, (M + wpb - 1) / wpb, wpb * 32, 0, stream, NO_PDL, dy,
+                lddy, reinterpret_cast<const __nv_bfloat16*>(xn), ldxn, inv_norm, M, C, dx, lddx);
 }
 
 extern "C" int ivb_pixel_targets(const void* video, const int* masked_idx, int n_mask, int B, int C,
@@ -656,18 +642,18 @@ extern "C" int ivb_pixel_targets(const void* video, const int* masked_idx, int n
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (B <= 0 || n_mask <= 0) return 0;
   if (C > 8) return set_error("ivb_pixel_targets: at most 8 channels");
-  pixel_target_kernel<<<B * n_mask, C * 32, 0, stream>>>(reinterpret_cast<const __nv_bfloat16*>(video), masked_idx, n_mask, B, C, T, H, W, tubelet, patch, normalize, mean3, std3, labels);
-  count_launch();
-  return check_launch("pixel_target_kernel");
+  return launch("pixel_target_kernel", pixel_target_kernel, B * n_mask, C * 32, 0, stream, NO_PDL,
+                reinterpret_cast<const __nv_bfloat16*>(video), masked_idx, n_mask, B, C, T, H, W, tubelet, patch,
+                normalize, mean3, std3, labels);
 }
 
 extern "C" int ivb_mse_loss(const void* pred_bf16, const float* label, long n, float* loss_sum,
                             float gscale_host, const float* gscale_dev, void* dpred_bf16, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (n <= 0) return 0;
-  mse_kernel<<<persistent_grid(n, 256, 8), 256, 0, stream>>>(reinterpret_cast<const __nv_bfloat16*>(pred_bf16), label, n, loss_sum, gscale_host, gscale_dev, reinterpret_cast<__nv_bfloat16*>(dpred_bf16));
-  count_launch();
-  return check_launch("mse_kernel");
+  return launch("mse_kernel", mse_kernel, persistent_grid(n, 256, 8), 256, 0, stream, NO_PDL,
+                reinterpret_cast<const __nv_bfloat16*>(pred_bf16), label, n, loss_sum, gscale_host, gscale_dev,
+                reinterpret_cast<__nv_bfloat16*>(dpred_bf16));
 }
 
 // ---------------------------------------------------------------- single-query attention pooling
@@ -794,11 +780,10 @@ extern "C" int ivb_pool_attn_fwd(const void* q, const void* k, long ldk, const v
   if ((d & 7) || (ldk & 7) || (ldv & 7)) return set_error("ivb_pool_attn_fwd: d/ld must be multiples of 8");
   const size_t smem = (static_cast<size_t>(d) + n + 8) * sizeof(float);
   if (smem > 48 * 1024) return set_error("ivb_pool_attn_fwd: sequence too long for the single-query kernel");
-  pool_attn_fwd_kernel<<<dim3(H, B), 128, smem, stream>>>(
-      reinterpret_cast<const __nv_bfloat16*>(q), reinterpret_cast<const __nv_bfloat16*>(k), ldk,
-      reinterpret_cast<const __nv_bfloat16*>(v), ldv, n, H, d, scale, reinterpret_cast<__nv_bfloat16*>(out), probs);
-  count_launch();
-  return check_launch("pool_attn_fwd_kernel");
+  return launch("pool_attn_fwd_kernel", pool_attn_fwd_kernel, dim3(H, B), 128, smem, stream, NO_PDL,
+                reinterpret_cast<const __nv_bfloat16*>(q), reinterpret_cast<const __nv_bfloat16*>(k), ldk,
+                reinterpret_cast<const __nv_bfloat16*>(v), ldv, n, H, d, scale, reinterpret_cast<__nv_bfloat16*>(out),
+                probs);
 }
 
 extern "C" int ivb_pool_attn_bwd(const void* q, const void* k, long ldk, const void* v, long ldv,
@@ -810,11 +795,9 @@ extern "C" int ivb_pool_attn_bwd(const void* q, const void* k, long ldk, const v
   if ((d & 7) || (ldk & 7) || (ldv & 7) || (lddk & 7) || (lddv & 7)) return set_error("ivb_pool_attn_bwd: d/ld must be multiples of 8");
   const size_t smem = (2 * static_cast<size_t>(d) + n + 8) * sizeof(float);
   if (smem > 48 * 1024) return set_error("ivb_pool_attn_bwd: sequence too long for the single-query kernel");
-  pool_attn_bwd_kernel<<<dim3(H, B), 128, smem, stream>>>(
-      reinterpret_cast<const __nv_bfloat16*>(q), reinterpret_cast<const __nv_bfloat16*>(k), ldk,
-      reinterpret_cast<const __nv_bfloat16*>(v), ldv, probs, reinterpret_cast<const __nv_bfloat16*>(dout), n, H, d,
-      scale, reinterpret_cast<__nv_bfloat16*>(dq), reinterpret_cast<__nv_bfloat16*>(dk), lddk,
-      reinterpret_cast<__nv_bfloat16*>(dv), lddv);
-  count_launch();
-  return check_launch("pool_attn_bwd_kernel");
+  return launch("pool_attn_bwd_kernel", pool_attn_bwd_kernel, dim3(H, B), 128, smem, stream, NO_PDL,
+                reinterpret_cast<const __nv_bfloat16*>(q), reinterpret_cast<const __nv_bfloat16*>(k), ldk,
+                reinterpret_cast<const __nv_bfloat16*>(v), ldv, probs, reinterpret_cast<const __nv_bfloat16*>(dout), n,
+                H, d, scale, reinterpret_cast<__nv_bfloat16*>(dq), reinterpret_cast<__nv_bfloat16*>(dk), lddk,
+                reinterpret_cast<__nv_bfloat16*>(dv), lddv);
 }

@@ -575,15 +575,15 @@ static int launch_rms_bwd_tma(const void* dy, long lddy, const void* x, long ldx
   if (int rc = raise_smem_limit<rms_bwd_tma_kernel>(226 * 1024, "cudaFuncSetAttribute(rms_bwd_tma)")) return rc;
   const int grid = persistent_grid(M, TMA_NW, 1);
   if (colred_check(3, grid, D, "rms_bwd_tma: gradient scratch too small")) return 1;
-  launch_pdl(rms_bwd_tma_kernel, dim3(grid), dim3(TMA_NW * 32), rms_bwd_tma_smem(D, dx_in != nullptr), stream,
-             reinterpret_cast<const __nv_bfloat16*>(dy), lddy, reinterpret_cast<const float*>(x), ldx,
-             reinterpret_cast<const __nv_bfloat16*>(w), rstd, M, D, dx_in, lddx_in,
-             reinterpret_cast<float*>(dx_out), lddx, dweight,
-             reinterpret_cast<const __nv_bfloat16*>(ybr), ldyb,
-             reinterpret_cast<const __nv_bfloat16*>(gamma), rowscale,
-             reinterpret_cast<__nv_bfloat16*>(dyb), lddyb, dgamma, dcolsum);
-  count_launch();
-  if (int rc = check_launch("rms_bwd_tma_kernel")) return rc;
+  if (int rc = launch("rms_bwd_tma_kernel", rms_bwd_tma_kernel, grid, TMA_NW * 32, rms_bwd_tma_smem(D, dx_in != nullptr),
+                      stream, ALLOW_PDL,
+                      reinterpret_cast<const __nv_bfloat16*>(dy), lddy, reinterpret_cast<const float*>(x), ldx,
+                      reinterpret_cast<const __nv_bfloat16*>(w), rstd, M, D, dx_in, lddx_in,
+                      reinterpret_cast<float*>(dx_out), lddx, dweight,
+                      reinterpret_cast<const __nv_bfloat16*>(ybr), ldyb,
+                      reinterpret_cast<const __nv_bfloat16*>(gamma), rowscale,
+                      reinterpret_cast<__nv_bfloat16*>(dyb), lddyb, dgamma, dcolsum))
+    return rc;
   return colred_finish(3, grid, D, dweight, dgamma, dcolsum, stream);
 }
 
@@ -592,11 +592,9 @@ static int launch_rms_fwd_reg(const void* x, long ldx, const void* w, float eps,
                               float* rstd, cudaStream_t stream, const void* w1 = nullptr, long x_pair_off = 0,
                               long y_pair_off = 0) {
   const long rows = PAIR ? 2L * M : M;
-  launch_pdl(rms_fwd_reg_kernel<XF32, NCH, PAIR>, dim3(persistent_grid(rows, 8, 8)), dim3(256), 0, stream,
-      x, ldx, reinterpret_cast<const __nv_bfloat16*>(w), eps, (int)rows, D, reinterpret_cast<__nv_bfloat16*>(y), ldy, rstd,
-      reinterpret_cast<const __nv_bfloat16*>(w1), x_pair_off, y_pair_off);
-  count_launch();
-  return check_launch("rms_fwd_reg_kernel");
+  return launch("rms_fwd_reg_kernel", rms_fwd_reg_kernel<XF32, NCH, PAIR>, persistent_grid(rows, 8, 8), 256, 0, stream,
+      ALLOW_PDL, x, ldx, reinterpret_cast<const __nv_bfloat16*>(w), eps, (int)rows, D, reinterpret_cast<__nv_bfloat16*>(y),
+      ldy, rstd, reinterpret_cast<const __nv_bfloat16*>(w1), x_pair_off, y_pair_off);
 }
 
 template <bool XF32, bool DXF32, int NCH, bool PAIR = false>
@@ -611,14 +609,13 @@ static int launch_rms_bwd_reg(const void* dy, long lddy, const void* x, long ldx
   const long rows = PAIR ? 2L * M : M;
   const int blocks = persistent_grid(rows, wpb * 2, 2);   // 2 CTAs/SM resident (<=128 registers): one persistent wave
   if (colred_check(2, blocks, D, "rms_bwd_reg: gradient scratch too small")) return 1;
-  launch_pdl(rms_bwd_reg_kernel<XF32, DXF32, NCH, PAIR>, dim3(blocks), dim3(wpb * 32), smem, stream,
-             reinterpret_cast<const __nv_bfloat16*>(dy), lddy, x, ldx,
-             reinterpret_cast<const __nv_bfloat16*>(w), rstd, (int)rows, D, dx_in,
-             lddx_in, dx_out, lddx, dweight,
-             reinterpret_cast<const __nv_bfloat16*>(w1), dweight1, x_pair_off,
-             dy_pair_off, dx_pair_off);
-  count_launch();
-  if (int rc = check_launch("rms_bwd_reg_kernel")) return rc;
+  if (int rc = launch("rms_bwd_reg_kernel", rms_bwd_reg_kernel<XF32, DXF32, NCH, PAIR>, blocks, wpb * 32, smem, stream,
+                      ALLOW_PDL, reinterpret_cast<const __nv_bfloat16*>(dy), lddy, x, ldx,
+                      reinterpret_cast<const __nv_bfloat16*>(w), rstd, (int)rows, D, dx_in,
+                      lddx_in, dx_out, lddx, dweight,
+                      reinterpret_cast<const __nv_bfloat16*>(w1), dweight1, x_pair_off,
+                      dy_pair_off, dx_pair_off))
+    return rc;
   if (dweight == nullptr) return 0;
   return colred_finish(PAIR ? 2 : 1, blocks, D, dweight, PAIR ? dweight1 : nullptr, nullptr, stream);
 }
@@ -640,12 +637,11 @@ static int launch_norm_bwd(const void* dy, long lddy, const void* x, long ldx, c
   // with 1.4 CTAs/SM).
   const int blocks = persistent_grid(M, wpb * 2, smem > 96 * 1024 ? 2 : 4);
   if (colred_check(2, blocks, D, "norm_bwd: gradient scratch too small")) return 1;
-  launch_pdl(norm_bwd_kernel<XF32, LN, DXF32>, dim3(blocks), dim3(wpb * 32), smem, stream,
-      reinterpret_cast<const __nv_bfloat16*>(dy), lddy, x, ldx,
-      reinterpret_cast<const __nv_bfloat16*>(weight), mean, rstd, M, D, dx_in, lddx_in, dx_out,
-      lddx, dweight, dbias);
-  count_launch();
-  if (int rc = check_launch("norm_bwd_kernel")) return rc;
+  if (int rc = launch("norm_bwd_kernel", norm_bwd_kernel<XF32, LN, DXF32>, blocks, wpb * 32, smem, stream, ALLOW_PDL,
+                      reinterpret_cast<const __nv_bfloat16*>(dy), lddy, x, ldx,
+                      reinterpret_cast<const __nv_bfloat16*>(weight), mean, rstd, M, D, dx_in, lddx_in, dx_out,
+                      lddx, dweight, dbias))
+    return rc;
   if (dweight == nullptr) return 0;
   return colred_finish(2, blocks, D, dweight, LN ? dbias : nullptr, nullptr, stream);
 }
@@ -679,13 +675,12 @@ extern "C" int ivb_norm_fwd(const void* x, int x_is_f32, long ldx, const void* w
   const __nv_bfloat16* w = reinterpret_cast<const __nv_bfloat16*>(weight);
   const __nv_bfloat16* b = reinterpret_cast<const __nv_bfloat16*>(bias);
   __nv_bfloat16* yo = reinterpret_cast<__nv_bfloat16*>(y);
-  pick_bool(x_is_f32, [&](auto xf) {
+  return pick_bool(x_is_f32, [&](auto xf) {
     return pick_bool(is_layernorm, [&](auto ln) {
-      return launch_pdl(norm_fwd_kernel<xf, ln>, dim3(blocks), dim3(256), 0, stream, x, ldx, w, b, eps, M, D, yo, ldy, mean, rstd);
+      return launch("norm_fwd_kernel", norm_fwd_kernel<xf, ln>, blocks, 256, 0, stream, ALLOW_PDL, x, ldx, w, b, eps, M,
+                    D, yo, ldy, mean, rstd);
     });
   });
-  count_launch();
-  return check_launch("norm_fwd_kernel");
 }
 
 extern "C" int ivb_norm_fwd_fp8(const void* x, int x_is_f32, long ldx, const void* weight, const void* bias, float eps,
@@ -708,19 +703,16 @@ extern "C" int ivb_norm_fwd_fp8(const void* x, int x_is_f32, long ldx, const voi
   const __nv_bfloat16* b = reinterpret_cast<const __nv_bfloat16*>(bias);
   uint8_t* o = reinterpret_cast<uint8_t*>(out);
   const int blocks = persistent_grid(M, 8, 8);
-  const cudaError_t e = pick_bool(x_is_f32, [&](auto xf) {
+  return pick_bool(x_is_f32, [&](auto xf) {
     return pick_bool(is_layernorm, [&](auto ln) {
       auto go = [&](auto nch) {
-        return launch_pdl(norm_fwd_fp8_kernel<xf, ln, nch>, dim3(blocks), dim3(256), 0, stream, x, ldx, w, b, eps, M, D,
-                          o, ldo, row_scale_inv);
+        return launch("norm_fwd_fp8_kernel", norm_fwd_fp8_kernel<xf, ln, nch>, blocks, 256, 0, stream, ALLOW_PDL, x, ldx,
+                      w, b, eps, M, D, o, ldo, row_scale_inv);
       };
       if (D > 1536) return go(std::integral_constant<int, 16>{});
-      return static_cast<cudaError_t>(pick_nch(D, [&](auto nch) { return static_cast<int>(go(nch)); }));
+      return pick_nch(D, go);
     });
   });
-  if (e != cudaSuccess) return set_error_cuda("launch(norm_fwd_fp8_kernel)", e);
-  count_launch();
-  return check_launch("norm_fwd_fp8_kernel");
 }
 
 extern "C" int ivb_norm_bwd(const void* dy, long lddy, const void* x, int x_is_f32, long ldx,
@@ -761,12 +753,10 @@ extern "C" int ivb_layerscale_bwd(const float* dx, long lddx, const void* y, lon
   const __nv_bfloat16* gg = reinterpret_cast<const __nv_bfloat16*>(gamma);
   __nv_bfloat16* dyo = reinterpret_cast<__nv_bfloat16*>(dy);
   if (colred_check(2, rbs, D, "ivb_layerscale_bwd: gradient scratch too small")) return 1;
-  if (y != nullptr)
-    launch_pdl(layerscale_bwd_kernel<true>, dim3(nstrips * rbs), dim3(256), 0, stream, dx, lddx, yy, ldy, gg, M, D, dyo, lddy, dgamma, dcolsum, nstrips, rowscale);
-  else
-    launch_pdl(layerscale_bwd_kernel<false>, dim3(nstrips * rbs), dim3(256), 0, stream, dx, lddx, yy, ldy, gg, M, D, dyo, lddy, dgamma, dcolsum, nstrips, rowscale);
-  count_launch();
-  if (int rc = check_launch("layerscale_bwd_kernel")) return rc;
+  if (int rc = launch("layerscale_bwd_kernel", y != nullptr ? layerscale_bwd_kernel<true> : layerscale_bwd_kernel<false>,
+                      nstrips * rbs, 256, 0, stream, ALLOW_PDL, dx, lddx, yy, ldy, gg, M, D, dyo, lddy, dgamma, dcolsum,
+                      nstrips, rowscale))
+    return rc;
   return colred_finish(2, rbs, D, y != nullptr ? dgamma : nullptr, dcolsum, nullptr, stream);
 }
 
@@ -778,10 +768,9 @@ extern "C" int ivb_colsum_bf16(const void* x, long ldx, int M, int N, float* out
   const int rows_per_cta = 128;
   const int rbs = (M + rows_per_cta - 1) / rows_per_cta;
   if (colred_check(1, rbs, N, "ivb_colsum_bf16: gradient scratch too small")) return 1;
-  launch_pdl(colsum_bf16_kernel, dim3(nstrips * rbs), dim3(256), 0, stream, reinterpret_cast<const __nv_bfloat16*>(x),
-                                                        ldx, M, N, out, nstrips, rows_per_cta);
-  count_launch();
-  if (int rc = check_launch("colsum_bf16_kernel")) return rc;
+  if (int rc = launch("colsum_bf16_kernel", colsum_bf16_kernel, nstrips * rbs, 256, 0, stream, ALLOW_PDL,
+                      reinterpret_cast<const __nv_bfloat16*>(x), ldx, M, N, out, nstrips, rows_per_cta))
+    return rc;
   return colred_finish(1, rbs, N, out, nullptr, nullptr, stream);
 }
 

@@ -114,9 +114,8 @@ extern "C" int ivb_nvls_allreduce_bf16(void* mc_base, long elem_off, long numel,
   uint4* mc = reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(mc_base) + elem_off);
   const long nvec = numel / 8;
   uint32_t* const* flags = reinterpret_cast<uint32_t* const*>(flag_ptrs_dev);
-  nvls_allreduce_bf16_kernel<<<nblocks, NVLS_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(mc, nvec, flags, rank, world);
-  count_launch();
-  return check_launch("nvls_allreduce_bf16_kernel");
+  return launch("nvls_allreduce_bf16_kernel", nvls_allreduce_bf16_kernel, nblocks, NVLS_THREADS, 0,
+                static_cast<cudaStream_t>(stream), NO_PDL, mc, nvec, flags, rank, world);
 }
 
 extern "C" int ivb_nvls_flag_words(void) { return NVLS_MAX_BLOCKS * NVLS_MAX_WORLD; }

@@ -21,11 +21,6 @@ int set_error_cuda(const char* what, cudaError_t e) {
   std::snprintf(g_err, sizeof(g_err), "%s: %s", what, cudaGetErrorString(e));
   return 2;
 }
-int check_launch(const char* what) {
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return set_error_cuda(what, e);
-  return 0;
-}
 void count_launch() { g_launches.fetch_add(1, std::memory_order_relaxed); }
 bool pdl_enabled() {
   static const bool on = [] { const char* e = getenv("IVB_PDL"); return e != nullptr && atoi(e) != 0; }();

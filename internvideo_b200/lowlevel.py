@@ -1,7 +1,8 @@
 """Thin tensor-level wrappers over the C ABI (no autograd): pointer/shape plumbing only.
 
-Every function checks that its tensors are CUDA tensors of the expected dtype and raises otherwise;
-nothing here computes on the CPU.
+Every function checks its tensor operands with _chk (a required operand must not be None; each given one must be a
+CUDA tensor of the expected dtype) and raises otherwise; nothing here computes on the CPU.  Every entry point that
+takes a stream is called through _call.
 """
 from __future__ import annotations
 
@@ -15,31 +16,33 @@ FLAG_FP8_VECTOR_SCALES = 64
 
 bf16 = torch.bfloat16
 f32 = torch.float32
-
-
-def _lib_():
-    return _lib.load()
+i32 = torch.int32
 
 
 def _stream() -> int:
     return torch.cuda.current_stream().cuda_stream
 
 
-def _p(t):
-    return None if t is None else t.data_ptr()
-
-
-def _chk(t, dtype, name):
-    if t is None:
-        return
-    if not t.is_cuda:
-        raise _lib.IvbError(f"{name}: expected a CUDA tensor (ivb200 has no CPU path)")
-    if t.dtype != dtype:
-        raise _lib.IvbError(f"{name}: expected dtype {dtype}, got {t.dtype}")
+def _chk(*operands):
+    """The one operand check.  Each operand is (name, tensor, dtype or tuple of dtypes); a name ending in "?" marks an
+    operand the entry point accepts as NULL, which may be None.  Every missing required operand is refused before any
+    device or dtype check."""
+    for name, t, _ in operands:
+        if t is None and not name.endswith("?"):
+            raise _lib.IvbError(f"{name}: required operand is None")
+    for name, t, dtype in operands:
+        if t is None:
+            continue
+        if not t.is_cuda:
+            raise _lib.IvbError(f"{name.rstrip('?')}: expected a CUDA tensor (ivb200 has no CPU path)")
+        if t.dtype not in (dtype if isinstance(dtype, tuple) else (dtype,)):
+            raise _lib.IvbError(f"{name.rstrip('?')}: expected dtype {dtype}, got {t.dtype}")
 
 
 def _rows2d(t, name):
-    """View as 2-D [rows, cols] with unit inner stride; returns (tensor, ld)."""
+    """Row pitch (elements) of a 2-D tensor with unit inner stride; 0 for an absent operand."""
+    if t is None:
+        return 0
     if t.dim() != 2:
         raise _lib.IvbError(f"{name}: expected 2-D tensor, got {tuple(t.shape)}")
     if t.stride(1) != 1:
@@ -47,20 +50,97 @@ def _rows2d(t, name):
     return t.stride(0)
 
 
+_PROFILERS = []     # the enabled OpProfiler / GemmProfiler objects
+
+
+def _call(name, *args, kind=None, flops=0.0):
+    """The one call path into the library: ivb_<name>(*args, current stream), with a tensor passed as its data_ptr() and
+    None as NULL.  Raises IvbError naming the entry point on a non-zero status.  Each enabled profiler that records
+    `kind` (default: `name`) gets one (name, kind, flops, start event, end event) record."""
+    fn = getattr(_lib.load(), "ivb_" + name)
+    args = [a.data_ptr() if isinstance(a, torch.Tensor) else a for a in args]
+    args.append(_stream())
+    kind = kind or name
+    profs = [p for p in _PROFILERS if p.kinds is None or kind in p.kinds] if _PROFILERS else None
+    if profs:
+        e0 = torch.cuda.Event(enable_timing=True); e0.record()
+    _lib.check(fn(*args), "ivb_" + name)
+    if profs:
+        e1 = torch.cuda.Event(enable_timing=True); e1.record()
+        rec = (_gemm_name(*args) if name == "gemm_bf16" else name, kind, flops, e0, e1)
+        for p in profs:
+            p.records.append(rec)
+
+
+def _gemm_name(a, a_t, lda, b, b_t, ldb, M, N, K, epi, *_):
+    return f"gemm[{'T' if a_t else 'N'}{'T' if b_t else 'N'} epi{epi}] {M}x{N}x{K}"
+
+
+class OpProfiler:
+    """CUDA-event timing of every library call, in situ (warm caches, real overlap): records holds one
+    (name, kind, flops, start, stop) per call, in call order; a bf16 GEMM is named by its layout, epilogue and shape."""
+    kinds = None
+
+    def __init__(self):
+        self.records = []
+
+    def enable(self):
+        if self not in _PROFILERS:
+            _PROFILERS.append(self)
+
+    def disable(self):
+        if self in _PROFILERS:
+            _PROFILERS.remove(self)
+
+    def summary(self):
+        torch.cuda.synchronize()
+        agg = {}
+        for name, _, _, e0, e1 in self.records:
+            c, t = agg.get(name, (0, 0.0))
+            agg[name] = (c + 1, t + e0.elapsed_time(e1))
+        return sorted(agg.items(), key=lambda kv: -kv[1][1])
+
+
+class GemmProfiler(OpProfiler):
+    """CUDA-event timing of every tensor-core launch (GEMMs, bf16 and fp8: kind "gemm"; attention forward / backward)
+    and of the fp8 casts that feed the fp8 GEMMs (kind "fp8_quantize", no flops) and the norms that write FP8 rows
+    (kind "norm_fwd_fp8", no flops) on the launching stream (bench.py roofline).  Records only those calls."""
+    kinds = frozenset(("gemm", "attn_fwd", "attn_bwd", "fp8_quantize", "norm_fwd_fp8"))
+
+    def __init__(self):
+        super().__init__()
+        self.count = 0
+
+    def totals(self, kind="gemm"):
+        """(total algorithmic FLOPs, total milliseconds) over the recorded launches of `kind`."""
+        torch.cuda.synchronize()
+        fl = ms = 0.0
+        cnt = 0
+        for _, k, f, e0, e1 in self.records:
+            if k != kind:
+                continue
+            fl += f
+            ms += e0.elapsed_time(e1)
+            cnt += 1
+        if kind == "gemm":
+            self.count = cnt
+        return fl, ms
+
+
 def launch_count() -> int:
-    return int(_lib_().ivb_launch_count())
+    return int(_lib.load().ivb_launch_count())
 
 
 def reset_launch_count() -> None:
-    _lib_().ivb_reset_launch_count()
+    _lib.load().ivb_reset_launch_count()
 
 
 def set_default_2cta(enable: bool) -> None:
-    _lib_().ivb_set_default_2cta(int(bool(enable)))
+    _lib.load().ivb_set_default_2cta(int(bool(enable)))
 
 
 def device_check() -> None:
-    _lib.check(_lib_().ivb_device_check(), "ivb_device_check")
+    _lib.check(_lib.load().ivb_device_check(), "ivb_device_check")
 
 
 # ----------------------------------------------------------------------------------------- GEMM
@@ -71,7 +151,7 @@ def gemm(a, b, *, a_t=False, b_t=False, epi=EPI_BF16, flags=0, out0=None, out1=N
     a_t=False: `a` is [M,K]; a_t=True: `a` is [K,M] (MN-major operand).
     b_t=False: `b` is [N,K]; b_t=True: `b` is [K,N].
     """
-    _chk(a, bf16, "a"); _chk(b, bf16, "b")
+    _chk(("a", a, bf16), ("b", b, bf16))
     lda = _rows2d(a, "a"); ldb = _rows2d(b, "b")
     if a_t:
         K, M = a.shape
@@ -83,33 +163,21 @@ def gemm(a, b, *, a_t=False, b_t=False, epi=EPI_BF16, flags=0, out0=None, out1=N
         N, Kb = b.shape
     if K != Kb:
         raise _lib.IvbError(f"gemm: contraction mismatch {K} vs {Kb}")
-    out0, ld0, ld1, ldaux = _epilogue_operands(M, N, epi, out0, out1, bias, gamma, aux, a.device)
-    ev0 = _prof_begin()
-    rc = _lib_().ivb_gemm_bf16(_p(a), int(a_t), lda, _p(b), int(b_t), ldb, M, N, K, epi, flags,
-                               _p(out0), ld0, _p(out1), ld1, _p(bias), _p(gamma), _p(aux), ldaux,
-                               _p(rowscale), tile_n, _stream())
-    _lib.check(rc, "ivb_gemm_bf16")
-    _prof_end(ev0, 2.0 * M * N * K, "gemm")
+    out0 = _epilogue_operands(M, N, epi, out0, out1, bias, gamma, aux, rowscale, a.device)
+    _call("gemm_bf16", a, int(a_t), lda, b, int(b_t), ldb, M, N, K, epi, flags, out0, _rows2d(out0, "out0"), out1,
+          _rows2d(out1, "out1"), bias, gamma, aux, _rows2d(aux, "aux"), rowscale, tile_n, kind="gemm",
+          flops=2.0 * M * N * K)
     return out0
 
 
-def _epilogue_operands(M, N, epi, out0, out1, bias, gamma, aux, device):
-    """Checks the fused epilogue's operands of an [M, N] GEMM (allocating out0 if it is None).
-    Returns (out0, ld0, ld1, ldaux), with 0 for an absent operand."""
+def _epilogue_operands(M, N, epi, out0, out1, bias, gamma, aux, rowscale, device):
+    """Checks the fused epilogue's operands of an [M, N] GEMM, allocating out0 if it is None.  Returns out0."""
     out_dtype = f32 if epi in (EPI_F32, EPI_RESID) else bf16
     if out0 is None:
         out0 = torch.empty((M, N), device=device, dtype=out_dtype)
-    _chk(out0, out_dtype, "out0")
-    ld0 = _rows2d(out0, "out0")
-    ld1 = 0
-    if out1 is not None:
-        _chk(out1, bf16, "out1"); ld1 = _rows2d(out1, "out1")
-    _chk(bias, bf16, "bias"); _chk(gamma, bf16, "gamma")
-    ldaux = 0
-    if aux is not None:
-        _chk(aux, f32 if epi == EPI_RESID else bf16, "aux")
-        ldaux = _rows2d(aux, "aux")
-    return out0, ld0, ld1, ldaux
+    _chk(("out0", out0, out_dtype), ("out1?", out1, bf16), ("bias?", bias, bf16), ("gamma?", gamma, bf16),
+         ("aux?", aux, f32 if epi == EPI_RESID else bf16), ("rowscale?", rowscale, f32))
+    return out0
 
 
 # ----------------------------------------------------------------------------------------- FP8
@@ -127,7 +195,7 @@ def fp8_quantize(x, fmt=FP8_E4M3, transpose=False):
     Returns (q [M, K], q_t [K, M] = q^T or None, scale_inv fp32 [1], amax fp32 [1]): x ~ q * scale_inv, with a
     power-of-two scale.  q and q_t are views of buffers whose row pitch is rounded up to 16 elements (the fp8 GEMM's
     operand rule)."""
-    _chk(x, bf16, "x")
+    _chk(("x", x, bf16))
     ldx = _rows2d(x, "x")
     M, K = x.shape
     dt = FP8_DTYPES[fmt]
@@ -135,11 +203,7 @@ def fp8_quantize(x, fmt=FP8_E4M3, transpose=False):
     q_t = torch.empty((K, _pad16(M)), device=x.device, dtype=dt)[:, :M] if transpose else None
     stats = torch.empty((2,), device=x.device, dtype=f32)
     amax, scale_inv = stats[0:1], stats[1:2]
-    ev0 = _prof_begin()
-    rc = _lib_().ivb_fp8_quantize(_p(x), ldx, M, K, fmt, _p(q), q.stride(0), _p(q_t),
-                                  q_t.stride(0) if transpose else 0, _p(amax), _p(scale_inv), _stream())
-    _lib.check(rc, "ivb_fp8_quantize")
-    _prof_end(ev0, 0.0, "fp8_quantize")
+    _call("fp8_quantize", x, ldx, M, K, fmt, q, q.stride(0), q_t, q_t.stride(0) if transpose else 0, amax, scale_inv)
     return q, q_t, scale_inv, amax
 
 
@@ -149,15 +213,12 @@ def fp8_quantize_rows(x):
     Returns (q [M, K], row_scale_inv fp32 [M]): x[m] ~ q[m] * row_scale_inv[m], each row with its own power-of-two
     scale.  A weight [N, K] quantised this way has one scale per output channel.  q is a view of a buffer whose row
     pitch is rounded up to 16 elements (the fp8 GEMM's operand rule)."""
-    _chk(x, bf16, "x")
+    _chk(("x", x, bf16))
     ldx = _rows2d(x, "x")
     M, K = x.shape
     q = torch.empty((M, _pad16(K)), device=x.device, dtype=torch.float8_e4m3fn)[:, :K]
     sinv = torch.empty((M,), device=x.device, dtype=f32)
-    ev0 = _prof_begin()
-    rc = _lib_().ivb_fp8_quantize_rows(_p(x), ldx, M, K, _p(q), q.stride(0), _p(sinv), _stream())
-    _lib.check(rc, "ivb_fp8_quantize_rows")
-    _prof_end(ev0, 0.0, "fp8_quantize")
+    _call("fp8_quantize_rows", x, ldx, M, K, q, q.stride(0), sinv, kind="fp8_quantize")
     return q, sinv
 
 
@@ -165,18 +226,13 @@ def norm_fwd_fp8(x, weight, bias=None, eps=1e-6, layernorm=False):
     """RMSNorm / LayerNorm of x [M, D] (fp32 or bf16, any row pitch) written only as E4M3 rows with per-row scales
     (ivb_norm_fwd_fp8).  Returns (q [M, D] float8_e4m3fn, row_scale_inv fp32 [M]): q[m] * row_scale_inv[m] is the
     row norm_fwd would round to bf16, rounded to E4M3 instead."""
-    if x.dtype not in (f32, bf16):
-        raise _lib.IvbError("norm_fwd_fp8: x must be fp32 or bf16")
-    _chk(x, x.dtype, "x"); _chk(weight, bf16, "weight"); _chk(bias, bf16, "bias")
+    _chk(("x", x, (f32, bf16)), ("weight", weight, bf16), ("bias?", bias, bf16))
     ldx = _rows2d(x, "x")
     M, D = x.shape
     q = torch.empty((M, _pad16(D)), device=x.device, dtype=torch.float8_e4m3fn)[:, :D]
     sinv = torch.empty((M,), device=x.device, dtype=f32)
-    ev0 = _prof_begin()
-    rc = _lib_().ivb_norm_fwd_fp8(_p(x), int(x.dtype == f32), ldx, _p(weight), _p(bias), float(eps), int(layernorm), M,
-                                  D, _p(q), q.stride(0), _p(sinv), _stream())
-    _lib.check(rc, "ivb_norm_fwd_fp8")
-    _prof_end(ev0, 0.0, "norm_fwd_fp8")
+    _call("norm_fwd_fp8", x, int(x.dtype == f32), ldx, weight, bias, float(eps), int(layernorm), M, D, q, q.stride(0),
+          sinv)
     return q, sinv
 
 
@@ -188,15 +244,14 @@ def gemm_fp8(a, a_scale_inv, b, b_scale_inv, *, epi=EPI_BF16, flags=0, out0=None
     transposed operand).  a_scale_inv / b_scale_inv: fp32 [1] CUDA tensors (per-tensor scales), or fp32 [M] and [N]
     vectors (per-row scales of a, per-output-channel scales of b, as fp8_quantize_rows / norm_fwd_fp8 give them; a
     must then be E4M3), which sets FLAG_FP8_VECTOR_SCALES.  Epilogue arguments as for gemm()."""
-    if a.dtype not in FP8_DTYPES.values() or not a.is_cuda:
-        raise _lib.IvbError(f"gemm_fp8: a must be a CUDA float8_e4m3fn / float8_e5m2 tensor, got {a.dtype}")
-    _chk(b, torch.float8_e4m3fn, "b"); _chk(a_scale_inv, f32, "a_scale_inv"); _chk(b_scale_inv, f32, "b_scale_inv")
+    _chk(("a", a, tuple(FP8_DTYPES.values())), ("a_scale_inv", a_scale_inv, f32), ("b", b, torch.float8_e4m3fn),
+         ("b_scale_inv", b_scale_inv, f32))
     lda = _rows2d(a, "a"); ldb = _rows2d(b, "b")
     M, K = a.shape
     N, Kb = b.shape
     if K != Kb:
         raise _lib.IvbError(f"gemm_fp8: contraction mismatch {K} vs {Kb}")
-    out0, ld0, ld1, ldaux = _epilogue_operands(M, N, epi, out0, out1, bias, gamma, aux, a.device)
+    out0 = _epilogue_operands(M, N, epi, out0, out1, bias, gamma, aux, rowscale, a.device)
     fmt = FP8_E5M2 if a.dtype == torch.float8_e5m2 else FP8_E4M3
     if a_scale_inv.numel() != 1 or b_scale_inv.numel() != 1:
         if (a_scale_inv.shape != (M,) or b_scale_inv.shape != (N,) or not a_scale_inv.is_contiguous()
@@ -204,446 +259,273 @@ def gemm_fp8(a, a_scale_inv, b, b_scale_inv, *, epi=EPI_BF16, flags=0, out0=None
             raise _lib.IvbError(f"gemm_fp8: vector scales must be contiguous [M] = [{M}] and [N] = [{N}], got "
                                 f"{tuple(a_scale_inv.shape)} and {tuple(b_scale_inv.shape)}")
         flags |= FLAG_FP8_VECTOR_SCALES
-    ev0 = _prof_begin()
-    rc = _lib_().ivb_gemm_fp8(_p(a), 0, lda, fmt, _p(a_scale_inv), _p(b), 0, ldb, _p(b_scale_inv), M, N, K, epi, flags,
-                              _p(out0), ld0, _p(out1), ld1, _p(bias), _p(gamma), _p(aux), ldaux, _p(rowscale), tile_n,
-                              _stream())
-    _lib.check(rc, "ivb_gemm_fp8")
-    _prof_end(ev0, 2.0 * M * N * K, "gemm")
+    _call("gemm_fp8", a, 0, lda, fmt, a_scale_inv, b, 0, ldb, b_scale_inv, M, N, K, epi, flags, out0,
+          _rows2d(out0, "out0"), out1, _rows2d(out1, "out1"), bias, gamma, aux, _rows2d(aux, "aux"), rowscale, tile_n,
+          kind="gemm", flops=2.0 * M * N * K)
     return out0
-
-
-_PROF = [None]
-
-
-class GemmProfiler:
-    """CUDA-event timing of every tensor-core launch (GEMMs, bf16 and fp8, attention forward / backward) and of the
-    fp8 casts that feed the fp8 GEMMs (kind "fp8_quantize", no flops) and the norms that write FP8 rows (kind
-    "norm_fwd_fp8", no flops) on the launching stream (bench.py roofline).
-    Records (start, stop, algorithmic flops, kind)."""
-
-    def __init__(self):
-        self.records = []
-        self.count = 0
-
-    def enable(self):
-        _PROF[0] = self
-
-    def disable(self):
-        _PROF[0] = None
-
-    def totals(self, kind="gemm"):
-        """(total algorithmic FLOPs, total milliseconds) over the recorded launches of `kind`."""
-        torch.cuda.synchronize()
-        fl = ms = 0.0
-        cnt = 0
-        for e0, e1, f, k in self.records:
-            if k != kind:
-                continue
-            fl += f
-            ms += e0.elapsed_time(e1)
-            cnt += 1
-        if kind == "gemm":
-            self.count = cnt
-        return fl, ms
-
-
-def _prof_begin():
-    prof = _PROF[0]
-    if prof is None:
-        return None
-    ev0 = torch.cuda.Event(enable_timing=True); ev0.record()
-    return ev0
-
-
-def _prof_end(ev0, flops, kind):
-    if ev0 is not None and _PROF[0] is not None:
-        ev1 = torch.cuda.Event(enable_timing=True); ev1.record()
-        _PROF[0].records.append((ev0, ev1, flops, kind))
 
 
 # ----------------------------------------------------------------------------------------- norms
 def norm_fwd(x, weight, bias=None, eps=1e-6, layernorm=False, out=None, want_stats=True):
     """x: [M,D] fp32 or bf16 (row stride arbitrary). Returns (y bf16, mean|None, rstd)."""
-    if x.dtype not in (f32, bf16):
-        raise _lib.IvbError("norm_fwd: x must be fp32 or bf16")
-    _chk(x, x.dtype, "x"); _chk(weight, bf16, "weight"); _chk(bias, bf16, "bias")
+    _chk(("x", x, (f32, bf16)), ("weight", weight, bf16), ("bias?", bias, bf16), ("out?", out, bf16))
     ldx = _rows2d(x, "x")
     M, D = x.shape
     if out is None:
         out = torch.empty((M, D), device=x.device, dtype=bf16)
-    _chk(out, bf16, "out")
-    ldy = _rows2d(out, "out")
     rstd = torch.empty((M,), device=x.device, dtype=f32) if want_stats else None
     mean = torch.empty((M,), device=x.device, dtype=f32) if (want_stats and layernorm) else None
-    rc = _lib_().ivb_norm_fwd(_p(x), int(x.dtype == f32), ldx, _p(weight), _p(bias), float(eps),
-                              int(layernorm), M, D, _p(out), ldy, _p(mean), _p(rstd), _stream())
-    _lib.check(rc, "ivb_norm_fwd")
+    _call("norm_fwd", x, int(x.dtype == f32), ldx, weight, bias, float(eps), int(layernorm), M, D, out,
+          _rows2d(out, "out"), mean, rstd)
     return out, mean, rstd
 
 
 def rmsnorm_pair_fwd(qkv, D, w0, w1, out, eps=1e-6, want_stats=True):
     """RMSNorm of the q and k column slices ([:, :D] and [:, D:2D]) of a bf16 [M, >=2D] projection buffer in one
     launch -> out[:, :D], out[:, D:2D] (bf16 [M, >=2D]).  Returns rstd fp32 [M, 2] (or None)."""
-    _chk(qkv, bf16, "qkv"); _chk(w0, bf16, "w0"); _chk(w1, bf16, "w1"); _chk(out, bf16, "out")
+    _chk(("qkv", qkv, bf16), ("w0", w0, bf16), ("w1", w1, bf16), ("out", out, bf16))
     M = qkv.shape[0]
     rstd = torch.empty((M, 2), device=qkv.device, dtype=f32) if want_stats else None
-    rc = _lib_().ivb_rmsnorm_pair_fwd(_p(qkv), _rows2d(qkv, "qkv"), D, _p(w0), _p(w1), float(eps), M, D,
-                                      _p(out), _rows2d(out, "out"), D, _p(rstd), _stream())
-    _lib.check(rc, "ivb_rmsnorm_pair_fwd")
+    _call("rmsnorm_pair_fwd", qkv, _rows2d(qkv, "qkv"), D, w0, w1, float(eps), M, D, out, _rows2d(out, "out"), D, rstd)
     return rstd
 
 
 def rmsnorm_pair_bwd(dqk, qkv, D, w0, w1, rstd, dw0=None, dw1=None):
     """Backward of rmsnorm_pair_fwd, IN PLACE on the gradient buffer: dqk[:, :D] / dqk[:, D:2D] hold d(normed q/k) on
     entry and d(q/k) on return.  dw0/dw1: optional fp32 [D] accumulators."""
-    _chk(dqk, bf16, "dqk"); _chk(qkv, bf16, "qkv"); _chk(rstd, f32, "rstd"); _chk(dw0, f32, "dw0"); _chk(dw1, f32, "dw1")
+    _chk(("dqk", dqk, bf16), ("qkv", qkv, bf16), ("w0", w0, bf16), ("w1", w1, bf16), ("rstd", rstd, f32),
+         ("dw0?", dw0, f32), ("dw1?", dw1, f32))
     M = qkv.shape[0]
-    rc = _lib_().ivb_rmsnorm_pair_bwd(_p(dqk), _rows2d(dqk, "dqk"), D, _p(qkv), _rows2d(qkv, "qkv"), D, _p(w0), _p(w1),
-                                      _p(rstd), M, D, _p(dqk), _rows2d(dqk, "dqk"), D, _p(dw0), _p(dw1), _stream())
-    _lib.check(rc, "ivb_rmsnorm_pair_bwd")
+    ld = _rows2d(dqk, "dqk")
+    _call("rmsnorm_pair_bwd", dqk, ld, D, qkv, _rows2d(qkv, "qkv"), D, w0, w1, rstd, M, D, dqk, ld, D, dw0, dw1)
     return dqk
 
 
 def norm_bwd(dy, x, weight, mean, rstd, layernorm=False, dx_in=None, dx_out=None,
              dx_dtype=f32, dweight=None, dbias=None):
-    _chk(dy, bf16, "dy"); _chk(weight, bf16, "weight")
-    _chk(rstd, f32, "rstd"); _chk(mean, f32, "mean")
-    _chk(dweight, f32, "dweight"); _chk(dbias, f32, "dbias"); _chk(dx_in, f32, "dx_in")
+    _chk(("dy", dy, bf16), ("x", x, (f32, bf16)), ("weight", weight, bf16), ("mean?", mean, f32), ("rstd", rstd, f32),
+         ("dx_in?", dx_in, f32), ("dx_out?", dx_out, (f32, bf16)), ("dweight?", dweight, f32), ("dbias?", dbias, f32))
     M, D = x.shape
     lddy = _rows2d(dy, "dy"); ldx = _rows2d(x, "x")
     if dx_out is None:
         dx_out = torch.empty((M, D), device=x.device, dtype=dx_dtype)
-    lddx = _rows2d(dx_out, "dx_out")
-    lddx_in = _rows2d(dx_in, "dx_in") if dx_in is not None else 0
-    rc = _lib_().ivb_norm_bwd(_p(dy), lddy, _p(x), int(x.dtype == f32), ldx, _p(weight), _p(mean),
-                              _p(rstd), int(layernorm), M, D, _p(dx_in), lddx_in, _p(dx_out),
-                              int(dx_out.dtype == f32), lddx, _p(dweight), _p(dbias), _stream())
-    _lib.check(rc, "ivb_norm_bwd")
+    _call("norm_bwd", dy, lddy, x, int(x.dtype == f32), ldx, weight, mean, rstd, int(layernorm), M, D, dx_in,
+          _rows2d(dx_in, "dx_in"), dx_out, int(dx_out.dtype == f32), _rows2d(dx_out, "dx_out"), dweight, dbias)
     return dx_out
 
 
 def rmsnorm_bwd_layerscale(dy, x, weight, rstd, dx_in, ybr, gamma, dweight, dgamma, dcolsum, rowscale=None):
     """RMSNorm backward on the fp32 stream fused with the LayerScale backward of the preceding branch (one pass over the
     rows).  Returns (dx fp32 [M,D], dyb bf16 [M,D])."""
-    _chk(dy, bf16, "dy"); _chk(x, f32, "x"); _chk(weight, bf16, "weight"); _chk(rstd, f32, "rstd"); _chk(dx_in, f32, "dx_in")
-    _chk(ybr, bf16, "ybr"); _chk(gamma, bf16, "gamma"); _chk(dweight, f32, "dweight"); _chk(dgamma, f32, "dgamma")
-    _chk(dcolsum, f32, "dcolsum"); _chk(rowscale, f32, "rowscale")
+    _chk(("dy", dy, bf16), ("x", x, f32), ("weight", weight, bf16), ("rstd", rstd, f32), ("dx_in?", dx_in, f32),
+         ("ybr", ybr, bf16), ("gamma", gamma, bf16), ("dweight?", dweight, f32), ("dgamma?", dgamma, f32),
+         ("dcolsum?", dcolsum, f32), ("rowscale?", rowscale, f32))
     M, D = x.shape
     dx = torch.empty((M, D), device=x.device, dtype=f32)
     dyb = torch.empty((M, D), device=x.device, dtype=bf16)
-    rc = _lib_().ivb_rmsnorm_bwd_layerscale(_p(dy), _rows2d(dy, "dy"), _p(x), _rows2d(x, "x"), _p(weight), _p(rstd), M, D,
-                                            _p(dx_in), _rows2d(dx_in, "dx_in") if dx_in is not None else 0, _p(dx), D,
-                                            _p(dweight), _p(ybr), _rows2d(ybr, "ybr"), _p(gamma), _p(rowscale), _p(dyb), D,
-                                            _p(dgamma), _p(dcolsum), _stream())
-    _lib.check(rc, "ivb_rmsnorm_bwd_layerscale")
+    _call("rmsnorm_bwd_layerscale", dy, _rows2d(dy, "dy"), x, _rows2d(x, "x"), weight, rstd, M, D, dx_in,
+          _rows2d(dx_in, "dx_in"), dx, D, dweight, ybr, _rows2d(ybr, "ybr"), gamma, rowscale, dyb, D, dgamma, dcolsum)
     return dx, dyb
 
 
 def layerscale_bwd(dx, y, gamma, dgamma=None, dcolsum=None, out=None, rowscale=None):
-    _chk(dx, f32, "dx"); _chk(y, bf16, "y"); _chk(gamma, bf16, "gamma")
-    _chk(dgamma, f32, "dgamma"); _chk(dcolsum, f32, "dcolsum")
+    _chk(("dx", dx, f32), ("y?", y, bf16), ("gamma?", gamma, bf16), ("dgamma?", dgamma, f32),
+         ("dcolsum?", dcolsum, f32), ("out?", out, bf16), ("rowscale?", rowscale, f32))
     M, D = dx.shape
     if out is None:
         out = torch.empty((M, D), device=dx.device, dtype=bf16)
-    rc = _lib_().ivb_layerscale_bwd(_p(dx), _rows2d(dx, "dx"), _p(y),
-                                    _rows2d(y, "y") if y is not None else 0, _p(gamma), M, D,
-                                    _p(out), _rows2d(out, "out"), _p(dgamma), _p(dcolsum), _p(rowscale), _stream())
-    _lib.check(rc, "ivb_layerscale_bwd")
+    _call("layerscale_bwd", dx, _rows2d(dx, "dx"), y, _rows2d(y, "y"), gamma, M, D, out, _rows2d(out, "out"), dgamma,
+          dcolsum, rowscale)
     return out
 
 
 def colsum(x, out=None):
-    _chk(x, bf16, "x")
+    _chk(("x", x, bf16), ("out?", out, f32))
     M, N = x.shape
     if out is None:
         out = torch.zeros((N,), device=x.device, dtype=f32)
-    _chk(out, f32, "out")
-    rc = _lib_().ivb_colsum_bf16(_p(x), _rows2d(x, "x"), M, N, _p(out), _stream())
-    _lib.check(rc, "ivb_colsum_bf16")
+    _call("colsum_bf16", x, _rows2d(x, "x"), M, N, out)
     return out
 
 
 # ----------------------------------------------------------------------------------------- attention
 def attn_fwd(q, k, v, B, n, H, d, scale, out=None, want_lse=True):
     """q/k/v: 2-D views [B*n, H*d] (any row pitch) of the projection buffers."""
+    _chk(("q", q, bf16), ("k", k, bf16), ("v", v, bf16), ("out?", out, bf16))
     for t, nm in ((q, "q"), (k, "k"), (v, "v")):
-        _chk(t, bf16, nm)
         if t.shape != (B * n, H * d):
             raise _lib.IvbError(f"attn_fwd: {nm} must be [B*n, H*d], got {tuple(t.shape)}")
     if out is None:
         out = torch.empty((B * n, H * d), device=q.device, dtype=bf16)
     lse = torch.empty((B, H, n), device=q.device, dtype=f32) if want_lse else None
-    ev0 = _prof_begin()
-    rc = _lib_().ivb_attn_fwd(_p(q), _rows2d(q, "q"), _p(k), _rows2d(k, "k"), _p(v), _rows2d(v, "v"),
-                              _p(out), _rows2d(out, "out"), _p(lse), B, n, H, d, float(scale), _stream())
-    _lib.check(rc, "ivb_attn_fwd")
-    _prof_end(ev0, 4.0 * B * H * n * n * d, "attn_fwd")          # QK^T + PV
+    _call("attn_fwd", q, _rows2d(q, "q"), k, _rows2d(k, "k"), v, _rows2d(v, "v"), out, _rows2d(out, "out"), lse,
+          B, n, H, d, float(scale), flops=4.0 * B * H * n * n * d)          # QK^T + PV
     return out, lse
 
 
 def headaxis_attn_fwd(qkv, B, N, H, d, scale):
     """The VideoMAEv2 teacher's attention as the reference runs it (softmax over the H heads of each token, see
     include/ivb200.h).  qkv bf16 [B*N, 3*H*d] -> bf16 [B, H, N, d] contiguous."""
-    _chk(qkv, bf16, "qkv")
+    _chk(("qkv", qkv, bf16))
     if qkv.shape != (B * N, 3 * H * d):
         raise _lib.IvbError(f"headaxis_attn_fwd: qkv must be [B*N, 3*H*d], got {tuple(qkv.shape)}")
     out = torch.empty((B, H, N, d), device=qkv.device, dtype=bf16)
-    rc = _lib_().ivb_headaxis_attn_fwd(_p(qkv), _rows2d(qkv, "qkv"), B, N, H, d, float(scale), _p(out), _stream())
-    _lib.check(rc, "ivb_headaxis_attn_fwd")
+    _call("headaxis_attn_fwd", qkv, _rows2d(qkv, "qkv"), B, N, H, d, float(scale), out)
     return out
 
 
 def attn_bwd(q, k, v, out, dout, lse, B, n, H, d, scale, dq, dk, dv):
     """dq/dk/dv: preallocated bf16 2-D views [B*n, H*d] (e.g. the three slots of a [B*n, 3D] buffer)."""
-    for t, nm in ((q, "q"), (k, "k"), (v, "v"), (out, "out"), (dout, "dout"), (dq, "dq"), (dk, "dk"), (dv, "dv")):
-        _chk(t, bf16, nm)
+    rows = (("q", q), ("k", k), ("v", v), ("out", out), ("dout", dout), ("dq", dq), ("dk", dk), ("dv", dv))
+    _chk(*((nm, t, bf16) for nm, t in rows), ("lse", lse, f32))
+    for nm, t in rows:
         if t.shape != (B * n, H * d):
             raise _lib.IvbError(f"attn_bwd: {nm} must be [B*n, H*d], got {tuple(t.shape)}")
-    _chk(lse, f32, "lse")
-    delta = torch.empty((int(_lib_().ivb_attn_bwd_workspace_floats(B, n, H)),), device=q.device, dtype=f32)
-    ev0 = _prof_begin()
-    rc = _lib_().ivb_attn_bwd(_p(q), _rows2d(q, "q"), _p(k), _rows2d(k, "k"), _p(v), _rows2d(v, "v"),
-                              _p(out), _rows2d(out, "out"), _p(dout), _rows2d(dout, "dout"), _p(lse),
-                              _p(delta), _p(dq), _rows2d(dq, "dq"), _p(dk), _rows2d(dk, "dk"),
-                              _p(dv), _rows2d(dv, "dv"), B, n, H, d, float(scale), _stream())
-    _lib.check(rc, "ivb_attn_bwd")
-    _prof_end(ev0, 10.0 * B * H * n * n * d, "attn_bwd")         # algorithmic: 5 GEMMs (SURVEY §8d: 2.5x forward)
+    delta = torch.empty((int(_lib.load().ivb_attn_bwd_workspace_floats(B, n, H)),), device=q.device, dtype=f32)
+    _call("attn_bwd", q, _rows2d(q, "q"), k, _rows2d(k, "k"), v, _rows2d(v, "v"), out, _rows2d(out, "out"), dout,
+          _rows2d(dout, "dout"), lse, delta, dq, _rows2d(dq, "dq"), dk, _rows2d(dk, "dk"), dv, _rows2d(dv, "dv"),
+          B, n, H, d, float(scale), flops=10.0 * B * H * n * n * d)  # algorithmic: 5 GEMMs (SURVEY §8d: 2.5x forward)
     return dq, dk, dv
 
 
 # ----------------------------------------------------------------------------------------- token front-end
-i32 = torch.int32
-
-
 def visible_indices(mask, n_keep):
     """mask: bool/uint8 [B, N] on CUDA (True = masked). Returns (idx int32 [B, n_keep], err int32[1])."""
-    if not mask.is_cuda:
-        raise _lib.IvbError("visible_indices: mask must be a CUDA tensor")
+    _chk(("mask", mask, (torch.bool, torch.uint8)))
     m = mask.contiguous()
     if m.dtype == torch.bool:
         m = m.view(torch.uint8)
-    if m.dtype != torch.uint8:
-        raise _lib.IvbError("visible_indices: mask must be bool or uint8")
     B, N = m.shape
     idx = torch.empty((B, n_keep), device=m.device, dtype=i32)
     err = torch.zeros((1,), device=m.device, dtype=i32)
-    rc = _lib_().ivb_visible_indices(_p(m), B, N, n_keep, _p(idx), _p(err), _stream())
-    _lib.check(rc, "ivb_visible_indices")
+    _call("visible_indices", m, B, N, n_keep, idx, err)
     return idx, err
 
 
 def im2col_visible(video, idx, j0, rows_per_clip, tubelet, patch, kpad):
-    _chk(video, bf16, "video"); _chk(idx, i32, "idx")
+    _chk(("video", video, bf16), ("idx", idx, i32))
     if not video.is_contiguous():
         raise _lib.IvbError("im2col_visible: video must be contiguous [B,C,T,H,W]")
     B, C, T, H, W = video.shape
     cols = torch.empty((B * rows_per_clip, kpad), device=video.device, dtype=bf16)
-    rc = _lib_().ivb_im2col_visible(_p(video), _p(idx), idx.stride(0), j0, rows_per_clip, B, C, T, H, W,
-                                    tubelet, patch, kpad, _p(cols), _stream())
-    _lib.check(rc, "ivb_im2col_visible")
+    _call("im2col_visible", video, idx, idx.stride(0), j0, rows_per_clip, B, C, T, H, W, tubelet, patch, kpad, cols)
     return cols
 
 
 def gather_add(src, src_bstride, table, idx, idx_bstride, idx_off, B, rows, D, out, out_bstride):
-    _chk(src, f32, "src"); _chk(table, bf16, "table"); _chk(idx, i32, "idx")
-    if out.dtype not in (f32, bf16) or not out.is_cuda:
-        raise _lib.IvbError("gather_add: out must be a CUDA fp32/bf16 tensor")
-    rc = _lib_().ivb_gather_add(_p(src), src_bstride, _p(table), _p(idx), idx_bstride, idx_off, B, rows, D,
-                                _p(out), int(out.dtype == f32), out_bstride, _stream())
-    _lib.check(rc, "ivb_gather_add")
+    _chk(("src?", src, f32), ("table?", table, bf16), ("idx?", idx, i32), ("out", out, (f32, bf16)))
+    _call("gather_add", src, src_bstride, table, idx, idx_bstride, idx_off, B, rows, D, out, int(out.dtype == f32),
+          out_bstride)
     return out
 
 
 def scatter_add(g, g_bstride, idx, idx_bstride, idx_off, B, rows, D, table_grad):
-    _chk(table_grad, f32, "table_grad"); _chk(idx, i32, "idx")
-    if g.dtype not in (f32, bf16) or not g.is_cuda:
-        raise _lib.IvbError("scatter_add: g must be a CUDA fp32/bf16 tensor")
-    rc = _lib_().ivb_scatter_add(_p(g), int(g.dtype == f32), g_bstride, _p(idx), idx_bstride, idx_off, B,
-                                 rows, D, _p(table_grad), _stream())
-    _lib.check(rc, "ivb_scatter_add")
+    _chk(("g", g, (f32, bf16)), ("idx?", idx, i32), ("table_grad", table_grad, f32))
+    _call("scatter_add", g, int(g.dtype == f32), g_bstride, idx, idx_bstride, idx_off, B, rows, D, table_grad)
     return table_grad
 
 
 # ----------------------------------------------------------------------------------------- heads / losses
 def ln_l2_fwd(z, weight, bias, eps=1e-5, want_out=True, target=None, loss_sum=None):
-    _chk(z, bf16, "z"); _chk(weight, bf16, "weight"); _chk(bias, bf16, "bias"); _chk(loss_sum, f32, "loss_sum")
+    _chk(("z", z, bf16), ("weight", weight, bf16), ("bias", bias, bf16), ("target?", target, (f32, bf16)),
+         ("loss_sum?", loss_sum, f32))
     M, Cc = z.shape
     out = torch.empty((M, Cc), device=z.device, dtype=bf16) if want_out else None
     stats = torch.empty((M, 3), device=z.device, dtype=f32)
-    tf32 = 0
-    ldt = 0
-    if target is not None:
-        if target.dtype not in (f32, bf16):
-            raise _lib.IvbError("ln_l2_fwd: target must be fp32/bf16")
-        _chk(target, target.dtype, "target")
-        tf32 = int(target.dtype == f32); ldt = _rows2d(target, "target")
-    rc = _lib_().ivb_ln_l2_fwd(_p(z), _rows2d(z, "z"), _p(weight), _p(bias), float(eps), M, Cc, _p(out),
-                               Cc if want_out else 0, _p(stats), _p(target), tf32, ldt, _p(loss_sum), _stream())
-    _lib.check(rc, "ivb_ln_l2_fwd")
+    _call("ln_l2_fwd", z, _rows2d(z, "z"), weight, bias, float(eps), M, Cc, out, Cc if want_out else 0, stats, target,
+          int(target is not None and target.dtype == f32), _rows2d(target, "target"), loss_sum)
     return out, stats
 
 
 def ln_l2_bwd(z, weight, bias, stats, dout, gscale_host=1.0, gscale_dev=None, dweight=None, dbias=None):
-    _chk(z, bf16, "z"); _chk(stats, f32, "stats"); _chk(dweight, f32, "dweight"); _chk(dbias, f32, "dbias")
-    _chk(gscale_dev, f32, "gscale_dev")
-    if dout.dtype not in (f32, bf16) or not dout.is_cuda:
-        raise _lib.IvbError("ln_l2_bwd: dout must be CUDA fp32/bf16")
+    _chk(("z", z, bf16), ("weight", weight, bf16), ("bias", bias, bf16), ("stats", stats, f32),
+         ("dout", dout, (f32, bf16)), ("gscale_dev?", gscale_dev, f32), ("dweight?", dweight, f32),
+         ("dbias?", dbias, f32))
     M, Cc = z.shape
     dz = torch.empty((M, Cc), device=z.device, dtype=bf16)
-    rc = _lib_().ivb_ln_l2_bwd(_p(z), _rows2d(z, "z"), _p(weight), _p(bias), _p(stats), M, Cc, _p(dout),
-                               int(dout.dtype == f32), _rows2d(dout, "dout"), float(gscale_host),
-                               _p(gscale_dev), _p(dz), Cc, _p(dweight), _p(dbias), _stream())
-    _lib.check(rc, "ivb_ln_l2_bwd")
+    _call("ln_l2_bwd", z, _rows2d(z, "z"), weight, bias, stats, M, Cc, dout, int(dout.dtype == f32),
+          _rows2d(dout, "dout"), float(gscale_host), gscale_dev, dz, Cc, dweight, dbias)
     return dz
 
 
 def vtc_loss_fwd(cosm, idx, temp, temp_dev=None):
     """temp_dev: optional CUDA fp32[1] temperature (overrides the host float `temp`)."""
-    _chk(cosm, f32, "cos"); _chk(idx, torch.int64, "idx"); _chk(temp_dev, f32, "temp_dev")
+    _chk(("cosm", cosm, f32), ("idx", idx, torch.int64), ("temp_dev?", temp_dev, f32))
     G = cosm.shape[0]
     lse_r = torch.empty((G,), device=cosm.device, dtype=f32)
     lse_c = torch.empty((G,), device=cosm.device, dtype=f32)
     loss = torch.zeros((1,), device=cosm.device, dtype=f32)
-    rc = _lib_().ivb_vtc_loss_fwd(_p(cosm), _p(idx), G, float(temp), _p(temp_dev), _p(lse_r), _p(lse_c), _p(loss), _stream())
-    _lib.check(rc, "ivb_vtc_loss_fwd")
+    _call("vtc_loss_fwd", cosm, idx, G, float(temp), temp_dev, lse_r, lse_c, loss)
     return loss, lse_r, lse_c
 
 
 def vtc_loss_bwd(cosm, idx, temp, lse_r, lse_c, gscale_host=1.0, gscale_dev=None, temp_dev=None):
-    _chk(temp_dev, f32, "temp_dev")
+    _chk(("cosm", cosm, f32), ("idx", idx, torch.int64), ("lse_r", lse_r, f32), ("lse_c", lse_c, f32),
+         ("gscale_dev?", gscale_dev, f32), ("temp_dev?", temp_dev, f32))
     G = cosm.shape[0]
     dcos = torch.empty((G, G), device=cosm.device, dtype=bf16)
     dtemp = torch.zeros((1,), device=cosm.device, dtype=f32)
-    rc = _lib_().ivb_vtc_loss_bwd(_p(cosm), _p(idx), G, float(temp), _p(temp_dev), _p(lse_r), _p(lse_c), float(gscale_host),
-                                  _p(gscale_dev), _p(dcos), _p(dtemp), _stream())
-    _lib.check(rc, "ivb_vtc_loss_bwd")
+    _call("vtc_loss_bwd", cosm, idx, G, float(temp), temp_dev, lse_r, lse_c, float(gscale_host), gscale_dev, dcos, dtemp)
     return dcos, dtemp
 
 
 def l2norm_rows_fwd(x):
-    if x.dtype not in (f32, bf16) or not x.is_cuda:
-        raise _lib.IvbError("l2norm_rows_fwd: x must be CUDA fp32/bf16")
+    _chk(("x", x, (f32, bf16)))
     M, Cc = x.shape
     out = torch.empty((M, Cc), device=x.device, dtype=bf16)
     inv = torch.empty((M,), device=x.device, dtype=f32)
-    rc = _lib_().ivb_l2norm_rows_fwd(_p(x), int(x.dtype == f32), _rows2d(x, "x"), M, Cc, _p(out), Cc, _p(inv), _stream())
-    _lib.check(rc, "ivb_l2norm_rows_fwd")
+    _call("l2norm_rows_fwd", x, int(x.dtype == f32), _rows2d(x, "x"), M, Cc, out, Cc, inv)
     return out, inv
 
 
 def l2norm_rows_bwd(dy, xn, inv):
-    _chk(dy, f32, "dy"); _chk(xn, bf16, "xn"); _chk(inv, f32, "inv")
+    _chk(("dy", dy, f32), ("xn", xn, bf16), ("inv", inv, f32))
     M, Cc = dy.shape
     dx = torch.empty((M, Cc), device=dy.device, dtype=f32)
-    rc = _lib_().ivb_l2norm_rows_bwd(_p(dy), _rows2d(dy, "dy"), _p(xn), _rows2d(xn, "xn"), _p(inv), M, Cc, _p(dx), Cc, _stream())
-    _lib.check(rc, "ivb_l2norm_rows_bwd")
+    _call("l2norm_rows_bwd", dy, _rows2d(dy, "dy"), xn, _rows2d(xn, "xn"), inv, M, Cc, dx, Cc)
     return dx
 
 
 def pixel_targets(video, masked_idx, n_mask, tubelet, patch, normalize, mean3, std3):
-    _chk(video, bf16, "video"); _chk(masked_idx, i32, "masked_idx"); _chk(mean3, f32, "mean3"); _chk(std3, f32, "std3")
+    _chk(("video", video, bf16), ("masked_idx", masked_idx, i32), ("mean3", mean3, f32), ("std3", std3, f32))
     B, C, T, H, W = video.shape
     labels = torch.empty((B * n_mask, tubelet * patch * patch * C), device=video.device, dtype=f32)
-    rc = _lib_().ivb_pixel_targets(_p(video.contiguous()), _p(masked_idx), n_mask, B, C, T, H, W, tubelet, patch,
-                                   int(normalize), _p(mean3), _p(std3), _p(labels), _stream())
-    _lib.check(rc, "ivb_pixel_targets")
+    _call("pixel_targets", video.contiguous(), masked_idx, n_mask, B, C, T, H, W, tubelet, patch, int(normalize),
+          mean3, std3, labels)
     return labels
 
 
 def mse_loss(pred, label, loss_sum, gscale_host=0.0, gscale_dev=None, dpred=None):
-    _chk(pred, bf16, "pred"); _chk(label, f32, "label"); _chk(loss_sum, f32, "loss_sum"); _chk(dpred, bf16, "dpred")
-    rc = _lib_().ivb_mse_loss(_p(pred), _p(label), pred.numel(), _p(loss_sum), float(gscale_host), _p(gscale_dev), _p(dpred), _stream())
-    _lib.check(rc, "ivb_mse_loss")
+    _chk(("pred", pred, bf16), ("label", label, f32), ("loss_sum?", loss_sum, f32), ("gscale_dev?", gscale_dev, f32),
+         ("dpred?", dpred, bf16))
+    _call("mse_loss", pred, label, pred.numel(), loss_sum, float(gscale_host), gscale_dev, dpred)
     return loss_sum
 
 
 def adamw_step(master, exp_avg, exp_avg_sq, grad, param_bf16, lr, beta1, beta2, eps, wd, step, grad_scale=1.0,
                grad_scale_dev=None, dyn_lr_step=None):
-    _chk(master, f32, "master"); _chk(exp_avg, f32, "exp_avg"); _chk(exp_avg_sq, f32, "exp_avg_sq"); _chk(param_bf16, bf16, "param")
-    _chk(dyn_lr_step, f32, "dyn_lr_step")
-    if grad.dtype not in (f32, bf16) or not grad.is_cuda:
-        raise _lib.IvbError("adamw_step: grad must be CUDA fp32/bf16")
-    rc = _lib_().ivb_adamw_step(_p(master), _p(exp_avg), _p(exp_avg_sq), _p(grad), int(grad.dtype == f32),
-                                _p(param_bf16), master.numel(), float(lr), float(beta1), float(beta2), float(eps),
-                                float(wd), int(step), float(grad_scale), _p(grad_scale_dev), _p(dyn_lr_step),
-                                _stream())
-    _lib.check(rc, "ivb_adamw_step")
+    _chk(("master", master, f32), ("exp_avg", exp_avg, f32), ("exp_avg_sq", exp_avg_sq, f32),
+         ("grad", grad, (f32, bf16)), ("param_bf16", param_bf16, bf16), ("grad_scale_dev?", grad_scale_dev, f32),
+         ("dyn_lr_step?", dyn_lr_step, f32))
+    _call("adamw_step", master, exp_avg, exp_avg_sq, grad, int(grad.dtype == f32), param_bf16, master.numel(),
+          float(lr), float(beta1), float(beta2), float(eps), float(wd), int(step), float(grad_scale), grad_scale_dev,
+          dyn_lr_step)
 
 
 def pool_attn_fwd(q, k, v, B, n, H, d, scale):
     """q: [B, H*d]; k, v: [B*n, H*d] 2-D views. Returns (out bf16 [B, H*d], probs fp32 [B,H,n])."""
-    _chk(q, bf16, "q"); _chk(k, bf16, "k"); _chk(v, bf16, "v")
+    _chk(("q", q, bf16), ("k", k, bf16), ("v", v, bf16))
     out = torch.empty((B, H * d), device=q.device, dtype=bf16)
     probs = torch.empty((B, H, n), device=q.device, dtype=f32)
-    rc = _lib_().ivb_pool_attn_fwd(_p(q), _p(k), _rows2d(k, "k"), _p(v), _rows2d(v, "v"), B, n, H, d, float(scale),
-                                   _p(out), _p(probs), _stream())
-    _lib.check(rc, "ivb_pool_attn_fwd")
+    _call("pool_attn_fwd", q, k, _rows2d(k, "k"), v, _rows2d(v, "v"), B, n, H, d, float(scale), out, probs)
     return out, probs
 
 
 def pool_attn_bwd(q, k, v, probs, dout, B, n, H, d, scale):
-    _chk(dout, bf16, "dout"); _chk(probs, f32, "probs")
+    _chk(("q", q, bf16), ("k", k, bf16), ("v", v, bf16), ("probs", probs, f32), ("dout", dout, bf16))
     dq = torch.empty((B, H * d), device=q.device, dtype=bf16)
     dk = torch.empty((B * n, H * d), device=q.device, dtype=bf16)
     dv = torch.empty((B * n, H * d), device=q.device, dtype=bf16)
-    rc = _lib_().ivb_pool_attn_bwd(_p(q), _p(k), _rows2d(k, "k"), _p(v), _rows2d(v, "v"), _p(probs), _p(dout), B, n,
-                                   H, d, float(scale), _p(dq), _p(dk), H * d, _p(dv), H * d, _stream())
-    _lib.check(rc, "ivb_pool_attn_bwd")
+    _call("pool_attn_bwd", q, k, _rows2d(k, "k"), v, _rows2d(v, "v"), probs, dout, B, n, H, d, float(scale), dq, dk,
+          H * d, dv, H * d)
     return dq, dk, dv
-
-
-# ----------------------------------------------------------------------------------------- op profiler (dev tool)
-_OPPROF = [None]
-
-
-class OpProfiler:
-    """CUDA-event timing of every lowlevel op, in situ (warm caches, real overlap)."""
-
-    def __init__(self):
-        self.records = []
-
-    def enable(self):
-        _OPPROF[0] = self
-
-    def disable(self):
-        _OPPROF[0] = None
-
-    def summary(self):
-        torch.cuda.synchronize()
-        agg = {}
-        for name, e0, e1 in self.records:
-            c, t = agg.get(name, (0, 0.0))
-            agg[name] = (c + 1, t + e0.elapsed_time(e1))
-        return sorted(agg.items(), key=lambda kv: -kv[1][1])
-
-
-def _timed(fn, namer=None):
-    import functools
-
-    @functools.wraps(fn)
-    def w(*a, **k):
-        prof = _OPPROF[0]
-        if prof is None:
-            return fn(*a, **k)
-        e0 = torch.cuda.Event(enable_timing=True); e0.record()
-        r = fn(*a, **k)
-        e1 = torch.cuda.Event(enable_timing=True); e1.record()
-        prof.records.append((namer(*a, **k) if namer else fn.__name__, e0, e1))
-        return r
-    return w
-
-
-def _gemm_name(a, b, *, a_t=False, b_t=False, epi=EPI_BF16, **_):
-    M = a.shape[1] if a_t else a.shape[0]
-    K = a.shape[0] if a_t else a.shape[1]
-    N = b.shape[1] if b_t else b.shape[0]
-    return f"gemm[{'T' if a_t else 'N'}{'T' if b_t else 'N'} epi{epi}] {M}x{N}x{K}"
-
-
-gemm = _timed(gemm, _gemm_name)
-for _n in ("norm_fwd", "norm_bwd", "layerscale_bwd", "colsum", "attn_fwd", "attn_bwd", "visible_indices",
-           "im2col_visible", "gather_add", "scatter_add", "ln_l2_fwd", "ln_l2_bwd", "vtc_loss_fwd", "vtc_loss_bwd",
-           "l2norm_rows_fwd", "l2norm_rows_bwd", "pixel_targets", "mse_loss", "adamw_step", "fp8_quantize", "gemm_fp8",
-           "fp8_quantize_rows", "norm_fwd_fp8"):
-    globals()[_n] = _timed(globals()[_n])

@@ -85,6 +85,5 @@ class NvlsBuffer:
         wide: four times the CTAs (the caller knows nothing else is competing for the SMs)."""
         end = self.numel if end is None else end
         end = min((end + 7) // 8 * 8, self.numel)      # entries are 16-byte aligned; the pad between them is nobody's
-        rc = _lib.load().ivb_nvls_allreduce_bf16(self.mc_ptr, start, end - start, self.flag_ptrs_dev, self.rank,
-                                                 self.world, min(self.nblocks * 4, 64) if wide else self.nblocks, ll._stream())
-        _lib.check(rc, "ivb_nvls_allreduce_bf16")
+        ll._call("nvls_allreduce_bf16", self.mc_ptr, start, end - start, self.flag_ptrs_dev, self.rank, self.world,
+                 min(self.nblocks * 4, 64) if wide else self.nblocks)
