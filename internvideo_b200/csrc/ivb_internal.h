@@ -28,6 +28,11 @@ inline int raise_smem_limit(int bytes, const char* what) {
   if (tracked) set[dev] = true;
   return 0;
 }
+// True when one of the pointers is not a multiple of `bytes` (a power of two); null pointers count as aligned.
+template <typename... P>
+inline bool misaligned(uintptr_t bytes, const P*... ps) {
+  return ((reinterpret_cast<uintptr_t>(ps) & (bytes - 1)) | ... | 0u) != 0;
+}
 // Grid of a persistent row kernel: one CTA per `rows_per_cta` rows, at most `per_sm` CTAs per SM, at least one.
 inline int persistent_grid(long rows, int rows_per_cta, int per_sm) {
   const long blocks = (rows + rows_per_cta - 1) / rows_per_cta;

@@ -182,15 +182,17 @@ template <bool G_F32>
 __global__ void adamw_kernel(float* __restrict__ master, float* __restrict__ m, float* __restrict__ v,
                              const void* __restrict__ grad, __nv_bfloat16* __restrict__ param_bf16,
                              long n, float lr, float beta1, float beta2, float eps, float wd,
-                             float bc1, float bc2, float grad_scale_host,
+                             float step, float grad_scale_host,
                              const float* __restrict__ grad_scale_dev, const float* __restrict__ dyn) {
   const long i = (static_cast<long>(blockIdx.x) * blockDim.x + threadIdx.x) * 4;
   if (i >= n) return;
   if (dyn != nullptr) {  // device-resident {lr, step}: keeps a captured CUDA graph valid across steps
     lr = dyn[0];
-    bc1 = 1.f - powf(beta1, dyn[1]);
-    bc2 = 1.f - powf(beta2, dyn[1]);
+    step = dyn[1];
   }
+  // The bias corrections are computed here for a host step too, so the two give the same bits.
+  const float bc1 = 1.f - powf(beta1, step);
+  const float bc2 = 1.f - powf(beta2, step);
   const float gs_dev = grad_scale_dev ? *grad_scale_dev : 1.f;
   // a device scale that is not a positive finite number marks a bad step (NaN/Inf global gradient norm:
   // engine.step(check_finite) — engine_for_pretraining.py:151-161 aborts there): leave every state untouched
@@ -514,7 +516,9 @@ extern "C" int ivb_ln_l2_fwd(const void* z, long ldz, const void* weight, const 
                              int target_is_f32, long ldt, float* loss_sum, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (M <= 0) return 0;
-  if ((C & 7) || (ldz & 7)) return set_error("ivb_ln_l2_fwd: C/ld must be multiples of 8");
+  if ((C & 7) || (ldz & 7) || (ldo & 7) || (ldt & 7)) return set_error("ivb_ln_l2_fwd: C/ld must be multiples of 8");
+  if (misaligned(16, z, weight, bias, out, target))
+    return set_error("ivb_ln_l2_fwd: z, weight, bias, out and target must be 16-byte aligned");
   const int blocks = persistent_grid(M, 8, 8);
   auto zz = reinterpret_cast<const __nv_bfloat16*>(z);
   auto ww = reinterpret_cast<const __nv_bfloat16*>(weight);
@@ -569,6 +573,8 @@ extern "C" int ivb_ln_l2_bwd(const void* z, long ldz, const void* weight, const 
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (M <= 0) return 0;
   if ((C & 7) || (ldz & 7) || (lddz & 7) || (lddo & 7)) return set_error("ivb_ln_l2_bwd: C/ld must be multiples of 8");
+  if (misaligned(16, z, weight, bias, dout, dz))
+    return set_error("ivb_ln_l2_bwd: z, weight, bias, dout and dz must be 16-byte aligned");
   if (!dout_is_f32 && C <= 256 * 13) {
     const int nchunks = (C + 255) / 256;
     if (nchunks <= 3) return launch_ln_l2_bwd_reg<3>(z, ldz, weight, bias, stats, M, C, dout, lddo, gscale_host, gscale_dev, dz, lddz, dweight, dbias, stream);
@@ -585,13 +591,11 @@ extern "C" int ivb_adamw_step(float* master, float* exp_avg, float* exp_avg_sq, 
                               const float* grad_scale_dev, const float* dyn_lr_step, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (n <= 0) return 0;
-  const float bc1 = 1.f - powf(beta1, static_cast<float>(step));
-  const float bc2 = 1.f - powf(beta2, static_cast<float>(step));
   const int threads = 256;
   const long blocks = (n + threads * 4 - 1) / (threads * 4);
   return launch("adamw_kernel", grad_is_f32 ? adamw_kernel<true> : adamw_kernel<false>, (unsigned)blocks, threads, 0,
                 stream, NO_PDL, master, exp_avg, exp_avg_sq, grad, reinterpret_cast<__nv_bfloat16*>(param_bf16), n, lr,
-                beta1, beta2, eps, weight_decay, bc1, bc2, grad_scale, grad_scale_dev, dyn_lr_step);
+                beta1, beta2, eps, weight_decay, static_cast<float>(step), grad_scale, grad_scale_dev, dyn_lr_step);
 }
 
 extern "C" int ivb_vtc_loss_fwd(const float* cos_v2t, const long long* idx, int G, float temp,
@@ -619,6 +623,7 @@ extern "C" int ivb_l2norm_rows_fwd(const void* x, int x_is_f32, long ldx, int M,
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (M <= 0) return 0;
   if ((C & 7) || (ldx & 7) || (ldo & 7)) return set_error("ivb_l2norm_rows_fwd: C/ld must be multiples of 8");
+  if (misaligned(16, x, out)) return set_error("ivb_l2norm_rows_fwd: x and out must be 16-byte aligned");
   const int wpb = 8;
   const unsigned grid = (M + wpb - 1) / wpb;
   return launch("l2norm_rows_kernel", x_is_f32 ? l2norm_rows_kernel<true> : l2norm_rows_kernel<false>, grid, wpb * 32, 0,
@@ -631,6 +636,7 @@ extern "C" int ivb_l2norm_rows_bwd(const float* dy, long lddy, const void* xn, l
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (M <= 0) return 0;
   if ((C & 7) || (lddy & 7) || (ldxn & 7) || (lddx & 7)) return set_error("ivb_l2norm_rows_bwd: C/ld must be multiples of 8");
+  if (misaligned(16, dy, xn, dx)) return set_error("ivb_l2norm_rows_bwd: dy, xn and dx must be 16-byte aligned");
   const int wpb = 8;
   return launch("l2norm_rows_bwd_kernel", l2norm_rows_bwd_kernel, (M + wpb - 1) / wpb, wpb * 32, 0, stream, NO_PDL, dy,
                 lddy, reinterpret_cast<const __nv_bfloat16*>(xn), ldxn, inv_norm, M, C, dx, lddx);
@@ -778,6 +784,7 @@ extern "C" int ivb_pool_attn_fwd(const void* q, const void* k, long ldk, const v
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (B <= 0) return 0;
   if ((d & 7) || (ldk & 7) || (ldv & 7)) return set_error("ivb_pool_attn_fwd: d/ld must be multiples of 8");
+  if (misaligned(16, k, v)) return set_error("ivb_pool_attn_fwd: k and v must be 16-byte aligned");
   const size_t smem = (static_cast<size_t>(d) + n + 8) * sizeof(float);
   if (smem > 48 * 1024) return set_error("ivb_pool_attn_fwd: sequence too long for the single-query kernel");
   return launch("pool_attn_fwd_kernel", pool_attn_fwd_kernel, dim3(H, B), 128, smem, stream, NO_PDL,
@@ -793,6 +800,7 @@ extern "C" int ivb_pool_attn_bwd(const void* q, const void* k, long ldk, const v
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (B <= 0) return 0;
   if ((d & 7) || (ldk & 7) || (ldv & 7) || (lddk & 7) || (lddv & 7)) return set_error("ivb_pool_attn_bwd: d/ld must be multiples of 8");
+  if (misaligned(16, k, v, dk, dv)) return set_error("ivb_pool_attn_bwd: k, v, dk and dv must be 16-byte aligned");
   const size_t smem = (2 * static_cast<size_t>(d) + n + 8) * sizeof(float);
   if (smem > 48 * 1024) return set_error("ivb_pool_attn_bwd: sequence too long for the single-query kernel");
   return launch("pool_attn_bwd_kernel", pool_attn_bwd_kernel, dim3(H, B), 128, smem, stream, NO_PDL,

@@ -667,6 +667,7 @@ extern "C" int ivb_norm_fwd(const void* x, int x_is_f32, long ldx, const void* w
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (M <= 0) return 0;
   if ((D & 7) || (ldx & 7) || (ldy & 7)) return set_error("ivb_norm_fwd: D/ld must be multiples of 8");
+  if (misaligned(16, x, weight, bias, y)) return set_error("ivb_norm_fwd: x, weight, bias and y must be 16-byte aligned");
   if (!is_layernorm && D <= 1536)   // register-resident RMSNorm: the row is read from HBM exactly once
     return pick_bool(x_is_f32, [&](auto xf) {
       return pick_nch(D, [&](auto nch) { return launch_rms_fwd_reg<xf, nch>(x, ldx, weight, eps, M, D, y, ldy, rstd, stream); });
@@ -722,8 +723,10 @@ extern "C" int ivb_norm_bwd(const void* dy, long lddy, const void* x, int x_is_f
                             float* dbias, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (M <= 0) return 0;
-  if ((D & 7) || (ldx & 7) || (lddy & 7) || (lddx & 7))
+  if ((D & 7) || (ldx & 7) || (lddy & 7) || (lddx & 7) || (lddx_in & 7))
     return set_error("ivb_norm_bwd: D/ld must be multiples of 8");
+  if (misaligned(16, dy, x, weight, dx_in, dx_out))
+    return set_error("ivb_norm_bwd: dy, x, weight, dx_in and dx_out must be 16-byte aligned");
   if (is_layernorm && mean == nullptr) return set_error("ivb_norm_bwd: LayerNorm needs mean");
   return pick_bool(x_is_f32, [&](auto xf) {
     return pick_bool(dx_out_is_f32, [&](auto dxf) {
@@ -746,7 +749,9 @@ extern "C" int ivb_layerscale_bwd(const float* dx, long lddx, const void* y, lon
                                   void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (M <= 0) return 0;
-  if ((D & 7) || (lddx & 7) || (lddy & 7)) return set_error("ivb_layerscale_bwd: D/ld must be multiples of 8");
+  if ((D & 7) || (lddx & 7) || (ldy & 7) || (lddy & 7)) return set_error("ivb_layerscale_bwd: D/ld must be multiples of 8");
+  if (misaligned(16, dx, y, gamma, dy))
+    return set_error("ivb_layerscale_bwd: dx, y, gamma and dy must be 16-byte aligned");
   const int nstrips = (D + 255) / 256;
   const int rbs = (M + 63) / 64;
   const __nv_bfloat16* yy = reinterpret_cast<const __nv_bfloat16*>(y);
@@ -764,6 +769,7 @@ extern "C" int ivb_colsum_bf16(const void* x, long ldx, int M, int N, float* out
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (M <= 0) return 0;
   if ((N & 7) || (ldx & 7)) return set_error("ivb_colsum_bf16: N/ld must be multiples of 8");
+  if (misaligned(16, x)) return set_error("ivb_colsum_bf16: x must be 16-byte aligned");
   const int nstrips = (N + 255) / 256;
   const int rows_per_cta = 128;
   const int rbs = (M + rows_per_cta - 1) / rows_per_cta;
@@ -784,6 +790,7 @@ extern "C" int ivb_rmsnorm_pair_fwd(const void* x, long ldx, long x_pair_off, co
   if ((D & 7) || (ldx & 7) || (ldy & 7) || (x_pair_off & 7) || (y_pair_off & 7))
     return set_error("ivb_rmsnorm_pair_fwd: D/ld/offsets must be multiples of 8");
   if (D > 1536) return set_error("ivb_rmsnorm_pair_fwd: D > 1536 (use two ivb_norm_fwd calls)");
+  if (misaligned(16, x, w0, w1, y)) return set_error("ivb_rmsnorm_pair_fwd: x, w0, w1 and y must be 16-byte aligned");
   return pick_nch(D, [&](auto nch) {
     return launch_rms_fwd_reg<false, nch, true>(x, ldx, w0, eps, M, D, y, ldy, rstd, stream, w1, x_pair_off, y_pair_off);
   });
@@ -799,6 +806,8 @@ extern "C" int ivb_rmsnorm_pair_bwd(const void* dy, long lddy, long dy_pair_off,
     return set_error("ivb_rmsnorm_pair_bwd: D/ld/offsets must be multiples of 8");
   if (D > 1536) return set_error("ivb_rmsnorm_pair_bwd: D > 1536 (use two ivb_norm_bwd calls)");
   if ((dweight0 == nullptr) != (dweight1 == nullptr)) return set_error("ivb_rmsnorm_pair_bwd: give both weight gradients or none");
+  if (misaligned(16, dy, x, w0, w1, dx_out))
+    return set_error("ivb_rmsnorm_pair_bwd: dy, x, w0, w1 and dx_out must be 16-byte aligned");
   return pick_nch(D, [&](auto nch) {
     return launch_rms_bwd_reg<false, false, nch, true>(dy, lddy, x, ldx, w0, rstd, M, D, nullptr, 0, dx_out, lddx, dweight0,
                                                        stream, w1, dweight1, x_pair_off, dy_pair_off, dx_pair_off);
@@ -818,6 +827,9 @@ extern "C" int ivb_rmsnorm_bwd_layerscale(const void* dy, long lddy, const float
   if ((D & 7) || (ldx & 3) || (lddy & 7) || (lddx & 3) || (ldyb & 7) || (lddyb & 7) || (lddx_in & 3))
     return set_error("ivb_rmsnorm_bwd_layerscale: D multiple of 8, pitches multiples of 16 bytes");
   if (ybr == nullptr || gamma == nullptr || dyb == nullptr) return set_error("ivb_rmsnorm_bwd_layerscale: ybr, gamma, dyb are required");
+  if (misaligned(16, dy, x, dx_in, dx_out, ybr, dyb) || misaligned(8, weight, gamma))
+    return set_error("ivb_rmsnorm_bwd_layerscale: dy, x, dx_in, dx_out, ybr and dyb must be 16-byte aligned, weight and "
+                     "gamma 8-byte aligned");
   if (rms_bwd_tma_smem(D, dx_in != nullptr) > 226 * 1024)
     return set_error("ivb_rmsnorm_bwd_layerscale: D too large for the shared-memory row ring (use the separate kernels)");
   return launch_rms_bwd_tma(dy, lddy, x, ldx, weight, rstd, M, D, dx_in, lddx_in, dx_out, lddx, dweight, ybr, ldyb, gamma,
