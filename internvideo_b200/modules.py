@@ -331,6 +331,102 @@ class Block(nn.Module):
         return out.reshape(B, n, D).to(x.dtype)
 
 
+class VideoMAEAttention(nn.Module):
+    """Parameters of the VideoMAE attention (videomae.py:62-101, IV1 modeling_finetune.py:77-129): qkv without bias plus
+    separate q_bias / v_bias.  Both fused block paths need heads * head_dim == dim."""
+
+    def __init__(self, dim, num_heads=8, qkv_bias=False, qk_scale=None, attn_head_dim=None):
+        super().__init__()
+        head_dim = attn_head_dim if attn_head_dim is not None else dim // num_heads
+        if head_dim * num_heads != dim:
+            raise NotImplementedError(f"ivb200 VideoMAEAttention: heads * head_dim ({num_heads} * {head_dim}) must be "
+                                      f"dim ({dim})")
+        self.num_heads = num_heads
+        self.scale = qk_scale or head_dim ** -0.5
+        self.qkv = nn.Linear(dim, dim * 3, bias=False)
+        if qkv_bias:
+            self.q_bias = nn.Parameter(torch.zeros(dim))
+            self.v_bias = nn.Parameter(torch.zeros(dim))
+        else:
+            self.q_bias = self.v_bias = None
+        self.proj = nn.Linear(dim, dim)
+
+    def qkv_bias_vector(self):
+        """q_bias | 0 | v_bias (k has no bias), or None."""
+        if self.q_bias is None:
+            return None
+        return torch.cat((self.q_bias, torch.zeros_like(self.v_bias), self.v_bias))
+
+
+class VideoMAEBlock(nn.Module):
+    """The VideoMAE LayerNorm block (videomae.py:104-132 for the VideoMAEv2 teacher, IV1 modeling_finetune.py:132-181):
+    LayerNorm pre-norm, q/v-bias attention, erf GELU MLP, optional gamma_1 / gamma_2, through ops.block_forward with
+    spec.layernorm and, when trained, ops.BlockFn.  with_cp: keep only the block input and recompute its forward in
+    backward (IV1's with_cp)."""
+
+    def __init__(self, dim, num_heads, mlp_ratio=4.0, qkv_bias=False, qk_scale=None, drop=0.0, attn_drop=0.0,
+                 drop_path=0.0, init_values=None, act_layer=nn.GELU, norm_layer=nn.LayerNorm, attn_head_dim=None,
+                 with_cp=False):
+        super().__init__()
+        if drop or attn_drop:
+            raise NotImplementedError("ivb200 VideoMAEBlock: dropout is 0 in every recipe")
+        self.norm1 = norm_layer(dim)
+        self.attn = VideoMAEAttention(dim, num_heads, qkv_bias, qk_scale, attn_head_dim)
+        self.norm2 = norm_layer(dim)
+        self.mlp = Mlp(dim, int(dim * mlp_ratio))
+        if init_values and init_values > 0:
+            self.gamma_1 = nn.Parameter(init_values * torch.ones(dim))
+            self.gamma_2 = nn.Parameter(init_values * torch.ones(dim))
+        else:
+            self.gamma_1 = self.gamma_2 = None
+        self.drop_prob = float(drop_path)
+        self.with_cp = bool(with_cp)
+        self.fp8_inference = None   # set_fp8_inference
+
+    def _drop_path_rows(self, B, n, device):
+        """IV1's DropPath draw (timm drop_path: Bernoulli(keep) / keep per sample, `rand < keep`), once per branch in
+        branch order, as per-row epilogue factors: (rs1, rs2) fp32 [B*n], or (None, None) in eval or at rate 0."""
+        if self.drop_prob == 0.0 or not self.training:
+            return None, None
+        keep = 1.0 - self.drop_prob
+        return tuple(((torch.rand(B, device=device) < keep).to(f32) / keep).repeat_interleave(n) for _ in range(2))
+
+    def _spec(self, B, n, training=False, head_axis=False):
+        a = self.attn
+        return ops.BlockSpec(B, n, a.num_heads, layernorm=True, eps1=self.norm1.eps, eps2=self.norm2.eps, scale=a.scale,
+                             head_axis=head_axis, checkpoint=self.with_cp, precision=block_precision(self, training))
+
+    def _param_tuple(self):
+        a = self.attn
+        return ops.BlockParams(
+            n1w=self.norm1.weight, n1b=self.norm1.bias, qkvw=a.qkv.weight, qkvb=a.qkv_bias_vector(), qnw=None, knw=None,
+            projw=a.proj.weight, projb=a.proj.bias, g1=self.gamma_1, n2w=self.norm2.weight, n2b=self.norm2.bias,
+            fc1w=self.mlp.fc1.weight, fc1b=self.mlp.fc1.bias, fc2w=self.mlp.fc2.weight, fc2b=self.mlp.fc2.bias,
+            g2=self.gamma_2)
+
+    def forward_stream(self, x2d, B, n):
+        """fp32 residual stream [B*n, D] -> same, through ops.BlockFn when a gradient is needed."""
+        rs = self._drop_path_rows(B, n, x2d.device)
+        if not torch.is_grad_enabled():
+            return self.forward_infer(x2d, B, n, rs)
+        return ops.BlockFn.apply(x2d, self._spec(B, n, training=True), *rs, *self._param_tuple())
+
+    def forward_infer(self, x2d, B, n, rowscale=(None, None), head_axis=False):
+        """No-grad form: ops.block_forward with nothing saved.  head_axis: the VideoMAEv2 teacher's attention over the
+        heads of each token, as the reference executes it (BlockSpec.head_axis)."""
+        with torch.no_grad():
+            out, _ = ops.block_forward(x2d, self._spec(B, n, head_axis=head_axis), self._param_tuple(), rowscale[0],
+                                       rowscale[1], save=False)
+        return out
+
+    def _fp8_linears(self):
+        return (self.attn.qkv, self.attn.proj, self.mlp.fc1, self.mlp.fc2)
+
+    def forward(self, x):
+        B, n, D = x.shape
+        return self.forward_stream(x.reshape(B * n, D).float().contiguous(), B, n).reshape(B, n, D)
+
+
 def set_fp8(model: nn.Module, enabled: bool = True) -> int:
     """Switch the FP8 mode of every ViT Block in `model` (stage-1 student, CLIP tower, stage-2 tower, InternVL teacher)
     on or off; returns how many blocks were switched.
@@ -370,7 +466,7 @@ class Fp8InferenceWeights:
 
 
 def block_precision(block, training=False):
-    """The ops.BlockSpec precision a forward of `block` (Block or teachers.TeacherBlock) runs at, from its switches:
+    """The ops.BlockSpec precision a forward of `block` (Block or VideoMAEBlock) runs at, from its switches:
     set_fp8 (Block.fp8) and set_fp8_inference (fp8_inference).  training: the forward needs a gradient."""
     fp8 = getattr(block, "fp8", False)
     if block.fp8_inference is None:
@@ -383,7 +479,7 @@ def block_precision(block, training=False):
 
 
 def set_fp8_inference(model: nn.Module, enabled: bool = True) -> int:
-    """Switch FP8 inference on or off for every ViT Block and VideoMAE TeacherBlock in `model` (frozen towers: the
+    """Switch FP8 inference on or off for every ViT Block and VideoMAEBlock in `model` (frozen towers: the
     InternVL and VideoMAE teachers, the frozen CLIP and stage-2 towers); returns how many blocks were switched.
 
     In this mode a block's no-grad forward runs its four GEMMs (qkv, proj, fc1, fc2) on the FP8 tensor cores with
@@ -392,8 +488,7 @@ def set_fp8_inference(model: nn.Module, enabled: bool = True) -> int:
     they are re-quantised only when a weight changes.  Attention, the q/k norms and the fp32 residual stream stay
     bf16 / fp32, and switching off restores the bf16 path bit for bit.  A switched Block refuses a forward that
     needs a gradient, and the mode excludes set_fp8 on the same block."""
-    from .teachers import TeacherBlock
-    blocks = [m for m in model.modules() if isinstance(m, (Block, TeacherBlock))]
+    blocks = [m for m in model.modules() if isinstance(m, (Block, VideoMAEBlock))]
     if enabled and any(getattr(m, "fp8", False) for m in blocks):
         raise ll._lib.IvbError("set_fp8_inference: a block is in FP8 training mode (set_fp8); switch that off first")
     for m in blocks:

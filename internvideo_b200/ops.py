@@ -193,10 +193,10 @@ BF16, FP8_TENSOR = "bf16", "fp8"
 
 
 class BlockSpec(NamedTuple):
-    """Everything a fused block call needs besides its tensors.  layernorm: the VideoMAEv2 teacher's LayerNorm block
-    (inference only) instead of the RMSNorm block; eps1 / eps2 are the eps of its two norms.  scale: the attention scale
-    (None: d ** -0.5).  head_axis: the VideoMAEv2 teacher's attention over the heads of each token (inference only).
-    checkpoint: BlockFn keeps only the block input and recomputes the forward in the backward."""
+    """Everything a fused block call needs besides its tensors.  layernorm: the VideoMAE LayerNorm block (InternVideo1,
+    VideoMAEv2 teacher) instead of the RMSNorm block; eps1 / eps2 are the eps of its two norms.  scale: the attention
+    scale (None: d ** -0.5).  head_axis: the VideoMAEv2 teacher's attention over the heads of each token (inference
+    only).  checkpoint: BlockFn keeps only the block input and recomputes the forward in the backward."""
     B: int
     n: int
     H: int
@@ -222,16 +222,17 @@ class BlockSpec(NamedTuple):
 BlockParams = namedtuple("BlockParams", "n1w qkvw qkvb qnw knw projw projb g1 n2w fc1w fc1b fc2w fc2b g2 n1b n2b",
                          defaults=(None, None))
 
-# What block_forward(save=True) keeps for block_backward: activations and norm statistics, and in FP8_TENSOR the E4M3
-# copies of the four weights' transposes with their scales (the input-gradient GEMMs' operands; None in bf16).
-BlockSaved = namedtuple("BlockSaved", "n1 qkv qkn a lse rstd1 rq rk x1 y1 n2 rstd2 h g y2 "
+# What block_forward(save=True) keeps for block_backward: activations and norm statistics (mean1 / mean2 None on RMSNorm
+# blocks), and in FP8_TENSOR the E4M3 copies of the four weights' transposes with their scales (the input-gradient
+# GEMMs' operands; None in bf16).
+BlockSaved = namedtuple("BlockSaved", "n1 qkv qkn a lse mean1 rstd1 rq rk x1 y1 n2 mean2 rstd2 h g y2 "
                                       "qkvw_t qkvw_s projw_t projw_s fc1w_t fc1w_s fc2w_t fc2w_s")
 
 
 def block_forward(x, spec, p, rs1=None, rs2=None, save=True):
     """One pre-norm ViT block over the fp32 residual stream [B*n, D]: spec a BlockSpec, p the BlockParams.  The
-    InternVideo2 block (Block.forward, internvideo2_pretrain.py:279-297), or with spec.layernorm the VideoMAEv2 teacher
-    block (videomae.py:104-132: LayerNorm with bias, q/v bias on qkv, no q/k norm, erf GELU):
+    InternVideo2 block (Block.forward, internvideo2_pretrain.py:279-297), or with spec.layernorm the VideoMAE block
+    (videomae.py:104-132, IV1 modeling_finetune.py:132-181: LayerNorm with bias, q/v bias on qkv, no q/k norm, erf GELU):
 
       n1 = Norm(x) ; qkv = n1 Wqkv^T + bqkv ; (q,k) = RMSNorm_C(q), RMSNorm_C(k) ; a = attn(q,k,v)
       x1 = x + rs1 * g1 * (a Wp^T + bp)                [LayerScale + DropPath + residual fused in the GEMM epilogue]
@@ -258,11 +259,10 @@ def block_forward(x, spec, p, rs1=None, rs2=None, save=True):
         # (q, q_t, scale_inv) per weight; q_t only when the backward will need it
         w8 = [ll.fp8_quantize(w, ll.FP8_E4M3, transpose=save)[:3] for w in (p.qkvw, p.projw, p.fc1w, p.fc2w)]
 
-    def norm(t, w, b, eps):   # n1, n2 (and rstd for the backward)
+    def norm(t, w, b, eps):   # n1, n2 (and mean, rstd for the backward)
         if per_token:
-            return ll.norm_fwd_fp8(t, w, b, eps=eps, layernorm=spec.layernorm), None
-        y, _, rstd = ll.norm_fwd(t, w, b, eps=eps, layernorm=spec.layernorm, want_stats=save)
-        return y, rstd
+            return ll.norm_fwd_fp8(t, w, b, eps=eps, layernorm=spec.layernorm), None, None
+        return ll.norm_fwd(t, w, b, eps=eps, layernorm=spec.layernorm, want_stats=save)
 
     def linear(act, i, w, **epilogue):
         if prec == BF16:
@@ -274,7 +274,7 @@ def block_forward(x, spec, p, rs1=None, rs2=None, save=True):
             q, _, s, _ = ll.fp8_quantize(act, ll.FP8_E4M3)
             wq, _, ws = w8[i]
         return ll.gemm_fp8(q, s, wq, ws, **epilogue)
-    n1, rstd1 = norm(x, p.n1w, p.n1b, spec.eps1)
+    n1, mean1, rstd1 = norm(x, p.n1w, p.n1b, spec.eps1)
     qkv = linear(n1, 0, p.qkvw, bias=p.qkvb)
     q, k, v = qkv[:, :D], qkv[:, D:2 * D], qkv[:, 2 * D:]
     qkn = rq = rk = lse = None
@@ -294,7 +294,7 @@ def block_forward(x, spec, p, rs1=None, rs2=None, save=True):
         a, lse = ll.attn_fwd(q, k, v, B, n, H, d, spec.attn_scale(d), want_lse=save)
     y1 = torch.empty((M, D), device=x.device, dtype=bf16) if (p.g1 is not None and save) else None
     x1 = linear(a, 1, p.projw, epi=ll.EPI_RESID, bias=p.projb, gamma=p.g1, aux=x, out1=y1, rowscale=rs1)
-    n2, rstd2 = norm(x1, p.n2w, p.n2b, spec.eps2)
+    n2, mean2, rstd2 = norm(x1, p.n2w, p.n2b, spec.eps2)
     h = torch.empty((M, p.fc1w.shape[0]), device=x.device, dtype=bf16) if save else None
     g = linear(n2, 2, p.fc1w, epi=ll.EPI_BIAS_GELU, flags=spec.gelu_flags(save), bias=p.fc1b, out1=h)
     y2 = torch.empty((M, D), device=x.device, dtype=bf16) if (p.g2 is not None and save) else None
@@ -302,15 +302,16 @@ def block_forward(x, spec, p, rs1=None, rs2=None, save=True):
     if not save:
         return x2, None
     wt8 = [t for _, q_t, s in w8 for t in (q_t, s)] if w8 is not None else [None] * 8
-    return x2, BlockSaved(n1, qkv, qkn, a, lse, rstd1, rq, rk, x1, y1, n2, rstd2, h, g, y2, *wt8)
+    return x2, BlockSaved(n1, qkv, qkn, a, lse, mean1, rstd1, rq, rk, x1, y1, n2, mean2, rstd2, h, g, y2, *wt8)
 
 
 def block_backward(x, s, spec, t, P, dx2, rs1, rs2):
-    """Backward of block_forward(save=True) for the RMSNorm block, from its BlockSaved s: 13 to 17 library calls in bf16
-    (with or without the q/k norms and the qkv bias, the fused norm2 + LayerScale backward), and in FP8_TENSOR one more
-    per input-gradient GEMM (the E5M2 cast of its gradient).  `t` are the block's tensors as autograd handed them back,
-    `P` the nn.Parameter objects (gradient sink), both BlockParams.  Returns (dx0, BlockParams of gradients | None when
-    the sink took them)."""
+    """Backward of block_forward(save=True), from its BlockSaved s: 13 to 17 library calls in bf16 (with or without the
+    q/k norms and the qkv bias, the fused RMSNorm norm2 + LayerScale backward), and in FP8_TENSOR one more per
+    input-gradient GEMM (the E5M2 cast of its gradient).  The LayerNorm block (spec.layernorm) also returns its norms'
+    bias gradients and always runs the attention branch's LayerScale backward as its own call.  `t` are the block's
+    tensors as autograd handed them back, `P` the nn.Parameter objects (gradient sink), both BlockParams.  Returns
+    (dx0, BlockParams of gradients | None when the sink took them)."""
     B, n, H = spec.B, spec.n, spec.H
     M, D = x.shape
     d = D // H
@@ -325,6 +326,8 @@ def block_backward(x, s, spec, t, P, dx2, rs1, rs2):
     sink = _common_sink(P)
     small = [(nm, getattr(t, nm), D) for nm in ("g2", "fc2b", "n2w", "g1", "projb", "qnw", "knw", "n1w")]
     small += [("fc1b", t.fc1b, Hd), ("qkvb", t.qkvb, 3 * D)]
+    if spec.layernorm:
+        small += [("n2b", t.n2b, D), ("n1b", t.n1b, D)]
     seg, vec, span, base = _plan_small(small, sink, x.device)
     if sink is not None and span is None:
         sink = None           # small parameters not contiguous in the flat buffer: autograd path
@@ -350,12 +353,13 @@ def block_backward(x, s, spec, t, P, dx2, rs1, rs2):
     dfc1w = wgrad(dh, s.n2, P.fc1w)
     dn2 = dgrad(dh, t.fc1w, s.fc1w_t, s.fc1w_s)
     # ---- attention branch
-    if t.g1 is not None and D <= 1536 and M >= 1024:
+    if not spec.layernorm and t.g1 is not None and D <= 1536 and M >= 1024:
         # norm2 backward fused with the attention branch's LayerScale backward: the gradient of the residual
         # stream is produced and consumed in one pass over the rows
         dx1, dy1 = ll.rmsnorm_bwd_layerscale(dn2, s.x1, t.n2w, s.rstd2, dx2, s.y1, t.g1, dn2w, dg1, dcs1, rowscale=rs1)
     else:
-        dx1 = ll.norm_bwd(dn2, s.x1, t.n2w, None, s.rstd2, dx_in=dx2, dweight=dn2w)
+        dx1 = ll.norm_bwd(dn2, s.x1, t.n2w, s.mean2, s.rstd2, layernorm=spec.layernorm, dx_in=dx2, dweight=dn2w,
+                          dbias=seg.get("n2b"))
         dy1 = ll.layerscale_bwd(dx1, s.y1, t.g1, dg1 if t.g1 is not None else None, dcs1, rowscale=rs1)
     dprojw = wgrad(dy1, s.a, P.projw)
     da = dgrad(dy1, t.projw, s.projw_t, s.projw_s)
@@ -372,7 +376,8 @@ def block_backward(x, s, spec, t, P, dx2, rs1, rs2):
     if t.qkvb is not None:
         ll.colsum(dqkv, out=seg["qkvb"])
     dn1 = dgrad(dqkv, t.qkvw, s.qkvw_t, s.qkvw_s)
-    dx0 = ll.norm_bwd(dn1, x, t.n1w, None, s.rstd1, dx_in=dx1, dweight=seg["n1w"])
+    dx0 = ll.norm_bwd(dn1, x, t.n1w, s.mean1, s.rstd1, layernorm=spec.layernorm, dx_in=dx1, dweight=seg["n1w"],
+                      dbias=seg.get("n1b"))
     # ---- O(D) glue: bias grads through LayerScale (layerscale_bwd already folds gamma into the
     # bias-gradient column sums), cast to the parameter dtype
     if sink is not None:
@@ -388,7 +393,7 @@ def block_backward(x, s, spec, t, P, dx2, rs1, rs2):
 
 
 class BlockFn(torch.autograd.Function):
-    """Differentiable block_forward of the RMSNorm block: apply(x, spec, rs1, rs2, *params) with spec a BlockSpec,
+    """Differentiable block_forward: apply(x, spec, rs1, rs2, *params) with spec a BlockSpec (spec.head_axis refused),
     params the BlockParams and rs1 / rs2 optional fp32 [B*n] per-row DropPath keep/scale factors of the two branches.
 
     spec.checkpoint is the reference's `with_cp` / `use_checkpoint` (internvideo2_pretrain.py:294-295,
@@ -398,6 +403,8 @@ class BlockFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, x, spec, rs1, rs2, *params):
+        if spec.head_axis:
+            raise ll._lib.IvbError("BlockFn: head-axis attention (the VideoMAEv2 teacher's) has no backward")
         params = BlockParams(*params)
         x2, saved = block_forward(x, spec, params, rs1, rs2, save=not spec.checkpoint)
         ctx.spec, ctx.params = spec, params

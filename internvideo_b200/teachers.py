@@ -17,8 +17,7 @@ import torch
 import torch.nn as nn
 
 from . import lowlevel as ll
-from . import ops
-from .modules import (LayerNormB, TubeletPatchEmbed, bf16, block_precision, check_input, embed_tokens,
+from .modules import (LayerNormB, TubeletPatchEmbed, VideoMAEBlock, bf16, check_input, embed_tokens,
                       get_sinusoid_encoding_table, init_weights, run_blocks, to_2tuple, vit_stack)
 
 
@@ -97,75 +96,6 @@ class InternVL_CLIP(nn.Module):
 
 
 # ------------------------------------------------------------------------------------------------ MAE teacher
-class TeacherAttention(nn.Module):
-    """videomae.py:62-101 (parameter layout: qkv without bias + separate q_bias / v_bias)."""
-
-    def __init__(self, dim, num_heads=8, qkv_bias=False, qk_scale=None, attn_drop=0.0, proj_drop=0.0, attn_head_dim=None):
-        super().__init__()
-        self.num_heads = num_heads
-        head_dim = attn_head_dim if attn_head_dim is not None else dim // num_heads
-        all_head_dim = head_dim * num_heads
-        self.scale = qk_scale or head_dim ** -0.5
-        self.qkv = nn.Linear(dim, all_head_dim * 3, bias=False)
-        if qkv_bias:
-            self.q_bias = nn.Parameter(torch.zeros(all_head_dim))
-            self.v_bias = nn.Parameter(torch.zeros(all_head_dim))
-        else:
-            self.q_bias = self.v_bias = None
-        self.proj = nn.Linear(all_head_dim, dim)
-
-    def qkv_bias_vector(self):
-        if self.q_bias is None:
-            return None
-        return torch.cat((self.q_bias, torch.zeros_like(self.v_bias), self.v_bias))       # :86
-
-
-class TeacherMlp(nn.Module):
-    def __init__(self, in_features, hidden_features=None, out_features=None, act_layer=nn.GELU, drop=0.0):
-        super().__init__()
-        self.fc1 = nn.Linear(in_features, hidden_features or in_features)
-        self.fc2 = nn.Linear(hidden_features or in_features, out_features or in_features)
-
-
-class TeacherBlock(nn.Module):
-    """videomae.py:104-132: LayerNorm pre-norm block, optional gamma_1 / gamma_2."""
-
-    def __init__(self, dim, num_heads, mlp_ratio=4.0, qkv_bias=False, qk_scale=None, drop=0.0, attn_drop=0.0,
-                 drop_path=0.0, init_values=None, act_layer=nn.GELU, norm_layer=nn.LayerNorm, attn_head_dim=None):
-        super().__init__()
-        self.norm1 = norm_layer(dim)
-        self.attn = TeacherAttention(dim, num_heads=num_heads, qkv_bias=qkv_bias, qk_scale=qk_scale,
-                                     attn_head_dim=attn_head_dim)
-        self.norm2 = norm_layer(dim)
-        self.mlp = TeacherMlp(dim, int(dim * mlp_ratio))
-        if init_values and init_values > 0:
-            self.gamma_1 = nn.Parameter(init_values * torch.ones(dim))
-            self.gamma_2 = nn.Parameter(init_values * torch.ones(dim))
-        else:
-            self.gamma_1 = self.gamma_2 = None
-        self.fp8_inference = None   # modules.set_fp8_inference
-
-    def _fp8_linears(self):
-        return (self.attn.qkv, self.attn.proj, self.mlp.fc1, self.mlp.fc2)
-
-    def _param_tuple(self):
-        a = self.attn
-        return ops.BlockParams(
-            n1w=self.norm1.weight, n1b=self.norm1.bias, qkvw=a.qkv.weight, qkvb=a.qkv_bias_vector(), qnw=None, knw=None,
-            projw=a.proj.weight, projb=a.proj.bias, g1=self.gamma_1, n2w=self.norm2.weight, n2b=self.norm2.bias,
-            fc1w=self.mlp.fc1.weight, fc1b=self.mlp.fc1.bias, fc2w=self.mlp.fc2.weight, fc2b=self.mlp.fc2.bias,
-            g2=self.gamma_2)
-
-    def forward_infer(self, x2d, B, n, head_axis_attention=True):
-        """fp32 residual stream [B*n, D] -> same: ops.block_forward's LayerNorm form, nothing saved."""
-        a = self.attn
-        with torch.no_grad():
-            params = self._param_tuple()
-            spec = ops.BlockSpec(B, n, a.num_heads, layernorm=True, eps1=self.norm1.eps, eps2=self.norm2.eps,
-                                 scale=a.scale, head_axis=head_axis_attention, precision=block_precision(self))
-            return ops.block_forward(x2d, spec, params, save=False)[0]
-
-
 class VisionTransformer(nn.Module):
     """videomae.py:207-313 — the VideoMAEv2 teacher.  forward(x[B,C,T,H,W]) -> [K, B, N, C] L2-normalised features of
     the last K blocks (the final LayerNorm is applied to the last block's output before it is tapped, :291-292)."""
@@ -192,8 +122,8 @@ class VisionTransformer(nn.Module):
         eps = getattr(ln(8), "eps", 1e-5)
         mk = lambda d: LayerNormB(d, eps=eps)  # noqa: E731
         self.blocks = nn.ModuleList([
-            TeacherBlock(embed_dim, num_heads, mlp_ratio, qkv_bias=qkv_bias, qk_scale=qk_scale, norm_layer=mk,
-                         init_values=init_values) for _ in range(depth)])
+            VideoMAEBlock(embed_dim, num_heads, mlp_ratio, qkv_bias=qkv_bias, qk_scale=qk_scale, norm_layer=mk,
+                          init_values=init_values) for _ in range(depth)])
         self.norm = mk(embed_dim)
         self.apply(init_weights)
 
@@ -211,7 +141,7 @@ class VisionTransformer(nn.Module):
         h = embed_tokens(self.patch_embed, x, idx, None, self.pos_embed.to(x.device).float())     # videomae.py:293
 
         def block(i, blk, h):
-            h = blk.forward_infer(h, B, N, self.head_axis_attention)
+            h = blk.forward_infer(h, B, N, head_axis=self.head_axis_attention)
             return self.norm(h) if i == self.depth - 1 else h                     # bf16 [B*N, D] after the last
 
         h, taps = run_blocks(self.blocks, h, block, self.return_index)

@@ -3,7 +3,7 @@ form of the hot path — tubelet embed of the visible tokens, LayerNorm/q-v-bias
 visible + mask tokens, pixel head on the masked tokens, MSE against per-patch normalised pixels).
 
 Mirrors InternVideo1/Pretrain/VideoMAE:
-  Attention, Block                      modeling_finetune.py:77-181   (qkv without bias + q_bias / v_bias, optional gamma_1/2)
+  Attention, Block                      modeling_finetune.py:77-181   (modules.VideoMAEBlock, shared with the VideoMAEv2 teacher)
   PatchEmbed                            modeling_finetune.py:184-219  (Conv3d k = s = (tubelet, p, p))
   get_sinusoid_encoding_table           modeling_finetune.py:224-242
   PretrainVisionTransformerEncoder      modeling_pretrain.py:34-171
@@ -13,8 +13,9 @@ Mirrors InternVideo1/Pretrain/VideoMAE:
 Same constructor arguments, same state_dict keys, same forward contract
 `model(x[B,3,T,H,W], mask[B,N] bool) -> [B, N_mask, 3*tubelet*p*p]`.
 
-Built from the differentiable primitives of ops.py (LayerNorm rows, wgmma GEMM with bias / GELU epilogues, wgmma flash
-attention, visible-only im2col embed); the residual stream is fp32, everything else bf16.  No CPU path.
+The blocks run through the fused block of ops.py (ops.BlockFn with spec.layernorm: LayerScale, DropPath and the residual
+add in the GEMM epilogues); the embed, final norms and heads through its primitives.  The residual stream is fp32,
+everything else bf16.  No CPU path.
 """
 from __future__ import annotations
 
@@ -26,109 +27,28 @@ import torch.nn as nn
 from . import lowlevel as ll
 from . import ops
 from .modules import TubeletPatchEmbed as PatchEmbed  # modeling_finetune.py:184-219 (parameters; im2col + GEMM)
-from .modules import bf16, check_input, embed_tokens, f32, get_sinusoid_encoding_table, index_poison, run_blocks
+from .modules import (VideoMAEBlock, bf16, check_input, embed_tokens, f32, get_sinusoid_encoding_table, index_poison,
+                      run_blocks)
 from .modules import to_2tuple  # noqa: F401  (a name of the reference module)
 
 IMAGENET_DEFAULT_MEAN = (0.485, 0.456, 0.406)
 IMAGENET_DEFAULT_STD = (0.229, 0.224, 0.225)
 
 
-def _drop_path_rows(a, B, n, p, training):
-    """timm drop_path on a [B*n, D] stream: one Bernoulli(keep)/keep factor per sample."""
-    if p == 0.0 or not training:
-        return a
-    keep = 1.0 - p
-    m = (torch.rand(B, device=a.device) < keep).to(a.dtype) / keep
-    return a * m.repeat_interleave(n)[:, None]
+def _blocks(dim, depth, num_heads, mlp_ratio, qkv_bias, qk_scale, drop, attn_drop, drop_path_rate, norm_layer,
+            init_values, with_cp):
+    """The encoder's or the decoder's blocks (modeling_pretrain.py:78-92, :208-222), DropPath rising linearly to
+    drop_path_rate; with_cp: each block keeps only its input and recomputes its forward in backward."""
+    dpr = [x.item() for x in torch.linspace(0, drop_path_rate, depth)]
+    return nn.ModuleList([
+        VideoMAEBlock(dim, num_heads, mlp_ratio, qkv_bias=qkv_bias, qk_scale=qk_scale, drop=drop, attn_drop=attn_drop,
+                      drop_path=dpr[i], init_values=init_values, norm_layer=norm_layer, with_cp=with_cp)
+        for i in range(depth)])
 
 
-class Mlp(nn.Module):
-    def __init__(self, in_features, hidden_features=None, out_features=None, act_layer=nn.GELU, drop=0.0):
-        super().__init__()
-        out_features = out_features or in_features
-        hidden_features = hidden_features or in_features
-        self.fc1 = nn.Linear(in_features, hidden_features)
-        self.act = act_layer()
-        self.fc2 = nn.Linear(hidden_features, out_features)
-        if drop:
-            raise NotImplementedError("ivb200 VideoMAE: dropout is 0 in every pre-training recipe")
-
-
-class Attention(nn.Module):
-    """modeling_finetune.py:77-129."""
-
-    def __init__(self, dim, num_heads=8, qkv_bias=False, qk_scale=None, attn_drop=0.0, proj_drop=0.0, attn_head_dim=None):
-        super().__init__()
-        self.num_heads = num_heads
-        head_dim = attn_head_dim if attn_head_dim is not None else dim // num_heads
-        self.head_dim = head_dim
-        all_head_dim = head_dim * num_heads
-        self.scale = qk_scale or head_dim ** -0.5
-        self.qkv = nn.Linear(dim, all_head_dim * 3, bias=False)
-        if qkv_bias:
-            self.q_bias = nn.Parameter(torch.zeros(all_head_dim))
-            self.v_bias = nn.Parameter(torch.zeros(all_head_dim))
-        else:
-            self.q_bias = self.v_bias = None
-        self.proj = nn.Linear(all_head_dim, dim)
-        if attn_drop or proj_drop:
-            raise NotImplementedError("ivb200 VideoMAE: attention / projection dropout are 0 in every pre-training recipe")
-
-    def forward_rows(self, h, B, n):
-        """h: bf16 [B*n, dim] -> fp32 [B*n, dim]."""
-        bias = None
-        if self.q_bias is not None:       # :111-115 — k has no bias
-            bias = torch.cat((self.q_bias, torch.zeros_like(self.v_bias, requires_grad=False), self.v_bias))
-        qkv = ops.linear(h, self.qkv.weight, bias)
-        A = self.num_heads * self.head_dim
-        o = ops.AttnFn.apply(qkv[:, :A], qkv[:, A:2 * A], qkv[:, 2 * A:], B, n, self.num_heads, self.head_dim, self.scale)
-        return ops.linear(o, self.proj.weight, self.proj.bias, True)
-
-
-class Block(nn.Module):
-    """modeling_finetune.py:132-181."""
-
-    def __init__(self, dim, num_heads, mlp_ratio=4.0, qkv_bias=False, qk_scale=None, drop=0.0, attn_drop=0.0,
-                 drop_path=0.0, init_values=None, act_layer=nn.GELU, norm_layer=nn.LayerNorm, attn_head_dim=None):
-        super().__init__()
-        self.norm1 = norm_layer(dim)
-        self.attn = Attention(dim, num_heads=num_heads, qkv_bias=qkv_bias, qk_scale=qk_scale, attn_drop=attn_drop,
-                              proj_drop=drop, attn_head_dim=attn_head_dim)
-        self.drop_prob = float(drop_path)
-        self.norm2 = norm_layer(dim)
-        self.mlp = Mlp(in_features=dim, hidden_features=int(dim * mlp_ratio), act_layer=act_layer, drop=drop)
-        if init_values is not None and init_values > 0:
-            self.gamma_1 = nn.Parameter(init_values * torch.ones(dim), requires_grad=True)
-            self.gamma_2 = nn.Parameter(init_values * torch.ones(dim), requires_grad=True)
-        else:
-            self.gamma_1 = self.gamma_2 = None
-
-    def forward_rows(self, x, B, n):
-        """x: fp32 residual stream [B*n, dim] -> same."""
-        a = self.attn.forward_rows(ops.layernorm(x, self.norm1.weight, self.norm1.bias, self.norm1.eps), B, n)
-        if self.gamma_1 is not None:
-            a = a * self.gamma_1.float()
-        x = x + _drop_path_rows(a, B, n, self.drop_prob, self.training)
-        h = ops.layernorm(x, self.norm2.weight, self.norm2.bias, self.norm2.eps)
-        g = ops.LinearGeluFn.apply(h, self.mlp.fc1.weight, self.mlp.fc1.bias, False)
-        m = ops.linear(g, self.mlp.fc2.weight, self.mlp.fc2.bias, True)
-        if self.gamma_2 is not None:
-            m = m * self.gamma_2.float()
-        return x + _drop_path_rows(m, B, n, self.drop_prob, self.training)
-
-    def forward(self, x):
-        B, n, D = x.shape
-        return self.forward_rows(x.reshape(B * n, D).float(), B, n).reshape(B, n, D)
-
-
-def _run_blocks(blocks, h, B, n, with_cp):
-    """The encoder's and the decoder's block loop over the fp32 stream [B*n, D]; with_cp: each block keeps only its
-    input and recomputes its forward in backward (torch.utils.checkpoint)."""
-    def block(i, blk, h):
-        if with_cp and torch.is_grad_enabled():
-            return torch.utils.checkpoint.checkpoint(blk.forward_rows, h, B, n, use_reentrant=False)
-        return blk.forward_rows(h, B, n)
-    return run_blocks(blocks, h, block)[0]
+def _run_blocks(blocks, h, B, n):
+    """The encoder's and the decoder's block loop over the fp32 stream [B*n, D]."""
+    return run_blocks(blocks, h, lambda i, blk, h: blk.forward_stream(h, B, n))[0]
 
 
 def _xavier_init(m):
@@ -164,16 +84,12 @@ class PretrainVisionTransformerEncoder(nn.Module):
         self.patch_embed = PatchEmbed(img_size=img_size, patch_size=patch_size, in_chans=in_chans, embed_dim=embed_dim,
                                       tubelet_size=tubelet_size)
         num_patches = self.patch_embed.num_patches
-        self.with_cp = with_cp
         if use_learnable_pos_emb:
             self.pos_embed = nn.Parameter(torch.zeros(1, num_patches + 1, embed_dim))
         else:
             self.pos_embed = get_sinusoid_encoding_table(num_patches, embed_dim)     # plain tensor, like the reference
-        dpr = [x.item() for x in torch.linspace(0, drop_path_rate, depth)]
-        self.blocks = nn.ModuleList([
-            Block(dim=embed_dim, num_heads=num_heads, mlp_ratio=mlp_ratio, qkv_bias=qkv_bias, qk_scale=qk_scale,
-                  drop=drop_rate, attn_drop=attn_drop_rate, drop_path=dpr[i], norm_layer=norm_layer,
-                  init_values=init_values) for i in range(depth)])
+        self.blocks = _blocks(embed_dim, depth, num_heads, mlp_ratio, qkv_bias, qk_scale, drop_rate, attn_drop_rate,
+                              drop_path_rate, norm_layer, init_values, with_cp)
         self.norm = norm_layer(embed_dim)
         self.head = nn.Linear(embed_dim, num_classes) if num_classes > 0 else nn.Identity()
         if use_learnable_pos_emb:
@@ -191,7 +107,7 @@ class PretrainVisionTransformerEncoder(nn.Module):
         """x bf16 video, idx int32 [B, 1+nv] (cls slot + visible patches) -> bf16 [B*nv, C_e] after the final LayerNorm."""
         pe = self.patch_embed
         pos = self.pos_embed[:, -pe.num_patches:].to(device=x.device)          # learnable table has an unused first row
-        h = _run_blocks(self.blocks, embed_tokens(pe, x, idx, None, pos), B, nv, self.with_cp)
+        h = _run_blocks(self.blocks, embed_tokens(pe, x, idx, None, pos), B, nv)
         h = ops.layernorm(h, self.norm.weight, self.norm.bias, self.norm.eps)
         if isinstance(self.head, nn.Linear):
             h = ops.linear(h, self.head.weight, self.head.bias)
@@ -215,12 +131,9 @@ class PretrainVisionTransformerDecoder(nn.Module):
         assert num_classes == 3 * tubelet_size * patch_size ** 2
         self.num_features = self.embed_dim = embed_dim
         self.patch_size = patch_size
-        self.with_cp, self.with_fp16 = with_cp, with_fp16
-        dpr = [x.item() for x in torch.linspace(0, drop_path_rate, depth)]
-        self.blocks = nn.ModuleList([
-            Block(dim=embed_dim, num_heads=num_heads, mlp_ratio=mlp_ratio, qkv_bias=qkv_bias, qk_scale=qk_scale,
-                  drop=drop_rate, attn_drop=attn_drop_rate, drop_path=dpr[i], norm_layer=norm_layer,
-                  init_values=init_values) for i in range(depth)])
+        self.with_fp16 = with_fp16
+        self.blocks = _blocks(embed_dim, depth, num_heads, mlp_ratio, qkv_bias, qk_scale, drop_rate, attn_drop_rate,
+                              drop_path_rate, norm_layer, init_values, with_cp)
         self.norm = norm_layer(embed_dim)
         self.head = nn.Linear(embed_dim, num_classes) if num_classes > 0 else nn.Identity()
         self.apply(_xavier_init)
@@ -230,7 +143,7 @@ class PretrainVisionTransformerDecoder(nn.Module):
 
     def forward_rows(self, h, B, N, return_token_num):
         """h fp32 [B*N, C_d] -> bf16 [B, return_token_num (or N), num_classes]."""
-        h = _run_blocks(self.blocks, h, B, N, self.with_cp)
+        h = _run_blocks(self.blocks, h, B, N)
         C = h.shape[-1]
         h = h.reshape(B, N, C)
         if return_token_num > 0:

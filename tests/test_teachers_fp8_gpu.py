@@ -48,10 +48,9 @@ def _ivl_block():
 
 
 def _mae_block():
-    from internvideo_b200.modules import LayerNormB
-    from internvideo_b200.teachers import TeacherBlock
+    from internvideo_b200.modules import LayerNormB, VideoMAEBlock
     torch.manual_seed(1)
-    blk = TeacherBlock(1408, 16, 48 / 11, qkv_bias=True, norm_layer=lambda d: LayerNormB(d, eps=1e-6))
+    blk = VideoMAEBlock(1408, 16, 48 / 11, qkv_bias=True, norm_layer=lambda d: LayerNormB(d, eps=1e-6))
     assert blk.mlp.fc1.out_features == 6144
     with torch.no_grad():
         blk.attn.q_bias.normal_(0, 0.02); blk.attn.v_bias.normal_(0, 0.02)
@@ -79,20 +78,21 @@ def test_internvl_block_full_width(cuda_lib):
     assert r <= BRANCH_BOUND
 
 
-def test_videomae_block_full_width(cuda_lib):
+def test_shared_videomae_block_full_width(cuda_lib):
+    """The VideoMAE-g teacher's block (modules.VideoMAEBlock, head-axis attention) at full width under FP8 inference."""
     from internvideo_b200.modules import set_fp8_inference
     blk = _mae_block()
     B, n = 2, 2048
     x = torch.randn((B * n, 1408), device="cuda")
-    y0 = blk.forward_infer(x, B, n, True)
+    y0 = blk.forward_infer(x, B, n, head_axis=True)
     assert set_fp8_inference(blk) == 1
-    y1 = blk.forward_infer(x, B, n, True)
+    y1 = blk.forward_infer(x, B, n, head_axis=True)
     r = _rel(y1 - x, y0 - x)
     print(f"VideoMAE-g block (D 1408, n 2048, head-axis attention): branch rel. error {r:.4f}")
-    assert torch.equal(y1, blk.forward_infer(x, B, n, True))
+    assert torch.equal(y1, blk.forward_infer(x, B, n, head_axis=True))
     assert r <= BRANCH_BOUND
     set_fp8_inference(blk, False)
-    assert torch.equal(blk.forward_infer(x, B, n, True), y0)
+    assert torch.equal(blk.forward_infer(x, B, n, head_axis=True), y0)
 
 
 def _teachers():
