@@ -147,6 +147,29 @@ int ivb_fp8_quantize_rows(const void* x, long ldx, int M, int K, void* out, long
 int ivb_norm_fwd_fp8(const void* x, int x_is_f32, long ldx, const void* weight, const void* bias, float eps,
                      int is_layernorm, int M, int D, void* out, long ldo, float* row_scale_inv, void* stream);
 
+/* ---- FP8 training with per-token scales (opt-in per-token FP8 mode of the ViT block) ---------------------------
+ * Activations and gradients are cast row by row (ivb_fp8_quantize_rows, E4M3 for both), weights with one scale per
+ * output channel for the forward and one per input channel for the input-gradient GEMM; every scale follows the
+ * ivb_fp8_quantize_rows rule for its row or column.  Same bits on every run; capturable in a CUDA graph.  A call that
+ * breaks a rule below is refused before any CUDA call.
+ *
+ * ivb_norm_fwd_fp8_train: ivb_norm_fwd_fp8 (same operand rules, same out and row_scale_inv bits) that also writes, from
+ *   the same single read of each row, the bf16 row y [M, D] (pitch ldy, a multiple of 8; 16-byte aligned), rstd [M]
+ *   and, for LayerNorm, mean [M]: the bits ivb_norm_fwd writes.  y, rstd and (LayerNorm) mean are required; mean,
+ *   rstd and row_scale_inv are 4-byte aligned.  One stream-ordered kernel.
+ * ivb_fp8_quantize_cols_t: x bf16 [M, K] (pitch ldx, a multiple of 8; a weight [N_out, K_in]) -> out_t E4M3 [K, M]
+ *   = (x * col_scale)^T (pitch ldt, a multiple of 16 and >= M) and col_scale_inv fp32 [K], one power-of-two scale per
+ *   column of x from the column's amax (NaN when the column holds an Inf or NaN).  out_t is the B operand of the
+ *   input-gradient GEMM dx = dy W with IVB_FLAG_FP8_VECTOR_SCALES, col_scale_inv its per-output-channel vector.
+ *   col_amax fp32 [K] is the call's workspace (zeroed first; afterwards the columns' amax).  x and out_t are 16-byte
+ *   aligned, col_amax and col_scale_inv 4-byte.  Columns M .. ldt of out_t are not written.  Three stream-ordered
+ *   operations (a memset of col_amax and two kernels).                                                             */
+int ivb_norm_fwd_fp8_train(const void* x, int x_is_f32, long ldx, const void* weight, const void* bias, float eps,
+                           int is_layernorm, int M, int D, void* out, long ldo, float* row_scale_inv, void* y, long ldy,
+                           float* mean, float* rstd, void* stream);
+int ivb_fp8_quantize_cols_t(const void* x, long ldx, int M, int K, void* out_t, long ldt, float* col_amax,
+                            float* col_scale_inv, void* stream);
+
 /* ---- RMSNorm / LayerNorm (row reductions, HBM-bound) -------------------------------------------
  * y(bf16) = norm(x) * weight (+ bias).  is_layernorm=0: RMSNorm (internvideo2_pretrain.py:117-128,
  * FA2 DropoutAddRMSNorm :467; eps 1e-6); 1: nn.LayerNorm (eps 1e-5, :525,:532).

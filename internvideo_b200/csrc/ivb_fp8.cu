@@ -11,6 +11,10 @@
 //
 // ivb_fp8_quantize_rows applies the same rule to each row on its own (E4M3 only): a row's scale comes from the row's
 // amax, so a row's grid is never coarser than the whole tensor's, and the cast error of an element never larger.
+//
+// ivb_fp8_quantize_cols_t applies it to each column of a weight and writes the transposed copy (the input-gradient
+// GEMM's B operand, one scale per input channel): a column amax (integer atomicMax, order-independent), then the
+// cast kernel's 64 x 64 transposing tile with one scale per column.
 #include "ivb_fp8.cuh"
 #include "ivb_internal.h"
 #include "ivb_rows.cuh"
@@ -49,16 +53,17 @@ __global__ void __launch_bounds__(256) fp8_amax_kernel(const __nv_bfloat16* __re
 
 // One 64 x 64 tile per CTA: thread t converts 16 elements of row t / 4 and writes them to `out`; with out_t, the tile
 // is transposed through shared memory and thread t writes 16 elements of row t / 4 of out_t's tile.
-template <bool E5M2>
-__global__ void __launch_bounds__(Q_THREADS) fp8_cast_kernel(const __nv_bfloat16* __restrict__ x, long ldx, int M,
-                                                             int K, const unsigned* amax_bits, uint8_t* out, long ldo,
-                                                             uint8_t* out_t, long ldt, float* scale_inv) {
+// COLS (E4M3 only): one scale per column, from amax_bits[K] and written to scale_inv[K]; only out_t is written.
+template <bool E5M2, bool COLS>
+__device__ __forceinline__ void fp8_cast_tile(const __nv_bfloat16* __restrict__ x, long ldx, int M, int K,
+                                              const unsigned* amax_bits, uint8_t* out, long ldo, uint8_t* out_t,
+                                              long ldt, float* scale_inv) {
   __shared__ __align__(16) uint8_t tile[Q_TILE * Q_PITCH];
-  pdl_wait();
-  pdl_launch_dependents();
   float scale, sinv;
-  fp8_scale(*amax_bits, E5M2 ? 15 : 8, scale, sinv);
-  if (blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0) *scale_inv = sinv;
+  if constexpr (!COLS) {
+    fp8_scale(*amax_bits, E5M2 ? 15 : 8, scale, sinv);
+    if (blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0) *scale_inv = sinv;
+  }
   const int m0 = blockIdx.y * Q_TILE, k0 = blockIdx.x * Q_TILE;
   const int r = threadIdx.x >> 2, c = (threadIdx.x & 3) * 16;
   const int row = m0 + r, col = k0 + c;
@@ -76,17 +81,30 @@ __global__ void __launch_bounds__(Q_THREADS) fp8_cast_kernel(const __nv_bfloat16
       v[k] = k < nv ? __bfloat162float(x[static_cast<long>(row) * ldx + col + k]) : 0.0f;
   }
   uint32_t q[4];
+  if constexpr (COLS) {
+    const int nc = min(16, K - col);   // columns of this thread's segment inside the tensor
 #pragma unroll
-  for (int k = 0; k < 4; ++k)
-    q[k] = cvt_fp8x2<E5M2>(v[4 * k] * scale, v[4 * k + 1] * scale) |
-           (cvt_fp8x2<E5M2>(v[4 * k + 2] * scale, v[4 * k + 3] * scale) << 16);
-  uint8_t* dst = out + static_cast<long>(row) * ldo + col;
-  if (nv == 16) {
-    *reinterpret_cast<uint4*>(dst) = make_uint4(q[0], q[1], q[2], q[3]);
+    for (int k = 0; k < 16; ++k) {
+      fp8_scale(k < nc ? amax_bits[col + k] : 0u, 8, scale, sinv);
+      v[k] *= scale;
+      if (blockIdx.y == 0 && r == 0 && k < nc) scale_inv[col + k] = sinv;
+    }
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+      q[k] = cvt_fp8x2<false>(v[4 * k], v[4 * k + 1]) | (cvt_fp8x2<false>(v[4 * k + 2], v[4 * k + 3]) << 16);
   } else {
-    for (int k = 0; k < nv; ++k) dst[k] = static_cast<uint8_t>(q[k >> 2] >> (8 * (k & 3)));
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+      q[k] = cvt_fp8x2<E5M2>(v[4 * k] * scale, v[4 * k + 1] * scale) |
+             (cvt_fp8x2<E5M2>(v[4 * k + 2] * scale, v[4 * k + 3] * scale) << 16);
+    uint8_t* dst = out + static_cast<long>(row) * ldo + col;
+    if (nv == 16) {
+      *reinterpret_cast<uint4*>(dst) = make_uint4(q[0], q[1], q[2], q[3]);
+    } else {
+      for (int k = 0; k < nv; ++k) dst[k] = static_cast<uint8_t>(q[k >> 2] >> (8 * (k & 3)));
+    }
+    if (out_t == nullptr) return;
   }
-  if (out_t == nullptr) return;
 #pragma unroll
   for (int k = 0; k < 16; ++k) tile[(c + k) * Q_PITCH + r] = static_cast<uint8_t>(q[k >> 2] >> (8 * (k & 3)));
   __syncthreads();
@@ -102,6 +120,74 @@ __global__ void __launch_bounds__(Q_THREADS) fp8_cast_kernel(const __nv_bfloat16
     const uint32_t tw[4] = {t.x, t.y, t.z, t.w};
     for (int k = 0; k < tn; ++k) tdst[k] = static_cast<uint8_t>(tw[k >> 2] >> (8 * (k & 3)));
   }
+}
+
+template <bool E5M2>
+__global__ void __launch_bounds__(Q_THREADS) fp8_cast_kernel(const __nv_bfloat16* __restrict__ x, long ldx, int M,
+                                                             int K, const unsigned* amax_bits, uint8_t* out, long ldo,
+                                                             uint8_t* out_t, long ldt, float* scale_inv) {
+  pdl_wait();
+  pdl_launch_dependents();
+  fp8_cast_tile<E5M2, false>(x, ldx, M, K, amax_bits, out, ldo, out_t, ldt, scale_inv);
+}
+
+// ------------------------------------------------------------------ per-column scaling (ivb_fp8_quantize_cols_t)
+// The column amax of a 64-column strip over Q_COL_ROWS rows per CTA: thread t reads the 8-column chunk t % 8 of rows
+// t / 8, t / 8 + 32, ...; the 32 row lanes of a chunk are reduced by shuffles and shared memory, then one integer
+// atomicMax per column (order-independent: the same bits on every run).
+constexpr int Q_COL_ROWS = 256;
+
+__global__ void __launch_bounds__(Q_THREADS) fp8_col_amax_kernel(const __nv_bfloat16* __restrict__ x, long ldx, int M,
+                                                                 int K, unsigned* col_amax_bits) {
+  __shared__ unsigned red[Q_THREADS / 32][Q_TILE];
+  pdl_wait();
+  pdl_launch_dependents();
+  const int c = blockIdx.x * Q_TILE + (threadIdx.x & 7) * 8;
+  const int r1 = min(M, (blockIdx.y + 1) * Q_COL_ROWS);
+  unsigned m[8] = {0u, 0u, 0u, 0u, 0u, 0u, 0u, 0u};   // bf16 magnitude bits: NaN > Inf > every finite value
+  if (c < K) {
+    for (int row = blockIdx.y * Q_COL_ROWS + (threadIdx.x >> 3); row < r1; row += Q_THREADS / 8) {
+      const __nv_bfloat16* src = x + static_cast<long>(row) * ldx + c;
+      if (c + 8 <= K) {
+        const uint4 v = *reinterpret_cast<const uint4*>(src);
+        const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          m[2 * k] = max(m[2 * k], w[k] & 0x7fffu);
+          m[2 * k + 1] = max(m[2 * k + 1], (w[k] >> 16) & 0x7fffu);
+        }
+      } else {
+        const uint16_t* s16 = reinterpret_cast<const uint16_t*>(src);
+        for (int k = 0; k < K - c; ++k) m[k] = max(m[k], static_cast<unsigned>(s16[k]) & 0x7fffu);
+      }
+    }
+  }
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {   // lanes l, l ^ 8, l ^ 16, l ^ 24 hold the same chunk
+    m[k] = max(m[k], __shfl_xor_sync(0xffffffffu, m[k], 8));
+    m[k] = max(m[k], __shfl_xor_sync(0xffffffffu, m[k], 16));
+  }
+  const int lane = threadIdx.x & 31;
+  if (lane < 8) {
+#pragma unroll
+    for (int k = 0; k < 8; ++k) red[threadIdx.x >> 5][lane * 8 + k] = m[k];
+  }
+  __syncthreads();
+  if (threadIdx.x < Q_TILE) {
+    unsigned mx = 0;
+#pragma unroll
+    for (int w = 0; w < Q_THREADS / 32; ++w) mx = max(mx, red[w][threadIdx.x]);
+    const int col = blockIdx.x * Q_TILE + threadIdx.x;
+    if (col < K && mx != 0) atomicMax(col_amax_bits + col, mx << 16);
+  }
+}
+
+__global__ void __launch_bounds__(Q_THREADS) fp8_cast_cols_kernel(const __nv_bfloat16* __restrict__ x, long ldx, int M,
+                                                                  int K, const unsigned* col_amax_bits, uint8_t* out_t,
+                                                                  long ldt, float* col_scale_inv) {
+  pdl_wait();
+  pdl_launch_dependents();
+  fp8_cast_tile<false, true>(x, ldx, M, K, col_amax_bits, nullptr, 0, out_t, ldt, col_scale_inv);
 }
 
 // ------------------------------------------------------------------ per-row scaling (ivb_fp8_quantize_rows)
@@ -189,6 +275,29 @@ extern "C" int ivb_fp8_quantize_rows(const void* x, long ldx, int M, int K, void
                   : chunks <= R_THREADS * 4 ? fp8_rows_kernel<4>
                   : chunks <= R_THREADS * 8 ? fp8_rows_kernel<8> : fp8_rows_kernel<16>;
   return launch("fp8_rows_kernel", kern, M, R_THREADS, 0, stream, ALLOW_PDL, xb, ldx, K, o, ldo, row_scale_inv);
+}
+
+extern "C" int ivb_fp8_quantize_cols_t(const void* x, long ldx, int M, int K, void* out_t, long ldt, float* col_amax,
+                                       float* col_scale_inv, void* stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  if (M <= 0 || K <= 0) return set_error("ivb_fp8_quantize_cols_t: empty tensor");
+  if (x == nullptr || out_t == nullptr || col_amax == nullptr || col_scale_inv == nullptr)
+    return set_error("ivb_fp8_quantize_cols_t: x, out_t, col_amax or col_scale_inv is null");
+  if ((ldx & 7) || ldx < K) return set_error("ivb_fp8_quantize_cols_t: ldx must be a multiple of 8 elements and >= K");
+  if ((ldt & 15) || ldt < M) return set_error("ivb_fp8_quantize_cols_t: ldt must be a multiple of 16 elements and >= M");
+  if (misaligned(16, x, out_t)) return set_error("ivb_fp8_quantize_cols_t: x and out_t must be 16-byte aligned");
+  if (misaligned(4, col_amax, col_scale_inv))
+    return set_error("ivb_fp8_quantize_cols_t: col_amax and col_scale_inv must be 4-byte aligned");
+  cudaError_t e = cudaMemsetAsync(col_amax, 0, sizeof(float) * static_cast<size_t>(K), stream);
+  if (e != cudaSuccess) return set_error_cuda("ivb_fp8_quantize_cols_t: cudaMemsetAsync", e);
+  const auto* xb = reinterpret_cast<const __nv_bfloat16*>(x);
+  unsigned* bits = reinterpret_cast<unsigned*>(col_amax);
+  const unsigned strips = (K + Q_TILE - 1) / Q_TILE;
+  if (int rc = launch("fp8_col_amax_kernel", fp8_col_amax_kernel, dim3(strips, (M + Q_COL_ROWS - 1) / Q_COL_ROWS),
+                      Q_THREADS, 0, stream, ALLOW_PDL, xb, ldx, M, K, bits))
+    return rc;
+  return launch("fp8_cast_cols_kernel", fp8_cast_cols_kernel, dim3(strips, (M + Q_TILE - 1) / Q_TILE), Q_THREADS, 0,
+                stream, ALLOW_PDL, xb, ldx, M, K, bits, reinterpret_cast<uint8_t*>(out_t), ldt, col_scale_inv);
 }
 
 extern "C" int ivb_fp8_quantize(const void* x, long ldx, int M, int K, int format, void* out, long ldo, void* out_t,

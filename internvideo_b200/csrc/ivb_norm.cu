@@ -311,13 +311,14 @@ rms_fwd_reg_kernel(const void* __restrict__ x, long ldx, const __nv_bfloat16* __
 // (one HBM read), so the row's amax, and with it the row's power-of-two scale (fp8_scale), is known before the first
 // byte is stored.  The statistics and y = (x - mean) * rstd * w (+ b) are the fp32 expressions of norm_fwd_kernel
 // (LayerNorm) and rms_fwd_reg_kernel (RMSNorm), so y is the value ivb_norm_fwd rounds to bf16.
-template <bool XF32, bool LN, int NCH>
-__global__ void __launch_bounds__(256)
-norm_fwd_fp8_kernel(const void* __restrict__ x, long ldx, const __nv_bfloat16* __restrict__ w,
-                    const __nv_bfloat16* __restrict__ b, float eps, int M, int D, uint8_t* __restrict__ out, long ldo,
-                    float* __restrict__ scale_inv) {
-  pdl_wait();
-  pdl_launch_dependents();
+// TRAIN (FP8 training with per-token scales): the same registers also give the bf16 row y and the statistics, the bits
+// ivb_norm_fwd writes, for the backward (the weight gradient reads the bf16 row, the norm backward mean and rstd).
+template <bool XF32, bool LN, int NCH, bool TRAIN>
+__device__ __forceinline__ void norm_fwd_fp8_rows(const void* __restrict__ x, long ldx, const __nv_bfloat16* __restrict__ w,
+                                                  const __nv_bfloat16* __restrict__ b, float eps, int M, int D,
+                                                  uint8_t* __restrict__ out, long ldo, float* __restrict__ scale_inv,
+                                                  __nv_bfloat16* __restrict__ y, long ldy, float* __restrict__ mean_out,
+                                                  float* __restrict__ rstd_out) {
   const int lane = threadIdx.x & 31;
   const int wpb = blockDim.x >> 5;
   const int nch = D >> 3;
@@ -371,10 +372,40 @@ norm_fwd_fp8_kernel(const void* __restrict__ x, long ldx, const __nv_bfloat16* _
 #pragma unroll
     for (int i = 0; i < NCH; ++i) {
       const int c = lane + 32 * i;
-      if (c < nch) *reinterpret_cast<uint2*>(out + row * ldo + c * 8) = cvt_e4m3x8(v[i], scale);
+      if (c < nch) {
+        *reinterpret_cast<uint2*>(out + row * ldo + c * 8) = cvt_e4m3x8(v[i], scale);
+        if constexpr (TRAIN) store8<false>(y, row * ldy + c * 8, v[i]);
+      }
     }
-    if (lane == 0) scale_inv[row] = sinv;
+    if (lane == 0) {
+      scale_inv[row] = sinv;
+      if constexpr (TRAIN) {
+        rstd_out[row] = rstd;
+        if (LN) mean_out[row] = mean;
+      }
+    }
   }
+}
+
+template <bool XF32, bool LN, int NCH>
+__global__ void __launch_bounds__(256)
+norm_fwd_fp8_kernel(const void* __restrict__ x, long ldx, const __nv_bfloat16* __restrict__ w,
+                    const __nv_bfloat16* __restrict__ b, float eps, int M, int D, uint8_t* __restrict__ out, long ldo,
+                    float* __restrict__ scale_inv) {
+  pdl_wait();
+  pdl_launch_dependents();
+  norm_fwd_fp8_rows<XF32, LN, NCH, false>(x, ldx, w, b, eps, M, D, out, ldo, scale_inv, nullptr, 0, nullptr, nullptr);
+}
+
+template <bool XF32, bool LN, int NCH>
+__global__ void __launch_bounds__(256)
+norm_fwd_fp8_train_kernel(const void* __restrict__ x, long ldx, const __nv_bfloat16* __restrict__ w,
+                          const __nv_bfloat16* __restrict__ b, float eps, int M, int D, uint8_t* __restrict__ out,
+                          long ldo, float* __restrict__ scale_inv, __nv_bfloat16* __restrict__ y, long ldy,
+                          float* __restrict__ mean_out, float* __restrict__ rstd_out) {
+  pdl_wait();
+  pdl_launch_dependents();
+  norm_fwd_fp8_rows<XF32, LN, NCH, true>(x, ldx, w, b, eps, M, D, out, ldo, scale_inv, y, ldy, mean_out, rstd_out);
 }
 
 // dynamic smem: colred rows [warps][1][D] (only when dweight != nullptr)
@@ -709,6 +740,41 @@ extern "C" int ivb_norm_fwd_fp8(const void* x, int x_is_f32, long ldx, const voi
       auto go = [&](auto nch) {
         return launch("norm_fwd_fp8_kernel", norm_fwd_fp8_kernel<xf, ln, nch>, blocks, 256, 0, stream, ALLOW_PDL, x, ldx,
                       w, b, eps, M, D, o, ldo, row_scale_inv);
+      };
+      if (D > 1536) return go(std::integral_constant<int, 16>{});
+      return pick_nch(D, go);
+    });
+  });
+}
+
+extern "C" int ivb_norm_fwd_fp8_train(const void* x, int x_is_f32, long ldx, const void* weight, const void* bias,
+                                      float eps, int is_layernorm, int M, int D, void* out, long ldo,
+                                      float* row_scale_inv, void* y, long ldy, float* mean, float* rstd,
+                                      void* stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  if (M <= 0) return set_error("ivb_norm_fwd_fp8_train: empty tensor");
+  if (D <= 0 || D > IVB_NORM_FP8_MAX_D || (D & 7))
+    return set_error("ivb_norm_fwd_fp8_train: D must be a multiple of 8 in [8, IVB_NORM_FP8_MAX_D]");
+  if ((ldx & 7) || ldx < D) return set_error("ivb_norm_fwd_fp8_train: ldx must be a multiple of 8 elements and >= D");
+  if ((ldo & 15) || ldo < D) return set_error("ivb_norm_fwd_fp8_train: ldo must be a multiple of 16 elements and >= D");
+  if ((ldy & 7) || ldy < D) return set_error("ivb_norm_fwd_fp8_train: ldy must be a multiple of 8 elements and >= D");
+  if (x == nullptr || weight == nullptr || out == nullptr || row_scale_inv == nullptr || y == nullptr ||
+      rstd == nullptr || (is_layernorm && mean == nullptr))
+    return set_error("ivb_norm_fwd_fp8_train: x, weight, out, row_scale_inv, y, rstd or (LayerNorm) mean is null");
+  if (misaligned(16, x, weight, bias, out, y))
+    return set_error("ivb_norm_fwd_fp8_train: x, weight, bias, out and y must be 16-byte aligned");
+  if (misaligned(4, row_scale_inv, mean, rstd))
+    return set_error("ivb_norm_fwd_fp8_train: row_scale_inv, mean and rstd must be 4-byte aligned");
+  const __nv_bfloat16* w = reinterpret_cast<const __nv_bfloat16*>(weight);
+  const __nv_bfloat16* b = reinterpret_cast<const __nv_bfloat16*>(bias);
+  uint8_t* o = reinterpret_cast<uint8_t*>(out);
+  __nv_bfloat16* yo = reinterpret_cast<__nv_bfloat16*>(y);
+  const int blocks = persistent_grid(M, 8, 8);
+  return pick_bool(x_is_f32, [&](auto xf) {
+    return pick_bool(is_layernorm, [&](auto ln) {
+      auto go = [&](auto nch) {
+        return launch("norm_fwd_fp8_train_kernel", norm_fwd_fp8_train_kernel<xf, ln, nch>, blocks, 256, 0, stream,
+                      ALLOW_PDL, x, ldx, w, b, eps, M, D, o, ldo, row_scale_inv, yo, ldy, mean, rstd);
       };
       if (D > 1536) return go(std::integral_constant<int, 16>{});
       return pick_nch(D, go);

@@ -207,33 +207,54 @@ def fp8_quantize(x, fmt=FP8_E4M3, transpose=False):
     return q, q_t, scale_inv, amax
 
 
-def fp8_quantize_rows(x):
+def fp8_quantize_rows(x, transposed=False):
     """Per-row current-scaling cast of a bf16 [M, K] tensor (any row pitch) to E4M3 (ivb_fp8_quantize_rows).
 
     Returns (q [M, K], row_scale_inv fp32 [M]): x[m] ~ q[m] * row_scale_inv[m], each row with its own power-of-two
     scale.  A weight [N, K] quantised this way has one scale per output channel.  q is a view of a buffer whose row
-    pitch is rounded up to 16 elements (the fp8 GEMM's operand rule)."""
+    pitch is rounded up to 16 elements (the fp8 GEMM's operand rule).
+
+    transposed=True casts the rows of x^T instead, reading x once (ivb_fp8_quantize_cols_t): (q_t [K, M], col_scale_inv
+    fp32 [K]) with x[:, k] ~ q_t[k] * col_scale_inv[k].  For a weight [N, K] that is the B operand of the input-gradient
+    GEMM dx = dy W, with one scale per input channel of the weight."""
     _chk(("x", x, bf16))
     ldx = _rows2d(x, "x")
     M, K = x.shape
+    if transposed:
+        q_t = torch.empty((K, _pad16(M)), device=x.device, dtype=torch.float8_e4m3fn)[:, :M]
+        amax = torch.empty((K,), device=x.device, dtype=f32)
+        sinv = torch.empty((K,), device=x.device, dtype=f32)
+        _call("fp8_quantize_cols_t", x, ldx, M, K, q_t, q_t.stride(0), amax, sinv, kind="fp8_quantize")
+        return q_t, sinv
     q = torch.empty((M, _pad16(K)), device=x.device, dtype=torch.float8_e4m3fn)[:, :K]
     sinv = torch.empty((M,), device=x.device, dtype=f32)
     _call("fp8_quantize_rows", x, ldx, M, K, q, q.stride(0), sinv, kind="fp8_quantize")
     return q, sinv
 
 
-def norm_fwd_fp8(x, weight, bias=None, eps=1e-6, layernorm=False):
+def norm_fwd_fp8(x, weight, bias=None, eps=1e-6, layernorm=False, save=False):
     """RMSNorm / LayerNorm of x [M, D] (fp32 or bf16, any row pitch) written only as E4M3 rows with per-row scales
     (ivb_norm_fwd_fp8).  Returns (q [M, D] float8_e4m3fn, row_scale_inv fp32 [M]): q[m] * row_scale_inv[m] is the
-    row norm_fwd would round to bf16, rounded to E4M3 instead."""
+    row norm_fwd would round to bf16, rounded to E4M3 instead.
+
+    save=True also writes what a backward needs, from the same read of each row (ivb_norm_fwd_fp8_train), and returns
+    (q, row_scale_inv, y, mean | None, rstd): q and row_scale_inv the same bits, y (bf16 [M, D]), mean (LayerNorm only)
+    and rstd norm_fwd's bits."""
     _chk(("x", x, (f32, bf16)), ("weight", weight, bf16), ("bias?", bias, bf16))
     ldx = _rows2d(x, "x")
     M, D = x.shape
     q = torch.empty((M, _pad16(D)), device=x.device, dtype=torch.float8_e4m3fn)[:, :D]
     sinv = torch.empty((M,), device=x.device, dtype=f32)
-    _call("norm_fwd_fp8", x, int(x.dtype == f32), ldx, weight, bias, float(eps), int(layernorm), M, D, q, q.stride(0),
-          sinv)
-    return q, sinv
+    if not save:
+        _call("norm_fwd_fp8", x, int(x.dtype == f32), ldx, weight, bias, float(eps), int(layernorm), M, D, q,
+              q.stride(0), sinv)
+        return q, sinv
+    y = torch.empty((M, D), device=x.device, dtype=bf16)
+    rstd = torch.empty((M,), device=x.device, dtype=f32)
+    mean = torch.empty((M,), device=x.device, dtype=f32) if layernorm else None
+    _call("norm_fwd_fp8_train", x, int(x.dtype == f32), ldx, weight, bias, float(eps), int(layernorm), M, D, q,
+          q.stride(0), sinv, y, y.stride(0), mean, rstd, kind="norm_fwd_fp8")
+    return q, sinv, y, mean, rstd
 
 
 def gemm_fp8(a, a_scale_inv, b, b_scale_inv, *, epi=EPI_BF16, flags=0, out0=None, out1=None, bias=None, gamma=None,

@@ -276,8 +276,10 @@ class Block(nn.Module):
         self.with_cp = bool(with_cp)
         self.use_fused_rmsnorm = use_fused_rmsnorm
         self.num_heads = num_heads
-        # FP8 GEMMs for the forward and input-gradient passes (set_fp8); read at call time
+        # FP8 GEMMs for the forward and input-gradient passes (set_fp8) and their scaling, "tensor" or "token"; read at
+        # call time
         self.fp8 = False
+        self.fp8_scaling = "tensor"
         # FP8 inference with per-channel weight copies (set_fp8_inference); None when off
         self.fp8_inference = None
 
@@ -427,18 +429,27 @@ class VideoMAEBlock(nn.Module):
         return self.forward_stream(x.reshape(B * n, D).float().contiguous(), B, n).reshape(B, n, D)
 
 
-def set_fp8(model: nn.Module, enabled: bool = True) -> int:
+FP8_SCALINGS = {"tensor": ops.FP8_TENSOR, "token": ops.FP8_TOKEN}
+
+
+def set_fp8(model: nn.Module, enabled: bool = True, scaling: str = "tensor") -> int:
     """Switch the FP8 mode of every ViT Block in `model` (stage-1 student, CLIP tower, stage-2 tower, InternVL teacher)
     on or off; returns how many blocks were switched.
 
     In FP8 mode a block runs its forward GEMMs (qkv, proj, fc1, fc2) and its input-gradient GEMMs on the FP8 tensor
-    cores: activations and weights in E4M3, gradients in E5M2, each tensor with a power-of-two scale from its own amax
-    (no state, nothing in the state_dict).  Weight gradients, attention, norms and everything outside the blocks stay
-    bf16.  The mode is read when a block runs: switch it before capturing a CUDA graph of the step."""
+    cores, every scale a power of two from the amax of what it scales (no state, nothing in the state_dict).
+    scaling="tensor": activations and weights in E4M3, gradients in E5M2, one scale per tensor.  scaling="token":
+    activations and gradients in E4M3 with one scale per row (token), cast in one pass over each row (n1 and n2 inside
+    the norm kernel), and the weights in E4M3 with one scale per output channel for the forward and per input channel
+    for the input-gradient GEMMs.  Weight gradients, attention, norms and everything outside the blocks stay bf16.  The
+    mode is read when a block runs: switch it before capturing a CUDA graph of the step."""
+    if scaling not in FP8_SCALINGS:
+        raise ValueError(f"set_fp8: scaling must be one of {sorted(FP8_SCALINGS)}, got {scaling!r}")
     n = 0
     for mod in model.modules():
         if isinstance(mod, Block):
             mod.fp8 = bool(enabled)
+            mod.fp8_scaling = scaling
             n += 1
     return n
 
@@ -470,7 +481,7 @@ def block_precision(block, training=False):
     set_fp8 (Block.fp8) and set_fp8_inference (fp8_inference).  training: the forward needs a gradient."""
     fp8 = getattr(block, "fp8", False)
     if block.fp8_inference is None:
-        return ops.FP8_TENSOR if fp8 else ops.BF16
+        return FP8_SCALINGS[block.fp8_scaling] if fp8 else ops.BF16
     if training:
         raise ll._lib.IvbError("Block: FP8 inference mode (set_fp8_inference) has no gradient; switch it off to train")
     if fp8:

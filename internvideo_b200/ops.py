@@ -187,9 +187,10 @@ class PoolAttnFn(torch.autograd.Function):
 
 # ------------------------------------------------------------------------------------------ fused ViT block
 # A block's precision (BlockSpec.precision): BF16; FP8_TENSOR, FP8 with per-tensor scales and the weights cast in the
-# call (modules.set_fp8); or per-token FP8 (modules.set_fp8_inference, no-grad calls only), given as the four weights'
-# per-channel E4M3 copies themselves: ((q, scale_inv) for qkv, proj, fc1, fc2).
-BF16, FP8_TENSOR = "bf16", "fp8"
+# call (modules.set_fp8); FP8_TOKEN, FP8 with per-token scales and the weights cast per channel in the call
+# (modules.set_fp8 with scaling="token"); or per-token FP8 inference (modules.set_fp8_inference, no-grad calls only),
+# given as the four weights' per-channel E4M3 copies themselves: ((q, scale_inv) for qkv, proj, fc1, fc2).
+BF16, FP8_TENSOR, FP8_TOKEN = "bf16", "fp8", "fp8_token"
 
 
 class BlockSpec(NamedTuple):
@@ -223,8 +224,8 @@ BlockParams = namedtuple("BlockParams", "n1w qkvw qkvb qnw knw projw projb g1 n2
                          defaults=(None, None))
 
 # What block_forward(save=True) keeps for block_backward: activations and norm statistics (mean1 / mean2 None on RMSNorm
-# blocks), and in FP8_TENSOR the E4M3 copies of the four weights' transposes with their scales (the input-gradient
-# GEMMs' operands; None in bf16).
+# blocks), and in FP8 the E4M3 copies of the four weights' transposes with their scales (the input-gradient GEMMs'
+# operands; per-tensor scalars in FP8_TENSOR, one scale per input channel in FP8_TOKEN; None in bf16).
 BlockSaved = namedtuple("BlockSaved", "n1 qkv qkn a lse mean1 rstd1 rq rk x1 y1 n2 mean2 rstd2 h g y2 "
                                       "qkvw_t qkvw_s projw_t projw_s fc1w_t fc1w_s fc2w_t fc2w_s")
 
@@ -244,38 +245,47 @@ def block_forward(x, spec, p, rs1=None, rs2=None, save=True):
 
     FP8_TENSOR (8 more calls): the four weights are cast to E4M3 (with save, also transposed, for the backward's dgrad)
     and n1, a, n2 and g before their GEMM, each with its own per-tensor scale; the GEMMs keep their fused epilogues.
-    Per-token FP8 (save=False only; 2 more calls): n1 and n2 come out of the norm kernel as E4M3 rows with per-row
-    scales, a and g are cast row by row, and the four GEMMs apply row and column scales before their fused epilogues.
-    Attention, the q/k norms and the residual stream stay as above."""
+    Per-token FP8 (FP8_TOKEN, or the inference weight copies; 2 more calls): n1 and n2 come out of the norm kernel as
+    E4M3 rows with per-row scales, a and g are cast row by row, and the four GEMMs apply row and column scales before
+    their fused epilogues.  FP8_TOKEN also casts the four weights per output channel (4 calls) and, with save, per input
+    channel into their transposed copies (4 more), and its norm kernel then also writes the bf16 row and statistics
+    the backward needs (without save: the same E4M3 bits from the inference norm kernel).  Attention, the q/k norms and
+    the residual stream stay as above."""
     B, n, H = spec.B, spec.n, spec.H
     M, D = x.shape
     d = D // H
     if x.dtype != f32 or not x.is_cuda:
         raise ll._lib.IvbError("block_forward: residual stream must be a CUDA fp32 tensor [B*n, D]")
     prec = spec.precision
-    per_token = not isinstance(prec, str)
-    w8 = None
+    per_token = prec == FP8_TOKEN or not isinstance(prec, str)
+    weights = (p.qkvw, p.projw, p.fc1w, p.fc2w)
+    # (q, scale_inv, q_t, scale_inv of q_t) per weight; q_t only when the backward will need it
     if prec == FP8_TENSOR:
-        # (q, q_t, scale_inv) per weight; q_t only when the backward will need it
-        w8 = [ll.fp8_quantize(w, ll.FP8_E4M3, transpose=save)[:3] for w in (p.qkvw, p.projw, p.fc1w, p.fc2w)]
+        w8 = [(q, s, q_t, s) for q, q_t, s, _ in (ll.fp8_quantize(w, ll.FP8_E4M3, transpose=save) for w in weights)]
+    elif prec == FP8_TOKEN:
+        w8 = [(*ll.fp8_quantize_rows(w), *(ll.fp8_quantize_rows(w, transposed=True) if save else (None, None))) for w in weights]
+    elif per_token:
+        w8 = [(q, s, None, None) for q, s in prec]
 
-    def norm(t, w, b, eps):   # n1, n2 (and mean, rstd for the backward)
-        if per_token:
-            return ll.norm_fwd_fp8(t, w, b, eps=eps, layernorm=spec.layernorm), None, None
-        return ll.norm_fwd(t, w, b, eps=eps, layernorm=spec.layernorm, want_stats=save)
+    def norm(t, w, b, eps):   # (n1 or n2 as its GEMM reads it, the bf16 row the backward reads, mean, rstd)
+        if not per_token:
+            y, mean, rstd = ll.norm_fwd(t, w, b, eps=eps, layernorm=spec.layernorm, want_stats=save)
+            return y, y, mean, rstd
+        if not save:
+            return ll.norm_fwd_fp8(t, w, b, eps=eps, layernorm=spec.layernorm), None, None, None
+        q, s, y, mean, rstd = ll.norm_fwd_fp8(t, w, b, eps=eps, layernorm=spec.layernorm, save=True)
+        return (q, s), y, mean, rstd
 
     def linear(act, i, w, **epilogue):
         if prec == BF16:
             return ll.gemm(act, w, **epilogue)
-        if per_token:     # act: bf16, or the (E4M3 rows, scale_inv) pair norm_fwd_fp8 wrote
+        if per_token:     # act: bf16, or the (E4M3 rows, scale_inv) pair the norm wrote
             q, s = ll.fp8_quantize_rows(act) if torch.is_tensor(act) else act
-            wq, ws = prec[i]
         else:
             q, _, s, _ = ll.fp8_quantize(act, ll.FP8_E4M3)
-            wq, _, ws = w8[i]
-        return ll.gemm_fp8(q, s, wq, ws, **epilogue)
-    n1, mean1, rstd1 = norm(x, p.n1w, p.n1b, spec.eps1)
-    qkv = linear(n1, 0, p.qkvw, bias=p.qkvb)
+        return ll.gemm_fp8(q, s, w8[i][0], w8[i][1], **epilogue)
+    n1_in, n1, mean1, rstd1 = norm(x, p.n1w, p.n1b, spec.eps1)
+    qkv = linear(n1_in, 0, p.qkvw, bias=p.qkvb)
     q, k, v = qkv[:, :D], qkv[:, D:2 * D], qkv[:, 2 * D:]
     qkn = rq = rk = lse = None
     if p.qnw is not None:
@@ -294,21 +304,22 @@ def block_forward(x, spec, p, rs1=None, rs2=None, save=True):
         a, lse = ll.attn_fwd(q, k, v, B, n, H, d, spec.attn_scale(d), want_lse=save)
     y1 = torch.empty((M, D), device=x.device, dtype=bf16) if (p.g1 is not None and save) else None
     x1 = linear(a, 1, p.projw, epi=ll.EPI_RESID, bias=p.projb, gamma=p.g1, aux=x, out1=y1, rowscale=rs1)
-    n2, mean2, rstd2 = norm(x1, p.n2w, p.n2b, spec.eps2)
+    n2_in, n2, mean2, rstd2 = norm(x1, p.n2w, p.n2b, spec.eps2)
     h = torch.empty((M, p.fc1w.shape[0]), device=x.device, dtype=bf16) if save else None
-    g = linear(n2, 2, p.fc1w, epi=ll.EPI_BIAS_GELU, flags=spec.gelu_flags(save), bias=p.fc1b, out1=h)
+    g = linear(n2_in, 2, p.fc1w, epi=ll.EPI_BIAS_GELU, flags=spec.gelu_flags(save), bias=p.fc1b, out1=h)
     y2 = torch.empty((M, D), device=x.device, dtype=bf16) if (p.g2 is not None and save) else None
     x2 = linear(g, 3, p.fc2w, epi=ll.EPI_RESID, bias=p.fc2b, gamma=p.g2, aux=x1, out1=y2, rowscale=rs2)
     if not save:
         return x2, None
-    wt8 = [t for _, q_t, s in w8 for t in (q_t, s)] if w8 is not None else [None] * 8
+    wt8 = [t for _, _, q_t, s_t in w8 for t in (q_t, s_t)] if prec != BF16 else [None] * 8
     return x2, BlockSaved(n1, qkv, qkn, a, lse, mean1, rstd1, rq, rk, x1, y1, n2, mean2, rstd2, h, g, y2, *wt8)
 
 
 def block_backward(x, s, spec, t, P, dx2, rs1, rs2):
     """Backward of block_forward(save=True), from its BlockSaved s: 13 to 17 library calls in bf16 (with or without the
-    q/k norms and the qkv bias, the fused RMSNorm norm2 + LayerScale backward), and in FP8_TENSOR one more per
-    input-gradient GEMM (the E5M2 cast of its gradient).  The LayerNorm block (spec.layernorm) also returns its norms'
+    q/k norms and the qkv bias, the fused RMSNorm norm2 + LayerScale backward), and in FP8 one more per input-gradient
+    GEMM (the cast of its gradient: E5M2 with a per-tensor scale in FP8_TENSOR, E4M3 rows with per-row scales in
+    FP8_TOKEN).  The LayerNorm block (spec.layernorm) also returns its norms'
     bias gradients and always runs the attention branch's LayerScale backward as its own call.  `t` are the block's
     tensors as autograd handed them back, `P` the nn.Parameter objects (gradient sink), both BlockParams.  Returns
     (dx0, BlockParams of gradients | None when the sink took them)."""
@@ -333,10 +344,13 @@ def block_backward(x, s, spec, t, P, dx2, rs1, rs2):
         sink = None           # small parameters not contiguous in the flat buffer: autograd path
     dg2, dcs2, dn2w, dg1, dcs1 = seg["g2"], seg["fc2b"], seg["n2w"], seg["g1"], seg["projb"]
 
-    def dgrad(dy, w, w_t, w_s, **epilogue):   # dx = dy W; in FP8_TENSOR on the E5M2 gradient and the E4M3 copy of W^T
-        if spec.precision != FP8_TENSOR:
+    def dgrad(dy, w, w_t, w_s, **epilogue):   # dx = dy W; in FP8 on the cast gradient and the E4M3 copy of W^T
+        if spec.precision == FP8_TOKEN:
+            q, sc = ll.fp8_quantize_rows(dy)
+        elif spec.precision == FP8_TENSOR:
+            q, _, sc, _ = ll.fp8_quantize(dy, ll.FP8_E5M2)
+        else:
             return ll.gemm(dy, w, b_t=True, **epilogue)
-        q, _, sc, _ = ll.fp8_quantize(dy, ll.FP8_E5M2)
         return ll.gemm_fp8(q, sc, w_t, w_s, **epilogue)
 
     def wgrad(dy, act, param):

@@ -100,7 +100,8 @@ def quant_table(iters):
           f"{tot_b / HBM * 1e3:.3f} ms)")
 
 
-def step_table(reps=3, steps=10):
+def step_table(reps=3, steps=10, modes=("off", "tensor")):
+    """modes: "off" (bf16) or a set_fp8 scaling, each captured and timed once per repetition, in turn."""
     import bench
     from internvideo_b200.engine import GraphedStep, PretrainEngine
     from internvideo_b200.modules import PretrainInternVideo2, set_fp8
@@ -135,10 +136,10 @@ def step_table(reps=3, steps=10):
         engine.step()
         return loss
 
-    res = {False: [], True: []}
+    res = {mode: [] for mode in modes}
     for _ in range(reps):
-        for fp8 in (False, True):
-            set_fp8(model, fp8)
+        for fp8 in modes:
+            set_fp8(model, fp8 != "off", scaling="tensor" if fp8 == "off" else fp8)
             gs = GraphedStep(step, [video, mask], warmup=1)
             gs(video, mask)
             torch.cuda.synchronize()
@@ -148,12 +149,12 @@ def step_table(reps=3, steps=10):
             torch.cuda.synchronize()
             ms = (time.perf_counter() - t0) * 1e3 / steps
             res[fp8].append(ms)
-            print(f"  fp8={int(fp8)}  {ms:8.2f} ms/step  {B / ms * 1e3:7.2f} clips/s  loss {float(loss):.4f}")
+            print(f"  fp8={fp8:6s}  {ms:8.2f} ms/step  {B / ms * 1e3:7.2f} clips/s  loss {float(loss):.4f}")
             del gs
             torch.cuda.empty_cache()
-    for fp8 in (False, True):
+    for fp8 in modes:
         best = min(res[fp8])
-        print(f"fp8={int(fp8)}: best {best:.2f} ms/step = {B / best * 1e3:.2f} clips/s "
+        print(f"fp8={fp8}: best {best:.2f} ms/step = {B / best * 1e3:.2f} clips/s "
               f"(all: {', '.join(f'{x:.2f}' for x in res[fp8])})")
 
 
