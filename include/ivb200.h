@@ -88,6 +88,32 @@ int ivb_gemm_bf16(const void* A, int a_mn_major, long lda, const void* B, int b_
                   long ld1, const void* bias, const void* gamma, const void* aux, long ldaux,
                   const float* rowscale, int tile_n, void* stream);
 
+/* ---- DropPath plans (stochastic depth: skip the work of the rows a draw drops) ----------------------------------
+ * ivb_droppath_plan: for each of `branches` rows b of DropPath factors rowscale [branches, M] (pitch ld_rs >= M; the
+ * EPI_RESID rowscale of one block branch each), writes the int32 plan [b, 0 .. ivb_droppath_plan_ints(M)) (pitch
+ * ld_plan): a row is live when its factor is not 0, a 128-row tile or 64-row k-block when one of its rows is.
+ *   plan[0 .. nm)               the nm = ceil(M/128) row tiles: the live ones ascending, then the dead ones ascending
+ *   plan[nm]                    the number of live row tiles                         (plan + 0: the M plan)
+ *   plan[nm+1 .. nm+1+c)        the c live k-blocks of the nk = ceil(M/64), ascending
+ *   plan[nm+1+nk]               c                                                    (plan + nm + 1: the K plan)
+ * One stream-ordered kernel; nothing is read by the host, so it is capturable in a CUDA graph.
+ * ivb_gemm_bf16_plan: ivb_gemm_bf16 with an M plan over its M rows and / or a K plan over its K (either may be NULL:
+ * ivb_gemm_bf16 itself).  The results are those of ivb_gemm_bf16 wherever a plan's dead rows hold DropPath factor 0:
+ *   M plan: a dead row tile runs no MMA.  Its rows get IVB_EPI_RESID out0 = aux (with rowscale 0 the sum is the
+ *     residual itself) and out1 = 0; every other epilogue writes 0 (IVB_EPI_GELU_BWD does not read aux).  Live tiles are
+ *     computed as ivb_gemm_bf16 computes them.  Not with IVB_FLAG_ACCUM.
+ *   K plan (A and B MN-major, the weight gradient over tokens): only the listed k-blocks are summed, in ascending order,
+ *     so when the left-out rows of dy are zero the result has ivb_gemm_bf16's bits; with none listed the sum is 0.
+ *     Epilogue IVB_EPI_BF16 or IVB_EPI_F32 (IVB_FLAG_ACCUM allowed), no bias.
+ * A plan runs on the single-CTA kernels: IVB_FLAG_2CTA is refused, the ivb_set_default_2cta default does not apply.
+ * The FP8 GEMMs take no plan.                                                                               */
+long ivb_droppath_plan_ints(int M);
+int ivb_droppath_plan(const float* rowscale, long ld_rs, int branches, int M, int* plan, long ld_plan, void* stream);
+int ivb_gemm_bf16_plan(const void* A, int a_mn_major, long lda, const void* B, int b_mn_major, long ldb,
+                       int M, int N, int K, int epilogue, int flags, void* out0, long ld0, void* out1,
+                       long ld1, const void* bias, const void* gamma, const void* aux, long ldaux,
+                       const float* rowscale, int tile_n, const int* m_plan, const int* k_plan, void* stream);
+
 /* ---- FP8 (opt-in FP8 mode of the ViT block) ---------------------------------------------------
  * Formats: IVB_FP8_E4M3 (4 exponent, 3 mantissa bits, max 448: activations and weights) and IVB_FP8_E5M2 (max 57 344:
  * gradients).  Per-tensor current scaling: the scale comes from the tensor's own amax in the same call.

@@ -38,6 +38,9 @@
 // rings, so B is read from L2 once per 256 rows instead of once per 128.  A stage is refilled only when the MMA
 // warpgroups of BOTH CTAs released it (each arrives on its own and on the peer's empty barrier).
 //
+// DropPath plans (ivb_gemm_bf16_plan, bf16 single-CTA kernels): an M plan puts the row tiles holding a kept row first,
+// and the tiles after its live count only store (dead_tile); a K plan lists the k-blocks the weight gradient sums.
+//
 // Both kernels are built from the same pieces (gemm_prologue, produce, mma_kblock, dequantise, epilogue_tile) and keep
 // only how their MMA warpgroups consume and release the ring: FP8 promotion and the CTA pair's remote arrivals in the
 // cooperative kernel, the token in the ping-pong kernel.  Both C entry points share choose_kernel, dispatch and
@@ -237,22 +240,48 @@ __device__ __forceinline__ Smem gemm_prologue(const CUtensorMap& tmA, const CUte
   return s;
 }
 
-// The TMA producer (one elected thread): every k-block of the tiles first_tile, first_tile + stride, ... in that order.
-// CL = 2: the cluster's tile has 256 rows; this CTA (rank) loads its own 128 A rows and half of the B tile, which TMA
-// multicasts into both CTAs' rings.
+// The tiles (tile order: row tile, then column tile) and k-blocks a kernel's MMAs run: all of them, or under a DropPath
+// plan the live tiles and the listed k-blocks (the counts after each list).  A K plan that lists no k-block leaves no
+// live tile: every tile then runs dead_tile, whose zeros are the empty sum.  Read after gemm_prologue's PDL wait.
+struct PlanCounts {
+  int live_tiles, num_kb;
+};
+// Only the bf16 single-CTA kernels are built with the plan code (PLANNED).
+template <class Op, int CL>
+constexpr bool PLANNED = !Op::FP8 && CL == 1;
+
+template <class Op, int BN, int CL>
+__device__ __forceinline__ PlanCounts plan_counts(const GemmParams& p) {
+  const int num_m = (p.M + CL * BM - 1) / (CL * BM), num_n = (p.N + BN - 1) / BN, num_kb = (p.K + Op::BK - 1) / Op::BK;
+  if constexpr (!PLANNED<Op, CL>) return {num_m * num_n, num_kb};
+  const int live_kb = p.k_plan != nullptr ? p.k_plan[num_kb] : num_kb;
+  return {live_kb > 0 ? (p.m_plan != nullptr ? p.m_plan[num_m] : num_m) * num_n : 0, live_kb};
+}
+
+// The row tile the kernels' mt-th tile covers: mt, or under an M plan the plan's mt-th tile.
+template <class Op, int CL>
+__device__ __forceinline__ int plan_tile(const GemmParams& p, int mt) {
+  if constexpr (PLANNED<Op, CL>) return p.m_plan != nullptr ? p.m_plan[mt] : mt;
+  return mt;
+}
+
+// The TMA producer (one elected thread): every k-block of the tiles first_tile, first_tile + stride, ... below
+// num_tiles, in that order.  CL = 2: the cluster's tile has 256 rows; this CTA (rank) loads its own 128 A rows and half
+// of the B tile, which TMA multicasts into both CTAs' rings.  Under a DropPath plan (p.m_plan / p.k_plan, CL = 1 only)
+// num_tiles counts the live tiles, which come first, and only the listed k-blocks are loaded.
 template <class Op, int BN, bool A_MN, bool B_MN, int CL>
 __device__ __forceinline__ void produce(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p,
-                                        const Smem& s, int first_tile, int stride, uint32_t rank) {
+                                        const Smem& s, int first_tile, int stride, int num_tiles, int num_kb,
+                                        uint32_t rank) {
   using Cfg = GemmCfg<BN, B_MN>;
   const int num_n = (p.N + BN - 1) / BN;
-  const int num_tiles = ((p.M + CL * BM - 1) / (CL * BM)) * num_n;
-  const int num_kb = (p.K + Op::BK - 1) / Op::BK;
   int stage = 0;
   uint32_t phase = 0;
   for (int tile = first_tile; tile < num_tiles; tile += stride) {
-    const int m0 = (tile / num_n) * (CL * BM) + rank * BM;
+    const int m0 = plan_tile<Op, CL>(p, tile / num_n) * (CL * BM) + rank * BM;
     const int n0 = (tile % num_n) * BN;
-    for (int kb = 0; kb < num_kb; ++kb) {
+    for (int i = 0; i < num_kb; ++i) {
+      const int kb = PLANNED<Op, CL> && p.k_plan != nullptr ? p.k_plan[i] : i;
       mbar_wait(&s.empty[stage], phase ^ 1);
       mbar_expect_tx(&s.full[stage], Cfg::STAGE_BYTES);
       uint8_t* sa = s.a + stage * A_STAGE_BYTES;
@@ -331,13 +360,14 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   const int num_n = (p.N + BN - 1) / BN;
   const int num_tiles = num_m * num_n;
   constexpr bool PROMOTE = Op::FP8;
-  const int num_kb = (p.K + Op::BK - 1) / Op::BK;
 
   const Smem s = gemm_prologue<BN, B_MN, CL>(tmA, tmB, 2 * CL);   // one arrival per MMA warpgroup of the cluster
+  const PlanCounts pc = plan_counts<Op, BN, CL>(p);
+  const int num_kb = pc.num_kb;
 
   if (wg == 0) {
     setmaxnreg_dec<40>();
-    if (warp == 0 && elect_one()) produce<Op, BN, A_MN, B_MN, CL>(tmA, tmB, p, s, cid, ncl, rank);
+    if (warp == 0 && elect_one()) produce<Op, BN, A_MN, B_MN, CL>(tmA, tmB, p, s, cid, ncl, pc.live_tiles, num_kb, rank);
   } else {
     setmaxnreg_inc<232>();
     // ===================== MMA + epilogue warpgroups =====================
@@ -356,8 +386,12 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     int stage = 0;
     uint32_t phase = 0;
     for (int tile = cid; tile < num_tiles; tile += ncl) {
-      const int m0 = (tile / num_n) * (CL * BM) + rank * BM;
+      const int m0 = plan_tile<Op, CL>(p, tile / num_n) * (CL * BM) + rank * BM;
       const int n0 = (tile % num_n) * BN;
+      if (PLANNED<Op, CL> && tile >= pc.live_tiles) {   // M plan: a tile of dropped rows, nothing loaded
+        dead_tile<BN>(p, m0 + cw * 64, 64, n0);
+        continue;
+      }
       int prev = 0;
       if constexpr (PROMOTE) {
 #pragma unroll
@@ -413,13 +447,15 @@ gemm_bf16_pingpong_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_
   const int wg = threadIdx.x >> 7;
   const int num_n = (p.N + PP_BN - 1) / PP_BN;
   const int num_tiles = ((p.M + BM - 1) / BM) * num_n;
-  const int num_kb = (p.K + Op::BK - 1) / Op::BK;
 
   const Smem s = gemm_prologue<PP_BN, B_MN, 1>(tmA, tmB, 1);   // each stage is read by exactly one MMA warpgroup
+  const PlanCounts pc = plan_counts<Op, PP_BN, 1>(p);
+  const int num_kb = pc.num_kb;
 
   if (wg == 0) {
     setmaxnreg_dec<40>();
-    if (warp == 0 && elect_one()) produce<Op, PP_BN, A_MN, B_MN, 1>(tmA, tmB, p, s, blockIdx.x, gridDim.x, 0);
+    if (warp == 0 && elect_one())
+      produce<Op, PP_BN, A_MN, B_MN, 1>(tmA, tmB, p, s, blockIdx.x, gridDim.x, pc.live_tiles, num_kb, 0);
   } else {
     setmaxnreg_inc<232>();
     // ===================== MMA + epilogue warpgroups, one whole tile each =====================
@@ -430,8 +466,14 @@ gemm_bf16_pingpong_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_
     if constexpr (Op::FP8 && !Op::VEC) dq = *p.a_scale_inv * *p.b_scale_inv;
     float acc[2][PP_BN / 2];            // rows [0, 64) and [64, 128) of the tile
     for (int j = cw, tile = blockIdx.x + cw * gridDim.x; tile < num_tiles; j += 2, tile += 2 * gridDim.x) {
-      const int m0 = (tile / num_n) * BM;
+      const int m0 = plan_tile<Op, 1>(p, tile / num_n) * BM;
       const int n0 = (tile % num_n) * PP_BN;
+      // M plan: live tiles come first, so the CTA's j-th tile is live exactly when j counts its live tiles; a dead
+      // tile takes no token and no ring stage
+      if (PLANNED<Op, 1> && tile >= pc.live_tiles) {
+        dead_tile<PP_BN>(p, m0, BM, n0);
+        continue;
+      }
       const int it = j * num_kb;        // ring position of this tile's first k-block
       int stage = it % STAGES;
       uint32_t phase = (it / STAGES) & 1;
@@ -449,7 +491,7 @@ gemm_bf16_pingpong_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
       // hand the token on (only if the CTA has a next tile: an arrival nobody waits for would outlive the CTA)
-      if (tile + gridDim.x < num_tiles) named_bar_arrive(2 - cw, 256);
+      if (tile + gridDim.x < pc.live_tiles) named_bar_arrive(2 - cw, 256);
       wgmma_wait<0>();
       wgmma_reg_fence(acc[0], PP_BN / 2);
       wgmma_reg_fence(acc[1], PP_BN / 2);
@@ -556,6 +598,7 @@ static GemmParams make_params(int M, int N, int K, int epilogue, int flags, void
   p.gamma = reinterpret_cast<const __nv_bfloat16*>(gamma);
   p.aux = aux; p.ldaux = ldaux; p.rowscale = rowscale;
   p.a_scale_inv = p.b_scale_inv = nullptr;
+  p.m_plan = p.k_plan = nullptr;
   return p;
 }
 
@@ -613,27 +656,59 @@ using namespace ivb;
 
 extern "C" void ivb_set_default_2cta(int enable) { g_default_2cta = enable != 0; }
 
+// ivb_gemm_bf16 and ivb_gemm_bf16_plan; `fn` names the entry point in messages.
+static int gemm_bf16(const char* fn, const void* A, int a_mn_major, long lda, const void* B, int b_mn_major, long ldb,
+                     int M, int N, int K, int epilogue, int flags, void* out0, long ld0, void* out1, long ld1,
+                     const void* bias, const void* gamma, const void* aux, long ldaux, const float* rowscale,
+                     int tile_n, const int* m_plan, const int* k_plan, cudaStream_t stream) {
+  char msg[128];
+  auto fail = [&](const char* what) {
+    std::snprintf(msg, sizeof(msg), "%s: %s", fn, what);
+    return set_error(msg);
+  };
+  if (M <= 0 || N <= 0 || K <= 0) return fail("empty problem");
+  if ((N & 7) || (lda & 7) || (ldb & 7) || (ld0 & 7)) return fail("N and leading dimensions must be multiples of 8 elements");
+  if (int rc = check_epilogue_args(fn, epilogue, out0, out1, ld1, aux, ldaux, bias, gamma)) return rc;
+  if (a_mn_major && !b_mn_major) return fail("(A MN-major, B K-major) unused");
+  GemmParams p = make_params(M, N, K, epilogue, flags, out0, ld0, out1, ld1, bias, gamma, aux, ldaux, rowscale);
+  const bool force2 = (flags & IVB_FLAG_2CTA) != 0, force1 = (flags & IVB_FLAG_1CTA) != 0;
+  const bool forcepp = (flags & IVB_FLAG_PINGPONG) != 0;
+  if ((int)force2 + (int)force1 + (int)forcepp > 1)
+    return fail("IVB_FLAG_1CTA, IVB_FLAG_2CTA and IVB_FLAG_PINGPONG exclude each other");
+  if (forcepp && tile_n != 0 && tile_n != PP_BN) return fail("the ping-pong kernel has tile_n 128");
+  const bool plan = m_plan != nullptr || k_plan != nullptr;
+  if (plan && force2) return fail("a DropPath plan needs a single-CTA kernel (no IVB_FLAG_2CTA)");
+  if (m_plan != nullptr && (flags & IVB_FLAG_ACCUM)) return fail("an M plan excludes IVB_FLAG_ACCUM");
+  if (k_plan != nullptr && !(a_mn_major && b_mn_major)) return fail("a K plan needs both operands MN-major (wgrad)");
+  if (k_plan != nullptr && (bias != nullptr || (epilogue != IVB_EPI_BF16 && epilogue != IVB_EPI_F32)))
+    return fail("a K plan needs IVB_EPI_BF16 or IVB_EPI_F32 without bias");
+  p.m_plan = m_plan;
+  p.k_plan = k_plan;
+  // a plan runs on the single-CTA kernels, whatever the process-wide CTA-pair default
+  const KernelChoice k = choose_kernel(M, N, K, flags, tile_n, false, g_default_2cta && !plan);
+  if (!a_mn_major && !b_mn_major) return dispatch<OpBf16, false, false>(k, A, lda, B, ldb, p, stream);
+  if (!a_mn_major) return dispatch<OpBf16, false, true>(k, A, lda, B, ldb, p, stream);
+  return dispatch<OpBf16, true, true>(k, A, lda, B, ldb, p, stream);
+}
+
 extern "C" int ivb_gemm_bf16(const void* A, int a_mn_major, long lda, const void* B,
                              int b_mn_major, long ldb, int M, int N, int K, int epilogue,
                              int flags, void* out0, long ld0, void* out1, long ld1,
                              const void* bias, const void* gamma, const void* aux, long ldaux,
-                             const float* rowscale, int tile_n, void* stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  if (M <= 0 || N <= 0 || K <= 0) return set_error("ivb_gemm_bf16: empty problem");
-  if ((N & 7) || (lda & 7) || (ldb & 7) || (ld0 & 7))
-    return set_error("ivb_gemm_bf16: N and leading dimensions must be multiples of 8 elements");
-  if (int rc = check_epilogue_args("ivb_gemm_bf16", epilogue, out0, out1, ld1, aux, ldaux, bias, gamma)) return rc;
-  if (a_mn_major && !b_mn_major) return set_error("ivb_gemm_bf16: (A MN-major, B K-major) unused");
-  const GemmParams p = make_params(M, N, K, epilogue, flags, out0, ld0, out1, ld1, bias, gamma, aux, ldaux, rowscale);
-  const bool force2 = (flags & IVB_FLAG_2CTA) != 0, force1 = (flags & IVB_FLAG_1CTA) != 0;
-  const bool forcepp = (flags & IVB_FLAG_PINGPONG) != 0;
-  if ((int)force2 + (int)force1 + (int)forcepp > 1)
-    return set_error("ivb_gemm_bf16: IVB_FLAG_1CTA, IVB_FLAG_2CTA and IVB_FLAG_PINGPONG exclude each other");
-  if (forcepp && tile_n != 0 && tile_n != PP_BN) return set_error("ivb_gemm_bf16: the ping-pong kernel has tile_n 128");
-  const KernelChoice k = choose_kernel(M, N, K, flags, tile_n, false, g_default_2cta);
-  if (!a_mn_major && !b_mn_major) return dispatch<OpBf16, false, false>(k, A, lda, B, ldb, p, stream);
-  if (!a_mn_major) return dispatch<OpBf16, false, true>(k, A, lda, B, ldb, p, stream);
-  return dispatch<OpBf16, true, true>(k, A, lda, B, ldb, p, stream);
+                             const float* rowscale, int tile_n, void* stream) {
+  return gemm_bf16("ivb_gemm_bf16", A, a_mn_major, lda, B, b_mn_major, ldb, M, N, K, epilogue, flags, out0, ld0, out1,
+                   ld1, bias, gamma, aux, ldaux, rowscale, tile_n, nullptr, nullptr,
+                   reinterpret_cast<cudaStream_t>(stream));
+}
+
+extern "C" int ivb_gemm_bf16_plan(const void* A, int a_mn_major, long lda, const void* B, int b_mn_major, long ldb,
+                                  int M, int N, int K, int epilogue, int flags, void* out0, long ld0, void* out1,
+                                  long ld1, const void* bias, const void* gamma, const void* aux, long ldaux,
+                                  const float* rowscale, int tile_n, const int* m_plan, const int* k_plan,
+                                  void* stream) {
+  return gemm_bf16("ivb_gemm_bf16_plan", A, a_mn_major, lda, B, b_mn_major, ldb, M, N, K, epilogue, flags, out0, ld0,
+                   out1, ld1, bias, gamma, aux, ldaux, rowscale, tile_n, m_plan, k_plan,
+                   reinterpret_cast<cudaStream_t>(stream));
 }
 
 extern "C" int ivb_gemm_fp8(const void* A, int a_mn_major, long lda, int a_format, const float* a_scale_inv,

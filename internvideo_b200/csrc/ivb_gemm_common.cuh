@@ -24,7 +24,43 @@ struct GemmParams {
   const float* rowscale;  // EPI_RESID: optional per-row multiplier of the branch (DropPath keep/scale)
   const float* a_scale_inv;  // fp8 operands: device scalars, the accumulator is multiplied by their product
   const float* b_scale_inv;
+  // DropPath plan (ivb_droppath_plan), bf16 single-CTA kernels only; null: every tile, every k-block.
+  // m_plan: the ceil(M/128) row tiles, live ones first, then their count; a dead tile runs dead_tile instead of its MMAs.
+  // k_plan: the ascending live 64-row k-blocks, then their count; the k-blocks it leaves out are skipped.
+  const int* m_plan;
+  const int* k_plan;
 };
+
+// The epilogue's outputs for a tile whose rows all have DropPath factor 0, with no MMA: EPI_RESID passes the residual
+// through (out0 = aux, out1 = 0), every other epilogue writes zeros (EPI_GELU_BWD without reading aux).  Also every
+// tile of a K plan that lists no k-block (EPI_BF16 / EPI_F32 without bias): zeros, or under IVB_FLAG_ACCUM nothing.
+// Rows [row0, row0 + rows) and columns [n0, n0 + BN) inside the matrix, in 16-byte vectors by the 128 threads of a
+// warpgroup.
+template <int BN>
+__device__ __forceinline__ void dead_tile(const GemmParams& p, long row0, int rows, int n0) {
+  if (p.flags & IVB_FLAG_ACCUM) return;
+  const int units = min(BN, p.N - n0) / 8;   // 8-column pieces per row (N is a multiple of 8)
+  const long nrows = min(static_cast<long>(rows), p.M - row0);
+  const uint4 z = make_uint4(0u, 0u, 0u, 0u);
+#pragma unroll 1
+  for (long i = threadIdx.x & 127; i < nrows * units; i += 128) {
+    const long row = row0 + i / units;
+    const int col = n0 + static_cast<int>(i % units) * 8;
+    if (p.epi == IVB_EPI_RESID || p.epi == IVB_EPI_F32) {
+      uint4* o = reinterpret_cast<uint4*>(reinterpret_cast<float*>(p.out0) + row * p.ld0 + col);
+      if (p.epi == IVB_EPI_RESID) {
+        const uint4* a = reinterpret_cast<const uint4*>(reinterpret_cast<const float*>(p.aux) + row * p.ldaux + col);
+        o[0] = a[0]; o[1] = a[1];
+      } else {
+        o[0] = z; o[1] = z;
+      }
+    } else {
+      *reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(p.out0) + row * p.ld0 + col) = z;
+    }
+    if (p.out1 != nullptr && (p.epi == IVB_EPI_RESID || p.epi == IVB_EPI_BIAS_GELU))
+      *reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(p.out1) + row * p.ld1 + col) = z;
+  }
+}
 
 // 32-byte row pieces as two 128-bit accesses (sm_90 has no 256-bit global load / store).
 __device__ __forceinline__ void st_global_256(void* p, const uint32_t r[8]) {

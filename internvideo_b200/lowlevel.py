@@ -67,7 +67,7 @@ def _call(name, *args, kind=None, flops=0.0):
     _lib.check(fn(*args), "ivb_" + name)
     if profs:
         e1 = torch.cuda.Event(enable_timing=True); e1.record()
-        rec = (_gemm_name(*args) if name == "gemm_bf16" else name, kind, flops, e0, e1)
+        rec = (_gemm_name(*args) if name.startswith("gemm_bf16") else name, kind, flops, e0, e1)
         for p in profs:
             p.records.append(rec)
 
@@ -145,13 +145,15 @@ def device_check() -> None:
 
 # ----------------------------------------------------------------------------------------- GEMM
 def gemm(a, b, *, a_t=False, b_t=False, epi=EPI_BF16, flags=0, out0=None, out1=None, bias=None,
-         gamma=None, aux=None, rowscale=None, tile_n=0):
+         gamma=None, aux=None, rowscale=None, tile_n=0, m_plan=None, k_plan=None):
     """D[M,N] = epi(sum_k A(m,k) B(n,k)).
 
     a_t=False: `a` is [M,K]; a_t=True: `a` is [K,M] (MN-major operand).
     b_t=False: `b` is [N,K]; b_t=True: `b` is [K,N].
+    m_plan / k_plan: the M and K plans of a DropPath plan over the GEMM's M rows / its K (ops.droppath_plan); with
+    either the call goes to ivb_gemm_bf16_plan, which skips the work of the dropped rows.
     """
-    _chk(("a", a, bf16), ("b", b, bf16))
+    _chk(("a", a, bf16), ("b", b, bf16), ("m_plan?", m_plan, i32), ("k_plan?", k_plan, i32))
     lda = _rows2d(a, "a"); ldb = _rows2d(b, "b")
     if a_t:
         K, M = a.shape
@@ -164,10 +166,12 @@ def gemm(a, b, *, a_t=False, b_t=False, epi=EPI_BF16, flags=0, out0=None, out1=N
     if K != Kb:
         raise _lib.IvbError(f"gemm: contraction mismatch {K} vs {Kb}")
     out0 = _epilogue_operands(M, N, epi, out0, out1, bias, gamma, aux, rowscale, a.device)
-    _call("gemm_bf16", a, int(a_t), lda, b, int(b_t), ldb, M, N, K, epi, flags, out0, _rows2d(out0, "out0"), out1,
-          _rows2d(out1, "out1"), bias, gamma, aux, _rows2d(aux, "aux"), rowscale, tile_n, kind="gemm",
-          flops=2.0 * M * N * K)
+    plan = () if m_plan is None and k_plan is None else (m_plan, k_plan)
+    _call("gemm_bf16_plan" if plan else "gemm_bf16", a, int(a_t), lda, b, int(b_t), ldb, M, N, K, epi, flags, out0,
+          _rows2d(out0, "out0"), out1, _rows2d(out1, "out1"), bias, gamma, aux, _rows2d(aux, "aux"), rowscale, tile_n,
+          *plan, kind="gemm", flops=2.0 * M * N * K)
     return out0
+
 
 
 def _epilogue_operands(M, N, epi, out0, out1, bias, gamma, aux, rowscale, device):

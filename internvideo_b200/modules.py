@@ -283,9 +283,11 @@ class Block(nn.Module):
         # FP8 inference with per-channel weight copies (set_fp8_inference); None when off
         self.fp8_inference = None
 
-    def forward_stream(self, x2d, B, n, rowscale=None):
+    def forward_stream(self, x2d, B, n, rowscale=None, plans=None):
         """fp32 residual stream [B*n, D] -> [B*n, D] (the hot path used by the model).
-        rowscale: optional (rs1, rs2) fp32 [B*n] DropPath factors sampled by the caller for all blocks at once."""
+        rowscale: optional (rs1, rs2) fp32 [B*n] DropPath factors sampled by the caller for all blocks at once.
+        plans: optional (plan1, plan2) DropPath plans of those factors (ops.droppath_plan rows, None for a branch
+        without one): the training GEMMs then skip the rows the draw dropped."""
         rs1 = rs2 = None
         if rowscale is not None:
             rs1, rs2 = rowscale
@@ -296,7 +298,8 @@ class Block(nn.Module):
             rs2 = s2.repeat_interleave(n) if s2 is not None else None
         if not torch.is_grad_enabled():
             return self.forward_infer(x2d, B, n, (rs1, rs2))
-        return ops.BlockFn.apply(x2d, self._spec(B, n, training=True), rs1, rs2, *self._param_tuple())
+        return ops.BlockFn.apply(x2d, self._spec(B, n, training=True), rs1, rs2, *self._param_tuple(),
+                                 *(plans or ()))
 
     def _spec(self, B, n, training):
         return ops.BlockSpec(B, n, self.num_heads, self.mlp.gelu_tanh, eps1=self.norm1.variance_epsilon,
@@ -430,6 +433,17 @@ class VideoMAEBlock(nn.Module):
 
 
 FP8_SCALINGS = {"tensor": ops.FP8_TENSOR, "token": ops.FP8_TOKEN}
+
+
+def set_droppath_skip(model: nn.Module, enabled: bool = True) -> int:
+    """Switch, in every PretrainInternVideo2 tower of `model`, whether a training step skips the GEMM work of the clips
+    its DropPath draw drops (on by default; ops.droppath_plan, ivb_gemm_bf16_plan).  Off runs every row, with the same
+    parameters and gradients; the switch is there to measure the two in one process.  Returns how many towers were
+    switched."""
+    towers = [m for m in model.modules() if isinstance(m, PretrainInternVideo2)]
+    for m in towers:
+        m.droppath_skip = bool(enabled)
+    return len(towers)
 
 
 def set_fp8(model: nn.Module, enabled: bool = True, scaling: str = "tensor") -> int:
@@ -791,6 +805,7 @@ class PretrainInternVideo2(InternVideo2Tower):
     """
 
     pos_prefixes = ("", "clip_", "mae_")
+    droppath_skip = True      # set_droppath_skip
 
     def __init__(self, in_chans=3, patch_size=14, img_size=224, qkv_bias=False, drop_path_rate=0.25,
                  embed_dim=1408, num_heads=16, mlp_ratio=4.3637, init_values=1e-5, qk_normalization=True,
@@ -843,8 +858,11 @@ class PretrainInternVideo2(InternVideo2Tower):
             rs = drop_path_factors.to(device=h.device, dtype=f32).repeat_interleave(n, dim=1).contiguous()
         else:
             rs = self._sample_drop_path(B, n, h.device)
+        plans = self._droppath_plans(rs)
+
         def block(i, blk, h):
-            return blk.forward_stream(h, B, n, None if rs is None else (rs[2 * i], rs[2 * i + 1]))
+            return blk.forward_stream(h, B, n, None if rs is None else (rs[2 * i], rs[2 * i + 1]),
+                                      None if plans is None else plans[2 * i:2 * i + 2])
         h, taps = run_blocks(self.blocks, h, block, self.clip_return_index + self.mae_return_index, last)
         return taps, h, idx, B, n
 
@@ -867,6 +885,16 @@ class PretrainInternVideo2(InternVideo2Tower):
             return None
         m = (torch.rand((keep.shape[0], B), device=device, dtype=f32) < keep).to(f32) / keep
         return m.repeat_interleave(n, dim=1).contiguous()
+
+    def _droppath_plans(self, rs):
+        """The DropPath plans of the step's factors rs [2*depth, B*n] (one launch, ops.droppath_plan): per branch its
+        plan row, or None for a branch of rate 0 (block 0), which runs every row.  None when there is nothing to skip:
+        no factors, no gradient (the no-grad block path takes no plan) or set_droppath_skip(model, False)."""
+        if rs is None or not self.droppath_skip or not torch.is_grad_enabled():
+            return None
+        plan = ops.droppath_plan(rs)
+        return [plan[2 * i + j] if isinstance(dp, DropPath) else None
+                for i, blk in enumerate(self.blocks) for j, dp in enumerate((blk.drop_path1, blk.drop_path2))]
 
     def _decoder_inputs(self, taps, idx, B, n):
         cpe, mpe = self._pos_table("clip_"), self._pos_table("mae_")

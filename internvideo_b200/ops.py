@@ -230,7 +230,27 @@ BlockSaved = namedtuple("BlockSaved", "n1 qkv qkn a lse mean1 rstd1 rq rk x1 y1 
                                       "qkvw_t qkvw_s projw_t projw_s fc1w_t fc1w_s fc2w_t fc2w_s")
 
 
-def block_forward(x, spec, p, rs1=None, rs2=None, save=True):
+def droppath_plan(rowscale):
+    """DropPath plans of the rows of rowscale fp32 [R, M], one block branch's per-row factors each (ivb_droppath_plan,
+    one launch): int32 [R, ivb_droppath_plan_ints(M)], row r the plan of branch r, for block_forward / block_backward."""
+    ll._chk(("rowscale", rowscale, f32))
+    R, M = rowscale.shape
+    plan = torch.empty((R, int(ll._lib.load().ivb_droppath_plan_ints(M))), device=rowscale.device, dtype=torch.int32)
+    ll._call("droppath_plan", rowscale, ll._rows2d(rowscale, "rowscale"), R, M, plan, plan.stride(0))
+    return plan
+
+
+def _branch_plans(plan, M, prec):
+    """(M plan, K plan) of a branch's DropPath plan row for the block's GEMMs over its M rows: the M plan for a GEMM
+    whose M rows are the block's rows, the K plan for a weight gradient whose K runs over them.  (None, None) without
+    a plan or in FP8 (the FP8 GEMMs take none)."""
+    if plan is None or prec != BF16:
+        return None, None
+    nm = (M + 127) // 128
+    return plan[:nm + 1], plan[nm + 1:]
+
+
+def block_forward(x, spec, p, rs1=None, rs2=None, save=True, plan1=None, plan2=None):
     """One pre-norm ViT block over the fp32 residual stream [B*n, D]: spec a BlockSpec, p the BlockParams.  The
     InternVideo2 block (Block.forward, internvideo2_pretrain.py:279-297), or with spec.layernorm the VideoMAE block
     (videomae.py:104-132, IV1 modeling_finetune.py:132-181: LayerNorm with bias, q/v bias on qkv, no q/k norm, erf GELU):
@@ -250,7 +270,11 @@ def block_forward(x, spec, p, rs1=None, rs2=None, save=True):
     their fused epilogues.  FP8_TOKEN also casts the four weights per output channel (4 calls) and, with save, per input
     channel into their transposed copies (4 more), and its norm kernel then also writes the bf16 row and statistics
     the backward needs (without save: the same E4M3 bits from the inference norm kernel).  Attention, the q/k norms and
-    the residual stream stay as above."""
+    the residual stream stay as above.
+
+    plan1 / plan2: optional DropPath plans of the two branches (rows of droppath_plan of rs1 / rs2): the bf16 GEMMs
+    of a branch then skip the row tiles whose rows rs zeroes, writing what the epilogue table of ivb_gemm_bf16_plan
+    gives them (x1 = x, zeros elsewhere); the rows they do compute and x2 are as without a plan."""
     B, n, H = spec.B, spec.n, spec.H
     M, D = x.shape
     d = D // H
@@ -276,9 +300,11 @@ def block_forward(x, spec, p, rs1=None, rs2=None, save=True):
         q, s, y, mean, rstd = ll.norm_fwd_fp8(t, w, b, eps=eps, layernorm=spec.layernorm, save=True)
         return (q, s), y, mean, rstd
 
+    mp = (_branch_plans(plan1, M, prec)[0], _branch_plans(plan2, M, prec)[0])
+
     def linear(act, i, w, **epilogue):
         if prec == BF16:
-            return ll.gemm(act, w, **epilogue)
+            return ll.gemm(act, w, m_plan=mp[i // 2], **epilogue)
         if per_token:     # act: bf16, or the (E4M3 rows, scale_inv) pair the norm wrote
             q, s = ll.fp8_quantize_rows(act) if torch.is_tensor(act) else act
         else:
@@ -315,14 +341,16 @@ def block_forward(x, spec, p, rs1=None, rs2=None, save=True):
     return x2, BlockSaved(n1, qkv, qkn, a, lse, mean1, rstd1, rq, rk, x1, y1, n2, mean2, rstd2, h, g, y2, *wt8)
 
 
-def block_backward(x, s, spec, t, P, dx2, rs1, rs2):
+def block_backward(x, s, spec, t, P, dx2, rs1, rs2, plan1=None, plan2=None):
     """Backward of block_forward(save=True), from its BlockSaved s: 13 to 17 library calls in bf16 (with or without the
     q/k norms and the qkv bias, the fused RMSNorm norm2 + LayerScale backward), and in FP8 one more per input-gradient
     GEMM (the cast of its gradient: E5M2 with a per-tensor scale in FP8_TENSOR, E4M3 rows with per-row scales in
     FP8_TOKEN).  The LayerNorm block (spec.layernorm) also returns its norms'
     bias gradients and always runs the attention branch's LayerScale backward as its own call.  `t` are the block's
     tensors as autograd handed them back, `P` the nn.Parameter objects (gradient sink), both BlockParams.  Returns
-    (dx0, BlockParams of gradients | None when the sink took them)."""
+    (dx0, BlockParams of gradients | None when the sink took them).  plan1 / plan2: the DropPath plans block_forward
+    ran with; the input-gradient GEMMs of a branch skip its dead row tiles (zeros) and its weight gradients the
+    64-row k-blocks of dropped rows, whose gradient rows layerscale_bwd made zero."""
     B, n, H = spec.B, spec.n, spec.H
     M, D = x.shape
     d = D // H
@@ -344,28 +372,30 @@ def block_backward(x, s, spec, t, P, dx2, rs1, rs2):
         sink = None           # small parameters not contiguous in the flat buffer: autograd path
     dg2, dcs2, dn2w, dg1, dcs1 = seg["g2"], seg["fc2b"], seg["n2w"], seg["g1"], seg["projb"]
 
-    def dgrad(dy, w, w_t, w_s, **epilogue):   # dx = dy W; in FP8 on the cast gradient and the E4M3 copy of W^T
+    (m1, k1), (m2, k2) = _branch_plans(plan1, M, spec.precision), _branch_plans(plan2, M, spec.precision)
+
+    def dgrad(dy, w, w_t, w_s, m_plan, **epilogue):   # dx = dy W; in FP8 on the cast gradient and the E4M3 copy of W^T
         if spec.precision == FP8_TOKEN:
             q, sc = ll.fp8_quantize_rows(dy)
         elif spec.precision == FP8_TENSOR:
             q, _, sc, _ = ll.fp8_quantize(dy, ll.FP8_E5M2)
         else:
-            return ll.gemm(dy, w, b_t=True, **epilogue)
+            return ll.gemm(dy, w, b_t=True, m_plan=m_plan, **epilogue)
         return ll.gemm_fp8(q, sc, w_t, w_s, **epilogue)
 
-    def wgrad(dy, act, param):
+    def wgrad(dy, act, param, k_plan):
         if sink is None:
-            return ll.gemm(dy, act, a_t=True, b_t=True)
-        ll.gemm(dy, act, a_t=True, b_t=True, out0=param.grad, flags=ll.FLAG_ACCUM)
+            return ll.gemm(dy, act, a_t=True, b_t=True, k_plan=k_plan)
+        ll.gemm(dy, act, a_t=True, b_t=True, out0=param.grad, flags=ll.FLAG_ACCUM, k_plan=k_plan)
         sink.grad_written(param)
         return None
     # ---- MLP branch
     dy2 = ll.layerscale_bwd(dx2, s.y2, t.g2, dg2 if t.g2 is not None else None, dcs2, rowscale=rs2)
-    dfc2w = wgrad(dy2, s.g, P.fc2w)
-    dh = dgrad(dy2, t.fc2w, s.fc2w_t, s.fc2w_s, epi=ll.EPI_GELU_BWD, flags=spec.gelu_flags(True), aux=s.h)
+    dfc2w = wgrad(dy2, s.g, P.fc2w, k2)
+    dh = dgrad(dy2, t.fc2w, s.fc2w_t, s.fc2w_s, m2, epi=ll.EPI_GELU_BWD, flags=spec.gelu_flags(True), aux=s.h)
     ll.colsum(dh, out=seg["fc1b"])
-    dfc1w = wgrad(dh, s.n2, P.fc1w)
-    dn2 = dgrad(dh, t.fc1w, s.fc1w_t, s.fc1w_s)
+    dfc1w = wgrad(dh, s.n2, P.fc1w, k2)
+    dn2 = dgrad(dh, t.fc1w, s.fc1w_t, s.fc1w_s, m2)
     # ---- attention branch
     if not spec.layernorm and t.g1 is not None and D <= 1536 and M >= 1024:
         # norm2 backward fused with the attention branch's LayerScale backward: the gradient of the residual
@@ -375,8 +405,8 @@ def block_backward(x, s, spec, t, P, dx2, rs1, rs2):
         dx1 = ll.norm_bwd(dn2, s.x1, t.n2w, s.mean2, s.rstd2, layernorm=spec.layernorm, dx_in=dx2, dweight=dn2w,
                           dbias=seg.get("n2b"))
         dy1 = ll.layerscale_bwd(dx1, s.y1, t.g1, dg1 if t.g1 is not None else None, dcs1, rowscale=rs1)
-    dprojw = wgrad(dy1, s.a, P.projw)
-    da = dgrad(dy1, t.projw, s.projw_t, s.projw_s)
+    dprojw = wgrad(dy1, s.a, P.projw, k1)
+    da = dgrad(dy1, t.projw, s.projw_t, s.projw_s, m1)
     dqkv = torch.empty((M, 3 * D), device=x.device, dtype=bf16)
     qk = s.qkn if s.qkn is not None else s.qkv
     ll.attn_bwd(qk[:, :D], qk[:, D:2 * D], s.qkv[:, 2 * D:], s.a, da, s.lse, B, n, H, d, spec.attn_scale(d),
@@ -386,10 +416,10 @@ def block_backward(x, s, spec, t, P, dx2, rs1, rs2):
     elif s.qkn is not None:
         ll.norm_bwd(dqkv[:, :D], s.qkv[:, :D], t.qnw, None, s.rq, dx_out=dqkv[:, :D], dweight=seg["qnw"])
         ll.norm_bwd(dqkv[:, D:2 * D], s.qkv[:, D:2 * D], t.knw, None, s.rk, dx_out=dqkv[:, D:2 * D], dweight=seg["knw"])
-    dqkvw = wgrad(dqkv, s.n1, P.qkvw)
+    dqkvw = wgrad(dqkv, s.n1, P.qkvw, k1)
     if t.qkvb is not None:
         ll.colsum(dqkv, out=seg["qkvb"])
-    dn1 = dgrad(dqkv, t.qkvw, s.qkvw_t, s.qkvw_s)
+    dn1 = dgrad(dqkv, t.qkvw, s.qkvw_t, s.qkvw_s, m1)
     dx0 = ll.norm_bwd(dn1, x, t.n1w, s.mean1, s.rstd1, layernorm=spec.layernorm, dx_in=dx1, dweight=seg["n1w"],
                       dbias=seg.get("n1b"))
     # ---- O(D) glue: bias grads through LayerScale (layerscale_bwd already folds gamma into the
@@ -407,36 +437,40 @@ def block_backward(x, s, spec, t, P, dx2, rs1, rs2):
 
 
 class BlockFn(torch.autograd.Function):
-    """Differentiable block_forward: apply(x, spec, rs1, rs2, *params) with spec a BlockSpec (spec.head_axis refused),
-    params the BlockParams and rs1 / rs2 optional fp32 [B*n] per-row DropPath keep/scale factors of the two branches.
+    """Differentiable block_forward: apply(x, spec, rs1, rs2, *params[, plan1, plan2]) with spec a BlockSpec
+    (spec.head_axis refused), params the BlockParams, rs1 / rs2 optional fp32 [B*n] per-row DropPath keep/scale factors
+    of the two branches and plan1 / plan2 their optional DropPath plans (block_forward).
 
     spec.checkpoint is the reference's `with_cp` / `use_checkpoint` (internvideo2_pretrain.py:294-295,
     torch.utils.checkpoint around the block): only the block INPUT (4 D bytes/token) is kept; backward first
     re-runs the forward to rebuild the 44 D bytes/token of saved activations, then the backward.  DropPath factors
-    are inputs, so the recomputation sees the same draw."""
+    and plans are inputs, so the recomputation sees the same draw."""
 
     @staticmethod
-    def forward(ctx, x, spec, rs1, rs2, *params):
+    def forward(ctx, x, spec, rs1, rs2, *args):
         if spec.head_axis:
             raise ll._lib.IvbError("BlockFn: head-axis attention (the VideoMAEv2 teacher's) has no backward")
-        params = BlockParams(*params)
-        x2, saved = block_forward(x, spec, params, rs1, rs2, save=not spec.checkpoint)
-        ctx.spec, ctx.params = spec, params
-        ctx.save_for_backward(x, rs1, rs2, *params, *(saved or ()))
+        nparams = len(BlockParams._fields)
+        params = BlockParams(*args[:nparams])
+        plans = tuple(args[nparams:]) or (None, None)
+        x2, saved = block_forward(x, spec, params, rs1, rs2, save=not spec.checkpoint, plan1=plans[0], plan2=plans[1])
+        ctx.spec, ctx.params, ctx.nplans = spec, params, len(args) - nparams
+        ctx.save_for_backward(x, rs1, rs2, *plans, *params, *(saved or ()))
         return x2
 
     @staticmethod
     def backward(ctx, dx2):
-        x, rs1, rs2, *rest = ctx.saved_tensors
+        x, rs1, rs2, plan1, plan2, *rest = ctx.saved_tensors
         nparams = len(BlockParams._fields)
         tensors = BlockParams._make(rest[:nparams])
         if ctx.spec.checkpoint:
             with torch.no_grad():
-                _, saved = block_forward(x, ctx.spec._replace(checkpoint=False), tensors, rs1, rs2, save=True)
+                _, saved = block_forward(x, ctx.spec._replace(checkpoint=False), tensors, rs1, rs2, save=True,
+                                         plan1=plan1, plan2=plan2)
         else:
             saved = BlockSaved._make(rest[nparams:])
-        dx0, grads = block_backward(x, saved, ctx.spec, tensors, ctx.params, dx2, rs1, rs2)
-        return (dx0, None, None, None) + (grads or (None,) * nparams)
+        dx0, grads = block_backward(x, saved, ctx.spec, tensors, ctx.params, dx2, rs1, rs2, plan1, plan2)
+        return (dx0, None, None, None) + (grads or (None,) * nparams) + (None,) * ctx.nplans
 
 
 def _common_sink(params):
