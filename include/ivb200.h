@@ -106,7 +106,8 @@ int ivb_gemm_bf16(const void* A, int a_mn_major, long lda, const void* B, int b_
  *     so when the left-out rows of dy are zero the result has ivb_gemm_bf16's bits; with none listed the sum is 0.
  *     Epilogue IVB_EPI_BF16 or IVB_EPI_F32 (IVB_FLAG_ACCUM allowed), no bias.
  * A plan runs on the single-CTA kernels: IVB_FLAG_2CTA is refused, the ivb_set_default_2cta default does not apply.
- * The FP8 GEMMs take no plan.                                                                               */
+ * The per-token FP8 GEMM takes an M plan (ivb_gemm_fp8_plan), and attention the factors themselves (ivb_attn_fwd_plan,
+ * ivb_attn_bwd_plan).                                                                                       */
 long ivb_droppath_plan_ints(int M);
 int ivb_droppath_plan(const float* rowscale, long ld_rs, int branches, int M, int* plan, long ld_plan, void* stream);
 int ivb_gemm_bf16_plan(const void* A, int a_mn_major, long lda, const void* B, int b_mn_major, long ldb,
@@ -195,6 +196,16 @@ int ivb_norm_fwd_fp8_train(const void* x, int x_is_f32, long ldx, const void* we
                            float* mean, float* rstd, void* stream);
 int ivb_fp8_quantize_cols_t(const void* x, long ldx, int M, int K, void* out_t, long ldt, float* col_amax,
                             float* col_scale_inv, void* stream);
+/* ivb_gemm_fp8_plan: ivb_gemm_fp8 with the M plan of a DropPath plan over its M rows (ivb_droppath_plan; NULL:
+ *   ivb_gemm_fp8 itself), with ivb_gemm_bf16_plan's M-plan rules: a dead row tile loads nothing and runs no MMA, its
+ *   rows get IVB_EPI_RESID out0 = aux and out1 = 0 and every other epilogue writes 0; live tiles get ivb_gemm_fp8's
+ *   values, on the kernel form it would pick (the cooperative one at tile_n 128: tile_n 192 is refused).  A plan needs
+ *   IVB_FLAG_FP8_VECTOR_SCALES (per-row scales are untouched by the other rows' values; a per-tensor scale is not) and
+ *   excludes IVB_FLAG_ACCUM.                                                                                      */
+int ivb_gemm_fp8_plan(const void* A, int a_mn_major, long lda, int a_format, const float* a_scale_inv, const void* B,
+                      int b_mn_major, long ldb, const float* b_scale_inv, int M, int N, int K, int epilogue, int flags,
+                      void* out0, long ld0, void* out1, long ld1, const void* bias, const void* gamma, const void* aux,
+                      long ldaux, const float* rowscale, int tile_n, const int* m_plan, void* stream);
 
 /* ---- RMSNorm / LayerNorm (row reductions, HBM-bound) -------------------------------------------
  * y(bf16) = norm(x) * weight (+ bias).  is_layernorm=0: RMSNorm (internvideo2_pretrain.py:117-128,
@@ -264,6 +275,20 @@ int ivb_attn_bwd(const void* q, long ldq, const void* k, long ldk, const void* v
                  const void* out, long ldo, const void* dout, long lddo, const float* lse2,
                  float* delta_ws, void* dq, long lddq, void* dk, long lddk, void* dv, long lddv,
                  int B, int n, int H, int d, float softmax_scale, void* stream);
+/* ivb_attn_fwd_plan / ivb_attn_bwd_plan: ivb_attn_fwd / ivb_attn_bwd that skip the clips a DropPath draw drops.
+ * rowscale: the attention branch's DropPath factors, fp32 [B*n] (required; the EPI_RESID rowscale of proj), one
+ * factor per clip repeated over its rows: clip b is dead when rowscale[b*n] is 0.  A dead clip's CTAs load nothing and
+ * run no MMA.  The forward writes its out rows 0 and its lse2 rows 0 (finite); the backward writes its dq, dk and dv
+ * rows 0, and its delta_ws entries as ivb_attn_bwd does.  Live clips get ivb_attn_fwd's / ivb_attn_bwd's bits.
+ * Those are the results of the plain calls wherever they matter: proj multiplies a dead clip's attention output by
+ * 0, so its gradient rows, and with them dq, dk and dv, are zero there too.                                        */
+int ivb_attn_fwd_plan(const void* q, long ldq, const void* k, long ldk, const void* v, long ldv,
+                      void* out, long ldo, float* lse2, int B, int n, int H, int d, float softmax_scale,
+                      const float* rowscale, void* stream);
+int ivb_attn_bwd_plan(const void* q, long ldq, const void* k, long ldk, const void* v, long ldv,
+                      const void* out, long ldo, const void* dout, long lddo, const float* lse2,
+                      float* delta_ws, void* dq, long lddq, void* dk, long lddk, void* dv, long lddv,
+                      int B, int n, int H, int d, float softmax_scale, const float* rowscale, void* stream);
 
 /* ---- token front-end (tubelet embed as visible-only gather-GEMM) --------------------------------
  * idx[b, 0..n_keep) = ascending positions where mask[b, :] == 0 — the order of `x[~mask]`

@@ -72,12 +72,19 @@ __device__ __forceinline__ void softmax_tile(float (&s)[ATT_COLS / 2], int valid
 
 // KA: number of 64-wide atoms covering head_dim (1: d<=64, 2: d<=128).  NO: wgmma N of P·V (d rounded up).
 // KS: k16 steps of S = Q K^T, ceil(d / 16).
-template <int KA, int NO, int KS>
-__global__ void __launch_bounds__(ATT_THREADS, 1)
-attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                const __grid_constant__ CUtensorMap tmV, const AttnFwdParams p) {
+// PLAN: the CTA of a dropped clip (attn_prologue) writes zeros to its out rows and lse2 0, a finite value, to its rows.
+template <int KA, int NO, int KS, bool PLAN>
+__device__ __forceinline__ void attn_fwd(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV,
+                                         const AttnFwdParams& p, const float* rowscale) {
   using Smem = FwdSmem<KA>;
-  const AttnCta c = attn_prologue<Smem>(p.n);
+  const AttnCta c = attn_prologue<Smem, PLAN>(p.n, rowscale);
+  if (PLAN && c.dead) {
+    zero_rows(p.out, p.ldo, c, p.n, p.d);
+    if (p.lse2 != nullptr)
+      for (int r = threadIdx.x; r < min(ATT_ROWS, p.n - c.row0); r += ATT_THREADS)
+        p.lse2[(static_cast<long>(c.b) * p.H + c.h) * p.n + c.row0 + r] = 0.0f;
+    return;
+  }
   attn_roles(c, [&] {
     // ===================== TMA producer =====================
     tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmK); tma_prefetch_desc(&tmV);
@@ -176,26 +183,60 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   });
 }
 
+template <int KA, int NO, int KS>
+__global__ void __launch_bounds__(ATT_THREADS, 1)
+attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+                const __grid_constant__ CUtensorMap tmV, const AttnFwdParams p) {
+  attn_fwd<KA, NO, KS, false>(tmQ, tmK, tmV, p, nullptr);
+}
+
+// rowscale: the attention branch's DropPath factors [B*n]
+template <int KA, int NO, int KS>
+__global__ void __launch_bounds__(ATT_THREADS, 1)
+attn_fwd_plan_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+                     const __grid_constant__ CUtensorMap tmV, const AttnFwdParams p, const float* rowscale) {
+  attn_fwd<KA, NO, KS, true>(tmQ, tmK, tmV, p, rowscale);
+}
+
 }  // namespace ivb
 
 using namespace ivb;
 
-extern "C" int ivb_attn_fwd(const void* q, long ldq, const void* k, long ldk, const void* v,
-                            long ldv, void* out, long ldo, float* lse2, int B, int n, int H, int d,
-                            float softmax_scale, void* stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+// ivb_attn_fwd and ivb_attn_fwd_plan (rowscale not null); `fn` names the entry point in messages.
+static int attn_fwd(const char* fn, const void* q, long ldq, const void* k, long ldk, const void* v, long ldv, void* out,
+                    long ldo, float* lse2, int B, int n, int H, int d, float softmax_scale, const float* rowscale,
+                    cudaStream_t stream) {
   if (B <= 0 || n <= 0) return 0;
   int rc;
-  if ((rc = check_head_args("ivb_attn_fwd", d, {ldq, ldk, ldv, ldo}))) return rc;
+  if ((rc = check_head_args(fn, d, {ldq, ldk, ldv, ldo}))) return rc;
   CUtensorMap tq, tk, tv;
   if ((rc = make_head_tmap(&tq, q, ldq, B, n, H, d, ATT_ROWS))) return rc;
   if ((rc = make_head_tmap(&tk, k, ldk, B, n, H, d, ATT_COLS))) return rc;
   if ((rc = make_head_tmap(&tv, v, ldv, B, n, H, d, ATT_COLS))) return rc;
   const AttnFwdParams p{B, n, H, d, softmax_scale * 1.4426950408889634f, reinterpret_cast<__nv_bfloat16*>(out), ldo, lse2};
   return dispatch_head_dim(d, [&](auto hd) {
+    if (rowscale != nullptr)
+      return launch_attn<attn_fwd_plan_kernel<hd.KA, hd.NO, hd.KS>, NO_PDL>(
+          "cudaFuncSetAttribute(attn_fwd_plan)", "attn_fwd_plan_kernel", FwdSmem<hd.KA>::BYTES, B, n, H, stream, tq, tk,
+          tv, p, rowscale);
     return launch_attn<attn_fwd_kernel<hd.KA, hd.NO, hd.KS>, NO_PDL>(
         "cudaFuncSetAttribute(attn_fwd)", "attn_fwd_kernel", FwdSmem<hd.KA>::BYTES, B, n, H, stream, tq, tk, tv, p);
   });
+}
+
+extern "C" int ivb_attn_fwd(const void* q, long ldq, const void* k, long ldk, const void* v,
+                            long ldv, void* out, long ldo, float* lse2, int B, int n, int H, int d,
+                            float softmax_scale, void* stream) {
+  return attn_fwd("ivb_attn_fwd", q, ldq, k, ldk, v, ldv, out, ldo, lse2, B, n, H, d, softmax_scale, nullptr,
+                  reinterpret_cast<cudaStream_t>(stream));
+}
+
+extern "C" int ivb_attn_fwd_plan(const void* q, long ldq, const void* k, long ldk, const void* v, long ldv, void* out,
+                                 long ldo, float* lse2, int B, int n, int H, int d, float softmax_scale,
+                                 const float* rowscale, void* stream) {
+  if (rowscale == nullptr) return set_error("ivb_attn_fwd_plan: rowscale is null");
+  return attn_fwd("ivb_attn_fwd_plan", q, ldq, k, ldk, v, ldv, out, ldo, lse2, B, n, H, d, softmax_scale, rowscale,
+                  reinterpret_cast<cudaStream_t>(stream));
 }
 
 // ---------------------------------------------------------------------------------------------------------------

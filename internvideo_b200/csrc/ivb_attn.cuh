@@ -60,10 +60,15 @@ struct AttnCta {
   int nblk, live;  // streamed tiles; MMA warpgroups that own a row < n (each arrives once on an `empty`)
   int rloc;        // in an MMA warpgroup: this thread's accumulator rows of the CTA are rloc and rloc + 8
   bool signal;     // the thread that arrives on `empty` for its warpgroup
+  bool dead;       // PLAN: the clip's DropPath factor is 0; the CTA only stores zero_rows
 };
 
-template <class Smem>
-__device__ __forceinline__ AttnCta attn_prologue(int n) {
+// PLAN (ivb_attn_fwd_plan, ivb_attn_bwd_plan): rowscale holds the attention branch's DropPath factors, one per clip
+// repeated over its n rows.  The CTA of a clip whose factor is 0 returns `dead` before it initialises or waits on a
+// barrier, so it issues no TMA and no MMA and every barrier count stays that of the live CTAs.  The factors may be
+// written by the kernel before (PDL), so they are read after its wait.
+template <class Smem, bool PLAN = false>
+__device__ __forceinline__ AttnCta attn_prologue(int n, const float* rowscale = nullptr) {
   AttnCta c;
   const int tid = threadIdx.x;
   c.warp = tid >> 5; c.lane = tid & 31; c.wg = tid >> 7;
@@ -72,6 +77,12 @@ __device__ __forceinline__ AttnCta attn_prologue(int n) {
   c.live = min(2, (n - c.row0 + 63) / 64);
   c.rloc = (c.wg - 1) * 64 + (c.warp & 3) * 16 + (c.lane >> 2);
   c.signal = (tid & 127) == 0;
+  c.dead = false;
+  if constexpr (PLAN) {
+    pdl_wait();
+    c.dead = rowscale[static_cast<long>(c.b) * n] == 0.0f;
+    if (c.dead) return c;
+  }
   if (tid == 0) {
     if ((smem_u32(attn_smem) & 1023u) != 0) __trap();
     mbar_init(Smem::bar_row(), 1);
@@ -126,6 +137,13 @@ __device__ __forceinline__ void store_rows(const float (&acc)[NO / 2], __nv_bflo
             pack_bf16(acc[4 * jn + 2 * r] * factor[r], acc[4 * jn + 2 * r + 1] * factor[r]);
     }
   }
+}
+
+// A dead CTA's rows (< n) of head h of the [B*n, ld] bf16 buffer out: zeros, by all the CTA's threads.
+__device__ __forceinline__ void zero_rows(__nv_bfloat16* out, long ld, const AttnCta& c, int n, int d) {
+  const int rows = min(ATT_ROWS, n - c.row0), pairs = d / 2;
+  for (int i = threadIdx.x; i < rows * pairs; i += ATT_THREADS)
+    reinterpret_cast<uint32_t*>(out + (static_cast<long>(c.b) * n + c.row0 + i / pairs) * ld + c.h * d)[i % pairs] = 0u;
 }
 
 // ------------------------------------------------------------------ host side

@@ -72,13 +72,17 @@ using BwdSmem = AttnSmem<KA, 2, BWD_NST, 2, 1>;
 
 // KA: 64-wide atoms covering head_dim (1: d <= 64, 2: d <= 128); NO: wgmma N of the accumulate MMAs;
 // KS: k16 steps of the S/dP MMAs, ceil(d / 16).
-template <int MODE, int KA, int NO, int KS>
-__global__ void __launch_bounds__(ATT_THREADS, 1)
-attn_bwd_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmY,
-                const __grid_constant__ CUtensorMap tmU, const __grid_constant__ CUtensorMap tmW,
-                const AttnBwdParams p) {
+// PLAN: the CTA of a dropped clip (attn_prologue) writes zeros to its output rows (dQ, or dV and dK).
+template <int MODE, int KA, int NO, int KS, bool PLAN>
+__device__ __forceinline__ void attn_bwd(const CUtensorMap& tmX, const CUtensorMap& tmY, const CUtensorMap& tmU,
+                                         const CUtensorMap& tmW, const AttnBwdParams& p, const float* rowscale) {
   using Smem = BwdSmem<KA>;
-  const AttnCta c = attn_prologue<Smem>(p.n);
+  const AttnCta c = attn_prologue<Smem, PLAN>(p.n, rowscale);
+  if (PLAN && c.dead) {
+    zero_rows(p.out1, p.ld1, c, p.n, p.d);
+    if (MODE == 1) zero_rows(p.out2, p.ld2, c, p.n, p.d);
+    return;
+  }
   const long hb = (static_cast<long>(c.b) * p.H + c.h) * p.n_pad;
   pdl_wait();
   pdl_launch_dependents();
@@ -186,6 +190,23 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__
   });
 }
 
+template <int MODE, int KA, int NO, int KS>
+__global__ void __launch_bounds__(ATT_THREADS, 1)
+attn_bwd_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmY,
+                const __grid_constant__ CUtensorMap tmU, const __grid_constant__ CUtensorMap tmW,
+                const AttnBwdParams p) {
+  attn_bwd<MODE, KA, NO, KS, false>(tmX, tmY, tmU, tmW, p, nullptr);
+}
+
+// rowscale: the attention branch's DropPath factors [B*n]
+template <int MODE, int KA, int NO, int KS>
+__global__ void __launch_bounds__(ATT_THREADS, 1)
+attn_bwd_plan_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmY,
+                     const __grid_constant__ CUtensorMap tmU, const __grid_constant__ CUtensorMap tmW,
+                     const AttnBwdParams p, const float* rowscale) {
+  attn_bwd<MODE, KA, NO, KS, true>(tmX, tmY, tmU, tmW, p, rowscale);
+}
+
 }  // namespace ivb
 
 using namespace ivb;
@@ -196,17 +217,21 @@ extern "C" long ivb_attn_bwd_workspace_floats(int B, int n, int H) {
   return 2 * static_cast<long>(B) * H * n_pad;
 }
 
-extern "C" int ivb_attn_bwd(const void* q, long ldq, const void* k, long ldk, const void* v,
-                            long ldv, const void* out, long ldo, const void* dout, long lddo,
-                            const float* lse2, float* delta_ws, void* dq, long lddq, void* dk,
-                            long lddk, void* dv, long lddv, int B, int n, int H, int d,
-                            float softmax_scale, void* stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+// ivb_attn_bwd and ivb_attn_bwd_plan (rowscale not null); `fn` names the entry point in messages.
+static int attn_bwd(const char* fn, const void* q, long ldq, const void* k, long ldk, const void* v, long ldv,
+                    const void* out, long ldo, const void* dout, long lddo, const float* lse2, float* delta_ws, void* dq,
+                    long lddq, void* dk, long lddk, void* dv, long lddv, int B, int n, int H, int d,
+                    float softmax_scale, const float* rowscale, cudaStream_t stream) {
   if (B <= 0 || n <= 0) return 0;
   int rc;
-  if ((rc = check_head_args("ivb_attn_bwd", d, {ldq, ldk, ldv, ldo, lddo, lddq, lddk, lddv}))) return rc;
-  if (lse2 == nullptr || delta_ws == nullptr) return set_error("ivb_attn_bwd: lse2 and the workspace are required");
-  if ((reinterpret_cast<uintptr_t>(delta_ws) & 15) != 0) return set_error("ivb_attn_bwd: workspace must be 16-byte aligned");
+  char msg[128];
+  auto fail = [&](const char* what) {
+    snprintf(msg, sizeof(msg), "%s: %s", fn, what);
+    return set_error(msg);
+  };
+  if ((rc = check_head_args(fn, d, {ldq, ldk, ldv, ldo, lddo, lddq, lddk, lddv}))) return rc;
+  if (lse2 == nullptr || delta_ws == nullptr) return fail("lse2 and the workspace are required");
+  if ((reinterpret_cast<uintptr_t>(delta_ws) & 15) != 0) return fail("workspace must be 16-byte aligned");
   const int n_pad = (n + ATT_COLS - 1) / ATT_COLS * ATT_COLS;
   const long half = static_cast<long>(B) * H * n_pad;
   float* lse2p = delta_ws;
@@ -232,6 +257,15 @@ extern "C" int ivb_attn_bwd(const void* q, long ldq, const void* k, long ldk, co
   const AttnBwdParams pq{B, n, H, d, n_pad, sc_log2, softmax_scale, lse2p, deltap, bf(dq), lddq, nullptr, 0};
   return dispatch_head_dim(d, [&](auto hd) {
     constexpr int smem = BwdSmem<hd.KA>::BYTES;
+    if (rowscale != nullptr) {
+      const char* attr = "cudaFuncSetAttribute(attn_bwd_plan)";
+      if ((rc = launch_attn<attn_bwd_plan_kernel<1, hd.KA, hd.NO, hd.KS>, ALLOW_PDL>(
+               attr, "attn_bwd_plan_kernel", smem, B, n, H, stream, rows[2], rows[3], tiles[0], tiles[1], pkv,
+               rowscale)))
+        return rc;
+      return launch_attn<attn_bwd_plan_kernel<0, hd.KA, hd.NO, hd.KS>, ALLOW_PDL>(
+          attr, "attn_bwd_plan_kernel", smem, B, n, H, stream, rows[0], rows[1], tiles[2], tiles[3], pq, rowscale);
+    }
     const char* attr = "cudaFuncSetAttribute(attn_bwd)";
     if ((rc = launch_attn<attn_bwd_kernel<1, hd.KA, hd.NO, hd.KS>, ALLOW_PDL>(attr, "attn_bwd_kernel", smem, B, n, H,
                                                                                stream, rows[2], rows[3], tiles[0],
@@ -240,4 +274,22 @@ extern "C" int ivb_attn_bwd(const void* q, long ldq, const void* k, long ldk, co
     return launch_attn<attn_bwd_kernel<0, hd.KA, hd.NO, hd.KS>, ALLOW_PDL>(attr, "attn_bwd_kernel", smem, B, n, H, stream,
                                                                             rows[0], rows[1], tiles[2], tiles[3], pq);
   });
+}
+
+extern "C" int ivb_attn_bwd(const void* q, long ldq, const void* k, long ldk, const void* v,
+                            long ldv, const void* out, long ldo, const void* dout, long lddo,
+                            const float* lse2, float* delta_ws, void* dq, long lddq, void* dk,
+                            long lddk, void* dv, long lddv, int B, int n, int H, int d,
+                            float softmax_scale, void* stream) {
+  return attn_bwd("ivb_attn_bwd", q, ldq, k, ldk, v, ldv, out, ldo, dout, lddo, lse2, delta_ws, dq, lddq, dk, lddk, dv,
+                  lddv, B, n, H, d, softmax_scale, nullptr, reinterpret_cast<cudaStream_t>(stream));
+}
+
+extern "C" int ivb_attn_bwd_plan(const void* q, long ldq, const void* k, long ldk, const void* v, long ldv,
+                                 const void* out, long ldo, const void* dout, long lddo, const float* lse2,
+                                 float* delta_ws, void* dq, long lddq, void* dk, long lddk, void* dv, long lddv, int B,
+                                 int n, int H, int d, float softmax_scale, const float* rowscale, void* stream) {
+  if (rowscale == nullptr) return set_error("ivb_attn_bwd_plan: rowscale is null");
+  return attn_bwd("ivb_attn_bwd_plan", q, ldq, k, ldk, v, ldv, out, ldo, dout, lddo, lse2, delta_ws, dq, lddq, dk, lddk,
+                  dv, lddv, B, n, H, d, softmax_scale, rowscale, reinterpret_cast<cudaStream_t>(stream));
 }

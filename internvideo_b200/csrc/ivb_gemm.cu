@@ -38,8 +38,9 @@
 // rings, so B is read from L2 once per 256 rows instead of once per 128.  A stage is refilled only when the MMA
 // warpgroups of BOTH CTAs released it (each arrives on its own and on the peer's empty barrier).
 //
-// DropPath plans (ivb_gemm_bf16_plan, bf16 single-CTA kernels): an M plan puts the row tiles holding a kept row first,
-// and the tiles after its live count only store (dead_tile); a K plan lists the k-blocks the weight gradient sums.
+// DropPath plans (ivb_gemm_bf16_plan: bf16 single-CTA kernels; ivb_gemm_fp8_plan: the OpPlannedFp8 instantiations of
+// both FP8 forms): an M plan puts the row tiles holding a kept row first, and the tiles after its live count only store
+// (dead_tile); a K plan lists the k-blocks the weight gradient sums.
 //
 // Both kernels are built from the same pieces (gemm_prologue, produce, mma_kblock, dequantise, epilogue_tile) and keep
 // only how their MMA warpgroups consume and release the ring: FP8 promotion and the CTA pair's remote arrivals in the
@@ -60,18 +61,23 @@ constexpr int EPI_BYTES = 8 * 16 * EPI_PITCH * 4;  // one 16 x 32 fp32 staging t
 
 // Operand formats: bf16 x bf16, or fp8 (A E4M3 or E5M2, B E4M3).  BK: elements in a 128-byte k-block.
 // VEC: per-row / per-column scale vectors instead of two scalars (E4M3 A only).
+// PLAN: the single-CTA kernels are built with the DropPath plan code (PLANNED); OpPlannedFp8 is OpVecFp8 with it, so
+// ivb_gemm_fp8 keeps kernels without it.
 struct OpBf16 {
-  static constexpr bool FP8 = false, VEC = false;
+  static constexpr bool FP8 = false, VEC = false, PLAN = true;
   static constexpr int BK = 64;
 };
 template <bool A_E5M2_>
 struct OpFp8 {
-  static constexpr bool FP8 = true, A_E5M2 = A_E5M2_, VEC = false;
+  static constexpr bool FP8 = true, A_E5M2 = A_E5M2_, VEC = false, PLAN = false;
   static constexpr int BK = 128;
 };
 struct OpVecFp8 {
-  static constexpr bool FP8 = true, A_E5M2 = false, VEC = true;
+  static constexpr bool FP8 = true, A_E5M2 = false, VEC = true, PLAN = false;
   static constexpr int BK = 128;
+};
+struct OpPlannedFp8 : OpVecFp8 {
+  static constexpr bool PLAN = true;
 };
 
 template <int BN, bool B_MN>
@@ -246,15 +252,18 @@ __device__ __forceinline__ Smem gemm_prologue(const CUtensorMap& tmA, const CUte
 struct PlanCounts {
   int live_tiles, num_kb;
 };
-// Only the bf16 single-CTA kernels are built with the plan code (PLANNED).
+// Only the single-CTA kernels of an Op with PLAN are built with the plan code (PLANNED).
 template <class Op, int CL>
-constexpr bool PLANNED = !Op::FP8 && CL == 1;
+constexpr bool PLANNED = Op::PLAN && CL == 1;
+// K plans only for bf16: FP8 operands are K-major, so an FP8 GEMM is never the weight gradient over tokens.
+template <class Op, int CL>
+constexpr bool K_PLANNED = PLANNED<Op, CL> && !Op::FP8;
 
 template <class Op, int BN, int CL>
 __device__ __forceinline__ PlanCounts plan_counts(const GemmParams& p) {
   const int num_m = (p.M + CL * BM - 1) / (CL * BM), num_n = (p.N + BN - 1) / BN, num_kb = (p.K + Op::BK - 1) / Op::BK;
   if constexpr (!PLANNED<Op, CL>) return {num_m * num_n, num_kb};
-  const int live_kb = p.k_plan != nullptr ? p.k_plan[num_kb] : num_kb;
+  const int live_kb = K_PLANNED<Op, CL> && p.k_plan != nullptr ? p.k_plan[num_kb] : num_kb;
   return {live_kb > 0 ? (p.m_plan != nullptr ? p.m_plan[num_m] : num_m) * num_n : 0, live_kb};
 }
 
@@ -281,7 +290,7 @@ __device__ __forceinline__ void produce(const CUtensorMap& tmA, const CUtensorMa
     const int m0 = plan_tile<Op, CL>(p, tile / num_n) * (CL * BM) + rank * BM;
     const int n0 = (tile % num_n) * BN;
     for (int i = 0; i < num_kb; ++i) {
-      const int kb = PLANNED<Op, CL> && p.k_plan != nullptr ? p.k_plan[i] : i;
+      const int kb = K_PLANNED<Op, CL> && p.k_plan != nullptr ? p.k_plan[i] : i;
       mbar_wait(&s.empty[stage], phase ^ 1);
       mbar_expect_tx(&s.full[stage], Cfg::STAGE_BYTES);
       uint8_t* sa = s.a + stage * A_STAGE_BYTES;
@@ -626,8 +635,9 @@ static KernelChoice choose_kernel(int M, int N, int K, int flags, int tile_n, bo
 }
 
 // The kernel k names, for operands of format Op and majors A_MN / B_MN.  Together with the entry points' choice of Op
-// and majors this instantiates the library's 36 kernels: the ping-pong kernel of every Op and major; the bf16
-// cooperative kernel at BN 256 / 192 / 176 / 128 and CL 1 or 2; the FP8 one (K-major only) at BN 192 or 128, CL 1.
+// and majors this instantiates the library's 38 kernels: the ping-pong kernel of every Op and major; the bf16
+// cooperative kernel at BN 256 / 192 / 176 / 128 and CL 1 or 2; the FP8 one (K-major only) at BN 192 or 128, CL 1,
+// and with a plan (OpPlannedFp8) at BN 128 only.
 template <class Op, bool A_MN, bool B_MN>
 static int dispatch(const KernelChoice& k, const void* A, long lda, const void* B, long ldb, const GemmParams& p,
                     cudaStream_t stream) {
@@ -644,7 +654,10 @@ static int dispatch(const KernelChoice& k, const void* A, long lda, const void* 
     }
   }
   switch (k.bn * 4 + k.cl) {
-    case 192 * 4 + 1: return launch_gemm<Op, false, 192, A_MN, B_MN, 1>(A, lda, B, ldb, p, stream);
+    case 192 * 4 + 1:
+      // with the plan code the promoting FP8 kernel does not hold 192 columns in registers: plans run it at 128
+      if constexpr (!(Op::FP8 && Op::PLAN)) return launch_gemm<Op, false, 192, A_MN, B_MN, 1>(A, lda, B, ldb, p, stream);
+      break;
     case 128 * 4 + 1: return launch_gemm<Op, false, 128, A_MN, B_MN, 1>(A, lda, B, ldb, p, stream);
   }
   return set_error("ivb_gemm_bf16: unsupported BN");
@@ -711,33 +724,65 @@ extern "C" int ivb_gemm_bf16_plan(const void* A, int a_mn_major, long lda, const
                    reinterpret_cast<cudaStream_t>(stream));
 }
 
+// ivb_gemm_fp8 and ivb_gemm_fp8_plan; `fn` names the entry point in messages.
+static int gemm_fp8(const char* fn, const void* A, int a_mn_major, long lda, int a_format, const float* a_scale_inv,
+                    const void* B, int b_mn_major, long ldb, const float* b_scale_inv, int M, int N, int K, int epilogue,
+                    int flags, void* out0, long ld0, void* out1, long ld1, const void* bias, const void* gamma,
+                    const void* aux, long ldaux, const float* rowscale, int tile_n, const int* m_plan,
+                    cudaStream_t stream) {
+  char msg[128];
+  auto fail = [&](const char* what) {
+    std::snprintf(msg, sizeof(msg), "%s: %s", fn, what);
+    return set_error(msg);
+  };
+  if (M <= 0 || N <= 0 || K <= 0) return fail("empty problem");
+  if (a_mn_major || b_mn_major) return fail("both operands must be K-major");
+  if ((lda & 15) || (ldb & 15)) return fail("lda and ldb must be multiples of 16 elements");
+  if ((N & 7) || (ld0 & 7)) return fail("N and ld0 must be multiples of 8 elements");
+  if (a_format != IVB_FP8_E4M3 && a_format != IVB_FP8_E5M2) return fail("unknown a_format");
+  if (a_scale_inv == nullptr || b_scale_inv == nullptr) return fail("scale_inv pointers are null");
+  const bool vec = (flags & IVB_FLAG_FP8_VECTOR_SCALES) != 0;
+  if (vec && a_format != IVB_FP8_E4M3) return fail("vector scales need an E4M3 A operand");
+  if (vec && ((reinterpret_cast<uintptr_t>(a_scale_inv) | reinterpret_cast<uintptr_t>(b_scale_inv)) & 7))
+    return fail("scale vectors must be 8-byte aligned");
+  if (int rc = check_epilogue_args(fn, epilogue, out0, out1, ld1, aux, ldaux, bias, gamma)) return rc;
+  const bool force1 = (flags & IVB_FLAG_1CTA) != 0, forcepp = (flags & IVB_FLAG_PINGPONG) != 0;
+  if (flags & IVB_FLAG_2CTA) return fail("no CTA-pair kernel");
+  if (force1 && forcepp) return fail("IVB_FLAG_1CTA and IVB_FLAG_PINGPONG exclude each other");
+  if (tile_n != 0 && tile_n != 128 && tile_n != 192) return fail("tile_n must be 0, 128 or 192");
+  if (forcepp && tile_n == 192) return fail("the ping-pong kernel has tile_n 128");
+  // a per-tensor scale comes from the whole tensor's amax, which the zeroed rows of dropped clips would change
+  if (m_plan != nullptr && !vec) return fail("a DropPath plan needs IVB_FLAG_FP8_VECTOR_SCALES");
+  if (m_plan != nullptr && (flags & IVB_FLAG_ACCUM)) return fail("an M plan excludes IVB_FLAG_ACCUM");
+  if (m_plan != nullptr && tile_n == 192) return fail("a DropPath plan runs the FP8 GEMM at tile_n 128");
+  GemmParams p = make_params(M, N, K, epilogue, flags, out0, ld0, out1, ld1, bias, gamma, aux, ldaux, rowscale);
+  p.a_scale_inv = a_scale_inv;
+  p.b_scale_inv = b_scale_inv;
+  p.m_plan = m_plan;
+  KernelChoice k = choose_kernel(M, N, K, flags, tile_n, true, false);
+  if (m_plan != nullptr) k.bn = 128;   // the cooperative kernel's width under a plan (dispatch); the ping-pong one's
+  if (m_plan != nullptr) return dispatch<OpPlannedFp8, false, false>(k, A, lda, B, ldb, p, stream);
+  if (vec) return dispatch<OpVecFp8, false, false>(k, A, lda, B, ldb, p, stream);
+  if (a_format == IVB_FP8_E5M2) return dispatch<OpFp8<true>, false, false>(k, A, lda, B, ldb, p, stream);
+  return dispatch<OpFp8<false>, false, false>(k, A, lda, B, ldb, p, stream);
+}
+
 extern "C" int ivb_gemm_fp8(const void* A, int a_mn_major, long lda, int a_format, const float* a_scale_inv,
                             const void* B, int b_mn_major, long ldb, const float* b_scale_inv, int M, int N, int K,
                             int epilogue, int flags, void* out0, long ld0, void* out1, long ld1, const void* bias,
                             const void* gamma, const void* aux, long ldaux, const float* rowscale, int tile_n,
-                            void* stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  if (M <= 0 || N <= 0 || K <= 0) return set_error("ivb_gemm_fp8: empty problem");
-  if (a_mn_major || b_mn_major) return set_error("ivb_gemm_fp8: both operands must be K-major");
-  if ((lda & 15) || (ldb & 15)) return set_error("ivb_gemm_fp8: lda and ldb must be multiples of 16 elements");
-  if ((N & 7) || (ld0 & 7)) return set_error("ivb_gemm_fp8: N and ld0 must be multiples of 8 elements");
-  if (a_format != IVB_FP8_E4M3 && a_format != IVB_FP8_E5M2) return set_error("ivb_gemm_fp8: unknown a_format");
-  if (a_scale_inv == nullptr || b_scale_inv == nullptr) return set_error("ivb_gemm_fp8: scale_inv pointers are null");
-  const bool vec = (flags & IVB_FLAG_FP8_VECTOR_SCALES) != 0;
-  if (vec && a_format != IVB_FP8_E4M3) return set_error("ivb_gemm_fp8: vector scales need an E4M3 A operand");
-  if (vec && ((reinterpret_cast<uintptr_t>(a_scale_inv) | reinterpret_cast<uintptr_t>(b_scale_inv)) & 7))
-    return set_error("ivb_gemm_fp8: scale vectors must be 8-byte aligned");
-  if (int rc = check_epilogue_args("ivb_gemm_fp8", epilogue, out0, out1, ld1, aux, ldaux, bias, gamma)) return rc;
-  const bool force1 = (flags & IVB_FLAG_1CTA) != 0, forcepp = (flags & IVB_FLAG_PINGPONG) != 0;
-  if (flags & IVB_FLAG_2CTA) return set_error("ivb_gemm_fp8: no CTA-pair kernel");
-  if (force1 && forcepp) return set_error("ivb_gemm_fp8: IVB_FLAG_1CTA and IVB_FLAG_PINGPONG exclude each other");
-  if (tile_n != 0 && tile_n != 128 && tile_n != 192) return set_error("ivb_gemm_fp8: tile_n must be 0, 128 or 192");
-  if (forcepp && tile_n == 192) return set_error("ivb_gemm_fp8: the ping-pong kernel has tile_n 128");
-  GemmParams p = make_params(M, N, K, epilogue, flags, out0, ld0, out1, ld1, bias, gamma, aux, ldaux, rowscale);
-  p.a_scale_inv = a_scale_inv;
-  p.b_scale_inv = b_scale_inv;
-  const KernelChoice k = choose_kernel(M, N, K, flags, tile_n, true, false);
-  if (vec) return dispatch<OpVecFp8, false, false>(k, A, lda, B, ldb, p, stream);
-  if (a_format == IVB_FP8_E5M2) return dispatch<OpFp8<true>, false, false>(k, A, lda, B, ldb, p, stream);
-  return dispatch<OpFp8<false>, false, false>(k, A, lda, B, ldb, p, stream);
+                            void* stream) {
+  return gemm_fp8("ivb_gemm_fp8", A, a_mn_major, lda, a_format, a_scale_inv, B, b_mn_major, ldb, b_scale_inv, M, N, K,
+                  epilogue, flags, out0, ld0, out1, ld1, bias, gamma, aux, ldaux, rowscale, tile_n, nullptr,
+                  reinterpret_cast<cudaStream_t>(stream));
+}
+
+extern "C" int ivb_gemm_fp8_plan(const void* A, int a_mn_major, long lda, int a_format, const float* a_scale_inv,
+                                 const void* B, int b_mn_major, long ldb, const float* b_scale_inv, int M, int N, int K,
+                                 int epilogue, int flags, void* out0, long ld0, void* out1, long ld1, const void* bias,
+                                 const void* gamma, const void* aux, long ldaux, const float* rowscale, int tile_n,
+                                 const int* m_plan, void* stream) {
+  return gemm_fp8("ivb_gemm_fp8_plan", A, a_mn_major, lda, a_format, a_scale_inv, B, b_mn_major, ldb, b_scale_inv, M, N,
+                  K, epilogue, flags, out0, ld0, out1, ld1, bias, gamma, aux, ldaux, rowscale, tile_n, m_plan,
+                  reinterpret_cast<cudaStream_t>(stream));
 }

@@ -24,7 +24,7 @@ struct GemmParams {
   const float* rowscale;  // EPI_RESID: optional per-row multiplier of the branch (DropPath keep/scale)
   const float* a_scale_inv;  // fp8 operands: device scalars, the accumulator is multiplied by their product
   const float* b_scale_inv;
-  // DropPath plan (ivb_droppath_plan), bf16 single-CTA kernels only; null: every tile, every k-block.
+  // DropPath plan (ivb_droppath_plan), planned kernels only (PLANNED, ivb_gemm.cu); null: every tile, every k-block.
   // m_plan: the ceil(M/128) row tiles, live ones first, then their count; a dead tile runs dead_tile instead of its MMAs.
   // k_plan: the ascending live 64-row k-blocks, then their count; the k-blocks it leaves out are skipped.
   const int* m_plan;

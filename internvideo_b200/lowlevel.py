@@ -269,8 +269,18 @@ def gemm_fp8(a, a_scale_inv, b, b_scale_inv, *, epi=EPI_BF16, flags=0, out0=None
     transposed operand).  a_scale_inv / b_scale_inv: fp32 [1] CUDA tensors (per-tensor scales), or fp32 [M] and [N]
     vectors (per-row scales of a, per-output-channel scales of b, as fp8_quantize_rows / norm_fwd_fp8 give them; a
     must then be E4M3), which sets FLAG_FP8_VECTOR_SCALES.  Epilogue arguments as for gemm()."""
+    return _gemm_fp8_plan(a, a_scale_inv, b, b_scale_inv, None, epi=epi, flags=flags, out0=out0, out1=out1, bias=bias,
+                          gamma=gamma, aux=aux, rowscale=rowscale, tile_n=tile_n)
+
+
+def _gemm_fp8_plan(a, a_scale_inv, b, b_scale_inv, m_plan, *, epi=EPI_BF16, flags=0, out0=None, out1=None, bias=None,
+                   gamma=None, aux=None, rowscale=None, tile_n=0):
+    """gemm_fp8 with the M plan of a DropPath plan over its M rows (as for gemm(); vector scales only), through
+    ivb_gemm_fp8_plan, which skips the row tiles of the dropped rows; m_plan None: gemm_fp8 itself.  The block's
+    per-token FP8 path (ops.block_forward / block_backward) is its caller, as ops.droppath_plan is the plans' maker:
+    gemm_fp8, the public FP8 GEMM, stays the unplanned call."""
     _chk(("a", a, tuple(FP8_DTYPES.values())), ("a_scale_inv", a_scale_inv, f32), ("b", b, torch.float8_e4m3fn),
-         ("b_scale_inv", b_scale_inv, f32))
+         ("b_scale_inv", b_scale_inv, f32), ("m_plan?", m_plan, i32))
     lda = _rows2d(a, "a"); ldb = _rows2d(b, "b")
     M, K = a.shape
     N, Kb = b.shape
@@ -284,9 +294,10 @@ def gemm_fp8(a, a_scale_inv, b, b_scale_inv, *, epi=EPI_BF16, flags=0, out0=None
             raise _lib.IvbError(f"gemm_fp8: vector scales must be contiguous [M] = [{M}] and [N] = [{N}], got "
                                 f"{tuple(a_scale_inv.shape)} and {tuple(b_scale_inv.shape)}")
         flags |= FLAG_FP8_VECTOR_SCALES
-    _call("gemm_fp8", a, 0, lda, fmt, a_scale_inv, b, 0, ldb, b_scale_inv, M, N, K, epi, flags, out0,
-          _rows2d(out0, "out0"), out1, _rows2d(out1, "out1"), bias, gamma, aux, _rows2d(aux, "aux"), rowscale, tile_n,
-          kind="gemm", flops=2.0 * M * N * K)
+    plan = () if m_plan is None else (m_plan,)
+    _call("gemm_fp8_plan" if plan else "gemm_fp8", a, 0, lda, fmt, a_scale_inv, b, 0, ldb, b_scale_inv, M, N, K, epi,
+          flags, out0, _rows2d(out0, "out0"), out1, _rows2d(out1, "out1"), bias, gamma, aux, _rows2d(aux, "aux"),
+          rowscale, tile_n, *plan, kind="gemm", flops=2.0 * M * N * K)
     return out0
 
 
@@ -374,17 +385,22 @@ def colsum(x, out=None):
 
 
 # ----------------------------------------------------------------------------------------- attention
-def attn_fwd(q, k, v, B, n, H, d, scale, out=None, want_lse=True):
-    """q/k/v: 2-D views [B*n, H*d] (any row pitch) of the projection buffers."""
-    _chk(("q", q, bf16), ("k", k, bf16), ("v", v, bf16), ("out?", out, bf16))
+def attn_fwd(q, k, v, B, n, H, d, scale, out=None, want_lse=True, rowscale=None):
+    """q/k/v: 2-D views [B*n, H*d] (any row pitch) of the projection buffers.  rowscale: optional fp32 [B*n] DropPath
+    factors of the attention branch (one per clip): the call goes to ivb_attn_fwd_plan, which skips the clips whose
+    factor is 0 and writes zeros to their rows."""
+    _chk(("q", q, bf16), ("k", k, bf16), ("v", v, bf16), ("out?", out, bf16), ("rowscale?", rowscale, f32))
+    _chk_rowscale("attn_fwd", rowscale, B * n)
     for t, nm in ((q, "q"), (k, "k"), (v, "v")):
         if t.shape != (B * n, H * d):
             raise _lib.IvbError(f"attn_fwd: {nm} must be [B*n, H*d], got {tuple(t.shape)}")
     if out is None:
         out = torch.empty((B * n, H * d), device=q.device, dtype=bf16)
     lse = torch.empty((B, H, n), device=q.device, dtype=f32) if want_lse else None
-    _call("attn_fwd", q, _rows2d(q, "q"), k, _rows2d(k, "k"), v, _rows2d(v, "v"), out, _rows2d(out, "out"), lse,
-          B, n, H, d, float(scale), flops=4.0 * B * H * n * n * d)          # QK^T + PV
+    plan = () if rowscale is None else (rowscale,)
+    _call("attn_fwd_plan" if plan else "attn_fwd", q, _rows2d(q, "q"), k, _rows2d(k, "k"), v, _rows2d(v, "v"), out,
+          _rows2d(out, "out"), lse, B, n, H, d, float(scale), *plan, kind="attn_fwd",
+          flops=4.0 * B * H * n * n * d)          # QK^T + PV
     return out, lse
 
 
@@ -399,18 +415,28 @@ def headaxis_attn_fwd(qkv, B, N, H, d, scale):
     return out
 
 
-def attn_bwd(q, k, v, out, dout, lse, B, n, H, d, scale, dq, dk, dv):
-    """dq/dk/dv: preallocated bf16 2-D views [B*n, H*d] (e.g. the three slots of a [B*n, 3D] buffer)."""
+def attn_bwd(q, k, v, out, dout, lse, B, n, H, d, scale, dq, dk, dv, rowscale=None):
+    """dq/dk/dv: preallocated bf16 2-D views [B*n, H*d] (e.g. the three slots of a [B*n, 3D] buffer).  rowscale: the
+    forward's DropPath factors (attn_fwd): ivb_attn_bwd_plan writes zeros to the dropped clips' rows."""
     rows = (("q", q), ("k", k), ("v", v), ("out", out), ("dout", dout), ("dq", dq), ("dk", dk), ("dv", dv))
-    _chk(*((nm, t, bf16) for nm, t in rows), ("lse", lse, f32))
+    _chk(*((nm, t, bf16) for nm, t in rows), ("lse", lse, f32), ("rowscale?", rowscale, f32))
+    _chk_rowscale("attn_bwd", rowscale, B * n)
     for nm, t in rows:
         if t.shape != (B * n, H * d):
             raise _lib.IvbError(f"attn_bwd: {nm} must be [B*n, H*d], got {tuple(t.shape)}")
     delta = torch.empty((int(_lib.load().ivb_attn_bwd_workspace_floats(B, n, H)),), device=q.device, dtype=f32)
-    _call("attn_bwd", q, _rows2d(q, "q"), k, _rows2d(k, "k"), v, _rows2d(v, "v"), out, _rows2d(out, "out"), dout,
-          _rows2d(dout, "dout"), lse, delta, dq, _rows2d(dq, "dq"), dk, _rows2d(dk, "dk"), dv, _rows2d(dv, "dv"),
-          B, n, H, d, float(scale), flops=10.0 * B * H * n * n * d)  # algorithmic: 5 GEMMs (SURVEY §8d: 2.5x forward)
+    plan = () if rowscale is None else (rowscale,)
+    _call("attn_bwd_plan" if plan else "attn_bwd", q, _rows2d(q, "q"), k, _rows2d(k, "k"), v, _rows2d(v, "v"), out,
+          _rows2d(out, "out"), dout, _rows2d(dout, "dout"), lse, delta, dq, _rows2d(dq, "dq"), dk, _rows2d(dk, "dk"), dv,
+          _rows2d(dv, "dv"), B, n, H, d, float(scale), *plan, kind="attn_bwd",
+          flops=10.0 * B * H * n * n * d)  # algorithmic: 5 GEMMs (SURVEY §8d: 2.5x forward)
     return dq, dk, dv
+
+
+def _chk_rowscale(fn, rowscale, rows):
+    """The attention plan calls read rowscale[b*n] for every clip b: a contiguous fp32 [B*n]."""
+    if rowscale is not None and (rowscale.shape != (rows,) or not rowscale.is_contiguous()):
+        raise _lib.IvbError(f"{fn}: rowscale must be a contiguous [B*n] = [{rows}], got {tuple(rowscale.shape)}")
 
 
 # ----------------------------------------------------------------------------------------- token front-end

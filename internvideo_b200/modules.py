@@ -436,10 +436,11 @@ FP8_SCALINGS = {"tensor": ops.FP8_TENSOR, "token": ops.FP8_TOKEN}
 
 
 def set_droppath_skip(model: nn.Module, enabled: bool = True) -> int:
-    """Switch, in every PretrainInternVideo2 tower of `model`, whether a training step skips the GEMM work of the clips
-    its DropPath draw drops (on by default; ops.droppath_plan, ivb_gemm_bf16_plan).  Off runs every row, with the same
-    parameters and gradients; the switch is there to measure the two in one process.  Returns how many towers were
-    switched."""
+    """Switch, in every PretrainInternVideo2 tower of `model`, whether a training step skips the GEMM and attention work
+    of the clips its DropPath draw drops (on by default; ops.droppath_plan, ivb_gemm_bf16_plan, ivb_gemm_fp8_plan,
+    ivb_attn_fwd_plan / ivb_attn_bwd_plan), in bf16 and in per-token FP8 (set_fp8 with scaling="token"; per-tensor FP8
+    runs every row).  Off runs every row, with the same parameters and gradients; the switch is there to measure the two
+    in one process.  Returns how many towers were switched."""
     towers = [m for m in model.modules() if isinstance(m, PretrainInternVideo2)]
     for m in towers:
         m.droppath_skip = bool(enabled)

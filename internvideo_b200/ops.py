@@ -242,9 +242,12 @@ def droppath_plan(rowscale):
 
 def _branch_plans(plan, M, prec):
     """(M plan, K plan) of a branch's DropPath plan row for the block's GEMMs over its M rows: the M plan for a GEMM
-    whose M rows are the block's rows, the K plan for a weight gradient whose K runs over them.  (None, None) without
-    a plan or in FP8 (the FP8 GEMMs take none)."""
-    if plan is None or prec != BF16:
+    whose M rows are the block's rows (bf16, or FP8 with per-token scales), the K plan for a weight gradient whose K runs
+    over them (bf16 in both modes).  (None, None) without a plan or in FP8_TENSOR: there a dropped clip's rows still
+    count in each activation's and gradient's per-tensor amax, and skipping them would zero those rows and change the
+    scales, so every row runs.  In FP8_TOKEN each scale belongs to one row: a dropped row's zeros change only its own
+    (finite) scale, and it feeds only dead tiles or rows the epilogue multiplies by 0."""
+    if plan is None or prec not in (BF16, FP8_TOKEN):
         return None, None
     nm = (M + 127) // 128
     return plan[:nm + 1], plan[nm + 1:]
@@ -272,9 +275,10 @@ def block_forward(x, spec, p, rs1=None, rs2=None, save=True, plan1=None, plan2=N
     the backward needs (without save: the same E4M3 bits from the inference norm kernel).  Attention, the q/k norms and
     the residual stream stay as above.
 
-    plan1 / plan2: optional DropPath plans of the two branches (rows of droppath_plan of rs1 / rs2): the bf16 GEMMs
-    of a branch then skip the row tiles whose rows rs zeroes, writing what the epilogue table of ivb_gemm_bf16_plan
-    gives them (x1 = x, zeros elsewhere); the rows they do compute and x2 are as without a plan."""
+    plan1 / plan2: optional DropPath plans of the two branches (rows of droppath_plan of rs1 / rs2): in bf16 and
+    FP8_TOKEN the GEMMs of a branch then skip the row tiles whose rows rs zeroes, writing what the epilogue table of
+    ivb_gemm_bf16_plan gives them (x1 = x, zeros elsewhere), and attention skips the clips rs1 drops (a = 0 there);
+    the rows they do compute and x2 are as without a plan."""
     B, n, H = spec.B, spec.n, spec.H
     M, D = x.shape
     d = D // H
@@ -309,7 +313,7 @@ def block_forward(x, spec, p, rs1=None, rs2=None, save=True, plan1=None, plan2=N
             q, s = ll.fp8_quantize_rows(act) if torch.is_tensor(act) else act
         else:
             q, _, s, _ = ll.fp8_quantize(act, ll.FP8_E4M3)
-        return ll.gemm_fp8(q, s, w8[i][0], w8[i][1], **epilogue)
+        return ll._gemm_fp8_plan(q, s, w8[i][0], w8[i][1], mp[i // 2], **epilogue)
     n1_in, n1, mean1, rstd1 = norm(x, p.n1w, p.n1b, spec.eps1)
     qkv = linear(n1_in, 0, p.qkvw, bias=p.qkvb)
     q, k, v = qkv[:, :D], qkv[:, D:2 * D], qkv[:, 2 * D:]
@@ -327,7 +331,8 @@ def block_forward(x, spec, p, rs1=None, rs2=None, save=True, plan1=None, plan2=N
         # [B, H, N, d] result as [B, N, H*d]: reproduced bit-for-layout
         a = ll.headaxis_attn_fwd(qkv, B, n, H, d, spec.attn_scale(d)).reshape(M, D)
     else:
-        a, lse = ll.attn_fwd(q, k, v, B, n, H, d, spec.attn_scale(d), want_lse=save)
+        a, lse = ll.attn_fwd(q, k, v, B, n, H, d, spec.attn_scale(d), want_lse=save,
+                             rowscale=rs1 if mp[0] is not None else None)
     y1 = torch.empty((M, D), device=x.device, dtype=bf16) if (p.g1 is not None and save) else None
     x1 = linear(a, 1, p.projw, epi=ll.EPI_RESID, bias=p.projb, gamma=p.g1, aux=x, out1=y1, rowscale=rs1)
     n2_in, n2, mean2, rstd2 = norm(x1, p.n2w, p.n2b, spec.eps2)
@@ -349,8 +354,8 @@ def block_backward(x, s, spec, t, P, dx2, rs1, rs2, plan1=None, plan2=None):
     bias gradients and always runs the attention branch's LayerScale backward as its own call.  `t` are the block's
     tensors as autograd handed them back, `P` the nn.Parameter objects (gradient sink), both BlockParams.  Returns
     (dx0, BlockParams of gradients | None when the sink took them).  plan1 / plan2: the DropPath plans block_forward
-    ran with; the input-gradient GEMMs of a branch skip its dead row tiles (zeros) and its weight gradients the
-    64-row k-blocks of dropped rows, whose gradient rows layerscale_bwd made zero."""
+    ran with; the input-gradient GEMMs of a branch skip its dead row tiles (zeros), its weight gradients the
+    64-row k-blocks of dropped rows, whose gradient rows layerscale_bwd made zero, and attention the dropped clips."""
     B, n, H = spec.B, spec.n, spec.H
     M, D = x.shape
     d = D // H
@@ -381,7 +386,7 @@ def block_backward(x, s, spec, t, P, dx2, rs1, rs2, plan1=None, plan2=None):
             q, _, sc, _ = ll.fp8_quantize(dy, ll.FP8_E5M2)
         else:
             return ll.gemm(dy, w, b_t=True, m_plan=m_plan, **epilogue)
-        return ll.gemm_fp8(q, sc, w_t, w_s, **epilogue)
+        return ll._gemm_fp8_plan(q, sc, w_t, w_s, m_plan, **epilogue)
 
     def wgrad(dy, act, param, k_plan):
         if sink is None:
@@ -410,7 +415,7 @@ def block_backward(x, s, spec, t, P, dx2, rs1, rs2, plan1=None, plan2=None):
     dqkv = torch.empty((M, 3 * D), device=x.device, dtype=bf16)
     qk = s.qkn if s.qkn is not None else s.qkv
     ll.attn_bwd(qk[:, :D], qk[:, D:2 * D], s.qkv[:, 2 * D:], s.a, da, s.lse, B, n, H, d, spec.attn_scale(d),
-                dqkv[:, :D], dqkv[:, D:2 * D], dqkv[:, 2 * D:])
+                dqkv[:, :D], dqkv[:, D:2 * D], dqkv[:, 2 * D:], rowscale=rs1 if m1 is not None else None)
     if s.qkn is not None and s.rk is None:
         ll.rmsnorm_pair_bwd(dqkv, s.qkv, D, t.qnw, t.knw, s.rq, seg["qnw"], seg["knw"])
     elif s.qkn is not None:

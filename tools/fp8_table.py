@@ -100,11 +100,12 @@ def quant_table(iters):
           f"{tot_b / HBM * 1e3:.3f} ms)")
 
 
-def step_table(reps=3, steps=10, modes=("off", "tensor")):
-    """modes: "off" (bf16) or a set_fp8 scaling, each captured and timed once per repetition, in turn."""
+def step_table(reps=3, steps=10, modes=("off", "tensor"), skips=(True,)):
+    """modes: "off" (bf16) or a set_fp8 scaling; skips: the set_droppath_skip settings.  Each (mode, skip) pair is
+    captured and timed once per repetition, in turn."""
     import bench
     from internvideo_b200.engine import GraphedStep, PretrainEngine
-    from internvideo_b200.modules import PretrainInternVideo2, set_fp8
+    from internvideo_b200.modules import PretrainInternVideo2, set_droppath_skip, set_fp8
     print("\n3. cfg-2 step, B = 32, one CUDA graph per step (alternated)")
     cfg = dict(bench.CFGS["1B"])
     B = cfg.pop("batch")
@@ -136,10 +137,13 @@ def step_table(reps=3, steps=10, modes=("off", "tensor")):
         engine.step()
         return loss
 
-    res = {mode: [] for mode in modes}
+    runs = [(fp8, skip) for fp8 in modes for skip in skips]
+    label = {r: f"fp8={r[0]:6s}" + (f" skip={'on ' if r[1] else 'off'}" if len(skips) > 1 else "") for r in runs}
+    res = {r: [] for r in runs}
     for _ in range(reps):
-        for fp8 in modes:
+        for fp8, skip in runs:
             set_fp8(model, fp8 != "off", scaling="tensor" if fp8 == "off" else fp8)
+            set_droppath_skip(model, skip)
             gs = GraphedStep(step, [video, mask], warmup=1)
             gs(video, mask)
             torch.cuda.synchronize()
@@ -148,14 +152,14 @@ def step_table(reps=3, steps=10, modes=("off", "tensor")):
                 loss = gs(video, mask)
             torch.cuda.synchronize()
             ms = (time.perf_counter() - t0) * 1e3 / steps
-            res[fp8].append(ms)
-            print(f"  fp8={fp8:6s}  {ms:8.2f} ms/step  {B / ms * 1e3:7.2f} clips/s  loss {float(loss):.4f}")
+            res[(fp8, skip)].append(ms)
+            print(f"  {label[(fp8, skip)]}  {ms:8.2f} ms/step  {B / ms * 1e3:7.2f} clips/s  loss {float(loss):.4f}")
             del gs
             torch.cuda.empty_cache()
-    for fp8 in modes:
-        best = min(res[fp8])
-        print(f"fp8={fp8}: best {best:.2f} ms/step = {B / best * 1e3:.2f} clips/s "
-              f"(all: {', '.join(f'{x:.2f}' for x in res[fp8])})")
+    for r in runs:
+        best = min(res[r])
+        print(f"{label[r]}: best {best:.2f} ms/step = {B / best * 1e3:.2f} clips/s "
+              f"(all: {', '.join(f'{x:.2f}' for x in res[r])})")
 
 
 def main():
