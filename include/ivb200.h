@@ -27,11 +27,12 @@
  *     library, so the same inputs give the same bits on every run.  That scratch holds one reduction at a time:
  *     these entry points must not be called concurrently from two streams of the same device.
  *   - the row kernels (ivb_norm_fwd, ivb_norm_bwd, ivb_rmsnorm_pair_*, ivb_rmsnorm_bwd_layerscale, ivb_layerscale_bwd,
- *     ivb_colsum_bf16, ivb_ln_l2_*, ivb_l2norm_rows_*, ivb_pool_attn_*) move each row in 16-byte vectors: the row width
- *     and every pitch are multiples of 8 elements (the fp32 pitches of ivb_rmsnorm_bwd_layerscale: of 4), and every
- *     row or vector operand is 16-byte aligned (weight and gamma of ivb_rmsnorm_bwd_layerscale: 8-byte).  Per-row and
- *     per-column scalars (mean, rstd, stats, parameter gradients) need only their type's alignment.  A call that
- *     breaks one of these rules is refused before any CUDA call.
+ *     ivb_colsum_bf16, ivb_ln_l2_*, ivb_l2norm_rows_*, ivb_pool_attn_*, ivb_gather_add, ivb_scatter_add) move each row
+ *     in 16-byte vectors: the row width and every pitch (and clip stride) are multiples of 8 elements (the fp32
+ *     pitches of ivb_rmsnorm_bwd_layerscale: of 4), and every row or vector operand is 16-byte aligned (weight and
+ *     gamma of ivb_rmsnorm_bwd_layerscale: 8-byte).  ivb_im2col_visible moves 4-byte words: video and cols are 4-byte
+ *     aligned.  Per-row and per-column scalars (mean, rstd, stats, parameter gradients) and index lists need only
+ *     their type's alignment.  A call that breaks one of these rules is refused before any CUDA call.
  */
 #ifndef IVB200_H_
 #define IVB200_H_

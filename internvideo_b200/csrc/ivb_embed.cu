@@ -153,6 +153,7 @@ extern "C" int ivb_im2col_visible(const void* video, const int* idx, int idx_str
   if (B <= 0 || rows_per_clip <= 0) return 0;
   if ((patch & 1) || (W & 1) || (Kpad & 7) || Kpad < C * tubelet * patch * patch)
     return set_error("ivb_im2col_visible: patch/W must be even, Kpad a multiple of 8 and >= C*t*p*p");
+  if (misaligned(4, video, cols)) return set_error("ivb_im2col_visible: video and cols must be 4-byte aligned");
   const long rows = static_cast<long>(B) * rows_per_clip;
   const int wpb = 8;
   return launch("im2col_visible_kernel", im2col_visible_kernel, (unsigned)((rows + wpb - 1) / wpb), wpb * 32, 0, stream,
@@ -166,6 +167,9 @@ extern "C" int ivb_gather_add(const float* src, long src_bstride, const void* ta
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (B <= 0 || rows <= 0) return 0;
   if (D & 7) return set_error("ivb_gather_add: D must be a multiple of 8");
+  if ((src_bstride & 7) || (out_bstride & 7))
+    return set_error("ivb_gather_add: src_bstride and out_bstride must be multiples of 8");
+  if (misaligned(16, src, table, out)) return set_error("ivb_gather_add: src, table and out must be 16-byte aligned");
   const long total = static_cast<long>(B) * rows;
   const int wpb = 8;
   const unsigned grid = (unsigned)((total + wpb - 1) / wpb);
@@ -180,6 +184,8 @@ extern "C" int ivb_scatter_add(const void* g, int g_is_f32, long g_bstride, cons
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (B <= 0 || rows <= 0) return 0;
   if (D & 7) return set_error("ivb_scatter_add: D must be a multiple of 8");
+  if (g_bstride & 7) return set_error("ivb_scatter_add: g_bstride must be a multiple of 8");
+  if (misaligned(16, g, table_grad)) return set_error("ivb_scatter_add: g and table_grad must be 16-byte aligned");
   // One launch per clip, in clip order: the rows of one clip name distinct table rows, so every table row receives its
   // contributions in the same order on every run (one launch over all clips would add them in whatever order the
   // clips' warps arrive, and the table's AdamW update would differ from run to run).

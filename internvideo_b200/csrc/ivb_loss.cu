@@ -380,6 +380,9 @@ __global__ void l2norm_rows_bwd_kernel(const float* __restrict__ dy, long lddy, 
 // ---------------------------------------------------------------- IV1 pixel targets + MSE
 // One CTA (C warps) per masked patch: warp c normalises channel c over the tub*P*P pixels
 // (mean / unbiased variance, +1e-6 on the std), labels layout 'b n (p c)'.
+// The sums run over u - pivot, the pivot being the channel's first pixel of the patch: a flat patch then sums to
+// exactly 0 and gets the label 0, where raw sums of u leave a rounding residue that the 1e-6 guard amplifies ~10^6
+// times; a near-flat patch keeps its small differences instead of losing them to the cancellation of large sums.
 __global__ void pixel_target_kernel(const __nv_bfloat16* __restrict__ video, const int* __restrict__ midx,
                                     int n_mask, int B, int C, int T, int H, int W, int tub, int P,
                                     int normalize, const float* __restrict__ mean3, const float* __restrict__ std3,
@@ -394,29 +397,29 @@ __global__ void pixel_target_kernel(const __nv_bfloat16* __restrict__ video, con
   const int f = tok / (gh * gw), py = (tok / gw) % gh, px = tok % gw;
   const int npix = tub * P * P;
   const float mu_c = mean3[c], sd_c = std3[c];
-  float s = 0.f;
-  for (int i = lane; i < npix; i += 32) {
+  // un-normalised pixel i of the patch: one rounding, the same bits wherever it is evaluated
+  auto pixel = [&](int i) {
     const int dx = i % P, dy = (i / P) % P, dt = i / (P * P);
     const long src = (((static_cast<long>(b) * C + c) * T + (f * tub + dt)) * H + (py * P + dy)) * W + (px * P + dx);
-    s += __bfloat162float(video[src]) * sd_c + mu_c;
+    return fmaf(__bfloat162float(video[src]), sd_c, mu_c);
+  };
+  float* out = labels + static_cast<long>(row) * npix * C;
+  if (!normalize) {
+    for (int i = lane; i < npix; i += 32) out[static_cast<long>(i) * C + c] = pixel(i);
+    return;
   }
-  const float mean = warp_sum(s) / npix;
+  const float pivot = __shfl_sync(0xffffffffu, lane == 0 ? pixel(0) : 0.f, 0);
+  float s = 0.f;
+  for (int i = lane; i < npix; i += 32) s += pixel(i) - pivot;
+  const float mean = warp_sum(s) / npix;        // relative to the pivot
   float ss = 0.f;
   for (int i = lane; i < npix; i += 32) {
-    const int dx = i % P, dy = (i / P) % P, dt = i / (P * P);
-    const long src = (((static_cast<long>(b) * C + c) * T + (f * tub + dt)) * H + (py * P + dy)) * W + (px * P + dx);
-    const float d = __bfloat162float(video[src]) * sd_c + mu_c - mean;
+    const float d = (pixel(i) - pivot) - mean;
     ss += d * d;
   }
   const float var = warp_sum(ss) / (npix - 1);
   const float inv = 1.f / (sqrtf(var) + 1e-6f);
-  float* out = labels + static_cast<long>(row) * npix * C;
-  for (int i = lane; i < npix; i += 32) {
-    const int dx = i % P, dy = (i / P) % P, dt = i / (P * P);
-    const long src = (((static_cast<long>(b) * C + c) * T + (f * tub + dt)) * H + (py * P + dy)) * W + (px * P + dx);
-    const float u = __bfloat162float(video[src]) * sd_c + mu_c;
-    out[static_cast<long>(i) * C + c] = normalize ? (u - mean) * inv : u;
-  }
+  for (int i = lane; i < npix; i += 32) out[static_cast<long>(i) * C + c] = ((pixel(i) - pivot) - mean) * inv;
 }
 
 // Register-resident backward (C <= 256*NCH, bf16 upstream gradient / target): z and dout rows read once, all loads

@@ -1,4 +1,5 @@
-"""Token front-end, decoder-head, contrastive, pixel-target and AdamW kernels (gpu)."""
+"""Decoder-head, contrastive, pixel-target and AdamW kernels against the golden fixtures and the oracle (gpu).  The token
+front end is tested in test_embed_gpu.py."""
 from pathlib import Path
 
 import numpy as np
@@ -13,71 +14,6 @@ GOLD = Path(__file__).parent / "golden"
 
 def _rel(a, b):
     return ((a.float() - b.float()).norm() / (b.float().norm() + 1e-30)).item()
-
-
-def _mask(B, T, L, keep, seed):
-    g = torch.Generator().manual_seed(seed)
-    m = torch.ones(B, 1 + T * L, dtype=torch.bool); m[:, 0] = False
-    for b in range(B):
-        for t in range(T):
-            m[b, 1 + t * L + torch.randperm(L, generator=g)[:keep]] = False
-    return m
-
-
-@pytest.mark.parametrize("B,T,L,keep", [(2, 2, 16, 6), (32, 8, 256, 52), (3, 4, 256, 256), (1, 1, 196, 1)])
-def test_visible_indices_bit_exact(cuda_lib, B, T, L, keep):
-    ll = cuda_lib
-    mask = _mask(B, T, L, keep, 5)
-    idx, err = ll.visible_indices(mask.cuda(), 1 + T * keep)
-    assert int(err.item()) == 0
-    ref = restate.visible_indices(mask)
-    assert torch.equal(idx.cpu().to(torch.int64), ref)          # bit-exact index parity
-    _, err2 = ll.visible_indices(mask.cuda(), T * keep)          # wrong count must be flagged
-    assert int(err2.item()) != 0
-
-
-@pytest.mark.parametrize("tub,P,T,HW", [(1, 14, 4, 56), (2, 16, 4, 64)])
-def test_im2col_and_patch_embed(cuda_lib, tub, P, T, HW):
-    ll = cuda_lib
-    torch.manual_seed(0)
-    B, C, D = 2, 3, 128
-    L = (HW // P) ** 2
-    Tt = T // tub
-    x = torch.randn(B, C, T, HW, HW).to(torch.bfloat16)
-    mask = _mask(B, Tt, L, 5, 1)
-    n = 1 + Tt * 5
-    idx, _ = ll.visible_indices(mask.cuda(), n)
-    K = C * tub * P * P
-    Kpad = (K + 7) // 8 * 8
-    cols = ll.im2col_visible(x.cuda(), idx, 1, n - 1, tub, P, Kpad)
-    # oracle: all-token im2col then gather
-    w = (torch.randn(D, C, tub, P, P) * 0.05).to(torch.bfloat16)
-    b = torch.zeros(D)
-    full = restate.patch_embed(x.float(), w.float(), b, tub, P).reshape(B, Tt * L, D)
-    ridx = restate.visible_indices(mask)[:, 1:] - 1
-    ref = torch.gather(full, 1, ridx[:, :, None].expand(-1, -1, D)).reshape(B * (n - 1), D)
-    assert torch.equal(cols[:, K:].cpu(), torch.zeros(B * (n - 1), Kpad - K, dtype=torch.bfloat16))
-    wp = torch.zeros(D, Kpad, dtype=torch.bfloat16); wp[:, :K] = w.reshape(D, K)
-    out = ll.gemm(cols, wp.cuda(), epi=ll.EPI_F32)
-    assert _rel(out.cpu(), ref) < 1e-4
-
-
-def test_gather_scatter(cuda_lib):
-    ll = cuda_lib
-    B, n, D, N = 3, 7, 64, 20
-    src = torch.randn(B, n, D, device="cuda")
-    table = torch.randn(N, D, device="cuda").to(torch.bfloat16)
-    idx = torch.stack([torch.randperm(N)[:n].sort().values for _ in range(B)]).to(torch.int32).cuda()
-    out = torch.empty(B, n, D, device="cuda")
-    ll.gather_add(src, n * D, table, idx, n, 0, B, n, D, out, n * D)
-    ref = src + table.float()[idx.long()]
-    assert torch.allclose(out, ref, atol=1e-6)
-    outb = torch.empty(B, n - 1, D, device="cuda", dtype=torch.bfloat16)
-    ll.gather_add(src[:, 1:].reshape(-1), n * D, table, idx[:, 1:], n, -1, B, n - 1, D, outb, (n - 1) * D) if False else None
-    tg = torch.zeros(N, D, device="cuda")
-    ll.scatter_add(src, n * D, idx, n, 0, B, n, D, tg)
-    ref_tg = torch.zeros(N, D, device="cuda").index_add_(0, idx.long().flatten(), src.reshape(-1, D))
-    assert torch.allclose(tg, ref_tg, atol=1e-5)
 
 
 @pytest.mark.parametrize("M,C", [(50, 3200), (417, 1408), (9, 768), (130, 160)])

@@ -1,6 +1,7 @@
-"""The row-kernel entry points of ivb_norm.cu and ivb_loss.cu refuse a bad pitch or a misaligned row operand before any
-CUDA call (include/ivb200.h, Conventions), checked through the raw C ABI: each returns non-zero with its message in
-ivb_last_error().  The refused calls pass null or fake device addresses; were a check missing, the call would go on to
+"""The row-kernel entry points of ivb_norm.cu, ivb_loss.cu and ivb_embed.cu refuse a bad pitch or a misaligned row
+operand before any CUDA call (include/ivb200.h, Conventions), checked through the raw C ABI: each returns non-zero with
+its message in ivb_last_error().  ivb_gather_add and ivb_scatter_add move rows in 16-byte vectors like the norm kernels;
+ivb_im2col_visible moves 4-byte words, so its video and cols need 4-byte alignment.  The refused calls pass null or fake device addresses; were a check missing, the call would go on to
 launch a kernel on them, so those cases run only where no CUDA device is present."""
 import pytest
 import torch
@@ -83,6 +84,21 @@ def _pool_bwd(p, ld):
                                          p["dq"], p["dk"], D, p["dv"], D, None)
 
 
+def _gather_add(p, ld):
+    return _lib.load().ivb_gather_add(p["src"], ld.get("src_bstride", 0), p["table"], p["idx"], 197, -1, 2, 196, D,
+                                      p["out"], 1, ld.get("out_bstride", 197 * D), None)
+
+
+def _scatter_add(p, ld):
+    return _lib.load().ivb_scatter_add(p["g"], 0, ld.get("g_bstride", 196 * D), p["idx"], 197, -1, 2, 196, D,
+                                       p["table_grad"], None)
+
+
+def _im2col(p, ld):
+    return _lib.load().ivb_im2col_visible(p["video"], p["idx"], 197, 1, 40, 2, 3, 16, 224, 224, 2, 14, 1176, p["cols"],
+                                          None)
+
+
 # entry point: (call, its pointer operands, the row operands among them that must be 16-byte aligned)
 ENTRIES = {
     "ivb_norm_fwd": (_norm_fwd, "x weight bias y mean rstd", "x weight bias y"),
@@ -100,6 +116,9 @@ ENTRIES = {
     "ivb_l2norm_rows_bwd": (_l2n_bwd, "dy xn inv dx", "dy xn dx"),
     "ivb_pool_attn_fwd": (_pool_fwd, "q k v out probs", "k v"),
     "ivb_pool_attn_bwd": (_pool_bwd, "q k v probs dout dq dk dv", "k v dk dv"),
+    "ivb_gather_add": (_gather_add, "src table idx out", "src table out"),
+    "ivb_scatter_add": (_scatter_add, "g idx table_grad", "g table_grad"),
+    "ivb_im2col_visible": (_im2col, "video idx cols", ""),
 }
 ROW_OPERANDS = [(e, op) for e, (_, _, ops) in ENTRIES.items() for op in ops.split()]
 
@@ -130,15 +149,29 @@ def test_fused_layerscale_weight_gamma_need_8_bytes(operand):
 
 
 @no_device
+@pytest.mark.parametrize("operand", ["video", "cols"])
+def test_im2col_video_cols_need_4_bytes(operand):
+    """im2col_visible reads and writes 2 bf16 at a time: a view starting at an odd element is refused."""
+    _expect(_im2col(_ptrs("ivb_im2col_visible", **{operand: A + 2}), {}), "video and cols must be 4-byte aligned")
+
+
+# the refusal text of each entry point's pitch check (default: the norm and loss kernels')
+PITCH_TEXT = {"ivb_gather_add": "src_bstride and out_bstride must be multiples of 8",
+              "ivb_scatter_add": "g_bstride must be a multiple of 8"}
+
+
+@no_device
 @pytest.mark.parametrize("entry,pitch", [("ivb_norm_bwd", "lddx_in"), ("ivb_norm_bwd", "lddx"),
                                          ("ivb_ln_l2_fwd", "ldo"), ("ivb_ln_l2_fwd", "ldt"),
                                          ("ivb_layerscale_bwd", "ldy"), ("ivb_layerscale_bwd", "lddx"),
-                                         ("ivb_norm_fwd", "ldx"), ("ivb_colsum_bf16", "ldx")])
+                                         ("ivb_norm_fwd", "ldx"), ("ivb_colsum_bf16", "ldx"),
+                                         ("ivb_gather_add", "src_bstride"), ("ivb_gather_add", "out_bstride"),
+                                         ("ivb_scatter_add", "g_bstride")])
 @pytest.mark.parametrize("bad", [D + 4, D + 1])
 def test_bad_pitch_refused(entry, pitch, bad):
     call = ENTRIES[entry][0]
     _expect(call(_ptrs(entry), {pitch: bad}), f"{entry}: ")
-    assert "/ld must be multiples of 8" in _lib.load().ivb_last_error().decode()
+    assert PITCH_TEXT.get(entry, "/ld must be multiples of 8") in _lib.load().ivb_last_error().decode()
 
 
 def test_empty_is_a_noop():
@@ -148,3 +181,5 @@ def test_empty_is_a_noop():
     assert lib.ivb_norm_bwd(None, 3, None, 1, 3, None, None, None, 0, 0, 12, None, 3, None, 1, 3, None, None, None) == 0
     assert lib.ivb_layerscale_bwd(None, 3, None, 3, None, 0, 12, None, 3, None, None, None, None) == 0
     assert lib.ivb_ln_l2_fwd(None, 3, None, None, 1e-5, 0, 12, None, 3, None, None, 0, 3, None, None) == 0
+    assert lib.ivb_gather_add(None, 3, None, None, 0, 0, 0, 5, 12, None, 1, 3, None) == 0
+    assert lib.ivb_scatter_add(None, 1, 3, None, 0, 0, 0, 5, 12, None, None) == 0
