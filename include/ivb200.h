@@ -208,6 +208,40 @@ int ivb_gemm_fp8_plan(const void* A, int a_mn_major, long lda, int a_format, con
                       void* out0, long ld0, void* out1, long ld1, const void* bias, const void* gamma, const void* aux,
                       long ldaux, const float* rowscale, int tile_n, const int* m_plan, void* stream);
 
+/* ---- FP8 weight gradients with per-(128-token block, channel) scales (set_fp8 with wgrad=True) -------------------
+ * The weight gradient dW = dy^T act sums over tokens, so per-token scales cannot be factored out of it, and fp8 wgmma
+ * reads only K-major operands.  Both operands are therefore cast transposed, with one power-of-two scale per channel
+ * per 128-token block (the DeepSeek-V3 technical report's 1 x 128 tiles, 3.3), and the GEMM applies the scales of each
+ * 128-token k-block as it adds that k-block's partial sum to its fp32 accumulator.  Same bits on every run; capturable
+ * in a CUDA graph.  A call that breaks a rule below is refused before any CUDA call.
+ *
+ * ivb_fp8_quantize_blocks_t: x bf16 [M, C] (M tokens; pitch ldx, a multiple of 8; C a multiple of 8) -> out_t E4M3
+ *   [C, M] (pitch ldt, a multiple of 16 and >= M; row c holds channel c over all tokens) and scale_inv fp32
+ *   [ceil(M/128), C] (block-major: one k-block's scales are contiguous).  Block b's scale of channel c follows the
+ *   ivb_fp8_quantize_rows rule on amax(|x[128b : 128b + 128, c]|) (the last block may be partial: its own rows): a
+ *   power of two, 1 when the amax is 0, scale_inv NaN when the block holds an Inf or NaN.  Columns M .. ldt of out_t
+ *   are not written.  x and out_t are 16-byte aligned, scale_inv 4-byte.  One stream-ordered kernel.
+ * ivb_fp8_quantize_blocks_t_plan: the same with the DropPath factors rowscale fp32 [M] of the branch (required): a
+ *   token whose factor is 0 is cast as 0.  Its gradient row is 0, so it adds nothing to the weight gradient, and with
+ *   it zeroed no scale depends on values a DropPath plan may or may not have computed (ivb_attn_fwd_plan writes 0 where
+ *   ivb_attn_fwd writes the attention output).
+ * ivb_gemm_fp8_wgrad: out0[M, N] = sum_kb sum_{k in kb} A_t[m, k] B_t[n, k] * a_scale_inv[kb, m] * b_scale_inv[kb, n]
+ *   (+ out0 under IVB_FLAG_ACCUM) over the 128-element k-blocks kb.  A_t: E4M3 [M, K] (dy^T; pitch lda), B_t: E4M3
+ *   [N, K] (act^T; pitch ldb), both ivb_fp8_quantize_blocks_t outputs; lda, ldb multiples of 16 and >= K.
+ *   a_scale_inv [ceil(K/128), M] and b_scale_inv [ceil(K/128), N], 16-byte aligned.  M and N multiples of 8; epilogue
+ *   IVB_EPI_BF16 or IVB_EPI_F32 (out0 16-byte aligned, ld0 a multiple of 8), no bias; flags 0 or IVB_FLAG_ACCUM.  One
+ *   kernel form: the cooperative kernel (128 x 128 tiles) that promotes each k-block to fp32 on the CUDA cores.
+ *   k_plan (optional, NULL: every k-block): the 128-token k-blocks to sum, ascending, then their count at
+ *   k_plan[ceil(K/128)]: the M plan of a DropPath plan over the tokens (ivb_droppath_plan, plan + 0) as it is.  When
+ *   the left-out rows of dy are zero the result has the unplanned call's bits; with none listed the sum is 0.        */
+int ivb_fp8_quantize_blocks_t(const void* x, long ldx, int M, int C, void* out_t, long ldt, float* scale_inv,
+                              void* stream);
+int ivb_fp8_quantize_blocks_t_plan(const void* x, long ldx, int M, int C, void* out_t, long ldt, float* scale_inv,
+                                   const float* rowscale, void* stream);
+int ivb_gemm_fp8_wgrad(const void* A_t, long lda, const float* a_scale_inv, const void* B_t, long ldb,
+                       const float* b_scale_inv, int M, int N, int K, int epilogue, int flags, void* out0, long ld0,
+                       const int* k_plan, void* stream);
+
 /* ---- RMSNorm / LayerNorm (row reductions, HBM-bound) -------------------------------------------
  * y(bf16) = norm(x) * weight (+ bias).  is_layernorm=0: RMSNorm (internvideo2_pretrain.py:117-128,
  * FA2 DropoutAddRMSNorm :467; eps 1e-6); 1: nn.LayerNorm (eps 1e-5, :525,:532).

@@ -15,6 +15,11 @@
 // ivb_fp8_quantize_cols_t applies it to each column of a weight and writes the transposed copy (the input-gradient
 // GEMM's B operand, one scale per input channel): a column amax (integer atomicMax, order-independent), then the
 // cast kernel's 64 x 64 transposing tile with one scale per column.
+//
+// ivb_fp8_quantize_blocks_t applies it to each column of each 128-row block of activations or gradients [tokens, C]
+// and writes the transposed copy (the K-major operands of the FP8 weight gradient over tokens): one kernel, one read.
+#include <cstdio>
+
 #include "ivb_fp8.cuh"
 #include "ivb_internal.h"
 #include "ivb_rows.cuh"
@@ -251,9 +256,127 @@ __global__ void __launch_bounds__(R_THREADS) fp8_rows_kernel(const __nv_bfloat16
   }
 }
 
+// ------------------------------------------------------------------ per-(128-token block, channel) scaling
+// (ivb_fp8_quantize_blocks_t: the operands of the FP8 weight gradient, ivb_gemm_fp8_wgrad)
+// One CTA per 128 tokens x 64 channels: thread t reads the 8-channel chunk t % 8 of tokens t / 8, t / 8 + 32, ...
+// into registers (x is read once), the column amax goes through shuffles and shared memory (no atomics: the same bits
+// on every run), then each element is scaled by its column's factor, cast and transposed through shared memory, and
+// thread t writes 32 tokens of channel t / 4.  rowscale (optional): tokens whose factor is 0 are cast as zeros.
+constexpr int B_TOK = 128, B_CH = 64;
+constexpr int B_PITCH = B_TOK + 16;    // bytes per channel row of the transposing tile (16-byte aligned rows)
+
+__global__ void __launch_bounds__(Q_THREADS) fp8_blocks_t_kernel(const __nv_bfloat16* __restrict__ x, long ldx, int M,
+                                                                 int C, const float* __restrict__ rowscale,
+                                                                 uint8_t* __restrict__ out_t, long ldt,
+                                                                 float* __restrict__ scale_inv) {
+  __shared__ unsigned red[Q_THREADS / 32][B_CH];
+  __shared__ __align__(16) uint8_t tile[B_CH * B_PITCH];
+  pdl_wait();
+  pdl_launch_dependents();
+  const int m0 = blockIdx.y * B_TOK, c0 = blockIdx.x * B_CH;
+  const int cc = (threadIdx.x & 7) * 8, r0 = threadIdx.x >> 3;   // chunk column in the strip, first token
+  const int col = c0 + cc;
+  uint4 v[B_TOK / 32];
+  unsigned m[8] = {0u, 0u, 0u, 0u, 0u, 0u, 0u, 0u};   // bf16 magnitude bits: NaN > Inf > every finite value
+#pragma unroll
+  for (int i = 0; i < B_TOK / 32; ++i) {
+    const int row = m0 + r0 + 32 * i;
+    v[i] = make_uint4(0u, 0u, 0u, 0u);
+    if (row < M && col < C && (rowscale == nullptr || rowscale[row] != 0.0f))
+      v[i] = *reinterpret_cast<const uint4*>(x + static_cast<long>(row) * ldx + col);
+    const uint32_t w[4] = {v[i].x, v[i].y, v[i].z, v[i].w};
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      m[2 * k] = max(m[2 * k], w[k] & 0x7fffu);
+      m[2 * k + 1] = max(m[2 * k + 1], (w[k] >> 16) & 0x7fffu);
+    }
+  }
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {   // lanes l, l ^ 8, l ^ 16, l ^ 24 hold the same chunk
+    m[k] = max(m[k], __shfl_xor_sync(0xffffffffu, m[k], 8));
+    m[k] = max(m[k], __shfl_xor_sync(0xffffffffu, m[k], 16));
+  }
+  const int lane = threadIdx.x & 31;
+  if (lane < 8) {
+#pragma unroll
+    for (int k = 0; k < 8; ++k) red[threadIdx.x >> 5][lane * 8 + k] = m[k];
+  }
+  __syncthreads();
+  float scale[8];
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    unsigned mx = 0;
+#pragma unroll
+    for (int w = 0; w < Q_THREADS / 32; ++w) mx = max(mx, red[w][cc + k]);
+    float sinv;
+    fp8_scale(mx << 16, 8, scale[k], sinv);
+    if (r0 == 0 && col < C) scale_inv[static_cast<long>(blockIdx.y) * C + col + k] = sinv;
+  }
+#pragma unroll
+  for (int i = 0; i < B_TOK / 32; ++i) {
+    float f[8];
+    unpack8(v[i], f);
+#pragma unroll
+    for (int k = 0; k < 8; k += 2) {
+      const uint32_t q = cvt_fp8x2<false>(f[k] * scale[k], f[k + 1] * scale[k + 1]);
+      tile[(cc + k) * B_PITCH + r0 + 32 * i] = static_cast<uint8_t>(q);
+      tile[(cc + k + 1) * B_PITCH + r0 + 32 * i] = static_cast<uint8_t>(q >> 8);
+    }
+  }
+  __syncthreads();
+  // out_t row c0 + t / 4 holds channel c0 + t / 4: tokens m0 + 32 (t % 4) .. + 31
+  const int trow = c0 + (threadIdx.x >> 2), tok = 32 * (threadIdx.x & 3);
+  const int tn = trow < C ? min(32, M - m0 - tok) : 0;
+  if (tn <= 0) return;
+  const uint8_t* src = tile + (threadIdx.x >> 2) * B_PITCH + tok;
+  uint8_t* dst = out_t + static_cast<long>(trow) * ldt + m0 + tok;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    if (tn >= 16 * (h + 1)) {
+      reinterpret_cast<uint4*>(dst)[h] = reinterpret_cast<const uint4*>(src)[h];
+    } else {
+      for (int k = 16 * h; k < tn; ++k) dst[k] = src[k];
+    }
+  }
+}
+
 }  // namespace ivb
 
 using namespace ivb;
+
+// ivb_fp8_quantize_blocks_t and ivb_fp8_quantize_blocks_t_plan; `fn` names the entry point in messages.
+static int quantize_blocks_t(const char* fn, const void* x, long ldx, int M, int C, void* out_t, long ldt,
+                             float* scale_inv, const float* rowscale, cudaStream_t stream) {
+  char msg[128];
+  auto fail = [&](const char* what) {
+    std::snprintf(msg, sizeof(msg), "%s: %s", fn, what);
+    return set_error(msg);
+  };
+  if (M <= 0 || C <= 0) return fail("empty tensor");
+  if (C & 7) return fail("C must be a multiple of 8");
+  if (x == nullptr || out_t == nullptr || scale_inv == nullptr) return fail("x, out_t or scale_inv is null");
+  if ((ldx & 7) || ldx < C) return fail("ldx must be a multiple of 8 elements and >= C");
+  if ((ldt & 15) || ldt < M) return fail("ldt must be a multiple of 16 elements and >= M");
+  if (misaligned(16, x, out_t)) return fail("x and out_t must be 16-byte aligned");
+  if (misaligned(4, scale_inv, rowscale)) return fail("scale_inv and rowscale must be 4-byte aligned");
+  const dim3 grid((C + B_CH - 1) / B_CH, (M + B_TOK - 1) / B_TOK);
+  return launch("fp8_blocks_t_kernel", fp8_blocks_t_kernel, grid, Q_THREADS, 0, stream, ALLOW_PDL,
+                reinterpret_cast<const __nv_bfloat16*>(x), ldx, M, C, rowscale, reinterpret_cast<uint8_t*>(out_t), ldt,
+                scale_inv);
+}
+
+extern "C" int ivb_fp8_quantize_blocks_t(const void* x, long ldx, int M, int C, void* out_t, long ldt,
+                                         float* scale_inv, void* stream) {
+  return quantize_blocks_t("ivb_fp8_quantize_blocks_t", x, ldx, M, C, out_t, ldt, scale_inv, nullptr,
+                           reinterpret_cast<cudaStream_t>(stream));
+}
+
+extern "C" int ivb_fp8_quantize_blocks_t_plan(const void* x, long ldx, int M, int C, void* out_t, long ldt,
+                                              float* scale_inv, const float* rowscale, void* stream) {
+  if (rowscale == nullptr) return set_error("ivb_fp8_quantize_blocks_t_plan: rowscale is null");
+  return quantize_blocks_t("ivb_fp8_quantize_blocks_t_plan", x, ldx, M, C, out_t, ldt, scale_inv, rowscale,
+                           reinterpret_cast<cudaStream_t>(stream));
+}
 
 extern "C" int ivb_fp8_quantize_rows(const void* x, long ldx, int M, int K, void* out, long ldo, float* row_scale_inv,
                                      void* stream_) {

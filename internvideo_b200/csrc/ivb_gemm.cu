@@ -28,6 +28,11 @@
 // each 128-element k-block goes into a fresh register tile, which the CUDA cores add to the fp32 accumulator.
 // Vector scales (IVB_FLAG_FP8_VECTOR_SCALES, Op = OpVecFp8): a_scale_inv[M] per row and b_scale_inv[N] per column;
 // the same in-place dequantisation multiplies each accumulator by its row's and its column's factor.
+// Block scales (ivb_gemm_fp8_wgrad, Op = OpBlockFp8: the weight gradient over tokens, DeepSeek-V3 technical report
+// 3.3): one scale per row and per column of each 128-element k-block, a_scale_inv [ceil(K/128), M] and b_scale_inv
+// [ceil(K/128), N].  They cannot be factored out of the k sum, so the cooperative kernel applies them where it
+// promotes: acc += part * a_s[row] * b_s[col] per k-block.  The producer copies a k-block's 128 row and BN column
+// scales into the ring stage with its operands, under the stage's full barrier.
 //
 // Ping-pong form (gemm_bf16_pingpong_kernel, the default for most shapes, see use_pingpong): same producer, ring and
 // epilogue, but each MMA warpgroup owns a whole 128 x 128 tile and the two alternate, so one runs its epilogue while
@@ -40,7 +45,8 @@
 //
 // DropPath plans (ivb_gemm_bf16_plan: bf16 single-CTA kernels; ivb_gemm_fp8_plan: the OpPlannedFp8 instantiations of
 // both FP8 forms): an M plan puts the row tiles holding a kept row first, and the tiles after its live count only store
-// (dead_tile); a K plan lists the k-blocks the weight gradient sums.
+// (dead_tile); a K plan lists the k-blocks the weight gradient sums (ivb_gemm_bf16_plan, and ivb_gemm_fp8_wgrad with
+// 128-token k-blocks).
 //
 // Both kernels are built from the same pieces (gemm_prologue, produce, mma_kblock, dequantise, epilogue_tile) and keep
 // only how their MMA warpgroups consume and release the ring: FP8 promotion and the CTA pair's remote arrivals in the
@@ -64,30 +70,39 @@ constexpr int EPI_BYTES = 8 * 16 * EPI_PITCH * 4;  // one 16 x 32 fp32 staging t
 // PLAN: the single-CTA kernels are built with the DropPath plan code (PLANNED); OpPlannedFp8 is OpVecFp8 with it, so
 // ivb_gemm_fp8 keeps kernels without it.
 struct OpBf16 {
-  static constexpr bool FP8 = false, VEC = false, PLAN = true;
+  static constexpr bool FP8 = false, VEC = false, PLAN = true, BLOCK = false;
   static constexpr int BK = 64;
 };
 template <bool A_E5M2_>
 struct OpFp8 {
-  static constexpr bool FP8 = true, A_E5M2 = A_E5M2_, VEC = false, PLAN = false;
+  static constexpr bool FP8 = true, A_E5M2 = A_E5M2_, VEC = false, PLAN = false, BLOCK = false;
   static constexpr int BK = 128;
 };
 struct OpVecFp8 {
-  static constexpr bool FP8 = true, A_E5M2 = false, VEC = true, PLAN = false;
+  static constexpr bool FP8 = true, A_E5M2 = false, VEC = true, PLAN = false, BLOCK = false;
   static constexpr int BK = 128;
 };
 struct OpPlannedFp8 : OpVecFp8 {
   static constexpr bool PLAN = true;
 };
+// BLOCK: per-k-block row and column scales (E4M3 A), applied as each k-block is promoted; built with the plan code for
+// its K plan.
+struct OpBlockFp8 {
+  static constexpr bool FP8 = true, A_E5M2 = false, VEC = false, PLAN = true, BLOCK = true;
+  static constexpr int BK = 128;
+};
 
-template <int BN, bool B_MN>
+// SCALES (OpBlockFp8): each stage also holds its k-block's BM row and BN column scales, after the barriers.
+template <int BN, bool B_MN, bool SCALES = false>
 struct GemmCfg {
   static constexpr int B_ATOMS = (BN + 63) / 64;
   static constexpr int B_STAGE_BYTES = B_MN ? B_ATOMS * 64 * 128 : BN * 128;
   static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
-  static constexpr int STAGES_RAW = (227 * 1024 - EPI_BYTES - 1024 - 256) / STAGE_BYTES;
+  static constexpr int SCALE_FLOATS = SCALES ? BM + BN : 0;
+  static constexpr int STAGES_RAW = (227 * 1024 - EPI_BYTES - 1024 - 256) / (STAGE_BYTES + 4 * SCALE_FLOATS);
   static constexpr int STAGES = STAGES_RAW > 8 ? 8 : STAGES_RAW;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + EPI_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+  static constexpr int SMEM_BYTES = STAGES * (STAGE_BYTES + 4 * SCALE_FLOATS) + EPI_BYTES + 1024 /*align slack*/ +
+                                    256 /*barriers*/;
 };
 
 // ------------------------------------------------------------------ epilogue of one warpgroup's accumulators
@@ -197,12 +212,40 @@ __device__ __forceinline__ void dequantise(const GemmParams& p, float (&acc)[NH]
           acc[h][4 * j + 2 * q + 1] *= ra[h][q] * cb.y;
         }
     }
-  } else if constexpr (Op::FP8) {
+  } else if constexpr (Op::FP8 && !Op::BLOCK) {   // block scales were applied as each k-block was promoted
 #pragma unroll
     for (int h = 0; h < NH; ++h)
 #pragma unroll
       for (int i = 0; i < BN / 2; ++i) acc[h][i] *= dq;
   }
+}
+
+// Block scales: one k-block's partial sums, times their row's and column's scale of that k-block (read from the ring
+// stage before it is released: rows row0 .. row0 + 63 of this warpgroup, fragment layout as in dequantise), added to
+// the fp32 accumulator.
+template <int BN>
+struct BlockScales {
+  float ra[2];
+  float2 cb[BN / 8];
+};
+template <int BN>
+__device__ __forceinline__ void load_block_scales(BlockScales<BN>& bs, const float* sc, int row0) {
+  const int lane = threadIdx.x & 31;
+  const int r = row0 + ((threadIdx.x >> 5) & 3) * 16 + (lane >> 2);
+  bs.ra[0] = sc[r];
+  bs.ra[1] = sc[r + 8];
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) bs.cb[j] = *reinterpret_cast<const float2*>(sc + BM + 8 * j + 2 * (lane & 3));
+}
+template <int BN>
+__device__ __forceinline__ void promote_block(float (&acc)[BN / 2], const float (&part)[BN / 2], const BlockScales<BN>& bs) {
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+    for (int q = 0; q < 2; ++q) {
+      acc[4 * j + 2 * q] = fmaf(part[4 * j + 2 * q], bs.ra[q] * bs.cb[j].x, acc[4 * j + 2 * q]);
+      acc[4 * j + 2 * q + 1] = fmaf(part[4 * j + 2 * q + 1], bs.ra[q] * bs.cb[j].y, acc[4 * j + 2 * q + 1]);
+    }
 }
 
 // ------------------------------------------------------------------ pieces of both kernels
@@ -214,13 +257,14 @@ struct Smem {
   float* epi;
   uint64_t* full;
   uint64_t* empty;
+  float* scales;   // SCALES: STAGES x (BM row + BN column) scales
 };
 
 // Carves up shared memory, initialises the barriers and waits for the previous kernel (PDL).  `empty_arrivals`: the
 // releases a stage waits for before the producer refills it.
-template <int BN, bool B_MN, int CL>
+template <int BN, bool B_MN, int CL, bool SCALES = false>
 __device__ __forceinline__ Smem gemm_prologue(const CUtensorMap& tmA, const CUtensorMap& tmB, uint32_t empty_arrivals) {
-  using Cfg = GemmCfg<BN, B_MN>;
+  using Cfg = GemmCfg<BN, B_MN, SCALES>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
@@ -230,6 +274,7 @@ __device__ __forceinline__ Smem gemm_prologue(const CUtensorMap& tmA, const CUte
   s.epi = reinterpret_cast<float*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES);
   s.full = reinterpret_cast<uint64_t*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES + EPI_BYTES);
   s.empty = s.full + Cfg::STAGES;
+  s.scales = reinterpret_cast<float*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES + EPI_BYTES + 256);
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
@@ -255,9 +300,9 @@ struct PlanCounts {
 // Only the single-CTA kernels of an Op with PLAN are built with the plan code (PLANNED).
 template <class Op, int CL>
 constexpr bool PLANNED = Op::PLAN && CL == 1;
-// K plans only for bf16: FP8 operands are K-major, so an FP8 GEMM is never the weight gradient over tokens.
+// K plans for bf16 and for the block-scaled FP8 weight gradient (over tokens; its K plan lists 128-token k-blocks).
 template <class Op, int CL>
-constexpr bool K_PLANNED = PLANNED<Op, CL> && !Op::FP8;
+constexpr bool K_PLANNED = PLANNED<Op, CL> && (!Op::FP8 || Op::BLOCK);
 
 template <class Op, int BN, int CL>
 __device__ __forceinline__ PlanCounts plan_counts(const GemmParams& p) {
@@ -282,7 +327,7 @@ template <class Op, int BN, bool A_MN, bool B_MN, int CL>
 __device__ __forceinline__ void produce(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p,
                                         const Smem& s, int first_tile, int stride, int num_tiles, int num_kb,
                                         uint32_t rank) {
-  using Cfg = GemmCfg<BN, B_MN>;
+  using Cfg = GemmCfg<BN, B_MN, Op::BLOCK>;
   const int num_n = (p.N + BN - 1) / BN;
   int stage = 0;
   uint32_t phase = 0;
@@ -292,7 +337,10 @@ __device__ __forceinline__ void produce(const CUtensorMap& tmA, const CUtensorMa
     for (int i = 0; i < num_kb; ++i) {
       const int kb = K_PLANNED<Op, CL> && p.k_plan != nullptr ? p.k_plan[i] : i;
       mbar_wait(&s.empty[stage], phase ^ 1);
-      mbar_expect_tx(&s.full[stage], Cfg::STAGE_BYTES);
+      // block scales: the rows and columns inside the matrix (M, N multiples of 8: whole 16-byte pieces)
+      const uint32_t a_sbytes = Op::BLOCK ? 4u * min(BM, p.M - m0) : 0u;
+      const uint32_t b_sbytes = Op::BLOCK ? 4u * min(BN, p.N - n0) : 0u;
+      mbar_expect_tx(&s.full[stage], Cfg::STAGE_BYTES + a_sbytes + b_sbytes);
       uint8_t* sa = s.a + stage * A_STAGE_BYTES;
       uint8_t* sb = s.b + stage * Cfg::B_STAGE_BYTES;
       const int k0 = kb * Op::BK;
@@ -320,6 +368,11 @@ __device__ __forceinline__ void produce(const CUtensorMap& tmA, const CUtensorMa
             if ((i & 1) == static_cast<int>(rank))
               tma_load_2d_mc(sb + i * 8192, &tmB, n0 + i * 64, k0, &s.full[stage], 0x3);
         }
+      }
+      if constexpr (Op::BLOCK) {
+        float* sc = s.scales + stage * Cfg::SCALE_FLOATS;
+        bulk_load_1d(sc, p.a_scale_inv + static_cast<long>(kb) * p.M + m0, a_sbytes, &s.full[stage]);
+        bulk_load_1d(sc + BM, p.b_scale_inv + static_cast<long>(kb) * p.N + n0, b_sbytes, &s.full[stage]);
       }
       if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
     }
@@ -359,7 +412,8 @@ template <class Op, int BN, bool A_MN, bool B_MN, int CL>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                  const GemmParams p) {
-  constexpr int STAGES = GemmCfg<BN, B_MN>::STAGES;
+  using Cfg = GemmCfg<BN, B_MN, Op::BLOCK>;
+  constexpr int STAGES = Cfg::STAGES;
   const int warp = threadIdx.x >> 5;
   const int wg = threadIdx.x >> 7;
 
@@ -370,7 +424,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   const int num_tiles = num_m * num_n;
   constexpr bool PROMOTE = Op::FP8;
 
-  const Smem s = gemm_prologue<BN, B_MN, CL>(tmA, tmB, 2 * CL);   // one arrival per MMA warpgroup of the cluster
+  const Smem s = gemm_prologue<BN, B_MN, CL, Op::BLOCK>(tmA, tmB, 2 * CL);   // one arrival per MMA warpgroup of the cluster
   const PlanCounts pc = plan_counts<Op, BN, CL>(p);
   const int num_kb = pc.num_kb;
 
@@ -389,7 +443,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     };
     float* st = s.epi + (warp - 4) * 16 * EPI_PITCH;
     float dq = 1.0f;
-    if constexpr (Op::FP8 && !Op::VEC) dq = *p.a_scale_inv * *p.b_scale_inv;
+    if constexpr (Op::FP8 && !Op::VEC && !Op::BLOCK) dq = *p.a_scale_inv * *p.b_scale_inv;
     float acc[1][BN / 2];
     float part[1][PROMOTE ? BN / 2 : 1];
     int stage = 0;
@@ -410,11 +464,20 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         mbar_wait(&s.full[stage], phase);
         if constexpr (PROMOTE) {  // this k-block's partial sum, added in fp32; its smem slot is free
           mma_kblock<Op, BN, A_MN, B_MN, 1>(part, s, stage, cw, false);
-          wgmma_wait<0>();
-          wgmma_reg_fence(part[0], BN / 2);
-          release(stage);
+          if constexpr (Op::BLOCK) {   // the k-block's scales, read while its MMAs run
+            BlockScales<BN> bs;
+            load_block_scales<BN>(bs, s.scales + stage * Cfg::SCALE_FLOATS, cw * 64);
+            wgmma_wait<0>();
+            wgmma_reg_fence(part[0], BN / 2);
+            release(stage);
+            promote_block<BN>(acc[0], part[0], bs);
+          } else {
+            wgmma_wait<0>();
+            wgmma_reg_fence(part[0], BN / 2);
+            release(stage);
 #pragma unroll
-          for (int i = 0; i < BN / 2; ++i) acc[0][i] += part[0][i];
+            for (int i = 0; i < BN / 2; ++i) acc[0][i] += part[0][i];
+          }
         } else {
           mma_kblock<Op, BN, A_MN, B_MN, 1>(acc, s, stage, cw, kb > 0);
           if (kb > 0) {  // the MMAs of the previous k-block retired: its smem slot is free
@@ -522,7 +585,7 @@ constexpr auto gemm_kernel() {
 template <class Op, bool PINGPONG, int BN, bool A_MN, bool B_MN, int CL>
 static int launch_gemm(const void* A, long lda, const void* B, long ldb, const GemmParams& p,
                        cudaStream_t stream) {
-  using Cfg = GemmCfg<BN, B_MN>;
+  using Cfg = GemmCfg<BN, B_MN, Op::BLOCK && !PINGPONG>;
   constexpr int EB = Op::FP8 ? 1 : 2;
   CUtensorMap tmA, tmB;
   int rc;
@@ -637,7 +700,8 @@ static KernelChoice choose_kernel(int M, int N, int K, int flags, int tile_n, bo
 // The kernel k names, for operands of format Op and majors A_MN / B_MN.  Together with the entry points' choice of Op
 // and majors this instantiates the library's 38 kernels: the ping-pong kernel of every Op and major; the bf16
 // cooperative kernel at BN 256 / 192 / 176 / 128 and CL 1 or 2; the FP8 one (K-major only) at BN 192 or 128, CL 1,
-// and with a plan (OpPlannedFp8) at BN 128 only.
+// and with a plan (OpPlannedFp8) at BN 128 only.  ivb_gemm_fp8_wgrad adds the 39th, the block-scaled cooperative
+// kernel (OpBlockFp8) at BN 128, which it launches itself.
 template <class Op, bool A_MN, bool B_MN>
 static int dispatch(const KernelChoice& k, const void* A, long lda, const void* B, long ldb, const GemmParams& p,
                     cudaStream_t stream) {
@@ -785,4 +849,32 @@ extern "C" int ivb_gemm_fp8_plan(const void* A, int a_mn_major, long lda, int a_
   return gemm_fp8("ivb_gemm_fp8_plan", A, a_mn_major, lda, a_format, a_scale_inv, B, b_mn_major, ldb, b_scale_inv, M, N,
                   K, epilogue, flags, out0, ld0, out1, ld1, bias, gamma, aux, ldaux, rowscale, tile_n, m_plan,
                   reinterpret_cast<cudaStream_t>(stream));
+}
+
+// The weight gradient over tokens from block-scaled E4M3 operands (ivb_fp8_quantize_blocks_t's transposed copies): the
+// promoting cooperative kernel at BN = 128 with OpBlockFp8, with or without a K plan.
+extern "C" int ivb_gemm_fp8_wgrad(const void* A_t, long lda, const float* a_scale_inv, const void* B_t, long ldb,
+                                  const float* b_scale_inv, int M, int N, int K, int epilogue, int flags, void* out0,
+                                  long ld0, const int* k_plan, void* stream) {
+  const char* fn = "ivb_gemm_fp8_wgrad";
+  char msg[128];
+  auto fail = [&](const char* what) {
+    std::snprintf(msg, sizeof(msg), "%s: %s", fn, what);
+    return set_error(msg);
+  };
+  if (M <= 0 || N <= 0 || K <= 0) return fail("empty problem");
+  if (A_t == nullptr || B_t == nullptr) return fail("A_t or B_t is null");
+  if ((lda & 15) || (ldb & 15) || lda < K || ldb < K) return fail("lda and ldb must be multiples of 16 elements and >= K");
+  if ((M & 7) || (N & 7)) return fail("M and N must be multiples of 8");
+  if ((ld0 & 7) || ld0 < N) return fail("ld0 must be a multiple of 8 elements and >= N");
+  if (a_scale_inv == nullptr || b_scale_inv == nullptr) return fail("scale_inv pointers are null");
+  if (misaligned(16, a_scale_inv, b_scale_inv)) return fail("scale vectors must be 16-byte aligned");
+  if (epilogue != IVB_EPI_BF16 && epilogue != IVB_EPI_F32) return fail("epilogue must be IVB_EPI_BF16 or IVB_EPI_F32");
+  if (flags & ~IVB_FLAG_ACCUM) return fail("the only flag is IVB_FLAG_ACCUM (one kernel form: cooperative, 1 CTA)");
+  if (int rc = check_epilogue_args(fn, epilogue, out0, nullptr, 0, nullptr, 0, nullptr, nullptr)) return rc;
+  GemmParams p = make_params(M, N, K, epilogue, flags, out0, ld0, nullptr, 0, nullptr, nullptr, nullptr, 0, nullptr);
+  p.a_scale_inv = a_scale_inv;
+  p.b_scale_inv = b_scale_inv;
+  p.k_plan = k_plan;
+  return launch_gemm<OpBlockFp8, false, 128, false, false, 1>(A_t, lda, B_t, ldb, p, reinterpret_cast<cudaStream_t>(stream));
 }

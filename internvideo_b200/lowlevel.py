@@ -301,6 +301,48 @@ def _gemm_fp8_plan(a, a_scale_inv, b, b_scale_inv, m_plan, *, epi=EPI_BF16, flag
     return out0
 
 
+def _fp8_quantize_blocks_t(x, rowscale=None):
+    """Transposing cast of a bf16 [M, C] tensor of M tokens (any row pitch) to E4M3 with one power-of-two scale per
+    channel per 128-token block (ivb_fp8_quantize_blocks_t): the operands of the FP8 weight gradient, _gemm_fp8_wgrad.
+
+    Returns (q_t [C, M] float8_e4m3fn, scale_inv fp32 [ceil(M/128), C]): x[128b + i, c] ~ q_t[c, 128b + i] *
+    scale_inv[b, c].  q_t is a view of a buffer whose row pitch is rounded up to 16 elements.  rowscale: optional fp32
+    [M] DropPath factors (ivb_fp8_quantize_blocks_t_plan): tokens whose factor is 0 are cast as zeros.  Private, as
+    _gemm_fp8_plan: the block backward's FP8 weight gradients (ops.block_backward) are its caller."""
+    _chk(("x", x, bf16), ("rowscale?", rowscale, f32))
+    ldx = _rows2d(x, "x")
+    M, C = x.shape
+    _chk_rowscale("fp8_quantize_blocks_t", rowscale, M)
+    q_t = torch.empty((C, _pad16(M)), device=x.device, dtype=torch.float8_e4m3fn)[:, :M]
+    sinv = torch.empty(((M + 127) // 128, C), device=x.device, dtype=f32)
+    plan = () if rowscale is None else (rowscale,)
+    _call("fp8_quantize_blocks_t_plan" if plan else "fp8_quantize_blocks_t", x, ldx, M, C, q_t, q_t.stride(0), sinv,
+          *plan, kind="fp8_quantize")
+    return q_t, sinv
+
+
+def _gemm_fp8_wgrad(a_t, a_scale_inv, b_t, b_scale_inv, *, epi=EPI_BF16, flags=0, out0=None, k_plan=None):
+    """The weight gradient D[M, N] = sum over tokens k of dy[k, m] act[k, n] on the FP8 tensor cores from the
+    block-scaled transposed copies _fp8_quantize_blocks_t makes (ivb_gemm_fp8_wgrad): a_t = dy^T [M, K] with a_scale_inv
+    [ceil(K/128), M], b_t = act^T [N, K] with b_scale_inv [ceil(K/128), N].  epi EPI_BF16 or EPI_F32; flags 0 or
+    FLAG_ACCUM (accumulate into out0).  k_plan: optional list of the 128-token k-blocks to sum, in the format of a
+    DropPath plan's M plan over the tokens (ops._branch_plans)."""
+    _chk(("a_t", a_t, torch.float8_e4m3fn), ("a_scale_inv", a_scale_inv, f32), ("b_t", b_t, torch.float8_e4m3fn),
+         ("b_scale_inv", b_scale_inv, f32), ("k_plan?", k_plan, i32))
+    M, K = a_t.shape
+    N, Kb = b_t.shape
+    if K != Kb:
+        raise _lib.IvbError(f"gemm_fp8_wgrad: contraction mismatch {K} vs {Kb}")
+    nkb = (K + 127) // 128
+    for nm, sc, n in (("a_scale_inv", a_scale_inv, M), ("b_scale_inv", b_scale_inv, N)):
+        if sc.shape != (nkb, n) or not sc.is_contiguous():
+            raise _lib.IvbError(f"gemm_fp8_wgrad: {nm} must be a contiguous [{nkb}, {n}], got {tuple(sc.shape)}")
+    out0 = _epilogue_operands(M, N, epi, out0, None, None, None, None, None, a_t.device)
+    _call("gemm_fp8_wgrad", a_t, _rows2d(a_t, "a_t"), a_scale_inv, b_t, _rows2d(b_t, "b_t"), b_scale_inv, M, N, K, epi,
+          flags, out0, _rows2d(out0, "out0"), k_plan, kind="gemm", flops=2.0 * M * N * K)
+    return out0
+
+
 # ----------------------------------------------------------------------------------------- norms
 def norm_fwd(x, weight, bias=None, eps=1e-6, layernorm=False, out=None, want_stats=True):
     """x: [M,D] fp32 or bf16 (row stride arbitrary). Returns (y bf16, mean|None, rstd)."""
@@ -434,7 +476,8 @@ def attn_bwd(q, k, v, out, dout, lse, B, n, H, d, scale, dq, dk, dv, rowscale=No
 
 
 def _chk_rowscale(fn, rowscale, rows):
-    """The attention plan calls read rowscale[b*n] for every clip b: a contiguous fp32 [B*n]."""
+    """The attention plan calls read rowscale[b*n] for every clip b (the block-scaled cast every row): a contiguous fp32
+    [B*n]."""
     if rowscale is not None and (rowscale.shape != (rows,) or not rowscale.is_contiguous()):
         raise _lib.IvbError(f"{fn}: rowscale must be a contiguous [B*n] = [{rows}], got {tuple(rowscale.shape)}")
 

@@ -276,10 +276,11 @@ class Block(nn.Module):
         self.with_cp = bool(with_cp)
         self.use_fused_rmsnorm = use_fused_rmsnorm
         self.num_heads = num_heads
-        # FP8 GEMMs for the forward and input-gradient passes (set_fp8) and their scaling, "tensor" or "token"; read at
-        # call time
+        # FP8 GEMMs for the forward and input-gradient passes (set_fp8), their scaling, "tensor" or "token", and with
+        # "token" whether the weight gradients run in FP8 too; read at call time
         self.fp8 = False
         self.fp8_scaling = "tensor"
+        self.fp8_wgrad = False
         # FP8 inference with per-channel weight copies (set_fp8_inference); None when off
         self.fp8_inference = None
 
@@ -447,7 +448,7 @@ def set_droppath_skip(model: nn.Module, enabled: bool = True) -> int:
     return len(towers)
 
 
-def set_fp8(model: nn.Module, enabled: bool = True, scaling: str = "tensor") -> int:
+def set_fp8(model: nn.Module, enabled: bool = True, scaling: str = "tensor", wgrad: bool = False) -> int:
     """Switch the FP8 mode of every ViT Block in `model` (stage-1 student, CLIP tower, stage-2 tower, InternVL teacher)
     on or off; returns how many blocks were switched.
 
@@ -456,15 +457,22 @@ def set_fp8(model: nn.Module, enabled: bool = True, scaling: str = "tensor") -> 
     scaling="tensor": activations and weights in E4M3, gradients in E5M2, one scale per tensor.  scaling="token":
     activations and gradients in E4M3 with one scale per row (token), cast in one pass over each row (n1 and n2 inside
     the norm kernel), and the weights in E4M3 with one scale per output channel for the forward and per input channel
-    for the input-gradient GEMMs.  Weight gradients, attention, norms and everything outside the blocks stay bf16.  The
-    mode is read when a block runs: switch it before capturing a CUDA graph of the step."""
+    for the input-gradient GEMMs.  Weight gradients, attention, norms and everything outside the blocks stay bf16.
+    wgrad=True (scaling="token" only; any other scaling raises ValueError) also runs the four weight gradients on the
+    FP8 tensor cores: dy and the saved bf16 activation are cast transposed to E4M3 with one scale per channel per
+    128-token block, applied as the GEMM promotes each 128-token k-block to fp32 (ops.FP8_TOKEN_WGRAD); every GEMM of
+    the block then runs in FP8.  The mode is read when a block runs: switch it before capturing a CUDA graph of the
+    step."""
     if scaling not in FP8_SCALINGS:
         raise ValueError(f"set_fp8: scaling must be one of {sorted(FP8_SCALINGS)}, got {scaling!r}")
+    if wgrad and scaling != "token":
+        raise ValueError(f"set_fp8: wgrad=True needs scaling='token', got {scaling!r}")
     n = 0
     for mod in model.modules():
         if isinstance(mod, Block):
             mod.fp8 = bool(enabled)
             mod.fp8_scaling = scaling
+            mod.fp8_wgrad = bool(wgrad)
             n += 1
     return n
 
@@ -496,7 +504,9 @@ def block_precision(block, training=False):
     set_fp8 (Block.fp8) and set_fp8_inference (fp8_inference).  training: the forward needs a gradient."""
     fp8 = getattr(block, "fp8", False)
     if block.fp8_inference is None:
-        return FP8_SCALINGS[block.fp8_scaling] if fp8 else ops.BF16
+        if not fp8:
+            return ops.BF16
+        return ops.FP8_TOKEN_WGRAD if getattr(block, "fp8_wgrad", False) else FP8_SCALINGS[block.fp8_scaling]
     if training:
         raise ll._lib.IvbError("Block: FP8 inference mode (set_fp8_inference) has no gradient; switch it off to train")
     if fp8:

@@ -188,9 +188,12 @@ class PoolAttnFn(torch.autograd.Function):
 # ------------------------------------------------------------------------------------------ fused ViT block
 # A block's precision (BlockSpec.precision): BF16; FP8_TENSOR, FP8 with per-tensor scales and the weights cast in the
 # call (modules.set_fp8); FP8_TOKEN, FP8 with per-token scales and the weights cast per channel in the call
-# (modules.set_fp8 with scaling="token"); or per-token FP8 inference (modules.set_fp8_inference, no-grad calls only),
-# given as the four weights' per-channel E4M3 copies themselves: ((q, scale_inv) for qkv, proj, fc1, fc2).
-BF16, FP8_TENSOR, FP8_TOKEN = "bf16", "fp8", "fp8_token"
+# (modules.set_fp8 with scaling="token"); FP8_TOKEN_WGRAD, FP8_TOKEN whose weight gradients also run in FP8, from
+# operands cast with one scale per channel per 128-token block (modules.set_fp8 with scaling="token", wgrad=True); or
+# per-token FP8 inference (modules.set_fp8_inference, no-grad calls only), given as the four weights' per-channel E4M3
+# copies themselves: ((q, scale_inv) for qkv, proj, fc1, fc2).
+BF16, FP8_TENSOR, FP8_TOKEN, FP8_TOKEN_WGRAD = "bf16", "fp8", "fp8_token", "fp8_token_wgrad"
+_PER_TOKEN = (FP8_TOKEN, FP8_TOKEN_WGRAD)      # the precisions whose forward and input gradients are FP8_TOKEN's
 
 
 class BlockSpec(NamedTuple):
@@ -225,7 +228,8 @@ BlockParams = namedtuple("BlockParams", "n1w qkvw qkvb qnw knw projw projb g1 n2
 
 # What block_forward(save=True) keeps for block_backward: activations and norm statistics (mean1 / mean2 None on RMSNorm
 # blocks), and in FP8 the E4M3 copies of the four weights' transposes with their scales (the input-gradient GEMMs'
-# operands; per-tensor scalars in FP8_TENSOR, one scale per input channel in FP8_TOKEN; None in bf16).
+# operands; per-tensor scalars in FP8_TENSOR, one scale per input channel in FP8_TOKEN and FP8_TOKEN_WGRAD; None in
+# bf16).
 BlockSaved = namedtuple("BlockSaved", "n1 qkv qkn a lse mean1 rstd1 rq rk x1 y1 n2 mean2 rstd2 h g y2 "
                                       "qkvw_t qkvw_s projw_t projw_s fc1w_t fc1w_s fc2w_t fc2w_s")
 
@@ -243,14 +247,17 @@ def droppath_plan(rowscale):
 def _branch_plans(plan, M, prec):
     """(M plan, K plan) of a branch's DropPath plan row for the block's GEMMs over its M rows: the M plan for a GEMM
     whose M rows are the block's rows (bf16, or FP8 with per-token scales), the K plan for a weight gradient whose K runs
-    over them (bf16 in both modes).  (None, None) without a plan or in FP8_TENSOR: there a dropped clip's rows still
-    count in each activation's and gradient's per-tensor amax, and skipping them would zero those rows and change the
-    scales, so every row runs.  In FP8_TOKEN each scale belongs to one row: a dropped row's zeros change only its own
-    (finite) scale, and it feeds only dead tiles or rows the epilogue multiplies by 0."""
-    if plan is None or prec not in (BF16, FP8_TOKEN):
+    over them (bf16: the plan's 64-row k-blocks; FP8_TOKEN_WGRAD: the M plan itself, whose live 128-row tiles are the
+    FP8 weight gradient's 128-token k-blocks).  (None, None) without a plan or in FP8_TENSOR: there a dropped clip's
+    rows still count in each activation's and gradient's per-tensor amax, and skipping them would zero those rows and
+    change the scales, so every row runs.  In FP8_TOKEN each scale belongs to one row: a dropped row's zeros change
+    only its own (finite) scale, and it feeds only dead tiles or rows the epilogue multiplies by 0.  The FP8 weight
+    gradient's block scales span 128 rows: its casts zero the dropped rows of both operands (block_backward), so they
+    do not depend on the plan either."""
+    if plan is None or prec not in (BF16, *_PER_TOKEN):
         return None, None
     nm = (M + 127) // 128
-    return plan[:nm + 1], plan[nm + 1:]
+    return plan[:nm + 1], plan[:nm + 1] if prec == FP8_TOKEN_WGRAD else plan[nm + 1:]
 
 
 def block_forward(x, spec, p, rs1=None, rs2=None, save=True, plan1=None, plan2=None):
@@ -273,7 +280,7 @@ def block_forward(x, spec, p, rs1=None, rs2=None, save=True, plan1=None, plan2=N
     their fused epilogues.  FP8_TOKEN also casts the four weights per output channel (4 calls) and, with save, per input
     channel into their transposed copies (4 more), and its norm kernel then also writes the bf16 row and statistics
     the backward needs (without save: the same E4M3 bits from the inference norm kernel).  Attention, the q/k norms and
-    the residual stream stay as above.
+    the residual stream stay as above.  FP8_TOKEN_WGRAD runs the forward exactly as FP8_TOKEN and saves the same state.
 
     plan1 / plan2: optional DropPath plans of the two branches (rows of droppath_plan of rs1 / rs2): in bf16 and
     FP8_TOKEN the GEMMs of a branch then skip the row tiles whose rows rs zeroes, writing what the epilogue table of
@@ -285,12 +292,12 @@ def block_forward(x, spec, p, rs1=None, rs2=None, save=True, plan1=None, plan2=N
     if x.dtype != f32 or not x.is_cuda:
         raise ll._lib.IvbError("block_forward: residual stream must be a CUDA fp32 tensor [B*n, D]")
     prec = spec.precision
-    per_token = prec == FP8_TOKEN or not isinstance(prec, str)
+    per_token = prec in _PER_TOKEN or not isinstance(prec, str)
     weights = (p.qkvw, p.projw, p.fc1w, p.fc2w)
     # (q, scale_inv, q_t, scale_inv of q_t) per weight; q_t only when the backward will need it
     if prec == FP8_TENSOR:
         w8 = [(q, s, q_t, s) for q, q_t, s, _ in (ll.fp8_quantize(w, ll.FP8_E4M3, transpose=save) for w in weights)]
-    elif prec == FP8_TOKEN:
+    elif prec in _PER_TOKEN:
         w8 = [(*ll.fp8_quantize_rows(w), *(ll.fp8_quantize_rows(w, transposed=True) if save else (None, None))) for w in weights]
     elif per_token:
         w8 = [(q, s, None, None) for q, s in prec]
@@ -350,12 +357,16 @@ def block_backward(x, s, spec, t, P, dx2, rs1, rs2, plan1=None, plan2=None):
     """Backward of block_forward(save=True), from its BlockSaved s: 13 to 17 library calls in bf16 (with or without the
     q/k norms and the qkv bias, the fused RMSNorm norm2 + LayerScale backward), and in FP8 one more per input-gradient
     GEMM (the cast of its gradient: E5M2 with a per-tensor scale in FP8_TENSOR, E4M3 rows with per-row scales in
-    FP8_TOKEN).  The LayerNorm block (spec.layernorm) also returns its norms'
+    FP8_TOKEN).  FP8_TOKEN_WGRAD also runs the four weight gradients in FP8, with two more calls each: the transposing
+    casts of dy and of the saved bf16 activation, one scale per channel per 128-token block (lowlevel._fp8_quantize_blocks_t;
+    the activation's rows whose DropPath factor is 0 are cast as zeros, as their gradient rows are), then
+    lowlevel._gemm_fp8_wgrad, with or without the gradient sink.  The LayerNorm block (spec.layernorm) also returns its norms'
     bias gradients and always runs the attention branch's LayerScale backward as its own call.  `t` are the block's
     tensors as autograd handed them back, `P` the nn.Parameter objects (gradient sink), both BlockParams.  Returns
     (dx0, BlockParams of gradients | None when the sink took them).  plan1 / plan2: the DropPath plans block_forward
     ran with; the input-gradient GEMMs of a branch skip its dead row tiles (zeros), its weight gradients the
-    64-row k-blocks of dropped rows, whose gradient rows layerscale_bwd made zero, and attention the dropped clips."""
+    64-row (FP8 weight gradients: 128-row) k-blocks of dropped rows, whose gradient rows layerscale_bwd made zero, and
+    attention the dropped clips."""
     B, n, H = spec.B, spec.n, spec.H
     M, D = x.shape
     d = D // H
@@ -380,7 +391,7 @@ def block_backward(x, s, spec, t, P, dx2, rs1, rs2, plan1=None, plan2=None):
     (m1, k1), (m2, k2) = _branch_plans(plan1, M, spec.precision), _branch_plans(plan2, M, spec.precision)
 
     def dgrad(dy, w, w_t, w_s, m_plan, **epilogue):   # dx = dy W; in FP8 on the cast gradient and the E4M3 copy of W^T
-        if spec.precision == FP8_TOKEN:
+        if spec.precision in _PER_TOKEN:
             q, sc = ll.fp8_quantize_rows(dy)
         elif spec.precision == FP8_TENSOR:
             q, _, sc, _ = ll.fp8_quantize(dy, ll.FP8_E5M2)
@@ -388,18 +399,23 @@ def block_backward(x, s, spec, t, P, dx2, rs1, rs2, plan1=None, plan2=None):
             return ll.gemm(dy, w, b_t=True, m_plan=m_plan, **epilogue)
         return ll._gemm_fp8_plan(q, sc, w_t, w_s, m_plan, **epilogue)
 
-    def wgrad(dy, act, param, k_plan):
+    def wgrad(dy, act, param, k_plan, rs):   # dW = dy^T act; with the sink accumulated into the flat gradient
+        out0, flags = (None, 0) if sink is None else (param.grad, ll.FLAG_ACCUM)
+        if spec.precision == FP8_TOKEN_WGRAD:
+            (qd, sd), (qa, sa) = ll._fp8_quantize_blocks_t(dy), ll._fp8_quantize_blocks_t(act, rowscale=rs)
+            dw = ll._gemm_fp8_wgrad(qd, sd, qa, sa, out0=out0, flags=flags, k_plan=k_plan)
+        else:
+            dw = ll.gemm(dy, act, a_t=True, b_t=True, out0=out0, flags=flags, k_plan=k_plan)
         if sink is None:
-            return ll.gemm(dy, act, a_t=True, b_t=True, k_plan=k_plan)
-        ll.gemm(dy, act, a_t=True, b_t=True, out0=param.grad, flags=ll.FLAG_ACCUM, k_plan=k_plan)
+            return dw
         sink.grad_written(param)
         return None
     # ---- MLP branch
     dy2 = ll.layerscale_bwd(dx2, s.y2, t.g2, dg2 if t.g2 is not None else None, dcs2, rowscale=rs2)
-    dfc2w = wgrad(dy2, s.g, P.fc2w, k2)
+    dfc2w = wgrad(dy2, s.g, P.fc2w, k2, rs2)
     dh = dgrad(dy2, t.fc2w, s.fc2w_t, s.fc2w_s, m2, epi=ll.EPI_GELU_BWD, flags=spec.gelu_flags(True), aux=s.h)
     ll.colsum(dh, out=seg["fc1b"])
-    dfc1w = wgrad(dh, s.n2, P.fc1w, k2)
+    dfc1w = wgrad(dh, s.n2, P.fc1w, k2, rs2)
     dn2 = dgrad(dh, t.fc1w, s.fc1w_t, s.fc1w_s, m2)
     # ---- attention branch
     if not spec.layernorm and t.g1 is not None and D <= 1536 and M >= 1024:
@@ -410,7 +426,7 @@ def block_backward(x, s, spec, t, P, dx2, rs1, rs2, plan1=None, plan2=None):
         dx1 = ll.norm_bwd(dn2, s.x1, t.n2w, s.mean2, s.rstd2, layernorm=spec.layernorm, dx_in=dx2, dweight=dn2w,
                           dbias=seg.get("n2b"))
         dy1 = ll.layerscale_bwd(dx1, s.y1, t.g1, dg1 if t.g1 is not None else None, dcs1, rowscale=rs1)
-    dprojw = wgrad(dy1, s.a, P.projw, k1)
+    dprojw = wgrad(dy1, s.a, P.projw, k1, rs1)
     da = dgrad(dy1, t.projw, s.projw_t, s.projw_s, m1)
     dqkv = torch.empty((M, 3 * D), device=x.device, dtype=bf16)
     qk = s.qkn if s.qkn is not None else s.qkv
@@ -421,7 +437,7 @@ def block_backward(x, s, spec, t, P, dx2, rs1, rs2, plan1=None, plan2=None):
     elif s.qkn is not None:
         ll.norm_bwd(dqkv[:, :D], s.qkv[:, :D], t.qnw, None, s.rq, dx_out=dqkv[:, :D], dweight=seg["qnw"])
         ll.norm_bwd(dqkv[:, D:2 * D], s.qkv[:, D:2 * D], t.knw, None, s.rk, dx_out=dqkv[:, D:2 * D], dweight=seg["knw"])
-    dqkvw = wgrad(dqkv, s.n1, P.qkvw, k1)
+    dqkvw = wgrad(dqkv, s.n1, P.qkvw, k1, rs1)
     if t.qkvb is not None:
         ll.colsum(dqkv, out=seg["qkvb"])
     dn1 = dgrad(dqkv, t.qkvw, s.qkvw_t, s.qkvw_s, m1)

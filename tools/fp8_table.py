@@ -101,7 +101,7 @@ def quant_table(iters):
 
 
 def step_table(reps=3, steps=10, modes=("off", "tensor"), skips=(True,)):
-    """modes: "off" (bf16) or a set_fp8 scaling; skips: the set_droppath_skip settings.  Each (mode, skip) pair is
+    """modes: "off" (bf16), a set_fp8 scaling or "token_wgrad" (scaling="token", wgrad=True); skips: the set_droppath_skip settings.  Each (mode, skip) pair is
     captured and timed once per repetition, in turn."""
     import bench
     from internvideo_b200.engine import GraphedStep, PretrainEngine
@@ -142,7 +142,8 @@ def step_table(reps=3, steps=10, modes=("off", "tensor"), skips=(True,)):
     res = {r: [] for r in runs}
     for _ in range(reps):
         for fp8, skip in runs:
-            set_fp8(model, fp8 != "off", scaling="tensor" if fp8 == "off" else fp8)
+            wgrad = fp8 == "token_wgrad"     # per-token FP8 with FP8 weight gradients
+            set_fp8(model, fp8 != "off", scaling="tensor" if fp8 == "off" else "token" if wgrad else fp8, wgrad=wgrad)
             set_droppath_skip(model, skip)
             gs = GraphedStep(step, [video, mask], warmup=1)
             gs(video, mask)
