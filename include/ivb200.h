@@ -324,6 +324,34 @@ int ivb_attn_bwd_plan(const void* q, long ldq, const void* k, long ldk, const vo
                       const void* out, long ldo, const void* dout, long lddo, const float* lse2,
                       float* delta_ws, void* dq, long lddq, void* dk, long lddk, void* dv, long lddv,
                       int B, int n, int H, int d, float softmax_scale, const float* rowscale, void* stream);
+/* ---- FP8 attention forward (FP8 inference of frozen towers; no lse, no backward) ------------------------------------
+ * Every scale is a power of two chosen from an amax by the ivb_fp8_quantize_rows rule (E4M3; 1 when the amax is 0,
+ * scale_inv NaN when the amax is Inf or NaN), so dequantisation is exact.  Same bits on every run; one stream-ordered
+ * kernel per call; capturable in a CUDA graph.  head_dim d: a multiple of 8 in [16, 128] (the model uses 64 / 88 / 128).
+ * B = 0 or n = 0 is a no-op.  A call that breaks a rule below is refused before any CUDA call.
+ *
+ * ivb_attn_fp8_pack: q, k, v as ivb_attn_fwd takes them (bf16 [B*n, H*d] views; ldq, ldk, ldv multiples of 8; 16-byte
+ *   aligned) ->
+ *   q8, k8 E4M3 [B*n, H*dp], dp = round_up(d, 32): head h in columns h*dp .. h*dp + d, then dp - d zero columns
+ *     (pitch ld8, a multiple of 16 and >= H*dp; columns H*dp .. ld8 are not written), one scale per (token, head) from
+ *     the amax of that head's d columns of the row: q_scale_inv, k_scale_inv fp32 [B, H, ns] with
+ *     ns = ivb_attn_fp8_scale_pitch(n) (n rounded up to 64; entries n .. ns are written 0), 16-byte aligned;
+ *   vt8 E4M3 [B, H, d, ldvt] = V^T per (clip, head) (ldvt a multiple of 16 and >= round_up(n, 16); keys n ..
+ *     round_up(n, 16) are written 0, later ones are not written), one scale per (clip, head, channel) from the amax over
+ *     the clip's n tokens: v_scale_inv fp32 [B, H, d].
+ *   q8, k8 and vt8 are 16-byte aligned.
+ * ivb_attn_fwd_fp8: out[b,q,h,:] = softmax(scale q k^T) v (bf16; pitch ldo, a multiple of 8; 4-byte aligned) from the
+ *   pack's outputs, on the FP8 tensor cores: S = q_scale_inv k_scale_inv (q8 k8^T), P = exp2(S scale log2e - max) cast
+ *   to E4M3 as P * 2^8, O = (P vt8^T) v_scale_inv / rowsum(P).  The operand rules are the pack's: ld8 and ldvt as above
+ *   (a vt8 pitch below round_up(n, 16) is refused); q8, k8, vt8, q_scale_inv and k_scale_inv 16-byte aligned,
+ *   v_scale_inv 8-byte.                                                                                           */
+int ivb_attn_fp8_scale_pitch(int n);
+int ivb_attn_fp8_pack(const void* q, long ldq, const void* k, long ldk, const void* v, long ldv, int B, int n, int H,
+                      int d, void* q8, void* k8, long ld8, float* q_scale_inv, float* k_scale_inv, void* vt8, long ldvt,
+                      float* v_scale_inv, void* stream);
+int ivb_attn_fwd_fp8(const void* q8, const void* k8, long ld8, const float* q_scale_inv, const float* k_scale_inv,
+                     const void* vt8, long ldvt, const float* v_scale_inv, void* out, long ldo, int B, int n, int H,
+                     int d, float softmax_scale, void* stream);
 
 /* ---- token front-end (tubelet embed as visible-only gather-GEMM) --------------------------------
  * idx[b, 0..n_keep) = ascending positions where mask[b, :] == 0 — the order of `x[~mask]`

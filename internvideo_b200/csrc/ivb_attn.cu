@@ -30,46 +30,6 @@ struct AttnFwdParams {
   float* lse2;       // [B, H, n]  log2-domain logsumexp of the scaled scores
 };
 
-// Quad reductions: the four threads (lane & 3) of a quad share an accumulator row.
-__device__ __forceinline__ float quad_max(float v) {
-  v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
-  return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
-}
-__device__ __forceinline__ float quad_sum(float v) {
-  v += __shfl_xor_sync(0xffffffffu, v, 1);
-  return v + __shfl_xor_sync(0xffffffffu, v, 2);
-}
-
-// Online-softmax update of one S tile in place: S -> P = exp2(S*sc - m_new) (columns >= valid get 0); returns the
-// rescale factor alpha = exp2(m_old - m_new) of each of the thread's two rows, and folds the row sums into l_run.
-__device__ __forceinline__ void softmax_tile(float (&s)[ATT_COLS / 2], int valid, int lane, float sc_log2,
-                                             float m_run[2], float l_run[2], float alpha[2]) {
-  float mx[2] = {-INFINITY, -INFINITY};
-#pragma unroll
-  for (int i = 0; i < ATT_COLS / 2; ++i) {
-    const int col = 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
-    float v = s[i] * sc_log2;
-    if (col >= valid) v = -INFINITY;
-    s[i] = v;
-    mx[(i >> 1) & 1] = fmaxf(mx[(i >> 1) & 1], v);
-  }
-#pragma unroll
-  for (int r = 0; r < 2; ++r) {
-    const float m_new = fmaxf(m_run[r], quad_max(mx[r]));
-    alpha[r] = exp2f(m_run[r] - m_new);
-    m_run[r] = m_new;
-  }
-  float rs[2] = {0.f, 0.f};
-#pragma unroll
-  for (int i = 0; i < ATT_COLS / 2; ++i) {
-    const int r = (i >> 1) & 1;
-    s[i] = exp2f(s[i] - m_run[r]);
-    rs[r] += s[i];
-  }
-#pragma unroll
-  for (int r = 0; r < 2; ++r) l_run[r] = l_run[r] * alpha[r] + rs[r];
-}
-
 // KA: number of 64-wide atoms covering head_dim (1: d<=64, 2: d<=128).  NO: wgmma N of P·V (d rounded up).
 // KS: k16 steps of S = Q K^T, ceil(d / 16).
 // PLAN: the CTA of a dropped clip (attn_prologue) writes zeros to its out rows and lse2 0, a finite value, to its rows.

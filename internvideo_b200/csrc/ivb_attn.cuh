@@ -1,6 +1,8 @@
-// ivb_attn.cuh — the pieces the attention forward (ivb_attn.cu) and backward (ivb_attn_bwd.cu) kernels share: one CTA
-// per (128-row block, head, clip) that streams 64-row tiles of the other operands through a ring.
+// ivb_attn.cuh — the pieces the attention forward (ivb_attn.cu), backward (ivb_attn_bwd.cu) and FP8 forward
+// (ivb_attn_fp8.cu) kernels share: one CTA per (128-row block, head, clip) that streams 64-row tiles of the other
+// operands through a ring.
 #pragma once
+#include <math.h>
 #include <stdio.h>
 
 #include <initializer_list>
@@ -14,8 +16,21 @@ constexpr int ATT_ROWS = 128;     // rows owned by a CTA (two MMA warpgroups of 
 constexpr int ATT_COLS = 64;      // rows of a streamed tile
 constexpr int ATT_THREADS = 384;  // the producer warpgroup and the two MMA warpgroups
 
-// 4-D view (d, head, token, clip) of a [B*n, ld] projection buffer starting at `base`, box_tokens rows per load.
+// The element type of the head rows a kernel loads: bf16 (64 columns per 128-byte atom) or E4M3 (128; the FP8 forward).
+enum class AttnElt { BF16, E4M3 };
+
+// 4-D TMA view of a [B*n, ld] projection buffer starting at `base`, box_tokens rows per load.  bf16: (d, head, token,
+// clip); the head dim is its own axis, so the columns past d of a 64-column atom (d = 88) are out of bounds and land as
+// zeros.  E4M3 (heads of d columns, d a multiple of 32): (H*d, 1, token, clip), a head addressed by its first column
+// h*d; its 128-column box reads on into the next head's columns (out of bounds, zeros, after the last head).
+template <AttnElt ELT = AttnElt::BF16>
 inline int make_head_tmap(CUtensorMap* tm, const void* base, long ld, int B, int n, int H, int d, int box_tokens) {
+  if constexpr (ELT == AttnElt::E4M3) {
+    const uint64_t dims[4] = {(uint64_t)H * d, 1, (uint64_t)n, (uint64_t)B};
+    const long strides[3] = {ld, ld, (long)n * ld};
+    const uint32_t box[4] = {128, 1, (uint32_t)box_tokens, 1};
+    return make_tmap_4d(tm, base, dims, strides, box, 1);
+  }
   const uint64_t dims[4] = {(uint64_t)d, (uint64_t)H, (uint64_t)n, (uint64_t)B};
   const long strides[3] = {(long)d, ld, (long)n * ld};
   const uint32_t box[4] = {64, 1, (uint32_t)box_tokens, 1};
@@ -111,19 +126,72 @@ __device__ __forceinline__ void attn_roles(const AttnCta& c, Produce&& produce, 
   }
 }
 
-// TMA of rows [row, row + BOX) of head h of clip b (a make_head_tmap view with a BOX-row box) into KA 64-column atoms.
-template <int KA, int BOX>
+// TMA of rows [row, row + BOX) of head h of clip b (a make_head_tmap<ELT> view with a BOX-row box) into KA 128-byte
+// atoms.  d: the E4M3 view's columns per head (make_head_tmap<E4M3>'s d), needed by that view only.
+template <int KA, int BOX, AttnElt ELT = AttnElt::BF16>
 __device__ __forceinline__ void load_head_rows(uint8_t* dst, const CUtensorMap* tm, int h, int row, int b,
-                                               uint64_t* bar) {
+                                               uint64_t* bar, int d = 0) {
 #pragma unroll
-  for (int a = 0; a < KA; ++a) tma_load_4d(dst + a * (BOX * 128), tm, a * 64, h, row, b, bar);
+  for (int a = 0; a < KA; ++a) {
+    if constexpr (ELT == AttnElt::E4M3)
+      tma_load_4d(dst + a * (BOX * 128), tm, h * d + a * 128, 0, row, b, bar);
+    else
+      tma_load_4d(dst + a * (BOX * 128), tm, a * 64, h, row, b, bar);
+  }
 }
 
-// Writes this thread's rows (< n) of a 64 x NO accumulator, row r times factor[r], as bf16 to head h of the [B*n, ld]
-// buffer out.  Fragment row r holds columns 8 jn + 2 (lane % 4) + {0, 1} in acc[4 jn + 2 r], acc[4 jn + 2 r + 1].
-template <int NO>
+// Quad reductions: the four threads (lane & 3) of a quad share an accumulator row.
+__device__ __forceinline__ float quad_max(float v) {
+  v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
+  return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
+}
+__device__ __forceinline__ float quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  return v + __shfl_xor_sync(0xffffffffu, v, 2);
+}
+
+// Online-softmax update of one S tile in place: S -> P = exp2(S*sc - m_new + P_SHIFT) (columns >= valid get 0); returns
+// the rescale factor alpha = exp2(m_old - m_new) of each of the thread's two rows, and folds the row sums into l_run.
+// P_SHIFT scales P (and l) by 2^P_SHIFT: the FP8 forward's E4M3 P keeps small probabilities in the normal range.
+template <int P_SHIFT = 0>
+__device__ __forceinline__ void softmax_tile(float (&s)[ATT_COLS / 2], int valid, int lane, float sc_log2,
+                                             float m_run[2], float l_run[2], float alpha[2]) {
+  float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+  for (int i = 0; i < ATT_COLS / 2; ++i) {
+    const int col = 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
+    float v = s[i] * sc_log2;
+    if (col >= valid) v = -INFINITY;
+    s[i] = v;
+    mx[(i >> 1) & 1] = fmaxf(mx[(i >> 1) & 1], v);
+  }
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const float m_new = fmaxf(m_run[r], quad_max(mx[r]));
+    alpha[r] = exp2f(m_run[r] - m_new);
+    m_run[r] = m_new;
+  }
+  float rs[2] = {0.f, 0.f};
+#pragma unroll
+  for (int i = 0; i < ATT_COLS / 2; ++i) {
+    const int r = (i >> 1) & 1;
+    if constexpr (P_SHIFT == 0)
+      s[i] = exp2f(s[i] - m_run[r]);
+    else
+      s[i] = exp2f(s[i] - (m_run[r] - static_cast<float>(P_SHIFT)));
+    rs[r] += s[i];
+  }
+#pragma unroll
+  for (int r = 0; r < 2; ++r) l_run[r] = l_run[r] * alpha[r] + rs[r];
+}
+
+// Writes this thread's rows (< n) of a 64 x NO accumulator, row r times factor[r] (and, with COLF, column j times
+// colf[j]), as bf16 to head h of the [B*n, ld] buffer out.  Fragment row r holds columns 8 jn + 2 (lane % 4) + {0, 1} in
+// acc[4 jn + 2 r], acc[4 jn + 2 r + 1].
+template <int NO, bool COLF = false>
 __device__ __forceinline__ void store_rows(const float (&acc)[NO / 2], __nv_bfloat16* out, long ld, const AttnCta& c,
-                                           int n, int d, const float (&factor)[2] = {1.f, 1.f}) {
+                                           int n, int d, const float (&factor)[2] = {1.f, 1.f},
+                                           const float* colf = nullptr) {
 #pragma unroll
   for (int r = 0; r < 2; ++r) {
     const int row = c.row0 + c.rloc + 8 * r;
@@ -132,9 +200,14 @@ __device__ __forceinline__ void store_rows(const float (&acc)[NO / 2], __nv_bflo
 #pragma unroll
     for (int jn = 0; jn < NO / 8; ++jn) {
       const int col = 8 * jn + 2 * (c.lane & 3);
-      if (col < d)
-        *reinterpret_cast<uint32_t*>(orow + col) =
-            pack_bf16(acc[4 * jn + 2 * r] * factor[r], acc[4 * jn + 2 * r + 1] * factor[r]);
+      if (col >= d) continue;
+      float f0 = factor[r], f1 = factor[r];
+      if constexpr (COLF) {
+        const float2 cf = *reinterpret_cast<const float2*>(colf + col);
+        f0 *= cf.x;
+        f1 *= cf.y;
+      }
+      *reinterpret_cast<uint32_t*>(orow + col) = pack_bf16(acc[4 * jn + 2 * r] * f0, acc[4 * jn + 2 * r + 1] * f1);
     }
   }
 }

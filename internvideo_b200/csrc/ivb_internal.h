@@ -85,8 +85,9 @@ inline int launch(const char* name, void (*kern)(KArgs...), dim3 grid, dim3 bloc
 // zero OOB fill.
 int make_tmap_2d(CUtensorMap* out, const void* base, uint64_t inner, uint64_t outer,
                  long ld_elems, uint32_t box_inner, uint32_t box_outer, int elem_bytes = 2);
-// 4-D bf16 tensor (dims[0] innermost/contiguous), strides in elements for dims 1..3.
+// 4-D bf16 (elem_bytes 2) or fp8 (elem_bytes 1) tensor (dims[0] innermost/contiguous), strides in elements for dims
+// 1..3, 128-byte (or, swizzle_bytes 64, 64-byte) swizzle, zero OOB fill.
 int make_tmap_4d(CUtensorMap* out, const void* base, const uint64_t dims[4],
-                 const long strides_elems[3], const uint32_t box[4]);
+                 const long strides_elems[3], const uint32_t box[4], int elem_bytes = 2, int swizzle_bytes = 128);
 
 }  // namespace ivb

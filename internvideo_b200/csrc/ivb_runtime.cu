@@ -83,19 +83,21 @@ int make_tmap_2d(CUtensorMap* out, const void* base, uint64_t inner, uint64_t ou
 }
 
 int make_tmap_4d(CUtensorMap* out, const void* base, const uint64_t dims_[4],
-                 const long strides_elems[3], const uint32_t box_[4]) {
+                 const long strides_elems[3], const uint32_t box_[4], int elem_bytes, int swizzle_bytes) {
   PFN_encodeTiled enc = get_encode();
   if (!enc) return set_error("cuTensorMapEncodeTiled unavailable (no CUDA driver?)");
   if ((reinterpret_cast<uintptr_t>(base) & 15) != 0)
     return set_error("TMA base pointer must be 16-byte aligned");
   cuuint64_t dims[4] = {dims_[0], dims_[1], dims_[2], dims_[3]};
-  cuuint64_t strides[3] = {static_cast<cuuint64_t>(strides_elems[0]) * 2,
-                           static_cast<cuuint64_t>(strides_elems[1]) * 2,
-                           static_cast<cuuint64_t>(strides_elems[2]) * 2};
+  cuuint64_t strides[3] = {static_cast<cuuint64_t>(strides_elems[0]) * elem_bytes,
+                           static_cast<cuuint64_t>(strides_elems[1]) * elem_bytes,
+                           static_cast<cuuint64_t>(strides_elems[2]) * elem_bytes};
   cuuint32_t box[4] = {box_[0], box_[1], box_[2], box_[3]};
   cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUresult r = enc(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(base), dims,
-                   strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+  const CUtensorMapDataType dtype = elem_bytes == 1 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+  const CUtensorMapSwizzle swz = swizzle_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B;
+  CUresult r = enc(out, dtype, 4, const_cast<void*>(base), dims,
+                   strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swz,
                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     char buf[200];

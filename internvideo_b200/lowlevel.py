@@ -103,8 +103,9 @@ class OpProfiler:
 
 class GemmProfiler(OpProfiler):
     """CUDA-event timing of every tensor-core launch (GEMMs, bf16 and fp8: kind "gemm"; attention forward / backward)
-    and of the fp8 casts that feed the fp8 GEMMs (kind "fp8_quantize", no flops) and the norms that write FP8 rows
-    (kind "norm_fwd_fp8", no flops) on the launching stream (bench.py roofline).  Records only those calls."""
+    and of the fp8 casts that feed the fp8 GEMMs and the fp8 attention (kind "fp8_quantize", no flops) and the norms that
+    write FP8 rows (kind "norm_fwd_fp8", no flops) on the launching stream (bench.py roofline).  Records only those
+    calls."""
     kinds = frozenset(("gemm", "attn_fwd", "attn_bwd", "fp8_quantize", "norm_fwd_fp8"))
 
     def __init__(self):
@@ -473,6 +474,58 @@ def attn_bwd(q, k, v, out, dout, lse, B, n, H, d, scale, dq, dk, dv, rowscale=No
           _rows2d(dv, "dv"), B, n, H, d, float(scale), *plan, kind="attn_bwd",
           flops=10.0 * B * H * n * n * d)  # algorithmic: 5 GEMMs (SURVEY §8d: 2.5x forward)
     return dq, dk, dv
+
+
+def _attn_fp8_pack(q, k, v, B, n, H, d):
+    """Casts the attention operands to E4M3 for attn_fwd_fp8 (ivb_attn_fp8_pack); q, k, v as attn_fwd takes them.
+
+    Returns (q8, k8, q_scale_inv, k_scale_inv, vt8, v_scale_inv): q8, k8 float8_e4m3fn [B*n, H*dp], dp = d rounded up
+    to 32 (a head's columns: d values, then zeros), with one power-of-two scale per (token, head), q_scale_inv /
+    k_scale_inv fp32 [B, H, ns] (ns: n rounded up to 64, the padding 0); vt8
+    float8_e4m3fn [B, H, d, round_up(n, 16)] = V^T per (clip, head), keys n.. zero, with one scale per (clip, head,
+    channel), v_scale_inv fp32 [B, H, d].  q8 and k8 are views of buffers whose row pitch is rounded up to 16.  Private,
+    as _gemm_fp8_plan: the FP8-inference block forward (ops.block_forward with spec.attn_fp8) is its caller."""
+    _chk(("q", q, bf16), ("k", k, bf16), ("v", v, bf16))
+    for t, nm in ((q, "q"), (k, "k"), (v, "v")):
+        if t.shape != (B * n, H * d):
+            raise _lib.IvbError(f"attn_fp8_pack: {nm} must be [B*n, H*d], got {tuple(t.shape)}")
+    dev, e4m3, dp = q.device, torch.float8_e4m3fn, (d + 31) // 32 * 32
+    q8 = torch.empty((B * n, H * dp), device=dev, dtype=e4m3)
+    k8 = torch.empty((B * n, H * dp), device=dev, dtype=e4m3)
+    ns = int(_lib.load().ivb_attn_fp8_scale_pitch(n))
+    sq = torch.empty((B, H, ns), device=dev, dtype=f32)
+    sk = torch.empty((B, H, ns), device=dev, dtype=f32)
+    vt8 = torch.empty((B, H, d, _pad16(n)), device=dev, dtype=e4m3)
+    sv = torch.empty((B, H, d), device=dev, dtype=f32)
+    _call("attn_fp8_pack", q, _rows2d(q, "q"), k, _rows2d(k, "k"), v, _rows2d(v, "v"), B, n, H, d, q8, k8,
+          q8.stride(0), sq, sk, vt8, vt8.stride(2), sv, kind="fp8_quantize")
+    return q8, k8, sq, sk, vt8, sv
+
+
+def _attn_fwd_fp8(q8, k8, q_scale_inv, k_scale_inv, vt8, v_scale_inv, B, n, H, d, scale, out=None):
+    """softmax(scale q k^T) v on the FP8 tensor cores from attn_fp8_pack's outputs (ivb_attn_fwd_fp8): bf16 [B*n, H*d]
+    (out: an optional bf16 [B*n, H*d] view, any row pitch).  Inference only: no lse, no backward.  Private, as
+    _attn_fp8_pack."""
+    _chk(("q8", q8, torch.float8_e4m3fn), ("k8", k8, torch.float8_e4m3fn), ("q_scale_inv", q_scale_inv, f32),
+         ("k_scale_inv", k_scale_inv, f32), ("vt8", vt8, torch.float8_e4m3fn), ("v_scale_inv", v_scale_inv, f32),
+         ("out?", out, bf16))
+    ns = int(_lib.load().ivb_attn_fp8_scale_pitch(n))
+    dp = (d + 31) // 32 * 32
+    if q8.shape != (B * n, H * dp) or k8.stride() != q8.stride() or k8.shape != q8.shape:
+        raise _lib.IvbError(f"attn_fwd_fp8: q8 and k8 must be [B*n, H*round_up(d, 32)] with one row pitch, got "
+                            f"{tuple(q8.shape)}, {tuple(k8.shape)}")
+    for nm, t, shape in (("q_scale_inv", q_scale_inv, (B, H, ns)), ("k_scale_inv", k_scale_inv, (B, H, ns)),
+                         ("v_scale_inv", v_scale_inv, (B, H, d))):
+        if t.shape != shape or not t.is_contiguous():
+            raise _lib.IvbError(f"attn_fwd_fp8: {nm} must be a contiguous {list(shape)}, got {tuple(t.shape)}")
+    if vt8.shape[:3] != (B, H, d) or vt8.stride(3) != 1 or vt8.stride(1) != d * vt8.stride(2) or \
+            vt8.stride(0) != H * vt8.stride(1):
+        raise _lib.IvbError(f"attn_fwd_fp8: vt8 must be [B, H, d, >= n] with packed B, H, d, got {tuple(vt8.shape)}")
+    if out is None:
+        out = torch.empty((B * n, H * d), device=q8.device, dtype=bf16)
+    _call("attn_fwd_fp8", q8, k8, _rows2d(q8, "q8"), q_scale_inv, k_scale_inv, vt8, vt8.stride(2), v_scale_inv, out,
+          _rows2d(out, "out"), B, n, H, d, float(scale), kind="attn_fwd", flops=4.0 * B * H * n * n * d)
+    return out
 
 
 def _chk_rowscale(fn, rowscale, rows):

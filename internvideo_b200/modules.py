@@ -281,8 +281,10 @@ class Block(nn.Module):
         self.fp8 = False
         self.fp8_scaling = "tensor"
         self.fp8_wgrad = False
-        # FP8 inference with per-channel weight copies (set_fp8_inference); None when off
+        # FP8 inference with per-channel weight copies (set_fp8_inference); None when off.  fp8_attention: its
+        # attention=True, attention on the FP8 tensor cores too
         self.fp8_inference = None
+        self.fp8_attention = False
 
     def forward_stream(self, x2d, B, n, rowscale=None, plans=None):
         """fp32 residual stream [B*n, D] -> [B*n, D] (the hot path used by the model).
@@ -305,7 +307,7 @@ class Block(nn.Module):
     def _spec(self, B, n, training):
         return ops.BlockSpec(B, n, self.num_heads, self.mlp.gelu_tanh, eps1=self.norm1.variance_epsilon,
                              eps2=self.norm2.variance_epsilon, checkpoint=self.with_cp,
-                             precision=block_precision(self, training))
+                             precision=block_precision(self, training), attn_fp8=block_attn_fp8(self))
 
     def _param_tuple(self):
         a = self.attn
@@ -388,6 +390,7 @@ class VideoMAEBlock(nn.Module):
         self.drop_prob = float(drop_path)
         self.with_cp = bool(with_cp)
         self.fp8_inference = None   # set_fp8_inference
+        self.fp8_attention = False  # set_fp8_inference(attention=True)
 
     def _drop_path_rows(self, B, n, device):
         """IV1's DropPath draw (timm drop_path: Bernoulli(keep) / keep per sample, `rand < keep`), once per branch in
@@ -400,7 +403,8 @@ class VideoMAEBlock(nn.Module):
     def _spec(self, B, n, training=False, head_axis=False):
         a = self.attn
         return ops.BlockSpec(B, n, a.num_heads, layernorm=True, eps1=self.norm1.eps, eps2=self.norm2.eps, scale=a.scale,
-                             head_axis=head_axis, checkpoint=self.with_cp, precision=block_precision(self, training))
+                             head_axis=head_axis, checkpoint=self.with_cp, precision=block_precision(self, training),
+                             attn_fp8=block_attn_fp8(self, head_axis))
 
     def _param_tuple(self):
         a = self.attn
@@ -514,20 +518,30 @@ def block_precision(block, training=False):
     return block.fp8_inference.get()
 
 
-def set_fp8_inference(model: nn.Module, enabled: bool = True) -> int:
+def block_attn_fp8(block, head_axis=False):
+    """The ops.BlockSpec attn_fp8 of a forward of `block`: set_fp8_inference(attention=True) is on for it and the call's
+    attention runs over the tokens (head-axis attention keeps its kernel)."""
+    return block.fp8_inference is not None and block.fp8_attention and not head_axis
+
+
+def set_fp8_inference(model: nn.Module, enabled: bool = True, attention: bool = False) -> int:
     """Switch FP8 inference on or off for every ViT Block and VideoMAEBlock in `model` (frozen towers: the
     InternVL and VideoMAE teachers, the frozen CLIP and stage-2 towers); returns how many blocks were switched.
 
     In this mode a block's no-grad forward runs its four GEMMs (qkv, proj, fc1, fc2) on the FP8 tensor cores with
     per-token activation scales, computed where each activation is produced (n1 and n2 inside the norm kernel, a and
     g by a row-wise cast), and per-output-channel weight scales.  Switching on quantises each block's weights once;
-    they are re-quantised only when a weight changes.  Attention, the q/k norms and the fp32 residual stream stay
-    bf16 / fp32, and switching off restores the bf16 path bit for bit.  A switched Block refuses a forward that
-    needs a gradient, and the mode excludes set_fp8 on the same block."""
+    they are re-quantised only when a weight changes.  The q/k norms and the fp32 residual stream stay bf16 / fp32.
+    attention=False (the default) keeps attention bf16; attention=True also runs the token-axis attention on the FP8
+    tensor cores: q and k cast to E4M3 with one scale per (token, head), v per (clip, head, channel), P in E4M3
+    (lowlevel._attn_fp8_pack, _attn_fwd_fp8).  The VideoMAEv2 teacher's head-axis attention (head_axis_attention=True)
+    keeps its own kernel either way.  Switching off restores the bf16 path bit for bit.  A switched Block refuses a
+    forward that needs a gradient, and the mode excludes set_fp8 on the same block."""
     blocks = [m for m in model.modules() if isinstance(m, (Block, VideoMAEBlock))]
     if enabled and any(getattr(m, "fp8", False) for m in blocks):
         raise ll._lib.IvbError("set_fp8_inference: a block is in FP8 training mode (set_fp8); switch that off first")
     for m in blocks:
+        m.fp8_attention = bool(enabled and attention)
         if not enabled:
             m.fp8_inference = None
         elif m.fp8_inference is None:

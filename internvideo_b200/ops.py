@@ -200,7 +200,9 @@ class BlockSpec(NamedTuple):
     """Everything a fused block call needs besides its tensors.  layernorm: the VideoMAE LayerNorm block (InternVideo1,
     VideoMAEv2 teacher) instead of the RMSNorm block; eps1 / eps2 are the eps of its two norms.  scale: the attention
     scale (None: d ** -0.5).  head_axis: the VideoMAEv2 teacher's attention over the heads of each token (inference
-    only).  checkpoint: BlockFn keeps only the block input and recomputes the forward in the backward."""
+    only).  checkpoint: BlockFn keeps only the block input and recomputes the forward in the backward.  attn_fp8: the
+    token-axis attention runs on the FP8 tensor cores (lowlevel._attn_fp8_pack + _attn_fwd_fp8; inference only:
+    block_forward refuses it with save=True or head_axis)."""
     B: int
     n: int
     H: int
@@ -212,6 +214,7 @@ class BlockSpec(NamedTuple):
     head_axis: bool = False
     checkpoint: bool = False
     precision: object = BF16
+    attn_fp8: bool = False
 
     def attn_scale(self, d):
         return d ** -0.5 if self.scale is None else self.scale
@@ -282,6 +285,9 @@ def block_forward(x, spec, p, rs1=None, rs2=None, save=True, plan1=None, plan2=N
     the backward needs (without save: the same E4M3 bits from the inference norm kernel).  Attention, the q/k norms and
     the residual stream stay as above.  FP8_TOKEN_WGRAD runs the forward exactly as FP8_TOKEN and saves the same state.
 
+    spec.attn_fp8 (save=False and token-axis attention only; anything else raises IvbError): attention casts q, k and v
+    to E4M3 (one more call) and runs on the FP8 tensor cores instead of ivb_attn_fwd.
+
     plan1 / plan2: optional DropPath plans of the two branches (rows of droppath_plan of rs1 / rs2): in bf16 and
     FP8_TOKEN the GEMMs of a branch then skip the row tiles whose rows rs zeroes, writing what the epilogue table of
     ivb_gemm_bf16_plan gives them (x1 = x, zeros elsewhere), and attention skips the clips rs1 drops (a = 0 there);
@@ -289,6 +295,9 @@ def block_forward(x, spec, p, rs1=None, rs2=None, save=True, plan1=None, plan2=N
     B, n, H = spec.B, spec.n, spec.H
     M, D = x.shape
     d = D // H
+    if spec.attn_fp8 and (save or spec.head_axis):
+        raise ll._lib.IvbError("block_forward: FP8 attention (spec.attn_fp8) is inference-only and token-axis: it needs "
+                               "save=False and head_axis=False")
     if x.dtype != f32 or not x.is_cuda:
         raise ll._lib.IvbError("block_forward: residual stream must be a CUDA fp32 tensor [B*n, D]")
     prec = spec.precision
@@ -337,6 +346,8 @@ def block_forward(x, spec, p, rs1=None, rs2=None, save=True, plan1=None, plan2=N
         # the reference's call (videomae.py:94-97) attends over the heads of each token and reinterprets the
         # [B, H, N, d] result as [B, N, H*d]: reproduced bit-for-layout
         a = ll.headaxis_attn_fwd(qkv, B, n, H, d, spec.attn_scale(d)).reshape(M, D)
+    elif spec.attn_fp8:
+        a = ll._attn_fwd_fp8(*ll._attn_fp8_pack(q, k, v, B, n, H, d), B, n, H, d, spec.attn_scale(d))
     else:
         a, lse = ll.attn_fwd(q, k, v, B, n, H, d, spec.attn_scale(d), want_lse=save,
                              rowscale=rs1 if mp[0] is not None else None)
