@@ -200,10 +200,9 @@ attn_fwd_fp8_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
 // One CTA per (head, tensor, clip): blockIdx.y 0 and 1 cast the head's q and k rows, 2 casts and transposes its v.
 // q / k: 16 lanes per row, lane i < d / 8 holding columns 8i .. 8i + 7; the row's amax is a 16-lane shuffle max, and
 // lanes d / 8 .. dp / 8 write the head's zero columns.
-// v: the same lanes first take each channel's amax over the clip's tokens (shuffles, then shared memory: no atomics),
-// then 64-token tiles are cast with the channel scales and transposed through shared memory.
+// v: the same lanes first take each channel's amax over the clip's tokens (col_amax: no atomics), then 64-token tiles
+// are cast with the channel scales and transposed through shared memory.
 constexpr int PK_THREADS = 256;
-constexpr int PK_PITCH = ATT_COLS + 16;   // bytes per channel row of the transposing tile (16-byte aligned rows)
 
 struct AttnPackParams {
   const __nv_bfloat16 *q, *k, *v;
@@ -220,9 +219,9 @@ struct AttnPackParams {
 __global__ void __launch_bounds__(PK_THREADS) attn_fp8_pack_kernel(const AttnPackParams p) {
   __shared__ unsigned red[PK_THREADS / 32][128];
   __shared__ float vscale[128];
-  __shared__ __align__(16) uint8_t tile[128 * PK_PITCH];
+  __shared__ Fp8TileT<128, ATT_COLS> tile;
   const int h = blockIdx.x, which = blockIdx.y, b = blockIdx.z;
-  const int G = p.d / 8, l16 = threadIdx.x & 15, grp = threadIdx.x >> 4, lane = threadIdx.x & 31;
+  const int G = p.d / 8, l16 = threadIdx.x & 15, grp = threadIdx.x >> 4;
   const long hb = static_cast<long>(b) * p.H + h;
   const long row0 = static_cast<long>(b) * p.n;
   if (which < 2) {
@@ -233,10 +232,7 @@ __global__ void __launch_bounds__(PK_THREADS) attn_fp8_pack_kernel(const AttnPac
     for (int t = grp; t < p.n64; t += PK_THREADS / 16) {   // the same trip count for every lane (n64 % 16 == 0)
       uint4 v = make_uint4(0u, 0u, 0u, 0u);
       if (t < p.n && l16 < G) v = *reinterpret_cast<const uint4*>(src + (row0 + t) * ld);
-      unsigned m = 0;   // bf16 magnitude bits: NaN > Inf > every finite value
-      const uint32_t w[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-      for (int k = 0; k < 4; ++k) m = max(m, max(w[k] & 0x7fffu, (w[k] >> 16) & 0x7fffu));
+      unsigned m = bf16_mag_max(v);
 #pragma unroll
       for (int o = 8; o > 0; o >>= 1) m = max(m, __shfl_xor_sync(0xffffffffu, m, o));
       float scale, sinv;
@@ -253,27 +249,11 @@ __global__ void __launch_bounds__(PK_THREADS) attn_fp8_pack_kernel(const AttnPac
   const __nv_bfloat16* src = p.v + h * p.d;
   unsigned m[8] = {0u, 0u, 0u, 0u, 0u, 0u, 0u, 0u};
   if (l16 < G) {
-    for (int t = grp; t < p.n; t += PK_THREADS / 16) {
-      const uint4 v = *reinterpret_cast<const uint4*>(src + (row0 + t) * p.ldv + 8 * l16);
-      const uint32_t w[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        m[2 * k] = max(m[2 * k], w[k] & 0x7fffu);
-        m[2 * k + 1] = max(m[2 * k + 1], (w[k] >> 16) & 0x7fffu);
-      }
-    }
+    for (int t = grp; t < p.n; t += PK_THREADS / 16)
+      bf16_mag_cols(*reinterpret_cast<const uint4*>(src + (row0 + t) * p.ldv + 8 * l16), m);
   }
-#pragma unroll
-  for (int k = 0; k < 8; ++k) m[k] = max(m[k], __shfl_xor_sync(0xffffffffu, m[k], 16));   // lanes l, l ^ 16: one chunk
-  if (lane < G) {
-#pragma unroll
-    for (int k = 0; k < 8; ++k) red[threadIdx.x >> 5][lane * 8 + k] = m[k];
-  }
-  __syncthreads();
+  const unsigned mx = col_amax<16, PK_THREADS>(m, red);
   if (threadIdx.x < p.d) {
-    unsigned mx = 0;
-#pragma unroll
-    for (int w = 0; w < PK_THREADS / 32; ++w) mx = max(mx, red[w][threadIdx.x]);
     float sinv;
     fp8_scale(mx << 16, 8, vscale[threadIdx.x], sinv);
     p.sv[hb * p.d + threadIdx.x] = sinv;
@@ -283,22 +263,15 @@ __global__ void __launch_bounds__(PK_THREADS) attn_fp8_pack_kernel(const AttnPac
   uint8_t* vt = p.vt8 + hb * p.d * p.ldvt;
   for (int t0 = 0; t0 < n16; t0 += ATT_COLS) {
     for (int i = threadIdx.x; i < ATT_COLS * G; i += PK_THREADS) {
-      const int tt = i / G, c8 = i % G, t = t0 + tt;
-      float f[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};   // keys n .. n16 are zeros
-      if (t < p.n) unpack8(*reinterpret_cast<const uint4*>(src + (row0 + t) * p.ldv + 8 * c8), f);
-#pragma unroll
-      for (int k = 0; k < 8; k += 2) {
-        const uint32_t q = cvt_fp8x2<false>(f[k] * vscale[8 * c8 + k], f[k + 1] * vscale[8 * c8 + k + 1]);
-        tile[(8 * c8 + k) * PK_PITCH + tt] = static_cast<uint8_t>(q);
-        tile[(8 * c8 + k + 1) * PK_PITCH + tt] = static_cast<uint8_t>(q >> 8);
-      }
+      const int tt = i / G, c8 = i % G, t = t0 + tt;   // keys n .. n16 are zeros
+      tile.put(8 * c8, tt, t < p.n ? *reinterpret_cast<const uint4*>(src + (row0 + t) * p.ldv + 8 * c8)
+                                   : make_uint4(0u, 0u, 0u, 0u), vscale + 8 * c8);
     }
     __syncthreads();
     const int tn = min(ATT_COLS, n16 - t0);   // a multiple of 16
     for (int i = threadIdx.x; i < p.d * (ATT_COLS / 16); i += PK_THREADS) {
       const int row = i / (ATT_COLS / 16), q16 = (i % (ATT_COLS / 16)) * 16;
-      if (q16 < tn)
-        *reinterpret_cast<uint4*>(vt + row * p.ldvt + t0 + q16) = *reinterpret_cast<const uint4*>(tile + row * PK_PITCH + q16);
+      tile.store<16>(row, q16, vt + row * p.ldvt + t0 + q16, tn - q16);
     }
     __syncthreads();
   }

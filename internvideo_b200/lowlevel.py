@@ -194,6 +194,12 @@ def _pad16(n):
     return (n + 15) // 16 * 16
 
 
+def _fp8_rows(rows, cols, device, dtype=torch.float8_e4m3fn):
+    """An uninitialised FP8 [rows, cols] view of a buffer whose row pitch is cols rounded up to 16 elements (the fp8
+    GEMM's operand rule)."""
+    return torch.empty((rows, _pad16(cols)), device=device, dtype=dtype)[:, :cols]
+
+
 def fp8_quantize(x, fmt=FP8_E4M3, transpose=False):
     """Per-tensor current-scaling cast of a bf16 [M, K] tensor (any row pitch) to FP8 (ivb_fp8_quantize).
 
@@ -204,8 +210,8 @@ def fp8_quantize(x, fmt=FP8_E4M3, transpose=False):
     ldx = _rows2d(x, "x")
     M, K = x.shape
     dt = FP8_DTYPES[fmt]
-    q = torch.empty((M, _pad16(K)), device=x.device, dtype=dt)[:, :K]
-    q_t = torch.empty((K, _pad16(M)), device=x.device, dtype=dt)[:, :M] if transpose else None
+    q = _fp8_rows(M, K, x.device, dt)
+    q_t = _fp8_rows(K, M, x.device, dt) if transpose else None
     stats = torch.empty((2,), device=x.device, dtype=f32)
     amax, scale_inv = stats[0:1], stats[1:2]
     _call("fp8_quantize", x, ldx, M, K, fmt, q, q.stride(0), q_t, q_t.stride(0) if transpose else 0, amax, scale_inv)
@@ -226,12 +232,12 @@ def fp8_quantize_rows(x, transposed=False):
     ldx = _rows2d(x, "x")
     M, K = x.shape
     if transposed:
-        q_t = torch.empty((K, _pad16(M)), device=x.device, dtype=torch.float8_e4m3fn)[:, :M]
+        q_t = _fp8_rows(K, M, x.device)
         amax = torch.empty((K,), device=x.device, dtype=f32)
         sinv = torch.empty((K,), device=x.device, dtype=f32)
         _call("fp8_quantize_cols_t", x, ldx, M, K, q_t, q_t.stride(0), amax, sinv, kind="fp8_quantize")
         return q_t, sinv
-    q = torch.empty((M, _pad16(K)), device=x.device, dtype=torch.float8_e4m3fn)[:, :K]
+    q = _fp8_rows(M, K, x.device)
     sinv = torch.empty((M,), device=x.device, dtype=f32)
     _call("fp8_quantize_rows", x, ldx, M, K, q, q.stride(0), sinv, kind="fp8_quantize")
     return q, sinv
@@ -248,7 +254,7 @@ def norm_fwd_fp8(x, weight, bias=None, eps=1e-6, layernorm=False, save=False):
     _chk(("x", x, (f32, bf16)), ("weight", weight, bf16), ("bias?", bias, bf16))
     ldx = _rows2d(x, "x")
     M, D = x.shape
-    q = torch.empty((M, _pad16(D)), device=x.device, dtype=torch.float8_e4m3fn)[:, :D]
+    q = _fp8_rows(M, D, x.device)
     sinv = torch.empty((M,), device=x.device, dtype=f32)
     if not save:
         _call("norm_fwd_fp8", x, int(x.dtype == f32), ldx, weight, bias, float(eps), int(layernorm), M, D, q,
@@ -314,7 +320,7 @@ def _fp8_quantize_blocks_t(x, rowscale=None):
     ldx = _rows2d(x, "x")
     M, C = x.shape
     _chk_rowscale("fp8_quantize_blocks_t", rowscale, M)
-    q_t = torch.empty((C, _pad16(M)), device=x.device, dtype=torch.float8_e4m3fn)[:, :M]
+    q_t = _fp8_rows(C, M, x.device)
     sinv = torch.empty(((M + 127) // 128, C), device=x.device, dtype=f32)
     plan = () if rowscale is None else (rowscale,)
     _call("fp8_quantize_blocks_t_plan" if plan else "fp8_quantize_blocks_t", x, ldx, M, C, q_t, q_t.stride(0), sinv,

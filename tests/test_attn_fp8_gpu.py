@@ -5,7 +5,8 @@ Kernel level, at d in {64, 88, 128} x n in {257, 417, 1025, 2049} (sequence tail
 clips, q / k / v the three column slots of one [B*n, 3*H*d] projection buffer (row pitch 3D), as the blocks pass them:
 1. The pack is bit-exact against a torch emulation of its scale rule (the power-of-two rule of ivb_fp8_quantize_rows
    per (token, head) and per (clip, head, channel)) and of the E4M3 cast: q8 and k8 with their zero head padding, vt8
-   with its zero key padding, and every scale.
+   with its zero key padding, and every scale; an Inf in one head of a q row or in one channel of v gives scale_inv NaN
+   and the satfinite cast's +-448 for that group alone.
 2. The forward against a float64 emulation of its own arithmetic on the dequantised q8, k8 and vt8: the online softmax
    over 64-key tiles with P = exp2(S - m + 8) rounded to E4M3 where the kernel rounds it.  That isolates the kernel's
    arithmetic from the casts.  The kernel's fp32 P (ex2.approx) and the emulation's float64 P fall on different sides
@@ -122,6 +123,21 @@ def test_pack_bit_exact(cuda_lib, d, H, n):
     again = ll._attn_fp8_pack(q, k, v, B, n, H, d)
     assert all(torch.equal(a.view(torch.uint8) if a.dtype == E4M3 else a, b.view(torch.uint8) if b.dtype == E4M3 else b)
                for a, b in zip(again, (q8, k8, sq, sk, vt8, sv)))
+    # an Inf in one head of a q row and a -Inf in one channel of v: that group's scale is 1 and its scale_inv NaN, the
+    # satfinite cast makes the Inf +-448, and every other group keeps its bits
+    t, h, c, dp = n // 2, H - 1, d - 1, (d + 31) // 32 * 32
+    q2, v2 = q.clone(), v.clone()
+    q2[t, h * d + c], v2[n + t, h * d + c] = float("inf"), -float("inf")
+    sat = lambda x: x.float().clamp(-448, 448).to(E4M3).view(torch.uint8)   # noqa: E731
+    e_q8, e_vt8 = q8.view(torch.uint8).clone(), vt8.view(torch.uint8).clone()
+    e_q8[t, h * dp:h * dp + d] = sat(q2[t, h * d:(h + 1) * d])
+    e_vt8[1, h, c, :n] = sat(v2[n:, h * d + c])
+    e_sq, e_sv = sq.clone(), sv.clone()
+    e_sq[0, h, t] = e_sv[1, h, c] = float("nan")
+    got = ll._attn_fp8_pack(q2, k, v2, B, n, H, d)
+    for a, b in zip(got, (e_q8, k8, e_sq, sk, e_vt8, e_sv)):
+        assert torch.equal(a.view(torch.uint8) if a.dtype == E4M3 else a.view(torch.int32),
+                           b.view(torch.uint8) if b.dtype in (E4M3, torch.uint8) else b.view(torch.int32))
 
 
 @pytest.mark.parametrize("d, H, n", SHAPES)

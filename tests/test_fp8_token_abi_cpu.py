@@ -80,7 +80,9 @@ def test_quantize_cols_t_refusals():
 
 
 @pytest.mark.parametrize("obj, pattern, count", [("ivb_norm.o", "norm_fwd_fp8_train_kernel", 16),
-                                                 ("ivb_fp8.o", "fp8_c(ol_amax|ast_cols)_kernel", 2)])
+                                                 ("ivb_fp8.o", "fp8_c(ol_amax|ast_cols)_kernel", 2),
+                                                 ("ivb_fp8.o", "fp8_(amax|cast|col_amax|cast_cols|rows|blocks_t)_kernel",
+                                                  10)])
 def test_new_kernels_keep_nothing_in_local_memory(obj, pattern, count):
     tool = next((c for c in (shutil.which("cuobjdump"), "/usr/local/cuda/bin/cuobjdump") if c and os.path.exists(c)),
                 None)

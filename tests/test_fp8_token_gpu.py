@@ -3,7 +3,7 @@
 - ivb_norm_fwd_fp8_train: bf16 row, mean and rstd bit-identical to ivb_norm_fwd; E4M3 rows and scales bit-identical
   to ivb_norm_fwd_fp8; padding of every output keeps its bits.
 - ivb_fp8_quantize_cols_t: element by element against a float64 restatement of the scale rule, with tails in both
-  dimensions, a zero column and an Inf column; the same bits on two runs.
+  dimensions, a zero column, an Inf column and a NaN column; the same bits on two runs.
 - Row independence of the input-gradient GEMM: scaling one gradient row by a power of two leaves every other row of dx
   bit-identical.
 - The block at the block_cfg2 size against the bf16 block, and the mode end to end on the pretrain_tiny model.
@@ -91,6 +91,8 @@ def test_quantize_cols_t_against_float64(cuda_lib, N, K):
     w = wb[:, :K]
     w[:, 5] = 0                                       # a zero column
     w[N // 2, 7] = float("inf")                       # an Inf column
+    w[N // 3, 7] = -float("inf")
+    w[1, 9] = float("nan")                            # a NaN column
     ldt = _pad16(N) + 16
     runs = []
     for _ in range(2):
@@ -109,6 +111,11 @@ def test_quantize_cols_t_against_float64(cuda_lib, N, K):
     assert torch.equal(amax[:K].double()[fin], a_ref[fin]) and float(sinv[5]) == 1.0
     assert torch.equal(q_t[:, :N][fin], q_ref.view(torch.uint8)[fin])
     assert (q_t[:, N:] == NAN8).all() and torch.isnan(amax[K]) and torch.isnan(sinv[K])
+    # the non-finite columns: scale 1 and a satfinite cast, so an Inf becomes +-448 and a NaN stays NaN
+    for k in (7, 9):
+        col, nan = w[:, k].float(), torch.isnan(w[:, k].float())
+        assert torch.equal(q_t[k, :N][~nan], col.clamp(-448, 448).to(e4m3).view(torch.uint8)[~nan])
+        assert bool(((q_t[k, :N][nan] & 0x7f) == 0x7f).all()) and bool(torch.isnan(sinv[k]))
     # the lowlevel form: the rows of w^T, the same bits as the per-row cast of w^T
     qt3, s3 = ll.fp8_quantize_rows(w, transposed=True)
     assert torch.equal(qt3.view(torch.uint8), q_t[:, :N])

@@ -1,7 +1,8 @@
 """FP8 weight gradients (modules.set_fp8(model, scaling="token", wgrad=True)) on the H100 (gpu).
 
 - ivb_fp8_quantize_blocks_t: element by element and scale by scale against a float64 restatement of the rule, with a
-  partial last block, an all-zero block, a zero column, a block holding an Inf and sizes that are not multiples of 128;
+  partial last block, an all-zero block, a zero column, blocks holding an Inf or a NaN (their E4M3 bytes included) and
+  sizes that are not multiples of 128;
   two calls give the same bytes; the _plan form equals the plain cast of x with the dropped rows zeroed.
 - ivb_gemm_fp8_wgrad: accumulation ratio against float64 at the four cfg-2 weight-gradient shapes and at tails; the
   four epilogue forms; a K plan gives the unplanned call's bits when the plan's dead rows of dy are zero.
@@ -67,6 +68,7 @@ def test_quantize_blocks_t_against_float64(cuda_lib, Mx, C):
         x[128:256] = 0                                    # an all-zero block
     x[:, 3] = 0                                           # a zero column in every block
     x[Mx - 1, 5] = float("inf")                           # an Inf in the last (partial) block
+    x[0, 6] = float("nan")                                # a NaN in the first block
     ldt = _pad16(Mx) + 16
     nb = (Mx + 127) // 128
     runs = []
@@ -87,6 +89,12 @@ def test_quantize_blocks_t_against_float64(cuda_lib, Mx, C):
         assert bool((s[1] == 1.0).all()) and bool((q_t[:, 128:256] == 0).all())
     assert torch.equal(q_t[:, :Mx][fin], q_ref.view(torch.uint8)[fin])
     assert (q_t[:, Mx:] == NAN8).all() and torch.isnan(sinv[nb * C])
+    # the non-finite block columns: scale 1 and a satfinite cast, so an Inf becomes +-448 and a NaN stays NaN
+    for blk, c in (~sfin).nonzero().tolist():
+        col = x[128 * blk:128 * blk + 128, c].float()
+        got, nan = q_t[c, 128 * blk:128 * blk + col.numel()], torch.isnan(col)
+        assert torch.equal(got[~nan], col.clamp(-448, 448).to(e4m3).view(torch.uint8)[~nan])
+        assert bool(((got[nan] & 0x7f) == 0x7f).all())
     # the lowlevel form gives the same bits; the _plan form casts the rows whose factor is 0 as zeros
     q3, s3 = ll._fp8_quantize_blocks_t(x)
     assert torch.equal(q3.view(torch.uint8), q_t[:, :Mx]) and torch.equal(s3.view(torch.int32), s.view(torch.int32))
