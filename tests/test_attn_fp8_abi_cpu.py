@@ -10,28 +10,18 @@
    refuses attn_fp8 where it cannot run it.
 """
 import ctypes as C
-import os
 import re
-import shutil
-import subprocess
 
 import pytest
 import torch
 
-from internvideo_b200 import _lib, build
+import sass
+from abi_fake import BASE, cpu_only, expect_refusal
+from internvideo_b200 import _lib
 
-BASE = 1 << 32                               # fake, 256-byte aligned device addresses
 B, N, H, D = 2, 1025, 16, 64
 N16 = 1040
 SQ, SK, SV = BASE + 0x700000, BASE + 0x710000, BASE + 0x720000
-
-cpu_only = pytest.mark.skipif(torch.cuda.is_available(), reason="passes fake device pointers: CPU-only check")
-
-
-def _expect(rc, text):
-    lib = _lib.load()
-    assert rc != 0
-    assert text in lib.ivb_last_error().decode(), lib.ivb_last_error()
 
 
 def _pack(q=BASE, ldq=3 * H * D, k=BASE + 2 * H * D, ldk=3 * H * D, v=BASE + 4 * H * D, ldv=3 * H * D, b=B, n=N, h=H,
@@ -48,22 +38,22 @@ def _fwd(q8=BASE + 0x100000, k8=BASE + 0x200000, ld8=H * D, sq=SQ, sk=SK, vt8=BA
 def test_pack_refusals():
     P = "ivb_attn_fp8_pack: "
     for d in (60, 136, 8):
-        _expect(_pack(d=d), P + "head_dim must be a multiple of 8 in [16,128]")
+        expect_refusal(_pack(d=d), P + "head_dim must be a multiple of 8 in [16,128]")
     for kw in (dict(ldq=3 * H * D + 4), dict(ldk=1020), dict(ldv=3)):
-        _expect(_pack(**kw), P + "pitches must be multiples of 8")
+        expect_refusal(_pack(**kw), P + "pitches must be multiples of 8")
     for kw in (dict(q=None), dict(k=None), dict(v=None), dict(q8=None), dict(k8=None), dict(vt8=None), dict(sq=None),
                dict(sk=None), dict(sv=None)):
-        _expect(_pack(**kw), P + "an operand is null")
+        expect_refusal(_pack(**kw), P + "an operand is null")
     for ld8 in (H * D + 8, H * D - 16):
-        _expect(_pack(ld8=ld8), P + "ld8 must be a multiple of 16 and >= H*round_up(d, 32)")
-    _expect(_pack(d=88, ld8=16 * 88), P + "ld8 must be a multiple of 16 and >= H*round_up(d, 32)")
+        expect_refusal(_pack(ld8=ld8), P + "ld8 must be a multiple of 16 and >= H*round_up(d, 32)")
+    expect_refusal(_pack(d=88, ld8=16 * 88), P + "ld8 must be a multiple of 16 and >= H*round_up(d, 32)")
     for ldvt in (N, 1032, 1048):   # unpadded, a multiple of 8 below round_up(n, 16), not a multiple of 16
-        _expect(_pack(ldvt=ldvt), P + "ldvt must be a multiple of 16 and >= round_up(n, 16)")
+        expect_refusal(_pack(ldvt=ldvt), P + "ldvt must be a multiple of 16 and >= round_up(n, 16)")
     for kw in (dict(q=BASE + 8), dict(k=BASE + 2 * H * D + 8), dict(v=BASE + 8), dict(q8=BASE + 0x100008),
                dict(k8=BASE + 0x200008), dict(vt8=BASE + 0x300008)):
-        _expect(_pack(**kw), P + "q, k, v, q8, k8 and vt8 must be 16-byte aligned")
+        expect_refusal(_pack(**kw), P + "q, k, v, q8, k8 and vt8 must be 16-byte aligned")
     for kw in (dict(sq=SQ + 4), dict(sk=SK + 8), dict(sv=SV + 2)):
-        _expect(_pack(**kw), P + "q_scale_inv and k_scale_inv must be 16-byte aligned, v_scale_inv 4-byte")
+        expect_refusal(_pack(**kw), P + "q_scale_inv and k_scale_inv must be 16-byte aligned, v_scale_inv 4-byte")
     assert _pack(b=0) == 0 and _pack(n=0) == 0   # empty: a no-op, as ivb_attn_fwd
 
 
@@ -71,21 +61,21 @@ def test_pack_refusals():
 def test_fwd_refusals():
     P = "ivb_attn_fwd_fp8: "
     for d in (60, 136, 8):
-        _expect(_fwd(d=d), P + "head_dim must be a multiple of 8 in [16,128]")
-    _expect(_fwd(ldo=H * D + 4), P + "pitches must be multiples of 8")
+        expect_refusal(_fwd(d=d), P + "head_dim must be a multiple of 8 in [16,128]")
+    expect_refusal(_fwd(ldo=H * D + 4), P + "pitches must be multiples of 8")
     for kw in (dict(q8=None), dict(k8=None), dict(vt8=None), dict(out=None), dict(sq=None), dict(sk=None),
                dict(sv=None)):
-        _expect(_fwd(**kw), P + "an operand is null")
+        expect_refusal(_fwd(**kw), P + "an operand is null")
     for ld8 in (H * D + 8, H * D - 16):
-        _expect(_fwd(ld8=ld8), P + "ld8 must be a multiple of 16 and >= H*round_up(d, 32)")
-    _expect(_fwd(d=88, ld8=16 * 88), P + "ld8 must be a multiple of 16 and >= H*round_up(d, 32)")
+        expect_refusal(_fwd(ld8=ld8), P + "ld8 must be a multiple of 16 and >= H*round_up(d, 32)")
+    expect_refusal(_fwd(d=88, ld8=16 * 88), P + "ld8 must be a multiple of 16 and >= H*round_up(d, 32)")
     for ldvt in (N, 1032, 1048):
-        _expect(_fwd(ldvt=ldvt), P + "ldvt must be a multiple of 16 and >= round_up(n, 16)")
+        expect_refusal(_fwd(ldvt=ldvt), P + "ldvt must be a multiple of 16 and >= round_up(n, 16)")
     for kw in (dict(q8=BASE + 0x100008), dict(k8=BASE + 0x200008), dict(vt8=BASE + 0x300008), dict(sq=SQ + 4),
                dict(sk=SK + 8)):
-        _expect(_fwd(**kw), P + "q8, k8, vt8, q_scale_inv and k_scale_inv must be 16-byte aligned")
+        expect_refusal(_fwd(**kw), P + "q8, k8, vt8, q_scale_inv and k_scale_inv must be 16-byte aligned")
     for kw in (dict(sv=SV + 4), dict(out=BASE + 2)):
-        _expect(_fwd(**kw), P + "v_scale_inv must be 8-byte aligned, out 4-byte")
+        expect_refusal(_fwd(**kw), P + "v_scale_inv must be 8-byte aligned, out 4-byte")
     assert _fwd(b=0) == 0 and _fwd(n=0) == 0
 
 
@@ -102,24 +92,8 @@ def test_prototypes_match_the_header():
     assert [lib.ivb_attn_fp8_scale_pitch(n) for n in (1, 64, 65, 257, 1025, 2049)] == [64, 64, 128, 320, 1088, 2112]
 
 
-def _sass_functions(obj):
-    tool = next((c for c in (shutil.which("cuobjdump"), "/usr/local/cuda/bin/cuobjdump") if c and os.path.exists(c)), None)
-    if tool is None or not (build.OBJ / obj).exists():
-        pytest.skip(f"needs cuobjdump and the built internvideo_b200/build/{obj}")
-    text = subprocess.run([tool, "-sass", str(build.OBJ / obj)], capture_output=True, text=True, check=True).stdout
-    funcs, cur = {}, None
-    for line in text.splitlines():
-        m = re.search(r"Function : (\S+)", line)
-        if m:
-            cur = m.group(1)
-            funcs[cur] = []
-        elif cur is not None and re.match(r"\s+/\*[0-9a-f]{4,}\*/\s+\S", line):
-            funcs[cur].append(line)
-    return funcs
-
-
 def test_fp8_attention_kernels_sass():
-    funcs = _sass_functions("ivb_attn_fp8.o")
+    funcs = sass.functions("ivb_attn_fp8.o")
     fwd = {k: v for k, v in funcs.items() if "attn_fwd_fp8_kernel" in k}
     pack = {k: v for k, v in funcs.items() if "attn_fp8_pack_kernel" in k}
     assert len(fwd) == 4 and len(pack) == 1, sorted(funcs)     # NO = 32, 64, 96, 128

@@ -3,20 +3,17 @@ ivb_attn_fwd_plan and ivb_attn_bwd_plan extend the plain calls by one pointer, t
 point refuses a call it cannot run before any CUDA call, and the new kernels keep their accumulators in registers."""
 import ctypes as C
 import inspect
-import os
 import re
-import shutil
-import subprocess
 
 import pytest
 import torch
 
-from internvideo_b200 import _lib, build
+import sass
+from abi_fake import BASE, cpu_only, expect_refusal
+from internvideo_b200 import _lib
 from internvideo_b200 import lowlevel as ll
 
 P = _lib.PROTOTYPES
-BASE = 1 << 32                               # fake, 256-byte aligned device addresses
-cpu_only = pytest.mark.skipif(torch.cuda.is_available(), reason="passes fake device pointers: CPU-only check")
 
 EPI_BF16, EPI_RESID = 0, 3
 FLAG_ACCUM, FLAG_1CTA, FLAG_2CTA, FLAG_PINGPONG, FLAG_VEC = 2, 4, 8, 32, 64
@@ -51,12 +48,6 @@ def _fp8(flags=FLAG_VEC, fmt=0, lda=1024, ldb=1024, ld0=512, tile_n=0, m_plan=BA
                                          m_plan, None)
 
 
-def _expect(rc, text):
-    assert rc != 0
-    msg = _lib.load().ivb_last_error().decode()
-    assert text in msg, msg
-
-
 @cpu_only
 @pytest.mark.parametrize("kw, text", [
     (dict(flags=FLAG_VEC | FLAG_2CTA), "ivb_gemm_fp8_plan: no CTA-pair kernel"),
@@ -74,7 +65,7 @@ def _expect(rc, text):
     (dict(epi=EPI_RESID), "ivb_gemm_fp8_plan: epilogue needs aux"),
 ])
 def test_gemm_fp8_plan_refuses(kw, text):
-    _expect(_fp8(**kw), text)
+    expect_refusal(_fp8(**kw), text)
 
 
 D16 = 16 * 88
@@ -92,23 +83,23 @@ def _attn_bwd(rs=BASE + 0x900000, d=88, ld=LD_BWD, ws=1024):
 
 
 def test_attn_plan_needs_the_factors():
-    _expect(_attn_fwd(rs=None), "ivb_attn_fwd_plan: rowscale is null")
-    _expect(_attn_bwd(rs=None), "ivb_attn_bwd_plan: rowscale is null")
+    expect_refusal(_attn_fwd(rs=None), "ivb_attn_fwd_plan: rowscale is null")
+    expect_refusal(_attn_bwd(rs=None), "ivb_attn_bwd_plan: rowscale is null")
 
 
 @pytest.mark.parametrize("slot", range(8))
 def test_attn_plan_pitch_refused(slot):
     ld = list(LD_BWD)
     ld[slot] += 4
-    _expect(_attn_bwd(ld=ld), "ivb_attn_bwd_plan: pitches must be multiples of 8")
+    expect_refusal(_attn_bwd(ld=ld), "ivb_attn_bwd_plan: pitches must be multiples of 8")
     if slot < 4:
-        _expect(_attn_fwd(ld=ld[:4]), "ivb_attn_fwd_plan: pitches must be multiples of 8")
+        expect_refusal(_attn_fwd(ld=ld[:4]), "ivb_attn_fwd_plan: pitches must be multiples of 8")
 
 
 def test_attn_plan_head_dim_and_workspace_refused():
-    _expect(_attn_fwd(d=136), "ivb_attn_fwd_plan: head_dim must be a multiple of 8 in [16,128]")
-    _expect(_attn_bwd(d=12), "ivb_attn_bwd_plan: head_dim must be a multiple of 8 in [16,128]")
-    _expect(_attn_bwd(ws=1032), "ivb_attn_bwd_plan: workspace must be 16-byte aligned")
+    expect_refusal(_attn_fwd(d=136), "ivb_attn_fwd_plan: head_dim must be a multiple of 8 in [16,128]")
+    expect_refusal(_attn_bwd(d=12), "ivb_attn_bwd_plan: head_dim must be a multiple of 8 in [16,128]")
+    expect_refusal(_attn_bwd(ws=1032), "ivb_attn_bwd_plan: workspace must be 16-byte aligned")
 
 
 def test_bindings_refuse_a_bad_rowscale():
@@ -122,24 +113,10 @@ def test_bindings_refuse_a_bad_rowscale():
 
 
 # ---- the new kernels, from the objects build.py compiled
-def _cuobjdump(*args):
-    tool = next((c for c in (shutil.which("cuobjdump"), "/usr/local/cuda/bin/cuobjdump") if c and os.path.exists(c)), None)
-    if tool is None or not (build.OBJ / args[-1]).exists():
-        pytest.skip(f"needs cuobjdump and the built internvideo_b200/build/{args[-1]}")
-    return subprocess.run([tool, *args[:-1], str(build.OBJ / args[-1])], capture_output=True, text=True,
-                          check=True).stdout
-
-
-def _resources(obj):
-    """{mangled kernel name: (registers, stack bytes, local bytes)} of obj."""
-    return {m.group(1): tuple(map(int, m.group(2, 3, 4))) for m in
-            re.finditer(r"Function (\S+):\s+REG:(\d+) STACK:(\d+) SHARED:\d+ LOCAL:(\d+)", _cuobjdump("-res-usage", obj))}
-
-
 def test_planned_kernels_do_not_spill():
     """Every GEMM instantiation with the plan code (bf16 single-CTA, OpPlannedFp8) and every attention plan kernel:
     168 registers (384 threads, one CTA per SM), no stack and no local memory."""
-    res = {**_resources("ivb_gemm.o"), **_resources("ivb_attn.o"), **_resources("ivb_attn_bwd.o")}
+    res = {**sass.resources("ivb_gemm.o"), **sass.resources("ivb_attn.o"), **sass.resources("ivb_attn_bwd.o")}
     planned = {k: v for k, v in res.items() if "OpPlannedFp8" in k or re.search(r"attn_\w+_plan_kernelI", k)
                or ("OpBf16" in k and ("pingpong" in k or "Li1EEEv" in k))}
     assert sum("OpPlannedFp8" in k for k in planned) == 2, sorted(planned)          # ping-pong, cooperative at BN 128
@@ -149,25 +126,12 @@ def test_planned_kernels_do_not_spill():
         assert v == (168, 0, 0), k
 
 
-def _sass(obj):
-    """{mangled kernel name: [SASS instruction lines]} of obj."""
-    out, cur = {}, None
-    for line in _cuobjdump("-sass", obj).splitlines():
-        m = re.search(r"Function : (\S+)", line)
-        if m:
-            cur = m.group(1)
-            out[cur] = []
-        elif cur is not None and re.match(r"\s+/\*[0-9a-f]{4,}\*/\s+\S", line):
-            out[cur].append(line)
-    return out
-
-
 @pytest.mark.parametrize("obj, plain, planned", [("ivb_attn.o", "15attn_fwd_kernelI", "20attn_fwd_plan_kernelI"),
                                                  ("ivb_attn_bwd.o", "15attn_bwd_kernelI", "20attn_bwd_plan_kernelI")])
 def test_attn_plan_kernels_keep_the_mma_pipeline(obj, plain, planned):
     """A plan kernel runs its live CTAs as the plain kernel of the same head dim: the same wgmmas, the same waits on
     them (WARPGROUP.DEPBAR), no local memory; the dead CTA's exit only adds instructions in front."""
-    k = _sass(obj)
+    k = sass.functions(obj)
     plans = {n: v for n, v in k.items() if planned in n}
     assert len(plans) == len([n for n in k if plain in n]) > 0
     for n, lines in plans.items():

@@ -3,10 +3,10 @@ the tile order, live count and k-block list that clip-level reasoning predicts f
 the GEMM refuses a plan it cannot run before any CUDA call."""
 import numpy as np
 import pytest
-import torch
 
 from internvideo_b200 import _lib
 import droppath_ref as ref
+from abi_fake import BASE, cpu_only, expect_refusal
 
 B = 32
 DRAWS = {
@@ -57,7 +57,6 @@ def test_tile_live_when_any_row_kept():
 
 
 # ---- refusals, through the raw C ABI with fake device addresses (never reach a launch: CPU-only)
-BASE = 1 << 32
 EPI_BF16, EPI_F32, EPI_RESID = 0, 1, 3
 FLAG_ACCUM, FLAG_2CTA = 2, 8
 
@@ -69,7 +68,7 @@ def _call(a_mn=0, b_mn=0, epi=EPI_BF16, flags=0, bias=None, m_plan=None, k_plan=
                                           N if aux else 0, None, 0, m_plan, k_plan, None)
 
 
-@pytest.mark.skipif(torch.cuda.is_available(), reason="passes fake device pointers: CPU-only check")
+@cpu_only
 @pytest.mark.parametrize("kw, text", [
     (dict(flags=FLAG_2CTA, m_plan=BASE + 0x300000), "a DropPath plan needs a single-CTA kernel"),
     (dict(a_mn=1, b_mn=1, flags=FLAG_2CTA, k_plan=BASE + 0x300000), "a DropPath plan needs a single-CTA kernel"),
@@ -80,8 +79,7 @@ def _call(a_mn=0, b_mn=0, epi=EPI_BF16, flags=0, bias=None, m_plan=None, k_plan=
      "a K plan needs IVB_EPI_BF16 or IVB_EPI_F32"),
 ])
 def test_gemm_refuses_a_plan_it_cannot_run(kw, text):
-    assert _call(**kw) != 0
-    assert text in _lib.load().ivb_last_error().decode()
+    expect_refusal(_call(**kw), text)
 
 
 def test_fp8_gemm_takes_no_plan():

@@ -5,30 +5,19 @@
    must never reach a launch, so these checks run only where no CUDA device is visible.
 2. The SASS of the vector-scale GEMM kernels: E4M3 x E4M3 QGMMA, no local memory, one epilogue body.
 """
-import os
 import re
-import shutil
-import subprocess
 
 import pytest
-import torch
 
-from internvideo_b200 import _lib, build
+import sass
+from abi_fake import BASE, cpu_only, expect_refusal
+from internvideo_b200 import _lib
 
 EPI_BF16 = 0
 FLAG_2CTA, FLAG_VEC = 8, 64
 E4M3, E5M2 = 0, 1
-BASE = 1 << 32                               # fake, 256-byte aligned device addresses
 M, N, K = 417, 1000, 592
 SA, SB = BASE + 0x700000, BASE + 0x710000    # fake scale vectors
-
-cpu_only = pytest.mark.skipif(torch.cuda.is_available(), reason="passes fake device pointers: CPU-only check")
-
-
-def _expect(rc, text):
-    lib = _lib.load()
-    assert rc != 0
-    assert text in lib.ivb_last_error().decode(), lib.ivb_last_error()
 
 
 def _rows(x=BASE, ldx=K, m=M, k=K, out=BASE + 0x300000, ldo=608, sinv=SA):
@@ -47,68 +36,53 @@ def _gemm(a_fmt=E4M3, sa=SA, sb=SB, flags=FLAG_VEC):
 
 @cpu_only
 def test_quantize_rows_refusals():
-    _expect(_rows(m=0), "ivb_fp8_quantize_rows: empty tensor")
-    _expect(_rows(k=0), "ivb_fp8_quantize_rows: empty tensor")
-    _expect(_rows(k=16392, ldx=16392, ldo=16400), "ivb_fp8_quantize_rows: K > IVB_FP8_ROWS_MAX_K")
-    _expect(_rows(x=None), "ivb_fp8_quantize_rows: x, out or row_scale_inv is null")
-    _expect(_rows(out=None), "ivb_fp8_quantize_rows: x, out or row_scale_inv is null")
-    _expect(_rows(sinv=None), "ivb_fp8_quantize_rows: x, out or row_scale_inv is null")
-    _expect(_rows(ldx=K + 4), "ivb_fp8_quantize_rows: ldx must be a multiple of 8 elements and >= K")
-    _expect(_rows(ldx=584), "ivb_fp8_quantize_rows: ldx must be a multiple of 8 elements and >= K")
-    _expect(_rows(ldo=600), "ivb_fp8_quantize_rows: ldo must be a multiple of 16 elements and >= K")
-    _expect(_rows(ldo=576), "ivb_fp8_quantize_rows: ldo must be a multiple of 16 elements and >= K")
-    _expect(_rows(x=BASE + 8), "ivb_fp8_quantize_rows: x and out must be 16-byte aligned")
-    _expect(_rows(out=BASE + 0x300008), "ivb_fp8_quantize_rows: x and out must be 16-byte aligned")
-    _expect(_rows(sinv=SA + 2), "ivb_fp8_quantize_rows: row_scale_inv must be 4-byte aligned")
+    expect_refusal(_rows(m=0), "ivb_fp8_quantize_rows: empty tensor")
+    expect_refusal(_rows(k=0), "ivb_fp8_quantize_rows: empty tensor")
+    expect_refusal(_rows(k=16392, ldx=16392, ldo=16400), "ivb_fp8_quantize_rows: K > IVB_FP8_ROWS_MAX_K")
+    expect_refusal(_rows(x=None), "ivb_fp8_quantize_rows: x, out or row_scale_inv is null")
+    expect_refusal(_rows(out=None), "ivb_fp8_quantize_rows: x, out or row_scale_inv is null")
+    expect_refusal(_rows(sinv=None), "ivb_fp8_quantize_rows: x, out or row_scale_inv is null")
+    expect_refusal(_rows(ldx=K + 4), "ivb_fp8_quantize_rows: ldx must be a multiple of 8 elements and >= K")
+    expect_refusal(_rows(ldx=584), "ivb_fp8_quantize_rows: ldx must be a multiple of 8 elements and >= K")
+    expect_refusal(_rows(ldo=600), "ivb_fp8_quantize_rows: ldo must be a multiple of 16 elements and >= K")
+    expect_refusal(_rows(ldo=576), "ivb_fp8_quantize_rows: ldo must be a multiple of 16 elements and >= K")
+    expect_refusal(_rows(x=BASE + 8), "ivb_fp8_quantize_rows: x and out must be 16-byte aligned")
+    expect_refusal(_rows(out=BASE + 0x300008), "ivb_fp8_quantize_rows: x and out must be 16-byte aligned")
+    expect_refusal(_rows(sinv=SA + 2), "ivb_fp8_quantize_rows: row_scale_inv must be 4-byte aligned")
 
 
 @cpu_only
 def test_norm_fwd_fp8_refusals():
-    _expect(_norm(m=0), "ivb_norm_fwd_fp8: empty tensor")
+    expect_refusal(_norm(m=0), "ivb_norm_fwd_fp8: empty tensor")
     for d in (0, 1404, 4104):
-        _expect(_norm(d=d, ldx=4104, ldo=4112), "ivb_norm_fwd_fp8: D must be a multiple of 8 in [8, IVB_NORM_FP8_MAX_D]")
-    _expect(_norm(ldx=1412), "ivb_norm_fwd_fp8: ldx must be a multiple of 8 elements and >= D")
-    _expect(_norm(ldx=1400), "ivb_norm_fwd_fp8: ldx must be a multiple of 8 elements and >= D")
-    _expect(_norm(ldo=1416), "ivb_norm_fwd_fp8: ldo must be a multiple of 16 elements and >= D")
-    _expect(_norm(ldo=1392), "ivb_norm_fwd_fp8: ldo must be a multiple of 16 elements and >= D")
+        expect_refusal(_norm(d=d, ldx=4104, ldo=4112),
+                       "ivb_norm_fwd_fp8: D must be a multiple of 8 in [8, IVB_NORM_FP8_MAX_D]")
+    expect_refusal(_norm(ldx=1412), "ivb_norm_fwd_fp8: ldx must be a multiple of 8 elements and >= D")
+    expect_refusal(_norm(ldx=1400), "ivb_norm_fwd_fp8: ldx must be a multiple of 8 elements and >= D")
+    expect_refusal(_norm(ldo=1416), "ivb_norm_fwd_fp8: ldo must be a multiple of 16 elements and >= D")
+    expect_refusal(_norm(ldo=1392), "ivb_norm_fwd_fp8: ldo must be a multiple of 16 elements and >= D")
     for kw in (dict(x=None), dict(w=None), dict(out=None), dict(sinv=None)):
-        _expect(_norm(**kw), "ivb_norm_fwd_fp8: x, weight, out or row_scale_inv is null")
+        expect_refusal(_norm(**kw), "ivb_norm_fwd_fp8: x, weight, out or row_scale_inv is null")
     for kw in (dict(x=BASE + 8), dict(w=BASE + 0x100008), dict(b=BASE + 0x200008), dict(out=BASE + 0x300008)):
-        _expect(_norm(**kw), "ivb_norm_fwd_fp8: x, weight, bias and out must be 16-byte aligned")
-    _expect(_norm(sinv=SA + 2), "ivb_norm_fwd_fp8: row_scale_inv must be 4-byte aligned")
+        expect_refusal(_norm(**kw), "ivb_norm_fwd_fp8: x, weight, bias and out must be 16-byte aligned")
+    expect_refusal(_norm(sinv=SA + 2), "ivb_norm_fwd_fp8: row_scale_inv must be 4-byte aligned")
 
 
 @cpu_only
 def test_gemm_vector_scale_refusals():
-    _expect(_gemm(a_fmt=E5M2), "ivb_gemm_fp8: vector scales need an E4M3 A operand")
-    _expect(_gemm(sa=None), "ivb_gemm_fp8: scale_inv pointers are null")
-    _expect(_gemm(sb=None), "ivb_gemm_fp8: scale_inv pointers are null")
-    _expect(_gemm(flags=FLAG_VEC | FLAG_2CTA), "ivb_gemm_fp8: no CTA-pair kernel")
-    _expect(_gemm(sa=SA + 4), "ivb_gemm_fp8: scale vectors must be 8-byte aligned")
-    _expect(_gemm(sb=SB + 4), "ivb_gemm_fp8: scale vectors must be 8-byte aligned")
+    expect_refusal(_gemm(a_fmt=E5M2), "ivb_gemm_fp8: vector scales need an E4M3 A operand")
+    expect_refusal(_gemm(sa=None), "ivb_gemm_fp8: scale_inv pointers are null")
+    expect_refusal(_gemm(sb=None), "ivb_gemm_fp8: scale_inv pointers are null")
+    expect_refusal(_gemm(flags=FLAG_VEC | FLAG_2CTA), "ivb_gemm_fp8: no CTA-pair kernel")
+    expect_refusal(_gemm(sa=SA + 4), "ivb_gemm_fp8: scale vectors must be 8-byte aligned")
+    expect_refusal(_gemm(sb=SB + 4), "ivb_gemm_fp8: scale vectors must be 8-byte aligned")
 
 
 # ------------------------------------------------------------------------------------------------ SASS
-OBJ = build.OBJ / "ivb_gemm.o"
-
-
 @pytest.fixture(scope="module")
 def vec_kernels():
     """{kernel name: [SASS instruction lines]} of the vector-scale FP8 GEMM kernels (Op = OpVecFp8) in ivb_gemm.o."""
-    tool = next((c for c in (shutil.which("cuobjdump"), "/usr/local/cuda/bin/cuobjdump") if c and os.path.exists(c)),
-                None)
-    if tool is None or not OBJ.exists():
-        pytest.skip("needs cuobjdump and the built internvideo_b200/build/ivb_gemm.o")
-    text = subprocess.run([tool, "-sass", str(OBJ)], capture_output=True, text=True, check=True).stdout
-    out, cur = {}, None
-    for line in text.splitlines():
-        m = re.search(r"Function : (\S+)", line)
-        if m:
-            cur = m.group(1)
-            out[cur] = []
-        elif cur is not None and re.match(r"\s+/\*[0-9a-f]{4,}\*/\s+\S", line):
-            out[cur].append(line)
-    out = {k: v for k, v in out.items() if "OpVecFp8" in k}
+    out = {k: v for k, v in sass.functions("ivb_gemm.o").items() if "OpVecFp8" in k}
     assert len(out) == 3, sorted(out)     # ping-pong, cooperative BN 128 and 192
     return out
 

@@ -6,27 +6,16 @@
 2. The new kernels keep nothing in local memory.
 3. modules.set_fp8 takes the scaling, and block_precision resolves it.
 """
-import os
 import re
-import shutil
-import subprocess
 
 import pytest
-import torch
 
-from internvideo_b200 import _lib, build
+import sass
+from abi_fake import BASE, cpu_only, expect_refusal
+from internvideo_b200 import _lib
 
-BASE = 1 << 32                               # fake, 256-byte aligned device addresses
 M, D = 417, 1408
 SA, SB, SC = BASE + 0x700000, BASE + 0x710000, BASE + 0x720000    # fake per-row / per-column vectors
-
-cpu_only = pytest.mark.skipif(torch.cuda.is_available(), reason="passes fake device pointers: CPU-only check")
-
-
-def _expect(rc, text):
-    lib = _lib.load()
-    assert rc != 0
-    assert text in lib.ivb_last_error().decode(), lib.ivb_last_error()
 
 
 def _norm(x=BASE, x_f32=1, ldx=D, w=BASE + 0x100000, b=None, ln=1, m=M, d=D, out=BASE + 0x300000, ldo=D, sinv=SA,
@@ -42,41 +31,42 @@ def _cols(x=BASE, ldx=1416, m=600, k=1410, out_t=BASE + 0x300000, ldt=608, amax=
 @cpu_only
 def test_norm_fwd_fp8_train_refusals():
     P = "ivb_norm_fwd_fp8_train: "
-    _expect(_norm(m=0), P + "empty tensor")
+    expect_refusal(_norm(m=0), P + "empty tensor")
     for d in (0, 1404, 4104):
-        _expect(_norm(d=d, ldx=4104, ldo=4112, ldy=4104), P + "D must be a multiple of 8 in [8, IVB_NORM_FP8_MAX_D]")
-    _expect(_norm(ldx=1412), P + "ldx must be a multiple of 8 elements and >= D")
-    _expect(_norm(ldx=1400), P + "ldx must be a multiple of 8 elements and >= D")
-    _expect(_norm(ldo=1416), P + "ldo must be a multiple of 16 elements and >= D")
-    _expect(_norm(ldo=1392), P + "ldo must be a multiple of 16 elements and >= D")
-    _expect(_norm(ldy=1412), P + "ldy must be a multiple of 8 elements and >= D")
-    _expect(_norm(ldy=1400), P + "ldy must be a multiple of 8 elements and >= D")
+        expect_refusal(_norm(d=d, ldx=4104, ldo=4112, ldy=4104),
+                       P + "D must be a multiple of 8 in [8, IVB_NORM_FP8_MAX_D]")
+    expect_refusal(_norm(ldx=1412), P + "ldx must be a multiple of 8 elements and >= D")
+    expect_refusal(_norm(ldx=1400), P + "ldx must be a multiple of 8 elements and >= D")
+    expect_refusal(_norm(ldo=1416), P + "ldo must be a multiple of 16 elements and >= D")
+    expect_refusal(_norm(ldo=1392), P + "ldo must be a multiple of 16 elements and >= D")
+    expect_refusal(_norm(ldy=1412), P + "ldy must be a multiple of 8 elements and >= D")
+    expect_refusal(_norm(ldy=1400), P + "ldy must be a multiple of 8 elements and >= D")
     null = P + "x, weight, out, row_scale_inv, y, rstd or (LayerNorm) mean is null"
     for kw in (dict(x=None), dict(w=None), dict(out=None), dict(sinv=None), dict(y=None), dict(rstd=None),
                dict(mean=None)):
-        _expect(_norm(**kw), null)
+        expect_refusal(_norm(**kw), null)
     for kw in (dict(x=BASE + 8), dict(w=BASE + 0x100008), dict(b=BASE + 0x200008), dict(out=BASE + 0x300008),
                dict(y=BASE + 0x400008)):
-        _expect(_norm(**kw), P + "x, weight, bias, out and y must be 16-byte aligned")
+        expect_refusal(_norm(**kw), P + "x, weight, bias, out and y must be 16-byte aligned")
     for kw in (dict(sinv=SA + 2), dict(mean=SB + 2), dict(rstd=SC + 2)):
-        _expect(_norm(**kw), P + "row_scale_inv, mean and rstd must be 4-byte aligned")
+        expect_refusal(_norm(**kw), P + "row_scale_inv, mean and rstd must be 4-byte aligned")
 
 
 @cpu_only
 def test_quantize_cols_t_refusals():
     P = "ivb_fp8_quantize_cols_t: "
-    _expect(_cols(m=0), P + "empty tensor")
-    _expect(_cols(k=0), P + "empty tensor")
+    expect_refusal(_cols(m=0), P + "empty tensor")
+    expect_refusal(_cols(k=0), P + "empty tensor")
     for kw in (dict(x=None), dict(out_t=None), dict(amax=None), dict(sinv=None)):
-        _expect(_cols(**kw), P + "x, out_t, col_amax or col_scale_inv is null")
-    _expect(_cols(ldx=1412), P + "ldx must be a multiple of 8 elements and >= K")
-    _expect(_cols(ldx=1408), P + "ldx must be a multiple of 8 elements and >= K")
-    _expect(_cols(ldt=600), P + "ldt must be a multiple of 16 elements and >= M")
-    _expect(_cols(ldt=592), P + "ldt must be a multiple of 16 elements and >= M")
-    _expect(_cols(x=BASE + 8), P + "x and out_t must be 16-byte aligned")
-    _expect(_cols(out_t=BASE + 0x300008), P + "x and out_t must be 16-byte aligned")
-    _expect(_cols(amax=SA + 2), P + "col_amax and col_scale_inv must be 4-byte aligned")
-    _expect(_cols(sinv=SB + 2), P + "col_amax and col_scale_inv must be 4-byte aligned")
+        expect_refusal(_cols(**kw), P + "x, out_t, col_amax or col_scale_inv is null")
+    expect_refusal(_cols(ldx=1412), P + "ldx must be a multiple of 8 elements and >= K")
+    expect_refusal(_cols(ldx=1408), P + "ldx must be a multiple of 8 elements and >= K")
+    expect_refusal(_cols(ldt=600), P + "ldt must be a multiple of 16 elements and >= M")
+    expect_refusal(_cols(ldt=592), P + "ldt must be a multiple of 16 elements and >= M")
+    expect_refusal(_cols(x=BASE + 8), P + "x and out_t must be 16-byte aligned")
+    expect_refusal(_cols(out_t=BASE + 0x300008), P + "x and out_t must be 16-byte aligned")
+    expect_refusal(_cols(amax=SA + 2), P + "col_amax and col_scale_inv must be 4-byte aligned")
+    expect_refusal(_cols(sinv=SB + 2), P + "col_amax and col_scale_inv must be 4-byte aligned")
 
 
 @pytest.mark.parametrize("obj, pattern, count", [("ivb_norm.o", "norm_fwd_fp8_train_kernel", 16),
@@ -84,21 +74,7 @@ def test_quantize_cols_t_refusals():
                                                  ("ivb_fp8.o", "fp8_(amax|cast|col_amax|cast_cols|rows|blocks_t)_kernel",
                                                   10)])
 def test_new_kernels_keep_nothing_in_local_memory(obj, pattern, count):
-    tool = next((c for c in (shutil.which("cuobjdump"), "/usr/local/cuda/bin/cuobjdump") if c and os.path.exists(c)),
-                None)
-    path = build.OBJ / obj
-    if tool is None or not path.exists():
-        pytest.skip(f"needs cuobjdump and the built internvideo_b200/build/{obj}")
-    text = subprocess.run([tool, "-sass", str(path)], capture_output=True, text=True, check=True).stdout
-    funcs, cur = {}, None
-    for line in text.splitlines():
-        m = re.search(r"Function : (\S+)", line)
-        if m:
-            cur = m.group(1)
-            funcs[cur] = []
-        elif cur is not None:
-            funcs[cur].append(line)
-    found = {k: v for k, v in funcs.items() if re.search(pattern, k)}
+    found = {k: v for k, v in sass.functions(obj).items() if re.search(pattern, k)}
     assert len(found) == count, sorted(found)
     for name, lines in found.items():
         assert not any(re.search(r"\b(LDL|STL)\b", l) for l in lines), name

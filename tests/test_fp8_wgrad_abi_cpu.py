@@ -8,26 +8,16 @@
 4. set_fp8's wgrad switch resolves to ops.FP8_TOKEN_WGRAD, and is refused with per-tensor scaling.
 """
 import ctypes as C
-import os
 import re
-import shutil
-import subprocess
 
 import pytest
 import torch
 
-from internvideo_b200 import _lib, build
+import sass
+from abi_fake import BASE, cpu_only, expect_refusal
+from internvideo_b200 import _lib
 
-BASE = 1 << 32                               # fake, 256-byte aligned device addresses
 SA, SB, PLAN = BASE + 0x700000, BASE + 0x710000, BASE + 0x720000
-
-cpu_only = pytest.mark.skipif(torch.cuda.is_available(), reason="passes fake device pointers: CPU-only check")
-
-
-def _expect(rc, text):
-    lib = _lib.load()
-    assert rc != 0
-    assert text in lib.ivb_last_error().decode(), lib.ivb_last_error()
 
 
 def _cast(x=BASE, ldx=1416, m=1251, c=1408, out_t=BASE + 0x300000, ldt=1264, sinv=SA, rs=None, plan=False):
@@ -47,47 +37,47 @@ def _wgrad(a=BASE, lda=1264, sa=SA, b=BASE + 0x100000, ldb=1264, sb=SB, m=1408, 
 def test_quantize_blocks_t_refusals(plan):
     P = ("ivb_fp8_quantize_blocks_t_plan: " if plan else "ivb_fp8_quantize_blocks_t: ")
     kw0 = dict(plan=plan, rs=SB if plan else None)
-    _expect(_cast(m=0, **kw0), P + "empty tensor")
-    _expect(_cast(c=0, **kw0), P + "empty tensor")
-    _expect(_cast(c=1404, **kw0), P + "C must be a multiple of 8")
+    expect_refusal(_cast(m=0, **kw0), P + "empty tensor")
+    expect_refusal(_cast(c=0, **kw0), P + "empty tensor")
+    expect_refusal(_cast(c=1404, **kw0), P + "C must be a multiple of 8")
     for kw in (dict(x=None), dict(out_t=None), dict(sinv=None)):
-        _expect(_cast(**kw, **kw0), P + "x, out_t or scale_inv is null")
-    _expect(_cast(ldx=1412, **kw0), P + "ldx must be a multiple of 8 elements and >= C")
-    _expect(_cast(ldx=1400, **kw0), P + "ldx must be a multiple of 8 elements and >= C")
-    _expect(_cast(ldt=1256, **kw0), P + "ldt must be a multiple of 16 elements and >= M")
-    _expect(_cast(ldt=1240, **kw0), P + "ldt must be a multiple of 16 elements and >= M")
-    _expect(_cast(x=BASE + 8, **kw0), P + "x and out_t must be 16-byte aligned")
-    _expect(_cast(out_t=BASE + 0x300008, **kw0), P + "x and out_t must be 16-byte aligned")
-    _expect(_cast(sinv=SA + 2, **kw0), P + "scale_inv and rowscale must be 4-byte aligned")
+        expect_refusal(_cast(**kw, **kw0), P + "x, out_t or scale_inv is null")
+    expect_refusal(_cast(ldx=1412, **kw0), P + "ldx must be a multiple of 8 elements and >= C")
+    expect_refusal(_cast(ldx=1400, **kw0), P + "ldx must be a multiple of 8 elements and >= C")
+    expect_refusal(_cast(ldt=1256, **kw0), P + "ldt must be a multiple of 16 elements and >= M")
+    expect_refusal(_cast(ldt=1240, **kw0), P + "ldt must be a multiple of 16 elements and >= M")
+    expect_refusal(_cast(x=BASE + 8, **kw0), P + "x and out_t must be 16-byte aligned")
+    expect_refusal(_cast(out_t=BASE + 0x300008, **kw0), P + "x and out_t must be 16-byte aligned")
+    expect_refusal(_cast(sinv=SA + 2, **kw0), P + "scale_inv and rowscale must be 4-byte aligned")
     if plan:
-        _expect(_cast(plan=True, rs=SB + 2), P + "scale_inv and rowscale must be 4-byte aligned")
-        _expect(_cast(plan=True, rs=None), P + "rowscale is null")
+        expect_refusal(_cast(plan=True, rs=SB + 2), P + "scale_inv and rowscale must be 4-byte aligned")
+        expect_refusal(_cast(plan=True, rs=None), P + "rowscale is null")
 
 
 @cpu_only
 def test_gemm_fp8_wgrad_refusals():
     P = "ivb_gemm_fp8_wgrad: "
     for kw in (dict(m=0), dict(n=0), dict(k=0)):
-        _expect(_wgrad(**kw), P + "empty problem")
+        expect_refusal(_wgrad(**kw), P + "empty problem")
     for kw in (dict(a=None), dict(b=None)):
-        _expect(_wgrad(**kw), P + "A_t or B_t is null")
+        expect_refusal(_wgrad(**kw), P + "A_t or B_t is null")
     for kw in (dict(lda=1256), dict(ldb=1256), dict(lda=1240), dict(ldb=1272)):
-        _expect(_wgrad(**kw), P + "lda and ldb must be multiples of 16 elements and >= K")
+        expect_refusal(_wgrad(**kw), P + "lda and ldb must be multiples of 16 elements and >= K")
     for kw in (dict(m=1404), dict(n=4220, ld0=4224)):
-        _expect(_wgrad(**kw), P + "M and N must be multiples of 8")
+        expect_refusal(_wgrad(**kw), P + "M and N must be multiples of 8")
     for kw in (dict(ld0=4228), dict(ld0=4216)):
-        _expect(_wgrad(**kw), P + "ld0 must be a multiple of 8 elements and >= N")
+        expect_refusal(_wgrad(**kw), P + "ld0 must be a multiple of 8 elements and >= N")
     for kw in (dict(sa=None), dict(sb=None)):
-        _expect(_wgrad(**kw), P + "scale_inv pointers are null")
+        expect_refusal(_wgrad(**kw), P + "scale_inv pointers are null")
     for kw in (dict(sa=SA + 8), dict(sb=SB + 4)):
-        _expect(_wgrad(**kw), P + "scale vectors must be 16-byte aligned")
+        expect_refusal(_wgrad(**kw), P + "scale vectors must be 16-byte aligned")
     for epi in (2, 3, 4, 7):
-        _expect(_wgrad(epi=epi), P + "epilogue must be IVB_EPI_BF16 or IVB_EPI_F32")
+        expect_refusal(_wgrad(epi=epi), P + "epilogue must be IVB_EPI_BF16 or IVB_EPI_F32")
     # ping-pong, CTA pair, forced cooperative, GELU flags, vector scales: one kernel form, and no other epilogue input
     for flags in (32, 8, 4, 1, 16, 64, 2 | 32):
-        _expect(_wgrad(flags=flags), P + "the only flag is IVB_FLAG_ACCUM")
-    _expect(_wgrad(out0=None), P + "out0 is null")
-    _expect(_wgrad(out0=BASE + 0x300008), P + "out0 must be 16-byte aligned")
+        expect_refusal(_wgrad(flags=flags), P + "the only flag is IVB_FLAG_ACCUM")
+    expect_refusal(_wgrad(out0=None), P + "out0 is null")
+    expect_refusal(_wgrad(out0=BASE + 0x300008), P + "out0 must be 16-byte aligned")
 
 
 def test_prototypes_match_the_header():
@@ -105,19 +95,9 @@ def test_prototypes_match_the_header():
     assert len(P["ivb_gemm_fp8"][1]) == 25
 
 
-def _cuobjdump(*args):
-    tool = next((c for c in (shutil.which("cuobjdump"), "/usr/local/cuda/bin/cuobjdump") if c and os.path.exists(c)), None)
-    if tool is None or not (build.OBJ / args[-1]).exists():
-        pytest.skip(f"needs cuobjdump and the built internvideo_b200/build/{args[-1]}")
-    return subprocess.run([tool, *args[:-1], str(build.OBJ / args[-1])], capture_output=True, text=True,
-                          check=True).stdout
-
-
 @pytest.mark.parametrize("obj, pattern", [("ivb_fp8.o", r"fp8_blocks_t_kernel"), ("ivb_gemm.o", r"OpBlockFp8")])
 def test_new_kernels_use_no_local_memory_and_no_stack(obj, pattern):
-    res = {m.group(1): tuple(map(int, m.group(2, 3, 4))) for m in
-           re.finditer(r"Function (\S+):\s+REG:(\d+) STACK:(\d+) SHARED:\d+ LOCAL:(\d+)", _cuobjdump("-res-usage", obj))}
-    found = {k: v for k, v in res.items() if re.search(pattern, k)}
+    found = {k: v for k, v in sass.resources(obj).items() if re.search(pattern, k)}
     assert len(found) == 1, sorted(found)
     for name, (regs, stack, local) in found.items():
         assert stack == 0 and local == 0, (name, regs, stack, local)
@@ -126,16 +106,7 @@ def test_new_kernels_use_no_local_memory_and_no_stack(obj, pattern):
 
 
 def test_block_fp8_gemm_issues_e4m3_qgmma_and_no_local_memory():
-    text = _cuobjdump("-sass", "ivb_gemm.o")
-    funcs, cur = {}, None
-    for line in text.splitlines():
-        m = re.search(r"Function : (\S+)", line)
-        if m:
-            cur = m.group(1)
-            funcs[cur] = []
-        elif cur is not None and re.match(r"\s+/\*[0-9a-f]{4,}\*/\s+\S", line):
-            funcs[cur].append(line)
-    (name, lines), = [(k, v) for k, v in funcs.items() if "OpBlockFp8" in k]
+    (name, lines), = [(k, v) for k, v in sass.functions("ivb_gemm.o").items() if "OpBlockFp8" in k]
     q = [l for l in lines if re.search(r"\bQGMMA\.", l)]
     assert q and all(re.search(r"QGMMA\.64x128x32\.F32\.E4M3\.E4M3\b", l) for l in q), name
     assert not any(re.search(r"\b(LDL|STL|HGMMA)\b", l) for l in lines), name

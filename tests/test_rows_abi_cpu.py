@@ -4,20 +4,12 @@ its message in ivb_last_error().  ivb_gather_add and ivb_scatter_add move rows i
 ivb_im2col_visible moves 4-byte words, so its video and cols need 4-byte alignment.  The refused calls pass null or fake device addresses; were a check missing, the call would go on to
 launch a kernel on them, so those cases run only where no CUDA device is present."""
 import pytest
-import torch
 
+from abi_fake import cpu_only, expect_refusal
 from internvideo_b200 import _lib
-
-no_device = pytest.mark.skipif(torch.cuda.is_available(), reason="passes fake device addresses")
 
 A = 1 << 20          # a fake 16-byte aligned device address
 M, D = 417, 1408
-
-
-def _expect(rc, text):
-    lib = _lib.load()
-    assert rc != 0
-    assert text in lib.ivb_last_error().decode(), lib.ivb_last_error()
 
 
 # One call per entry point, taking a {operand: address} dict and a {pitch name: pitch} dict (default pitch D).
@@ -130,29 +122,30 @@ def _ptrs(entry, **override):
     return p
 
 
-@no_device
+@cpu_only
 @pytest.mark.parametrize("entry,operand", ROW_OPERANDS)
 def test_misaligned_row_operand_refused(entry, operand):
     """A view starting at a column that is not a multiple of 8 (bf16) or 4 (fp32) is refused, not read or written
     with misaligned vector accesses."""
     call = ENTRIES[entry][0]
-    _expect(call(_ptrs(entry, **{operand: A + 8}), {}), f"{entry}: ")
+    expect_refusal(call(_ptrs(entry, **{operand: A + 8}), {}), f"{entry}: ")
     assert "aligned" in _lib.load().ivb_last_error().decode()
 
 
-@no_device
+@cpu_only
 @pytest.mark.parametrize("operand", ["weight", "gamma"])
 def test_fused_layerscale_weight_gamma_need_8_bytes(operand):
     """The bulk-copy kernel reads weight and gamma 4 bf16 at a time: 8-byte alignment is its rule for them."""
-    _expect(_bwd_layerscale(_ptrs("ivb_rmsnorm_bwd_layerscale", **{operand: A + 4}), {}),
-            "weight and gamma 8-byte aligned")
+    expect_refusal(_bwd_layerscale(_ptrs("ivb_rmsnorm_bwd_layerscale", **{operand: A + 4}), {}),
+                   "weight and gamma 8-byte aligned")
 
 
-@no_device
+@cpu_only
 @pytest.mark.parametrize("operand", ["video", "cols"])
 def test_im2col_video_cols_need_4_bytes(operand):
     """im2col_visible reads and writes 2 bf16 at a time: a view starting at an odd element is refused."""
-    _expect(_im2col(_ptrs("ivb_im2col_visible", **{operand: A + 2}), {}), "video and cols must be 4-byte aligned")
+    expect_refusal(_im2col(_ptrs("ivb_im2col_visible", **{operand: A + 2}), {}),
+                   "video and cols must be 4-byte aligned")
 
 
 # the refusal text of each entry point's pitch check (default: the norm and loss kernels')
@@ -160,7 +153,7 @@ PITCH_TEXT = {"ivb_gather_add": "src_bstride and out_bstride must be multiples o
               "ivb_scatter_add": "g_bstride must be a multiple of 8"}
 
 
-@no_device
+@cpu_only
 @pytest.mark.parametrize("entry,pitch", [("ivb_norm_bwd", "lddx_in"), ("ivb_norm_bwd", "lddx"),
                                          ("ivb_ln_l2_fwd", "ldo"), ("ivb_ln_l2_fwd", "ldt"),
                                          ("ivb_layerscale_bwd", "ldy"), ("ivb_layerscale_bwd", "lddx"),
@@ -170,7 +163,7 @@ PITCH_TEXT = {"ivb_gather_add": "src_bstride and out_bstride must be multiples o
 @pytest.mark.parametrize("bad", [D + 4, D + 1])
 def test_bad_pitch_refused(entry, pitch, bad):
     call = ENTRIES[entry][0]
-    _expect(call(_ptrs(entry), {pitch: bad}), f"{entry}: ")
+    expect_refusal(call(_ptrs(entry), {pitch: bad}), f"{entry}: ")
     assert PITCH_TEXT.get(entry, "/ld must be multiples of 8") in _lib.load().ivb_last_error().decode()
 
 

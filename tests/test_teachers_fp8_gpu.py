@@ -3,7 +3,7 @@
 Bounds.  Every GEMM of a switched block reads two E4M3 operands, each rounded with relative error at most
 u = 2^-4 per element (per-row and per-channel power-of-two scales keep every element in E4M3's normal range unless it is
 below 2^-6 of its row's amax), so each product, and the Frobenius norm of each branch, errs by at most 2u = 0.125
-relative to the bf16 block (the bound tests/test_block_fp8_gpu.py uses).
+relative to the bf16 block (the bound tests/test_fp8_modes_gpu.py uses).
 
 For the whole teachers: a tap is t = z / |z| of a token's fp32 stream z.  For unit t_bf16,
     |t_fp8 - t_bf16| <= 2 |z_fp8 - z_bf16| / |z_bf16|,
