@@ -324,6 +324,19 @@ int ivb_attn_bwd_plan(const void* q, long ldq, const void* k, long ldk, const vo
                       const void* out, long ldo, const void* dout, long lddo, const float* lse2,
                       float* delta_ws, void* dq, long lddq, void* dk, long lddk, void* dv, long lddv,
                       int B, int n, int H, int d, float softmax_scale, const float* rowscale, void* stream);
+/* ivb_attn_fwd_causal / ivb_attn_bwd_causal: ivb_attn_fwd / ivb_attn_bwd with a causal mask, key index > query index
+ * masked out (the additive -inf upper triangle of the MobileCLIP text tower, text_encoder.py:149-158, 185-191), with
+ * the same operands, operand rules and workspace.  Every row keeps its own key, so no row is empty.  The forward and
+ * the dQ pass stream the key tiles up to the one that holds the CTA's last query, the dK/dV pass the query tiles from
+ * the one that holds the CTA's first key; only the tiles that cross the diagonal are masked element by element.  There
+ * is no causal form of the DropPath plans or of the FP8 forward.                                                      */
+int ivb_attn_fwd_causal(const void* q, long ldq, const void* k, long ldk, const void* v, long ldv,
+                        void* out, long ldo, float* lse2, int B, int n, int H, int d, float softmax_scale,
+                        void* stream);
+int ivb_attn_bwd_causal(const void* q, long ldq, const void* k, long ldk, const void* v, long ldv,
+                        const void* out, long ldo, const void* dout, long lddo, const float* lse2,
+                        float* delta_ws, void* dq, long lddq, void* dk, long lddk, void* dv, long lddv,
+                        int B, int n, int H, int d, float softmax_scale, void* stream);
 /* ---- FP8 attention forward (FP8 inference of frozen towers; no lse, no backward) ------------------------------------
  * Every scale is a power of two chosen from an amax by the ivb_fp8_quantize_rows rule (E4M3; 1 when the amax is 0,
  * scale_inv NaN when the amax is Inf or NaN), so dequantisation is exact.  Same bits on every run; one stream-ordered
@@ -374,6 +387,23 @@ int ivb_gather_add(const float* src, long src_bstride, const void* table, const 
  * added in order; when idx[b,:] has no repeats within a clip the result is the same on every run. */
 int ivb_scatter_add(const void* g, int g_is_f32, long g_bstride, const int* idx, int idx_bstride,
                     int idx_off, int B, int rows, int D, float* table_grad, void* stream);
+
+/* ---- text-tower token embedding (MobileCLIP TextTransformer.forward_embedding, text_encoder.py:131-147) ------------
+ * ivb_token_embed_fwd: out[b*L + l, :] = table[ids[b, l]] + pos[l] in fp32 (the residual stream; pitch ldo).  ids:
+ *   int64 [B, L] (8-byte aligned); table: bf16 [V, D]; pos: bf16 [L, D].  An id outside [0, V) sets *err_flag (int32,
+ *   device) to 1 + its row and reads table row 0 instead; nothing is read by the host.
+ * ivb_token_embed_bwd: dtable[v] = sum of g[p] over the positions p with ids[p] == v, in position order, for every id
+ *   present (the other rows of dtable are not written: zero them first); dpos[l] = sum over b = 0 .. B-1 of
+ *   g[b*L + l].  g fp32 [B*L, D] (pitch ldg), dtable fp32 [V, D], dpos fp32 [L, D], all written, not accumulated.  No
+ *   float atomics: the positions are sorted by id in ws (int32, ivb_token_embed_bwd_workspace_ints(V, B, L) elements),
+ *   so the same inputs give the same bits on every run.  Out-of-range ids count as id 0, as in the forward.
+ * D, ldo and ldg are multiples of 8; table, pos, out, g, dtable and dpos are 16-byte aligned.  Stream-ordered;
+ *   capturable in a CUDA graph.  A call that breaks a rule is refused before any CUDA call.                          */
+int ivb_token_embed_fwd(const long long* ids, int B, int L, const void* table, int V, const void* pos, int D,
+                        float* out, long ldo, int* err_flag, void* stream);
+long ivb_token_embed_bwd_workspace_ints(int V, int B, int L);
+int ivb_token_embed_bwd(const long long* ids, int B, int L, const float* g, long ldg, int V, int D, float* dtable,
+                        float* dpos, int* ws, void* stream);
 
 /* ---- decoder heads: LayerNorm(1e-5) -> x/||x|| (+ optional fused (2-2<out,tgt>) loss sum) --------
  * Linear_Decoder / MLP_Decoder.forward tail (internvideo2_pretrain.py:356-359, 394-397) and the

@@ -6,8 +6,8 @@ Mirrors (constructor kwargs, attribute names, state_dict keys, forward contracts
   InternVideo2/multi_modality/models/internvideo2_clip_small.py:18-257                           `InternVideo2_CLIP_small`
   InternVideo2/multi_modality/models/backbones/internvideo2/pos_embed.py:137-182                 `interpolate_pos_embed`
 
-The text tower (MobileCLIP `TextTransformer`, mobileclip/ sub-package) is OUT of the hot path (SURVEY §8): the
-wrapper takes any module/callable as `text_encoder`; the default accepts pre-computed text embeddings.
+The wrapper takes any module/callable as `text_encoder`: text_modules.TextTransformer is the recipe's MobileCLIP-B tower
+on the libivb200 kernels; the default accepts pre-computed text embeddings.
 """
 from __future__ import annotations
 
@@ -95,6 +95,8 @@ class InternVideo2_CLIP_small(nn.Module):
             for name, p in self.vision_encoder.named_parameters():
                 if not (_get(m, "open_vision_clip_projector", False) and name.startswith("clip_projector")):
                     p.requires_grad = False
+        # The reference's loop (internvideo2_clip_small.py:55-58) logs "Freeze" but never sets requires_grad, so its text
+        # tower keeps training; here freeze_text freezes it.  Leave freeze_text off to train the tower end to end.
         if _get(m, "freeze_text", False) and isinstance(self.text_encoder, nn.Module):
             for name, p in self.text_encoder.named_parameters():
                 if not (_get(m, "open_text_projection", False) and name.startswith("projection_layer")):

@@ -1,4 +1,4 @@
-// ivb_attn.cu — non-causal multi-head attention forward on Hopper wgmma (flash-style, online softmax).
+// ivb_attn.cu — multi-head attention forward, non-causal or causal, on Hopper wgmma (flash-style, online softmax).
 //
 // Stands in for FA2 flash_attn_varlen_qkvpacked_func as called by the reference's
 // FlashAttention.forward (InternVideo2/single_modality/models/flash_attention_class.py:47-50) and for
@@ -33,7 +33,8 @@ struct AttnFwdParams {
 // KA: number of 64-wide atoms covering head_dim (1: d<=64, 2: d<=128).  NO: wgmma N of P·V (d rounded up).
 // KS: k16 steps of S = Q K^T, ceil(d / 16).
 // PLAN: the CTA of a dropped clip (attn_prologue) writes zeros to its out rows and lse2 0, a finite value, to its rows.
-template <int KA, int NO, int KS, bool PLAN>
+// CAUSAL: key tiles stream up to causal_tile_end, and a warpgroup masks the tiles that cross its diagonal.
+template <int KA, int NO, int KS, bool PLAN, bool CAUSAL = false>
 __device__ __forceinline__ void attn_fwd(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV,
                                          const AttnFwdParams& p, const float* rowscale) {
   using Smem = FwdSmem<KA>;
@@ -45,12 +46,13 @@ __device__ __forceinline__ void attn_fwd(const CUtensorMap& tmQ, const CUtensorM
         p.lse2[(static_cast<long>(c.b) * p.H + c.h) * p.n + c.row0 + r] = 0.0f;
     return;
   }
+  const int nblk = CAUSAL ? causal_tile_end(c, p.n) : c.nblk;
   attn_roles(c, [&] {
     // ===================== TMA producer =====================
     tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmK); tma_prefetch_desc(&tmV);
     mbar_expect_tx(Smem::bar_row(), Smem::ROW_BYTES);
     load_head_rows<KA, ATT_ROWS>(Smem::rows(0), &tmQ, c.h, c.row0, c.b, Smem::bar_row());
-    for (int j = 0; j < c.nblk; ++j) {
+    for (int j = 0; j < nblk; ++j) {
       const RingSlot<ATT_NS> s(j);
       mbar_wait(Smem::empty(0, s.st), s.ph ^ 1);
       mbar_expect_tx(Smem::full(0, s.st), Smem::TILE_BYTES);
@@ -72,6 +74,10 @@ __device__ __forceinline__ void attn_fwd(const CUtensorMap& tmQ, const CUtensorM
     float s[ATT_COLS / 2];
     float alpha[2];
     uint32_t pa[ATT_COLS / 16][4];
+    const int q0 = c.row0 + c.rloc;       // this thread's first query row
+    auto mask = [&](int j) {              // CAUSAL: tile j holds a key after one of the warpgroup's queries
+      if (CAUSAL && (j + 1) * ATT_COLS > c.row0 + cw * 64) causal_mask_tile<false>(s, q0, j * ATT_COLS, c.lane);
+    };
 
     auto issue_s = [&](int j) {
       const uint32_t ka = smem_u32(Smem::tile(0, RingSlot<ATT_NS>(j).st));
@@ -91,6 +97,7 @@ __device__ __forceinline__ void attn_fwd(const CUtensorMap& tmQ, const CUtensorM
     wgmma_wait<0>();
     wgmma_reg_fence(s, ATT_COLS / 2);
     if (c.signal) mbar_arrive(Smem::empty(0, 0));
+    mask(0);
     softmax_tile(s, p.n, c.lane, p.sc_log2, m_run, l_run, alpha);
 #pragma unroll
     for (int kk = 0; kk < ATT_COLS / 16; ++kk) acc_to_a_frag(s, kk, pa[kk]);
@@ -105,7 +112,7 @@ __device__ __forceinline__ void attn_fwd(const CUtensorMap& tmQ, const CUtensorM
         Wgmma<NO>::rs<1>(o, pa[kk], gmma_desc(va + kk * 2048, ATT_COLS * 128, 1024), 1u);
       wgmma_commit();
     };
-    for (int j = 0; j + 1 < c.nblk; ++j) {
+    for (int j = 0; j + 1 < nblk; ++j) {
       const RingSlot<ATT_NS> k(j + 1);
       mbar_wait(Smem::full(0, k.st), k.ph);
       issue_s(j + 1);
@@ -113,6 +120,7 @@ __device__ __forceinline__ void attn_fwd(const CUtensorMap& tmQ, const CUtensorM
       wgmma_wait<1>();
       wgmma_reg_fence(s, ATT_COLS / 2);
       if (c.signal) mbar_arrive(Smem::empty(0, k.st));
+      mask(j + 1);
       softmax_tile(s, p.n - (j + 1) * ATT_COLS, c.lane, p.sc_log2, m_run, l_run, alpha);
       wgmma_wait<0>();
       wgmma_reg_fence(o, NO / 2);
@@ -122,7 +130,7 @@ __device__ __forceinline__ void attn_fwd(const CUtensorMap& tmQ, const CUtensorM
 #pragma unroll
       for (int kk = 0; kk < ATT_COLS / 16; ++kk) acc_to_a_frag(s, kk, pa[kk]);
     }
-    issue_pv(c.nblk - 1);
+    issue_pv(nblk - 1);
     wgmma_wait<0>();
     wgmma_reg_fence(o, NO / 2);
 
@@ -158,14 +166,22 @@ attn_fwd_plan_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
   attn_fwd<KA, NO, KS, true>(tmQ, tmK, tmV, p, rowscale);
 }
 
+template <int KA, int NO, int KS>
+__global__ void __launch_bounds__(ATT_THREADS, 1)
+attn_fwd_causal_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+                       const __grid_constant__ CUtensorMap tmV, const AttnFwdParams p) {
+  attn_fwd<KA, NO, KS, false, true>(tmQ, tmK, tmV, p, nullptr);
+}
+
 }  // namespace ivb
 
 using namespace ivb;
 
-// ivb_attn_fwd and ivb_attn_fwd_plan (rowscale not null); `fn` names the entry point in messages.
+// ivb_attn_fwd, ivb_attn_fwd_plan (rowscale not null) and ivb_attn_fwd_causal (causal, no rowscale); `fn` names the
+// entry point in messages.
 static int attn_fwd(const char* fn, const void* q, long ldq, const void* k, long ldk, const void* v, long ldv, void* out,
                     long ldo, float* lse2, int B, int n, int H, int d, float softmax_scale, const float* rowscale,
-                    cudaStream_t stream) {
+                    cudaStream_t stream, bool causal = false) {
   if (B <= 0 || n <= 0) return 0;
   int rc;
   if ((rc = check_head_args(fn, d, {ldq, ldk, ldv, ldo}))) return rc;
@@ -175,6 +191,10 @@ static int attn_fwd(const char* fn, const void* q, long ldq, const void* k, long
   if ((rc = make_head_tmap(&tv, v, ldv, B, n, H, d, ATT_COLS))) return rc;
   const AttnFwdParams p{B, n, H, d, softmax_scale * 1.4426950408889634f, reinterpret_cast<__nv_bfloat16*>(out), ldo, lse2};
   return dispatch_head_dim(d, [&](auto hd) {
+    if (causal)
+      return launch_attn<attn_fwd_causal_kernel<hd.KA, hd.NO, hd.KS>, NO_PDL>(
+          "cudaFuncSetAttribute(attn_fwd_causal)", "attn_fwd_causal_kernel", FwdSmem<hd.KA>::BYTES, B, n, H, stream, tq,
+          tk, tv, p);
     if (rowscale != nullptr)
       return launch_attn<attn_fwd_plan_kernel<hd.KA, hd.NO, hd.KS>, NO_PDL>(
           "cudaFuncSetAttribute(attn_fwd_plan)", "attn_fwd_plan_kernel", FwdSmem<hd.KA>::BYTES, B, n, H, stream, tq, tk,
@@ -197,6 +217,13 @@ extern "C" int ivb_attn_fwd_plan(const void* q, long ldq, const void* k, long ld
   if (rowscale == nullptr) return set_error("ivb_attn_fwd_plan: rowscale is null");
   return attn_fwd("ivb_attn_fwd_plan", q, ldq, k, ldk, v, ldv, out, ldo, lse2, B, n, H, d, softmax_scale, rowscale,
                   reinterpret_cast<cudaStream_t>(stream));
+}
+
+extern "C" int ivb_attn_fwd_causal(const void* q, long ldq, const void* k, long ldk, const void* v, long ldv,
+                                   void* out, long ldo, float* lse2, int B, int n, int H, int d, float softmax_scale,
+                                   void* stream) {
+  return attn_fwd("ivb_attn_fwd_causal", q, ldq, k, ldk, v, ldv, out, ldo, lse2, B, n, H, d, softmax_scale, nullptr,
+                  reinterpret_cast<cudaStream_t>(stream), true);
 }
 
 // ---------------------------------------------------------------------------------------------------------------

@@ -185,6 +185,29 @@ __device__ __forceinline__ void softmax_tile(float (&s)[ATT_COLS / 2], int valid
   for (int r = 0; r < 2; ++r) l_run[r] = l_run[r] * alpha[r] + rs[r];
 }
 
+// Causal attention (ivb_attn_fwd_causal, ivb_attn_bwd_causal) keeps key <= query.  The streamed tiles a CTA needs:
+// [causal_tile_begin, causal_tile_end).  With queries streamed (the dK/dV pass) they start at the first query tile that
+// reaches the CTA's first key; with keys streamed (the forward and the dQ pass) they end at the tile that holds the
+// CTA's last live query.  A 128-row CTA covers whole 64-row tiles, so the tile holding key == query is always streamed
+// and every live row keeps at least one key.
+static_assert(ATT_ROWS % ATT_COLS == 0, "causal tile bounds: a CTA's rows are whole streamed tiles");
+__device__ __forceinline__ int causal_tile_begin(const AttnCta& c) { return c.row0 / ATT_COLS; }
+__device__ __forceinline__ int causal_tile_end(const AttnCta& c, int n) {
+  return (min(n, c.row0 + ATT_ROWS) + ATT_COLS - 1) / ATT_COLS;
+}
+
+// Causal mask of a 64 x 64 score tile in the accumulator layout softmax_tile reads: S = -inf where key > query, the
+// reference's additive -inf upper triangle.  row0: the first row of this thread's fragment rows (the thread holds rows
+// row0 and row0 + 8); col0: the tile's first column.  ROWS_ARE_KEYS: the tile is S^T (the dK/dV pass).
+template <bool ROWS_ARE_KEYS>
+__device__ __forceinline__ void causal_mask_tile(float (&s)[ATT_COLS / 2], int row0, int col0, int lane) {
+#pragma unroll
+  for (int i = 0; i < ATT_COLS / 2; ++i) {
+    const int col = col0 + 8 * (i >> 2) + 2 * (lane & 3) + (i & 1), row = row0 + 8 * ((i >> 1) & 1);
+    if (ROWS_ARE_KEYS ? row > col : col > row) s[i] = -INFINITY;
+  }
+}
+
 // Writes this thread's rows (< n) of a 64 x NO accumulator, row r times factor[r] (and, with COLF, column j times
 // colf[j]), as bf16 to head h of the [B*n, ld] buffer out.  Fragment row r holds columns 8 jn + 2 (lane % 4) + {0, 1} in
 // acc[4 jn + 2 r], acc[4 jn + 2 r + 1].

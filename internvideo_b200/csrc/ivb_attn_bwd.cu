@@ -1,4 +1,4 @@
-// ivb_attn_bwd.cu — attention backward on Hopper wgmma (two passes, no atomics, recompute of P from lse).
+// ivb_attn_bwd.cu — attention backward, non-causal or causal, on Hopper wgmma (two passes, no atomics, recompute of P from lse).
 //
 // Stands in for FA2's backward of flash_attn_varlen_qkvpacked_func (the autograd of
 // FlashAttention.forward, flash_attention_class.py:47-50) / autograd of _naive_attn
@@ -73,7 +73,9 @@ using BwdSmem = AttnSmem<KA, 2, BWD_NST, 2, 1>;
 // KA: 64-wide atoms covering head_dim (1: d <= 64, 2: d <= 128); NO: wgmma N of the accumulate MMAs;
 // KS: k16 steps of the S/dP MMAs, ceil(d / 16).
 // PLAN: the CTA of a dropped clip (attn_prologue) writes zeros to its output rows (dQ, or dV and dK).
-template <int MODE, int KA, int NO, int KS, bool PLAN>
+// CAUSAL: MODE 1 streams the query tiles from causal_tile_begin, MODE 0 the key tiles up to causal_tile_end, and a
+// warpgroup masks the tiles that cross its diagonal (P = 0 where key > query).
+template <int MODE, int KA, int NO, int KS, bool PLAN, bool CAUSAL = false>
 __device__ __forceinline__ void attn_bwd(const CUtensorMap& tmX, const CUtensorMap& tmY, const CUtensorMap& tmU,
                                          const CUtensorMap& tmW, const AttnBwdParams& p, const float* rowscale) {
   using Smem = BwdSmem<KA>;
@@ -84,6 +86,8 @@ __device__ __forceinline__ void attn_bwd(const CUtensorMap& tmX, const CUtensorM
     return;
   }
   const long hb = (static_cast<long>(c.b) * p.H + c.h) * p.n_pad;
+  const int jb = CAUSAL && MODE == 1 ? causal_tile_begin(c) : 0;         // streamed tiles [jb, je)
+  const int je = CAUSAL && MODE == 0 ? causal_tile_end(c, p.n) : c.nblk;
   pdl_wait();
   pdl_launch_dependents();
 
@@ -93,8 +97,8 @@ __device__ __forceinline__ void attn_bwd(const CUtensorMap& tmX, const CUtensorM
     mbar_expect_tx(Smem::bar_row(), 2 * Smem::ROW_BYTES);
     load_head_rows<KA, ATT_ROWS>(Smem::rows(0), &tmX, c.h, c.row0, c.b, Smem::bar_row());
     load_head_rows<KA, ATT_ROWS>(Smem::rows(1), &tmY, c.h, c.row0, c.b, Smem::bar_row());
-    for (int j = 0; j < c.nblk; ++j) {
-      const RingSlot<BWD_NST> s(j);
+    for (int j = jb; j < je; ++j) {
+      const RingSlot<BWD_NST> s(j - jb);
       uint64_t* full = Smem::full(0, s.st);
       mbar_wait(Smem::empty(0, s.st), s.ph ^ 1);
       mbar_expect_tx(full, 2 * Smem::TILE_BYTES + (MODE == 1 ? 2 * Smem::VEC_BYTES : 0));
@@ -127,8 +131,8 @@ __device__ __forceinline__ void attn_bwd(const CUtensorMap& tmX, const CUtensorM
     // Named barrier 1 + cw: "warpgroup cw may issue S/dP".  Warpgroup 0 goes first.
     if (pingpong && cw == 1) named_bar_arrive(1, 256);
     mbar_wait(Smem::bar_row(), 0);
-    for (int j = 0; j < c.nblk; ++j) {
-      const RingSlot<BWD_NST> s(j);
+    for (int j = jb; j < je; ++j) {
+      const RingSlot<BWD_NST> s(j - jb);
       mbar_wait(Smem::full(0, s.st), s.ph);
       const uint32_t ua = smem_u32(Smem::tile(0, s.st)), wa = smem_u32(Smem::tile(1, s.st));
       const float* lse_tile = Smem::vec(0, s.st);
@@ -145,10 +149,15 @@ __device__ __forceinline__ void attn_bwd(const CUtensorMap& tmX, const CUtensorM
       }
       wgmma_commit();
       // Hand the turn over; warpgroup 1 skips its last hand-over, which no one would wait for.
-      if (pingpong && !(cw == 1 && j == c.nblk - 1)) named_bar_arrive(2 - cw, 256);
+      if (pingpong && !(cw == 1 && j == je - 1)) named_bar_arrive(2 - cw, 256);
       wgmma_wait<0>();
       wgmma_reg_fence(sc, ATT_COLS / 2);
       wgmma_reg_fence(dp, ATT_COLS / 2);
+      if constexpr (CAUSAL) {   // S = -inf gives P = 0 and so dS = 0; only the tiles that cross the diagonal
+        const int r0 = c.row0 + cw * 64;
+        if (MODE == 1 ? j * ATT_COLS < r0 + 64 : (j + 1) * ATT_COLS > r0)
+          causal_mask_tile<MODE == 1>(sc, c.row0 + c.rloc, j * ATT_COLS, c.lane);
+      }
 
       // P and dS in place of S and dP.  Columns beyond the sequence get P = 0.
 #pragma unroll
@@ -207,6 +216,14 @@ attn_bwd_plan_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_const
   attn_bwd<MODE, KA, NO, KS, true>(tmX, tmY, tmU, tmW, p, rowscale);
 }
 
+template <int MODE, int KA, int NO, int KS>
+__global__ void __launch_bounds__(ATT_THREADS, 1)
+attn_bwd_causal_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmY,
+                       const __grid_constant__ CUtensorMap tmU, const __grid_constant__ CUtensorMap tmW,
+                       const AttnBwdParams p) {
+  attn_bwd<MODE, KA, NO, KS, false, true>(tmX, tmY, tmU, tmW, p, nullptr);
+}
+
 }  // namespace ivb
 
 using namespace ivb;
@@ -217,11 +234,12 @@ extern "C" long ivb_attn_bwd_workspace_floats(int B, int n, int H) {
   return 2 * static_cast<long>(B) * H * n_pad;
 }
 
-// ivb_attn_bwd and ivb_attn_bwd_plan (rowscale not null); `fn` names the entry point in messages.
+// ivb_attn_bwd, ivb_attn_bwd_plan (rowscale not null) and ivb_attn_bwd_causal (causal, no rowscale); `fn` names the
+// entry point in messages.
 static int attn_bwd(const char* fn, const void* q, long ldq, const void* k, long ldk, const void* v, long ldv,
                     const void* out, long ldo, const void* dout, long lddo, const float* lse2, float* delta_ws, void* dq,
                     long lddq, void* dk, long lddk, void* dv, long lddv, int B, int n, int H, int d,
-                    float softmax_scale, const float* rowscale, cudaStream_t stream) {
+                    float softmax_scale, const float* rowscale, cudaStream_t stream, bool causal = false) {
   if (B <= 0 || n <= 0) return 0;
   int rc;
   char msg[128];
@@ -257,6 +275,14 @@ static int attn_bwd(const char* fn, const void* q, long ldq, const void* k, long
   const AttnBwdParams pq{B, n, H, d, n_pad, sc_log2, softmax_scale, lse2p, deltap, bf(dq), lddq, nullptr, 0};
   return dispatch_head_dim(d, [&](auto hd) {
     constexpr int smem = BwdSmem<hd.KA>::BYTES;
+    if (causal) {
+      const char* attr = "cudaFuncSetAttribute(attn_bwd_causal)";
+      if ((rc = launch_attn<attn_bwd_causal_kernel<1, hd.KA, hd.NO, hd.KS>, ALLOW_PDL>(
+               attr, "attn_bwd_causal_kernel", smem, B, n, H, stream, rows[2], rows[3], tiles[0], tiles[1], pkv)))
+        return rc;
+      return launch_attn<attn_bwd_causal_kernel<0, hd.KA, hd.NO, hd.KS>, ALLOW_PDL>(
+          attr, "attn_bwd_causal_kernel", smem, B, n, H, stream, rows[0], rows[1], tiles[2], tiles[3], pq);
+    }
     if (rowscale != nullptr) {
       const char* attr = "cudaFuncSetAttribute(attn_bwd_plan)";
       if ((rc = launch_attn<attn_bwd_plan_kernel<1, hd.KA, hd.NO, hd.KS>, ALLOW_PDL>(
@@ -292,4 +318,12 @@ extern "C" int ivb_attn_bwd_plan(const void* q, long ldq, const void* k, long ld
   if (rowscale == nullptr) return set_error("ivb_attn_bwd_plan: rowscale is null");
   return attn_bwd("ivb_attn_bwd_plan", q, ldq, k, ldk, v, ldv, out, ldo, dout, lddo, lse2, delta_ws, dq, lddq, dk, lddk,
                   dv, lddv, B, n, H, d, softmax_scale, rowscale, reinterpret_cast<cudaStream_t>(stream));
+}
+
+extern "C" int ivb_attn_bwd_causal(const void* q, long ldq, const void* k, long ldk, const void* v, long ldv,
+                                   const void* out, long ldo, const void* dout, long lddo, const float* lse2,
+                                   float* delta_ws, void* dq, long lddq, void* dk, long lddk, void* dv, long lddv, int B,
+                                   int n, int H, int d, float softmax_scale, void* stream) {
+  return attn_bwd("ivb_attn_bwd_causal", q, ldq, k, ldk, v, ldv, out, ldo, dout, lddo, lse2, delta_ws, dq, lddq, dk,
+                  lddk, dv, lddv, B, n, H, d, softmax_scale, nullptr, reinterpret_cast<cudaStream_t>(stream), true);
 }

@@ -434,12 +434,19 @@ def colsum(x, out=None):
 
 
 # ----------------------------------------------------------------------------------------- attention
-def attn_fwd(q, k, v, B, n, H, d, scale, out=None, want_lse=True, rowscale=None):
+def _chk_causal(fn, causal, rowscale):
+    if causal and rowscale is not None:
+        raise _lib.IvbError(f"{fn}: causal attention has no DropPath plan form (rowscale must be None)")
+
+
+def attn_fwd(q, k, v, B, n, H, d, scale, out=None, want_lse=True, rowscale=None, causal=False):
     """q/k/v: 2-D views [B*n, H*d] (any row pitch) of the projection buffers.  rowscale: optional fp32 [B*n] DropPath
     factors of the attention branch (one per clip): the call goes to ivb_attn_fwd_plan, which skips the clips whose
-    factor is 0 and writes zeros to their rows."""
+    factor is 0 and writes zeros to their rows.  causal: key index > query index is masked (ivb_attn_fwd_causal; not
+    with rowscale)."""
     _chk(("q", q, bf16), ("k", k, bf16), ("v", v, bf16), ("out?", out, bf16), ("rowscale?", rowscale, f32))
     _chk_rowscale("attn_fwd", rowscale, B * n)
+    _chk_causal("attn_fwd", causal, rowscale)
     for t, nm in ((q, "q"), (k, "k"), (v, "v")):
         if t.shape != (B * n, H * d):
             raise _lib.IvbError(f"attn_fwd: {nm} must be [B*n, H*d], got {tuple(t.shape)}")
@@ -447,9 +454,9 @@ def attn_fwd(q, k, v, B, n, H, d, scale, out=None, want_lse=True, rowscale=None)
         out = torch.empty((B * n, H * d), device=q.device, dtype=bf16)
     lse = torch.empty((B, H, n), device=q.device, dtype=f32) if want_lse else None
     plan = () if rowscale is None else (rowscale,)
-    _call("attn_fwd_plan" if plan else "attn_fwd", q, _rows2d(q, "q"), k, _rows2d(k, "k"), v, _rows2d(v, "v"), out,
+    _call("attn_fwd_causal" if causal else "attn_fwd_plan" if plan else "attn_fwd", q, _rows2d(q, "q"), k, _rows2d(k, "k"), v, _rows2d(v, "v"), out,
           _rows2d(out, "out"), lse, B, n, H, d, float(scale), *plan, kind="attn_fwd",
-          flops=4.0 * B * H * n * n * d)          # QK^T + PV
+          flops=(2.0 if causal else 4.0) * B * H * n * n * d)          # QK^T + PV (causal: about half)
     return out, lse
 
 
@@ -464,21 +471,23 @@ def headaxis_attn_fwd(qkv, B, N, H, d, scale):
     return out
 
 
-def attn_bwd(q, k, v, out, dout, lse, B, n, H, d, scale, dq, dk, dv, rowscale=None):
+def attn_bwd(q, k, v, out, dout, lse, B, n, H, d, scale, dq, dk, dv, rowscale=None, causal=False):
     """dq/dk/dv: preallocated bf16 2-D views [B*n, H*d] (e.g. the three slots of a [B*n, 3D] buffer).  rowscale: the
-    forward's DropPath factors (attn_fwd): ivb_attn_bwd_plan writes zeros to the dropped clips' rows."""
+    forward's DropPath factors (attn_fwd): ivb_attn_bwd_plan writes zeros to the dropped clips' rows.  causal: the
+    backward of attn_fwd(causal=True) (ivb_attn_bwd_causal; not with rowscale)."""
     rows = (("q", q), ("k", k), ("v", v), ("out", out), ("dout", dout), ("dq", dq), ("dk", dk), ("dv", dv))
     _chk(*((nm, t, bf16) for nm, t in rows), ("lse", lse, f32), ("rowscale?", rowscale, f32))
     _chk_rowscale("attn_bwd", rowscale, B * n)
+    _chk_causal("attn_bwd", causal, rowscale)
     for nm, t in rows:
         if t.shape != (B * n, H * d):
             raise _lib.IvbError(f"attn_bwd: {nm} must be [B*n, H*d], got {tuple(t.shape)}")
     delta = torch.empty((int(_lib.load().ivb_attn_bwd_workspace_floats(B, n, H)),), device=q.device, dtype=f32)
     plan = () if rowscale is None else (rowscale,)
-    _call("attn_bwd_plan" if plan else "attn_bwd", q, _rows2d(q, "q"), k, _rows2d(k, "k"), v, _rows2d(v, "v"), out,
+    _call("attn_bwd_causal" if causal else "attn_bwd_plan" if plan else "attn_bwd", q, _rows2d(q, "q"), k, _rows2d(k, "k"), v, _rows2d(v, "v"), out,
           _rows2d(out, "out"), dout, _rows2d(dout, "dout"), lse, delta, dq, _rows2d(dq, "dq"), dk, _rows2d(dk, "dk"), dv,
           _rows2d(dv, "dv"), B, n, H, d, float(scale), *plan, kind="attn_bwd",
-          flops=10.0 * B * H * n * n * d)  # algorithmic: 5 GEMMs (SURVEY §8d: 2.5x forward)
+          flops=(5.0 if causal else 10.0) * B * H * n * n * d)  # algorithmic: 5 GEMMs (SURVEY §8d: 2.5x forward)
     return dq, dk, dv
 
 
@@ -576,6 +585,38 @@ def scatter_add(g, g_bstride, idx, idx_bstride, idx_off, B, rows, D, table_grad)
     _chk(("g", g, (f32, bf16)), ("idx?", idx, i32), ("table_grad", table_grad, f32))
     _call("scatter_add", g, int(g.dtype == f32), g_bstride, idx, idx_bstride, idx_off, B, rows, D, table_grad)
     return table_grad
+
+
+def _token_embed_fwd(ids, table, pos):
+    """The text tower's token embedding (ivb_token_embed_fwd): ids int64 [B, L], table bf16 [V, D], pos bf16 [L, D] ->
+    (fp32 residual stream [B*L, D] = table[ids] + pos, int32[1] device flag: 1 + the first row seen with an id outside
+    [0, V), else 0).  Private, as _attn_fp8_pack: ops.TokenEmbedFn is its caller."""
+    _chk(("ids", ids, torch.int64), ("table", table, bf16), ("pos", pos, bf16))
+    B, L = ids.shape
+    V, D = table.shape
+    if pos.shape != (L, D) or not (ids.is_contiguous() and table.is_contiguous() and pos.is_contiguous()):
+        raise _lib.IvbError(f"token_embed_fwd: contiguous ids [B, L], table [V, D] and pos [L, D] needed, got "
+                            f"{tuple(ids.shape)}, {tuple(table.shape)}, {tuple(pos.shape)}")
+    out = torch.empty((B * L, D), device=ids.device, dtype=f32)
+    err = torch.zeros((1,), device=ids.device, dtype=i32)
+    _call("token_embed_fwd", ids, B, L, table, V, pos, D, out, out.stride(0), err)
+    return out, err
+
+
+def _token_embed_bwd(ids, g, V):
+    """Backward of _token_embed_fwd (ivb_token_embed_bwd): ids int64 [B, L], g fp32 [B*L, D] -> (dtable fp32 [V, D],
+    zero in the rows of ids not present, dpos fp32 [L, D]), each summed in a fixed order.  Private, as
+    _token_embed_fwd."""
+    _chk(("ids", ids, torch.int64), ("g", g, f32))
+    B, L = ids.shape
+    D = g.shape[1]
+    if g.shape[0] != B * L or not ids.is_contiguous():
+        raise _lib.IvbError(f"token_embed_bwd: g must be [B*L, D] for contiguous ids [B, L], got {tuple(g.shape)}")
+    dtable = torch.zeros((V, D), device=g.device, dtype=f32)
+    dpos = torch.empty((L, D), device=g.device, dtype=f32)
+    ws = torch.empty((int(_lib.load().ivb_token_embed_bwd_workspace_ints(V, B, L)),), device=g.device, dtype=i32)
+    _call("token_embed_bwd", ids, B, L, g, _rows2d(g, "g"), V, D, dtable, dpos, ws)
+    return dtable, dpos
 
 
 # ----------------------------------------------------------------------------------------- heads / losses

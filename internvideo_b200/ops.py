@@ -24,19 +24,22 @@ def _pdt(g, p):
 
 # ------------------------------------------------------------------------------------------ Linear
 class LinearFn(torch.autograd.Function):
-    """y = x W^T + b on the wgmma GEMM (nn.Linear: internvideo2_pretrain.py:61-77,195,211,356)."""
+    """y = x W^T + b on the wgmma GEMM (nn.Linear: internvideo2_pretrain.py:61-77,195,211,356).  w_t: W is stored
+    transposed, [in, out], and y = x W + b reads it as the GEMM's MN-major operand (the text tower's projection_layer,
+    text_encoder.py:219)."""
 
     @staticmethod
-    def forward(ctx, x, w, b, out_f32=False):
+    def forward(ctx, x, w, b, out_f32=False, w_t=False):
         x2 = x.reshape(-1, x.shape[-1])
         if x2.stride(-1) != 1:
             x2 = x2.contiguous()
-        y = ll.gemm(x2, w, bias=b, epi=ll.EPI_F32 if out_f32 else ll.EPI_BF16)
+        y = ll.gemm(x2, w, b_t=w_t, bias=b, epi=ll.EPI_F32 if out_f32 else ll.EPI_BF16)
         ctx.save_for_backward(x2, w)
+        ctx.w_t = w_t
         ctx.has_bias = b is not None
         ctx.bias_dtype = b.dtype if b is not None else None
         ctx.in_shape = x.shape
-        return y.reshape(*x.shape[:-1], w.shape[0])
+        return y.reshape(*x.shape[:-1], w.shape[1] if w_t else w.shape[0])
 
     @staticmethod
     def backward(ctx, dy):
@@ -48,16 +51,16 @@ class LinearFn(torch.autograd.Function):
             dy2 = dy2.contiguous()
         dx = dw = db = None
         if ctx.needs_input_grad[0]:
-            dx = ll.gemm(dy2, w, b_t=True).reshape(ctx.in_shape)
+            dx = ll.gemm(dy2, w, b_t=not ctx.w_t).reshape(ctx.in_shape)
         if ctx.needs_input_grad[1]:
-            dw = ll.gemm(dy2, x2, a_t=True, b_t=True)
+            dw = ll.gemm(x2, dy2, a_t=True, b_t=True) if ctx.w_t else ll.gemm(dy2, x2, a_t=True, b_t=True)
         if ctx.has_bias and ctx.needs_input_grad[2]:
             db = ll.colsum(dy2).to(ctx.bias_dtype)
-        return dx, dw, db, None
+        return dx, dw, db, None, None
 
 
-def linear(x, w, b=None, out_f32=False):
-    return LinearFn.apply(x, w, b, out_f32)
+def linear(x, w, b=None, out_f32=False, w_t=False):
+    return LinearFn.apply(x, w, b, out_f32, w_t)
 
 
 class LinearGeluFn(torch.autograd.Function):
@@ -202,7 +205,8 @@ class BlockSpec(NamedTuple):
     scale (None: d ** -0.5).  head_axis: the VideoMAEv2 teacher's attention over the heads of each token (inference
     only).  checkpoint: BlockFn keeps only the block input and recomputes the forward in the backward.  attn_fp8: the
     token-axis attention runs on the FP8 tensor cores (lowlevel._attn_fp8_pack + _attn_fwd_fp8; inference only:
-    block_forward refuses it with save=True or head_axis)."""
+    block_forward refuses it with save=True or head_axis).  causal: token-axis attention masks every key after its
+    query (the MobileCLIP text tower; block_forward refuses it with head_axis, attn_fp8 or a DropPath plan)."""
     B: int
     n: int
     H: int
@@ -215,6 +219,7 @@ class BlockSpec(NamedTuple):
     checkpoint: bool = False
     precision: object = BF16
     attn_fp8: bool = False
+    causal: bool = False
 
     def attn_scale(self, d):
         return d ** -0.5 if self.scale is None else self.scale
@@ -298,6 +303,9 @@ def block_forward(x, spec, p, rs1=None, rs2=None, save=True, plan1=None, plan2=N
     if spec.attn_fp8 and (save or spec.head_axis):
         raise ll._lib.IvbError("block_forward: FP8 attention (spec.attn_fp8) is inference-only and token-axis: it needs "
                                "save=False and head_axis=False")
+    if spec.causal and (spec.attn_fp8 or spec.head_axis or plan1 is not None or plan2 is not None):
+        raise ll._lib.IvbError("block_forward: causal attention runs in bf16 over the tokens, without DropPath plans: "
+                               "it excludes attn_fp8, head_axis and plan1 / plan2")
     if x.dtype != f32 or not x.is_cuda:
         raise ll._lib.IvbError("block_forward: residual stream must be a CUDA fp32 tensor [B*n, D]")
     prec = spec.precision
@@ -350,7 +358,7 @@ def block_forward(x, spec, p, rs1=None, rs2=None, save=True, plan1=None, plan2=N
         a = ll._attn_fwd_fp8(*ll._attn_fp8_pack(q, k, v, B, n, H, d), B, n, H, d, spec.attn_scale(d))
     else:
         a, lse = ll.attn_fwd(q, k, v, B, n, H, d, spec.attn_scale(d), want_lse=save,
-                             rowscale=rs1 if mp[0] is not None else None)
+                             rowscale=rs1 if mp[0] is not None else None, causal=spec.causal)
     y1 = torch.empty((M, D), device=x.device, dtype=bf16) if (p.g1 is not None and save) else None
     x1 = linear(a, 1, p.projw, epi=ll.EPI_RESID, bias=p.projb, gamma=p.g1, aux=x, out1=y1, rowscale=rs1)
     n2_in, n2, mean2, rstd2 = norm(x1, p.n2w, p.n2b, spec.eps2)
@@ -442,7 +450,8 @@ def block_backward(x, s, spec, t, P, dx2, rs1, rs2, plan1=None, plan2=None):
     dqkv = torch.empty((M, 3 * D), device=x.device, dtype=bf16)
     qk = s.qkn if s.qkn is not None else s.qkv
     ll.attn_bwd(qk[:, :D], qk[:, D:2 * D], s.qkv[:, 2 * D:], s.a, da, s.lse, B, n, H, d, spec.attn_scale(d),
-                dqkv[:, :D], dqkv[:, D:2 * D], dqkv[:, 2 * D:], rowscale=rs1 if m1 is not None else None)
+                dqkv[:, :D], dqkv[:, D:2 * D], dqkv[:, 2 * D:], rowscale=rs1 if m1 is not None else None,
+                causal=spec.causal)
     if s.qkn is not None and s.rk is None:
         ll.rmsnorm_pair_bwd(dqkv, s.qkv, D, t.qnw, t.knw, s.rq, seg["qnw"], seg["knw"])
     elif s.qkn is not None:
@@ -586,6 +595,28 @@ class EmbedFn(torch.autograd.Function):
         ll.scatter_add(dx0, n * D, idx, n, 0, B, n, D, dpos)
         dcls = dx0[:, 0].sum(0)
         return (None, None, dw, db, dcls.reshape(cshape).to(pdt), dpos.reshape(pshape).to(pdt), None, None)
+
+
+class TokenEmbedFn(torch.autograd.Function):
+    """The text tower's token embedding (TextTransformer.forward_embedding, text_encoder.py:131-147): the fp32
+    residual stream [B*L, D] = table[ids] + pos[:L] (ll._token_embed_fwd), and the fixed-order table and position
+    gradients (ll._token_embed_bwd).  Returns (stream, int32[1] bad-id flag)."""
+
+    @staticmethod
+    def forward(ctx, ids, table, pos):
+        ids = ids.contiguous()
+        out, err = ll._token_embed_fwd(ids, table, pos.reshape(ids.shape[1], table.shape[1]))
+        ctx.save_for_backward(ids)
+        ctx.meta = (table.shape[0], table.dtype, pos.shape, pos.dtype)
+        ctx.mark_non_differentiable(err)
+        return out, err
+
+    @staticmethod
+    def backward(ctx, dout, _derr):
+        (ids,) = ctx.saved_tensors
+        V, tdt, pshape, pdt = ctx.meta
+        dtable, dpos = ll._token_embed_bwd(ids, dout.contiguous().float(), V)
+        return None, dtable.to(tdt), dpos.reshape(pshape).to(pdt)
 
 
 class GatherAddFn(torch.autograd.Function):
