@@ -337,6 +337,16 @@ int ivb_attn_bwd_causal(const void* q, long ldq, const void* k, long ldk, const 
                         const void* out, long ldo, const void* dout, long lddo, const float* lse2,
                         float* delta_ws, void* dq, long lddq, void* dk, long lddk, void* dv, long lddv,
                         int B, int n, int H, int d, float softmax_scale, void* stream);
+/* ivb_attn_fwd_keylen: ivb_attn_fwd with a key-padding mask given as per-clip key lengths, with the same operands and
+ * operand rules.  kv_len: int32 [B] (device, required): in clip b every key >= kv_len[b] is masked out for every query
+ * (the additive -10000 of right-padded BERT captions, xbert.py:1099-1119, underflows to the same 0 in fp32).  All n
+ * query rows are computed and written, padded ones included.  A clip's CTAs stream only the ceil(kv_len[b] / 64) key
+ * tiles that hold its keys.  kv_len is read on the device, never by the host, so the call is capturable in a CUDA
+ * graph.  An entry outside [1, n] makes that clip's out rows (and lse2 rows) NaN; the call still returns 0.  A null
+ * kv_len is refused before any CUDA call.  There is no backward, causal, DropPath-plan or FP8 form.                 */
+int ivb_attn_fwd_keylen(const void* q, long ldq, const void* k, long ldk, const void* v, long ldv,
+                        void* out, long ldo, float* lse2, int B, int n, int H, int d, float softmax_scale,
+                        const int* kv_len, void* stream);
 /* ---- FP8 attention forward (FP8 inference of frozen towers; no lse, no backward) ------------------------------------
  * Every scale is a power of two chosen from an amax by the ivb_fp8_quantize_rows rule (E4M3; 1 when the amax is 0,
  * scale_inv NaN when the amax is Inf or NaN), so dequantisation is exact.  Same bits on every run; one stream-ordered

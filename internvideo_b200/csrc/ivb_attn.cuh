@@ -1,6 +1,6 @@
-// ivb_attn.cuh — the pieces the attention forward (ivb_attn.cu), backward (ivb_attn_bwd.cu) and FP8 forward
-// (ivb_attn_fp8.cu) kernels share: one CTA per (128-row block, head, clip) that streams 64-row tiles of the other
-// operands through a ring.
+// ivb_attn.cuh — the pieces the attention forward (ivb_attn_fwd.cuh, instantiated in ivb_attn.cu and
+// ivb_attn_keylen.cu), backward (ivb_attn_bwd.cu) and FP8 forward (ivb_attn_fp8.cu) kernels share: one CTA per
+// (128-row block, head, clip) that streams 64-row tiles of the other operands through a ring.
 #pragma once
 #include <math.h>
 #include <stdio.h>
@@ -235,11 +235,17 @@ __device__ __forceinline__ void store_rows(const float (&acc)[NO / 2], __nv_bflo
   }
 }
 
-// A dead CTA's rows (< n) of head h of the [B*n, ld] bf16 buffer out: zeros, by all the CTA's threads.
-__device__ __forceinline__ void zero_rows(__nv_bfloat16* out, long ld, const AttnCta& c, int n, int d) {
+// The CTA's rows (< n) of head h of the [B*n, ld] bf16 buffer out, every element pair set to the bits `pair`, by all
+// the CTA's threads.
+__device__ __forceinline__ void fill_rows(__nv_bfloat16* out, long ld, const AttnCta& c, int n, int d, uint32_t pair) {
   const int rows = min(ATT_ROWS, n - c.row0), pairs = d / 2;
   for (int i = threadIdx.x; i < rows * pairs; i += ATT_THREADS)
-    reinterpret_cast<uint32_t*>(out + (static_cast<long>(c.b) * n + c.row0 + i / pairs) * ld + c.h * d)[i % pairs] = 0u;
+    reinterpret_cast<uint32_t*>(out + (static_cast<long>(c.b) * n + c.row0 + i / pairs) * ld + c.h * d)[i % pairs] = pair;
+}
+
+// A dead CTA's rows: zeros.
+__device__ __forceinline__ void zero_rows(__nv_bfloat16* out, long ld, const AttnCta& c, int n, int d) {
+  fill_rows(out, ld, c, n, d, 0u);
 }
 
 // ------------------------------------------------------------------ host side

@@ -439,24 +439,33 @@ def _chk_causal(fn, causal, rowscale):
         raise _lib.IvbError(f"{fn}: causal attention has no DropPath plan form (rowscale must be None)")
 
 
-def attn_fwd(q, k, v, B, n, H, d, scale, out=None, want_lse=True, rowscale=None, causal=False):
+def attn_fwd(q, k, v, B, n, H, d, scale, out=None, want_lse=True, rowscale=None, causal=False, kv_len=None):
     """q/k/v: 2-D views [B*n, H*d] (any row pitch) of the projection buffers.  rowscale: optional fp32 [B*n] DropPath
     factors of the attention branch (one per clip): the call goes to ivb_attn_fwd_plan, which skips the clips whose
     factor is 0 and writes zeros to their rows.  causal: key index > query index is masked (ivb_attn_fwd_causal; not
-    with rowscale)."""
-    _chk(("q", q, bf16), ("k", k, bf16), ("v", v, bf16), ("out?", out, bf16), ("rowscale?", rowscale, f32))
+    with rowscale).  kv_len: optional contiguous int32 [B], the keys each clip keeps (ivb_attn_fwd_keylen: keys >=
+    kv_len[b] are masked for every query of clip b; an entry outside [1, n] makes the clip's rows NaN; not with
+    rowscale or causal)."""
+    _chk(("q", q, bf16), ("k", k, bf16), ("v", v, bf16), ("out?", out, bf16), ("rowscale?", rowscale, f32),
+         ("kv_len?", kv_len, i32))
     _chk_rowscale("attn_fwd", rowscale, B * n)
     _chk_causal("attn_fwd", causal, rowscale)
+    if kv_len is not None and (causal or rowscale is not None):
+        raise _lib.IvbError("attn_fwd: key lengths (kv_len) have no causal or DropPath plan form")
+    if kv_len is not None and (kv_len.shape != (B,) or not kv_len.is_contiguous()):
+        raise _lib.IvbError(f"attn_fwd: kv_len must be a contiguous [B] = [{B}], got {tuple(kv_len.shape)}")
     for t, nm in ((q, "q"), (k, "k"), (v, "v")):
         if t.shape != (B * n, H * d):
             raise _lib.IvbError(f"attn_fwd: {nm} must be [B*n, H*d], got {tuple(t.shape)}")
     if out is None:
         out = torch.empty((B * n, H * d), device=q.device, dtype=bf16)
     lse = torch.empty((B, H, n), device=q.device, dtype=f32) if want_lse else None
-    plan = () if rowscale is None else (rowscale,)
-    _call("attn_fwd_causal" if causal else "attn_fwd_plan" if plan else "attn_fwd", q, _rows2d(q, "q"), k, _rows2d(k, "k"), v, _rows2d(v, "v"), out,
-          _rows2d(out, "out"), lse, B, n, H, d, float(scale), *plan, kind="attn_fwd",
-          flops=(2.0 if causal else 4.0) * B * H * n * n * d)          # QK^T + PV (causal: about half)
+    extra = (rowscale,) if rowscale is not None else (kv_len,) if kv_len is not None else ()
+    name = ("attn_fwd_causal" if causal else "attn_fwd_plan" if rowscale is not None
+            else "attn_fwd_keylen" if kv_len is not None else "attn_fwd")
+    # QK^T + PV; causal: about half.  With kv_len the host does not know the lengths: n is the upper bound.
+    _call(name, q, _rows2d(q, "q"), k, _rows2d(k, "k"), v, _rows2d(v, "v"), out, _rows2d(out, "out"), lse, B, n, H, d,
+          float(scale), *extra, kind="attn_fwd", flops=(2.0 if causal else 4.0) * B * H * n * n * d)
     return out, lse
 
 
