@@ -1,8 +1,9 @@
 """FP8 attention for inference (lowlevel._attn_fp8_pack + _attn_fwd_fp8, modules.set_fp8_inference(attention=True))
 on the H100 (gpu).
 
-Kernel level, at d in {64, 88, 128} x n in {257, 417, 1025, 2049} (sequence tails at every n but 1025's 1024 + 1), two
-clips, q / k / v the three column slots of one [B*n, 3*H*d] projection buffer (row pitch 3D), as the blocks pass them:
+Kernel level, at d in {64, 88, 128} x n in {257, 417, 1025, 2049} (sequence tails at every n but 1025's 1024 + 1), at
+every head dim at n = 190, and at n in {1, 63, 64, 65, 129} (SHAPES), two clips, q / k / v the three column slots of
+one [B*n, 3*H*d] projection buffer (row pitch 3D), as the blocks pass them:
 1. The pack is bit-exact against a torch emulation of its scale rule (the power-of-two rule of ivb_fp8_quantize_rows
    per (token, head) and per (clip, head, channel)) and of the E4M3 cast: q8 and k8 with their zero head padding, vt8
    with its zero key padding, and every scale; an Inf in one head of a q row or in one channel of v gives scale_inv NaN
@@ -13,14 +14,15 @@ clips, q / k / v the three column slots of one [B*n, 3*H*d] projection buffer (r
    of an E4M3 rounding midpoint for a few elements; each such element moves its output row by up to 2^-4 of one term
    P v, which next to an output element near 0 is a large relative error.  So the bound is on the tile error of
    attn_ref.tile_errors (rms error of a 64-row band over the rms of its head): EMULATION_BOUND, about twice the largest
-   value measured on an H100 (0.0059-0.0267 over the twelve shapes; the largest in one-row tail bands, where no
-   averaging over rows takes place).
+   value measured on an H100 (0.0059-0.0267 over the twelve model shapes; the largest in one-row tail bands, where no
+   averaging over rows takes place; the head-dim and short-sequence shapes at most 0.0077, H100 80GB HBM3 at 700 W).
 3. The forward against the bf16 kernel on the same bf16 inputs, which adds the casts' error: the tile error of
    attn_ref.tile_errors is held to FP8_VS_BF16.  E4M3 rounds with relative error at most u = 2^-4, about 0.036 rms;
    q and k each carry one rounding, so S errs by about 0.05 rms of its terms' scale, which P inherits as a relative
    error, and P and V each carry one more: about 0.07 rms in all.  Measured on an H100: 0.058-0.106, the largest again in
-   a one-row tail band; FP8_VS_BF16 is about twice that.  The inputs are N(0, 1) as in a normed block; spreading the
-   tokens' magnitudes (the pack test's inputs) makes the softmax peaked and the same casts err by 0.15-0.43.
+   a one-row tail band (the head-dim and short-sequence shapes: at most 0.086); FP8_VS_BF16 is about twice that.  The
+   inputs are N(0, 1) as in a normed block; spreading the tokens' magnitudes (the pack test's inputs) makes the
+   softmax peaked and the same casts err by 0.15-0.43.
 
 Model level: set_fp8_inference(model, attention=True) against set_fp8_inference(model) (FP8 GEMMs, bf16 attention) on a
 depth-2 L-dims CLIP tower (n = 1025, d = 64), the unmasked stage-2 tower (n = 2049, d = 88) and the VideoMAEv2 teacher
@@ -45,7 +47,11 @@ EMULATION_BOUND = 0.06
 FP8_VS_BF16 = 0.2
 MODEL_BOUND = 2 * 2.0 ** -4
 MODEL_LIMIT = 0.01       # about three times the largest H100 value (0.0026-0.0033)
-SHAPES = [(d, H, n) for d, H in ((64, 16), (88, 16), (128, 25)) for n in (257, 417, 1025, 2049)]
+# (d, H, n): the model head dims at their sequence lengths; every head dim the ABI accepts at a ragged n = 190 (d <= 32:
+# the NO = 32 kernel; d = 16, 24: head columns padded to 32); and one key (n = 1) and either side of the 64-key tile
+# and the 128-row block at d = 64 and 88
+SHAPES = ([(d, H, n) for d, H in ((64, 16), (88, 16), (128, 25)) for n in (257, 417, 1025, 2049)]
+          + [(d, 4, 190) for d in range(16, 129, 8)] + [(d, 4, n) for d in (64, 88) for n in (1, 63, 64, 65, 129)])
 
 
 def _qkv(B, n, H, d, seed, spread=0.0):
