@@ -7,6 +7,10 @@
 // One warp per row, 16-byte vector loads, warp-shuffle reductions; parameter gradients are
 // accumulated per warp in shared memory, stored as one partial per column per CTA and summed in a fixed
 // order by colred_finish (ivb_colred.cuh).
+// The forward has two kernels: norm_fwd_kernel streams the row (LayerNorm, and RMSNorm above D = 1536, to bf16), and
+// norm_rows_kernel holds it in registers and writes it as bf16 (RMSNorm, the q/k pair), as E4M3 with a per-row
+// scale (FP8 inference), or as both (FP8 training), all launched by launch_norm_fwd.
+#include <stdio.h>
 #include <stdlib.h>
 #include <type_traits>
 
@@ -256,17 +260,31 @@ colsum_bf16_kernel(const __nv_bfloat16* __restrict__ x, long ldx, int M, int N,
 }
 
 
-// ------------------------------------------------------------------ register-resident RMSNorm (D <= 256*NCH)
-// The generic kernels above stream every row twice (statistics pass + output pass, second pass from L1/L2).
-// For the block norms (D = 384..1536) the row fits in registers: one HBM read per operand, period.
-// PAIR: the q-norm and the k-norm of a block in ONE launch (internvideo2_pretrain.py:198-206).  Virtual row r covers
-// token r>>1, part r&1; part p reads/writes at column offset p*pair_off of its token's row and uses weight w / w1.
-// rstd_out is indexed by the virtual row ([M][2]).  (Two 37 MB launches were each ~3x off the HBM time.)
-template <bool XF32, int NCH, bool PAIR>
+// ------------------------------------------------------------------ register-resident rows (D <= 256*NCH)
+// norm_fwd_kernel streams every row twice (statistics pass + output pass, the second from L1/L2).  Where the row fits
+// in registers (the block norms, D = 384..1536, and the FP8 forms up to IVB_NORM_FP8_MAX_D) one warp holds it: one HBM
+// read per operand, and the row's amax, and with it the row's power-of-two E4M3 scale (fp8_scale), is known before the
+// first byte is stored.  The statistics and y = (x - mean) * rstd * w (+ b) are the fp32 expressions of
+// norm_fwd_kernel (RMSNorm: mean = 0, and v - 0.f == v exactly), so every form holds the row ivb_norm_fwd rounds to bf16.
+// OUT is what the row becomes:
+//   NORM_Y   the bf16 row y, and rstd and (LN) mean where their pointers are non-null (ivb_norm_fwd, RMSNorm);
+//   NORM_Q   only the E4M3 row q and its scale_inv: the frozen towers' FP8 inference writes no bf16 row;
+//   NORM_QY  both, for FP8 training with per-token scales: the weight gradient reads the bf16 row y, the norm backward
+//            mean and rstd.
+// PAIR (NORM_Y only): the q-norm and the k-norm of a block in ONE launch (internvideo2_pretrain.py:198-206).  Virtual
+// row r covers token r>>1, part r&1; part p reads/writes at column offset p*pair_off of its token's row and uses weight
+// w / w1.  rstd_out is indexed by the virtual row ([M][2]).  (Two 37 MB launches were each ~3x off the HBM time.)
+enum NormOut { NORM_Y, NORM_Q, NORM_QY };
+
+template <bool XF32, bool LN, int NCH, NormOut OUT, bool PAIR>
 __global__ void __launch_bounds__(256)
-rms_fwd_reg_kernel(const void* __restrict__ x, long ldx, const __nv_bfloat16* __restrict__ w, float eps,
-                   int M, int D, __nv_bfloat16* __restrict__ y, long ldy, float* __restrict__ rstd_out,
-                   const __nv_bfloat16* __restrict__ w1, long x_pair_off, long y_pair_off) {
+norm_rows_kernel(const void* __restrict__ x, long ldx, const __nv_bfloat16* __restrict__ w,
+                 const __nv_bfloat16* __restrict__ b, float eps, int M, int D, __nv_bfloat16* __restrict__ y, long ldy,
+                 float* __restrict__ mean_out, float* __restrict__ rstd_out, uint8_t* __restrict__ q, long ldq,
+                 float* __restrict__ q_scale_inv, const __nv_bfloat16* __restrict__ w1, long x_pair_off,
+                 long y_pair_off) {
+  static_assert(!PAIR || OUT == NORM_Y, "norm_rows_kernel: PAIR writes bf16 rows only");
+  constexpr bool kQ = OUT != NORM_Y, kY = OUT != NORM_Q;
   pdl_wait();
   pdl_launch_dependents();
   const int lane = threadIdx.x & 31;
@@ -277,57 +295,25 @@ rms_fwd_reg_kernel(const void* __restrict__ x, long ldx, const __nv_bfloat16* __
     const long tok = PAIR ? (row >> 1) : row;
     const int part = PAIR ? static_cast<int>(row & 1) : 0;
     const long xo = tok * ldx + part * x_pair_off;
-    const long yo = tok * ldy + part * y_pair_off;
+    // y's offset is formed at the store: held from here, it cost the E4M3 + bf16 form two registers
+    auto yo = [&](int c) { return tok * ldy + part * y_pair_off + c * 8; };
     const __nv_bfloat16* wp = (PAIR && part) ? w1 : w;
+    // The bf16 RMSNorm sums the squares as its chunks arrive, the other forms once the row is loaded: the same sums in
+    // the same order, and each form keeps its schedule.  The other order costs the bf16 NCH-6 form 4 registers, and
+    // the E4M3 RMSNorm of bf16 rows at D = 3200 1.6 % of its time (73.7 against 72.5 us at M = 13344; H100 SXM 80 GB,
+    // 700 W power limit).
+    constexpr bool kSumAtLoad = !kQ && !LN;
     float v[NCH][8];
     float ss = 0.f;
 #pragma unroll
-    for (int i = 0; i < NCH; ++i) {
-      const int c = lane + 32 * i;
-      if (c < nch) {
-        load8<XF32>(x, xo + c * 8, v[i]);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) ss += v[i][j] * v[i][j];
-      }
-    }
-    const float rstd = rsqrtf(warp_sum(ss) * invD + eps);
-#pragma unroll
-    for (int i = 0; i < NCH; ++i) {
-      const int c = lane + 32 * i;
-      if (c < nch) {
-        float wv[8], o[8];
-        load8<false>(wp, c * 8, wv);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) o[j] = v[i][j] * rstd * wv[j];
-        store8<false>(y, yo + c * 8, o);
-      }
-    }
-    if (lane == 0 && rstd_out) rstd_out[row] = rstd;
-  }
-}
-
-// ------------------------------------------------------------------ norm -> E4M3 row (D <= 256*NCH)
-// The frozen towers' FP8 inference: the normalised row never exists in bf16.  One warp per row holds it in registers
-// (one HBM read), so the row's amax, and with it the row's power-of-two scale (fp8_scale), is known before the first
-// byte is stored.  The statistics and y = (x - mean) * rstd * w (+ b) are the fp32 expressions of norm_fwd_kernel
-// (LayerNorm) and rms_fwd_reg_kernel (RMSNorm), so y is the value ivb_norm_fwd rounds to bf16.
-// TRAIN (FP8 training with per-token scales): the same registers also give the bf16 row y and the statistics, the bits
-// ivb_norm_fwd writes, for the backward (the weight gradient reads the bf16 row, the norm backward mean and rstd).
-template <bool XF32, bool LN, int NCH, bool TRAIN>
-__device__ __forceinline__ void norm_fwd_fp8_rows(const void* __restrict__ x, long ldx, const __nv_bfloat16* __restrict__ w,
-                                                  const __nv_bfloat16* __restrict__ b, float eps, int M, int D,
-                                                  uint8_t* __restrict__ out, long ldo, float* __restrict__ scale_inv,
-                                                  __nv_bfloat16* __restrict__ y, long ldy, float* __restrict__ mean_out,
-                                                  float* __restrict__ rstd_out) {
-  const int lane = threadIdx.x & 31;
-  const int wpb = blockDim.x >> 5;
-  const int nch = D >> 3;
-  const float invD = 1.0f / static_cast<float>(D);
-  for (long row = (long)blockIdx.x * wpb + (threadIdx.x >> 5); row < M; row += (long)gridDim.x * wpb) {
-    float v[NCH][8];
-#pragma unroll
     for (int i = 0; i < NCH; ++i)
-      if (lane + 32 * i < nch) load8<XF32>(x, row * ldx + (lane + 32 * i) * 8, v[i]);
+      if (lane + 32 * i < nch) {
+        load8<XF32>(x, xo + (lane + 32 * i) * 8, v[i]);
+        if (kSumAtLoad) {
+#pragma unroll
+          for (int j = 0; j < 8; ++j) ss += v[i][j] * v[i][j];
+        }
+      }
     float mean = 0.f;
     if (LN) {
       float s = 0.f;
@@ -339,73 +325,58 @@ __device__ __forceinline__ void norm_fwd_fp8_rows(const void* __restrict__ x, lo
         }
       mean = warp_sum(s) * invD;
     }
-    float ss = 0.f;
+    if (!kSumAtLoad) {
 #pragma unroll
-    for (int i = 0; i < NCH; ++i)
-      if (lane + 32 * i < nch) {
+      for (int i = 0; i < NCH; ++i)
+        if (lane + 32 * i < nch) {
 #pragma unroll
-        for (int j = 0; j < 8; ++j) { const float d = v[i][j] - mean; ss += d * d; }
-      }
+          for (int j = 0; j < 8; ++j) { const float d = v[i][j] - mean; ss += d * d; }
+        }
+    }
     const float rstd = rsqrtf(warp_sum(ss) * invD + eps);
     unsigned m = 0;   // fp32 magnitude bits: NaN > Inf > every finite value
 #pragma unroll
     for (int i = 0; i < NCH; ++i) {
       const int c = lane + 32 * i;
       if (c < nch) {
-        float wv[8];
-        load8<false>(w, c * 8, wv);
+        float wv[8], t[8];
+        float* o = kQ ? v[i] : t;   // the E4M3 forms keep the row in v until its scale is known
+        load8<false>(wp, c * 8, wv);
 #pragma unroll
-        for (int j = 0; j < 8; ++j) v[i][j] = (v[i][j] - mean) * rstd * wv[j];
+        for (int j = 0; j < 8; ++j) o[j] = (v[i][j] - mean) * rstd * wv[j];
         if (LN && b != nullptr) {
           float bv[8];
           load8<false>(b, c * 8, bv);
 #pragma unroll
-          for (int j = 0; j < 8; ++j) v[i][j] += bv[j];
+          for (int j = 0; j < 8; ++j) o[j] += bv[j];
         }
+        if constexpr (kQ) {
 #pragma unroll
-        for (int j = 0; j < 8; ++j) m = max(m, __float_as_uint(v[i][j]) & 0x7fffffffu);
+          for (int j = 0; j < 8; ++j) m = max(m, __float_as_uint(o[j]) & 0x7fffffffu);
+        } else {
+          store8<false>(y, yo(c), o);
+        }
       }
     }
-    m = __reduce_max_sync(0xffffffffu, m);
-    float scale, sinv;
-    fp8_scale(m, 8, scale, sinv);
+    if constexpr (kQ) {
+      m = __reduce_max_sync(0xffffffffu, m);
+      float scale, sinv;
+      fp8_scale(m, 8, scale, sinv);
 #pragma unroll
-    for (int i = 0; i < NCH; ++i) {
-      const int c = lane + 32 * i;
-      if (c < nch) {
-        *reinterpret_cast<uint2*>(out + row * ldo + c * 8) = cvt_e4m3x8(v[i], scale);
-        if constexpr (TRAIN) store8<false>(y, row * ldy + c * 8, v[i]);
+      for (int i = 0; i < NCH; ++i) {
+        const int c = lane + 32 * i;
+        if (c < nch) {
+          *reinterpret_cast<uint2*>(q + row * ldq + c * 8) = cvt_e4m3x8(v[i], scale);
+          if constexpr (kY) store8<false>(y, yo(c), v[i]);
+        }
       }
+      if (lane == 0) q_scale_inv[row] = sinv;
     }
-    if (lane == 0) {
-      scale_inv[row] = sinv;
-      if constexpr (TRAIN) {
-        rstd_out[row] = rstd;
-        if (LN) mean_out[row] = mean;
-      }
+    if (kY && lane == 0) {   // NORM_QY: the caller guarantees rstd_out and (LN) mean_out
+      if (kQ || rstd_out) rstd_out[row] = rstd;
+      if (LN && (kQ || mean_out)) mean_out[row] = mean;
     }
   }
-}
-
-template <bool XF32, bool LN, int NCH>
-__global__ void __launch_bounds__(256)
-norm_fwd_fp8_kernel(const void* __restrict__ x, long ldx, const __nv_bfloat16* __restrict__ w,
-                    const __nv_bfloat16* __restrict__ b, float eps, int M, int D, uint8_t* __restrict__ out, long ldo,
-                    float* __restrict__ scale_inv) {
-  pdl_wait();
-  pdl_launch_dependents();
-  norm_fwd_fp8_rows<XF32, LN, NCH, false>(x, ldx, w, b, eps, M, D, out, ldo, scale_inv, nullptr, 0, nullptr, nullptr);
-}
-
-template <bool XF32, bool LN, int NCH>
-__global__ void __launch_bounds__(256)
-norm_fwd_fp8_train_kernel(const void* __restrict__ x, long ldx, const __nv_bfloat16* __restrict__ w,
-                          const __nv_bfloat16* __restrict__ b, float eps, int M, int D, uint8_t* __restrict__ out,
-                          long ldo, float* __restrict__ scale_inv, __nv_bfloat16* __restrict__ y, long ldy,
-                          float* __restrict__ mean_out, float* __restrict__ rstd_out) {
-  pdl_wait();
-  pdl_launch_dependents();
-  norm_fwd_fp8_rows<XF32, LN, NCH, true>(x, ldx, w, b, eps, M, D, out, ldo, scale_inv, y, ldy, mean_out, rstd_out);
 }
 
 // dynamic smem: colred rows [warps][1][D] (only when dweight != nullptr)
@@ -618,16 +589,6 @@ static int launch_rms_bwd_tma(const void* dy, long lddy, const void* x, long ldx
   return colred_finish(3, grid, D, dweight, dgamma, dcolsum, stream);
 }
 
-template <bool XF32, int NCH, bool PAIR = false>
-static int launch_rms_fwd_reg(const void* x, long ldx, const void* w, float eps, int M, int D, void* y, long ldy,
-                              float* rstd, cudaStream_t stream, const void* w1 = nullptr, long x_pair_off = 0,
-                              long y_pair_off = 0) {
-  const long rows = PAIR ? 2L * M : M;
-  return launch("rms_fwd_reg_kernel", rms_fwd_reg_kernel<XF32, NCH, PAIR>, persistent_grid(rows, 8, 8), 256, 0, stream,
-      ALLOW_PDL, x, ldx, reinterpret_cast<const __nv_bfloat16*>(w), eps, (int)rows, D, reinterpret_cast<__nv_bfloat16*>(y),
-      ldy, rstd, reinterpret_cast<const __nv_bfloat16*>(w1), x_pair_off, y_pair_off);
-}
-
 template <bool XF32, bool DXF32, int NCH, bool PAIR = false>
 static int launch_rms_bwd_reg(const void* dy, long lddy, const void* x, long ldx, const void* w, const float* rstd,
                               int M, int D, const float* dx_in, long lddx_in, void* dx_out, long lddx,
@@ -678,14 +639,91 @@ static int launch_norm_bwd(const void* dy, long lddy, const void* x, long ldx, c
 }
 
 // Runtime flags and row widths to template arguments: f(std::bool_constant<b>{}), and f(NCH) for the
-// register-resident RMSNorm kernels, whose rows hold NCH 256-column chunks (D <= 512, 1024, 1536).
+// register-resident row kernels, whose rows hold NCH 256-column chunks (D <= 512, 1024, 1536; with MAX_NCH 16, the FP8
+// forward, D <= 4096).
 template <typename F>
 static auto pick_bool(bool b, F f) { return b ? f(std::true_type{}) : f(std::false_type{}); }
-template <typename F>
+template <int MAX_NCH = 6, typename F>
 static int pick_nch(int D, F f) {
   if (D <= 512) return f(std::integral_constant<int, 2>{});
   if (D <= 1024) return f(std::integral_constant<int, 4>{});
+  if constexpr (MAX_NCH == 16) {
+    if (D > 1536) return f(std::integral_constant<int, 16>{});
+  }
   return f(std::integral_constant<int, 6>{});
+}
+
+// The operands of one norm forward; outputs that are null are not written.  q: the E4M3 row (NORM_Q / NORM_QY);
+// w1 and the pair offsets: the second part of a PAIR launch.
+struct NormFwd {
+  const void* x; long ldx; bool x_f32;
+  const void* w; const void* b; float eps; bool ln; int M; int D;
+  void* y; long ldy; float* mean; float* rstd;
+  void* q = nullptr; long ldq = 0; float* q_scale_inv = nullptr;
+  const void* w1 = nullptr; long x_pair_off = 0, y_pair_off = 0;
+};
+
+// The one forward launch path.  NORM_Y: RMSNorm rows up to D = 1536 (and every PAIR launch) on the register-resident
+// kernel, read from HBM exactly once; LayerNorm and wider RMSNorm rows on the streaming norm_fwd_kernel.  The E4M3
+// forms always hold the row in registers.
+template <NormOut OUT, bool PAIR = false>
+static int launch_norm_fwd(const NormFwd& a, cudaStream_t stream) {
+  const __nv_bfloat16* w = reinterpret_cast<const __nv_bfloat16*>(a.w);
+  const __nv_bfloat16* b = reinterpret_cast<const __nv_bfloat16*>(a.b);
+  __nv_bfloat16* y = reinterpret_cast<__nv_bfloat16*>(a.y);
+  const long rows = PAIR ? 2L * a.M : a.M;
+  const int blocks = persistent_grid(rows, 8, 8);
+  auto in_registers = [&](auto xf, auto ln) {
+    return pick_nch<OUT == NORM_Y ? 6 : 16>(a.D, [&](auto nch) {
+      return launch("norm_rows_kernel", norm_rows_kernel<xf, ln, nch, OUT, PAIR>, blocks, 256, 0, stream, ALLOW_PDL,
+                    a.x, a.ldx, w, b, a.eps, (int)rows, a.D, y, a.ldy, a.mean, a.rstd,
+                    reinterpret_cast<uint8_t*>(a.q), a.ldq, a.q_scale_inv,
+                    reinterpret_cast<const __nv_bfloat16*>(a.w1), a.x_pair_off, a.y_pair_off);
+    });
+  };
+  if constexpr (PAIR) {   // the q/k norms: RMSNorm of bf16 rows
+    return in_registers(std::false_type{}, std::false_type{});
+  } else {
+    return pick_bool(a.x_f32, [&](auto xf) {
+      if constexpr (OUT == NORM_Y) {
+        if (!a.ln && a.D <= 1536) return in_registers(xf, std::false_type{});
+        return pick_bool(a.ln, [&](auto ln) {
+          return launch("norm_fwd_kernel", norm_fwd_kernel<xf, ln>, blocks, 256, 0, stream, ALLOW_PDL, a.x, a.ldx, w, b,
+                        a.eps, a.M, a.D, y, a.ldy, a.mean, a.rstd);
+        });
+      } else {
+        return pick_bool(a.ln, [&](auto ln) { return in_registers(xf, ln); });
+      }
+    });
+  }
+}
+
+// Sets the error text "<fn>: <what>"; returns set_error's status.
+static int fail(const char* fn, const char* what) {
+  char msg[128];
+  snprintf(msg, sizeof(msg), "%s: %s", fn, what);
+  return set_error(msg);
+}
+
+// The checks of ivb_norm_fwd_fp8 and, with train, of ivb_norm_fwd_fp8_train (which also needs y, rstd and the
+// LayerNorm mean); fn names the entry point in messages.
+static int check_norm_fwd_fp8(const char* fn, bool train, const NormFwd& a) {
+  if (a.M <= 0) return fail(fn, "empty tensor");
+  if (a.D <= 0 || a.D > IVB_NORM_FP8_MAX_D || (a.D & 7))
+    return fail(fn, "D must be a multiple of 8 in [8, IVB_NORM_FP8_MAX_D]");
+  if ((a.ldx & 7) || a.ldx < a.D) return fail(fn, "ldx must be a multiple of 8 elements and >= D");
+  if ((a.ldq & 15) || a.ldq < a.D) return fail(fn, "ldo must be a multiple of 16 elements and >= D");
+  if (train && ((a.ldy & 7) || a.ldy < a.D)) return fail(fn, "ldy must be a multiple of 8 elements and >= D");
+  if (a.x == nullptr || a.w == nullptr || a.q == nullptr || a.q_scale_inv == nullptr ||
+      (train && (a.y == nullptr || a.rstd == nullptr || (a.ln && a.mean == nullptr))))
+    return fail(fn, train ? "x, weight, out, row_scale_inv, y, rstd or (LayerNorm) mean is null"
+                          : "x, weight, out or row_scale_inv is null");
+  if (misaligned(16, a.x, a.w, a.b, a.q, a.y))
+    return fail(fn, train ? "x, weight, bias, out and y must be 16-byte aligned"
+                          : "x, weight, bias and out must be 16-byte aligned");
+  if (misaligned(4, a.q_scale_inv, a.mean, a.rstd))
+    return fail(fn, train ? "row_scale_inv, mean and rstd must be 4-byte aligned" : "row_scale_inv must be 4-byte aligned");
+  return 0;
 }
 
 }  // namespace ivb
@@ -695,91 +733,30 @@ using namespace ivb;
 extern "C" int ivb_norm_fwd(const void* x, int x_is_f32, long ldx, const void* weight,
                             const void* bias, float eps, int is_layernorm, int M, int D, void* y,
                             long ldy, float* mean, float* rstd, void* stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (M <= 0) return 0;
   if ((D & 7) || (ldx & 7) || (ldy & 7)) return set_error("ivb_norm_fwd: D/ld must be multiples of 8");
   if (misaligned(16, x, weight, bias, y)) return set_error("ivb_norm_fwd: x, weight, bias and y must be 16-byte aligned");
-  if (!is_layernorm && D <= 1536)   // register-resident RMSNorm: the row is read from HBM exactly once
-    return pick_bool(x_is_f32, [&](auto xf) {
-      return pick_nch(D, [&](auto nch) { return launch_rms_fwd_reg<xf, nch>(x, ldx, weight, eps, M, D, y, ldy, rstd, stream); });
-    });
-  const int blocks = persistent_grid(M, 8, 8);
-  const __nv_bfloat16* w = reinterpret_cast<const __nv_bfloat16*>(weight);
-  const __nv_bfloat16* b = reinterpret_cast<const __nv_bfloat16*>(bias);
-  __nv_bfloat16* yo = reinterpret_cast<__nv_bfloat16*>(y);
-  return pick_bool(x_is_f32, [&](auto xf) {
-    return pick_bool(is_layernorm, [&](auto ln) {
-      return launch("norm_fwd_kernel", norm_fwd_kernel<xf, ln>, blocks, 256, 0, stream, ALLOW_PDL, x, ldx, w, b, eps, M,
-                    D, yo, ldy, mean, rstd);
-    });
-  });
+  return launch_norm_fwd<NORM_Y>({x, ldx, x_is_f32 != 0, weight, bias, eps, is_layernorm != 0, M, D, y, ldy, mean, rstd},
+                                 reinterpret_cast<cudaStream_t>(stream_));
 }
 
 extern "C" int ivb_norm_fwd_fp8(const void* x, int x_is_f32, long ldx, const void* weight, const void* bias, float eps,
                                 int is_layernorm, int M, int D, void* out, long ldo, float* row_scale_inv,
                                 void* stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  if (M <= 0) return set_error("ivb_norm_fwd_fp8: empty tensor");
-  if (D <= 0 || D > IVB_NORM_FP8_MAX_D || (D & 7))
-    return set_error("ivb_norm_fwd_fp8: D must be a multiple of 8 in [8, IVB_NORM_FP8_MAX_D]");
-  if ((ldx & 7) || ldx < D) return set_error("ivb_norm_fwd_fp8: ldx must be a multiple of 8 elements and >= D");
-  if ((ldo & 15) || ldo < D) return set_error("ivb_norm_fwd_fp8: ldo must be a multiple of 16 elements and >= D");
-  if (x == nullptr || weight == nullptr || out == nullptr || row_scale_inv == nullptr)
-    return set_error("ivb_norm_fwd_fp8: x, weight, out or row_scale_inv is null");
-  if ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(weight) | reinterpret_cast<uintptr_t>(bias) |
-       reinterpret_cast<uintptr_t>(out)) & 15)
-    return set_error("ivb_norm_fwd_fp8: x, weight, bias and out must be 16-byte aligned");
-  if (reinterpret_cast<uintptr_t>(row_scale_inv) & 3)
-    return set_error("ivb_norm_fwd_fp8: row_scale_inv must be 4-byte aligned");
-  const __nv_bfloat16* w = reinterpret_cast<const __nv_bfloat16*>(weight);
-  const __nv_bfloat16* b = reinterpret_cast<const __nv_bfloat16*>(bias);
-  uint8_t* o = reinterpret_cast<uint8_t*>(out);
-  const int blocks = persistent_grid(M, 8, 8);
-  return pick_bool(x_is_f32, [&](auto xf) {
-    return pick_bool(is_layernorm, [&](auto ln) {
-      auto go = [&](auto nch) {
-        return launch("norm_fwd_fp8_kernel", norm_fwd_fp8_kernel<xf, ln, nch>, blocks, 256, 0, stream, ALLOW_PDL, x, ldx,
-                      w, b, eps, M, D, o, ldo, row_scale_inv);
-      };
-      if (D > 1536) return go(std::integral_constant<int, 16>{});
-      return pick_nch(D, go);
-    });
-  });
+  const NormFwd a{x, ldx, x_is_f32 != 0, weight, bias, eps, is_layernorm != 0, M, D, nullptr, 0, nullptr, nullptr,
+                  out, ldo, row_scale_inv};
+  if (int rc = check_norm_fwd_fp8("ivb_norm_fwd_fp8", false, a)) return rc;
+  return launch_norm_fwd<NORM_Q>(a, reinterpret_cast<cudaStream_t>(stream_));
 }
 
 extern "C" int ivb_norm_fwd_fp8_train(const void* x, int x_is_f32, long ldx, const void* weight, const void* bias,
                                       float eps, int is_layernorm, int M, int D, void* out, long ldo,
                                       float* row_scale_inv, void* y, long ldy, float* mean, float* rstd,
                                       void* stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  if (M <= 0) return set_error("ivb_norm_fwd_fp8_train: empty tensor");
-  if (D <= 0 || D > IVB_NORM_FP8_MAX_D || (D & 7))
-    return set_error("ivb_norm_fwd_fp8_train: D must be a multiple of 8 in [8, IVB_NORM_FP8_MAX_D]");
-  if ((ldx & 7) || ldx < D) return set_error("ivb_norm_fwd_fp8_train: ldx must be a multiple of 8 elements and >= D");
-  if ((ldo & 15) || ldo < D) return set_error("ivb_norm_fwd_fp8_train: ldo must be a multiple of 16 elements and >= D");
-  if ((ldy & 7) || ldy < D) return set_error("ivb_norm_fwd_fp8_train: ldy must be a multiple of 8 elements and >= D");
-  if (x == nullptr || weight == nullptr || out == nullptr || row_scale_inv == nullptr || y == nullptr ||
-      rstd == nullptr || (is_layernorm && mean == nullptr))
-    return set_error("ivb_norm_fwd_fp8_train: x, weight, out, row_scale_inv, y, rstd or (LayerNorm) mean is null");
-  if (misaligned(16, x, weight, bias, out, y))
-    return set_error("ivb_norm_fwd_fp8_train: x, weight, bias, out and y must be 16-byte aligned");
-  if (misaligned(4, row_scale_inv, mean, rstd))
-    return set_error("ivb_norm_fwd_fp8_train: row_scale_inv, mean and rstd must be 4-byte aligned");
-  const __nv_bfloat16* w = reinterpret_cast<const __nv_bfloat16*>(weight);
-  const __nv_bfloat16* b = reinterpret_cast<const __nv_bfloat16*>(bias);
-  uint8_t* o = reinterpret_cast<uint8_t*>(out);
-  __nv_bfloat16* yo = reinterpret_cast<__nv_bfloat16*>(y);
-  const int blocks = persistent_grid(M, 8, 8);
-  return pick_bool(x_is_f32, [&](auto xf) {
-    return pick_bool(is_layernorm, [&](auto ln) {
-      auto go = [&](auto nch) {
-        return launch("norm_fwd_fp8_train_kernel", norm_fwd_fp8_train_kernel<xf, ln, nch>, blocks, 256, 0, stream,
-                      ALLOW_PDL, x, ldx, w, b, eps, M, D, o, ldo, row_scale_inv, yo, ldy, mean, rstd);
-      };
-      if (D > 1536) return go(std::integral_constant<int, 16>{});
-      return pick_nch(D, go);
-    });
-  });
+  const NormFwd a{x, ldx, x_is_f32 != 0, weight, bias, eps, is_layernorm != 0, M, D, y, ldy, mean, rstd,
+                  out, ldo, row_scale_inv};
+  if (int rc = check_norm_fwd_fp8("ivb_norm_fwd_fp8_train", true, a)) return rc;
+  return launch_norm_fwd<NORM_QY>(a, reinterpret_cast<cudaStream_t>(stream_));
 }
 
 extern "C" int ivb_norm_bwd(const void* dy, long lddy, const void* x, int x_is_f32, long ldx,
@@ -851,15 +828,16 @@ extern "C" int ivb_colsum_bf16(const void* x, long ldx, int M, int N, float* out
 extern "C" int ivb_rmsnorm_pair_fwd(const void* x, long ldx, long x_pair_off, const void* w0, const void* w1,
                                     float eps, int M, int D, void* y, long ldy, long y_pair_off, float* rstd,
                                     void* stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (M <= 0) return 0;
   if ((D & 7) || (ldx & 7) || (ldy & 7) || (x_pair_off & 7) || (y_pair_off & 7))
     return set_error("ivb_rmsnorm_pair_fwd: D/ld/offsets must be multiples of 8");
   if (D > 1536) return set_error("ivb_rmsnorm_pair_fwd: D > 1536 (use two ivb_norm_fwd calls)");
   if (misaligned(16, x, w0, w1, y)) return set_error("ivb_rmsnorm_pair_fwd: x, w0, w1 and y must be 16-byte aligned");
-  return pick_nch(D, [&](auto nch) {
-    return launch_rms_fwd_reg<false, nch, true>(x, ldx, w0, eps, M, D, y, ldy, rstd, stream, w1, x_pair_off, y_pair_off);
-  });
+  NormFwd a{x, ldx, false, w0, nullptr, eps, false, M, D, y, ldy, nullptr, rstd};
+  a.w1 = w1;
+  a.x_pair_off = x_pair_off;
+  a.y_pair_off = y_pair_off;
+  return launch_norm_fwd<NORM_Y, true>(a, reinterpret_cast<cudaStream_t>(stream_));
 }
 
 extern "C" int ivb_rmsnorm_pair_bwd(const void* dy, long lddy, long dy_pair_off, const void* x, long ldx,
