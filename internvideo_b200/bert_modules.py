@@ -18,7 +18,8 @@ The path of forward(input_ids, attention_mask, mode="text"), the reference's enc
              LN(h1 + g W2^T + b2)
 Precision of the residual path: bf16, as the reference keeps it when it runs in bf16.  Each LayerNorm writes its row in
 bf16, and the next residual sum is formed in the GEMM epilogue in fp32 (acc + bias + the bf16 residual) and rounded to
-bf16 once, in place over the residual; the LayerNorm statistics are fp32.
+bf16 once, in place over the residual; the LayerNorm statistics are fp32.  modules.set_fp8_inference switches the text
+layers to FP8 GEMMs (BertLayer.forward_text); the residual path stays as above.
 
 Key lengths come from attention_mask on the device: kv_len[b] = attention_mask[b].sum().  The reference masks the
 padded keys with an additive -10000, which underflows to the same zero probability as the kernel's -inf; padded
@@ -41,7 +42,7 @@ import torch
 import torch.nn as nn
 
 from . import lowlevel as ll
-from .modules import check_input, index_poison
+from .modules import Fp8InferenceSwitch, block_precision, check_input, index_poison
 
 # configs/config_bert_large.json of the multi-modality recipes (fusion_layer 19: the text layers are 0..18)
 BERT_LARGE = {"architectures": ["BertForMaskedLM"], "attention_probs_dropout_prob": 0.1, "gradient_checkpointing": False,
@@ -122,8 +123,19 @@ class BertOutput(nn.Module):
         self.LayerNorm = nn.LayerNorm(config.hidden_size, eps=config.layer_norm_eps)
 
 
-class BertLayer(nn.Module):
-    """xbert.py:599-687; the cross-attention of layers >= fusion_layer is a parameter container only."""
+def layer_norm(x, ln, fp8):
+    """A post-LN LayerNorm of the bf16 rows x: (bf16 rows, None), or with fp8 (the next GEMM runs in FP8) the same bf16
+    rows and, from the same read of each row, their E4M3 rows with per-row scales (lowlevel.norm_fwd_fp8, save=True;
+    its statistics are not used)."""
+    if not fp8:
+        return ll.norm_fwd(x, ln.weight, ln.bias, eps=ln.eps, layernorm=True, want_stats=False)[0], None
+    q, s, y, _, _ = ll.norm_fwd_fp8(x, ln.weight, ln.bias, eps=ln.eps, layernorm=True, save=True)
+    return y, (q, s)
+
+
+class BertLayer(Fp8InferenceSwitch, nn.Module):
+    """xbert.py:599-687; the cross-attention of layers >= fusion_layer is a parameter container only.  A text layer
+    (below fusion_layer) runs in FP8 under modules.set_fp8_inference."""
 
     def __init__(self, config, layer_num):
         super().__init__()
@@ -134,25 +146,46 @@ class BertLayer(nn.Module):
         self.intermediate = BertIntermediate(config)
         self.output = BertOutput(config)
 
-    def forward_text(self, h, B, L, kv_len):
+    def _fp8_linears(self):
+        """The six GEMM weights of a text layer: query, key, value, attention output, intermediate, output; none for a
+        fusion layer, which text mode never runs."""
+        if self.has_cross_attention:
+            return ()
+        sa = self.attention.self
+        return (sa.query, sa.key, sa.value, self.attention.output.dense, self.intermediate.dense, self.output.dense)
+
+    def forward_text(self, h, B, L, kv_len, h8=None, fp8_out=False):
         """The self-attention layer over h, bf16 [B*L, D] (overwritten: it holds the first residual sum afterwards),
-        with per-caption key lengths kv_len int32 [B] -> the layer output, bf16 [B*L, D].  7 library calls."""
+        with per-caption key lengths kv_len int32 [B] -> (the layer output, bf16 [B*L, D], and with fp8_out its E4M3
+        rows and row scales, else None).  7 library calls in bf16.
+
+        Under set_fp8_inference the six GEMMs run on the FP8 tensor cores (lowlevel.gemm_fp8) with per-token
+        activation scales and the per-output-channel weight copies, each keeping its bf16 epilogue (bias, GELU, the
+        in-place residual sum); h8: h's E4M3 rows and scales as the previous LayerNorm wrote them (None: cast here),
+        the attention output and g are cast row by row, and the first LayerNorm writes the intermediate GEMM's E4M3
+        rows with the residual.  Attention stays bf16."""
         sa, so = self.attention.self, self.attention.output
         M, D = h.shape
         H, d = sa.num_attention_heads, sa.attention_head_size
+        w8 = None if self.fp8_inference is None else block_precision(self)
+
+        def linear(act, act8, i, lin, **epilogue):
+            if w8 is None:
+                return ll.gemm(act, lin.weight, bias=lin.bias, **epilogue)
+            q, s = act8 if act8 is not None else ll.fp8_quantize_rows(act)
+            return ll.gemm_fp8(q, s, *w8[i], bias=lin.bias, **epilogue)
+        if w8 is not None and h8 is None:
+            h8 = ll.fp8_quantize_rows(h)
         qkv = torch.empty((M, 3 * D), device=h.device, dtype=torch.bfloat16)
         for i, lin in enumerate((sa.query, sa.key, sa.value)):
-            ll.gemm(h, lin.weight, bias=lin.bias, out0=qkv[:, i * D:(i + 1) * D])
+            linear(h, h8, i, lin, out0=qkv[:, i * D:(i + 1) * D])
         a, _ = ll.attn_fwd(qkv[:, :D], qkv[:, D:2 * D], qkv[:, 2 * D:], B, L, H, d, d ** -0.5, want_lse=False,
                            kv_len=kv_len)
-        ll.gemm(a, so.dense.weight, bias=so.dense.bias, flags=ll.FLAG_ACCUM, out0=h)          # h + a Wo^T + bo
-        h1, _, _ = ll.norm_fwd(h, so.LayerNorm.weight, so.LayerNorm.bias, eps=so.LayerNorm.eps, layernorm=True,
-                               want_stats=False)
-        g = ll.gemm(h1, self.intermediate.dense.weight, bias=self.intermediate.dense.bias, epi=ll.EPI_BIAS_GELU)
-        ll.gemm(g, self.output.dense.weight, bias=self.output.dense.bias, flags=ll.FLAG_ACCUM, out0=h1)  # h1 + g W2^T + b2
-        out, _, _ = ll.norm_fwd(h1, self.output.LayerNorm.weight, self.output.LayerNorm.bias,
-                                eps=self.output.LayerNorm.eps, layernorm=True, want_stats=False)
-        return out
+        linear(a, None, 3, so.dense, flags=ll.FLAG_ACCUM, out0=h)                        # h + a Wo^T + bo
+        h1, h1_8 = layer_norm(h, so.LayerNorm, w8 is not None)
+        g = linear(h1, h1_8, 4, self.intermediate.dense, epi=ll.EPI_BIAS_GELU)
+        linear(g, None, 5, self.output.dense, flags=ll.FLAG_ACCUM, out0=h1)             # h1 + g W2^T + b2
+        return layer_norm(h1, self.output.LayerNorm, fp8_out)
 
 
 class BertEncoder(nn.Module):
@@ -238,9 +271,10 @@ class BertModel(nn.Module):
         emb = self.embeddings
         pos = (emb.position_embeddings.weight[:L].float() + emb.token_type_embeddings.weight[0].float()).to(torch.bfloat16)
         x, err = ll._token_embed_fwd(input_ids.long().contiguous(), emb.word_embeddings.weight, pos)
-        h, _, _ = ll.norm_fwd(x, emb.LayerNorm.weight, emb.LayerNorm.bias, eps=emb.LayerNorm.eps, layernorm=True,
-                              want_stats=False)
+        layers = self.encoder.layer[:self.config.fusion_layer]
+        fp8 = [layer.fp8_inference is not None for layer in layers] + [False]
+        h, h8 = layer_norm(x, emb.LayerNorm, fp8[0])     # each LayerNorm also writes E4M3 rows for an FP8 layer after it
         kv_len = key_lengths(attention_mask, B, L, input_ids.device)
-        for layer in self.encoder.layer[:self.config.fusion_layer]:
-            h = layer.forward_text(h, B, L, kv_len)
+        for i, layer in enumerate(layers):
+            h, h8 = layer.forward_text(h, B, L, kv_len, h8, fp8_out=fp8[i + 1])
         return BertTextOutput(h.reshape(B, L, -1) + index_poison(err))

@@ -250,7 +250,32 @@ class Mlp(nn.Module):
 FusedMLP = partial(Mlp, gelu_tanh=True)
 
 
-class Block(nn.Module):
+class Fp8InferenceSwitch:
+    """The switch set_fp8_inference sets on a module, read when it runs: fp8_inference holds the Fp8InferenceWeights of
+    its _fp8_linears() while the mode is on (None when off), fp8_attention whether set_fp8_inference(attention=True)
+    asked for attention on the FP8 tensor cores too."""
+    fp8_inference = None
+    fp8_attention = False
+
+    def _fp8_linears(self):
+        raise NotImplementedError
+
+
+class Fp8Block(Fp8InferenceSwitch):
+    """The fused blocks both FP8 switches set (Block, VideoMAEBlock, text_modules.TransformerEncoder): set_fp8's
+    training mode, its scaling, "tensor" or "token", and with "token" whether the weight gradients run in FP8 too, read
+    at call time through block_precision; and set_fp8_inference's switch."""
+    fp8 = False
+    fp8_scaling = "tensor"
+    fp8_wgrad = False
+
+    def _fp8_linears(self):
+        """The block's four GEMM weights' Linears: qkv, proj, fc1, fc2."""
+        a, mlp = self.attn, self.mlp
+        return (a.qkv, a.proj, mlp.fc1, mlp.fc2)
+
+
+class Block(Fp8Block, nn.Module):
     """internvideo2_pretrain.py:247-297.  Both call forms are supported: `blk(x)` (naive, returns x) and
     `blk(x, residual)` (fused pre-norm form, returns `(branch, residual)` such that x_out = branch + residual)."""
 
@@ -276,15 +301,6 @@ class Block(nn.Module):
         self.with_cp = bool(with_cp)
         self.use_fused_rmsnorm = use_fused_rmsnorm
         self.num_heads = num_heads
-        # FP8 GEMMs for the forward and input-gradient passes (set_fp8), their scaling, "tensor" or "token", and with
-        # "token" whether the weight gradients run in FP8 too; read at call time
-        self.fp8 = False
-        self.fp8_scaling = "tensor"
-        self.fp8_wgrad = False
-        # FP8 inference with per-channel weight copies (set_fp8_inference); None when off.  fp8_attention: its
-        # attention=True, attention on the FP8 tensor cores too
-        self.fp8_inference = None
-        self.fp8_attention = False
 
     def forward_stream(self, x2d, B, n, rowscale=None, plans=None):
         """fp32 residual stream [B*n, D] -> [B*n, D] (the hot path used by the model).
@@ -326,9 +342,6 @@ class Block(nn.Module):
                                        rowscale[1], save=False)
         return out
 
-    def _fp8_linears(self):
-        return (self.attn.qkv, self.attn.proj, self.mlp.fc1, self.mlp.fc2)
-
     def forward(self, x, residual=None):
         B, n, D = x.shape
         if residual is not None:
@@ -366,7 +379,7 @@ class VideoMAEAttention(nn.Module):
         return torch.cat((self.q_bias, torch.zeros_like(self.v_bias), self.v_bias))
 
 
-class VideoMAEBlock(nn.Module):
+class VideoMAEBlock(Fp8Block, nn.Module):
     """The VideoMAE LayerNorm block (videomae.py:104-132 for the VideoMAEv2 teacher, IV1 modeling_finetune.py:132-181):
     LayerNorm pre-norm, q/v-bias attention, erf GELU MLP, optional gamma_1 / gamma_2, through ops.block_forward with
     spec.layernorm and, when trained, ops.BlockFn.  with_cp: keep only the block input and recompute its forward in
@@ -389,8 +402,6 @@ class VideoMAEBlock(nn.Module):
             self.gamma_1 = self.gamma_2 = None
         self.drop_prob = float(drop_path)
         self.with_cp = bool(with_cp)
-        self.fp8_inference = None   # set_fp8_inference
-        self.fp8_attention = False  # set_fp8_inference(attention=True)
 
     def _drop_path_rows(self, B, n, device):
         """IV1's DropPath draw (timm drop_path: Bernoulli(keep) / keep per sample, `rand < keep`), once per branch in
@@ -429,9 +440,6 @@ class VideoMAEBlock(nn.Module):
                                        rowscale[1], save=False)
         return out
 
-    def _fp8_linears(self):
-        return (self.attn.qkv, self.attn.proj, self.mlp.fc1, self.mlp.fc2)
-
     def forward(self, x):
         B, n, D = x.shape
         return self.forward_stream(x.reshape(B * n, D).float().contiguous(), B, n).reshape(B, n, D)
@@ -453,8 +461,12 @@ def set_droppath_skip(model: nn.Module, enabled: bool = True) -> int:
 
 
 def set_fp8(model: nn.Module, enabled: bool = True, scaling: str = "tensor", wgrad: bool = False) -> int:
-    """Switch the FP8 mode of every ViT Block in `model` (stage-1 student, CLIP tower, stage-2 tower, InternVL teacher)
-    on or off; returns how many blocks were switched.
+    """Switch the FP8 mode of every fused block in `model` on or off; returns how many blocks were switched.  The
+    blocks: the RMSNorm Blocks (stage-1 student, CLIP tower, stage-2 tower, InternVL teacher), the LayerNorm
+    VideoMAEBlocks (InternVideo1's VideoMAE encoder and decoder, the VideoMAEv2 teacher) and the MobileCLIP text
+    tower's text_modules.TransformerEncoder blocks.  The LayerNorm blocks take every scaling the RMSNorm block takes;
+    their norms write the same E4M3 rows (with the LayerNorm bias), their GEMMs the same epilogues (the VideoMAE q/v
+    bias and gamma, the text tower's full qkv bias), and the text tower's causal attention stays bf16.
 
     In FP8 mode a block runs its forward GEMMs (qkv, proj, fc1, fc2) and its input-gradient GEMMs on the FP8 tensor
     cores, every scale a power of two from the amax of what it scales (no state, nothing in the state_dict).
@@ -473,7 +485,7 @@ def set_fp8(model: nn.Module, enabled: bool = True, scaling: str = "tensor", wgr
         raise ValueError(f"set_fp8: wgrad=True needs scaling='token', got {scaling!r}")
     n = 0
     for mod in model.modules():
-        if isinstance(mod, Block):
+        if isinstance(mod, Fp8Block):
             mod.fp8 = bool(enabled)
             mod.fp8_scaling = scaling
             mod.fp8_wgrad = bool(wgrad)
@@ -504,8 +516,8 @@ class Fp8InferenceWeights:
 
 
 def block_precision(block, training=False):
-    """The ops.BlockSpec precision a forward of `block` (Block or VideoMAEBlock) runs at, from its switches:
-    set_fp8 (Block.fp8) and set_fp8_inference (fp8_inference).  training: the forward needs a gradient."""
+    """The ops.BlockSpec precision a forward of `block` (an Fp8Block, or a BertLayer for its fp8_inference) runs at,
+    from its switches: set_fp8 (fp8) and set_fp8_inference (fp8_inference).  training: the forward needs a gradient."""
     fp8 = getattr(block, "fp8", False)
     if block.fp8_inference is None:
         if not fp8:
@@ -525,8 +537,10 @@ def block_attn_fp8(block, head_axis=False):
 
 
 def set_fp8_inference(model: nn.Module, enabled: bool = True, attention: bool = False) -> int:
-    """Switch FP8 inference on or off for every ViT Block and VideoMAEBlock in `model` (frozen towers: the
-    InternVL and VideoMAE teachers, the frozen CLIP and stage-2 towers); returns how many blocks were switched.
+    """Switch FP8 inference on or off for every fused block (Block, VideoMAEBlock, text_modules.TransformerEncoder)
+    and every text layer of bert_modules.BertModel in `model` (frozen towers: the InternVL and VideoMAE teachers, the
+    frozen CLIP and stage-2 towers, the MobileCLIP text tower, the stage-2 BERT text encoder); returns how many blocks
+    and layers were switched (a BERT layer from fusion_layer on runs nothing in text mode and is not switched).
 
     In this mode a block's no-grad forward runs its four GEMMs (qkv, proj, fc1, fc2) on the FP8 tensor cores with
     per-token activation scales, computed where each activation is produced (n1 and n2 inside the norm kernel, a and
@@ -535,9 +549,12 @@ def set_fp8_inference(model: nn.Module, enabled: bool = True, attention: bool = 
     attention=False (the default) keeps attention bf16; attention=True also runs the token-axis attention on the FP8
     tensor cores: q and k cast to E4M3 with one scale per (token, head), v per (clip, head, channel), P in E4M3
     (lowlevel._attn_fp8_pack, _attn_fwd_fp8).  The VideoMAEv2 teacher's head-axis attention (head_axis_attention=True)
-    keeps its own kernel either way.  Switching off restores the bf16 path bit for bit.  A switched Block refuses a
-    forward that needs a gradient, and the mode excludes set_fp8 on the same block."""
-    blocks = [m for m in model.modules() if isinstance(m, (Block, VideoMAEBlock))]
+    keeps its own kernel either way, and so do the text tower's causal attention and BERT's key-length attention, which
+    stay bf16.  A BERT layer runs its qkv, attention-output, intermediate and output GEMMs on the FP8 tensor cores;
+    each post-LN LayerNorm writes its row once as the bf16 residual and as the E4M3 rows of the next GEMM
+    (lowlevel.norm_fwd_fp8 with save=True).  Switching off restores the bf16 path bit for bit.  A switched block
+    refuses a forward that needs a gradient, and the mode excludes set_fp8 on the same block."""
+    blocks = [m for m in model.modules() if isinstance(m, Fp8InferenceSwitch) and m._fp8_linears()]
     if enabled and any(getattr(m, "fp8", False) for m in blocks):
         raise ll._lib.IvbError("set_fp8_inference: a block is in FP8 training mode (set_fp8); switch that off first")
     for m in blocks:

@@ -21,7 +21,7 @@ import torch.nn as nn
 
 from . import lowlevel as ll
 from . import ops
-from .modules import check_input, index_poison
+from .modules import Fp8Block, block_attn_fp8, block_precision, check_input, index_poison
 
 # text_cfg and embed_dim of mobileclip/configs/mobileclip_b.json
 MOBILECLIP_B = {"context_length": 77, "vocab_size": 49408, "dim": 512, "ffn_multiplier_per_layer": 4.0,
@@ -60,10 +60,11 @@ class MultiHeadAttention(nn.Module):
         self.num_heads, self.embed_dim = num_heads, embed_dim
 
 
-class TransformerEncoder(nn.Module):
+class TransformerEncoder(Fp8Block, nn.Module):
     """transformer.py:333-450: pre-norm block, LayerNorm (eps 1e-5, fp32 statistics) -> MHA -> residual, LayerNorm ->
     Linear -> GELU (erf) -> Linear -> residual, no LayerScale, dropout 0.  Runs as one fused block (ops.BlockFn, or
-    ops.block_forward without saving anything when no gradient is needed)."""
+    ops.block_forward without saving anything when no gradient is needed), at the precision modules.set_fp8 and
+    modules.set_fp8_inference choose; causal attention stays bf16 in every precision."""
 
     def __init__(self, embed_dim, ffn_latent_dim, num_heads=8):
         super().__init__()
@@ -73,10 +74,15 @@ class TransformerEncoder(nn.Module):
                                           nn.Dropout(p=0.0), nn.Linear(ffn_latent_dim, embed_dim), nn.Dropout(p=0.0))
         self.embed_dim, self.ffn_dim = embed_dim, ffn_latent_dim
 
-    def _spec(self, B, n, causal):
+    def _spec(self, B, n, causal, training=False):
         ln1, a, ln2 = self.pre_norm_mha[0], self.pre_norm_mha[1], self.pre_norm_ffn[0]
         return ops.BlockSpec(B, n, a.num_heads, layernorm=True, eps1=ln1.eps, eps2=ln2.eps, scale=a.scaling,
-                             causal=causal)
+                             causal=causal, precision=block_precision(self, training),
+                             attn_fp8=block_attn_fp8(self) and not causal)
+
+    def _fp8_linears(self):
+        a = self.pre_norm_mha[1]
+        return (a.qkv_proj, a.out_proj, self.pre_norm_ffn[1], self.pre_norm_ffn[4])
 
     def _param_tuple(self):
         ln1, a, ln2 = self.pre_norm_mha[0], self.pre_norm_mha[1], self.pre_norm_ffn[0]
@@ -89,7 +95,7 @@ class TransformerEncoder(nn.Module):
         """fp32 residual stream [B*n, D] -> same.  Differentiated (ops.BlockFn) when grad mode is on and the stream or a
         parameter of the block needs a gradient; otherwise the no-grad block forward."""
         if torch.is_grad_enabled() and (x2d.requires_grad or any(p.requires_grad for p in self.parameters())):
-            return ops.BlockFn.apply(x2d, self._spec(B, n, causal), None, None, *self._param_tuple())
+            return ops.BlockFn.apply(x2d, self._spec(B, n, causal, training=True), None, None, *self._param_tuple())
         with torch.no_grad():
             out, _ = ops.block_forward(x2d, self._spec(B, n, causal), self._param_tuple(), save=False)
         return out

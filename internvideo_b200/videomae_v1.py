@@ -51,6 +51,19 @@ def _run_blocks(blocks, h, B, n):
     return run_blocks(blocks, h, lambda i, blk, h: blk.forward_stream(h, B, n))[0]
 
 
+def _device_table(module, device):
+    """module.pos_embed on `device`.  The fixed sinusoid table is a plain host tensor, not module state (as in the
+    reference): it is copied to the device once and the copy kept, so a forward makes no host-to-device copy and the
+    training step can be captured in a CUDA graph.  A learnable table (nn.Parameter) is returned as it is."""
+    pe = module.pos_embed
+    if isinstance(pe, nn.Parameter) or pe.device == device:
+        return pe
+    dev = getattr(module, "_pos_embed_on_device", None)
+    if dev is None or dev.device != device:
+        dev = module._pos_embed_on_device = pe.to(device)
+    return dev
+
+
 def _xavier_init(m):
     if isinstance(m, nn.Linear):
         nn.init.xavier_uniform_(m.weight)
@@ -106,7 +119,7 @@ class PretrainVisionTransformerEncoder(nn.Module):
     def forward_rows(self, x, idx, B, nv):
         """x bf16 video, idx int32 [B, 1+nv] (cls slot + visible patches) -> bf16 [B*nv, C_e] after the final LayerNorm."""
         pe = self.patch_embed
-        pos = self.pos_embed[:, -pe.num_patches:].to(device=x.device)          # learnable table has an unused first row
+        pos = _device_table(self, x.device)[:, -pe.num_patches:]              # learnable table has an unused first row
         h = _run_blocks(self.blocks, embed_tokens(pe, x, idx, None, pos), B, nv)
         h = ops.layernorm(h, self.norm.weight, self.norm.bias, self.norm.eps)
         if isinstance(self.head, nn.Linear):
@@ -204,7 +217,7 @@ class PretrainVisionTransformer(nn.Module):
         self.index_error = err_v + err_m                         # non-zero: clips keep different numbers of tokens
         h = self.encoder.forward_rows(x.to(bf16), vis, B, nv)                                 # bf16 [B*nv, C_e]
         h = ops.linear(h, self.encoder_to_decoder.weight, None, True).reshape(B, nv, -1)      # fp32 [B, nv, C_d]
-        pos = self.pos_embed[0].to(device=x.device, dtype=f32)                                # [N, C_d], no gradient
+        pos = _device_table(self, x.device)[0].to(dtype=f32)                                 # [N, C_d], no gradient
         pos_vis = pos[(vis[:, 1:] - 1).long()]                   # the visible tokens keep their order, the table follows it
         pos_msk = pos[(msk[:, 1:] - 1).long()]
         x_full = torch.cat([h + pos_vis, self.mask_token.float() + pos_msk], dim=1)           # :380-383
@@ -213,14 +226,23 @@ class PretrainVisionTransformer(nn.Module):
         return (out, msk[:, 1:] - 1) if return_indices else out
 
 
+_MEAN_STD = {}
+
+
+def _imagenet_mean_std(device):
+    """fp32 [3] ImageNet mean and std on `device`, made once per device (no host-to-device copy in a captured step)."""
+    if device not in _MEAN_STD:
+        _MEAN_STD[device] = tuple(torch.tensor(v, device=device, dtype=f32)
+                                  for v in (IMAGENET_DEFAULT_MEAN, IMAGENET_DEFAULT_STD))
+    return _MEAN_STD[device]
+
+
 def pixel_labels(images, masked_idx, patch_size, tubelet_size=2, normalize_target=True):
     """engine_for_pretraining.py:66-96 — targets of the masked tubelets: un-normalise the frames, cut (tubelet, p, p)
     tubelets, optionally normalise each tubelet per channel (unbiased variance, +1e-6).  fp32 [B, N_mask, tubelet*p*p*3]."""
     B, n_mask = masked_idx.shape
-    dev = images.device
-    mean3 = torch.tensor(IMAGENET_DEFAULT_MEAN, device=dev, dtype=f32)
-    std3 = torch.tensor(IMAGENET_DEFAULT_STD, device=dev, dtype=f32)
-    lab = ll.pixel_targets(images.to(bf16), masked_idx.to(torch.int32).contiguous().flatten(), n_mask, tubelet_size,
+    mean3, std3 = _imagenet_mean_std(images.device)
+    lab =ll.pixel_targets(images.to(bf16), masked_idx.to(torch.int32).contiguous().flatten(), n_mask, tubelet_size,
                            patch_size, bool(normalize_target), mean3, std3)
     return lab.reshape(B, n_mask, -1)
 
