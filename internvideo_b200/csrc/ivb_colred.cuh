@@ -6,7 +6,7 @@
 // runs of the same training step would disagree.  Instead every CTA stores its partial in a scratch slot
 //   g_colred[(out * nslots + slot) * D + col]
 // and colred_finish() adds the partials into the gradient in slot order: same inputs, same bits.
-// The scratch is static device memory of the including translation unit (24 MB in ivb_norm.cu, 16 MB in ivb_loss.cu).
+// The scratch is static device memory of the one translation unit that includes this header (24 MB in ivb_norm.cu).
 // It holds ONE reduction at a time per device: the entry points that use it must not run concurrently on two streams of
 // the same device (include/ivb200.h, Conventions).  A call whose partials would not fit returns an error.
 #pragma once
@@ -14,9 +14,7 @@
 
 namespace ivb {
 
-#ifndef IVB_COLRED_FLOATS
 #define IVB_COLRED_FLOATS (6L << 20)   // 24 MB: the largest bench user is the cfg-3 LayerScale / bias backward, ~4.2 M
-#endif
 
 static __device__ float g_colred[IVB_COLRED_FLOATS];
 

@@ -1,181 +1,16 @@
-// ivb_loss.cu — decoder heads' normalisation + alignment losses, contrastive loss, pixel targets,
-// and the flat AdamW step: HBM-bound kernels with warp-shuffle row reductions.
+// ivb_loss.cu — contrastive loss, L2 row normalisation, pixel targets + MSE, the flat AdamW step and single-query
+// attention pooling: HBM-bound kernels with warp-shuffle row reductions.  The decoder heads' LN -> L2 alignment loss
+// is in ivb_norm.cu.
 //
-//   LayerNorm -> L2-normalise   Linear_Decoder / MLP_Decoder.forward  internvideo2_pretrain.py:355-365,393-403
-//   (2 - 2 sum_c out*tgt).mean() engines/engine_for_pretraining.py:131-136
 //   video-text contrastive       InternVideo2/multi_modality/models/criterions.py:15-55,65-103,200-216
 //   pixel-reconstruction target  InternVideo1/Pretrain/VideoMAE/engine_for_pretraining.py:66-98 + MSE :43,106
 #include <math.h>
 
-#define IVB_COLRED_FLOATS (4L << 20)
-#include "ivb_colred.cuh"
 #include "ivb_internal.h"
 #include "ivb_ptx.cuh"
 #include "ivb_rows.cuh"
 
 namespace ivb {
-
-// ---------------------------------------------------------------- LayerNorm + L2 normalise
-// out = y / ||y||,  y = LN(z) * w + b.   stats[row] = {mean, rstd, 1/||y||}.
-// If tgt != nullptr also accumulates loss_sum += sum_rows (2 - 2 <out, tgt>)  (engine :131-136).
-template <bool TGT_F32>
-__global__ void __launch_bounds__(256)
-ln_l2_fwd_kernel(const __nv_bfloat16* __restrict__ z, long ldz, const __nv_bfloat16* __restrict__ w,
-                 const __nv_bfloat16* __restrict__ bsh, float eps, int M, int C,
-                 __nv_bfloat16* __restrict__ out, long ldo, float* __restrict__ stats,
-                 const void* __restrict__ tgt, long ldt, float* __restrict__ loss_sum) {
-  const int lane = threadIdx.x & 31;
-  const int wpb = blockDim.x >> 5;
-  const float invC = 1.f / C;
-  float loss_acc = 0.f;
-  for (long row = static_cast<long>(blockIdx.x) * wpb + (threadIdx.x >> 5); row < M;
-       row += static_cast<long>(gridDim.x) * wpb) {
-    const __nv_bfloat16* zr = z + row * ldz;
-    float s = 0.f;
-    for (int c = lane * 8; c < C; c += 256) { float v[8]; load8<false>(zr, c, v);
-#pragma unroll
-      for (int k = 0; k < 8; ++k) s += v[k]; }
-    const float mean = warp_sum(s) * invC;
-    float ss = 0.f;
-    for (int c = lane * 8; c < C; c += 256) { float v[8]; load8<false>(zr, c, v);
-#pragma unroll
-      for (int k = 0; k < 8; ++k) { const float d = v[k] - mean; ss += d * d; } }
-    const float rstd = rsqrtf(warp_sum(ss) * invC + eps);
-    float n2 = 0.f, dot = 0.f;
-    for (int c = lane * 8; c < C; c += 256) {
-      float v[8], wv[8], bv[8];
-      load8<false>(zr, c, v); load8<false>(w, c, wv); load8<false>(bsh, c, bv);
-      float t[8];
-      if (tgt) load8<TGT_F32>(tgt, row * ldt + c, t);
-#pragma unroll
-      for (int k = 0; k < 8; ++k) {
-        const float y = (v[k] - mean) * rstd * wv[k] + bv[k];
-        n2 += y * y;
-        if (tgt) dot += y * t[k];
-      }
-    }
-    n2 = warp_sum(n2);
-    const float inv_n = rsqrtf(n2);
-    if (tgt) { dot = warp_sum(dot); if (lane == 0) loss_acc += 2.f - 2.f * dot * inv_n; }
-    if (out) {
-      for (int c = lane * 8; c < C; c += 256) {
-        float v[8], wv[8], bv[8], o[8];
-        load8<false>(zr, c, v); load8<false>(w, c, wv); load8<false>(bsh, c, bv);
-#pragma unroll
-        for (int k = 0; k < 8; ++k) o[k] = ((v[k] - mean) * rstd * wv[k] + bv[k]) * inv_n;
-        store8<false>(out, row * ldo + c, o);
-      }
-    }
-    if (lane == 0 && stats) { stats[row * 3 + 0] = mean; stats[row * 3 + 1] = rstd; stats[row * 3 + 2] = inv_n; }
-  }
-  if (tgt && loss_sum) {
-    __shared__ float red[8];
-    if (lane == 0) red[threadIdx.x >> 5] = loss_acc;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      float t = 0.f;
-      for (int k = 0; k < wpb; ++k) t += red[k];
-      atomicAdd(loss_sum, t);
-    }
-  }
-}
-
-// LN -> L2 backward of 8 columns of a row (v = z, g = upstream gradient, col = first column):
-//   xh = (z - mean) * rstd, out = (xh*w + b) * inv_n, dy = inv_n * (g*gs - out*a) with a = <g*gs, out>,
-//   dz = rstd * (dy*w - s1 - xh*s2) with s1 = mean(dy*w), s2 = mean(dy*w*xh); dweight += dy*xh, dbias += dy.
-// The three sweeps over a row: ln_l2_dot8 sums a, ln_l2_sums8 sums s1 and s2, ln_l2_dz8 writes dz.
-struct LnL2Bwd {
-  const __nv_bfloat16* w;
-  const __nv_bfloat16* b;
-  float mean, rstd, inv_n, gs;
-};
-__device__ __forceinline__ void ln_l2_dot8(const LnL2Bwd& p, const float v[8], const float g[8], int col, float& a) {
-  float wv[8], bv[8];
-  load8<false>(p.w, col, wv); load8<false>(p.b, col, bv);
-#pragma unroll
-  for (int k = 0; k < 8; ++k) a += g[k] * p.gs * ((v[k] - p.mean) * p.rstd * wv[k] + bv[k]) * p.inv_n;
-}
-__device__ __forceinline__ void ln_l2_dy8(const LnL2Bwd& p, const float v[8], const float g[8], const float wv[8],
-                                          const float bv[8], float a, float dy[8], float xh[8]) {
-#pragma unroll
-  for (int k = 0; k < 8; ++k) {
-    xh[k] = (v[k] - p.mean) * p.rstd;
-    const float o = (xh[k] * wv[k] + bv[k]) * p.inv_n;
-    dy[k] = p.inv_n * (g[k] * p.gs - o * a);
-  }
-}
-__device__ __forceinline__ void ln_l2_sums8(const LnL2Bwd& p, const float v[8], const float g[8], int col, float a,
-                                            float& s1, float& s2) {
-  float wv[8], bv[8], dy[8], xh[8];
-  load8<false>(p.w, col, wv); load8<false>(p.b, col, bv);
-  ln_l2_dy8(p, v, g, wv, bv, a, dy, xh);
-#pragma unroll
-  for (int k = 0; k < 8; ++k) {
-    s1 += dy[k] * wv[k];
-    s2 += dy[k] * wv[k] * xh[k];
-  }
-}
-// acc: the warp's colred rows [2][C] offset by col, or null when no parameter gradient is wanted
-__device__ __forceinline__ void ln_l2_dz8(const LnL2Bwd& p, const float v[8], const float g[8], int col, float a,
-                                          float s1, float s2, __nv_bfloat16* dz, long dz_off, float* acc, int C) {
-  float wv[8], bv[8], dy[8], xh[8], o[8];
-  load8<false>(p.w, col, wv); load8<false>(p.b, col, bv);
-  ln_l2_dy8(p, v, g, wv, bv, a, dy, xh);
-#pragma unroll
-  for (int k = 0; k < 8; ++k) o[k] = p.rstd * (dy[k] * wv[k] - s1 - xh[k] * s2);
-  store8<false>(dz, dz_off, o);
-  if (acc != nullptr) {
-    colred_add<8>(acc, dy, xh);
-    colred_add<8>(acc + C, dy);
-  }
-}
-
-// d_out = gscale * dout_tensor  (dout_tensor is the upstream gradient, or the TARGET itself when the
-// loss is (2-2<out,tgt>).mean(): then gscale = -2 * g / rows).  Computes dz (bf16), dw, db (fp32, accumulated in a fixed order).
-// dynamic smem: colred rows [warps][2][C]
-template <bool DO_F32>
-__global__ void __launch_bounds__(256)
-ln_l2_bwd_kernel(const __nv_bfloat16* __restrict__ z, long ldz, const __nv_bfloat16* __restrict__ w,
-                 const __nv_bfloat16* __restrict__ bsh, const float* __restrict__ stats, int M, int C,
-                 const void* __restrict__ dout, long lddo, float gscale_host,
-                 const float* __restrict__ gscale_dev, __nv_bfloat16* __restrict__ dz, long lddz,
-                 float* __restrict__ dw, float* __restrict__ db) {
-  extern __shared__ float acc_smem[];
-  const int lane = threadIdx.x & 31;
-  const int warp = threadIdx.x >> 5;
-  const int wpb = blockDim.x >> 5;
-  const float invC = 1.f / C;
-  const float gs = gscale_host * (gscale_dev ? *gscale_dev : 1.f);
-  const bool want = dw != nullptr;
-  float* acc = want ? colred_zero(acc_smem, 2, C) : nullptr;
-  for (long row = static_cast<long>(blockIdx.x) * wpb + warp; row < M; row += static_cast<long>(gridDim.x) * wpb) {
-    const __nv_bfloat16* zr = z + row * ldz;
-    const LnL2Bwd p{w, bsh, stats[row * 3], stats[row * 3 + 1], stats[row * 3 + 2], gs};
-    float a = 0.f;
-    for (int c = lane * 8; c < C; c += 256) {
-      float v[8], g[8];
-      load8<false>(zr, c, v); load8<DO_F32>(dout, row * lddo + c, g);
-      ln_l2_dot8(p, v, g, c, a);
-    }
-    a = warp_sum(a);
-    float s1 = 0.f, s2 = 0.f;
-    for (int c = lane * 8; c < C; c += 256) {
-      float v[8], g[8];
-      load8<false>(zr, c, v); load8<DO_F32>(dout, row * lddo + c, g);
-      ln_l2_sums8(p, v, g, c, a, s1, s2);
-    }
-    s1 = warp_sum(s1) * invC; s2 = warp_sum(s2) * invC;
-    for (int c = lane * 8; c < C; c += 256) {
-      float v[8], g[8];
-      load8<false>(zr, c, v); load8<DO_F32>(dout, row * lddo + c, g);
-      ln_l2_dz8(p, v, g, c, a, s1, s2, dz, row * lddz + c, want ? acc + c : nullptr, C);
-    }
-  }
-  if (want) {
-    __syncthreads();
-    colred_flush<2>(acc_smem, wpb, C, db ? 3u : 1u);
-  }
-}
 
 // ---------------------------------------------------------------- flat AdamW (fp32 master, bf16 model copy)
 template <bool G_F32>
@@ -422,75 +257,6 @@ __global__ void pixel_target_kernel(const __nv_bfloat16* __restrict__ video, con
   for (int i = lane; i < npix; i += 32) out[static_cast<long>(i) * C + c] = ((pixel(i) - pivot) - mean) * inv;
 }
 
-// Register-resident backward (C <= 256*NCH, bf16 upstream gradient / target): z and dout rows read once, all loads
-// in flight together, the three sweeps run over registers (210 us vs 247 us for the streaming kernel at C = 3200;
-// the same treatment of the FORWARD was slower — see ivb_ln_l2_fwd — and is not kept).
-// dynamic smem: colred rows [warps][2][C]
-template <int NCH>
-__global__ void __launch_bounds__(128, 2)
-ln_l2_bwd_reg_kernel(const __nv_bfloat16* __restrict__ z, long ldz, const __nv_bfloat16* __restrict__ w,
-                     const __nv_bfloat16* __restrict__ bsh, const float* __restrict__ stats, int M, int C,
-                     const __nv_bfloat16* __restrict__ dout, long lddo, float gscale_host,
-                     const float* __restrict__ gscale_dev, __nv_bfloat16* __restrict__ dz, long lddz,
-                     float* __restrict__ dw, float* __restrict__ db) {
-  extern __shared__ float acc_smem[];
-  const int lane = threadIdx.x & 31;
-  const int warp = threadIdx.x >> 5;
-  const int wpb = blockDim.x >> 5;
-  const int nch = C >> 3;
-  const float invC = 1.f / C;
-  const float gs = gscale_host * (gscale_dev ? *gscale_dev : 1.f);
-  const bool want = dw != nullptr;
-  float* acc = want ? colred_zero(acc_smem, 2, C) : nullptr;
-  for (long row = static_cast<long>(blockIdx.x) * wpb + warp; row < M; row += static_cast<long>(gridDim.x) * wpb) {
-    uint4 zq[NCH], gq[NCH];
-#pragma unroll
-    for (int i = 0; i < NCH; ++i) {
-      const int c = lane + 32 * i;
-      if (c < nch) {
-        zq[i] = *reinterpret_cast<const uint4*>(z + row * ldz + c * 8);
-        gq[i] = *reinterpret_cast<const uint4*>(dout + row * lddo + c * 8);
-      }
-    }
-    const LnL2Bwd p{w, bsh, stats[row * 3], stats[row * 3 + 1], stats[row * 3 + 2], gs};
-    float a = 0.f;
-#pragma unroll
-    for (int i = 0; i < NCH; ++i) {
-      const int c = lane + 32 * i;
-      if (c < nch) {
-        float v[8], g[8];
-        unpack8(zq[i], v); unpack8(gq[i], g);
-        ln_l2_dot8(p, v, g, c * 8, a);
-      }
-    }
-    a = warp_sum(a);
-    float s1 = 0.f, s2 = 0.f;
-#pragma unroll
-    for (int i = 0; i < NCH; ++i) {
-      const int c = lane + 32 * i;
-      if (c < nch) {
-        float v[8], g[8];
-        unpack8(zq[i], v); unpack8(gq[i], g);
-        ln_l2_sums8(p, v, g, c * 8, a, s1, s2);
-      }
-    }
-    s1 = warp_sum(s1) * invC; s2 = warp_sum(s2) * invC;
-#pragma unroll
-    for (int i = 0; i < NCH; ++i) {
-      const int c = lane + 32 * i;
-      if (c < nch) {
-        float v[8], g[8];
-        unpack8(zq[i], v); unpack8(gq[i], g);
-        ln_l2_dz8(p, v, g, c * 8, a, s1, s2, dz, row * lddz + c * 8, want ? acc + c * 8 : nullptr, C);
-      }
-    }
-  }
-  if (want) {
-    __syncthreads();
-    colred_flush<2>(acc_smem, wpb, C, db ? 3u : 1u);
-  }
-}
-
 // loss_sum += sum (pred - label)^2 ; dpred(bf16) = gscale * 2 (pred - label) (optional)
 __global__ void __launch_bounds__(256)
 mse_kernel(const __nv_bfloat16* __restrict__ pred, const float* __restrict__ label, long n,
@@ -513,80 +279,6 @@ mse_kernel(const __nv_bfloat16* __restrict__ pred, const float* __restrict__ lab
 }  // namespace ivb
 
 using namespace ivb;
-
-extern "C" int ivb_ln_l2_fwd(const void* z, long ldz, const void* weight, const void* bias, float eps,
-                             int M, int C, void* out, long ldo, float* stats, const void* target,
-                             int target_is_f32, long ldt, float* loss_sum, void* stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  if (M <= 0) return 0;
-  if ((C & 7) || (ldz & 7) || (ldo & 7) || (ldt & 7)) return set_error("ivb_ln_l2_fwd: C/ld must be multiples of 8");
-  if (misaligned(16, z, weight, bias, out, target))
-    return set_error("ivb_ln_l2_fwd: z, weight, bias, out and target must be 16-byte aligned");
-  const int blocks = persistent_grid(M, 8, 8);
-  auto zz = reinterpret_cast<const __nv_bfloat16*>(z);
-  auto ww = reinterpret_cast<const __nv_bfloat16*>(weight);
-  auto bb = reinterpret_cast<const __nv_bfloat16*>(bias);
-  auto oo = reinterpret_cast<__nv_bfloat16*>(out);
-  return launch("ln_l2_fwd_kernel", target_is_f32 ? ln_l2_fwd_kernel<true> : ln_l2_fwd_kernel<false>, blocks, 256, 0,
-                stream, NO_PDL, zz, ldz, ww, bb, eps, M, C, oo, ldo, stats, target, ldt, loss_sum);
-}
-
-template <bool DO_F32>
-static int launch_ln_l2_bwd(const void* z, long ldz, const void* weight, const void* bias,
-                            const float* stats, int M, int C, const void* dout, long lddo, float gh,
-                            const float* gd, void* dz, long lddz, float* dw, float* db, cudaStream_t stream) {
-  int wpb = 8;
-  size_t smem = dw ? static_cast<size_t>(2) * wpb * C * sizeof(float) : 0;
-  while (smem > 200 * 1024 && wpb > 1) { wpb /= 2; smem /= 2; }
-  if (smem > 48 * 1024)
-    if (int rc = raise_smem_limit<ln_l2_bwd_kernel<DO_F32>>(220 * 1024, "cudaFuncSetAttribute(ln_l2_bwd)")) return rc;
-  const int blocks = persistent_grid(M, wpb * 2, smem > 96 * 1024 ? 2 : 4);
-  if (colred_check(2, blocks, C, "ln_l2_bwd: gradient scratch too small")) return 1;
-  if (int rc = launch("ln_l2_bwd_kernel", ln_l2_bwd_kernel<DO_F32>, blocks, wpb * 32, smem, stream, NO_PDL,
-                      reinterpret_cast<const __nv_bfloat16*>(z), ldz, reinterpret_cast<const __nv_bfloat16*>(weight),
-                      reinterpret_cast<const __nv_bfloat16*>(bias), stats, M, C, dout, lddo, gh, gd,
-                      reinterpret_cast<__nv_bfloat16*>(dz), lddz, dw, db))
-    return rc;
-  return dw ? colred_finish(2, blocks, C, dw, db, nullptr, stream) : 0;
-}
-
-template <int NCH>
-static int launch_ln_l2_bwd_reg(const void* z, long ldz, const void* weight, const void* bias,
-                                const float* stats, int M, int C, const void* dout, long lddo, float gh,
-                                const float* gd, void* dz, long lddz, float* dw, float* db, cudaStream_t stream) {
-  const int wpb = 4;
-  const size_t smem = dw ? static_cast<size_t>(2) * wpb * C * sizeof(float) : 0;   // <= 104 KB at C = 3200: 2 CTAs/SM
-  if (smem > 48 * 1024)
-    if (int rc = raise_smem_limit<ln_l2_bwd_reg_kernel<NCH>>(110 * 1024, "cudaFuncSetAttribute(ln_l2_bwd_reg)")) return rc;
-  const int blocks = persistent_grid(M, wpb * 2, 2);
-  if (colred_check(2, blocks, C, "ln_l2_bwd: gradient scratch too small")) return 1;
-  if (int rc = launch("ln_l2_bwd_reg_kernel", ln_l2_bwd_reg_kernel<NCH>, blocks, wpb * 32, smem, stream, NO_PDL,
-                      reinterpret_cast<const __nv_bfloat16*>(z), ldz, reinterpret_cast<const __nv_bfloat16*>(weight),
-                      reinterpret_cast<const __nv_bfloat16*>(bias), stats, M, C,
-                      reinterpret_cast<const __nv_bfloat16*>(dout), lddo, gh, gd, reinterpret_cast<__nv_bfloat16*>(dz),
-                      lddz, dw, db))
-    return rc;
-  return dw ? colred_finish(2, blocks, C, dw, db, nullptr, stream) : 0;
-}
-
-extern "C" int ivb_ln_l2_bwd(const void* z, long ldz, const void* weight, const void* bias,
-                             const float* stats, int M, int C, const void* dout, int dout_is_f32,
-                             long lddo, float gscale_host, const float* gscale_dev, void* dz, long lddz,
-                             float* dweight, float* dbias, void* stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  if (M <= 0) return 0;
-  if ((C & 7) || (ldz & 7) || (lddz & 7) || (lddo & 7)) return set_error("ivb_ln_l2_bwd: C/ld must be multiples of 8");
-  if (misaligned(16, z, weight, bias, dout, dz))
-    return set_error("ivb_ln_l2_bwd: z, weight, bias, dout and dz must be 16-byte aligned");
-  if (!dout_is_f32 && C <= 256 * 13) {
-    const int nchunks = (C + 255) / 256;
-    if (nchunks <= 3) return launch_ln_l2_bwd_reg<3>(z, ldz, weight, bias, stats, M, C, dout, lddo, gscale_host, gscale_dev, dz, lddz, dweight, dbias, stream);
-    if (nchunks <= 6) return launch_ln_l2_bwd_reg<6>(z, ldz, weight, bias, stats, M, C, dout, lddo, gscale_host, gscale_dev, dz, lddz, dweight, dbias, stream);
-    return launch_ln_l2_bwd_reg<13>(z, ldz, weight, bias, stats, M, C, dout, lddo, gscale_host, gscale_dev, dz, lddz, dweight, dbias, stream);
-  }
-  if (dout_is_f32) return launch_ln_l2_bwd<true>(z, ldz, weight, bias, stats, M, C, dout, lddo, gscale_host, gscale_dev, dz, lddz, dweight, dbias, stream);
-  return launch_ln_l2_bwd<false>(z, ldz, weight, bias, stats, M, C, dout, lddo, gscale_host, gscale_dev, dz, lddz, dweight, dbias, stream);
-}
 
 extern "C" int ivb_adamw_step(float* master, float* exp_avg, float* exp_avg_sq, const void* grad,
                               int grad_is_f32, void* param_bf16, long n, float lr, float beta1,

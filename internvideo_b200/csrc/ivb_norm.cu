@@ -4,12 +4,17 @@
 //                                             nn.LayerNorm of the pooling block / decoders :525,:532)
 //   LayerScale backward                      (internvideo2_pretrain.py:131-146)
 //   bias-gradient column sums
+//   decoder head: LayerNorm -> L2-normalise  (Linear_Decoder / MLP_Decoder.forward internvideo2_pretrain.py:355-365,
+//                 and the (2 - 2 <out, tgt>).mean() loss   393-403; engines/engine_for_pretraining.py:131-136)
 // One warp per row, 16-byte vector loads, warp-shuffle reductions; parameter gradients are
 // accumulated per warp in shared memory, stored as one partial per column per CTA and summed in a fixed
 // order by colred_finish (ivb_colred.cuh).
 // The forward has two kernels: norm_fwd_kernel streams the row (LayerNorm, and RMSNorm above D = 1536, to bf16), and
 // norm_rows_kernel holds it in registers and writes it as bf16 (RMSNorm, the q/k pair), as E4M3 with a per-row
 // scale (FP8 inference), or as both (FP8 training), all launched by launch_norm_fwd.
+// The backward has two kernels too, norm_bwd_kernel (streamed) and norm_bwd_rows_kernel (held in registers), both
+// launched by launch_norm_bwd; each also runs the decoder head's LN -> L2 backward, a LayerNorm backward whose dy is
+// formed from the upstream gradient.
 #include <stdio.h>
 #include <stdlib.h>
 #include <type_traits>
@@ -78,6 +83,71 @@ norm_fwd_kernel(const void* __restrict__ x, long ldx, const __nv_bfloat16* __res
   }
 }
 
+// ------------------------------------------------------------------ decoder head: LayerNorm + L2 normalise
+// out = y / ||y||,  y = LN(z) * w + b.   stats[row] = {mean, rstd, 1/||y||}.
+// If tgt != nullptr also accumulates loss_sum += sum_rows (2 - 2 <out, tgt>)  (engine :131-136).
+template <bool TGT_F32>
+__global__ void __launch_bounds__(256)
+ln_l2_fwd_kernel(const __nv_bfloat16* __restrict__ z, long ldz, const __nv_bfloat16* __restrict__ w,
+                 const __nv_bfloat16* __restrict__ bsh, float eps, int M, int C,
+                 __nv_bfloat16* __restrict__ out, long ldo, float* __restrict__ stats,
+                 const void* __restrict__ tgt, long ldt, float* __restrict__ loss_sum) {
+  const int lane = threadIdx.x & 31;
+  const int wpb = blockDim.x >> 5;
+  const float invC = 1.f / C;
+  float loss_acc = 0.f;
+  for (long row = static_cast<long>(blockIdx.x) * wpb + (threadIdx.x >> 5); row < M;
+       row += static_cast<long>(gridDim.x) * wpb) {
+    const __nv_bfloat16* zr = z + row * ldz;
+    float s = 0.f;
+    for (int c = lane * 8; c < C; c += 256) { float v[8]; load8<false>(zr, c, v);
+#pragma unroll
+      for (int k = 0; k < 8; ++k) s += v[k]; }
+    const float mean = warp_sum(s) * invC;
+    float ss = 0.f;
+    for (int c = lane * 8; c < C; c += 256) { float v[8]; load8<false>(zr, c, v);
+#pragma unroll
+      for (int k = 0; k < 8; ++k) { const float d = v[k] - mean; ss += d * d; } }
+    const float rstd = rsqrtf(warp_sum(ss) * invC + eps);
+    float n2 = 0.f, dot = 0.f;
+    for (int c = lane * 8; c < C; c += 256) {
+      float v[8], wv[8], bv[8];
+      load8<false>(zr, c, v); load8<false>(w, c, wv); load8<false>(bsh, c, bv);
+      float t[8];
+      if (tgt) load8<TGT_F32>(tgt, row * ldt + c, t);
+#pragma unroll
+      for (int k = 0; k < 8; ++k) {
+        const float y = (v[k] - mean) * rstd * wv[k] + bv[k];
+        n2 += y * y;
+        if (tgt) dot += y * t[k];
+      }
+    }
+    n2 = warp_sum(n2);
+    const float inv_n = rsqrtf(n2);
+    if (tgt) { dot = warp_sum(dot); if (lane == 0) loss_acc += 2.f - 2.f * dot * inv_n; }
+    if (out) {
+      for (int c = lane * 8; c < C; c += 256) {
+        float v[8], wv[8], bv[8], o[8];
+        load8<false>(zr, c, v); load8<false>(w, c, wv); load8<false>(bsh, c, bv);
+#pragma unroll
+        for (int k = 0; k < 8; ++k) o[k] = ((v[k] - mean) * rstd * wv[k] + bv[k]) * inv_n;
+        store8<false>(out, row * ldo + c, o);
+      }
+    }
+    if (lane == 0 && stats) { stats[row * 3 + 0] = mean; stats[row * 3 + 1] = rstd; stats[row * 3 + 2] = inv_n; }
+  }
+  if (tgt && loss_sum) {
+    __shared__ float red[8];
+    if (lane == 0) red[threadIdx.x >> 5] = loss_acc;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      float t = 0.f;
+      for (int k = 0; k < wpb; ++k) t += red[k];
+      atomicAdd(loss_sum, t);
+    }
+  }
+}
+
 // ------------------------------------------------------------------ backward
 // RMSNorm (LN = false: mean = 0, s1 = 0) / LayerNorm backward of 8 columns of a row; g = dy, xh = normalised x.
 // Sweep 1: s1 += g*w, s2 += g*w*xh.
@@ -114,52 +184,115 @@ __device__ __forceinline__ void norm_bwd_dx8(const float g[8], const float wv[8]
   }
 }
 
+// The decoder head's LN -> L2 backward (the L2 forms) is the LayerNorm backward of dy = inv_n * (g*gs - out*a), where
+// out = (xh*w + b) * inv_n is the forward's output, g*gs the gradient reaching it and a = <g*gs, out> over the row:
+// ln_l2_dot8 sums a over 8 columns (v = z), and ln_l2_dy8 turns g into dy and sets xh = (z - mean) * rstd.
+__device__ __forceinline__ void ln_l2_dot8(const float v[8], const float g[8], const float wv[8], const float bv[8],
+                                           float mean, float rstd, float inv_n, float gs, float& a) {
+#pragma unroll
+  for (int k = 0; k < 8; ++k) a += g[k] * gs * ((v[k] - mean) * rstd * wv[k] + bv[k]) * inv_n;
+}
+__device__ __forceinline__ void ln_l2_dy8(const float v[8], float g[8], const float wv[8], const float bv[8], float mean,
+                                          float rstd, float inv_n, float gs, float a, float xh[8]) {
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    xh[k] = (v[k] - mean) * rstd;
+    const float o = (xh[k] * wv[k] + bv[k]) * inv_n;
+    g[k] = inv_n * (g[k] * gs - o * a);
+  }
+}
+
+// dy and dx_out of the norm forms may be one buffer (the in-place q-norm backward); the LN -> L2 gradient and dz never
+// alias, and are declared so.
+template <bool NOALIAS>
+using GradIn = std::conditional_t<NOALIAS, const __nv_bfloat16* __restrict__, const __nv_bfloat16*>;
+template <bool NOALIAS> using GradOut = std::conditional_t<NOALIAS, void* __restrict__, void*>;
+
 // dynamic smem: colred rows [warps][LN ? 2 : 1][D]
-template <bool XF32, bool LN, bool DXF32>
+// L2 (LN, bf16 x = z and dx, no dx_in): dy is the upstream gradient g, fp32 with GF32, scaled by gscale_host *
+// *gscale_dev; mean_in is the forward's stats[M][3] = {mean, rstd, inv_n}, and rstd_in is not read.
+template <bool XF32, bool LN, bool DXF32, bool L2, bool GF32>
 __global__ void __launch_bounds__(256)
-norm_bwd_kernel(const __nv_bfloat16* dy, long lddy, const void* __restrict__ x, long ldx,
-                const __nv_bfloat16* __restrict__ w, const float* __restrict__ mean_in,
-                const float* __restrict__ rstd_in, int M, int D, const float* __restrict__ dx_in,
-                long lddx_in, void* dx_out, long lddx, float* __restrict__ dweight,
-                float* __restrict__ dbias) {
-  pdl_wait();
-  pdl_launch_dependents();
+norm_bwd_kernel(GradIn<L2> dy, long lddy, const void* __restrict__ x, long ldx, const __nv_bfloat16* __restrict__ w,
+                const __nv_bfloat16* __restrict__ b, const float* __restrict__ mean_in,
+                const float* __restrict__ rstd_in, int M, int D, const float* __restrict__ dx_in, long lddx_in,
+                GradOut<L2> dx_out, long lddx, float* __restrict__ dweight, float* __restrict__ dbias, float gscale_host,
+                const float* __restrict__ gscale_dev) {
+  if constexpr (!L2) {   // the L2 forms are launched without PDL
+    pdl_wait();
+    pdl_launch_dependents();
+  }
   extern __shared__ float acc_smem[];
   const int lane = threadIdx.x & 31;
   const int warp = threadIdx.x >> 5;
   const int warps_per_block = blockDim.x >> 5;
   const int nch = D >> 3;
   const float invD = 1.0f / static_cast<float>(D);
+  const float gs = L2 ? gscale_host * (gscale_dev ? *gscale_dev : 1.f) : 1.f;
   const bool want_dw = dweight != nullptr;
   float* acc = want_dw ? colred_zero(acc_smem, LN ? 2 : 1, D) : nullptr;
   for (long row = (long)blockIdx.x * warps_per_block + warp; row < M;
        row += (long)gridDim.x * warps_per_block) {
     const long xo = row * ldx;
     const long go = row * lddy;
-    const float rstd = rstd_in[row];
-    const float mean = LN ? mean_in[row] : 0.f;
-    float s1 = 0.f, s2 = 0.f;  // sum g, sum g*xhat
-    for (int c = lane; c < nch; c += 32) {
-      float v[8], g[8], wv[8], xh[8];
-      load8<XF32>(x, xo + c * 8, v);
-      load8<false>(dy, go + c * 8, g);
-      load8<false>(w, c * 8, wv);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) xh[j] = (v[j] - mean) * rstd;
-      norm_bwd_sums8<LN>(g, wv, xh, s1, s2);
+    float mean = 0.f, rstd, inv_n = 0.f;
+    if constexpr (L2) {
+      mean = mean_in[row * 3]; rstd = mean_in[row * 3 + 1]; inv_n = mean_in[row * 3 + 2];
+    } else {
+      rstd = rstd_in[row];
+      if (LN) mean = mean_in[row];
     }
+    // f(c) for the row's 8-column chunks c = lane, lane + 32, ... in order.  The L2 forms count the loop in columns:
+    // counted in chunks, the bf16 form takes 64 registers instead of 48, and counted in columns, the norm forms' code
+    // changes.
+    auto each_chunk = [&](auto f) {
+      if constexpr (L2) {
+        for (int col = lane * 8; col < D; col += 256) f(col >> 3);
+      } else {
+        for (int c = lane; c < nch; c += 32) f(c);
+      }
+    };
+    float a = 0.f;
+    if (L2) {
+      each_chunk([&](int c) {
+        float v[8], g[8], wv[8], bv[8];
+        load8<XF32>(x, xo + c * 8, v);
+        load8<GF32>(dy, go + c * 8, g);
+        load8<false>(w, c * 8, wv);
+        load8<false>(b, c * 8, bv);
+        ln_l2_dot8(v, g, wv, bv, mean, rstd, inv_n, gs, a);
+      });
+      a = warp_sum(a);
+    }
+    // chunk c's dy, weights and normalised x, for each of the two sweeps
+    auto chunk = [&](int c, float g[8], float wv[8], float xh[8]) {
+      float v[8];
+      load8<XF32>(x, xo + c * 8, v);
+      load8<GF32>(dy, go + c * 8, g);
+      load8<false>(w, c * 8, wv);
+      if (L2) {
+        float bv[8];
+        load8<false>(b, c * 8, bv);
+        ln_l2_dy8(v, g, wv, bv, mean, rstd, inv_n, gs, a, xh);
+      } else {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) xh[j] = (v[j] - mean) * rstd;
+      }
+    };
+    float s1 = 0.f, s2 = 0.f;  // sum dy*w, sum dy*w*xhat
+    each_chunk([&](int c) {
+      float g[8], wv[8], xh[8];
+      chunk(c, g, wv, xh);
+      norm_bwd_sums8<LN>(g, wv, xh, s1, s2);
+    });
     s1 = LN ? warp_sum(s1) * invD : 0.f;
     s2 = warp_sum(s2) * invD;
-    for (int c = lane; c < nch; c += 32) {
-      float v[8], g[8], wv[8], xh[8];
-      load8<XF32>(x, xo + c * 8, v);
-      load8<false>(dy, go + c * 8, g);
-      load8<false>(w, c * 8, wv);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) xh[j] = (v[j] - mean) * rstd;
-      norm_bwd_dx8<LN, DXF32>(g, wv, xh, rstd, s1, s2, dx_in, row * lddx_in + c * 8, dx_out, row * lddx + c * 8,
-                              want_dw ? acc + c * 8 : nullptr, D);
-    }
+    each_chunk([&](int c) {
+      float g[8], wv[8], xh[8];
+      chunk(c, g, wv, xh);
+      norm_bwd_dx8<LN, DXF32>(g, wv, xh, rstd, s1, s2, L2 ? nullptr : dx_in, row * lddx_in + c * 8, dx_out,
+                              row * lddx + c * 8, want_dw ? acc + c * 8 : nullptr, D);
+    });
   }
   if (want_dw) {
     __syncthreads();
@@ -379,26 +512,37 @@ norm_rows_kernel(const void* __restrict__ x, long ldx, const __nv_bfloat16* __re
   }
 }
 
-// dynamic smem: colred rows [warps][1][D] (only when dweight != nullptr)
-// Registers: the normalised row in fp32 (8*NCH) + dy as the raw packed bf16 it was loaded as (4*NCH);
-// keeping dy*w in fp32 as well pushed the kernel to 150 registers / 1 CTA per SM and made it 2x slower.
-template <bool XF32, bool DXF32, int NCH, bool PAIR>
-__global__ void __launch_bounds__(256, 2)
-rms_bwd_reg_kernel(const __nv_bfloat16* dy, long lddy, const void* __restrict__ x, long ldx,
-                   const __nv_bfloat16* __restrict__ w, const float* __restrict__ rstd_in, int M, int D,
-                   const float* __restrict__ dx_in, long lddx_in, void* dx_out, long lddx,
-                   float* __restrict__ dweight, const __nv_bfloat16* __restrict__ w1,
-                   float* __restrict__ dweight1, long x_pair_off, long dy_pair_off, long dx_pair_off) {
-  pdl_wait();
-  pdl_launch_dependents();
+// The backward over rows held in registers (D <= 256*NCH): RMSNorm, the q/k pair and, with L2, the LN -> L2 backward
+// (operands as in norm_bwd_kernel).  Each row is read from HBM once, all its loads in flight together.
+// dynamic smem: colred rows [warps][L2 ? 2 : 1][D] (only when dweight != nullptr)
+// PAIR: virtual row r covers token r>>1, part r&1; part p reads and writes at column offset p*pair_off of its token's
+// rows and uses weight w / w1; its weight gradient is the pair's second colred output.
+template <bool XF32, bool DXF32, int NCH, bool PAIR, bool L2>
+__global__ void __launch_bounds__(L2 ? 128 : 256, 2)
+norm_bwd_rows_kernel(GradIn<L2> dy, long lddy, const void* __restrict__ x, long ldx, const __nv_bfloat16* __restrict__ w,
+                     const __nv_bfloat16* __restrict__ b, const float* __restrict__ mean_in,
+                     const float* __restrict__ rstd_in, int M, int D, const float* __restrict__ dx_in, long lddx_in,
+                     GradOut<L2> dx_out, long lddx, float* __restrict__ dweight, float* __restrict__ dbias, float gscale_host,
+                     const float* __restrict__ gscale_dev, const __nv_bfloat16* __restrict__ w1, long x_pair_off,
+                     long dy_pair_off, long dx_pair_off) {
+  // What a row is held as.  RMSNorm and the pair hold the normalised row in fp32 (8*NCH registers) and dy as the raw
+  // packed bf16 it was loaded as (4*NCH): keeping dy*w in fp32 as well pushed the kernel to 150 registers / 1 CTA per
+  // SM and made it 2x slower.  LN -> L2 holds z and g packed and forms xh and dy again in each sweep: its 13-chunk rows
+  // at C = 3200 do not fit in registers as fp32.
+  constexpr bool kHoldXh = !L2;
+  if constexpr (!L2) {   // the L2 form is launched without PDL
+    pdl_wait();
+    pdl_launch_dependents();
+  }
   extern __shared__ float acc_smem[];
   const int lane = threadIdx.x & 31;
   const int warp = threadIdx.x >> 5;
   const int wpb = blockDim.x >> 5;
   const int nch = D >> 3;
   const float invD = 1.0f / static_cast<float>(D);
+  const float gs = L2 ? gscale_host * (gscale_dev ? *gscale_dev : 1.f) : 1.f;
   const bool want_dw = dweight != nullptr;
-  float* acc = want_dw ? colred_zero(acc_smem, 1, D) : nullptr;
+  float* acc = want_dw ? colred_zero(acc_smem, L2 ? 2 : 1, D) : nullptr;
   // PAIR: the virtual-row stride gridDim.x * wpb is even (wpb = 8), so a warp only ever sees ONE part
   // (row parity == warp parity): its accumulator belongs to that part's weight gradient.
   for (long row = (long)blockIdx.x * wpb + warp; row < M; row += (long)gridDim.x * wpb) {
@@ -408,46 +552,81 @@ rms_bwd_reg_kernel(const __nv_bfloat16* dy, long lddy, const void* __restrict__ 
     const long go = tok * lddy + part * dy_pair_off;
     const long oo = tok * lddx + part * dx_pair_off;
     const __nv_bfloat16* wp = (PAIR && part) ? w1 : w;
-    const float rstd = rstd_in[row];
-    float xh[NCH][8];
-    uint4 gq[NCH];
-    float s1 = 0.f, s2 = 0.f;  // s1 stays 0 (RMSNorm)
+    float mean = 0.f, rstd = L2 ? 0.f : rstd_in[row], inv_n = 0.f;   // L2: read after the row is in flight
+    float xh[kHoldXh ? NCH : 1][8];
+    uint4 zq[kHoldXh ? 1 : NCH], gq[NCH];
 #pragma unroll
     for (int i = 0; i < NCH; ++i) {
       const int c = lane + 32 * i;
       if (c < nch) {
-        load8<XF32>(x, xo + c * 8, xh[i]);
+        if constexpr (kHoldXh) load8<XF32>(x, xo + c * 8, xh[i]);
+        else zq[i] = *reinterpret_cast<const uint4*>(reinterpret_cast<const __nv_bfloat16*>(x) + xo + c * 8);
         gq[i] = *reinterpret_cast<const uint4*>(dy + go + c * 8);
       }
     }
+    float a = 0.f;
+    if constexpr (L2) {
+      mean = mean_in[row * 3]; rstd = mean_in[row * 3 + 1]; inv_n = mean_in[row * 3 + 2];
 #pragma unroll
-    for (int i = 0; i < NCH; ++i) {
+      for (int i = 0; i < NCH; ++i) {
+        const int c = lane + 32 * i;
+        if (c < nch) {
+          float v[8], g[8], wv[8], bv[8];
+          unpack8(zq[i], v);
+          unpack8(gq[i], g);
+          load8<false>(w, c * 8, wv);
+          load8<false>(b, c * 8, bv);
+          ln_l2_dot8(v, g, wv, bv, mean, rstd, inv_n, gs, a);
+        }
+      }
+      a = warp_sum(a);
+    }
+    // chunk i's dy and weights; returns its normalised x, held or formed in xl
+    auto chunk = [&](int i, float g[8], float wv[8], float xl[8]) -> const float* {
       const int c = lane + 32 * i;
-      if (c < nch) {
-        float wv[8], g[8];
+      if constexpr (kHoldXh) {
         load8<false>(wp, c * 8, wv);
         unpack8(gq[i], g);
+        return xh[i];
+      } else {
+        float v[8], bv[8];
+        unpack8(zq[i], v);
+        unpack8(gq[i], g);
+        load8<false>(w, c * 8, wv);
+        load8<false>(b, c * 8, bv);
+        ln_l2_dy8(v, g, wv, bv, mean, rstd, inv_n, gs, a, xl);
+        return xl;
+      }
+    };
+    float s1 = 0.f, s2 = 0.f;  // s1 stays 0 (RMSNorm)
 #pragma unroll
-        for (int j = 0; j < 8; ++j) xh[i][j] *= rstd;
-        norm_bwd_sums8<false>(g, wv, xh[i], s1, s2);
+    for (int i = 0; i < NCH; ++i) {
+      if (lane + 32 * i < nch) {
+        float g[8], wv[8], xl[8];
+        const float* xhi = chunk(i, g, wv, xl);
+        if constexpr (kHoldXh) {
+#pragma unroll
+          for (int j = 0; j < 8; ++j) xh[i][j] *= rstd;
+        }
+        norm_bwd_sums8<L2>(g, wv, xhi, s1, s2);
       }
     }
+    s1 = L2 ? warp_sum(s1) * invD : 0.f;
     s2 = warp_sum(s2) * invD;
 #pragma unroll
     for (int i = 0; i < NCH; ++i) {
       const int c = lane + 32 * i;
       if (c < nch) {
-        float wv[8], g[8];
-        load8<false>(wp, c * 8, wv);
-        unpack8(gq[i], g);
-        norm_bwd_dx8<false, DXF32>(g, wv, xh[i], rstd, s1, s2, dx_in, row * lddx_in + c * 8, dx_out, oo + c * 8,
-                                   want_dw ? acc + c * 8 : nullptr, D);
+        float g[8], wv[8], xl[8];
+        const float* xhi = chunk(i, g, wv, xl);
+        norm_bwd_dx8<L2, DXF32>(g, wv, xhi, rstd, s1, s2, L2 ? nullptr : dx_in, row * lddx_in + c * 8, dx_out,
+                                oo + c * 8, want_dw ? acc + c * 8 : nullptr, D);
       }
     }
   }
   if (want_dw) {
     __syncthreads();
-    colred_flush<1, PAIR ? 2 : 1>(acc_smem, wpb, D, 3u);
+    colred_flush<L2 ? 2 : 1, PAIR ? 2 : 1>(acc_smem, wpb, D, PAIR || dbias != nullptr ? 3u : 1u);
   }
 }
 
@@ -589,68 +768,15 @@ static int launch_rms_bwd_tma(const void* dy, long lddy, const void* x, long ldx
   return colred_finish(3, grid, D, dweight, dgamma, dcolsum, stream);
 }
 
-template <bool XF32, bool DXF32, int NCH, bool PAIR = false>
-static int launch_rms_bwd_reg(const void* dy, long lddy, const void* x, long ldx, const void* w, const float* rstd,
-                              int M, int D, const float* dx_in, long lddx_in, void* dx_out, long lddx,
-                              float* dweight, cudaStream_t stream, const void* w1 = nullptr, float* dweight1 = nullptr,
-                              long x_pair_off = 0, long dy_pair_off = 0, long dx_pair_off = 0) {
-  constexpr int wpb = 8;
-  static_assert(wpb * 256 * NCH * sizeof(float) <= 48 * 1024,
-                "rms_bwd_reg: the weight-gradient rows of D <= 256 * NCH must fit the default 48 KB of shared memory");
-  const size_t smem = dweight ? (size_t)wpb * D * sizeof(float) : 0;
-  const long rows = PAIR ? 2L * M : M;
-  const int blocks = persistent_grid(rows, wpb * 2, 2);   // 2 CTAs/SM resident (<=128 registers): one persistent wave
-  if (colred_check(2, blocks, D, "rms_bwd_reg: gradient scratch too small")) return 1;
-  if (int rc = launch("rms_bwd_reg_kernel", rms_bwd_reg_kernel<XF32, DXF32, NCH, PAIR>, blocks, wpb * 32, smem, stream,
-                      ALLOW_PDL, reinterpret_cast<const __nv_bfloat16*>(dy), lddy, x, ldx,
-                      reinterpret_cast<const __nv_bfloat16*>(w), rstd, (int)rows, D, dx_in,
-                      lddx_in, dx_out, lddx, dweight,
-                      reinterpret_cast<const __nv_bfloat16*>(w1), dweight1, x_pair_off,
-                      dy_pair_off, dx_pair_off))
-    return rc;
-  if (dweight == nullptr) return 0;
-  return colred_finish(PAIR ? 2 : 1, blocks, D, dweight, PAIR ? dweight1 : nullptr, nullptr, stream);
-}
-
-template <bool XF32, bool LN, bool DXF32>
-static int launch_norm_bwd(const void* dy, long lddy, const void* x, long ldx, const void* weight,
-                           const float* mean, const float* rstd, int M, int D, const float* dx_in,
-                           long lddx_in, void* dx_out, long lddx, float* dweight, float* dbias,
-                           cudaStream_t stream) {
-  int wpb = 8;
-  size_t smem = dweight ? (size_t)(LN ? 2 : 1) * wpb * D * sizeof(float) : 0;
-  if (smem > 200 * 1024) { wpb = 4; smem /= 2; }
-  if (smem > 200 * 1024) { wpb = 2; smem /= 2; }
-  if (smem > 48 * 1024)
-    if (int rc = raise_smem_limit<norm_bwd_kernel<XF32, LN, DXF32>>(220 * 1024, "cudaFuncSetAttribute(norm_bwd)"))
-      return rc;
-  // >= 2 rows per warp so the smem flush amortises, but enough CTAs to keep ~32 warps/SM in flight:
-  // this kernel is pure HBM streaming and latency-bound below that (measured 2.8x off the HBM time
-  // with 1.4 CTAs/SM).
-  const int blocks = persistent_grid(M, wpb * 2, smem > 96 * 1024 ? 2 : 4);
-  if (colred_check(2, blocks, D, "norm_bwd: gradient scratch too small")) return 1;
-  if (int rc = launch("norm_bwd_kernel", norm_bwd_kernel<XF32, LN, DXF32>, blocks, wpb * 32, smem, stream, ALLOW_PDL,
-                      reinterpret_cast<const __nv_bfloat16*>(dy), lddy, x, ldx,
-                      reinterpret_cast<const __nv_bfloat16*>(weight), mean, rstd, M, D, dx_in, lddx_in, dx_out,
-                      lddx, dweight, dbias))
-    return rc;
-  if (dweight == nullptr) return 0;
-  return colred_finish(2, blocks, D, dweight, LN ? dbias : nullptr, nullptr, stream);
-}
-
 // Runtime flags and row widths to template arguments: f(std::bool_constant<b>{}), and f(NCH) for the
-// register-resident row kernels, whose rows hold NCH 256-column chunks (D <= 512, 1024, 1536; with MAX_NCH 16, the FP8
-// forward, D <= 4096).
+// register-resident row kernels, whose rows hold NCH 256-column chunks: pick_nch<L...> picks the first L with
+// D <= 256 * L, else the last.
 template <typename F>
 static auto pick_bool(bool b, F f) { return b ? f(std::true_type{}) : f(std::false_type{}); }
-template <int MAX_NCH = 6, typename F>
+template <int L, int... Ls, typename F>
 static int pick_nch(int D, F f) {
-  if (D <= 512) return f(std::integral_constant<int, 2>{});
-  if (D <= 1024) return f(std::integral_constant<int, 4>{});
-  if constexpr (MAX_NCH == 16) {
-    if (D > 1536) return f(std::integral_constant<int, 16>{});
-  }
-  return f(std::integral_constant<int, 6>{});
+  if constexpr (sizeof...(Ls) == 0) return f(std::integral_constant<int, L>{});
+  else return D <= 256 * L ? f(std::integral_constant<int, L>{}) : pick_nch<Ls...>(D, f);
 }
 
 // The operands of one norm forward; outputs that are null are not written.  q: the E4M3 row (NORM_Q / NORM_QY);
@@ -674,7 +800,8 @@ static int launch_norm_fwd(const NormFwd& a, cudaStream_t stream) {
   const long rows = PAIR ? 2L * a.M : a.M;
   const int blocks = persistent_grid(rows, 8, 8);
   auto in_registers = [&](auto xf, auto ln) {
-    return pick_nch<OUT == NORM_Y ? 6 : 16>(a.D, [&](auto nch) {
+    // bf16 rows up to D = 1536, the E4M3 forms up to IVB_NORM_FP8_MAX_D = 4096
+    return pick_nch<2, 4, 6, OUT == NORM_Y ? 6 : 16>(a.D, [&](auto nch) {
       return launch("norm_rows_kernel", norm_rows_kernel<xf, ln, nch, OUT, PAIR>, blocks, 256, 0, stream, ALLOW_PDL,
                     a.x, a.ldx, w, b, a.eps, (int)rows, a.D, y, a.ldy, a.mean, a.rstd,
                     reinterpret_cast<uint8_t*>(a.q), a.ldq, a.q_scale_inv,
@@ -696,6 +823,80 @@ static int launch_norm_fwd(const NormFwd& a, cudaStream_t stream) {
       }
     });
   }
+}
+
+// The operands of one norm backward; dw and db may be null.  l2: the decoder head's LN -> L2 backward (see
+// norm_bwd_kernel); gs and gs_dev scale its gradient dy.  w1, dw1 and the pair offsets: the second part of a PAIR launch.
+struct NormBwd {
+  const void* dy; long lddy; bool dy_f32;
+  const void* x; long ldx; bool x_f32;
+  const void* w; const void* b; const float* mean; const float* rstd; bool ln; int M; int D;
+  const float* dx_in; long lddx_in; void* dx; long lddx; bool dx_f32;
+  float* dw; float* db;
+  bool l2 = false; float gs = 1.f; const float* gs_dev = nullptr;
+  const void* w1 = nullptr; float* dw1 = nullptr; long x_pair_off = 0, dy_pair_off = 0, dx_pair_off = 0;
+};
+
+// Launches Kern, first raising its shared-memory limit to `limit` where smem passes the default 48 KB.
+template <auto Kern, typename... Args>
+static int launch_smem(const char* name, int limit, int grid, int threads, size_t smem, cudaStream_t stream,
+                       LaunchPdl pdl, Args... args) {
+  if (smem > 48 * 1024)
+    if (int rc = raise_smem_limit<Kern>(limit, "cudaFuncSetAttribute(norm_bwd)")) return rc;
+  return launch(name, Kern, grid, threads, smem, stream, pdl, args...);
+}
+
+// The one backward launch path.  norm_bwd_rows_kernel reads each row from HBM once: RMSNorm rows up to D = 1536, every
+// PAIR launch, and LN -> L2 rows of a bf16 gradient up to C = 3328; norm_bwd_kernel streams the rest.  The weight and
+// bias gradients are summed per warp in shared memory (nacc rows of D per warp) and then across CTAs by colred_finish.
+template <bool PAIR = false>
+static int launch_norm_bwd(const NormBwd& a, cudaStream_t stream) {
+  const bool in_registers = PAIR || (!a.ln && a.D <= 1536) || (a.l2 && !a.dy_f32 && a.D <= 256 * 13);
+  const long rows = PAIR ? 2L * a.M : a.M;
+  const int nacc = a.ln ? 2 : 1;
+  int wpb = in_registers && a.l2 ? 4 : 8;
+  size_t smem = a.dw ? static_cast<size_t>(nacc) * wpb * a.D * sizeof(float) : 0;
+  while (smem > 200 * 1024 && wpb > 1) { wpb /= 2; smem /= 2; }   // streaming rows only: the register forms need <= 104 KB
+  // >= 2 rows per warp so the shared-memory flush amortises.  The register forms run 2 CTAs per SM, one persistent
+  // wave; the streaming one keeps ~32 warps/SM in flight: it is pure HBM streaming and latency-bound below that
+  // (measured 2.8x off the HBM time with 1.4 CTAs/SM).
+  const int grid = in_registers ? persistent_grid(rows, 2 * wpb, 2) : persistent_grid(a.M, 2 * wpb, smem > 96 * 1024 ? 2 : 4);
+  if (colred_check(2, grid, a.D, a.l2 ? "ln_l2_bwd: gradient scratch too small" : "norm_bwd: gradient scratch too small"))
+    return 1;
+  const LaunchPdl pdl = a.l2 ? NO_PDL : ALLOW_PDL;
+  const __nv_bfloat16* w = reinterpret_cast<const __nv_bfloat16*>(a.w);
+  const __nv_bfloat16* b = reinterpret_cast<const __nv_bfloat16*>(a.b);
+  const __nv_bfloat16* dy = reinterpret_cast<const __nv_bfloat16*>(a.dy);   // or fp32 (L2 with dy_f32)
+  auto streamed = [&](auto xf, auto ln, auto dxf, auto l2, auto gf) {
+    return launch_smem<norm_bwd_kernel<xf, ln, dxf, l2, gf>>(
+        "norm_bwd_kernel", 220 * 1024, grid, wpb * 32, smem, stream, pdl, dy, a.lddy, a.x, a.ldx, w, b, a.mean, a.rstd,
+        a.M, a.D, a.dx_in, a.lddx_in, a.dx, a.lddx, a.dw, a.db, a.gs, a.gs_dev);
+  };
+  auto in_regs = [&](auto xf, auto dxf, auto nch, auto l2) {
+    return launch_smem<norm_bwd_rows_kernel<xf, dxf, nch, PAIR, l2>>(
+        "norm_bwd_rows_kernel", 110 * 1024, grid, wpb * 32, smem, stream, pdl, dy, a.lddy, a.x, a.ldx, w, b, a.mean,
+        a.rstd, (int)rows, a.D, a.dx_in, a.lddx_in, a.dx, a.lddx, a.dw, a.db, a.gs, a.gs_dev,
+        reinterpret_cast<const __nv_bfloat16*>(a.w1), a.x_pair_off, a.dy_pair_off, a.dx_pair_off);
+  };
+  constexpr std::false_type F{};
+  constexpr std::true_type T{};
+  int rc;
+  if constexpr (PAIR) {   // the q/k norms: RMSNorm of bf16 rows
+    rc = pick_nch<2, 4, 6>(a.D, [&](auto nch) { return in_regs(F, F, nch, F); });
+  } else if (a.l2) {   // LayerNorm of bf16 z to bf16 dz
+    rc = in_registers ? pick_nch<3, 6, 13>(a.D, [&](auto nch) { return in_regs(F, F, nch, T); })
+                      : pick_bool(a.dy_f32, [&](auto gf) { return streamed(F, T, F, T, gf); });
+  } else {
+    rc = pick_bool(a.x_f32, [&](auto xf) {
+      return pick_bool(a.dx_f32, [&](auto dxf) {
+        if (in_registers) return pick_nch<2, 4, 6>(a.D, [&](auto nch) { return in_regs(xf, dxf, nch, F); });
+        return pick_bool(a.ln, [&](auto ln) { return streamed(xf, ln, dxf, F, F); });
+      });
+    });
+  }
+  float* out1 = PAIR ? a.dw1 : a.ln ? a.db : nullptr;   // the second gradient: the pair's second weight, or the bias
+  if (rc != 0 || a.dw == nullptr) return rc;
+  return colred_finish(out1 ? 2 : 1, grid, a.D, a.dw, out1, nullptr, stream);
 }
 
 // Sets the error text "<fn>: <what>"; returns set_error's status.
@@ -771,19 +972,9 @@ extern "C" int ivb_norm_bwd(const void* dy, long lddy, const void* x, int x_is_f
   if (misaligned(16, dy, x, weight, dx_in, dx_out))
     return set_error("ivb_norm_bwd: dy, x, weight, dx_in and dx_out must be 16-byte aligned");
   if (is_layernorm && mean == nullptr) return set_error("ivb_norm_bwd: LayerNorm needs mean");
-  return pick_bool(x_is_f32, [&](auto xf) {
-    return pick_bool(dx_out_is_f32, [&](auto dxf) {
-      if (!is_layernorm && D <= 1536)
-        return pick_nch(D, [&](auto nch) {
-          return launch_rms_bwd_reg<xf, dxf, nch>(dy, lddy, x, ldx, weight, rstd, M, D, dx_in, lddx_in, dx_out, lddx,
-                                                  dweight, stream);
-        });
-      return pick_bool(is_layernorm, [&](auto ln) {
-        return launch_norm_bwd<xf, ln, dxf>(dy, lddy, x, ldx, weight, mean, rstd, M, D, dx_in, lddx_in, dx_out, lddx,
-                                            dweight, dbias, stream);
-      });
-    });
-  });
+  return launch_norm_bwd({dy, lddy, false, x, ldx, x_is_f32 != 0, weight, nullptr, mean, rstd, is_layernorm != 0, M, D,
+                          dx_in, lddx_in, dx_out, lddx, dx_out_is_f32 != 0, dweight, dbias},
+                         stream);
 }
 
 extern "C" int ivb_layerscale_bwd(const float* dx, long lddx, const void* y, long ldy,
@@ -852,10 +1043,14 @@ extern "C" int ivb_rmsnorm_pair_bwd(const void* dy, long lddy, long dy_pair_off,
   if ((dweight0 == nullptr) != (dweight1 == nullptr)) return set_error("ivb_rmsnorm_pair_bwd: give both weight gradients or none");
   if (misaligned(16, dy, x, w0, w1, dx_out))
     return set_error("ivb_rmsnorm_pair_bwd: dy, x, w0, w1 and dx_out must be 16-byte aligned");
-  return pick_nch(D, [&](auto nch) {
-    return launch_rms_bwd_reg<false, false, nch, true>(dy, lddy, x, ldx, w0, rstd, M, D, nullptr, 0, dx_out, lddx, dweight0,
-                                                       stream, w1, dweight1, x_pair_off, dy_pair_off, dx_pair_off);
-  });
+  NormBwd a{dy, lddy, false, x, ldx, false, w0, nullptr, nullptr, rstd, false, M, D, nullptr, 0, dx_out, lddx, false,
+            dweight0, nullptr};
+  a.w1 = w1;
+  a.dw1 = dweight1;
+  a.x_pair_off = x_pair_off;
+  a.dy_pair_off = dy_pair_off;
+  a.dx_pair_off = dx_pair_off;
+  return launch_norm_bwd<true>(a, stream);
 }
 
 // RMSNorm backward (fp32 stream) fused with the LayerScale backward of the branch that produced the stream
@@ -878,4 +1073,38 @@ extern "C" int ivb_rmsnorm_bwd_layerscale(const void* dy, long lddy, const float
     return set_error("ivb_rmsnorm_bwd_layerscale: D too large for the shared-memory row ring (use the separate kernels)");
   return launch_rms_bwd_tma(dy, lddy, x, ldx, weight, rstd, M, D, dx_in, lddx_in, dx_out, lddx, dweight, ybr, ldyb, gamma,
                             rowscale, dyb, lddyb, dgamma, dcolsum, stream);
+}
+
+extern "C" int ivb_ln_l2_fwd(const void* z, long ldz, const void* weight, const void* bias, float eps,
+                             int M, int C, void* out, long ldo, float* stats, const void* target,
+                             int target_is_f32, long ldt, float* loss_sum, void* stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  if (M <= 0) return 0;
+  if ((C & 7) || (ldz & 7) || (ldo & 7) || (ldt & 7)) return set_error("ivb_ln_l2_fwd: C/ld must be multiples of 8");
+  if (misaligned(16, z, weight, bias, out, target))
+    return set_error("ivb_ln_l2_fwd: z, weight, bias, out and target must be 16-byte aligned");
+  const int blocks = persistent_grid(M, 8, 8);
+  auto zz = reinterpret_cast<const __nv_bfloat16*>(z);
+  auto ww = reinterpret_cast<const __nv_bfloat16*>(weight);
+  auto bb = reinterpret_cast<const __nv_bfloat16*>(bias);
+  auto oo = reinterpret_cast<__nv_bfloat16*>(out);
+  return launch("ln_l2_fwd_kernel", target_is_f32 ? ln_l2_fwd_kernel<true> : ln_l2_fwd_kernel<false>, blocks, 256, 0,
+                stream, NO_PDL, zz, ldz, ww, bb, eps, M, C, oo, ldo, stats, target, ldt, loss_sum);
+}
+
+extern "C" int ivb_ln_l2_bwd(const void* z, long ldz, const void* weight, const void* bias,
+                             const float* stats, int M, int C, const void* dout, int dout_is_f32,
+                             long lddo, float gscale_host, const float* gscale_dev, void* dz, long lddz,
+                             float* dweight, float* dbias, void* stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  if (M <= 0) return 0;
+  if ((C & 7) || (ldz & 7) || (lddz & 7) || (lddo & 7)) return set_error("ivb_ln_l2_bwd: C/ld must be multiples of 8");
+  if (misaligned(16, z, weight, bias, dout, dz))
+    return set_error("ivb_ln_l2_bwd: z, weight, bias, dout and dz must be 16-byte aligned");
+  NormBwd a{dout, lddo, dout_is_f32 != 0, z, ldz, false, weight, bias, stats, nullptr, true, M, C, nullptr, 0, dz, lddz,
+            false, dweight, dbias};
+  a.l2 = true;
+  a.gs = gscale_host;
+  a.gs_dev = gscale_dev;
+  return launch_norm_bwd(a, stream);
 }

@@ -12,7 +12,7 @@ views -- padding, the untouched q/k/v slots, neighbouring rows -- must keep its 
 outputs start from nonzero values, so the documented `+=` is checked too.
 
 Each limit in LIMITS is at most twice the worst value measured over this file on an H100 80GB HBM3 (SXM, 700 W power
-limit); the measured value is beside it.  The file (688 tests) runs in 20 to 30 s there.
+limit); the measured value is beside it.  The file (692 tests) runs in 20 to 30 s there.
 """
 import math
 import zlib
@@ -208,10 +208,21 @@ def _stats(x, w, b, ln):
 @pytest.mark.parametrize("with_in", [True, False])
 @pytest.mark.parametrize("with_grads", [True, False])
 def test_norm_bwd(cuda_lib, kind, D, xdt, dxdt, with_in, with_grads):
+    _check_norm_bwd(kind, D, 1031, xdt, dxdt, with_in, with_grads)
+
+
+@pytest.mark.parametrize("xdt", [f32, bf16])
+@pytest.mark.parametrize("with_in", [True, False])
+def test_norm_bwd_one_warp_per_cta(cuda_lib, xdt, with_in):
+    """LayerNorm at D = 14 088 with weight gradients: a warp's two gradient rows take 110 KB of shared memory, so each
+    CTA runs one warp.  At M = 400 the partials of its 200 CTAs fit the gradient scratch."""
+    _check_norm_bwd("ln", 14088, 400, xdt, bf16, with_in, True)
+
+
+def _check_norm_bwd(kind, D, M, xdt, dxdt, with_in, with_grads):
     from internvideo_b200 import lowlevel as ll
     _seed("bwd", kind, D, str(xdt), str(dxdt), with_in, with_grads)
     ln = kind == "ln"
-    M = 1031
     fr = Frame()
     x = fr.mat(M, D, xdt, torch.randn(M, D, device="cuda") * 2 + 0.3, writes=False)
     w, b = _weights(D, ln)
