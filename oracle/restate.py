@@ -114,12 +114,13 @@ def mlp(p, pre, x, gelu_mode="none"):
     return linear(h, p[pre + "fc2.weight"], p[pre + "fc2.bias"])
 
 
-def block(p, i, x, num_heads, gelu_mode="none", drop_path=None):
+def block(p, i, x, num_heads, gelu_mode="none", drop_path=None, qk_norm=True):
     """Block.forward naive branch — {SM}:290-291 (LayerScale fp32 :139-143).
     drop_path: None (eval / rate 0) or (f1, f2), per-sample factors [B] = Bernoulli(keep)/keep that timm's
-    DropPath multiplies the attention / MLP branch with in training ({SM}:264,274)."""
+    DropPath multiplies the attention / MLP branch with in training ({SM}:264,274).
+    qk_norm: the block's qk_normalization (the q/k RMSNorms, {SM}:178-181); False skips them."""
     pre = f"blocks.{i}."
-    a = attention(p, pre + "attn.", rmsnorm(x, p[pre + "norm1.weight"]), num_heads)
+    a = attention(p, pre + "attn.", rmsnorm(x, p[pre + "norm1.weight"]), num_heads, qk_norm)
     if pre + "ls1.gamma" in p:
         a = a * p[pre + "ls1.gamma"]
     if drop_path is not None:
