@@ -23,9 +23,10 @@
  *   - there is no CPU fallback: without a CUDA device of compute capability 9.0 every compute
  *     entry point returns an error.
  *   - parameter gradients (ivb_norm_bwd, ivb_rmsnorm_pair_bwd, ivb_rmsnorm_bwd_layerscale, ivb_layerscale_bwd,
- *     ivb_colsum_bf16, ivb_ln_l2_bwd) are summed over rows in a fixed order through a per-device scratch of the
- *     library, so the same inputs give the same bits on every run.  That scratch holds one reduction at a time:
- *     these entry points must not be called concurrently from two streams of the same device.
+ *     ivb_colsum_bf16, ivb_ln_l2_bwd), the losses (ivb_ln_l2_fwd with a target, ivb_vtc_loss_fwd, ivb_mse_loss) and
+ *     dtemp (ivb_vtc_loss_bwd) are summed in a fixed order through a per-device scratch of the library, so the same
+ *     inputs give the same bits on every run.  That scratch holds one reduction at a time: these entry points must
+ *     not be called concurrently from two streams of the same device (the package runs them on one compute stream).
  *   - the row kernels (ivb_norm_fwd, ivb_norm_bwd, ivb_rmsnorm_pair_*, ivb_rmsnorm_bwd_layerscale, ivb_layerscale_bwd,
  *     ivb_colsum_bf16, ivb_ln_l2_*, ivb_l2norm_rows_*, ivb_pool_attn_*, ivb_gather_add, ivb_scatter_add) move each row
  *     in 16-byte vectors: the row width and every pitch (and clip stride) are multiples of 8 elements (the fp32
@@ -431,7 +432,8 @@ int ivb_ln_l2_bwd(const void* z, long ldz, const void* weight, const void* bias,
 
 /* ---- video-text contrastive loss (criterions.py:15-55, 65-103, 200-216) --------------------------
  * cos_v2t [G,G] fp32 = normalize(v) @ normalize(t)^T over the GATHERED batch; idx int64 [G].
- * *loss += 1/2 (CE_v2t + CE_t2v) with soft targets (idx==idx^T)/rowsum.  lse_row/lse_col: fp32 [G]. */
+ * *loss += 1/2 (CE_v2t + CE_t2v) with soft targets (idx==idx^T)/rowsum.  lse_row/lse_col: fp32 [G].
+ * The loss sums one partial per row and per column in the library's scratch: G <= 3 145 728.         */
 /* temp_dev (optional, device fp32[1]) overrides `temp`: the learnable temperature stays on the device
  * (internvideo2_clip_small.py:45,96-99), no host read per step, valid inside a captured CUDA graph.  */
 int ivb_vtc_loss_fwd(const float* cos_v2t, const long long* idx, int G, float temp,

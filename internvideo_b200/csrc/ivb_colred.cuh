@@ -6,7 +6,9 @@
 // runs of the same training step would disagree.  Instead every CTA stores its partial in a scratch slot
 //   g_colred[(out * nslots + slot) * D + col]
 // and colred_finish() adds the partials into the gradient in slot order: same inputs, same bits.
-// The scratch is static device memory of the one translation unit that includes this header (24 MB in ivb_norm.cu).
+// The same scratch, with D = 1, sums the loss kernels' scalars (the losses and dtemp) in CTA order.
+// The scratch is static device memory of the one translation unit that includes this header (24 MB in ivb_norm.cu);
+// kernels of other translation units reach it through scalar_slots / scalar_finish (ivb_internal.h).
 // It holds ONE reduction at a time per device: the entry points that use it must not run concurrently on two streams of
 // the same device (include/ivb200.h, Conventions).  A call whose partials would not fit returns an error.
 #pragma once

@@ -40,6 +40,13 @@ inline int persistent_grid(long rows, int rows_per_cta, int per_sm) {
   return static_cast<int>(blocks > cap ? cap : (blocks < 1 ? 1 : blocks));
 }
 
+// Fixed-order scalar sums (the losses and dtemp of ivb_loss.cu) through the one per-device reduction scratch of
+// ivb_colred.cuh, which lives in ivb_norm.cu: each CTA of a kernel stores its partial in slot blockIdx.x of
+// scalar_slots(n), and scalar_finish(n, dst) then adds slots [0, n) in slot order into *dst (nothing when dst is null).
+// scalar_slots returns null, with `who` as the error text, when n slots do not fit or the address cannot be read.
+float* scalar_slots(long n, const char* who);
+int scalar_finish(int n, float* dst, cudaStream_t stream);
+
 // Programmatic dependent launch (PDL) is opt-in: pdl_enabled() is true only when IVB_PDL is set to a non-zero value.
 // A PDL-launched kernel may be scheduled while the previous kernel of the stream is still draining, so it must execute
 // pdl_wait() (ivb_ptx.cuh) before its first global-memory access; only such kernels are launched with ALLOW_PDL.

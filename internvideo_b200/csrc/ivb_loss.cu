@@ -94,10 +94,11 @@ __global__ void adamw_kernel(float* __restrict__ master, float* __restrict__ m, 
 // cosv2t [G,G] fp32 = vn @ tn^T (wgmma GEMM).  S = cos / temp.  idx int64 [G].
 // row pass: lse_r[i], tsum_r[i] = sum_j tg[i,j] S[i,j] ; col pass: lse_c[i], tsum_c[i] = sum_j tg[i,j] S[j,i]
 // loss = 1/(2G) sum_i [(lse_r[i] - tsum_r[i]) + (lse_c[i] - tsum_c[i])]          (criterions.py:93-102)
+// Each CTA stores its term in loss_part[blockIdx.x]; scalar_finish adds them into the loss in slot order.
 __global__ void __launch_bounds__(256)
 vtc_stats_kernel(const float* __restrict__ cosm, const long long* __restrict__ idx, int G, float inv_temp,
                  const float* __restrict__ temp_dev,
-                 float* __restrict__ lse_r, float* __restrict__ lse_c, float* __restrict__ loss) {
+                 float* __restrict__ lse_r, float* __restrict__ lse_c, float* __restrict__ loss_part) {
   // a device-resident temperature (the learnable `temp` parameter) overrides the host value: no D2H
   // sync per step and a captured CUDA graph follows the parameter as it trains
   if (temp_dev != nullptr) inv_temp = 1.f / *temp_dev;
@@ -110,40 +111,30 @@ vtc_stats_kernel(const float* __restrict__ cosm, const long long* __restrict__ i
     const float s = (which == 0 ? cosm[static_cast<long>(i) * G + j] : cosm[static_cast<long>(j) * G + i]) * inv_temp;
     mx = fmaxf(mx, s);
   }
-  __shared__ float red[8];
-  __shared__ float bc;
-  mx = warp_max(mx);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = mx;
-  __syncthreads();
-  if (threadIdx.x == 0) { float t = red[0]; for (int k = 1; k < 8; ++k) t = fmaxf(t, red[k]); bc = t; }
-  __syncthreads();
-  mx = bc;
-  float se = 0.f, ts = 0.f, cnt = 0.f;
+  __shared__ float red[3 * 8];
+  mx = block_reduce<true>(mx, red);
+  float sums[3] = {0.f, 0.f, 0.f};   // sum exp(S - mx), sum of the target entries' S, their count
   for (int j = threadIdx.x; j < G; j += blockDim.x) {
     const float s = (which == 0 ? cosm[static_cast<long>(i) * G + j] : cosm[static_cast<long>(j) * G + i]) * inv_temp;
-    se += __expf(s - mx);
-    if (idx[j] == my) { ts += s; cnt += 1.f; }
+    sums[0] += __expf(s - mx);
+    if (idx[j] == my) { sums[1] += s; sums[2] += 1.f; }
   }
-  __shared__ float r2[3][8];
-  se = warp_sum(se); ts = warp_sum(ts); cnt = warp_sum(cnt);
-  if ((threadIdx.x & 31) == 0) { r2[0][threadIdx.x >> 5] = se; r2[1][threadIdx.x >> 5] = ts; r2[2][threadIdx.x >> 5] = cnt; }
-  __syncthreads();
+  block_reduce(sums, red);
   if (threadIdx.x == 0) {
-    float a = 0.f, b2 = 0.f, c = 0.f;
-    for (int k = 0; k < 8; ++k) { a += r2[0][k]; b2 += r2[1][k]; c += r2[2][k]; }
-    const float lse = mx + __logf(a);
+    const float lse = mx + __logf(sums[0]);
     (which == 0 ? lse_r : lse_c)[i] = lse;
-    atomicAdd(loss, (lse - b2 / c) * (0.5f / G));
+    loss_part[blockIdx.x] = (lse - sums[1] / sums[2]) * (0.5f / G);
   }
 }
 
 // dS[a,b] = gs/(2G) * [ exp(S-lse_r[a]) + exp(S-lse_c[b]) - 2*tg[a,b] ] ; written as bf16 d(cos) = dS/temp
-// and dtemp accumulated: dtemp += sum dS * (-S/temp).
+// and row a's share of dtemp = sum dS * (-S/temp) stored in dtemp_part[a] (null: not wanted).
 __global__ void __launch_bounds__(256)
 vtc_grad_kernel(const float* __restrict__ cosm, const long long* __restrict__ idx, int G, float inv_temp,
                 const float* __restrict__ temp_dev,
                 const float* __restrict__ lse_r, const float* __restrict__ lse_c, float gscale_host,
-                const float* __restrict__ gscale_dev, __nv_bfloat16* __restrict__ dcos, float* __restrict__ dtemp) {
+                const float* __restrict__ gscale_dev, __nv_bfloat16* __restrict__ dcos,
+                float* __restrict__ dtemp_part) {
   if (temp_dev != nullptr) inv_temp = 1.f / *temp_dev;
   const int a = blockIdx.x;
   const float gs = gscale_host * (gscale_dev ? *gscale_dev : 1.f) * (0.5f / G);
@@ -151,13 +142,7 @@ vtc_grad_kernel(const float* __restrict__ cosm, const long long* __restrict__ id
   float cnt = 0.f;
   for (int j = threadIdx.x; j < G; j += blockDim.x) cnt += (idx[j] == my) ? 1.f : 0.f;
   __shared__ float red[8];
-  __shared__ float bc;
-  cnt = warp_sum(cnt);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = cnt;
-  __syncthreads();
-  if (threadIdx.x == 0) { float t = 0.f; for (int k = 0; k < 8; ++k) t += red[k]; bc = t; }
-  __syncthreads();
-  const float inv_cnt = 1.f / bc;
+  const float inv_cnt = 1.f / block_reduce(cnt, red);
   const float la = lse_r[a];
   float dt = 0.f;
   for (int b = threadIdx.x; b < G; b += blockDim.x) {
@@ -167,11 +152,8 @@ vtc_grad_kernel(const float* __restrict__ cosm, const long long* __restrict__ id
     dcos[static_cast<long>(a) * G + b] = __float2bfloat16(ds * inv_temp);
     dt += ds * (-s * inv_temp);
   }
-  dt = warp_sum(dt);
-  __syncthreads();
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = dt;
-  __syncthreads();
-  if (threadIdx.x == 0 && dtemp) { float t = 0.f; for (int k = 0; k < 8; ++k) t += red[k]; atomicAdd(dtemp, t); }
+  dt = block_reduce(dt, red);
+  if (threadIdx.x == 0 && dtemp_part) dtemp_part[a] = dt;
 }
 
 // F.normalize(x, dim=-1) rows (eps 1e-12): out bf16, inv_norm saved.   x fp32 or bf16.
@@ -257,10 +239,11 @@ __global__ void pixel_target_kernel(const __nv_bfloat16* __restrict__ video, con
   for (int i = lane; i < npix; i += 32) out[static_cast<long>(i) * C + c] = ((pixel(i) - pivot) - mean) * inv;
 }
 
-// loss_sum += sum (pred - label)^2 ; dpred(bf16) = gscale * 2 (pred - label) (optional)
+// the CTA's sum (pred - label)^2 -> loss_part[blockIdx.x] (null: not wanted) ; dpred(bf16) = gscale * 2 (pred - label)
+// (optional)
 __global__ void __launch_bounds__(256)
 mse_kernel(const __nv_bfloat16* __restrict__ pred, const float* __restrict__ label, long n,
-           float* __restrict__ loss_sum, float gscale_host, const float* __restrict__ gscale_dev,
+           float* __restrict__ loss_part, float gscale_host, const float* __restrict__ gscale_dev,
            __nv_bfloat16* __restrict__ dpred) {
   const float gs = gscale_host * (gscale_dev ? *gscale_dev : 1.f);
   float acc = 0.f;
@@ -270,10 +253,8 @@ mse_kernel(const __nv_bfloat16* __restrict__ pred, const float* __restrict__ lab
     if (dpred) dpred[i] = __float2bfloat16(2.f * gs * d);
   }
   __shared__ float red[8];
-  acc = warp_sum(acc);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = acc;
-  __syncthreads();
-  if (threadIdx.x == 0 && loss_sum) { float t = 0.f; for (int k = 0; k < 8; ++k) t += red[k]; atomicAdd(loss_sum, t); }
+  acc = block_reduce(acc, red);
+  if (threadIdx.x == 0 && loss_part) loss_part[blockIdx.x] = acc;
 }
 
 }  // namespace ivb
@@ -299,8 +280,12 @@ extern "C" int ivb_vtc_loss_fwd(const float* cos_v2t, const long long* idx, int 
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (G <= 0) return 0;
   if (temp_dev == nullptr && !(temp > 0.f)) return set_error("ivb_vtc_loss_fwd: temp must be > 0");
-  return launch("vtc_stats_kernel", vtc_stats_kernel, 2 * G, 256, 0, stream, NO_PDL, cos_v2t, idx, G, 1.f / temp, temp_dev,
-                lse_row, lse_col, loss);
+  float* part = scalar_slots(2L * G, "ivb_vtc_loss_fwd: G too large for the loss scratch");
+  if (part == nullptr) return 1;
+  if (int rc = launch("vtc_stats_kernel", vtc_stats_kernel, 2 * G, 256, 0, stream, NO_PDL, cos_v2t, idx, G, 1.f / temp,
+                      temp_dev, lse_row, lse_col, part))
+    return rc;
+  return scalar_finish(2 * G, loss, stream);
 }
 
 extern "C" int ivb_vtc_loss_bwd(const float* cos_v2t, const long long* idx, int G, float temp,
@@ -309,8 +294,14 @@ extern "C" int ivb_vtc_loss_bwd(const float* cos_v2t, const long long* idx, int 
                                 const float* gscale_dev, void* dcos_bf16, float* dtemp, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (G <= 0) return 0;
-  return launch("vtc_grad_kernel", vtc_grad_kernel, G, 256, 0, stream, NO_PDL, cos_v2t, idx, G, 1.f / temp, temp_dev,
-                lse_row, lse_col, gscale_host, gscale_dev, reinterpret_cast<__nv_bfloat16*>(dcos_bf16), dtemp);
+  float* part = nullptr;
+  if (dtemp != nullptr && (part = scalar_slots(G, "ivb_vtc_loss_bwd: G too large for the dtemp scratch")) == nullptr)
+    return 1;
+  if (int rc = launch("vtc_grad_kernel", vtc_grad_kernel, G, 256, 0, stream, NO_PDL, cos_v2t, idx, G, 1.f / temp,
+                      temp_dev, lse_row, lse_col, gscale_host, gscale_dev, reinterpret_cast<__nv_bfloat16*>(dcos_bf16),
+                      part))
+    return rc;
+  return scalar_finish(G, dtemp, stream);
 }
 
 extern "C" int ivb_l2norm_rows_fwd(const void* x, int x_is_f32, long ldx, int M, int C, void* out,
@@ -352,25 +343,21 @@ extern "C" int ivb_mse_loss(const void* pred_bf16, const float* label, long n, f
                             float gscale_host, const float* gscale_dev, void* dpred_bf16, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (n <= 0) return 0;
-  return launch("mse_kernel", mse_kernel, persistent_grid(n, 256, 8), 256, 0, stream, NO_PDL,
-                reinterpret_cast<const __nv_bfloat16*>(pred_bf16), label, n, loss_sum, gscale_host, gscale_dev,
-                reinterpret_cast<__nv_bfloat16*>(dpred_bf16));
+  const int grid = persistent_grid(n, 256, 8);
+  float* part = nullptr;
+  if (loss_sum != nullptr && (part = scalar_slots(grid, "ivb_mse_loss: too many CTAs for the loss scratch")) == nullptr)
+    return 1;
+  if (int rc = launch("mse_kernel", mse_kernel, grid, 256, 0, stream, NO_PDL,
+                      reinterpret_cast<const __nv_bfloat16*>(pred_bf16), label, n, part, gscale_host, gscale_dev,
+                      reinterpret_cast<__nv_bfloat16*>(dpred_bf16)))
+    return rc;
+  return scalar_finish(grid, loss_sum, stream);
 }
 
 // ---------------------------------------------------------------- single-query attention pooling
 // AttentionPoolingBlock / CrossAttention with ONE query per clip (internvideo2_pretrain.py:61-76, 107-114):
 //   s_j = scale * <q_h, k_{j,h}> ; p = softmax_j(s) ; o_h = sum_j p_j v_{j,h}.   One CTA per (head, clip).
 namespace ivb {
-
-__device__ __forceinline__ float block_reduce_128(float v, float* red, bool is_max) {
-  v = is_max ? warp_max(v) : warp_sum(v);
-  __syncthreads();
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-  __syncthreads();
-  float r = red[0];
-  for (int k = 1; k < 4; ++k) r = is_max ? fmaxf(r, red[k]) : r + red[k];
-  return r;
-}
 
 __global__ void __launch_bounds__(128)
 pool_attn_fwd_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ k, long ldk,
@@ -396,10 +383,10 @@ pool_attn_fwd_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* _
     sp[j] = s;
     mx = fmaxf(mx, s);
   }
-  mx = block_reduce_128(mx, red, true);
+  mx = block_reduce<true>(mx, red);
   float se = 0.f;
   for (int j = threadIdx.x; j < n; j += blockDim.x) { const float e = __expf(sp[j] - mx); sp[j] = e; se += e; }
-  se = block_reduce_128(se, red, false);
+  se = block_reduce(se, red);
   const float inv = 1.f / se;
   __syncthreads();
   for (int j = threadIdx.x; j < n; j += blockDim.x) {
@@ -447,7 +434,7 @@ pool_attn_bwd_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* _
     sds[j] = dp;
     acc += pr[j] * dp;
   }
-  acc = block_reduce_128(acc, red, false);
+  acc = block_reduce(acc, red);
   __syncthreads();
   for (int j = threadIdx.x; j < n; j += blockDim.x) {
     const float pj = pr[j];

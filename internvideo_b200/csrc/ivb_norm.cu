@@ -85,13 +85,14 @@ norm_fwd_kernel(const void* __restrict__ x, long ldx, const __nv_bfloat16* __res
 
 // ------------------------------------------------------------------ decoder head: LayerNorm + L2 normalise
 // out = y / ||y||,  y = LN(z) * w + b.   stats[row] = {mean, rstd, 1/||y||}.
-// If tgt != nullptr also accumulates loss_sum += sum_rows (2 - 2 <out, tgt>)  (engine :131-136).
+// If tgt != nullptr and want_loss, also stores the CTA's sum over its rows of (2 - 2 <out, tgt>)  (engine :131-136)
+// in colred slot blockIdx.x, for colred_finish to add into the loss.
 template <bool TGT_F32>
 __global__ void __launch_bounds__(256)
 ln_l2_fwd_kernel(const __nv_bfloat16* __restrict__ z, long ldz, const __nv_bfloat16* __restrict__ w,
                  const __nv_bfloat16* __restrict__ bsh, float eps, int M, int C,
                  __nv_bfloat16* __restrict__ out, long ldo, float* __restrict__ stats,
-                 const void* __restrict__ tgt, long ldt, float* __restrict__ loss_sum) {
+                 const void* __restrict__ tgt, long ldt, bool want_loss) {
   const int lane = threadIdx.x & 31;
   const int wpb = blockDim.x >> 5;
   const float invC = 1.f / C;
@@ -124,7 +125,7 @@ ln_l2_fwd_kernel(const __nv_bfloat16* __restrict__ z, long ldz, const __nv_bfloa
     }
     n2 = warp_sum(n2);
     const float inv_n = rsqrtf(n2);
-    if (tgt) { dot = warp_sum(dot); if (lane == 0) loss_acc += 2.f - 2.f * dot * inv_n; }
+    if (tgt) { dot = warp_sum(dot); loss_acc += 2.f - 2.f * dot * inv_n; }   // the same in every lane
     if (out) {
       for (int c = lane * 8; c < C; c += 256) {
         float v[8], wv[8], bv[8], o[8];
@@ -136,15 +137,10 @@ ln_l2_fwd_kernel(const __nv_bfloat16* __restrict__ z, long ldz, const __nv_bfloa
     }
     if (lane == 0 && stats) { stats[row * 3 + 0] = mean; stats[row * 3 + 1] = rstd; stats[row * 3 + 2] = inv_n; }
   }
-  if (tgt && loss_sum) {
+  if (tgt && want_loss) {
     __shared__ float red[8];
-    if (lane == 0) red[threadIdx.x >> 5] = loss_acc;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      float t = 0.f;
-      for (int k = 0; k < wpb; ++k) t += red[k];
-      atomicAdd(loss_sum, t);
-    }
+    loss_acc = block_reduce(lane == 0 ? loss_acc : 0.f, red);
+    if (threadIdx.x == 0) colred_put(0, gridDim.x, blockIdx.x, 1, 0, loss_acc);
   }
 }
 
@@ -927,6 +923,27 @@ static int check_norm_fwd_fp8(const char* fn, bool train, const NormFwd& a) {
   return 0;
 }
 
+float* scalar_slots(long n, const char* who) {
+  if (colred_check(1, n, 1, who)) return nullptr;
+  static float* base[64] = {};
+  int dev = 0;
+  cudaGetDevice(&dev);
+  const bool tracked = dev >= 0 && dev < 64;
+  if (tracked && base[dev] != nullptr) return base[dev];
+  void* p = nullptr;
+  const cudaError_t e = cudaGetSymbolAddress(&p, g_colred);
+  if (e != cudaSuccess) {
+    set_error_cuda(who, e);
+    return nullptr;
+  }
+  if (tracked) base[dev] = static_cast<float*>(p);
+  return static_cast<float*>(p);
+}
+
+int scalar_finish(int n, float* dst, cudaStream_t stream) {
+  return colred_finish(1, n, 1, dst, nullptr, nullptr, stream);
+}
+
 }  // namespace ivb
 
 using namespace ivb;
@@ -1084,12 +1101,16 @@ extern "C" int ivb_ln_l2_fwd(const void* z, long ldz, const void* weight, const 
   if (misaligned(16, z, weight, bias, out, target))
     return set_error("ivb_ln_l2_fwd: z, weight, bias, out and target must be 16-byte aligned");
   const int blocks = persistent_grid(M, 8, 8);
+  float* loss = target != nullptr ? loss_sum : nullptr;
+  if (loss != nullptr && colred_check(1, blocks, 1, "ivb_ln_l2_fwd: loss scratch too small")) return 1;
   auto zz = reinterpret_cast<const __nv_bfloat16*>(z);
   auto ww = reinterpret_cast<const __nv_bfloat16*>(weight);
   auto bb = reinterpret_cast<const __nv_bfloat16*>(bias);
   auto oo = reinterpret_cast<__nv_bfloat16*>(out);
-  return launch("ln_l2_fwd_kernel", target_is_f32 ? ln_l2_fwd_kernel<true> : ln_l2_fwd_kernel<false>, blocks, 256, 0,
-                stream, NO_PDL, zz, ldz, ww, bb, eps, M, C, oo, ldo, stats, target, ldt, loss_sum);
+  if (int rc = launch("ln_l2_fwd_kernel", target_is_f32 ? ln_l2_fwd_kernel<true> : ln_l2_fwd_kernel<false>, blocks,
+                      256, 0, stream, NO_PDL, zz, ldz, ww, bb, eps, M, C, oo, ldo, stats, target, ldt, loss != nullptr))
+    return rc;
+  return colred_finish(1, blocks, 1, loss, nullptr, nullptr, stream);
 }
 
 extern "C" int ivb_ln_l2_bwd(const void* z, long ldz, const void* weight, const void* bias,

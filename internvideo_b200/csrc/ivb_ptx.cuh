@@ -425,6 +425,33 @@ __device__ __forceinline__ float warp_max(float v) {
   for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
   return v;
 }
+// CTA-wide sum (or max) of N values per thread: each warp reduces its values, then every thread gets the warps'
+// results combined in warp-index order, so the result does not depend on warp scheduling.  red holds N floats per warp;
+// the leading __syncthreads() lets a second call reuse it while threads may still read the first call's results.
+template <int N, bool MAX = false>
+__device__ __forceinline__ void block_reduce(float (&v)[N], float* red) {
+  const int nw = blockDim.x >> 5;
+#pragma unroll
+  for (int i = 0; i < N; ++i) v[i] = MAX ? warp_max(v[i]) : warp_sum(v[i]);
+  __syncthreads();
+  if ((threadIdx.x & 31) == 0) {
+#pragma unroll
+    for (int i = 0; i < N; ++i) red[i * nw + (threadIdx.x >> 5)] = v[i];
+  }
+  __syncthreads();
+#pragma unroll
+  for (int i = 0; i < N; ++i) {
+    float r = red[i * nw];
+    for (int k = 1; k < nw; ++k) r = MAX ? fmaxf(r, red[i * nw + k]) : r + red[i * nw + k];
+    v[i] = r;
+  }
+}
+template <bool MAX = false>
+__device__ __forceinline__ float block_reduce(float v, float* red) {
+  float a[1] = {v};
+  block_reduce<1, MAX>(a, red);
+  return a[0];
+}
 // exact-erf GELU (nn.GELU) and its derivative without libm's branchy erff: Abramowitz-Stegun 7.1.26,
 //   erfc(z) = (a1 t + ... + a5 t^5) e^{-z^2},  t = 1/(1 + p z),  z >= 0,  |error| <= 1.5e-7,
 // one MUFU.RCP + one MUFU.EX2 + 8 FMA; the derivative reuses the same exponential (phi(x) ~ e^{-x^2/2}).

@@ -92,6 +92,34 @@ def test_pixel_targets_and_mse(cuda_lib):
     assert _rel(dp, 2 * (pred.float() - lab) / pred.numel()) < 5e-3
 
 
+def test_loss_sums_repeat_bit_for_bit(cuda_lib):
+    """The alignment loss, the contrastive loss, dtemp and the MSE sum their CTAs' partials in a fixed order: two calls
+    on the same inputs, each over hundreds of CTAs, give the same bits."""
+    ll = cuda_lib
+    torch.manual_seed(0)
+    M, C, G, n = 13312, 1408, 1024, 1 << 24
+    z = torch.randn(M, C, device="cuda").to(torch.bfloat16)
+    w = (1 + 0.1 * torch.randn(C, device="cuda")).to(torch.bfloat16)
+    b = (0.1 * torch.randn(C, device="cuda")).to(torch.bfloat16)
+    tgt = torch.nn.functional.normalize(torch.randn(M, C, device="cuda"), dim=-1).to(torch.bfloat16)
+    cosm = torch.nn.functional.normalize(torch.randn(G, 64, device="cuda"), dim=-1)
+    cosm = (cosm @ cosm.t()).contiguous()
+    idx = torch.randint(0, G // 2, (G,), device="cuda")
+    pred = torch.randn(n, device="cuda").to(torch.bfloat16)
+    label = torch.randn(n, device="cuda")
+
+    def scalars():
+        align = torch.zeros(1, device="cuda")
+        ll.ln_l2_fwd(z, w, b, 1e-5, want_out=False, target=tgt, loss_sum=align)
+        vtc, lse_r, lse_c = ll.vtc_loss_fwd(cosm, idx, 0.07)
+        _, dtemp = ll.vtc_loss_bwd(cosm, idx, 0.07, lse_r, lse_c)
+        mse = ll.mse_loss(pred, label, torch.zeros(1, device="cuda"))
+        return torch.cat([align, vtc, dtemp, mse])
+
+    first, second = scalars(), scalars()
+    assert torch.equal(first.view(torch.int32), second.view(torch.int32)), (first.tolist(), second.tolist())
+
+
 def test_adamw_matches_torch(cuda_lib):
     ll = cuda_lib
     torch.manual_seed(0)
