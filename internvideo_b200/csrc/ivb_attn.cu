@@ -15,7 +15,7 @@ template <int KA, int NO, int KS>
 __global__ void __launch_bounds__(ATT_THREADS, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                 const __grid_constant__ CUtensorMap tmV, const AttnFwdParams p) {
-  attn_fwd<KA, NO, KS, false>(tmQ, tmK, tmV, p, nullptr);
+  attn_fwd<AttnElt::BF16, KA, NO, KS>(tmQ, tmK, tmV, p, nullptr);
 }
 
 // rowscale: the attention branch's DropPath factors [B*n]
@@ -23,14 +23,14 @@ template <int KA, int NO, int KS>
 __global__ void __launch_bounds__(ATT_THREADS, 1)
 attn_fwd_plan_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                      const __grid_constant__ CUtensorMap tmV, const AttnFwdParams p, const float* rowscale) {
-  attn_fwd<KA, NO, KS, true>(tmQ, tmK, tmV, p, rowscale);
+  attn_fwd<AttnElt::BF16, KA, NO, KS, true>(tmQ, tmK, tmV, p, rowscale);
 }
 
 template <int KA, int NO, int KS>
 __global__ void __launch_bounds__(ATT_THREADS, 1)
 attn_fwd_causal_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                        const __grid_constant__ CUtensorMap tmV, const AttnFwdParams p) {
-  attn_fwd<KA, NO, KS, false, true>(tmQ, tmK, tmV, p, nullptr);
+  attn_fwd<AttnElt::BF16, KA, NO, KS, false, true>(tmQ, tmK, tmV, p, nullptr);
 }
 
 }  // namespace ivb

@@ -1,5 +1,5 @@
-// ivb_attn.cuh — the pieces the attention forward (ivb_attn_fwd.cuh, instantiated in ivb_attn.cu and
-// ivb_attn_keylen.cu), backward (ivb_attn_bwd.cu) and FP8 forward (ivb_attn_fp8.cu) kernels share: one CTA per
+// ivb_attn.cuh — the pieces the attention forward (ivb_attn_fwd.cuh: bf16 kernels in ivb_attn.cu and
+// ivb_attn_keylen.cu, the E4M3 kernel in ivb_attn_fp8.cu) and backward (ivb_attn_bwd.cu) kernels share: one CTA per
 // (128-row block, head, clip) that streams 64-row tiles of the other operands through a ring.
 #pragma once
 #include <math.h>

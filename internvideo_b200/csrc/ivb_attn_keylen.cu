@@ -12,7 +12,7 @@ template <int KA, int NO, int KS>
 __global__ void __launch_bounds__(ATT_THREADS, 1)
 attn_fwd_keylen_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                        const __grid_constant__ CUtensorMap tmV, const AttnFwdParams p, const int* kv_len) {
-  attn_fwd<KA, NO, KS, false, false, true>(tmQ, tmK, tmV, p, nullptr, kv_len);
+  attn_fwd<AttnElt::BF16, KA, NO, KS, false, false, true>(tmQ, tmK, tmV, p, nullptr, kv_len);
 }
 
 }  // namespace ivb
