@@ -53,6 +53,8 @@ extern "C" {
 #define IVB_EPI_GELU_BWD 4  /* out0(bf16) = acc * gelu'(aux(bf16))                                 */
 
 #define IVB_FLAG_GELU_TANH 1 /* tanh-approx GELU (FA2 FusedMLP) instead of erf (nn.GELU)           */
+/* IVB_FLAG_GELU_QUICK (128, below): QuickGELU x * sigmoid(1.702 x) (OpenAI-CLIP blocks, ViCLIP) instead of erf; for
+   IVB_EPI_BIAS_GELU and IVB_EPI_GELU_BWD, with or without IVB_FLAG_GELU_SAVE_GRAD.  Excludes IVB_FLAG_GELU_TANH.  */
 #define IVB_FLAG_ACCUM 2     /* accumulate into out0                                               */
 #define IVB_FLAG_1CTA 4      /* force the cooperative single-CTA kernel (128-row tiles, both MMA warpgroups on one tile) */
 #define IVB_FLAG_2CTA 8      /* force the CTA-pair kernel (cluster of 2, 256-row tiles, B tile TMA-multicast)     */
@@ -169,6 +171,7 @@ int ivb_gemm_fp8(const void* A, int a_mn_major, long lda, int a_format, const fl
  *   accumulator (m, n) is multiplied by a_scale_inv[m] * b_scale_inv[n] before the epilogue.  A must be E4M3 and both
  *   vectors 8-byte aligned; the flag with IVB_FLAG_2CTA or a null vector is refused.                                              */
 #define IVB_FLAG_FP8_VECTOR_SCALES 64
+#define IVB_FLAG_GELU_QUICK 128   /* QuickGELU in the GELU epilogues (documented beside IVB_FLAG_GELU_TANH) */
 #define IVB_FP8_ROWS_MAX_K 16384
 #define IVB_NORM_FP8_MAX_D 4096
 int ivb_fp8_quantize_rows(const void* x, long ldx, int M, int K, void* out, long ldo, float* row_scale_inv,

@@ -144,6 +144,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float (
   const int half = lane & 1;
   const bool accum = (p.flags & IVB_FLAG_ACCUM) != 0;
   const bool tanh_mode = (p.flags & IVB_FLAG_GELU_TANH) != 0;
+  const bool quick_mode = (p.flags & IVB_FLAG_GELU_QUICK) != 0;
   const bool save_grad = (p.flags & IVB_FLAG_GELU_SAVE_GRAD) != 0;
   // this thread's row, first column (in the tile) and columns inside the matrix in chunk i
   auto row_of = [&](int i) { return row_b0 + 64 * (i % NH); };
@@ -178,7 +179,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float (
         const float4 f = reinterpret_cast<const float4*>(src)[k];
         v[4 * k] = f.x; v[4 * k + 1] = f.y; v[4 * k + 2] = f.z; v[4 * k + 3] = f.w;
       }
-      epilogue_chunk<16>(p, accum, tanh_mode, save_grad, v, in, bias, gamma, row, n0 + col, nvalid);
+      epilogue_chunk<16>(p, accum, tanh_mode, quick_mode, save_grad, v, in, bias, gamma, row, n0 + col, nvalid);
     }
     __syncwarp();
   }
@@ -640,7 +641,7 @@ static bool use_pingpong(int M, int N, int K) {
 static bool g_default_2cta = false;
 
 // Operand rules of the fused epilogue (ivb200.h), shared by both entry points; `fn` names the entry point in messages.
-static int check_epilogue_args(const char* fn, int epilogue, const void* out0, const void* out1, long ld1,
+static int check_epilogue_args(const char* fn, int epilogue, int flags, const void* out0, const void* out1, long ld1,
                                const void* aux, long ldaux, const void* bias, const void* gamma) {
   char msg[128];
   auto fail = [&](const char* what) {
@@ -648,6 +649,8 @@ static int check_epilogue_args(const char* fn, int epilogue, const void* out0, c
     return set_error(msg);
   };
   if (out0 == nullptr) return fail("out0 is null");
+  if ((flags & IVB_FLAG_GELU_TANH) && (flags & IVB_FLAG_GELU_QUICK))
+    return fail("IVB_FLAG_GELU_TANH and IVB_FLAG_GELU_QUICK exclude each other");
   if ((epilogue == IVB_EPI_RESID || epilogue == IVB_EPI_GELU_BWD) && aux == nullptr) return fail("epilogue needs aux");
   // the epilogue reads and writes every operand in 16-byte vectors (epilogue_chunk): each row must start on 16 bytes
   if (out1 != nullptr && (ld1 & 7)) return fail("ld1 must be a multiple of 8 elements");
@@ -745,7 +748,7 @@ static int gemm_bf16(const char* fn, const void* A, int a_mn_major, long lda, co
   };
   if (M <= 0 || N <= 0 || K <= 0) return fail("empty problem");
   if ((N & 7) || (lda & 7) || (ldb & 7) || (ld0 & 7)) return fail("N and leading dimensions must be multiples of 8 elements");
-  if (int rc = check_epilogue_args(fn, epilogue, out0, out1, ld1, aux, ldaux, bias, gamma)) return rc;
+  if (int rc = check_epilogue_args(fn, epilogue, flags, out0, out1, ld1, aux, ldaux, bias, gamma)) return rc;
   if (a_mn_major && !b_mn_major) return fail("(A MN-major, B K-major) unused");
   GemmParams p = make_params(M, N, K, epilogue, flags, out0, ld0, out1, ld1, bias, gamma, aux, ldaux, rowscale);
   const bool force2 = (flags & IVB_FLAG_2CTA) != 0, force1 = (flags & IVB_FLAG_1CTA) != 0;
@@ -809,7 +812,7 @@ static int gemm_fp8(const char* fn, const void* A, int a_mn_major, long lda, int
   if (vec && a_format != IVB_FP8_E4M3) return fail("vector scales need an E4M3 A operand");
   if (vec && ((reinterpret_cast<uintptr_t>(a_scale_inv) | reinterpret_cast<uintptr_t>(b_scale_inv)) & 7))
     return fail("scale vectors must be 8-byte aligned");
-  if (int rc = check_epilogue_args(fn, epilogue, out0, out1, ld1, aux, ldaux, bias, gamma)) return rc;
+  if (int rc = check_epilogue_args(fn, epilogue, flags, out0, out1, ld1, aux, ldaux, bias, gamma)) return rc;
   const bool force1 = (flags & IVB_FLAG_1CTA) != 0, forcepp = (flags & IVB_FLAG_PINGPONG) != 0;
   if (flags & IVB_FLAG_2CTA) return fail("no CTA-pair kernel");
   if (force1 && forcepp) return fail("IVB_FLAG_1CTA and IVB_FLAG_PINGPONG exclude each other");
@@ -871,7 +874,7 @@ extern "C" int ivb_gemm_fp8_wgrad(const void* A_t, long lda, const float* a_scal
   if (misaligned(16, a_scale_inv, b_scale_inv)) return fail("scale vectors must be 16-byte aligned");
   if (epilogue != IVB_EPI_BF16 && epilogue != IVB_EPI_F32) return fail("epilogue must be IVB_EPI_BF16 or IVB_EPI_F32");
   if (flags & ~IVB_FLAG_ACCUM) return fail("the only flag is IVB_FLAG_ACCUM (one kernel form: cooperative, 1 CTA)");
-  if (int rc = check_epilogue_args(fn, epilogue, out0, nullptr, 0, nullptr, 0, nullptr, nullptr)) return rc;
+  if (int rc = check_epilogue_args(fn, epilogue, flags, out0, nullptr, 0, nullptr, 0, nullptr, nullptr)) return rc;
   GemmParams p = make_params(M, N, K, epilogue, flags, out0, ld0, nullptr, 0, nullptr, nullptr, nullptr, 0, nullptr);
   p.a_scale_inv = a_scale_inv;
   p.b_scale_inv = b_scale_inv;

@@ -185,8 +185,8 @@ __device__ __forceinline__ void epilogue_load(const GemmParams& p, bool accum, E
 // v: the W fp32 accumulators of (row, col0 .. col0+W-1), 0 < nvalid <= W of them inside the matrix.  in: what
 // epilogue_load read for them.  bias_bits / gamma_bits: the W bf16 of bias / gamma at col0 (when the GEMM has them).
 template <int W>
-__device__ __forceinline__ void epilogue_chunk(const GemmParams& p, bool accum, bool tanh_mode, bool save_grad,
-                                               float* v, const EpiIn<W>& in, const uint32_t* bias_bits,
+__device__ __forceinline__ void epilogue_chunk(const GemmParams& p, bool accum, bool tanh_mode, bool quick_mode,
+                                               bool save_grad, float* v, const EpiIn<W>& in, const uint32_t* bias_bits,
                                                const uint32_t* gamma_bits, long row, int col0, int nvalid) {
   if (p.bias != nullptr) {
     float bv[W];
@@ -212,7 +212,7 @@ __device__ __forceinline__ void epilogue_chunk(const GemmParams& p, bool accum, 
       store_row_f32<W>(reinterpret_cast<float*>(p.out0) + row * p.ld0 + col0, v, nvalid);
     } break;
     case IVB_EPI_BIAS_GELU: {
-      // NOTE: the erf/tanh choice is hoisted out of the element loops on purpose.  With the branch inside,
+      // NOTE: the erf/tanh/quick choice is hoisted out of the element loops on purpose.  With the branch inside,
       // every element became its own basic block and the MUFU latency chains of the 32 elements could not
       // be interleaved: the epilogue ran at ~8K cycles per 32-column chunk instead of ~1K.
       if (p.out1 != nullptr && save_grad) {
@@ -221,6 +221,13 @@ __device__ __forceinline__ void epilogue_chunk(const GemmParams& p, bool accum, 
         if (tanh_mode) {
 #pragma unroll
           for (int i = 0; i < W; ++i) { dv[i] = gelu_tanh_grad(v[i]); v[i] = gelu_tanh(v[i]); }
+        } else if (quick_mode) {
+#pragma unroll
+          for (int i = 0; i < W; ++i) {
+            const float s = gelu_quick_sig(v[i]);
+            dv[i] = fmaf(1.702f * v[i] * s, 1.0f - s, s);
+            v[i] *= s;
+          }
         } else {
 #pragma unroll
           for (int i = 0; i < W; ++i) {
@@ -237,6 +244,9 @@ __device__ __forceinline__ void epilogue_chunk(const GemmParams& p, bool accum, 
         if (tanh_mode) {
 #pragma unroll
           for (int i = 0; i < W; ++i) v[i] = gelu_tanh(v[i]);
+        } else if (quick_mode) {
+#pragma unroll
+          for (int i = 0; i < W; ++i) v[i] = gelu_quick(v[i]);
         } else {
 #pragma unroll
           for (int i = 0; i < W; ++i) v[i] = gelu_erf(v[i]);
@@ -271,6 +281,9 @@ __device__ __forceinline__ void epilogue_chunk(const GemmParams& p, bool accum, 
       } else if (tanh_mode) {
 #pragma unroll
         for (int i = 0; i < W; ++i) v[i] *= gelu_tanh_grad(hv[i]);
+      } else if (quick_mode) {
+#pragma unroll
+        for (int i = 0; i < W; ++i) v[i] *= gelu_quick_grad(hv[i]);
       } else {
 #pragma unroll
         for (int i = 0; i < W; ++i) v[i] *= gelu_erf_grad(hv[i]);

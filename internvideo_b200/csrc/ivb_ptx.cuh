@@ -497,5 +497,26 @@ __device__ __forceinline__ float gelu_tanh_grad(float x) {
   const float du = 0.7978845608028654f * (1.0f + 3.0f * 0.044715f * x2);
   return 0.5f * (1.0f + t) + 0.5f * x * (1.0f - t * t) * du;
 }
+// QuickGELU (OpenAI CLIP): gelu_quick(x) = x s, gelu_quick_grad(x) = s + 1.702 x s (1 - s), s = sigmoid(1.702 x) =
+// 1 / (1 + e^{-1.702 x}): one MUFU.EX2 and one MUFU.RCP, shared by the value and the derivative (gelu_quick_sig).
+// Domain (pinned by tests/test_gemm_quickgelu_gpu.py::test_gelu_quick_every_bf16_value):
+//   - s is finite for every x.  Below x = -51.3 the denominator 1 + e^{-1.702 x} passes 2^126 (and overflows to +inf
+//     further out), where the fast divide gives 0, so both functions return 0 there; the exact values are below 1e-36.
+//     For large positive x, s = 1.  gelu_quick is finite for every finite x; gelu_quick_grad is finite for |x| < 2^127
+//     and NaN above about 2e38, where 1.702 x overflows and inf * 0 is formed.  Live activations are many orders of
+//     magnitude below that; a guard would cost an instruction per element.
+//   - error: ex2.approx and rcp.approx each carry a relative error of about 2^-22, so s has a relative error of a few
+//     2^-23 and gelu_quick a relative error of a few 2^-23 wherever it is normal; gelu_quick_grad has an ABSOLUTE error
+//     of a few 2^-23 (it sums s and a term of opposite sign near x = -1.28, where it crosses 0).  Far below half a bf16
+//     ulp (2^-9), the precision of what the epilogue stores.
+//   - NaN in gives NaN out; subnormal inputs and results flush to zero (the library builds with --use_fast_math).
+__device__ __forceinline__ float gelu_quick_sig(float x) {
+  return __fdividef(1.0f, 1.0f + exp2f(-1.702f * 1.4426950408889634f * x));
+}
+__device__ __forceinline__ float gelu_quick(float x) { return x * gelu_quick_sig(x); }
+__device__ __forceinline__ float gelu_quick_grad(float x) {
+  const float s = gelu_quick_sig(x);
+  return fmaf(1.702f * x * s, 1.0f - s, s);
+}
 
 }  // namespace ivb

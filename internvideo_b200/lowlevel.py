@@ -12,6 +12,7 @@ from . import _lib
 
 EPI_BF16, EPI_F32, EPI_BIAS_GELU, EPI_RESID, EPI_GELU_BWD = 0, 1, 2, 3, 4
 FLAG_GELU_TANH, FLAG_ACCUM, FLAG_1CTA, FLAG_2CTA, FLAG_GELU_SAVE_GRAD, FLAG_PINGPONG = 1, 2, 4, 8, 16, 32
+FLAG_GELU_QUICK = 128      # QuickGELU x * sigmoid(1.702 x) in the GELU epilogues (excludes FLAG_GELU_TANH)
 FLAG_FP8_VECTOR_SCALES = 64
 
 bf16 = torch.bfloat16

@@ -206,7 +206,9 @@ class BlockSpec(NamedTuple):
     only).  checkpoint: BlockFn keeps only the block input and recomputes the forward in the backward.  attn_fp8: the
     token-axis attention runs on the FP8 tensor cores (lowlevel._attn_fp8_pack + _attn_fwd_fp8; inference only:
     block_forward refuses it with save=True or head_axis).  causal: token-axis attention masks every key after its
-    query (the MobileCLIP text tower; block_forward refuses it with head_axis, attn_fp8 or a DropPath plan)."""
+    query (the MobileCLIP text tower; block_forward refuses it with head_axis, attn_fp8 or a DropPath plan).
+    gelu_quick: the MLP's activation is QuickGELU, x * sigmoid(1.702 x) (OpenAI-CLIP blocks: ViCLIP), instead of the
+    erf GELU; it excludes gelu_tanh."""
     B: int
     n: int
     H: int
@@ -220,13 +222,17 @@ class BlockSpec(NamedTuple):
     precision: object = BF16
     attn_fp8: bool = False
     causal: bool = False
+    gelu_quick: bool = False
 
     def attn_scale(self, d):
         return d ** -0.5 if self.scale is None else self.scale
 
     def gelu_flags(self, save):
         """fc1's epilogue flags; with save, h holds gelu'(pre-activation), the only thing the backward needs of it."""
-        return (ll.FLAG_GELU_TANH if self.gelu_tanh else 0) | (ll.FLAG_GELU_SAVE_GRAD if save else 0)
+        if self.gelu_tanh and self.gelu_quick:
+            raise ll._lib.IvbError("BlockSpec: gelu_tanh and gelu_quick exclude each other")
+        return ((ll.FLAG_GELU_TANH if self.gelu_tanh else 0) | (ll.FLAG_GELU_QUICK if self.gelu_quick else 0)
+                | (ll.FLAG_GELU_SAVE_GRAD if save else 0))
 
 
 # A block's tensors.  qkvb, qnw / knw (q/k norms) and g1 / g2 (LayerScale) may be None; n1b / n2b are the LayerNorm
