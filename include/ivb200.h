@@ -23,7 +23,7 @@
  *   - there is no CPU fallback: without a CUDA device of compute capability 9.0 every compute
  *     entry point returns an error.
  *   - parameter gradients (ivb_norm_bwd, ivb_rmsnorm_pair_bwd, ivb_rmsnorm_bwd_layerscale, ivb_layerscale_bwd,
- *     ivb_colsum_bf16, ivb_ln_l2_bwd), the losses (ivb_ln_l2_fwd with a target, ivb_vtc_loss_fwd, ivb_mse_loss) and
+ *     ivb_colsum_bf16, ivb_ln_l2_bwd, ivb_prenorm_wgrad), the losses (ivb_ln_l2_fwd with a target, ivb_vtc_loss_fwd, ivb_mse_loss) and
  *     dtemp (ivb_vtc_loss_bwd) are summed in a fixed order through a per-device scratch of the library, so the same
  *     inputs give the same bits on every run.  That scratch holds one reduction at a time: these entry points must
  *     not be called concurrently from two streams of the same device (the package runs them on one compute stream).
@@ -392,6 +392,22 @@ int ivb_visible_indices(const void* mask_u8, int B, int N, int n_keep, int* idx,
 int ivb_im2col_visible(const void* video, const int* idx, int idx_stride, int j0, int rows_per_clip,
                        int B, int C, int T, int H, int W, int tubelet, int patch, int Kpad,
                        void* cols, void* stream);
+/* ivb_im2col_visible's rows, each normalised by the RMSNorm that InternVideo-Next's patch embed applies to a patch's
+ * K = C*t*p*p pixels before the Conv3d (`norm_before`, InternVideo_next.py:302-342): per row
+ * r = rsqrt(mean_k a_k^2 + eps) in fp32, cols[row, k] = bf16(weight[pi(k)] * bf16(a_k * r)), zeros for K <= k < Kpad,
+ * and rstd[row] = r (fp32 [B*rows_per_clip], for ivb_prenorm_wgrad).  weight: bf16 [K] in the reference's
+ * (t hp wp c) order; pi maps the column (c, dt, dy, dx) to ((dt*p + dy)*p + dx)*C + c.  Kpad <= 1536; video, idx,
+ * cols and rstd 4-byte aligned, weight 2-byte aligned.                                                              */
+int ivb_im2col_prenorm(const void* video, const int* idx, int idx_stride, int j0, int rows_per_clip, int B, int C,
+                       int T, int H, int W, int tubelet, int patch, int Kpad, const void* weight, float eps, void* cols,
+                       float* rstd, void* stream);
+/* Weight gradient of that RMSNorm: dweight[pi(k)] += sum over rows of dcols[row, k] * bf16(a_k * rstd[row]) (fp32 [K]),
+ * the normalised pixels recomputed from the video and ivb_im2col_prenorm's rstd; summed in a fixed order (see
+ * Conventions).  dcols: bf16 [B*rows_per_clip, lddc], the gradient of the im2col rows (lddc a multiple of 8, >= Kpad).
+ * Same row selection and limits as ivb_im2col_prenorm; dcols and dweight 4-byte aligned.                          */
+int ivb_prenorm_wgrad(const void* video, const int* idx, int idx_stride, int j0, int rows_per_clip, int B, int C,
+                      int T, int H, int W, int tubelet, int patch, int Kpad, const float* rstd, const void* dcols,
+                      long lddc, float* dweight, void* stream);
 /* out[b,j,:] = src[b*src_bstride + j*D + :] (fp32, optional) + table[idx[b*idx_bstride + j] + idx_off]
  * (bf16 table, optional; idx NULL means j).  cls/pos-embed adds :635-656, decoder pos adds :712-737. */
 int ivb_gather_add(const float* src, long src_bstride, const void* table, const int* idx,

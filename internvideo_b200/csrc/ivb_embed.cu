@@ -8,6 +8,8 @@
 //   * the scatter-add backward of those gathers
 //   * the token embedding of the MobileCLIP text tower (text_encoder.py:131-147) and its backward, whose table gradient
 //     sums each id's rows in a fixed order through a device counting sort of the positions by id.
+#include <cstdio>
+
 #include "ivb_internal.h"
 #include "ivb_ptx.cuh"
 #include "ivb_rows.cuh"
@@ -77,6 +79,151 @@ __global__ void im2col_visible_kernel(const __nv_bfloat16* __restrict__ video, c
     dst[u] = val;
   }
   (void)halfP;
+}
+
+// ------------------------------------------------------------------ pre-norm im2col (dual-RMSNorm patch embed)
+// InternVideo-Next's PatchEmbed (InternVideo_next.py:302-342) applies an RMSNorm (`norm_before`) to each patch's
+// K = C*t*p*p raw pixels before the Conv3d.  Its weight is indexed in the reference's `(t hp wp c)` order, so the
+// column (c, dt, dy, dx) of a row meets weight element pi(c, dt, dy, dx) = ((dt*p + dy)*p + dx)*C + c.  A warp holds
+// its row's pixels in registers (word u = lane + 32 i, two pixels per word), so each pixel is read from HBM once.
+constexpr int PRENORM_MAX_KPAD = 1536;
+constexpr int PRENORM_NU = PRENORM_MAX_KPAD / 64;     // 2-pixel words per lane
+
+struct PatchRow {
+  int b, f, py, px;
+};
+
+__device__ __forceinline__ PatchRow patch_row(const int* idx, int idx_stride, int j0, int rows_per_clip, long row,
+                                              int H, int W, int P) {
+  const int b = static_cast<int>(row / rows_per_clip);
+  const int j = static_cast<int>(row % rows_per_clip);
+  const int tok = idx[static_cast<long>(b) * idx_stride + j0 + j] - 1;
+  const int gw = W / P, gh = H / P;
+  return {b, tok / (gh * gw), (tok / gw) % gh, tok % gw};
+}
+
+// Video element of column e (even: dx and dx + 1 share one 4-byte word) and pi(e); pi(e + 1) = pi(e) + C.
+__device__ __forceinline__ long prenorm_col(const PatchRow& r, int e, int C, int T, int H, int W, int tub, int P,
+                                            int* wi) {
+  const int dx = e % P;
+  int rest = e / P;
+  const int dy = rest % P; rest /= P;
+  const int dt = rest % tub;
+  const int c = rest / tub;
+  *wi = ((dt * P + dy) * P + dx) * C + c;
+  return (((static_cast<long>(r.b) * C + c) * T + (r.f * tub + dt)) * H + (r.py * P + dy)) * W + (r.px * P + dx);
+}
+
+__device__ __forceinline__ float bf16_round(float x) { return __bfloat162float(__float2bfloat16_rn(x)); }
+
+// Loads the row's pixel words into v (zero past K) and returns r = rsqrt(mean a^2 + eps), the same in every lane
+// (a butterfly sum: the same bits on every run).
+__device__ __forceinline__ float prenorm_load(const uint32_t* vid32, const PatchRow& pr, int C, int T, int H, int W,
+                                              int tub, int P, int K, float eps, int lane, uint32_t v[PRENORM_NU]) {
+  float ss = 0.f;
+#pragma unroll
+  for (int i = 0; i < PRENORM_NU; ++i) {
+    const int e = (lane + 32 * i) * 2;
+    v[i] = 0u;
+    if (e < K) {
+      int wi;
+      v[i] = vid32[prenorm_col(pr, e, C, T, H, W, tub, P, &wi) >> 1];
+      const float2 a = unpack_bf16(v[i]);
+      ss = fmaf(a.x, a.x, fmaf(a.y, a.y, ss));
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
+  return rsqrtf(ss / static_cast<float>(K) + eps);
+}
+
+// cols[row, e] = bf16(w[pi(e)] * bf16(a_e * r)), zero for K <= e < Kpad; rstd[row] = r.  Rows as im2col_visible_kernel.
+__global__ void im2col_prenorm_kernel(const __nv_bfloat16* __restrict__ video, const int* __restrict__ idx,
+                                      int idx_stride, int j0, int rows_per_clip, int B, int C, int T, int H, int W,
+                                      int tub, int P, int Kpad, const __nv_bfloat16* __restrict__ weight, float eps,
+                                      __nv_bfloat16* __restrict__ cols, float* __restrict__ rstd) {
+  const long row = static_cast<long>(blockIdx.x) * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  if (row >= static_cast<long>(B) * rows_per_clip) return;
+  const PatchRow pr = patch_row(idx, idx_stride, j0, rows_per_clip, row, H, W, P);
+  const int K = C * tub * P * P;
+  uint32_t v[PRENORM_NU];
+  const float r = prenorm_load(reinterpret_cast<const uint32_t*>(video), pr, C, T, H, W, tub, P, K, eps, lane, v);
+  uint32_t* dst = reinterpret_cast<uint32_t*>(cols + row * Kpad);
+#pragma unroll
+  for (int i = 0; i < PRENORM_NU; ++i) {
+    const int u = lane + 32 * i;
+    if (u >= (Kpad >> 1)) break;
+    uint32_t val = 0u;
+    if (2 * u < K) {
+      int wi;
+      prenorm_col(pr, 2 * u, C, T, H, W, tub, P, &wi);
+      const float2 a = unpack_bf16(v[i]);
+      val = pack_bf16(__bfloat162float(weight[wi]) * bf16_round(a.x * r),
+                      __bfloat162float(weight[wi + C]) * bf16_round(a.y * r));
+    }
+    dst[u] = val;
+  }
+  if (lane == 0) rstd[row] = r;
+}
+
+// Weight gradient of norm_before: dw[pi(e)] = sum over rows of dcols[row, e] * bf16(a_e * rstd[row]), the normalised
+// pixels recomputed from the video (cols cannot give them back: w may hold zeros).  CTA c takes rows
+// [c * PRENORM_WG_ROWS, (c + 1) * PRENORM_WG_ROWS); warp k of it adds rows k, k + 8, ... in order in registers, the
+// warps are added in warp order, and the CTA's K sums go to slot c of the fixed-order column scratch (ivb_colred.cuh),
+// whose slots the host then adds in slot order.
+constexpr int PRENORM_WG_WARPS = 8, PRENORM_WG_ROWS = 128;
+
+__global__ void __launch_bounds__(PRENORM_WG_WARPS * 32)
+    prenorm_wgrad_kernel(const __nv_bfloat16* __restrict__ video, const int* __restrict__ idx, int idx_stride, int j0,
+                         int rows_per_clip, int B, int C, int T, int H, int W, int tub, int P, int Kpad,
+                         const float* __restrict__ rstd, const __nv_bfloat16* __restrict__ dcols, long lddc,
+                         float* __restrict__ slots) {
+  extern __shared__ float part[];      // [warp][Kpad]
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int K = C * tub * P * P;
+  const long total = static_cast<long>(B) * rows_per_clip;
+  const long r0 = static_cast<long>(blockIdx.x) * PRENORM_WG_ROWS;
+  const long r1 = min(total, r0 + PRENORM_WG_ROWS);
+  const uint32_t* vid32 = reinterpret_cast<const uint32_t*>(video);
+  float acc[2 * PRENORM_NU];
+#pragma unroll
+  for (int i = 0; i < 2 * PRENORM_NU; ++i) acc[i] = 0.f;
+  for (long row = r0 + warp; row < r1; row += PRENORM_WG_WARPS) {
+    const PatchRow pr = patch_row(idx, idx_stride, j0, rows_per_clip, row, H, W, P);
+    const float r = rstd[row];
+    const uint32_t* dc = reinterpret_cast<const uint32_t*>(dcols + row * lddc);
+#pragma unroll
+    for (int i = 0; i < PRENORM_NU; ++i) {
+      const int e = (lane + 32 * i) * 2;
+      if (e < K) {
+        int wi;
+        const float2 a = unpack_bf16(vid32[prenorm_col(pr, e, C, T, H, W, tub, P, &wi) >> 1]);
+        const float2 g = unpack_bf16(dc[lane + 32 * i]);
+        acc[2 * i] = fmaf(g.x, bf16_round(a.x * r), acc[2 * i]);
+        acc[2 * i + 1] = fmaf(g.y, bf16_round(a.y * r), acc[2 * i + 1]);
+      }
+    }
+  }
+  float* mine = part + static_cast<long>(warp) * Kpad;
+#pragma unroll
+  for (int i = 0; i < PRENORM_NU; ++i) {
+    const int e = (lane + 32 * i) * 2;
+    if (e < K) {
+      mine[e] = acc[2 * i];
+      mine[e + 1] = acc[2 * i + 1];
+    }
+  }
+  __syncthreads();
+  for (int e = threadIdx.x; e < K; e += blockDim.x) {
+    float s = 0.f;
+    for (int k = 0; k < PRENORM_WG_WARPS; ++k) s += part[static_cast<long>(k) * Kpad + e];
+    const int dx = e % P;
+    int rest = e / P;
+    const int dy = rest % P; rest /= P;
+    const int dt = rest % tub;
+    slots[static_cast<long>(blockIdx.x) * K + ((dt * P + dy) * P + dx) * C + rest / tub] = s;
+  }
 }
 
 // out[b, j, :] = (src ? src[b*src_bstride + j*D ..] : 0) + (table ? table[(idx[b*idx_bstride + j] + idx_off) * D ..] : 0)
@@ -280,6 +427,64 @@ extern "C" int ivb_im2col_visible(const void* video, const int* idx, int idx_str
   return launch("im2col_visible_kernel", im2col_visible_kernel, (unsigned)((rows + wpb - 1) / wpb), wpb * 32, 0, stream,
                 NO_PDL, reinterpret_cast<const __nv_bfloat16*>(video), idx, idx_stride, j0, rows_per_clip, B, C, T, H, W,
                 tubelet, patch, Kpad, reinterpret_cast<__nv_bfloat16*>(cols));
+}
+
+// The operand rules the two pre-norm entry points share; fn names the entry point in messages.
+static int check_prenorm(const char* fn, const void* video, const int* idx, int C, int W, int tubelet, int patch,
+                         int Kpad, const float* rstd) {
+  char msg[160];
+  const char* what = nullptr;
+  if (C <= 0 || tubelet <= 0 || patch <= 0 || (patch & 1) || (W & 1))
+    what = "C, tubelet and patch must be positive, patch and W even";
+  else if ((Kpad & 7) || Kpad < C * tubelet * patch * patch || Kpad > PRENORM_MAX_KPAD)
+    what = "Kpad must be a multiple of 8, >= C*t*p*p and <= 1536";
+  else if (video == nullptr || idx == nullptr || rstd == nullptr)
+    what = "video, idx and rstd must not be null";
+  else if (misaligned(4, video, idx, rstd))
+    what = "video, idx and rstd must be 4-byte aligned";
+  if (what == nullptr) return 0;
+  snprintf(msg, sizeof(msg), "%s: %s", fn, what);
+  return set_error(msg);
+}
+
+extern "C" int ivb_im2col_prenorm(const void* video, const int* idx, int idx_stride, int j0, int rows_per_clip, int B,
+                                  int C, int T, int H, int W, int tubelet, int patch, int Kpad, const void* weight,
+                                  float eps, void* cols, float* rstd, void* stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  if (B <= 0 || rows_per_clip <= 0) return 0;
+  if (int rc = check_prenorm("ivb_im2col_prenorm", video, idx, C, W, tubelet, patch, Kpad, rstd)) return rc;
+  if (weight == nullptr || cols == nullptr) return set_error("ivb_im2col_prenorm: weight and cols must not be null");
+  if (misaligned(4, cols) || misaligned(2, weight))
+    return set_error("ivb_im2col_prenorm: cols must be 4-byte and weight 2-byte aligned");
+  const long rows = static_cast<long>(B) * rows_per_clip;
+  const int wpb = 8;
+  return launch("im2col_prenorm_kernel", im2col_prenorm_kernel, (unsigned)((rows + wpb - 1) / wpb), wpb * 32, 0,
+                stream, NO_PDL, reinterpret_cast<const __nv_bfloat16*>(video), idx, idx_stride, j0, rows_per_clip, B, C,
+                T, H, W, tubelet, patch, Kpad, reinterpret_cast<const __nv_bfloat16*>(weight), eps,
+                reinterpret_cast<__nv_bfloat16*>(cols), rstd);
+}
+
+extern "C" int ivb_prenorm_wgrad(const void* video, const int* idx, int idx_stride, int j0, int rows_per_clip, int B,
+                                 int C, int T, int H, int W, int tubelet, int patch, int Kpad, const float* rstd,
+                                 const void* dcols, long lddc, float* dweight, void* stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  if (B <= 0 || rows_per_clip <= 0) return 0;
+  if (int rc = check_prenorm("ivb_prenorm_wgrad", video, idx, C, W, tubelet, patch, Kpad, rstd)) return rc;
+  if (dcols == nullptr || dweight == nullptr) return set_error("ivb_prenorm_wgrad: dcols and dweight must not be null");
+  if ((lddc & 7) || lddc < Kpad) return set_error("ivb_prenorm_wgrad: lddc must be a multiple of 8 and >= Kpad");
+  if (misaligned(4, dcols, dweight)) return set_error("ivb_prenorm_wgrad: dcols and dweight must be 4-byte aligned");
+  const int K = C * tubelet * patch * patch;
+  const long rows = static_cast<long>(B) * rows_per_clip;
+  const long nslots = (rows + PRENORM_WG_ROWS - 1) / PRENORM_WG_ROWS;
+  float* slots = colred_cols(nslots, K, "ivb_prenorm_wgrad: gradient scratch too small");
+  if (slots == nullptr) return 1;
+  const size_t smem = static_cast<size_t>(PRENORM_WG_WARPS) * Kpad * sizeof(float);
+  if (int rc = launch("prenorm_wgrad_kernel", prenorm_wgrad_kernel, (unsigned)nslots, PRENORM_WG_WARPS * 32, smem,
+                      stream, NO_PDL, reinterpret_cast<const __nv_bfloat16*>(video), idx, idx_stride, j0,
+                      rows_per_clip, B, C, T, H, W, tubelet, patch, Kpad, rstd,
+                      reinterpret_cast<const __nv_bfloat16*>(dcols), lddc, slots))
+    return rc;
+  return colred_cols_finish(static_cast<int>(nslots), K, dweight, stream);
 }
 
 extern "C" int ivb_gather_add(const float* src, long src_bstride, const void* table, const int* idx,

@@ -46,6 +46,11 @@ inline int persistent_grid(long rows, int rows_per_cta, int per_sm) {
 // scalar_slots returns null, with `who` as the error text, when n slots do not fit or the address cannot be read.
 float* scalar_slots(long n, const char* who);
 int scalar_finish(int n, float* dst, cudaStream_t stream);
+// The same scratch for column sums of another translation unit (ivb_embed.cu): colred_cols(n, D) is the base of n
+// partial rows of D fp32 (slot s at s * D; null as scalar_slots), and colred_cols_finish(n, D, dst) adds slots [0, n)
+// in slot order into dst[0, D).
+float* colred_cols(long n, int D, const char* who);
+int colred_cols_finish(int n, int D, float* dst, cudaStream_t stream);
 
 // Programmatic dependent launch (PDL) is opt-in: pdl_enabled() is true only when IVB_PDL is set to a non-zero value.
 // A PDL-launched kernel may be scheduled while the previous kernel of the stream is still draining, so it must execute

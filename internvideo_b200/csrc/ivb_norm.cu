@@ -944,6 +944,14 @@ int scalar_finish(int n, float* dst, cudaStream_t stream) {
   return colred_finish(1, n, 1, dst, nullptr, nullptr, stream);
 }
 
+float* colred_cols(long n, int D, const char* who) {
+  return scalar_slots(n * D, who);
+}
+
+int colred_cols_finish(int n, int D, float* dst, cudaStream_t stream) {
+  return colred_finish(1, n, D, dst, nullptr, nullptr, stream);
+}
+
 }  // namespace ivb
 
 using namespace ivb;

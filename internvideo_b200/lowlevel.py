@@ -584,6 +584,35 @@ def im2col_visible(video, idx, j0, rows_per_clip, tubelet, patch, kpad):
     return cols
 
 
+def _im2col_prenorm(video, idx, j0, rows_per_clip, tubelet, patch, kpad, weight, eps=1e-6):
+    """im2col_visible's rows through the patch embed's pre-conv RMSNorm (ivb_im2col_prenorm): weight bf16 [C*t*p*p] in
+    the reference's (t hp wp c) order.  Returns (cols bf16 [B*rows_per_clip, kpad], rstd fp32 [B*rows_per_clip])."""
+    _chk(("video", video, bf16), ("idx", idx, i32), ("weight", weight, bf16))
+    if not video.is_contiguous():
+        raise _lib.IvbError("im2col_prenorm: video must be contiguous [B,C,T,H,W]")
+    B, C, T, H, W = video.shape
+    cols = torch.empty((B * rows_per_clip, kpad), device=video.device, dtype=bf16)
+    rstd = torch.empty((B * rows_per_clip,), device=video.device, dtype=f32)
+    _call("im2col_prenorm", video, idx, idx.stride(0), j0, rows_per_clip, B, C, T, H, W, tubelet, patch, kpad, weight,
+          float(eps), cols, rstd)
+    return cols, rstd
+
+
+def _prenorm_wgrad(video, idx, j0, rows_per_clip, tubelet, patch, kpad, rstd, dcols, dweight=None):
+    """Weight gradient of im2col_prenorm's RMSNorm from dcols bf16 [B*rows_per_clip, >=kpad], the gradient of its rows
+    (ivb_prenorm_wgrad, fixed order).  dweight: optional fp32 [C*t*p*p] accumulator.  Returns dweight."""
+    _chk(("video", video, bf16), ("idx", idx, i32), ("rstd", rstd, f32), ("dcols", dcols, bf16),
+         ("dweight?", dweight, f32))
+    if not video.is_contiguous():
+        raise _lib.IvbError("prenorm_wgrad: video must be contiguous [B,C,T,H,W]")
+    B, C, T, H, W = video.shape
+    if dweight is None:
+        dweight = torch.zeros((C * tubelet * patch * patch,), device=video.device, dtype=f32)
+    _call("prenorm_wgrad", video, idx, idx.stride(0), j0, rows_per_clip, B, C, T, H, W, tubelet, patch, kpad, rstd,
+          dcols, _rows2d(dcols, "dcols"), dweight)
+    return dweight
+
+
 def gather_add(src, src_bstride, table, idx, idx_bstride, idx_off, B, rows, D, out, out_bstride):
     _chk(("src?", src, f32), ("table?", table, bf16), ("idx?", idx, i32), ("out", out, (f32, bf16)))
     _call("gather_add", src, src_bstride, table, idx, idx_bstride, idx_off, B, rows, D, out, int(out.dtype == f32),

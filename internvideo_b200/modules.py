@@ -38,8 +38,9 @@ def _sincos_1d(dim, pos):
     return np.concatenate([np.sin(out), np.cos(out)], axis=1)
 
 
-def get_3d_sincos_pos_embed(embed_dim, grid_size, t_size, cls_token=False):
-    """Same table as models/pos_embed.py:9-54 (3/4 of the channels spatial, 1/4 temporal)."""
+def get_3d_sincos_pos_embed(embed_dim, grid_size, t_size, cls_token=False, cls_token_num=1):
+    """Same table as models/pos_embed.py:9-54 (3/4 of the channels spatial, 1/4 temporal), behind cls_token_num zero
+    rows with cls_token (InternVideo-Next/models/pos_embed.py:9-54)."""
     assert embed_dim % 4 == 0
     ds, dt = embed_dim // 4 * 3, embed_dim // 4
     gh = np.arange(grid_size, dtype=np.float32)
@@ -53,7 +54,7 @@ def get_3d_sincos_pos_embed(embed_dim, grid_size, t_size, cls_token=False):
     pos_s = np.repeat(pos_s[np.newaxis, :, :], t_size, axis=0)
     pe = np.concatenate([pos_t, pos_s], axis=-1).reshape([-1, embed_dim])
     if cls_token:
-        pe = np.concatenate([np.zeros([1, embed_dim]), pe], axis=0)
+        pe = np.concatenate([np.zeros([cls_token_num, embed_dim]), pe], axis=0)
     return pe
 
 
@@ -118,16 +119,20 @@ def embed_tokens(patch_embed, x, idx, cls_token, table):
     im2col + wgmma GEMM, plus their rows of the position table, behind `cls_token + table[0]`.  x: video [B,C,T,H,W];
     idx: int32 [B, n], column 0 the cls slot.  Returns the fp32 residual stream [B*n, D].
     cls_token None (towers without one): `table` holds the patch rows only; EmbedFn gets a zero cls token and a zero
-    table row, and the cls row is dropped again, giving [B*(n-1), D]."""
+    table row, and the cls row is dropped again, giving [B*(n-1), D].  A cls_token [1, k, D] puts k cls rows in front
+    (the stream is then [B*(k+n-1), D]), and a patch embed with `norm_before` (InternVideo-Next's dual-RMSNorm
+    PatchEmbed) runs its two norms inside EmbedFn."""
     tubelet, patch, _ = patch_embed.proj.kernel_size
     w, b = patch_embed.proj.weight, patch_embed.proj.bias
+    nb = getattr(patch_embed, "norm_before", None)
+    norms = () if nb is None else (patch_embed.norm.weight, nb.weight, nb.variance_epsilon)
     if cls_token is not None:
-        return ops.EmbedFn.apply(x.to(bf16), idx, w, b, cls_token, table, tubelet, patch)
+        return ops.EmbedFn.apply(x.to(bf16), idx, w, b, cls_token, table, tubelet, patch, cls_token.shape[1], *norms)
     B, n = idx.shape
     D = w.shape[0]
     table = torch.cat([table.new_zeros(1, 1, D), table], 1).to(bf16)
     zcls = torch.zeros((1, 1, D), device=x.device, dtype=bf16)
-    h = ops.EmbedFn.apply(x.to(bf16), idx, w, b, zcls, table, tubelet, patch)
+    h = ops.EmbedFn.apply(x.to(bf16), idx, w, b, zcls, table, tubelet, patch, 1, *norms)
     return h.reshape(B, n, D)[:, 1:].reshape(B * (n - 1), D)
 
 
@@ -739,31 +744,36 @@ class InternVideo2Tower(nn.Module):
     """What the InternVideo2 towers share (the student, the stage-2 tower and the CLIP tower): `patch_embed`,
     `cls_token`, the position tables of `pos_prefixes` ('' for the blocks, 'clip_' / 'mae_' for the decoders; joint,
     or spatial / temporal / cls with sep_pos_embed), `blocks` and `clip_projector`, registered in this order.
-    A subclass registers its heads and then calls init_tower(), so the init draws follow every constructor draw."""
+    A subclass registers its heads and then calls init_tower(), so the init draws follow every constructor draw.
+    cls_token_num: the number of cls tokens (InternVideo-Next: 4), each with its own zero row in front of the joint
+    tables; patch_embed_layer: the patch embed's class."""
 
     pos_prefixes = ("",)
+    patch_embed_layer = PatchEmbed
     sep_image_video_pos_embed = False
 
     def __init__(self, in_chans, patch_size, img_size, qkv_bias, drop_path_rate, embed_dim, num_heads, mlp_ratio,
                  init_values, qk_normalization, depth, use_flash_attn, use_fused_rmsnorm, use_fused_mlp,
                  fused_mlp_heuristic, attn_pool_num_heads, clip_embed_dim, layerscale_no_force_fp32, num_frames,
-                 tubelet_size, sep_pos_embed, use_checkpoint, checkpoint_num):
+                 tubelet_size, sep_pos_embed, use_checkpoint, checkpoint_num, cls_token_num=1):
         super().__init__()
         assert use_flash_attn == use_fused_rmsnorm == use_fused_mlp, \
             "use_flash_attn, use_fused_rmsnorm and use_fused_mlp should be consistent"
         self.use_flash_attn = use_flash_attn
         self.embed_dim = embed_dim
         self.depth = depth
-        self.patch_embed = PatchEmbed(img_size, patch_size, in_chans, embed_dim, num_frames=num_frames,
-                                      tubelet_size=tubelet_size)
-        self.cls_token = nn.Parameter(torch.zeros(1, 1, embed_dim))
+        self.patch_embed = self.patch_embed_layer(img_size, patch_size, in_chans, embed_dim, num_frames=num_frames,
+                                                  tubelet_size=tubelet_size)
+        self.cls_token_num = cls_token_num
+        self.cls_token = nn.Parameter(torch.zeros(1, cls_token_num, embed_dim))
         self.sep_pos_embed = bool(sep_pos_embed)
         gs = self.grid_size = self.patch_embed.grid_size
         self.image_pos_groups = gs[0]        # an image's joint table: the mean over these groups of the video table
         Z = lambda *shape: nn.Parameter(torch.zeros(*shape))  # noqa: E731
         for pre in self.pos_prefixes:        # :481-493 — a table (set) per consumer; the MAE decoder's has no cls row
             if not self.sep_pos_embed:
-                setattr(self, pre + "pos_embed", Z(1, self.patch_embed.num_patches + (pre != "mae_"), embed_dim))
+                setattr(self, pre + "pos_embed", Z(1, self.patch_embed.num_patches + (pre != "mae_") * cls_token_num,
+                                                   embed_dim))
                 continue
             setattr(self, pre + "pos_embed_spatial", Z(1, gs[1] * gs[2], embed_dim))
             setattr(self, pre + "pos_embed_temporal", Z(1, gs[0], embed_dim))
@@ -791,7 +801,7 @@ class InternVideo2Tower(nn.Module):
                 getattr(self, pre + "pos_embed_spatial").data.copy_(sp)
                 getattr(self, pre + "pos_embed_temporal").data.copy_(tp)
             return
-        t = _pos_tensor(get_3d_sincos_pos_embed(D, gs[1], gs[0], cls_token=True))
+        t = _pos_tensor(get_3d_sincos_pos_embed(D, gs[1], gs[0], cls_token=True, cls_token_num=self.cls_token_num))
         for pre in self.pos_prefixes:
             pe = getattr(self, pre + "pos_embed")
             pe.data.copy_(t[:, -pe.shape[1]:])

@@ -566,41 +566,74 @@ class EmbedFn(torch.autograd.Function):
     Embeds only the kept patches (the reference convolves all T*L patches and drops 80 %); token
     order is the bit-exact `x[~mask]` order given by `idx` (ivb_visible_indices).
     Returns the fp32 residual stream [B*n, D].
+
+    idx: int32 [B, 1 + m], column 0 the cls slot, then the m patch tokens.  ncls: the number k of cls rows in front of
+    the patch rows (InternVideo-Next has 4): row i < k is cls[i] + pos[i], and a patch token t >= 1 takes position row
+    t + k - 1, so n = k + m.  norm_w / norm_before_w: the RMSNorm weights of InternVideo-Next's dual-norm patch embed
+    (InternVideo_next.py:302-342), eps their eps: the patch's pixels go through norm_before inside the im2col
+    (ivb_im2col_prenorm), the bf16 conv output through norm (ivb_norm_fwd).  With k = 1 and no norms the calls are the
+    single-cls ones of every other tower.
     """
 
     @staticmethod
-    def forward(ctx, video, idx, w, b, cls, pos, tubelet, patch):
+    def forward(ctx, video, idx, w, b, cls, pos, tubelet, patch, ncls=1, norm_w=None, norm_before_w=None, eps=1e-6):
         B, C, T, H, W = video.shape
-        n = idx.shape[1]
+        ni = idx.shape[1]
+        m, k = ni - 1, ncls
+        n = k + m
         D = w.shape[0]
         K = C * tubelet * patch * patch
         Kpad = (K + 7) // 8 * 8
-        cols = ll.im2col_visible(video.contiguous(), idx, 1, n - 1, tubelet, patch, Kpad)
+        video = video.contiguous()
+        if norm_before_w is not None:
+            cols, rstd_pix = ll._im2col_prenorm(video, idx, 1, m, tubelet, patch, Kpad, norm_before_w, eps)
+        else:
+            cols, rstd_pix = ll.im2col_visible(video, idx, 1, m, tubelet, patch, Kpad), None
         wp = torch.zeros((D, Kpad), device=w.device, dtype=bf16)
         wp[:, :K] = w.reshape(D, K)
-        emb = ll.gemm(cols, wp, bias=b, epi=ll.EPI_F32)                      # fp32 [B*(n-1), D]
+        if norm_w is None:
+            conv = rstd_emb = None
+            emb = ll.gemm(cols, wp, bias=b, epi=ll.EPI_F32)                  # fp32 [B*m, D]
+        else:     # the reference normalises the bf16 conv output; the bf16 norm output is widened for the stream
+            conv = ll.gemm(cols, wp, bias=b, epi=ll.EPI_BF16)
+            y, _, rstd_emb = ll.norm_fwd(conv, norm_w, eps=eps)
+            emb = y.float()
         x0 = torch.empty((B, n, D), device=w.device, dtype=f32)
         pos2 = pos.reshape(-1, D)
-        ll.gather_add(emb, (n - 1) * D, pos2, idx[:, 1:], n, 0, B, n - 1, D, x0[:, 1:], n * D)
-        c0 = (cls.reshape(D).float() + pos2[0].float()).contiguous()
-        ll.gather_add(c0, 0, None, None, 0, 0, B, 1, D, x0[:, 0], n * D)
-        ctx.save_for_backward(cols, idx)
-        ctx.meta = (B, n, D, K, Kpad, w.shape, pos.shape, cls.shape, w.dtype)
+        ll.gather_add(emb, m * D, pos2, idx[:, 1:], ni, k - 1, B, m, D, x0[:, k:], n * D)
+        c0 = (cls.reshape(k, D).float() + pos2[:k].float()).contiguous()
+        ll.gather_add(c0, 0, None, None, 0, 0, B, k, D, x0[:, :k], n * D)
+        ctx.save_for_backward(cols, idx, wp if norm_before_w is not None else None,
+                              video if norm_before_w is not None else None, rstd_pix, conv, norm_w, rstd_emb)
+        ctx.meta = (B, n, k, D, K, Kpad, tubelet, patch, w.shape, pos.shape, cls.shape, w.dtype)
         return x0.reshape(B * n, D)
 
     @staticmethod
     def backward(ctx, dx0):
-        cols, idx = ctx.saved_tensors
-        B, n, D, K, Kpad, wshape, pshape, cshape, pdt = ctx.meta
+        cols, idx, wp, video, rstd_pix, conv, norm_w, rstd_emb = ctx.saved_tensors
+        B, n, k, D, K, Kpad, tubelet, patch, wshape, pshape, cshape, pdt = ctx.meta
+        m = n - k
         dx0 = dx0.contiguous().reshape(B, n, D)
-        demb = torch.empty((B * (n - 1), D), device=dx0.device, dtype=bf16)
-        ll.gather_add(dx0[:, 1:], n * D, None, None, 0, 0, B, n - 1, D, demb, (n - 1) * D)
+        demb = torch.empty((B * m, D), device=dx0.device, dtype=bf16)
+        ll.gather_add(dx0[:, k:], n * D, None, None, 0, 0, B, m, D, demb, m * D)
+        dnw = dnbw = None
+        if conv is not None:
+            dnw = torch.zeros(D, device=dx0.device, dtype=f32)
+            demb = ll.norm_bwd(demb, conv, norm_w, None, rstd_emb, dx_dtype=bf16, dweight=dnw)
+            dnw = dnw.to(pdt)
         dw = ll.gemm(demb, cols, a_t=True, b_t=True)[:, :K].reshape(wshape)
         db = ll.colsum(demb).to(pdt)
+        if video is not None:
+            dcols = ll.gemm(demb, wp, b_t=True)                               # bf16 [B*m, Kpad]
+            dnbw = ll._prenorm_wgrad(video, idx, 1, m, tubelet, patch, Kpad, rstd_pix, dcols).to(pdt)
         dpos = torch.zeros((pshape[-2], D), device=dx0.device, dtype=f32)
-        ll.scatter_add(dx0, n * D, idx, n, 0, B, n, D, dpos)
-        dcls = dx0[:, 0].sum(0)
-        return (None, None, dw, db, dcls.reshape(cshape).to(pdt), dpos.reshape(pshape).to(pdt), None, None)
+        # the last cls row and the patch rows: idx's cls slot (0) lands on table row k - 1
+        ll.scatter_add(dx0[:, k - 1:], n * D, idx, m + 1, k - 1, B, m + 1, D, dpos)
+        dcls = dx0[:, :k].sum(0)
+        if k > 1:
+            dpos[:k - 1] += dcls[:k - 1]
+        return (None, None, dw, db, dcls.reshape(cshape).to(pdt), dpos.reshape(pshape).to(pdt), None, None, None,
+                dnw, dnbw, None)
 
 
 class TokenEmbedFn(torch.autograd.Function):
