@@ -51,6 +51,13 @@ extern "C" {
 #define IVB_EPI_RESID 3     /* y = acc+bias; out1(bf16)=y (opt); out0(f32)=aux(f32)+rowscale[m]*gamma*y
                                (rowscale: optional fp32 [M], the per-sample DropPath keep/scale factor) */
 #define IVB_EPI_GELU_BWD 4  /* out0(bf16) = acc * gelu'(aux(bf16))                                 */
+#define IVB_EPI_SWIGLU 5    /* LLaMA's SwiGLU MLP: B = [gate; up], one K-major bf16 [N = 2I, K] operand (rows [0, I)
+                               the gate weight, [I, 2I) the up weight; I a multiple of 8); out0(bf16) [M, I] (pitch ld0)
+                               = silu(x gate^T) * (x up^T), both products from the fp32 accumulators, one rounding.
+                               The kernels load B's rows interleaved in groups of 8 (gate 8g..8g+7, then up 8g..8g+7)
+                               through a 4-D TMA map: no copy of the weight.  Single-CTA bf16 kernels only (cooperative
+                               or ping-pong, any tile_n); refused: an MN-major B, bias, out1, IVB_FLAG_ACCUM,
+                               IVB_FLAG_2CTA, a DropPath plan, and FP8 (ivb_gemm_fp8).                                */
 
 #define IVB_FLAG_GELU_TANH 1 /* tanh-approx GELU (FA2 FusedMLP) instead of erf (nn.GELU)           */
 /* IVB_FLAG_GELU_QUICK (128, below): QuickGELU x * sigmoid(1.702 x) (OpenAI-CLIP blocks, ViCLIP) instead of erf; for
@@ -434,6 +441,18 @@ int ivb_token_embed_fwd(const long long* ids, int B, int L, const void* table, i
 long ivb_token_embed_bwd_workspace_ints(int V, int B, int L);
 int ivb_token_embed_bwd(const long long* ids, int B, int L, const float* g, long ldg, int V, int D, float* dtable,
                         float* dpos, int* ws, void* stream);
+
+/* ---- rotary position embedding (LLaMA's apply_rotary_pos_emb with rotate_half, transformers modeling_llama; the
+ * InternVideo2-CLIP text tower, backbones/internvideo2/internvideo2_clip_text.py) ---------------------------------
+ * ivb_rope_qk: rotates heads h = 0 .. H-1 of the q and k rows of B clips of L tokens in place; row r = b*L + l is at
+ *   q + r*ldq and k + r*ldk (bf16; q and k may be column slots of one qkv buffer), its head h at columns h*d .. h*d + d.
+ *   With half = d/2 and c, s = cos_t[l, j], sin_t[l, j] (fp32 [L, half], contiguous; l the position in the clip):
+ *     x_j' = x_j c - x_{j+half} s,   x_{j+half}' = x_{j+half} c + x_j s   (j < half),
+ *   in fp32, each result rounded to bf16 once.  d a multiple of 16 in [16, 128]; ldq, ldk multiples of 8 and >= H*d;
+ *   q, k, cos_t and sin_t 16-byte aligned.  B = 0 or L = 0 is a no-op.  One stream-ordered kernel; capturable in a
+ *   CUDA graph.  A call that breaks a rule is refused before any CUDA call.                                          */
+int ivb_rope_qk(void* q, long ldq, void* k, long ldk, int B, int L, int H, int d, const float* cos_t,
+                const float* sin_t, void* stream);
 
 /* ---- decoder heads: LayerNorm(1e-5) -> x/||x|| (+ optional fused (2-2<out,tgt>) loss sum) --------
  * Linear_Decoder / MLP_Decoder.forward tail (internvideo2_pretrain.py:356-359, 394-397) and the

@@ -4,10 +4,12 @@ InternVideo2_CLIP_small wrapper, on the same libivb200 kernels as the masked stu
 Mirrors (constructor kwargs, attribute names, state_dict keys, forward contracts):
   InternVideo2/multi_modality/models/backbones/internvideo2/internvideo2_clip_vision.py:340-548  `InternVideo2`
   InternVideo2/multi_modality/models/internvideo2_clip_small.py:18-257                           `InternVideo2_CLIP_small`
+  InternVideo2/multi_modality/models/internvideo2_clip.py:16-254                                  `InternVideo2_CLIP`
   InternVideo2/multi_modality/models/backbones/internvideo2/pos_embed.py:137-182                 `interpolate_pos_embed`
 
-The wrapper takes any module/callable as `text_encoder`: text_modules.TextTransformer is the recipe's MobileCLIP-B tower
-on the libivb200 kernels; the default accepts pre-computed text embeddings.
+InternVideo2_CLIP_small takes any module/callable as `text_encoder`: text_modules.TextTransformer is the recipe's
+MobileCLIP-B tower on the libivb200 kernels; the default accepts pre-computed text embeddings.  InternVideo2_CLIP (the
+1B and 6B recipes) builds llama_modules.LLaMA, the frozen LLaMA-7B tower, unless it is given one.
 """
 from __future__ import annotations
 
@@ -16,6 +18,7 @@ import torch.nn as nn
 
 from . import ops
 from .contrastive import VTC_VTM_Loss
+from .llama_modules import LLaMA
 from .modules import InternVideo2Tower, LayerNormB, check_input, embed_tokens, run_blocks
 
 
@@ -123,22 +126,10 @@ class InternVideo2_CLIP_small(nn.Module):
                 "checkpoint_num")
         return InternVideo2(**{k: _get(ve, k) for k in keys if _get(ve, k) is not None})
 
-    def _vision_trainable(self):
-        return any(p.requires_grad for n, p in self.vision_encoder.named_parameters() if not n.startswith("clip_projector"))
-
     def encode_vision(self, image, test=False):
         """image [B,T,C,H,W] -> [B, align_dim] (:125-142).  With the recipe's frozen tower the blocks run on the
         no-grad path (nothing saved) and only the attention-pooling projector + vision_align are differentiated."""
-        T = image.shape[1]
-        use_image = T == 1
-        image = image.permute(0, 2, 1, 3, 4)
-        enc = self.vision_encoder
-        if self._vision_trainable() and torch.is_grad_enabled():
-            v = enc(image, use_image=use_image)
-        else:
-            with torch.no_grad():
-                h, B, n = enc.forward_tokens(image.contiguous(), use_image)
-            v = enc.fc_norm(enc.clip_projector(h.reshape(B, n, enc.embed_dim)))
+        v = tower_embeds(self.vision_encoder, image)
         ln, fc = self.vision_align[0], self.vision_align[1]
         return ops.linear(ln(v), fc.weight, fc.bias)
 
@@ -169,6 +160,99 @@ class InternVideo2_CLIP_small(nn.Module):
             ek = torch.load(extra_ckpt_path, map_location="cpu")
             new_ckpt.update(ek.get("module", ek))
         return self.load_state_dict(new_ckpt, strict=False)
+
+
+class InternVideo2_CLIP(nn.Module):
+    """internvideo2_clip.py:16-192: the InternVideo2-CLIP 1B / 6B recipes.  `config.model.vision_encoder.*`,
+    `config.model.text_encoder.{use_flash_attn,transformer_width,llama_path,use_lora}` and `config.model.{temp,temp_min,
+    freeze_vision,open_vision_clip_projector,freeze_text,open_text_projection,open_text_lora}` as in
+    scripts/pretraining/clip/{1B,6B}/config.py.  text_encoder: an llama_modules.LLaMA to use instead of building one
+    from config.model.text_encoder.  forward(image[B,T,C,H,W], text ids [B, L], idx) -> dict(loss_vtc=...).
+
+    The tokenizer stays host code: `text` is the id tensor the reference's Tokenizer returns.  The text tower has no
+    LoRA parameters (llama_modules), so open_text_lora unfreezes nothing; the recipes leave it off."""
+
+    def __init__(self, config, tokenizer=None, is_pretrain=True, text_encoder=None, process_group=None):
+        super().__init__()
+        self.config = config
+        self.tokenizer = tokenizer
+        self.is_pretrain = is_pretrain
+        m = _get(config, "model")
+        self.vision_encoder = InternVideo2_CLIP_small.build_vision_encoder(self)
+        self.text_encoder = text_encoder if text_encoder is not None else self.build_text_encoder()
+        self.temp = nn.Parameter(torch.ones([]) * _get(m, "temp"))
+        self.temp_min = _get(m, "temp_min")
+        if _get(m, "freeze_vision", False):
+            for name, p in self.vision_encoder.named_parameters():
+                if not (_get(m, "open_vision_clip_projector", False) and name.startswith("clip_projector")):
+                    p.requires_grad = False
+        if _get(m, "freeze_text", False):
+            for name, p in self.text_encoder.named_parameters():
+                if not (_get(m, "open_text_projection", False) and name.startswith("text_projection")):
+                    p.requires_grad = False
+        self.clip_loss = VTC_VTM_Loss(False, process_group=process_group)
+
+    def build_text_encoder(self):
+        te = _get(_get(self.config, "model"), "text_encoder")
+        return LLaMA(use_flash_attn=_get(te, "use_flash_attn", True), transformer_width=_get(te, "transformer_width"),
+                     llama_path=_get(te, "llama_path"), use_lora=_get(te, "use_lora", True))
+
+    def no_weight_decay(self):
+        ret = {"temp"}
+        ret.update({"vision_encoder." + k for k in self.vision_encoder.no_weight_decay()})
+        ret.update({"text_encoder." + k for k, _ in self.text_encoder.named_parameters()})
+        return ret
+
+    clip_contrastive_temperature = InternVideo2_CLIP_small.clip_contrastive_temperature
+
+    def encode_vision(self, image, test=False):
+        """image [B,T,C,H,W] -> the tower's [B, clip_embed_dim] (:115-131), on tower_embeds' frozen-tower path."""
+        return tower_embeds(self.vision_encoder, image)
+
+    def encode_text(self, text):
+        return self.text_encoder(text)
+
+    forward = InternVideo2_CLIP_small.forward
+
+    def load_checkpoint(self, vision_ckpt_path=None, text_ckpt_path=None, extra_ckpt_path=None):
+        """:194-254: the vision side through remap_vision_checkpoint, the text side through remap_text_checkpoint, then
+        the extra checkpoint's keys as they are; loaded with strict=False."""
+        m = _get(self.config, "model")
+        new_ckpt = {}
+        if vision_ckpt_path is not None:
+            ck = torch.load(vision_ckpt_path, map_location="cpu")
+            new_ckpt.update(remap_vision_checkpoint(
+                ck, self.vision_encoder, from_stage2=_get(m, "load_vision_ckpt_from_internvideo2_stage2", False),
+                orig_t_size=_get(m, "vision_ckpt_t_size", 4)))
+        if text_ckpt_path is not None:
+            new_ckpt.update(remap_text_checkpoint(torch.load(text_ckpt_path, map_location="cpu")))
+        if extra_ckpt_path is not None:
+            ek = torch.load(extra_ckpt_path, map_location="cpu")
+            new_ckpt.update(ek.get("module", ek))
+        return self.load_state_dict(new_ckpt, strict=False)
+
+
+def tower_embeds(enc, image):
+    """The frozen-tower path of both wrappers: image [B,T,C,H,W] -> the vision tower's [B, clip_embed_dim].  While no
+    parameter before the projector trains (the recipes' freeze_vision with open_vision_clip_projector), the blocks run
+    without autograd (nothing saved) and only the attention-pooling projector is differentiated."""
+    use_image = image.shape[1] == 1
+    image = image.permute(0, 2, 1, 3, 4)
+    trainable = any(p.requires_grad for n, p in enc.named_parameters() if not n.startswith("clip_projector"))
+    if trainable and torch.is_grad_enabled():
+        return enc(image, use_image=use_image)
+    with torch.no_grad():
+        h, B, n = enc.forward_tokens(image.contiguous(), use_image)
+    return enc.fc_norm(enc.clip_projector(h.reshape(B, n, enc.embed_dim)))
+
+
+def remap_text_checkpoint(ckpt):
+    """Text-side key surgery of InternVideo2_CLIP.load_checkpoint (internvideo2_clip.py:231-241): unwrap DeepSpeed
+    'module', keep `transformer.*` and `text_projection` under 'text_encoder.'.  LLaMA's load hook then maps a use_lora
+    checkpoint's keys."""
+    if "module" in ckpt:
+        ckpt = ckpt["module"]
+    return {"text_encoder." + k: v for k, v in ckpt.items() if k.startswith("transformer.") or k == "text_projection"}
 
 
 def interpolate_pos_embed(checkpoint_model, model, orig_t_size=4, pos_name="vision_encoder.pos_embed"):

@@ -134,7 +134,7 @@ __device__ __forceinline__ void epilogue_stage(const float (&acc)[NH][BN / 2], f
   }
 }
 
-template <int BN, int NH>
+template <int BN, int NH, bool SWIGLU>
 __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float (&acc)[NH][BN / 2], float* st, long row0,
                                               int n0) {
   constexpr int CHUNKS = NH * ((BN + 31) / 32);
@@ -179,7 +179,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float (
         const float4 f = reinterpret_cast<const float4*>(src)[k];
         v[4 * k] = f.x; v[4 * k + 1] = f.y; v[4 * k + 2] = f.z; v[4 * k + 3] = f.w;
       }
-      epilogue_chunk<16>(p, accum, tanh_mode, quick_mode, save_grad, v, in, bias, gamma, row, n0 + col, nvalid);
+      epilogue_chunk<16, SWIGLU>(p, accum, tanh_mode, quick_mode, save_grad, v, in, bias, gamma, row, n0 + col, nvalid);
     }
     __syncwarp();
   }
@@ -354,7 +354,12 @@ __device__ __forceinline__ void produce(const CUtensorMap& tmA, const CUtensorMa
       }
       if (CL == 1) {
         if (!B_MN) {
-          tma_load_2d(sb, &tmB, k0, n0, &s.full[stage]);
+          // IVB_EPI_SWIGLU: tmB is the 4-D (k, row, half, 8-row group) map of launch_gemm, so the tile's BN rows come in
+          // as gate rows 8g .. 8g + 7, then the up rows of the same output columns, for each of its BN / 16 groups
+          if (!Op::FP8 && p.epi == IVB_EPI_SWIGLU)
+            tma_load_4d(sb, &tmB, k0, 0, 0, n0 / 16, &s.full[stage]);
+          else
+            tma_load_2d(sb, &tmB, k0, n0, &s.full[stage]);
         } else {
 #pragma unroll
           for (int i = 0; i < Cfg::B_ATOMS; ++i)
@@ -495,7 +500,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         release(prev);
       }
       dequantise<Op, BN, 1>(p, acc, dq, m0 + cw * 64, n0);
-      epilogue_tile<BN, 1>(p, acc, st, m0 + cw * 64, n0);
+      epilogue_tile<BN, 1, !Op::FP8>(p, acc, st, m0 + cw * 64, n0);
     }
   }
   if (CL == 2) cluster_sync_all();   // the peer may still multicast into / arrive on this CTA's ring
@@ -570,7 +575,7 @@ gemm_bf16_pingpong_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_
       wgmma_reg_fence(acc[1], PP_BN / 2);
       if (signal) mbar_arrive(&s.empty[prev]);
       dequantise<Op, PP_BN, 2>(p, acc, dq, m0, n0);
-      epilogue_tile<PP_BN, 2>(p, acc, st, m0, n0);
+      epilogue_tile<PP_BN, 2, !Op::FP8>(p, acc, st, m0, n0);
     }
   }
 }
@@ -593,8 +598,19 @@ static int launch_gemm(const void* A, long lda, const void* B, long ldb, const G
   if (!A_MN) rc = make_tmap_2d(&tmA, A, (uint64_t)p.K, (uint64_t)p.M, lda, Op::BK, BM, EB);
   else       rc = make_tmap_2d(&tmA, A, (uint64_t)p.M, (uint64_t)p.K, lda, 64, 64);
   if (rc) return rc;
-  if (!B_MN) rc = make_tmap_2d(&tmB, B, (uint64_t)p.K, (uint64_t)p.N, ldb, Op::BK, BN / CL, EB);
-  else       rc = make_tmap_2d(&tmB, B, (uint64_t)p.N, (uint64_t)p.K, ldb, 64, 64);
+  if (p.epi == IVB_EPI_SWIGLU) {
+    // B = [gate; up], [2I, K]: dims (k, row in an 8-row group, half [I rows apart], group [8 rows apart]).  An 8-row
+    // group is one 128-byte swizzle atom, so the box lands in shared memory as a 2-D box of the same BN rows would.
+    const long I = p.N / 2;
+    const uint64_t dims[4] = {(uint64_t)p.K, 8, 2, (uint64_t)(I / 8)};
+    const long strides[3] = {ldb, I * ldb, 8 * ldb};
+    const uint32_t box[4] = {64, 8, 2, BN / 16};
+    rc = make_tmap_4d(&tmB, B, dims, strides, box);
+  } else if (!B_MN) {
+    rc = make_tmap_2d(&tmB, B, (uint64_t)p.K, (uint64_t)p.N, ldb, Op::BK, BN / CL, EB);
+  } else {
+    rc = make_tmap_2d(&tmB, B, (uint64_t)p.N, (uint64_t)p.K, ldb, 64, 64);
+  }
   if (rc) return rc;
   constexpr auto kern = gemm_kernel<Op, PINGPONG, BN, A_MN, B_MN, CL>();
   if ((rc = raise_smem_limit<kern>(Cfg::SMEM_BYTES, "cudaFuncSetAttribute(gemm)"))) return rc;
@@ -762,10 +778,18 @@ static int gemm_bf16(const char* fn, const void* A, int a_mn_major, long lda, co
   if (k_plan != nullptr && !(a_mn_major && b_mn_major)) return fail("a K plan needs both operands MN-major (wgrad)");
   if (k_plan != nullptr && (bias != nullptr || (epilogue != IVB_EPI_BF16 && epilogue != IVB_EPI_F32)))
     return fail("a K plan needs IVB_EPI_BF16 or IVB_EPI_F32 without bias");
+  if (epilogue == IVB_EPI_SWIGLU) {
+    if (b_mn_major) return fail("IVB_EPI_SWIGLU needs a K-major B");
+    if (N & 15) return fail("IVB_EPI_SWIGLU needs N = 2I with I a multiple of 8");
+    if (bias != nullptr || out1 != nullptr) return fail("IVB_EPI_SWIGLU takes no bias and no out1");
+    if (flags & (IVB_FLAG_ACCUM | IVB_FLAG_2CTA)) return fail("IVB_EPI_SWIGLU excludes IVB_FLAG_ACCUM and IVB_FLAG_2CTA");
+    if (plan) return fail("IVB_EPI_SWIGLU has no DropPath plan form");
+  }
   p.m_plan = m_plan;
   p.k_plan = k_plan;
-  // a plan runs on the single-CTA kernels, whatever the process-wide CTA-pair default
-  const KernelChoice k = choose_kernel(M, N, K, flags, tile_n, false, g_default_2cta && !plan);
+  // a plan and the SwiGLU epilogue run on the single-CTA kernels, whatever the process-wide CTA-pair default
+  const KernelChoice k = choose_kernel(M, N, K, flags, tile_n, false,
+                                       g_default_2cta && !plan && epilogue != IVB_EPI_SWIGLU);
   if (!a_mn_major && !b_mn_major) return dispatch<OpBf16, false, false>(k, A, lda, B, ldb, p, stream);
   if (!a_mn_major) return dispatch<OpBf16, false, true>(k, A, lda, B, ldb, p, stream);
   return dispatch<OpBf16, true, true>(k, A, lda, B, ldb, p, stream);
@@ -807,6 +831,7 @@ static int gemm_fp8(const char* fn, const void* A, int a_mn_major, long lda, int
   if ((lda & 15) || (ldb & 15)) return fail("lda and ldb must be multiples of 16 elements");
   if ((N & 7) || (ld0 & 7)) return fail("N and ld0 must be multiples of 8 elements");
   if (a_format != IVB_FP8_E4M3 && a_format != IVB_FP8_E5M2) return fail("unknown a_format");
+  if (epilogue == IVB_EPI_SWIGLU) return fail("IVB_EPI_SWIGLU is bf16 only (ivb_gemm_bf16)");
   if (a_scale_inv == nullptr || b_scale_inv == nullptr) return fail("scale_inv pointers are null");
   const bool vec = (flags & IVB_FLAG_FP8_VECTOR_SCALES) != 0;
   if (vec && a_format != IVB_FP8_E4M3) return fail("vector scales need an E4M3 A operand");

@@ -184,7 +184,9 @@ __device__ __forceinline__ void epilogue_load(const GemmParams& p, bool accum, E
 
 // v: the W fp32 accumulators of (row, col0 .. col0+W-1), 0 < nvalid <= W of them inside the matrix.  in: what
 // epilogue_load read for them.  bias_bits / gamma_bits: the W bf16 of bias / gamma at col0 (when the GEMM has them).
-template <int W>
+// SWIGLU: build the IVB_EPI_SWIGLU case (the bf16 kernels).  The FP8 kernels, whose entry points refuse it, leave it
+// out: compiled in, it costs the cooperative E4M3 kernel at BN 192 an 8-byte spill.
+template <int W, bool SWIGLU>
 __device__ __forceinline__ void epilogue_chunk(const GemmParams& p, bool accum, bool tanh_mode, bool quick_mode,
                                                bool save_grad, float* v, const EpiIn<W>& in, const uint32_t* bias_bits,
                                                const uint32_t* gamma_bits, long row, int col0, int nvalid) {
@@ -289,6 +291,21 @@ __device__ __forceinline__ void epilogue_chunk(const GemmParams& p, bool accum, 
         for (int i = 0; i < W; ++i) v[i] *= gelu_erf_grad(hv[i]);
       }
       store_row_bf16<W>(reinterpret_cast<__nv_bfloat16*>(p.out0) + row * p.ld0 + col0, v, nvalid);
+    } break;
+    case IVB_EPI_SWIGLU: if constexpr (SWIGLU) {
+      // The B tile interleaves gate and up rows in groups of 8 (ivb_gemm.cu, launch_gemm), so each 16 columns of the
+      // segment are the gate (v[i .. i+8)) and up (v[i+8 .. i+16)) products of the 8 output columns from (col0 + i) / 2:
+      // out0(bf16) [M, N/2] = silu(gate) * up, one 16-byte piece each.
+#pragma unroll
+      for (int i = 0; i < W; i += 16) {
+        if (i >= nvalid) break;
+        uint32_t r[4];
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+          r[k] = pack_bf16(silu(v[i + 2 * k]) * v[i + 8 + 2 * k], silu(v[i + 2 * k + 1]) * v[i + 9 + 2 * k]);
+        *reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(p.out0) + row * p.ld0 + (col0 + i) / 2) =
+            make_uint4(r[0], r[1], r[2], r[3]);
+      }
     } break;
     default:
       break;

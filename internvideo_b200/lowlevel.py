@@ -11,6 +11,7 @@ import torch
 from . import _lib
 
 EPI_BF16, EPI_F32, EPI_BIAS_GELU, EPI_RESID, EPI_GELU_BWD = 0, 1, 2, 3, 4
+EPI_SWIGLU = 5             # silu(x gate^T) * (x up^T) from one [gate; up] weight [2I, K]; out0 is [M, I]
 FLAG_GELU_TANH, FLAG_ACCUM, FLAG_1CTA, FLAG_2CTA, FLAG_GELU_SAVE_GRAD, FLAG_PINGPONG = 1, 2, 4, 8, 16, 32
 FLAG_GELU_QUICK = 128      # QuickGELU x * sigmoid(1.702 x) in the GELU epilogues (excludes FLAG_GELU_TANH)
 FLAG_FP8_VECTOR_SCALES = 64
@@ -154,6 +155,7 @@ def gemm(a, b, *, a_t=False, b_t=False, epi=EPI_BF16, flags=0, out0=None, out1=N
     b_t=False: `b` is [N,K]; b_t=True: `b` is [K,N].
     m_plan / k_plan: the M and K plans of a DropPath plan over the GEMM's M rows / its K (ops.droppath_plan); with
     either the call goes to ivb_gemm_bf16_plan, which skips the work of the dropped rows.
+    epi=EPI_SWIGLU: `b` is [gate; up], [N = 2I, K] (K-major), and out0 is [M, I] = silu(x gate^T) * (x up^T).
     """
     _chk(("a", a, bf16), ("b", b, bf16), ("m_plan?", m_plan, i32), ("k_plan?", k_plan, i32))
     lda = _rows2d(a, "a"); ldb = _rows2d(b, "b")
@@ -180,7 +182,7 @@ def _epilogue_operands(M, N, epi, out0, out1, bias, gamma, aux, rowscale, device
     """Checks the fused epilogue's operands of an [M, N] GEMM, allocating out0 if it is None.  Returns out0."""
     out_dtype = f32 if epi in (EPI_F32, EPI_RESID) else bf16
     if out0 is None:
-        out0 = torch.empty((M, N), device=device, dtype=out_dtype)
+        out0 = torch.empty((M, N // 2 if epi == EPI_SWIGLU else N), device=device, dtype=out_dtype)
     _chk(("out0", out0, out_dtype), ("out1?", out1, bf16), ("bias?", bias, bf16), ("gamma?", gamma, bf16),
          ("aux?", aux, f32 if epi == EPI_RESID else bf16), ("rowscale?", rowscale, f32))
     return out0
@@ -468,6 +470,21 @@ def attn_fwd(q, k, v, B, n, H, d, scale, out=None, want_lse=True, rowscale=None,
     _call(name, q, _rows2d(q, "q"), k, _rows2d(k, "k"), v, _rows2d(v, "v"), out, _rows2d(out, "out"), lse, B, n, H, d,
           float(scale), *extra, kind="attn_fwd", flops=(2.0 if causal else 4.0) * B * H * n * n * d)
     return out, lse
+
+
+def _rope_qk(q, k, B, L, H, d, cos, sin):
+    """Rotary position embedding of the heads of q and k, in place (ivb_rope_qk): q, k bf16 2-D views [B*L, H*d] (any
+    row pitch; e.g. two column slots of one qkv buffer), cos and sin contiguous fp32 [L, d/2], row l for position l of
+    each clip (LLaMA's rotate_half pairing: column j with column j + d/2).  Private, as _token_embed_fwd: the LLaMA
+    layer (llama_modules.LlamaDecoderLayer) is its caller."""
+    _chk(("q", q, bf16), ("k", k, bf16), ("cos", cos, f32), ("sin", sin, f32))
+    for t, nm in ((q, "q"), (k, "k")):
+        if t.shape != (B * L, H * d):
+            raise _lib.IvbError(f"rope_qk: {nm} must be [B*L, H*d], got {tuple(t.shape)}")
+    for t, nm in ((cos, "cos"), (sin, "sin")):
+        if t.shape != (L, d // 2) or not t.is_contiguous():
+            raise _lib.IvbError(f"rope_qk: {nm} must be a contiguous [L, d/2] = [{L}, {d // 2}], got {tuple(t.shape)}")
+    _call("rope_qk", q, _rows2d(q, "q"), k, _rows2d(k, "k"), B, L, H, d, cos, sin)
 
 
 def headaxis_attn_fwd(qkv, B, N, H, d, scale):
