@@ -508,6 +508,23 @@ int ivb_pool_attn_bwd(const void* q, const void* k, long ldk, const void* v, lon
                       const float* probs, const void* dout, int B, int n, int H, int d, float scale,
                       void* dq, void* dk, long lddk, void* dv, long lddv, void* stream);
 
+/* ---- InternVideo-MM global extractor: position conv + key LayerNorm (clip_vit_only_global.py:203-231, 147) ----------
+ * ivb_dpe_ln_fwd: x holds one extractor tap of the backbone stream, N clips of T frames of 1 + H*W rows each: row
+ *   (n*T + t)*(1 + H*W) + l, l = 0 the frame's cls row, l = 1 + h*W + w its patch (h, w).  x is fp32 (x_is_f32 = 1,
+ *   the residual stream) or bf16, pitch ldx.  y bf16 (pitch ldy), the same rows:
+ *     patch row:  y = LN(x + conv_b + sum_{dt,dh,dw in {-1,0,1}} conv_w[c, dt, dh, dw] * x[n, t+dt, h+dh, w+dw, c])
+ *     cls row:    y = LN(x)
+ *   with zero padding at the edges of the T x H x W grid (the depthwise Conv3d `dpe`, kernel 3, padding 1, bias, added
+ *   to the patch tokens, then `ln_3`).  LN: LayerNorm over C with ln_w, ln_b and eps.  conv_w: bf16 [C, 1, 3, 3, 3] as
+ *   the reference stores it (2-byte aligned); conv_b, ln_w, ln_b: bf16 [C].  Every sum in fp32, one bf16 rounding of y;
+ *   the same bits on every run (no atomics).  T, H, W >= 1 (T = 1: only the centre temporal tap contributes); C a
+ *   multiple of 8 in [8, 4096]; ldx, ldy multiples of 8 and >= C; x, conv_b, ln_w, ln_b and y 16-byte aligned; y must
+ *   not overlap x (a CTA reads the neighbour rows that other CTAs write).  N = 0
+ *   is a no-op.  One stream-ordered kernel; capturable in a CUDA graph.  A call that breaks a rule is refused before
+ *   any CUDA call.                                                                                                  */
+int ivb_dpe_ln_fwd(const void* x, int x_is_f32, long ldx, const void* conv_w, const void* conv_b, const void* ln_w,
+                   const void* ln_b, float eps, int N, int T, int H, int W, int C, void* y, long ldy, void* stream);
+
 /* ---- flat AdamW (decoupled weight decay; fp32 master/moments, bf16 model copy) --------------------
  * torch.optim.AdamW semantics (optim_factory.py:141-142; DeepSpeed adam_w_mode utils.py:821-834).
  * Gradients are multiplied by grad_scale * (*grad_scale_dev) first (1/world_size, clip coefficient; grad_scale_dev

@@ -487,6 +487,35 @@ def _rope_qk(q, k, B, L, H, d, cos, sin):
     _call("rope_qk", q, _rows2d(q, "q"), k, _rows2d(k, "k"), B, L, H, d, cos, sin)
 
 
+def _dpe_ln_fwd(x, conv_w, conv_b, ln_w, ln_b, eps, N, T, H, W, out=None):
+    """InternVideo-MM's extractor position conv + key LayerNorm (ivb_dpe_ln_fwd): x fp32 or bf16 [N*T*(1+H*W), C] (any
+    row pitch), conv_w bf16 [C, 1, 3, 3, 3], conv_b / ln_w / ln_b bf16 [C] -> bf16 [N*T*(1+H*W), C]: each patch row
+    LN(x + dpe(x)), each frame's cls row LN(x).  out (optional, any row pitch) must not overlap x: the kernel reads
+    the neighbour rows that other CTAs write.  Private, as _rope_qk: InternVideo-MM's extractor
+    (internvideo_mm.Transformer) is its caller."""
+    _chk(("x", x, (f32, bf16)), ("conv_w", conv_w, bf16), ("conv_b", conv_b, bf16), ("ln_w", ln_w, bf16),
+         ("ln_b", ln_b, bf16), ("out?", out, bf16))
+    M, C = x.shape
+    if M != N * T * (1 + H * W) or conv_w.shape != (C, 1, 3, 3, 3) or not conv_w.is_contiguous():
+        raise _lib.IvbError(f"dpe_ln_fwd: x must be [N*T*(1+H*W), C] = [{N * T * (1 + H * W)}, C] and conv_w a "
+                            f"contiguous [C, 1, 3, 3, 3], got {tuple(x.shape)}, {tuple(conv_w.shape)}")
+    for t, nm in ((conv_b, "conv_b"), (ln_w, "ln_w"), (ln_b, "ln_b")):
+        if t.shape != (C,) or not t.is_contiguous():
+            raise _lib.IvbError(f"dpe_ln_fwd: {nm} must be a contiguous [C] = [{C}], got {tuple(t.shape)}")
+    if out is None:
+        out = torch.empty((M, C), device=x.device, dtype=bf16)
+    elif out.shape != (M, C):
+        raise _lib.IvbError(f"dpe_ln_fwd: out must be [{M}, {C}], got {tuple(out.shape)}")
+    else:
+        xs, xe = x.data_ptr(), x.data_ptr() + ((M - 1) * x.stride(0) + C) * x.element_size()
+        os_, oe = out.data_ptr(), out.data_ptr() + ((M - 1) * out.stride(0) + C) * out.element_size()
+        if xs < oe and os_ < xe:
+            raise _lib.IvbError("dpe_ln_fwd: out must not overlap x (the kernel reads rows other CTAs write)")
+    _call("dpe_ln_fwd", x, int(x.dtype == f32), _rows2d(x, "x"), conv_w, conv_b, ln_w, ln_b, float(eps), N, T, H, W, C,
+          out, _rows2d(out, "out"))
+    return out
+
+
 def headaxis_attn_fwd(qkv, B, N, H, d, scale):
     """The VideoMAEv2 teacher's attention as the reference runs it (softmax over the H heads of each token, see
     include/ivb200.h).  qkv bf16 [B*N, 3*H*d] -> bf16 [B, H, N, d] contiguous."""
